@@ -278,10 +278,6 @@ int gmpi_debug_plane_coords_packed(const int32_t* view2mpi, const float* dhw, co
 /* Test hook: force the forward kernel variant: 0 auto (default), 1 direct-gather, 2 TMA-staged. */
 int gmpi_debug_set_fwd_variant(int variant);
 
-/* GMPI_ZERO_GRAD of the staged backward as stream memsets before the kernel (0, default) or inside the kernel, one MPI slab
- * ahead of use (1: correct for any view order; see mpi_bwd_box.cuh). */
-int gmpi_debug_set_bwd_zero(int in_kernel);
-
 /* Test hook (host only): the TMA copies the expanded forward issues for a footprint of n_rows staged rows, as (first row, rows)
  * pairs: the binary digits of n_rows / 4 (copies of 32, 16, 8, 4 rows).  Returns the number of copies. */
 int gmpi_debug_copy_plan(int n_rows, int* out_row_rows, int max_copies);

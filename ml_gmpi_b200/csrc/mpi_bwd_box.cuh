@@ -30,18 +30,7 @@
 
 namespace gmpi {
 
-// Build-time tunables, for A/B builds: consumer / flusher warp counts (tile height = 2 x consumer warps) and where the consumers
-// wait for the emptied gradient box (before the first scatter, or before the sampling).
-#ifndef GMPI_BWD_CONS_WARPS
-#define GMPI_BWD_CONS_WARPS 12
-#endif
-#ifndef GMPI_BWD_FLUSH_WARPS
-#define GMPI_BWD_FLUSH_WARPS 3
-#endif
-#ifndef GMPI_BWD_LATE_WAIT
-#define GMPI_BWD_LATE_WAIT 1
-#endif
-constexpr int kBwdConsWarps = GMPI_BWD_CONS_WARPS, kBwdFlushWarps = GMPI_BWD_FLUSH_WARPS;
+constexpr int kBwdConsWarps = 12, kBwdFlushWarps = 3;
 constexpr int kBwdTileH = kPairs * kBwdConsWarps;                                   // 64 x 24 pixel tiles
 constexpr int kBwdConsThreads = kBwdConsWarps * 32;
 constexpr int kBwdThreads = (kBwdConsWarps + 1 + kBwdFlushWarps) * 32;              // 16 warps: 12 consumers, producer, 3 flushers
@@ -57,10 +46,7 @@ struct BwdRing {
     static constexpr int kTileRows = kBwdTileH, kRingStages = kBwdStages, kBoxMaxH = kBwdMaxBH;
     static constexpr int kPlaneFloats = kBwdPlaneFloats, kStride = kBwdStride;
     static constexpr bool kReverse = true;       // planes back to front; each stage also carries the tile's saved transmittance
-#ifndef GMPI_BWD_SLEEP
-#define GMPI_BWD_SLEEP 1
-#endif
-    static constexpr bool kSleepPolls = GMPI_BWD_SLEEP != 0;
+    static constexpr bool kSleepPolls = true;
     static constexpr bool kWideFact = false;     // the backward keeps the 56..88-wide classes: its shared memory is full
     static constexpr bool kBinaryCopies = false; // expanded MPI: one 4-row copy per lane (see staged_producer)
     // factored MPI: colour box = 3 copies of 12 rows (row offset r * 3 * bw * 4 bytes must be a multiple of 128 for bw = 56..88,
@@ -231,7 +217,7 @@ __device__ __forceinline__ bool bwd_box_pairs(const float* __restrict__ sb, int*
         R[P] = fma2(a, d, R[P]);
         // ---- scatter (grid_sampler_2d_backward), fixed point: colour channels one-step, alpha two-step ----
         // The gradient box is needed only from here on: the flushers get the first pair's sampling time to finish emptying it.
-        if (GMPI_BWD_LATE_WAIT && P == 0) mbar_wait(g_empty_bar, g_empty_parity);
+        if (P == 0) mbar_wait(g_empty_bar, g_empty_parity);
         const f2 wF = mul2(wT, Fs_rgb);                 // exact (power of two)
         int* ga = gb + idx[2 * P];
         int* gq = gb + idx[2 * P + 1];
@@ -287,95 +273,6 @@ __device__ __forceinline__ void flush_box(int* __restrict__ gb, const GradMeta& 
     }
 }
 
-// ---- in-kernel zeroing of the gradient (opt-in: gmpi_debug_set_bwd_zero(1); GMPI_ZERO_GRAD defaults to stream memsets) -----------
-// A memset of the gradient (16 B per texel-plane, 6.4 GB for the headline train step: 0.87 ms at the write peak) cannot overlap
-// the persistent kernels -- they own every register of every SM, the memset kernel runs strictly before or after them
-// (tools/zero_overlap_probe.py: forward + side-stream memset = the sum of the two).  This is the attempt to hide it in the
-// backward, which is far from HBM-bound: the producer warp zeroes the gradient with plain 16-byte stores between the polls of
-// its wait for a free ring stage, ONE MPI SLAB AHEAD of the tiles that add to it.  Every CTA owns 1/grid of each slab;
-// zero_flags[m] counts the CTAs that are done with slab m.
-// Correct and deadlock-free, but the stores go through the same l1tex data path as the consumers' LDS/ATOMS, so it is off by
-// default.  Kept as a tested option (a TMA bulk store from a zero page would bypass that path; the backward has no shared memory
-// left for one).
-// Protocol (any view order is safe, sorted-by-MPI views -- MPI.forward's layout -- are fast):
-//   * before issuing the copies of a tile of MPI m the producer has zeroed, fenced and signalled its share of slabs 0..m;
-//   * while it walks the tiles of MPI m it zeroes slab m + 1, eight stores at a time between the polls of its wait for a free
-//     ring stage (at most zero_rate stores per stage on average); at the end of its walk, the rest;
-//   * whoever adds to slab m with red.global (flushers; consumers on the rare generic path) first waits for zero_flags[m] ==
-//     gridDim.x (one acquire load once the slab is known to be ready).
-// No deadlock: a CTA only ever waits for flags of slabs <= its current tile's, every CTA signals those before it can block on its
-// own ring, and all CTAs are co-resident (grid <= SMs, one CTA per SM).
-struct GradZeroPacer {
-    static constexpr bool kActive = true;
-    float4* base;
-    unsigned long long slab, off, end;      // float4 units: slab size; [off, end) = what is left of this CTA's share of slab `next`
-    unsigned* flags;
-    int M, rate, lane, next, allowed;       // next: first slab not yet signalled; slabs < allowed may be zeroed in the background
-    int budget;                             // warp-wide stores this CTA may still issue in the current ring stage
-    unsigned cta, n_cta;
-    __device__ __forceinline__ void set_share() {
-        if (next >= M) { off = end = 0; return; }
-        const unsigned long long per = (slab + n_cta - 1) / n_cta;
-        const unsigned long long lo = min(slab, per * cta), hi = min(slab, lo + per);
-        off = (unsigned long long)next * slab + lo; end = (unsigned long long)next * slab + hi;
-    }
-    __device__ __forceinline__ void init(const RenderParams& p, int lane_) {
-        base = p.zero_base; slab = p.zero_slab16; flags = p.zero_flags; M = flags ? p.M : 0; rate = p.zero_rate; lane = lane_;
-        next = 0; allowed = 0; budget = 0; cta = blockIdx.x; n_cta = gridDim.x;
-        set_share();
-    }
-    __device__ __forceinline__ void store8() {                     // eight warp-wide 512-byte stores
-        float4* ptr = base + off + (unsigned)lane;
-        const float4 z = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
-        if (off + 256 <= end) {
-#pragma unroll
-            for (int k = 0; k < 8; ++k) ptr[32 * k] = z;
-        } else {
-#pragma unroll
-            for (int k = 0; k < 8; ++k)
-                if (off + 32 * k + (unsigned)lane < end) ptr[32 * k] = z;
-        }
-        off += 256;
-    }
-    __device__ __forceinline__ void signal() {
-        __threadfence();
-        __syncwarp();
-        if (lane == 0) { __threadfence(); atomicAdd(flags + next, 1u); }
-        ++next;
-        set_share();
-    }
-    __device__ __forceinline__ void finish_through(int m) {
-        while (next < M && next <= m) {
-            while (off < end) store8();
-            signal();
-        }
-    }
-    __device__ __forceinline__ void before_tile(int m) { finish_through(m); allowed = max(allowed, m + 2); }
-    __device__ __forceinline__ void new_stage() { budget = min(budget + rate, 8 * rate); }
-    // between two polls of the producer's wait for a free stage: false = nothing to do (slab not yet allowed, or this stage's
-    // budget is spent -- the stores must not crowd the copies out of the memory system, nor delay their issue by more than a chunk)
-    __device__ __forceinline__ bool chunk() {
-        if (budget <= 0 || next >= M || next >= allowed) return false;
-        store8();
-        budget -= 8;
-        if (off >= end) signal();
-        return true;
-    }
-    __device__ __forceinline__ void at_end() { finish_through(M - 1); }
-};
-
-// Called by every lane that is about to add to slab m with red.global: returns once all CTAs have zeroed their share of it.
-__device__ __forceinline__ void wait_grad_zeroed(const RenderParams& p, int m) {
-    if (!p.zero_flags) return;
-    const unsigned* f = p.zero_flags + m;
-    for (;;) {
-        unsigned v;
-        asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(f) : "memory");
-        if (v >= gridDim.x) return;
-        __nanosleep(256);
-    }
-}
-
 __device__ __forceinline__ void bwd_consumer_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kBwdConsThreads) : "memory"); }
 
 template <bool kAlignCorners, bool kFactored>
@@ -417,27 +314,22 @@ mpi_bwd_box_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps, c
     if (warp == kBwdConsWarps) {
         // ================================ producer ================================
         if (lane == 0) tma_prefetch_desc(&maps.t);
-        GradZeroPacer pacer;
-        pacer.init(p, lane);
-        staged_producer<kAlignCorners, BwdRing, kFactored>(p, maps, s_buf, s_meta, s_full, s_empty, &s_walk, lane, pacer);
+        staged_producer<kAlignCorners, BwdRing, kFactored>(p, maps, s_buf, s_meta, s_full, s_empty, &s_walk, lane);
     } else if (warp > kBwdConsWarps) {
         // ================================ flushers ================================
         const int fw = warp - kBwdConsWarps - 1;
         int f_box = 0;
         uint32_t f_phase = 0;
-        int f_zeroed = -1;      // last slab known to be zeroed by all CTAs
         TileXY txy;
         for (int j = 0; s_walk.at(j, txy); ++j) {
             for (int ii = 0; ii < N; ++ii) {
                 const int b = f_box;
                 const uint32_t ph = f_phase;
                 if (++f_box == kBwdBoxes) { f_box = 0; f_phase ^= 1u; }
-                if (BwdRing::kSleepPolls) mbar_wait_sleep(&g_full[b], ph);
-                else mbar_wait(&g_full[b], ph);
+                mbar_wait_sleep(&g_full[b], ph);
                 const GradMeta gm = s_gmeta[b];
                 int* gb = s_grad + b * kBwdPlaneFloats;
                 if (gm.rows > 0) {
-                    if ((gm.mpi_bg >> 1) != f_zeroed) { f_zeroed = gm.mpi_bg >> 1; wait_grad_zeroed(p, f_zeroed); }
                     switch (gm.cls) {     // warp-uniform
                         case 0: flush_box<56, kFactored>(gb, gm, p, tex, Ht, Wt, fw, lane); break;
                         case 1: flush_box<64, kFactored>(gb, gm, p, tex, Ht, Wt, fw, lane); break;
@@ -566,7 +458,6 @@ mpi_bwd_box_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps, c
                     T[P] = make_float2(tr[0], tr[32]);
                 }
                 // ---- gradient box of this (tile, plane): sample, wait until the flushers have emptied it, scatter ----
-                if (!GMPI_BWD_LATE_WAIT) mbar_wait(&g_empty[b], gph ^ 1u);
                 int* gb = s_grad + b * kBwdPlaneFloats;
                 constexpr int AO = kFactored ? kBwdAlphaOff : 0;
                 bool done = false;
@@ -580,7 +471,7 @@ mpi_bwd_box_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps, c
                 const int cls = done ? 0 : -1;
                 // a warp that did not use the box still waits: it must not arrive on g_full[b] a second time before the flushers
                 // have taken the previous fill (the arrival counts of two fills would mix)
-                if (GMPI_BWD_LATE_WAIT && !done) mbar_wait(&g_empty[b], gph ^ 1u);
+                if (!done) mbar_wait(&g_empty[b], gph ^ 1u);
                 __syncwarp();
                 mbar_arrive_if(&s_empty[s], lane_ == 0);    // taps and transmittance are consumed: hand the stage back
                 if (warp == 0 && lane == 0) {               // (warp 0 always has a row inside the image)
@@ -602,7 +493,6 @@ mpi_bwd_box_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps, c
                     // taken when the producer's corner-ray estimate says "nothing under the tile": a hint, never trusted ----
                     const float* plane = kFactored ? nullptr : p.rgba + ((size_t)m * N + i) * 4 * tex;
                     float* gplane = kFactored ? nullptr : p.g_rgba + ((size_t)m * N + i) * 4 * tex;
-                    wait_grad_zeroed(p, m);       // (in-kernel GMPI_ZERO_GRAD: slab m must be zero before anything is added to it)
                     float* Rs = reinterpret_cast<float*>(R);
                     const float* Ts = reinterpret_cast<const float*>(T);
 #pragma unroll

@@ -49,13 +49,6 @@ struct RenderParams {
     float* g_bg_rgb;          // bwd, factored with a separate background: [M,3,Ht,Wt] of the last plane
     float* g_alpha;           // bwd, factored: [M,N,1,Ht,Wt]
     int view_group;           // > 1: every `view_group` consecutive views share one MPI (tile order hint, see TileWalk)
-    // staged backward with GMPI_ZERO_GRAD: the kernel zeroes the large gradient buffer itself, one MPI slab ahead of its use
-    // (GradZeroPacer, mpi_bwd_box.cuh).  zero_base = g_rgba or g_alpha, zero_slab16 = float4s per MPI, zero_flags[M] = number of
-    // CTAs that have zeroed their share of MPI m (zero on entry), zero_rate = warp-wide 512-byte stores per ring stage.
-    float4* zero_base;
-    unsigned long long zero_slab16;
-    unsigned* zero_flags;
-    int zero_rate;
 };
 
 // The four channel slabs (Ht*Wt floats each) of one (MPI, plane): expanded rgba or the generator's factored form.

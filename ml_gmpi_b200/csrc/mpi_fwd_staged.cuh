@@ -16,15 +16,11 @@
 
 namespace gmpi {
 
-#ifndef GMPI_CONS_WARPS
-#define GMPI_CONS_WARPS 15   // 15 consumer warps + producer = 16 warps = 4 per scheduler, 128 registers per thread
-#endif
-#ifndef GMPI_PAIRS
-#define GMPI_PAIRS 2         // packed pixel pairs per thread (each pair = x and x+32 of one tile row)
-#endif
-constexpr int kPairs = GMPI_PAIRS, kPix = 2 * GMPI_PAIRS;
-constexpr int kTileW = 64, kTileH = kPairs * GMPI_CONS_WARPS;
-constexpr int kConsWarps = GMPI_CONS_WARPS, kConsThreads = kConsWarps * 32, kStagedThreads = kConsThreads + 32;
+constexpr int kConsWarps = 15;   // 15 consumer warps + producer = 16 warps = 4 per scheduler, 128 registers per thread
+constexpr int kPairs = 2;        // packed pixel pairs per thread (each pair = x and x+32 of one tile row)
+constexpr int kPix = 2 * kPairs;
+constexpr int kTileW = 64, kTileH = kPairs * kConsWarps;
+constexpr int kConsThreads = kConsWarps * 32, kStagedThreads = kConsThreads + 32;
 constexpr int kStages = 3;
 constexpr int kRowsPerOp = 4;
 constexpr int kMaxBW = 88;
@@ -33,14 +29,7 @@ constexpr int kMaxBH = (((kTileH * 5) / 4 + 6 + kRowsPerOp - 1) / kRowsPerOp) * 
 // sixteen taps are LDS [reg + immediate]; the producer picks the narrowest class that covers the footprint.
 constexpr int kMinBW = 56, kBWStep = 8;
 constexpr int kNumMaps = (kMaxBW - kMinBW) / kBWStep + 1;
-#ifndef GMPI_MAX_PLANES_STAGED
-#define GMPI_MAX_PLANES_STAGED 512
-#endif
-#ifndef GMPI_CTAS_PER_SM
-#define GMPI_CTAS_PER_SM 1
-#endif
-constexpr int kMaxPlanesStaged = GMPI_MAX_PLANES_STAGED;   // plane-constant table: 32 B per plane in shared memory
-constexpr int kCtasPerSm = GMPI_CTAS_PER_SM;
+constexpr int kMaxPlanesStaged = 512;   // plane-constant table: 32 B per plane in shared memory
 constexpr int kStageFloats = kMaxBW * kMaxBH * 4;
 constexpr size_t kStagedSmem = (size_t)kStages * kStageFloats * 4 + (size_t)kMaxPlanesStaged * 32;
 // Factored forward: box widths 64 and 96 only.  Its boxes are [row][3][bw] (colour) and [row][bw] (alpha): row pitches of 3 bw and
@@ -291,28 +280,23 @@ __device__ __forceinline__ void consumer_idle_tile(uint64_t* s_full, uint64_t* s
 // this CTA, estimate the tile's texel footprint from its four corner rays, pick the narrowest box class, publish the stage
 // header and issue the TMA copies.
 // Ring geometry of a kernel: tile height, ring depth, the largest staged box and what a stage holds.
-struct FwdRing {
+struct FwdRing {          // the expanded forward's ring
     static constexpr int kTileRows = kTileH, kRingStages = kStages, kBoxMaxH = kMaxBH;
     static constexpr int kPlaneFloats = kStageFloats;      // floats of one staged plane box
     static constexpr int kStride = kStageFloats;           // floats per ring stage
     static constexpr bool kReverse = false;                // planes front to back; no transmittance box
-#ifndef GMPI_FWD_SLEEP
-#define GMPI_FWD_SLEEP 0      // measured: sleeping between polls costs the forward 1 % (the 3-stage ring wants its producer prompt)
-#endif
-    static constexpr bool kSleepPolls = GMPI_FWD_SLEEP != 0;   // producer sleeps between polls of a full ring (see mbar_wait_sleep)
+    // producer sleeps between polls of a full ring (see mbar_wait_sleep).  Measured: sleeping costs the forward 1 % (the 3-stage
+    // ring wants its producer prompt)
+    static constexpr bool kSleepPolls = false;
     static constexpr bool kWideFact = false;
     static constexpr bool kBinaryCopies = true;            // expanded MPI: copies of 32/16/8/4 rows (see staged_producer)
-    static constexpr int kColourCopyRows = kMaxBH;         // factored MPI (only with GMPI_FWD_WIDE_FACT=0): one colour copy
 };
-#ifndef GMPI_FWD_WIDE_FACT
-#define GMPI_FWD_WIDE_FACT 1
-#endif
 static_assert(kMaxBH % 2 == 0 && kMaxBH / kRowsPerOp < 16, "half-height colour copies; binary digits of the chunk count");
 struct FwdRingWide {      // the factored forward's ring: 64- or 96-wide boxes (see kWideBW)
     static constexpr int kTileRows = kTileH, kRingStages = kStages, kBoxMaxH = kMaxBH;
     static constexpr int kPlaneFloats = kWideStageFloats, kStride = kWideStageFloats;
     static constexpr bool kReverse = false;
-    static constexpr bool kSleepPolls = GMPI_FWD_SLEEP != 0;
+    static constexpr bool kSleepPolls = false;
     static constexpr bool kWideFact = true;
     static constexpr bool kBinaryCopies = true;
     // factored MPI: colour box = 2 copies of 22 rows.  A copy lands at row offset r * 3 * bw * 4 bytes, which must be a multiple
@@ -332,14 +316,9 @@ __host__ __device__ __forceinline__ int binary_copy_of_lane(int n_chunks, int la
     return ((n_chunks >> bit) & 1) << bit;
 }
 
-struct NoPacer { static constexpr bool kActive = false; };      // the forward's producer has no side job
-
-// Pacer: an optional side job of the producer warp (the backward's gradient zeroing): before_tile(mpi) ahead of a tile's first
-// copy; new_stage() then chunk() between the polls of the wait for a free ring stage (chunk() returns false when there is nothing
-// to do); at_end() after the last tile.
-template <bool kAlignCorners, class Ring, bool kFact, class Pacer>
+template <bool kAlignCorners, class Ring, bool kFact>
 __device__ __forceinline__ void staged_producer(const RenderParams& p, const TmaMaps& maps, float* s_buf, StageMeta* s_meta,
-                                            uint64_t* s_full, uint64_t* s_empty, const TileWalk* s_walk, int lane, Pacer& pacer) {
+                                            uint64_t* s_full, uint64_t* s_empty, const TileWalk* s_walk, int lane) {
     constexpr bool kReverse = Ring::kReverse;
     constexpr int kStride = Ring::kStride;      // floats per ring stage
     constexpr int kTileH = Ring::kTileRows, kStages = Ring::kRingStages, kMaxBH = Ring::kBoxMaxH, kStageFloats = Ring::kPlaneFloats;
@@ -358,7 +337,6 @@ __device__ __forceinline__ void staged_producer(const RenderParams& p, const Tma
     for (int j = 0; s_walk->at(j, txy); ++j) {
         const int v = txy.v, px0 = txy.px0, py0 = txy.py0;
         const int m = __ldg(p.view2mpi + v);
-        if constexpr (Pacer::kActive) pacer.before_tile(m);
         float ev[3], zd[3];
         load_eye_z(p, v, ev, zd);
         // the four corner pixels of the tile (replicated over the warp), clamped into the image
@@ -394,15 +372,8 @@ __device__ __forceinline__ void staged_producer(const RenderParams& p, const Tma
             const int bw = (kWide && k == 4) ? kWideBW : kMinBW + k * kBWStep;
             const int n_ops = mode == 0 ? (need_h + kRowsPerOp - 1) / kRowsPerOp : 0;
             const int rows = n_ops * kRowsPerOp;
-            if constexpr (Pacer::kActive) {      // the side job fills the wait for a free stage, a few stores between polls
-                pacer.new_stage();
-                while (!mbar_try_wait(&s_empty[s], ph ^ 1))
-                    if (!pacer.chunk()) __nanosleep(96);
-            } else if (Ring::kSleepPolls) {
-                mbar_wait_sleep(&s_empty[s], ph ^ 1);
-            } else {
-                mbar_wait(&s_empty[s], ph ^ 1);
-            }
+            if (Ring::kSleepPolls) mbar_wait_sleep(&s_empty[s], ph ^ 1);
+            else mbar_wait(&s_empty[s], ph ^ 1);
             if (lane == 0) {
                 StageMeta mt;
                 mt.cx = kFloorMagicBits + bx0; mt.cy = kFloorMagicBits + by0;
@@ -421,7 +392,7 @@ __device__ __forceinline__ void staged_producer(const RenderParams& p, const Tma
             // 4-row copy per lane (9-11 per stage, twice that for the factored MPI) the producer was the bottleneck of its own ring.
             if (n_ops > 0) {
                 float* stage = s_buf + (size_t)s * kStride;
-                if (kFact) {
+                if constexpr (kFact) {
                     // factored MPI: the colour box (shared image, or the last plane's own) as two or three copies that tile the
                     // ring's box height, the alpha box as one copy of the full height.  Rows beyond the footprint are fetched and never
                     // read: the colour image is shared by all planes and comes from L2, alpha is a quarter of the bytes.
@@ -447,7 +418,6 @@ __device__ __forceinline__ void staged_producer(const RenderParams& p, const Tma
             }
         }
     }
-    if constexpr (Pacer::kActive) pacer.at_end();
 }
 
 // 4x4 transpose inside every quad of lanes (4 q .. 4 q + 3): on entry lane k of a quad holds a[c] = M[k][c], on return
@@ -500,15 +470,12 @@ __device__ __forceinline__ void store_tile_pixels(const RenderParams& p, int v, 
     store_pixel(p, v, img, (size_t)py * p.W + px, o[0], o[1], o[2], o[3]);
 }
 
-template <bool kFactored>
-using FwdRingFor = typename std::conditional<kFactored && GMPI_FWD_WIDE_FACT != 0, FwdRingWide, FwdRing>::type;
-
 template <bool kAlignCorners, bool kEmitT, bool kFactored>
-__global__ void __launch_bounds__(kStagedThreads, kCtasPerSm)
+__global__ void __launch_bounds__(kStagedThreads, 1)
 mpi_fwd_staged_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps, const int tiles_x, const int tiles_y) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     float* s_buf = reinterpret_cast<float*>(smem_raw);   // the ring starts the dynamic segment (1024-byte aligned)
-    using Ring = FwdRingFor<kFactored>;
+    using Ring = typename std::conditional<kFactored, FwdRingWide, FwdRing>::type;
     constexpr int kRingFloats = Ring::kPlaneFloats;         // floats per ring stage
     constexpr int kAOff = kFactored ? 3 * (kRingFloats / 4) : 0;      // factored: alpha box behind the colour box
     PlaneConst* s_pc = reinterpret_cast<PlaneConst*>(smem_raw + (size_t)kStages * kRingFloats * 4);   // [N] of the current view
@@ -539,8 +506,7 @@ mpi_fwd_staged_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps
     const size_t img = (size_t)p.H * p.W;
 
     if (warp == kConsWarps) {
-        NoPacer np;
-        staged_producer<kAlignCorners, Ring, kFactored>(p, maps, s_buf, s_meta, s_full, s_empty, &s_walk, lane, np);
+        staged_producer<kAlignCorners, Ring, kFactored>(p, maps, s_buf, s_meta, s_full, s_empty, &s_walk, lane);
     } else {
         // ================================ consumer warps ================================
         // warp w owns rows kPairs*w .. kPairs*w + kPairs-1 of the tile; a lane owns x = lane and lane+32 on each of them

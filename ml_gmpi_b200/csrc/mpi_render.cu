@@ -402,7 +402,7 @@ static int device_sms(int* sms) {
 template <bool AC, bool EMIT, bool FAC>
 static cudaError_t launch_fwd_staged(const RenderParams& p, const TmaMaps& maps, int grid, int tiles_x, int tiles_y, cudaStream_t st) {
     auto kernel = mpi_fwd_staged_kernel<AC, EMIT, FAC>;
-    constexpr size_t smem = FwdRingFor<FAC>::kWideFact ? kStagedSmemWide : kStagedSmem;
+    constexpr size_t smem = FAC ? kStagedSmemWide : kStagedSmem;
     cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     kernel<<<grid, kStagedThreads, smem, st>>>(p, maps, tiles_x, tiles_y);
@@ -431,14 +431,14 @@ static int launch_fwd(RenderParams p, cudaStream_t st) {
     const bool ac = (p.options & GMPI_ALIGN_CORNERS) != 0, emit = p.transmittance != nullptr, fac = p.alpha != nullptr;
     if (staged_eligible(p.V, p.N, p.Ht, p.Wt, p.H, p.W) && mpi_aligned(p) && (size_t)p.M * p.N < ((size_t)1 << 31)) {
         TmaMaps maps;
-        if (encode_mpi_maps(maps, p, kMaxBH, FwdRingFor<true>::kColourCopyRows, fac && FwdRingFor<true>::kWideFact) != 0) {
+        if (encode_mpi_maps(maps, p, kMaxBH, FwdRingWide::kColourCopyRows, fac) != 0) {
             if (g_fwd_variant.load(std::memory_order_relaxed) == 2) return fail(GMPI_ERR_CUDA, "cuTensorMapEncodeTiled failed");
         } else {
             int sms = 0;
             if ((rc = device_sms(&sms)) != 0) return rc;
             const int tiles_x = (p.W + kTileW - 1) / kTileW, tiles_y = (p.H + kTileH - 1) / kTileH;
             const long n_tiles = (long)tiles_x * tiles_y * p.V;
-            const int grid = (int)(n_tiles < (long)sms * kCtasPerSm ? n_tiles : (long)sms * kCtasPerSm);
+            const int grid = (int)(n_tiles < sms ? n_tiles : sms);
             cudaError_t e;
             if (fac) {
                 if (ac && emit) e = launch_fwd_staged<true, true, true>(p, maps, grid, tiles_x, tiles_y, st);
@@ -475,8 +475,6 @@ static int launch_fwd(RenderParams p, cudaStream_t st) {
     GMPI_CUDA_OK(cudaGetLastError());
     return GMPI_OK;
 }
-
-static std::atomic<int> g_bwd_zero_in_kernel{0};      // 1: GMPI_ZERO_GRAD inside the staged backward kernel (gmpi_debug_set_bwd_zero; measured slower)
 
 static int zero_grads(const RenderParams& p, cudaStream_t st) {
     const size_t tex = (size_t)p.Ht * p.Wt;
@@ -553,41 +551,10 @@ static int launch_bwd(RenderParams p, cudaStream_t st) {
     const long n_tiles = (long)tiles_x * tiles_y * p.V;
     const int grid = (int)(n_tiles < sms ? n_tiles : sms);
     const bool ac = (p.options & GMPI_ALIGN_CORNERS) != 0;
-    // GMPI_ZERO_GRAD: stream memsets before the kernel (default), or -- gmpi_debug_set_bwd_zero(1) -- the kernel zeroes the large
-    // buffer (g_rgba / g_alpha) itself, one MPI slab ahead of the tiles that add to it (GradZeroPacer, measured 4.5 % slower); the
-    // small factored colour gradients and the counters then take stream-ordered memsets.
-    unsigned* zero_flags = nullptr;
-    if (p.options & GMPI_ZERO_GRAD) {
-        const size_t tex = (size_t)p.Ht * p.Wt;
-        if (g_bwd_zero_in_kernel.load(std::memory_order_relaxed) &&
-            cudaMallocAsync(reinterpret_cast<void**>(&zero_flags), sizeof(unsigned) * (size_t)p.M, st) == cudaSuccess) {
-            cudaError_t ez = cudaMemsetAsync(zero_flags, 0, sizeof(unsigned) * (size_t)p.M, st);
-            if (ez == cudaSuccess && fac) {
-                ez = cudaMemsetAsync(p.g_rgb, 0, sizeof(float) * (size_t)p.M * 3 * tex, st);
-                if (ez == cudaSuccess && p.g_bg_rgb) ez = cudaMemsetAsync(p.g_bg_rgb, 0, sizeof(float) * (size_t)p.M * 3 * tex, st);
-            }
-            if (ez != cudaSuccess) {
-                (void)cudaFreeAsync(zero_flags, st);
-                GMPI_CUDA_OK(ez);
-            }
-            p.zero_base = reinterpret_cast<float4*>(fac ? p.g_alpha : p.g_rgba);
-            p.zero_slab16 = (unsigned long long)p.N * (fac ? 1 : 4) * tex / 4;            // Wt % 4 == 0: whole float4s
-            p.zero_flags = zero_flags;
-            // pace: a CTA's share of one slab within half of the stages it spends on one MPI's tiles
-            const double stages_per_mpi = (double)n_tiles / p.M / grid * p.N;
-            const double stores = (double)p.zero_slab16 / grid / 32.0;
-            double rate = stores / (0.5 * stages_per_mpi > 1.0 ? 0.5 * stages_per_mpi : 1.0);
-            p.zero_rate = rate < 4.0 ? 4 : rate > 4096.0 ? 4096 : (int)rate + 1;
-        } else {
-            (void)cudaGetLastError();
-            zero_flags = nullptr;
-            if ((rc = zero_grads(p, st)) != 0) return rc;
-        }
-    }
+    if ((p.options & GMPI_ZERO_GRAD) && (rc = zero_grads(p, st)) != 0) return rc;
     cudaError_t e;
     if (fac) e = ac ? launch_bwd_box<true, true>(p, maps, grid, tiles_x, tiles_y, st) : launch_bwd_box<false, true>(p, maps, grid, tiles_x, tiles_y, st);
     else e = ac ? launch_bwd_box<true, false>(p, maps, grid, tiles_x, tiles_y, st) : launch_bwd_box<false, false>(p, maps, grid, tiles_x, tiles_y, st);
-    if (zero_flags) (void)cudaFreeAsync(zero_flags, st);
     GMPI_CUDA_OK(e);
     GMPI_CUDA_OK(cudaGetLastError());
     return GMPI_OK;
@@ -630,11 +597,6 @@ extern "C" {
 int gmpi_abi_version(void) { return GMPI_ABI_VERSION; }
 
 const char* gmpi_last_error(void) { return g_err; }
-
-int gmpi_debug_set_bwd_zero(int in_kernel) {
-    g_bwd_zero_in_kernel.store(in_kernel != 0, std::memory_order_relaxed);
-    return GMPI_OK;
-}
 
 int gmpi_debug_set_fwd_variant(int variant) {
     if (variant < 0 || variant > 2) return fail(GMPI_ERR_INVALID_ARGUMENT, "variant must be 0 (auto), 1 (direct) or 2 (staged)");

@@ -1,8 +1,7 @@
 #!/usr/bin/env python
-"""Where does the zeroing of the gradient go?  CUDA-event times on the headline train shape (4 MPIs x 1 view, 96 planes, 1024^2):
-(1) the training-mode forward alone, a memset of the gradient alone, and both at once on two streams -- does a memset overlap a
-persistent kernel?  (2) the whole train step with GMPI_ZERO_GRAD as stream memsets before the backward kernel, and with the
-backward kernel zeroing the gradient itself, one MPI slab ahead of use (opt-in).   python tools/zero_overlap_probe.py"""
+"""Does a memset of the gradient overlap a persistent kernel?  CUDA-event times on the headline train shape (4 MPIs x 1 view,
+96 planes, 1024^2): the training-mode forward alone, a memset of the gradient alone, and both at once on two streams.
+python tools/zero_overlap_probe.py"""
 import sys
 
 import torch
@@ -14,7 +13,6 @@ from ml_gmpi_b200 import _lib, synth         # noqa: E402
 dev = torch.device("cuda:0")
 case = synth.make_case(device=dev, n_mpi=4, views_per_mpi=1, n_planes=96, tex=1024, img=1024, seed=0)
 rg = case.rgba.requires_grad_(True)
-gcol = torch.randn((4, 3, 1024, 1024), device=dev)
 lib = _lib.load()
 side = torch.cuda.Stream(device=dev)
 main = torch.cuda.current_stream(dev)
@@ -51,14 +49,5 @@ def both():
     fwd()
 
 
-def step():
-    rg.grad = None
-    (fwd() * gcol).sum().backward()
-
-
 t_fwd, t_zero, t_both = timed(fwd), timed(zero_side), timed(both)
 print(f"forward(train) alone {t_fwd:.3f} ms; memset alone {t_zero:.3f} ms; both on two streams {t_both:.3f} ms (sum {t_fwd + t_zero:.3f})")
-for mode in (0, 1, 0, 1):
-    lib.gmpi_debug_set_bwd_zero(mode)
-    print(f"train step, gradient zeroed {'inside the backward kernel' if mode else 'by memsets before the backward kernel'}: {timed(step, n=5):.3f} ms")
-lib.gmpi_debug_set_bwd_zero(0)
