@@ -3,7 +3,7 @@
 // One CTA per SM walks (tile, plane) pairs: a 64x30-pixel output tile, planes front to back.  A producer warp computes,
 // from the tile's four corner rays, the texel footprint of the tile on the next plane and issues cp.async.bulk.tensor
 // copies of exactly that footprint (all four channels, rows in units of 4 issued as a few tall copies, origin aligned to 16 bytes,
-// width rounded up to one of five compile-time classes) into a 3-stage shared-memory ring; 15 consumer warps (4 pixels = 2 pixel pairs per
+// width rounded up to one of five compile-time classes) into a 2- or 3-stage shared-memory ring; 15 consumer warps (4 pixels = 2 pixel pairs per
 // thread) take their 16 bilinear taps per pixel and plane from shared memory (a warp reads 32 consecutive x of one row:
 // conflict-free while the texel/pixel scale is <= 1) and composite in registers.  TMA's out-of-bounds zero fill implements
 // padding_mode="zeros".  Every consumer warp verifies (one vote) that all its taps lie inside the staged box; otherwise it
@@ -21,7 +21,9 @@ constexpr int kPairs = 2;        // packed pixel pairs per thread (each pair = x
 constexpr int kPix = 2 * kPairs;
 constexpr int kTileW = 64, kTileH = kPairs * kConsWarps;
 constexpr int kConsThreads = kConsWarps * 32, kStagedThreads = kConsThreads + 32;
-constexpr int kStages = 3;
+// Ring depth of the expanded forward, chosen at launch (fwd_ring_stages): kStages when the boxes come from L2, kStreamStages
+// when they stream from HBM.  DESIGN.md section 4.1 has the measurements.
+constexpr int kStages = 3, kStreamStages = 2;
 constexpr int kRowsPerOp = 4;
 constexpr int kMaxBW = 88;
 constexpr int kMaxBH = (((kTileH * 5) / 4 + 6 + kRowsPerOp - 1) / kRowsPerOp) * kRowsPerOp;   // footprint rows at scale 1.25 + taps/slack, whole chunks                 // largest staged footprint (texels)
@@ -31,7 +33,6 @@ constexpr int kMinBW = 56, kBWStep = 8;
 constexpr int kNumMaps = (kMaxBW - kMinBW) / kBWStep + 1;
 constexpr int kMaxPlanesStaged = 512;   // plane-constant table: 32 B per plane in shared memory
 constexpr int kStageFloats = kMaxBW * kMaxBH * 4;
-constexpr size_t kStagedSmem = (size_t)kStages * kStageFloats * 4 + (size_t)kMaxPlanesStaged * 32;
 // Factored forward: box widths 64 and 96 only.  Its boxes are [row][3][bw] (colour) and [row][bw] (alpha): row pitches of 3 bw and
 // bw words, and only a pitch that is a multiple of the 32 banks keeps a warp whose 32 taps straddle two texture rows (any rotated
 // view) at one wavefront per LDS -- the expanded box [row][4][bw] has that for every bw % 8 == 0.
@@ -265,11 +266,12 @@ struct TileWalk {
 };
 
 // A consumer warp without a single row inside the image: hand every stage of this tile straight back to the producer.
-__device__ __forceinline__ void consumer_idle_tile(uint64_t* s_full, uint64_t* s_empty, int N, int lane, int& c_stage, uint32_t& c_phase) {
+__device__ __forceinline__ void consumer_idle_tile(uint64_t* s_full, uint64_t* s_empty, int N, int n_stages, int lane, int& c_stage,
+                                                   uint32_t& c_phase) {
     for (int i = 0; i < N; ++i) {
         const int s = c_stage;
         const uint32_t ph = c_phase;
-        if (++c_stage == kStages) { c_stage = 0; c_phase ^= 1u; }
+        if (++c_stage == n_stages) { c_stage = 0; c_phase ^= 1u; }
         mbar_wait(&s_full[s], ph);
         __syncwarp();
         mbar_arrive_if(&s_empty[s], lane == 0);
@@ -285,7 +287,7 @@ struct FwdRing {          // the expanded forward's ring
     static constexpr int kPlaneFloats = kStageFloats;      // floats of one staged plane box
     static constexpr int kStride = kStageFloats;           // floats per ring stage
     static constexpr bool kReverse = false;                // planes front to back; no transmittance box
-    // producer sleeps between polls of a full ring (see mbar_wait_sleep).  Measured: sleeping costs the forward 1 % (the 3-stage
+    // producer sleeps between polls of a full ring (see mbar_wait_sleep).  Measured: sleeping costs the forward 1 % (a shallow
     // ring wants its producer prompt)
     static constexpr bool kSleepPolls = false;
     static constexpr bool kWideFact = false;
@@ -306,7 +308,7 @@ struct FwdRingWide {      // the factored forward's ring: 64- or 96-wide boxes (
 // factored MPI: the colour box [row][3][bw] starts the stage, the alpha box [row][bw] follows after 3/4 of the stage
 
 // kFact: factored MPI (compile time: a run-time test of p.alpha in this loop cost the forward 1 %, the producer's per-stage latency
-// being on the critical path of a three-stage ring).
+// being on the critical path of a shallow ring).
 // The expanded forward's copies of one stage: the footprint's n_chunks 4-row chunks as the binary digits of n_chunks.  Lane 0..3
 // owns the digit 8, 4, 2, 1: returns the copy's height in chunks (0: this lane issues nothing) and, in `before`, the chunks
 // covered by the taller copies, i.e. where this copy starts.  (Host-evaluable: gmpi_debug_copy_plan, tests/test_tile_walk.py.)
@@ -318,7 +320,8 @@ __host__ __device__ __forceinline__ int binary_copy_of_lane(int n_chunks, int la
 
 template <bool kAlignCorners, class Ring, bool kFact>
 __device__ __forceinline__ void staged_producer(const RenderParams& p, const TmaMaps& maps, float* s_buf, StageMeta* s_meta,
-                                            uint64_t* s_full, uint64_t* s_empty, const TileWalk* s_walk, int lane) {
+                                            uint64_t* s_full, uint64_t* s_empty, const TileWalk* s_walk, int lane,
+                                            int n_stages = Ring::kRingStages) {
     constexpr bool kReverse = Ring::kReverse;
     constexpr int kStride = Ring::kStride;      // floats per ring stage
     constexpr int kTileH = Ring::kTileRows, kStages = Ring::kRingStages, kMaxBH = Ring::kBoxMaxH, kStageFloats = Ring::kPlaneFloats;
@@ -349,7 +352,7 @@ __device__ __forceinline__ void staged_producer(const RenderParams& p, const Tma
             const int i = kReverse ? N - 1 - ii : ii;
             const int s = p_stage;
             const uint32_t ph = p_phase;
-            if (++p_stage == kStages) { p_stage = 0; p_phase ^= 1u; }
+            if (++p_stage == n_stages) { p_stage = 0; p_phase ^= 1u; }
             const PlaneConst pc = make_plane_const(p.dhw + ((size_t)m * N + i) * 3, ev[2]);
             const TexCoord tc = plane_coord<kAlignCorners>(pc, rc, hsx, hsy, fWt, fHt);
             // footprint of the tile = bounding box of the corner coordinates (the pixel -> texel map is projective,
@@ -472,13 +475,16 @@ __device__ __forceinline__ void store_tile_pixels(const RenderParams& p, int v, 
 
 template <bool kAlignCorners, bool kEmitT, bool kFactored>
 __global__ void __launch_bounds__(kStagedThreads, 1)
-mpi_fwd_staged_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps, const int tiles_x, const int tiles_y) {
+mpi_fwd_staged_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps, const int tiles_x, const int tiles_y,
+                      const int ring_stages) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     float* s_buf = reinterpret_cast<float*>(smem_raw);   // the ring starts the dynamic segment (1024-byte aligned)
     using Ring = typename std::conditional<kFactored, FwdRingWide, FwdRing>::type;
+    constexpr int kStages = Ring::kRingStages;              // ring stages allocated; the expanded MPI uses ring_stages of them
+    const int n_stages = kFactored ? kStages : ring_stages;
     constexpr int kRingFloats = Ring::kPlaneFloats;         // floats per ring stage
     constexpr int kAOff = kFactored ? 3 * (kRingFloats / 4) : 0;      // factored: alpha box behind the colour box
-    PlaneConst* s_pc = reinterpret_cast<PlaneConst*>(smem_raw + (size_t)kStages * kRingFloats * 4);   // [N] of the current view
+    PlaneConst* s_pc = reinterpret_cast<PlaneConst*>(smem_raw + (size_t)n_stages * kRingFloats * 4);   // [N] of the current view
     __shared__ StageMeta s_meta[kStages];
     __shared__ __align__(8) uint64_t s_full[kStages], s_empty[kStages];
     __shared__ TileWalk s_walk;
@@ -486,7 +492,7 @@ mpi_fwd_staged_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (threadIdx.x == 0) {
         s_walk.init(tiles_x, p.H, p.V, (int)blockIdx.x, (int)gridDim.x, kTileH, p.view_group);
-        for (int s = 0; s < kStages; ++s) {
+        for (int s = 0; s < n_stages; ++s) {
             mbar_init(&s_full[s], 1);
             mbar_init(&s_empty[s], kConsWarps);
         }
@@ -506,7 +512,7 @@ mpi_fwd_staged_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps
     const size_t img = (size_t)p.H * p.W;
 
     if (warp == kConsWarps) {
-        staged_producer<kAlignCorners, Ring, kFactored>(p, maps, s_buf, s_meta, s_full, s_empty, &s_walk, lane);
+        staged_producer<kAlignCorners, Ring, kFactored>(p, maps, s_buf, s_meta, s_full, s_empty, &s_walk, lane, n_stages);
     } else {
         // ================================ consumer warps ================================
         // warp w owns rows kPairs*w .. kPairs*w + kPairs-1 of the tile; a lane owns x = lane and lane+32 on each of them
@@ -535,7 +541,7 @@ mpi_fwd_staged_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps
                 v_table = v;
             }
             if (py0 + kPairs * warp >= p.H) {      // warp-uniform: no row of this warp is inside the image
-                consumer_idle_tile(s_full, s_empty, N, lane, c_stage, c_phase);
+                consumer_idle_tile(s_full, s_empty, N, n_stages, lane, c_stage, c_phase);
                 continue;
             }
             RayConst rc[kPix];   // scalar copies, only for the generic (rare) body and the epilogue
@@ -567,7 +573,7 @@ mpi_fwd_staged_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps
             for (int i = 0; i < N; ++i) {
                 const int s = c_stage;
                 const uint32_t ph = c_phase;
-                if (++c_stage == kStages) { c_stage = 0; c_phase ^= 1u; }
+                if (++c_stage == n_stages) { c_stage = 0; c_phase ^= 1u; }
                 const PlaneConst pcc = pc_next;            // loaded one plane ahead: no shared-memory latency in front of the
                 pc_next = s_pc[min(i + 1, N - 1)];         // coordinate chain (+1.3 %)
                 CoordPairs cc;

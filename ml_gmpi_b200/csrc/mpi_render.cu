@@ -399,13 +399,23 @@ static int device_sms(int* sms) {
     return GMPI_OK;
 }
 
+// Ring depth of the expanded forward.  When every view has an MPI of its own that is larger than L2, each box streams from
+// HBM, and a shallower ring is faster: 2 stages take 0.85x the time of 3 at 4 MPIs x 96 planes x 1024^2, 4 stages 1.10x.
+// When the boxes come from L2 (views sharing an MPI, or an MPI that fits L2) 3 stages are faster (DESIGN.md section 4.1).
+static int fwd_ring_stages(const RenderParams& p, int l2_bytes) {
+    const bool shared_mpi = p.view_group > 1 || p.V > p.M;
+    const bool fits_l2 = (double)p.N * p.Ht * p.Wt * 16.0 <= (double)l2_bytes;
+    return shared_mpi || fits_l2 ? kStages : kStreamStages;
+}
+
 template <bool AC, bool EMIT, bool FAC>
-static cudaError_t launch_fwd_staged(const RenderParams& p, const TmaMaps& maps, int grid, int tiles_x, int tiles_y, cudaStream_t st) {
+static cudaError_t launch_fwd_staged(const RenderParams& p, const TmaMaps& maps, int grid, int tiles_x, int tiles_y, int stages,
+                                     cudaStream_t st) {
     auto kernel = mpi_fwd_staged_kernel<AC, EMIT, FAC>;
-    constexpr size_t smem = FAC ? kStagedSmemWide : kStagedSmem;
+    const size_t smem = FAC ? kStagedSmemWide : (size_t)stages * kStageFloats * 4 + (size_t)kMaxPlanesStaged * 32;
     cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
-    kernel<<<grid, kStagedThreads, smem, st>>>(p, maps, tiles_x, tiles_y);
+    kernel<<<grid, kStagedThreads, smem, st>>>(p, maps, tiles_x, tiles_y, stages);
     return cudaSuccess;
 }
 
@@ -434,22 +444,25 @@ static int launch_fwd(RenderParams p, cudaStream_t st) {
         if (encode_mpi_maps(maps, p, kMaxBH, FwdRingWide::kColourCopyRows, fac) != 0) {
             if (g_fwd_variant.load(std::memory_order_relaxed) == 2) return fail(GMPI_ERR_CUDA, "cuTensorMapEncodeTiled failed");
         } else {
-            int sms = 0;
+            int sms = 0, dev = 0, l2 = 0;
             if ((rc = device_sms(&sms)) != 0) return rc;
+            GMPI_CUDA_OK(cudaGetDevice(&dev));
+            GMPI_CUDA_OK(cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, dev));
+            const int stages = fwd_ring_stages(p, l2);
             const int tiles_x = (p.W + kTileW - 1) / kTileW, tiles_y = (p.H + kTileH - 1) / kTileH;
             const long n_tiles = (long)tiles_x * tiles_y * p.V;
             const int grid = (int)(n_tiles < sms ? n_tiles : sms);
             cudaError_t e;
             if (fac) {
-                if (ac && emit) e = launch_fwd_staged<true, true, true>(p, maps, grid, tiles_x, tiles_y, st);
-                else if (ac) e = launch_fwd_staged<true, false, true>(p, maps, grid, tiles_x, tiles_y, st);
-                else if (emit) e = launch_fwd_staged<false, true, true>(p, maps, grid, tiles_x, tiles_y, st);
-                else e = launch_fwd_staged<false, false, true>(p, maps, grid, tiles_x, tiles_y, st);
+                if (ac && emit) e = launch_fwd_staged<true, true, true>(p, maps, grid, tiles_x, tiles_y, stages, st);
+                else if (ac) e = launch_fwd_staged<true, false, true>(p, maps, grid, tiles_x, tiles_y, stages, st);
+                else if (emit) e = launch_fwd_staged<false, true, true>(p, maps, grid, tiles_x, tiles_y, stages, st);
+                else e = launch_fwd_staged<false, false, true>(p, maps, grid, tiles_x, tiles_y, stages, st);
             } else {
-                if (ac && emit) e = launch_fwd_staged<true, true, false>(p, maps, grid, tiles_x, tiles_y, st);
-                else if (ac) e = launch_fwd_staged<true, false, false>(p, maps, grid, tiles_x, tiles_y, st);
-                else if (emit) e = launch_fwd_staged<false, true, false>(p, maps, grid, tiles_x, tiles_y, st);
-                else e = launch_fwd_staged<false, false, false>(p, maps, grid, tiles_x, tiles_y, st);
+                if (ac && emit) e = launch_fwd_staged<true, true, false>(p, maps, grid, tiles_x, tiles_y, stages, st);
+                else if (ac) e = launch_fwd_staged<true, false, false>(p, maps, grid, tiles_x, tiles_y, stages, st);
+                else if (emit) e = launch_fwd_staged<false, true, false>(p, maps, grid, tiles_x, tiles_y, stages, st);
+                else e = launch_fwd_staged<false, false, false>(p, maps, grid, tiles_x, tiles_y, stages, st);
             }
             GMPI_CUDA_OK(e);
             GMPI_CUDA_OK(cudaGetLastError());
