@@ -278,6 +278,14 @@ int gmpi_debug_plane_coords_packed(const int32_t* view2mpi, const float* dhw, co
 /* Test hook: force the forward kernel variant: 0 auto (default), 1 direct-gather, 2 TMA-staged. */
 int gmpi_debug_set_fwd_variant(int variant);
 
+/* Test hook: force the ring depth of the expanded TMA-staged forward: 0 auto (default), 2 or 3 stages.  The factored forward
+ * keeps its 3-stage ring. */
+int gmpi_debug_set_fwd_stages(int stages);
+
+/* Test hook: the ring depth (2 or 3) the expanded staged forward picks on the current device for M MPIs, V views, N planes of
+ * Ht x Wt texels and view_group (gmpi_render_desc.view_group); a negative GMPI_ERR_* code on bad arguments. */
+int gmpi_debug_fwd_ring_stages(int M, int V, int N, int Ht, int Wt, int view_group);
+
 /* Test hook (host only): the TMA copies the expanded forward issues for a footprint of n_rows staged rows, as (first row, rows)
  * pairs: the binary digits of n_rows / 4 (copies of 32, 16, 8, 4 rows).  Returns the number of copies. */
 int gmpi_debug_copy_plan(int n_rows, int* out_row_rows, int max_copies);

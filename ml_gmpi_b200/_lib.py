@@ -27,7 +27,7 @@ EXPORTS = [
     "gmpi_abi_version", "gmpi_last_error", "gmpi_mpi_render_fwd_variant", "gmpi_mpi_render_fwd",
     "gmpi_mpi_render_fwd_gather", "gmpi_mpi_render_fwd_train", "gmpi_mpi_render_bwd", "gmpi_mpi_render_bwd_saved", "gmpi_mpi_check_range", "gmpi_mpi_render_fwd_host", "gmpi_mpi_release_host_cache", "gmpi_debug_plane_coords", "gmpi_debug_division", "gmpi_debug_set_fwd_variant", "gmpi_debug_copy_plan", "gmpi_debug_plane_coords_packed", "gmpi_debug_tile_walk",
     "gmpi_mpi_render_fwd_plan", "gmpi_mpi_render_fwd_ex", "gmpi_mpi_render_bwd_ex", "gmpi_mpi_render_host_ex",
-    "gmpi_debug_tile_walk_ex", "gmpi_debug_cam_rays",
+    "gmpi_debug_tile_walk_ex", "gmpi_debug_cam_rays", "gmpi_debug_set_fwd_stages", "gmpi_debug_fwd_ring_stages",
     "gmpi_mpi_zero_async", "gmpi_mpi_alpha_depth_fwd", "gmpi_mpi_alpha_depth_bwd", "gmpi_mpi_apply_shading_fwd", "gmpi_mpi_apply_shading_bwd",
 ]
 
@@ -109,6 +109,10 @@ def load():
     lib.gmpi_debug_division.argtypes = [vp, vp, vp, vp, ctypes.c_size_t, vp]
     lib.gmpi_debug_set_fwd_variant.restype = i
     lib.gmpi_debug_set_fwd_variant.argtypes = [i]
+    lib.gmpi_debug_set_fwd_stages.restype = i
+    lib.gmpi_debug_set_fwd_stages.argtypes = [i]
+    lib.gmpi_debug_fwd_ring_stages.restype = i
+    lib.gmpi_debug_fwd_ring_stages.argtypes = [i] * 6
     lib.gmpi_debug_copy_plan.restype = i
     lib.gmpi_debug_copy_plan.argtypes = [i, vp, i]
     lib.gmpi_debug_tile_walk.restype = i

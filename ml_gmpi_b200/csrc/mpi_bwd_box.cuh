@@ -53,6 +53,18 @@ struct BwdRing {
     // i.e. r a multiple of 4; 18-row halves gave cudaErrorMisalignedAddress)
     static constexpr int kColourCopyRows = 12;
     static_assert(kBwdMaxBH % kColourCopyRows == 0 && kColourCopyRows % 4 == 0, "colour copies tile the box, 128-byte aligned");
+    // Magnification limit of the gradient box.  A fixed-point contribution is |c| 2^(kFixBits - e) < 2^25 w for alpha (2^21 w for
+    // colour; w = the tap's bilinear weight, see tile_scale_exponent), plus 1/2 of rounding, and a tile has 64 x 24 = 1536 pixels:
+    // a texel's int32 sum cannot wrap while the bilinear weights it collects from one tile add up to at most 63.  Over one tile a
+    // pinhole camera maps pixels to texels at a nearly uniform scale of s texels per pixel, and one texel's weights summed along a
+    // pixel row are at most 1/s + 1 (samples of a unit-area tent at spacing s); so the sum is at most (1/s + 1)^2 <= 49 when
+    // s >= 1/kMagLimit.  The producer estimates s per (tile, plane) from the floored corner coordinates: a span of d texels over
+    // ext pixels has s >= (d - 1) / ext.  It publishes a stage with kMagLimit (d - 1) < ext in either direction as not usable by
+    // the fast body, which then takes the generic body (fp32 red.global.add, no limit).  The margin from 49 to 63 covers a rolled
+    // camera (the corner box overstates s by up to 6 %) and the perspective change of s across a tile.  Magnifications beyond
+    // about 6x (a 64^2 texture rendered at 512^2) pay for it; ray tensors that are not a pinhole camera's are judged by their
+    // corner rays like any other footprint.
+    static constexpr int kMagLimit = 6;
 };
 
 struct GradPairs {
@@ -115,9 +127,8 @@ __device__ __noinline__ void scatter_pixel_global(const GradChans gch, int Wt, i
 //   R is a sub-convex combination of the q's).  With 2^e > 4 qmax (a factor 2 of slack for inputs that leave [0,1] by rounding)
 // contributions are rounded to multiples of 2^(e - kFixBits): |c| 2^(kFixBits - e) < 2^(kFixBits - 1), i.e. 25 bits + sign per
 // contribution (finer than the fp32 accumulation it replaces whenever the running sum is within 4x of the bound), and a texel
-// may collect 2^(31 - kFixBits + 1) = 64 contributions of maximum size in int32 -- each pixel has one footprint per plane, so
-// that takes a 8x8 minification... of the PIXEL grid onto one texel (scale < 1/4) at maximum gradient everywhere; wrap-around
-// beyond that is the documented limit of this kernel (the direct kernel has none).
+// may collect 2^(31 - kFixBits + 1) = 64 contributions of maximum size in int32.  Magnified footprints, where one texel collects
+// more than that from one tile, take the generic body (BwdRing::kMagLimit).
 constexpr int kFixBits = 26, kFixSplit = 4;              // alpha: low kFixSplit bits come from the second conversion step
 // The three colour channels have their own, tighter bound -- |dL/d rgb contribution| = |G_c| a T w <= gmax = max |G_c| over the
 // tile, without the depth term and the factor 2 of the alpha bound -- and take the one-step conversion: 2^e_rgb > 2 gmax,
@@ -126,11 +137,15 @@ constexpr int kFixBits = 26, kFixSplit = 4;              // alpha: low kFixSplit
 constexpr int kFixBitsRgb = 22;
 constexpr float kMagicHi = 12582912.0f * 16.0f;          // 1.5 * 2^(23 + kFixSplit): ulp = 2^kFixSplit
 constexpr int kMagicHiBits = 0x4b400000 + (kFixSplit << 23);
+// Exponents for which 2^(kFixBits - e), 2^(e - kFixBits), 2^(kFixBitsRgb - e) and 2^(e - kFixBitsRgb) are all normal floats, so that
+// scaling and flushing are exact: e >= -100 (2^(e - 26) >= 2^-126); every finite b gives e <= 128, and an infinite one 129.
+// A tile whose exponents fall outside (an inf/NaN upstream gradient, |G| beyond about 1e37 or below about 1e-31) takes the
+// generic body, which has no such limits.
+constexpr int kMinScaleExp = -100, kMaxScaleExp = 128;
 __device__ __forceinline__ int tile_scale_exponent(float qmax) {
     const float b = 4.0f * qmax;
     if (!(b > 0.0f)) return 0;
-    int e = (int)((__float_as_uint(b) >> 23) & 0xffu) - 126;     // 2^e > b  (b = 1.m * 2^(E-127) < 2^(E-126))
-    return max(-90, min(90, e));
+    return (int)((__float_as_uint(b) >> 23) & 0xffu) - 126;     // 2^e > b  (b = 1.m * 2^(E-127) < 2^(E-126))
 }
 // RN(x) for |x| < 2^(22 + kFixSplit), two pixels at once, as integers: the high part is read from the mantissa of x + 1.5 * 2^27
 // (a multiple of 16), the exact remainder (|r| <= 8) from the mantissa of r + 1.5 * 2^23.  x = vF * w is never formed: both steps
@@ -396,7 +411,9 @@ mpi_bwd_box_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps, c
                 gq[q][1] = valid ? gscale * __ldg(gc + img) : 0.0f;
                 gq[q][2] = valid ? gscale * __ldg(gc + 2 * img) : 0.0f;
                 gq[q][3] = (valid && p.g_depth) ? __ldg(p.g_depth + (size_t)v * img + pix) * rc[q].dz : 0.0f;
-                qmax = fmaxf(qmax, fabsf(gq[q][0]) + fabsf(gq[q][1]) + fabsf(gq[q][2]) + fabsf(gq[q][3]) * (zmax * fabsf(rc[q].yrz)));
+                const float ga = fabsf(gq[q][0]) + fabsf(gq[q][1]) + fabsf(gq[q][2]), gd = fabsf(gq[q][3]);
+                qmax = fmaxf(qmax, ga + gd * (zmax * fabsf(rc[q].yrz)));
+                if (!(ga + gd <= 0x1.fffffep127f)) qmax = INFINITY;     // inf/NaN upstream gradient (fmaxf would drop a NaN)
                 gmax = fmaxf(gmax, fmaxf(fabsf(gq[q][0]), fmaxf(fabsf(gq[q][1]), fabsf(gq[q][2]))));
             }
             // ---- the tile's fixed-point scale: max over all consumer threads (three slots in rotation, see below) ----
@@ -406,18 +423,21 @@ mpi_bwd_box_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps, c
                     qmax = fmaxf(qmax, __shfl_xor_sync(0xffffffffu, qmax, o));
                     gmax = fmaxf(gmax, __shfl_xor_sync(0xffffffffu, gmax, o));
                 }
-                if (!(qmax < 0x1p100f)) qmax = 0x1p100f;             // inf/NaN upstream gradients: keep the exponents finite
-                if (!(gmax < 0x1p100f)) gmax = 0x1p100f;
                 if (lane == 0) { atomicMax(&s_qmax[slot], __float_as_uint(qmax)); atomicMax(&s_gmax[slot], __float_as_uint(gmax)); }
                 if (threadIdx.x == 0) s_qmax[(j + 1) % 3] = s_gmax[(j + 1) % 3] = 0u;   // next tile's slots: their last readers passed the previous tile's barrier
                 bwd_consumer_bar_sync();
                 qmax = __uint_as_float(s_qmax[slot]);
                 gmax = __uint_as_float(s_gmax[slot]);
             }
-            const int e_fix = tile_scale_exponent(qmax);
+            int e_fix = tile_scale_exponent(qmax);
+            int e_rgb = tile_scale_exponent(0.5f * gmax);                                         // 2^e_rgb > 2 gmax
+            // CTA-uniform: the bounds are reduced over the tile.  Out of range, the tile takes the generic body (and the clamp
+            // only keeps the unused constants well-formed)
+            const bool scale_ok = e_fix >= kMinScaleExp && e_fix <= kMaxScaleExp && e_rgb >= kMinScaleExp && e_rgb <= kMaxScaleExp;
+            e_fix = max(kMinScaleExp, min(kMaxScaleExp, e_fix));
+            e_rgb = max(kMinScaleExp, min(kMaxScaleExp, e_rgb));
             const f2 Fs = splat(__uint_as_float((unsigned)(127 + kFixBits - e_fix) << 23));      // 2^(kFixBits - e)
             const float inv_scale = __uint_as_float((unsigned)(127 - kFixBits + e_fix) << 23);    // 2^(e - kFixBits)
-            const int e_rgb = tile_scale_exponent(0.5f * gmax);                                   // 2^e_rgb > 2 gmax
             const f2 Fs_rgb = splat(__uint_as_float((unsigned)(127 + kFixBitsRgb - e_rgb) << 23));
             const float inv_scale_rgb = __uint_as_float((unsigned)(127 - kFixBitsRgb + e_rgb) << 23);
 
@@ -434,7 +454,7 @@ mpi_bwd_box_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps, c
                 G.gs[P] = make_float2(gq[2 * P][3], gq[2 * P + 1][3]);
             }
             const f2 ex2 = splat(rc[0].ex2), ey2 = splat(rc[0].ey2), hsx2 = splat(hsx), hsy2 = splat(hsy);
-            const bool warp_fast = __all_sync(0xffffffffu, rays_fast) && !idle;
+            const bool warp_fast = __all_sync(0xffffffffu, rays_fast) && !idle && scale_ok;
             f2 R[kPairs];
 #pragma unroll
             for (int P = 0; P < kPairs; ++P) R[P] = splat(0.0f);

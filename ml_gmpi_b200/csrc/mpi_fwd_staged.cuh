@@ -59,7 +59,8 @@ struct __align__(16) StageMeta {
     int sel;               // bits 0-7 staged width (row pitch = 4*bw floats), bits 8-9 mode (0 staged, 1 nothing under the
                            // tile, 2 sample from global), bits 16-20 width class for the packed fast body, ONE-HOT (a chain of
                            // single-bit tests, most frequent first, is shorter than a jump table), or 0 (not usable: mode != 0,
-                           // or plane constants outside the exact-division range)
+                           // or plane constants outside the exact-division range, or -- backward only -- a footprint too
+                           // magnified for the gradient box)
 };
 
 // ---- pixel-pair arithmetic: two pixels per operation, IEEE rn per element ----
@@ -382,6 +383,10 @@ __device__ __forceinline__ void staged_producer(const RenderParams& p, const Tma
                 mt.cx = kFloorMagicBits + bx0; mt.cy = kFloorMagicBits + by0;
                 mt.rows2 = rows - 2;
                 mt.sel = bw | (mode << 8) | ((mode == 0 && pc.fast != 0.0f ? (1 << k) : kSelSlow) << 16);
+                if constexpr (kReverse) {   // backward: a footprint too magnified for the int32 gradient box (BwdRing::kMagLimit)
+                    const int ext_x = min(px0 + kTileW - 1, p.W - 1) - px0, ext_y = min(py0 + kTileH - 1, p.H - 1) - py0;
+                    if (Ring::kMagLimit * (xmax - xmin - 1) < ext_x || Ring::kMagLimit * (ymax - ymin - 1) < ext_y) mt.sel &= 0xffff;
+                }
                 s_meta[s] = mt;
                 // bytes the copies of this stage will deliver (a box counts whole, zero-filled parts included)
                 const uint32_t tx = (uint32_t)((kFact ? kMaxBH : rows) * bw * 16);

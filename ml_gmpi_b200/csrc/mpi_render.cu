@@ -329,6 +329,7 @@ __global__ void mpi_debug_cam_rays_kernel(const float* __restrict__ cam, float* 
 using namespace gmpi;
 
 static std::atomic<int> g_fwd_variant{0};   // 0 auto, 1 direct, 2 staged (test hook; relaxed atomic: any thread may set it)
+static std::atomic<int> g_fwd_stages{0};    // expanded staged forward's ring depth: 0 auto (fwd_ring_stages), 2 or 3 (test hook)
 
 // Argument checks shared by every entry point.  `bwd`: gradients instead of outputs.
 static int check_params(const RenderParams& p, bool bwd) {
@@ -408,6 +409,13 @@ static int fwd_ring_stages(const RenderParams& p, int l2_bytes) {
     return shared_mpi || fits_l2 ? kStages : kStreamStages;
 }
 
+static int device_l2_bytes(int* l2) {
+    int dev = 0;
+    GMPI_CUDA_OK(cudaGetDevice(&dev));
+    GMPI_CUDA_OK(cudaDeviceGetAttribute(l2, cudaDevAttrL2CacheSize, dev));
+    return GMPI_OK;
+}
+
 template <bool AC, bool EMIT, bool FAC>
 static cudaError_t launch_fwd_staged(const RenderParams& p, const TmaMaps& maps, int grid, int tiles_x, int tiles_y, int stages,
                                      cudaStream_t st) {
@@ -444,11 +452,11 @@ static int launch_fwd(RenderParams p, cudaStream_t st) {
         if (encode_mpi_maps(maps, p, kMaxBH, FwdRingWide::kColourCopyRows, fac) != 0) {
             if (g_fwd_variant.load(std::memory_order_relaxed) == 2) return fail(GMPI_ERR_CUDA, "cuTensorMapEncodeTiled failed");
         } else {
-            int sms = 0, dev = 0, l2 = 0;
+            int sms = 0, l2 = 0;
             if ((rc = device_sms(&sms)) != 0) return rc;
-            GMPI_CUDA_OK(cudaGetDevice(&dev));
-            GMPI_CUDA_OK(cudaDeviceGetAttribute(&l2, cudaDevAttrL2CacheSize, dev));
-            const int stages = fwd_ring_stages(p, l2);
+            if ((rc = device_l2_bytes(&l2)) != 0) return rc;
+            const int forced_stages = g_fwd_stages.load(std::memory_order_relaxed);
+            const int stages = forced_stages ? forced_stages : fwd_ring_stages(p, l2);
             const int tiles_x = (p.W + kTileW - 1) / kTileW, tiles_y = (p.H + kTileH - 1) / kTileH;
             const long n_tiles = (long)tiles_x * tiles_y * p.V;
             const int grid = (int)(n_tiles < sms ? n_tiles : sms);
@@ -615,6 +623,24 @@ int gmpi_debug_set_fwd_variant(int variant) {
     if (variant < 0 || variant > 2) return fail(GMPI_ERR_INVALID_ARGUMENT, "variant must be 0 (auto), 1 (direct) or 2 (staged)");
     g_fwd_variant.store(variant, std::memory_order_relaxed);
     return GMPI_OK;
+}
+
+int gmpi_debug_set_fwd_stages(int stages) {
+    if (stages != 0 && stages != kStreamStages && stages != kStages)
+        return fail(GMPI_ERR_INVALID_ARGUMENT, "stages must be 0 (auto), %d or %d", kStreamStages, kStages);
+    g_fwd_stages.store(stages, std::memory_order_relaxed);
+    return GMPI_OK;
+}
+
+int gmpi_debug_fwd_ring_stages(int M, int V, int N, int Ht, int Wt, int view_group) {
+    if (M < 1 || V < 1 || N < 1 || Ht < 1 || Wt < 1 || view_group < 0)
+        return -fail(GMPI_ERR_INVALID_ARGUMENT, "gmpi_debug_fwd_ring_stages: bad argument");
+    RenderParams p{};
+    p.M = M; p.V = V; p.N = N; p.Ht = Ht; p.Wt = Wt;
+    p.view_group = view_group < 1 ? 1 : view_group;
+    int l2 = 0, rc = device_l2_bytes(&l2);
+    if (rc) return -rc;
+    return fwd_ring_stages(p, l2);
 }
 
 // Host evaluation of the staged kernels' tile order (same TileWalk code): tiles of CTA `cta` in a grid of `grid` CTAs, as

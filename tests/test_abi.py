@@ -55,6 +55,15 @@ def test_argument_validation_needs_no_gpu(lib):
     assert rc == 1
 
 
+def test_ring_depth_hooks_validate_without_gpu(lib):
+    for bad in (-1, 1, 4):
+        assert lib.gmpi_debug_set_fwd_stages(bad) == 1 and b"stages must be" in lib.gmpi_last_error()
+    for ok in (2, 3, 0):                        # ends on auto
+        assert lib.gmpi_debug_set_fwd_stages(ok) == 0
+    assert lib.gmpi_debug_fwd_ring_stages(1, 1, 0, 64, 64, 1) < 0
+    assert lib.gmpi_debug_fwd_ring_stages(1, 1, 8, 64, 64, -1) < 0
+
+
 def test_cubin_is_sm90a():
     import subprocess
     out = subprocess.run(["cuobjdump", "-lelf", g._build.LIB_PATH], capture_output=True, text=True).stdout

@@ -1,0 +1,233 @@
+"""The staged backward's fixed-point gradient box at its limits (run on an H100: pytest -m gpu).
+
+The box kernel adds every (pixel, plane) contribution to a shared-memory int32 box, scaled by a per-tile power of two taken
+from the tile's largest upstream gradient (csrc/mpi_bwd_box.cuh).  These tests push that scheme where it cannot hold -- many
+pixels per texel (magnification), upstream gradients near the ends of the fp32 range, inf/NaN upstream gradients -- and
+compare with the oracle (fp32 autograd formula), through the expanded and the factored backward.  The kernel must then take
+its generic body (fp32 global atomics) instead of wrapping or rounding to garbage."""
+import os
+
+import numpy as np
+import pytest
+import torch
+
+import mpi_oracle
+import ml_gmpi_b200 as g
+from ml_gmpi_b200 import _lib, synth
+from conftest import rel_err
+
+pytestmark = pytest.mark.gpu
+EXPECT = 2e-5
+_NT = max(1, min(64, (os.cpu_count() or 8)))
+
+
+def dev():
+    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
+    return torch.device("cuda:0")
+
+
+def _force(variant):
+    lib = _lib.load()
+    _lib.check(lib.gmpi_debug_set_fwd_variant(variant))
+
+
+@pytest.fixture
+def staged():
+    """TMA-staged forward and box backward whatever the number of tiles."""
+    _force(2)
+    yield
+    _force(0)
+
+
+@pytest.fixture(params=["staged", "direct"])
+def bwd_variant(request):
+    _force({"direct": 1, "staged": 2}[request.param])
+    yield request.param
+    _force(0)
+
+
+n = lambda t: t.detach().cpu().numpy()
+
+
+def _expanded_grad(rgba, case, gc, gd, ray=None):
+    x = rgba.clone().requires_grad_(True)
+    color, depth = g.render_views(x, case.dhw, case.view2mpi, case.ray_dir if ray is None else ray, case.eye, case.z_dir)
+    loss = (color * gc).sum()
+    if gd is not None:
+        loss = loss + (depth * gd).sum()
+    loss.backward()
+    return n(x.grad)
+
+
+def _factored_grads(rgb, alpha, bg, case, gc, gd, ray=None):
+    r, a, b = (t.clone().requires_grad_(True) for t in (rgb, alpha, bg))
+    color, depth = g.render_views_factored(r, a, case.dhw, case.view2mpi, case.ray_dir if ray is None else ray, case.eye, case.z_dir,
+                                           bg_rgb=b)
+    loss = (color * gc).sum()
+    if gd is not None:
+        loss = loss + (depth * gd).sum()
+    loss.backward()
+    return n(r.grad), n(a.grad), n(b.grad)
+
+
+def _oracle(rgba, case, gc, gd, ray=None):
+    return mpi_oracle.backward(n(rgba), n(case.view2mpi), n(case.dhw), n(case.ray_dir if ray is None else ray), n(case.eye),
+                               n(case.z_dir), n(gc), None if gd is None else n(gd), nthreads=_NT)
+
+
+def _factored_refs(ref):
+    """The oracle's expanded gradient -> (d rgb, d alpha, d bg) of a factored MPI with a background plane: d rgb is the sum over
+    the planes that share the colour image."""
+    return ref[:, :-1, :3].astype(np.float64).sum(1), ref[:, :, 3:4], ref[:, -1, :3]
+
+
+def _check_factored(ours, ref, tol=EXPECT):
+    """d rgb sums N-1 planes' rounding errors (fixed point here, fp32 in the oracle): twice the per-plane bar, as in
+    test_gpu_features.test_factored_backward_equals_expanded_autograd."""
+    r_rgb, r_alpha, r_bg = _factored_refs(ref)
+    e = (rel_err(ours[0], r_rgb), rel_err(ours[1], r_alpha), rel_err(ours[2], r_bg))
+    assert e[0] <= 2 * tol and e[1] <= tol and e[2] <= tol, e
+
+
+# ------------------------------------------------------------------------------------------------------------------------
+# 1. magnification: many pixels per texel within one 64x24 tile
+# ------------------------------------------------------------------------------------------------------------------------
+def _coherent_mpi(tex, N, d):
+    """Plane 0 red with alpha 0.5, black planes behind it, an opaque black last plane: with g_color = (1, 0, 0) every pixel's
+    alpha contribution on plane 0 has the same sign and the largest size the tile's scale allows."""
+    rgba = torch.zeros((1, N, 4, tex, tex), device=d)
+    rgba[0, 0, 0] = 1.0
+    rgba[0, 0, 3] = 0.5
+    rgba[0, 1:N - 1, 3] = 0.3
+    rgba[0, N - 1, 3] = 1.0
+    # factored form: red shared colour, black background, the same alphas (the middle planes are red here, not black)
+    rgb = torch.zeros((1, 3, tex, tex), device=d)
+    rgb[0, 0] = 1.0
+    alpha = rgba[:, :, 3:4].clone()
+    bg = torch.zeros((1, 3, tex, tex), device=d)
+    return rgba, rgb, alpha, bg
+
+
+@pytest.mark.parametrize("loss", ["red", "color_and_depth"])
+@pytest.mark.parametrize("pose", ["identity", "oblique"])
+@pytest.mark.parametrize("tex", [256, 64, 32, 16, 8])
+def test_magnified_texture_gradient_box_does_not_wrap(tex, pose, loss, staged):
+    """Textures of 256^2 down to 8^2 rendered at 512^2 (up to ~60 pixels per texel in each direction)."""
+    d = dev()
+    N, img = 4, 512
+    yaws, pitches = ([0.0], [0.0]) if pose == "identity" else ([0.35], [-0.15])
+    case = synth.make_case(n_planes=N, tex=tex, img=img, n_mpi=1, seed=3, device=d, yaws=yaws, pitches=pitches, rgba=False)
+    rgba, rgb, alpha, bg = _coherent_mpi(tex, N, d)
+    if loss == "red":
+        gc = torch.zeros((1, 3, img, img), device=d)
+        gc[:, 0] = 1.0
+        gd = None
+    else:
+        gc, gd = torch.ones((1, 3, img, img), device=d), torch.ones((1, 1, img, img), device=d)
+    ref = _oracle(rgba, case, gc, gd)
+    assert float(np.abs(ref).max()) > 0
+    e = rel_err(_expanded_grad(rgba, case, gc, gd), ref)
+    assert e <= EXPECT, e
+    rgba_f = g.expand_factored(rgb, alpha, bg)
+    _check_factored(_factored_grads(rgb, alpha, bg, case, gc, gd), _oracle(rgba_f, case, gc, gd))
+
+
+# ------------------------------------------------------------------------------------------------------------------------
+# 2. the tile exponent tracks the gradient exactly
+# ------------------------------------------------------------------------------------------------------------------------
+def _one_tile_per_mpi_case(d):
+    """Two MPIs, one near-frontal view each, of ONE 64 x 24 backward tile (rows 20..43 of a 64^2 pinhole image): every
+    (tile, plane) takes the box, and every texel of g_rgba receives exactly one flush per plane, so the result does not
+    depend on the order of fp32 atomics."""
+    import dataclasses
+    case = synth.make_case(n_planes=6, tex=64, img=64, n_mpi=2, seed=13, device=d, last_alpha_one=True,
+                           yaws=[0.05, -0.08], pitches=[0.02, -0.03])
+    return dataclasses.replace(case, ray_dir=case.ray_dir[:, :, 20:44].contiguous())
+
+
+@pytest.mark.parametrize("k", [-40, -13, 0, 7, 40])
+def test_power_of_two_scaled_upstream_gradient_scales_the_result_bitwise(k, staged):
+    d = dev()
+    case = _one_tile_per_mpi_case(d)
+    gen = torch.Generator().manual_seed(4)
+    gc = torch.randn((2, 3, 24, 64), generator=gen).to(d)
+    gd = torch.randn((2, 1, 24, 64), generator=gen).to(d)
+    s = 2.0 ** k
+    base = _expanded_grad(case.rgba, case, gc, gd)
+    scaled = _expanded_grad(case.rgba, case, gc * s, gd * s)
+    assert np.array_equal(scaled, base * np.float32(s))
+    assert rel_err(base, _oracle(case.rgba, case, gc, gd)) <= EXPECT
+    # factored: per-plane alpha and the background colour get one flush per texel; the shared colour image sums the planes'
+    # flushes with fp32 atomics in flusher order, which is exact only up to that order
+    gen = torch.Generator(device=d).manual_seed(6)
+    rgb, alpha, bg = (torch.rand(sh, generator=gen, device=d) for sh in ((2, 3, 64, 64), (2, 6, 1, 64, 64), (2, 3, 64, 64)))
+    # thin planes keep the background visible (T ~ 0.4 in front of it): its gradient is then not a small fraction of the tile's
+    # colour scale, where the box's error is bounded relative to that scale rather than to the background gradient itself
+    alpha[:, :-1] *= 0.3
+    alpha[:, -1] = 1.0
+    fb = _factored_grads(rgb, alpha, bg, case, gc, gd)
+    fs = _factored_grads(rgb, alpha, bg, case, gc * s, gd * s)
+    assert np.array_equal(fs[1], fb[1] * np.float32(s)) and np.array_equal(fs[2], fb[2] * np.float32(s))
+    assert rel_err(fs[0], fb[0] * np.float32(s)) <= 1e-6
+    _check_factored(fb, _oracle(g.expand_factored(rgb, alpha, bg), case, gc, gd))
+
+
+# ------------------------------------------------------------------------------------------------------------------------
+# 3. upstream gradients near the ends of the fp32 range
+# ------------------------------------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("scale", [1e-32, 1e-30, 1e27])
+def test_extreme_upstream_gradient_magnitudes(scale, staged):
+    """1e27: the tile exponent is past 90; 1e-30: the colour quantum at exponent -90 would be 1e-3 of the gradient; 1e-32: the
+    scale constants would no longer be normal floats.  The oracle is fp32 too and handles all three."""
+    d = dev()
+    case = synth.make_case(n_planes=6, tex=128, img=128, n_mpi=2, seed=17, device=d, last_alpha_one=True)
+    gen = torch.Generator().manual_seed(8)
+    gc = (torch.randn((2, 3, 128, 128), generator=gen) * scale).to(d)
+    gd = (torch.randn((2, 1, 128, 128), generator=gen) * scale).to(d)
+    ref = _oracle(case.rgba, case, gc, gd)
+    assert np.isfinite(ref).all() and float(np.abs(ref).max()) > 0
+    e = rel_err(_expanded_grad(case.rgba, case, gc, gd), ref)
+    assert e <= EXPECT, e
+    gen = torch.Generator(device=d).manual_seed(9)
+    rgb, alpha, bg = (torch.rand(sh, generator=gen, device=d) for sh in ((2, 3, 128, 128), (2, 6, 1, 128, 128), (2, 3, 128, 128)))
+    alpha[:, -1] = 1.0
+    _check_factored(_factored_grads(rgb, alpha, bg, case, gc, gd), _oracle(g.expand_factored(rgb, alpha, bg), case, gc, gd))
+
+
+# ------------------------------------------------------------------------------------------------------------------------
+# 4. inf / NaN upstream gradients
+# ------------------------------------------------------------------------------------------------------------------------
+def _check_poisoned(ours, ref, variant, tol=EXPECT):
+    """Texels the bad pixels do not reach match the oracle.  Under the bad pixels' footprints the staged kernel, like the
+    oracle (grid_sampler_2d_backward), adds every in-texture tap, zero-weight taps included, so 0 * NaN poisons exactly the
+    oracle's texels.  The direct kernel skips zero-weight taps: there a poisoned oracle texel may stay finite, but no texel may
+    be poisoned that the oracle's is not."""
+    ours, ref = np.asarray(ours, np.float64), np.asarray(ref, np.float64)
+    bad_ref, bad_ours = ~np.isfinite(ref), ~np.isfinite(ours)
+    assert bad_ref.any() and bad_ours.any()
+    if variant == "staged":
+        assert np.array_equal(bad_ours, bad_ref), (int(bad_ours.sum()), int(bad_ref.sum()))
+    else:
+        assert not np.any(bad_ours & ~bad_ref)
+    ok = ~bad_ref & ~bad_ours
+    e = rel_err(ours[ok], ref[ok])
+    assert e <= tol, e
+
+
+def test_nan_and_inf_upstream_gradients_propagate_like_autograd(bwd_variant):
+    d = dev()
+    case = synth.make_case(n_planes=6, tex=128, img=128, n_mpi=1, seed=23, device=d, last_alpha_one=True)
+    gen = torch.Generator().manual_seed(10)
+    gc = torch.randn((1, 3, 128, 128), generator=gen).to(d)
+    gd = torch.randn((1, 1, 128, 128), generator=gen).to(d)
+    gc[0, 0, 30, 40] = float("nan")          # backward tile (px0, py0) = (0, 24)
+    gd[0, 0, 100, 100] = float("inf")        # backward tile (64, 96)
+    ref = _oracle(case.rgba, case, gc, gd)
+    _check_poisoned(_expanded_grad(case.rgba, case, gc, gd), ref, bwd_variant)
+    gen = torch.Generator(device=d).manual_seed(11)
+    rgb, alpha, bg = (torch.rand(sh, generator=gen, device=d) for sh in ((1, 3, 128, 128), (1, 6, 1, 128, 128), (1, 3, 128, 128)))
+    alpha[:, -1] = 1.0
+    ours = _factored_grads(rgb, alpha, bg, case, gc, gd)
+    refs = _factored_refs(_oracle(g.expand_factored(rgb, alpha, bg), case, gc, gd))
+    for o, r, tol in zip(ours, refs, (2 * EXPECT, EXPECT, EXPECT)):      # d rgb: see _check_factored
+        _check_poisoned(o, r, bwd_variant, tol)

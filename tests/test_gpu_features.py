@@ -30,12 +30,17 @@ def dev():
     return torch.device("cuda:0")
 
 
-@pytest.fixture(params=["direct", "staged"])
+@pytest.fixture(params=["direct", "staged", "staged2", "staged3"])
 def fwd_variant(request):
+    """Direct gather, or the TMA-staged forward at the ring depth it picks itself or forced to a 2- or 3-stage ring (expanded MPI;
+    the factored forward's ring is 3 deep)."""
     lib = _lib.load()
-    _lib.check(lib.gmpi_debug_set_fwd_variant({"direct": 1, "staged": 2}[request.param]))
+    variant, stages = {"direct": (1, 0), "staged": (2, 0), "staged2": (2, 2), "staged3": (2, 3)}[request.param]
+    _lib.check(lib.gmpi_debug_set_fwd_variant(variant))
+    _lib.check(lib.gmpi_debug_set_fwd_stages(stages))
     yield request.param
     _lib.check(lib.gmpi_debug_set_fwd_variant(0))
+    _lib.check(lib.gmpi_debug_set_fwd_stages(0))
 
 
 def factored_case(n_planes, tex, img, n_mpi, views_per_mpi, seed, with_bg):

@@ -24,13 +24,31 @@ def dev():
     return torch.device("cuda:0")
 
 
-@pytest.fixture(params=["direct", "staged"])
-def fwd_variant(request):
-    """Runs a forward test once per kernel variant (1 = direct gather, 2 = TMA-staged), then restores auto."""
+_VARIANTS = {"direct": (1, 0), "staged": (2, 0), "staged2": (2, 2), "staged3": (2, 3)}   # (kernel variant, ring depth)
+
+
+def _variant(request):
     lib = _lib.load()
-    _lib.check(lib.gmpi_debug_set_fwd_variant({"direct": 1, "staged": 2}[request.param]))
+    variant, stages = _VARIANTS[request.param]
+    _lib.check(lib.gmpi_debug_set_fwd_variant(variant))
+    _lib.check(lib.gmpi_debug_set_fwd_stages(stages))
     yield request.param
     _lib.check(lib.gmpi_debug_set_fwd_variant(0))
+    _lib.check(lib.gmpi_debug_set_fwd_stages(0))
+
+
+@pytest.fixture(params=["direct", "staged", "staged2", "staged3"])
+def fwd_variant(request):
+    """Runs a test once per forward kernel: the direct gather (1), and the TMA-staged kernel (2) at the ring depth it picks itself
+    and forced to a 2- and a 3-stage ring (the expanded forward's two depths; the factored forward's ring is always 3 deep).
+    Then restores auto."""
+    yield from _variant(request)
+
+
+@pytest.fixture(params=["direct", "staged"])
+def fwd_variant_auto(request):
+    """Direct gather, or the TMA-staged kernel at the ring depth it picks itself (the full-size cases)."""
+    yield from _variant(request)
 
 
 def groups(gd, device):
@@ -197,7 +215,7 @@ def _ffhq_case(N, res, V, seed=1234, device=None):
 
 
 @pytest.mark.parametrize("N,res,V", [(32, 256, 8), (96, 512, 2), (96, 1024, 1)])
-def test_full_size_against_oracle(N, res, V, fwd_variant):
+def test_full_size_against_oracle(N, res, V, fwd_variant_auto):
     d = dev()
     case = _ffhq_case(N, res, V, device=d)
     color, depth = g.render_views(case.rgba, case.dhw, case.view2mpi, case.ray_dir, case.eye, case.z_dir,
@@ -391,7 +409,7 @@ def _grad_check(case, with_depth, minus1_1=False, seed=3):
     return rel_err(ours, ref)
 
 
-def test_full_size_backward_c3_one_view_96x1024_vs_oracle(fwd_variant):
+def test_full_size_backward_c3_one_view_96x1024_vs_oracle(fwd_variant_auto):
     """BASELINE configs[2] (FFHQ1024 forward+backward): one 96-plane 1024^2 view, production alpha==1 last plane, colour and
     depth upstream gradients.  (gmpi/core/mpi.py:411-436 autograd; train.py:733-740.)"""
     from ml_gmpi_b200 import synth
@@ -399,7 +417,7 @@ def test_full_size_backward_c3_one_view_96x1024_vs_oracle(fwd_variant):
     assert _grad_check(case, with_depth=True) <= EXPECT
 
 
-def test_full_size_backward_c5_batch4_96x512_vs_oracle(fwd_variant):
+def test_full_size_backward_c5_batch4_96x512_vs_oracle(fwd_variant_auto):
     """BASELINE configs[4] per-GPU shape: M = V = 4, 96 planes, 512^2, alpha==1 last plane, colour-only upstream gradient w.r.t.
     2c-1 (what train.py:740,779 backpropagates; the depth output is discarded there)."""
     from ml_gmpi_b200 import synth
@@ -407,14 +425,14 @@ def test_full_size_backward_c5_batch4_96x512_vs_oracle(fwd_variant):
     assert _grad_check(case, with_depth=False, minus1_1=True) <= EXPECT
 
 
-def test_full_size_backward_four_views_share_one_mpi_512_vs_oracle(fwd_variant):
+def test_full_size_backward_four_views_share_one_mpi_512_vs_oracle(fwd_variant_auto):
     """Gradient accumulation over 4 views of ONE MPI at 512^2 (the expand of train.py:733-738, train_helpers.py:181-186)."""
     from ml_gmpi_b200 import synth
     case = synth.make_case(n_planes=48, tex=512, img=512, n_mpi=1, views_per_mpi=4, seed=21, device=dev(), last_alpha_one=True)
     assert _grad_check(case, with_depth=True) <= EXPECT
 
 
-def test_full_size_forward_c4_video_every_view_vs_oracle(fwd_variant):
+def test_full_size_forward_c4_video_every_view_vs_oracle(fwd_variant_auto):
     """BASELINE configs[3] shape: ONE 96-plane 512^2 MPI, 15 views (one rank's share of the 120) spread over the whole
     yaw = linspace(0.5, -0.5, 120) sweep, pitch 0 (render_video.py:95-107); every view against the oracle."""
     from ml_gmpi_b200 import synth
@@ -550,3 +568,67 @@ def test_zero_grad_one_mpi_many_views_poisoned_allocator_block():
     poison = torch.full_like(case.rgba, float("nan"))
     del poison                                                  # the next same-size torch.empty gets this block back
     assert _grad_check(case, with_depth=True) <= 2e-5
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# Shapes at the edges of the staged forward's ring (fwd_variant runs each at both ring depths): one plane, kMaxPlanesStaged = 512
+# planes (the plane table then ends the shared-memory allocation of either depth), partial tiles with align_corners=False
+# ------------------------------------------------------------------------------------------------------------------------------
+def _fwd_bwd_vs_oracle(rgba, case, ray, align_corners=True, seed=0):
+    d = rgba.device
+    x = rgba.clone().requires_grad_(True)
+    color, depth = g.render_views(x, case.dhw, case.view2mpi, ray, case.eye, case.z_dir, align_corners=align_corners,
+                                  check_last_plane=True)
+    gen = torch.Generator().manual_seed(seed)
+    gc, gdp = torch.randn(color.shape, generator=gen).to(d), torch.randn(depth.shape, generator=gen).to(d)
+    ((color * gc).sum() + (depth * gdp).sum()).backward()
+    n = lambda t: t.detach().cpu().numpy()
+    args = (n(rgba), n(case.view2mpi), n(case.dhw), n(ray), n(case.eye), n(case.z_dir))
+    rc, rd, _ = mpi_oracle.forward(*args, align_corners=align_corners, nthreads=_NT)
+    assert rel_err(n(color), rc) <= EXPECT and rel_err(n(depth), rd) <= EXPECT
+    ref = mpi_oracle.backward(*args, n(gc), n(gdp), align_corners=align_corners, nthreads=_NT)
+    assert rel_err(n(x.grad), ref) <= EXPECT
+
+
+def test_single_plane_vs_oracle(fwd_variant):
+    from ml_gmpi_b200 import synth
+    import dataclasses
+    case = synth.make_case(n_planes=8, tex=128, img=160, n_mpi=2, seed=41, device=dev())
+    case = dataclasses.replace(case, rgba=case.rgba[:, 3:4].contiguous(), dhw=case.dhw[:, 3:4].contiguous())
+    _fwd_bwd_vs_oracle(case.rgba, case, case.ray_dir, seed=1)
+
+
+def test_512_planes_vs_oracle(fwd_variant):
+    """N = kMaxPlanesStaged, 96^2 textures at 128^2.  Alpha is scaled down so that the back planes still show through."""
+    from ml_gmpi_b200 import synth
+    case = synth.make_case(n_planes=512, tex=96, img=128, n_mpi=2, seed=43, device=dev())
+    rgba = case.rgba.clone()
+    rgba[:, :, 3] *= 0.02
+    rgba[:, -1, 3] = 1.0
+    _fwd_bwd_vs_oracle(rgba, case, case.ray_dir, seed=2)
+
+
+def test_partial_tiles_align_corners_false_nonsquare_vs_oracle(fwd_variant):
+    """100 x 136 pixels (partial tiles in both directions for the forward's 64 x 30 and the backward's 64 x 24 tiles) cut out of
+    a pinhole image, 72 x 116 textures, align_corners=False."""
+    from ml_gmpi_b200 import synth
+    d = dev()
+    case = synth.make_case(n_planes=10, tex=8, img=136, n_mpi=2, views_per_mpi=2, seed=47, device=d, rgba=False)
+    gen = torch.Generator(device=d).manual_seed(47)
+    rgba = torch.rand((2, 10, 4, 72, 116), generator=gen, device=d)
+    rgba[:, -1, 3] = 1.0
+    ray = case.ray_dir[:, :, 18:118].contiguous()
+    _fwd_bwd_vs_oracle(rgba, case, ray, align_corners=False, seed=3)
+
+
+def test_ring_depth_policy():
+    """fwd_ring_stages: 2 stages when every view has its own MPI larger than L2 (the headline forward and every training batch),
+    3 when the boxes come from L2 (views sharing one MPI, or an MPI that fits)."""
+    lib = _lib.load()
+    dev()
+    assert lib.gmpi_debug_fwd_ring_stages(4, 4, 96, 1024, 1024, 1) == 2      # 4 MPIs x 1 view, 96 x 1024^2
+    assert lib.gmpi_debug_fwd_ring_stages(8, 8, 32, 256, 256, 1) == 3        # the 256^2 batch: 32 x 256^2 fits L2
+    assert lib.gmpi_debug_fwd_ring_stages(1, 120, 96, 512, 512, 120) == 3    # 120 views of one 96 x 512^2 MPI, grouped
+    assert lib.gmpi_debug_fwd_ring_stages(1, 120, 96, 512, 512, 1) == 3      # ... or not: the views still share the MPI
+    assert lib.gmpi_debug_fwd_ring_stages(4, 4, 96, 512, 512, 1) == 2
+    assert lib.gmpi_debug_fwd_ring_stages(0, 4, 96, 512, 512, 1) < 0
