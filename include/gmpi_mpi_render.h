@@ -60,6 +60,7 @@ extern "C" {
 #define GMPI_ZERO_GRAD 8u              /* bwd: zero the gradient buffers on the stream before accumulating */
 #define GMPI_U8_ROUND_HALF_UP 16u       /* uint8 epilogue: clamp, x*255+0.5 (torchvision save_image, fid_evaluation.py:125-130)
                                           instead of numpy's truncating astype (render_video.py:119-126) */
+#define GMPI_EARLY_STOP 32u            /* forward only: early ray termination at gmpi_render_desc.early_stop (see there) */
 
 int gmpi_abi_version(void);
 const char* gmpi_last_error(void);
@@ -207,7 +208,23 @@ typedef struct gmpi_render_desc {
     float* g_alpha;
     uint32_t* flags;
     void* stream;
+    float early_stop;
 } gmpi_render_desc;
+
+/*
+ * early_stop (with GMPI_EARLY_STOP in options; off by default): a threshold 0 <= tau < 1.  After plane i is composited, a pixel
+ * whose transmittance satisfies |T| <= tau composites no further plane; its colour and depth are what it accumulated so far.  The
+ * planes dropped carry a total weight of at most T <= tau, so each colour channel moves by at most tau (2 tau with
+ * GMPI_COLOR_MINUS1_1), depth by at most tau * (the pixel's largest z-depth over the planes) and a uint8 output by at most one
+ * code.  tau = 0 gives bit-identical output to early stop off.  The decision is per pixel, so the output does not depend on
+ * timing.  The staged kernels skip the plane loads of a tile once all its pixels have stopped.  Forward only: a descriptor that
+ * also sets transmittance, and every backward call with the bit, return GMPI_ERR_UNSUPPORTED.  The classic entry points have no
+ * threshold field and refuse the bit.
+ *
+ * struct_bytes: sizeof(gmpi_render_desc), or GMPI_RENDER_DESC_V2_BYTES, the size before early_stop was appended (callers built
+ * against that header keep working; early stop is then off and GMPI_EARLY_STOP is refused).
+ */
+#define GMPI_RENDER_DESC_V2_BYTES offsetof(gmpi_render_desc, early_stop)
 
 /* cudaMemsetAsync(ptr, 0, bytes) on `stream`, for callers that accumulate into their own buffers (no GMPI_ZERO_GRAD).  Note that a
  * memset cannot overlap the staged kernels, on whatever stream (they own every SM: measured, tools/zero_overlap_probe.py). */
@@ -281,6 +298,10 @@ int gmpi_debug_set_fwd_variant(int variant);
 /* Test hook: force the ring depth of the expanded TMA-staged forward: 0 auto (default), 2 or 3 stages.  The factored forward
  * keeps its 3-stage ring. */
 int gmpi_debug_set_fwd_stages(int stages);
+
+/* Test hook: the last GMPI_EARLY_STOP launch on this device (synchronises the device): *skipped = the (tile, plane) stages the
+ * staged kernel armed without loading their box, *total = the stages it walked (tiles x N; 0 when the direct kernel ran). */
+int gmpi_debug_fwd_early_stop_stats(unsigned long long* skipped, unsigned long long* total);
 
 /* Test hook: the ring depth (2 or 3) the expanded staged forward picks on the current device for M MPIs, V views, N planes of
  * Ht x Wt texels and view_group (gmpi_render_desc.view_group); a negative GMPI_ERR_* code on bad arguments. */

@@ -28,10 +28,11 @@ EXPORTS = [
     "gmpi_mpi_render_fwd_gather", "gmpi_mpi_render_fwd_train", "gmpi_mpi_render_bwd", "gmpi_mpi_render_bwd_saved", "gmpi_mpi_check_range", "gmpi_mpi_render_fwd_host", "gmpi_mpi_release_host_cache", "gmpi_debug_plane_coords", "gmpi_debug_division", "gmpi_debug_set_fwd_variant", "gmpi_debug_copy_plan", "gmpi_debug_plane_coords_packed", "gmpi_debug_tile_walk",
     "gmpi_mpi_render_fwd_plan", "gmpi_mpi_render_fwd_ex", "gmpi_mpi_render_bwd_ex", "gmpi_mpi_render_host_ex",
     "gmpi_debug_tile_walk_ex", "gmpi_debug_cam_rays", "gmpi_debug_set_fwd_stages", "gmpi_debug_fwd_ring_stages",
-    "gmpi_mpi_zero_async", "gmpi_mpi_alpha_depth_fwd", "gmpi_mpi_alpha_depth_bwd", "gmpi_mpi_apply_shading_fwd", "gmpi_mpi_apply_shading_bwd",
+    "gmpi_debug_fwd_early_stop_stats", "gmpi_mpi_zero_async", "gmpi_mpi_alpha_depth_fwd", "gmpi_mpi_alpha_depth_bwd", "gmpi_mpi_apply_shading_fwd", "gmpi_mpi_apply_shading_bwd",
 ]
 
 OPT_U8_ROUND_HALF_UP = 16
+OPT_EARLY_STOP = 32
 
 
 class RenderDesc(ctypes.Structure):
@@ -43,7 +44,11 @@ class RenderDesc(ctypes.Structure):
                 ("depth_near", ctypes.c_float), ("depth_range", ctypes.c_float)] + \
                [(n, ctypes.c_void_p) for n in ("rgba", "rgb", "alpha", "bg_rgb", "view2mpi", "dhw", "ray_dir", "eye", "z_dir", "cam",
                                                "color", "depth", "transmittance", "peer_frames", "video_rgb", "video_depth",
-                                               "g_color", "g_depth", "g_rgba", "g_rgb", "g_bg_rgb", "g_alpha", "flags", "stream")]
+                                               "g_color", "g_depth", "g_rgba", "g_rgb", "g_bg_rgb", "g_alpha", "flags", "stream")] + \
+               [("early_stop", ctypes.c_float)]
+
+# struct_bytes of a descriptor built against the header before early_stop was appended (GMPI_RENDER_DESC_V2_BYTES)
+RENDER_DESC_V2_BYTES = RenderDesc.early_stop.offset
 
 
 def make_desc(**kw) -> RenderDesc:
@@ -111,6 +116,8 @@ def load():
     lib.gmpi_debug_set_fwd_variant.argtypes = [i]
     lib.gmpi_debug_set_fwd_stages.restype = i
     lib.gmpi_debug_set_fwd_stages.argtypes = [i]
+    lib.gmpi_debug_fwd_early_stop_stats.restype = i
+    lib.gmpi_debug_fwd_early_stop_stats.argtypes = [vp, vp]
     lib.gmpi_debug_fwd_ring_stages.restype = i
     lib.gmpi_debug_fwd_ring_stages.argtypes = [i] * 6
     lib.gmpi_debug_copy_plan.restype = i

@@ -49,7 +49,11 @@ struct RenderParams {
     float* g_bg_rgb;          // bwd, factored with a separate background: [M,3,Ht,Wt] of the last plane
     float* g_alpha;           // bwd, factored: [M,N,1,Ht,Wt]
     int view_group;           // > 1: every `view_group` consecutive views share one MPI (tile order hint, see TileWalk)
+    // GMPI_EARLY_STOP (forward only): a pixel composites no further plane once |T| <= early_stop.  Read only by the early-stop
+    // kernels; it fills what was the struct's tail padding, so the parameter layout of every other kernel is unchanged.
+    float early_stop;
 };
+static_assert(sizeof(RenderParams) == 248, "RenderParams layout (kernel parameter offsets)");
 
 // The four channel slabs (Ht*Wt floats each) of one (MPI, plane): expanded rgba or the generator's factored form.
 struct PlaneChans { const float* c[4]; };

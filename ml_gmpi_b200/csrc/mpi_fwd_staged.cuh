@@ -130,9 +130,11 @@ __device__ __forceinline__ void coords_pairs(const PlaneConst& pc, const RayPair
 // if any of the four footprints is not inside the box.
 // AOFF == 0: expanded stage [row][4 channels][BW].  AOFF > 0 (factored MPI): colour box [row][3][BW] at the stage base and
 // the alpha box [row][BW] AOFF floats further on.
-template <int BW, int AOFF = 0>
+// kES (early stop): a pixel whose |T| <= tau adds nothing; its weight is selected to 0, so its T stays where it stopped.
+template <int BW, int AOFF = 0, bool kES = false>
 __device__ __forceinline__ bool sample_pairs(const float* __restrict__ sb, int cx, int cy, int rows2, const CoordPairs& c,
-                                             f2 (&T)[kPairs], f2 (&cr)[kPairs], f2 (&cg)[kPairs], f2 (&cb)[kPairs], f2 (&cws)[kPairs]) {
+                                             f2 (&T)[kPairs], f2 (&cr)[kPairs], f2 (&cg)[kPairs], f2 (&cb)[kPairs], f2 (&cws)[kPairs],
+                                             float tau = 0.0f) {
     constexpr int RP = AOFF ? 3 * BW : 4 * BW;       // colour row pitch
     constexpr int AP = AOFF ? BW : 4 * BW;           // alpha row pitch
     constexpr int A0 = AOFF ? AOFF : 3 * BW;         // alpha offset from the colour index (factored: separate box)
@@ -177,7 +179,11 @@ __device__ __forceinline__ bool sample_pairs(const float* __restrict__ sb, int c
                      fma2(make_float2(aa[AP], ab[AP]), w10, fma2(make_float2(aa[1], ab[1]), w01, mul2(make_float2(aa[0], ab[0]), w00))));
         }
 #undef GMPI_TAP
-        const f2 w = mul2(a, T[P]);                     // mpi.py:423
+        f2 w = mul2(a, T[P]);                           // mpi.py:423
+        if (kES) {
+            if (fabsf(T[P].x) <= tau) w.x = 0.0f;
+            if (fabsf(T[P].y) <= tau) w.y = 0.0f;
+        }
         cr[P] = fma2(w, r, cr[P]);                      // mpi.py:430
         cg[P] = fma2(w, g, cg[P]);
         cb[P] = fma2(w, b, cb[P]);
@@ -319,10 +325,29 @@ __host__ __device__ __forceinline__ int binary_copy_of_lane(int n_chunks, int la
     return ((n_chunks >> bit) & 1) << bit;
 }
 
-template <bool kAlignCorners, class Ring, bool kFact>
+// Early stop (kES, forward only).  s_stop[j % kStopSlots] holds one bit per consumer warp that has stopped in the CTA's j-th tile.
+// The producer sets it to the warps without a row in the image when it arms the tile's first stage; a consumer warp ORs its bit
+// in once all its pixels have stopped, before it releases the stage it stopped on.  Before each later stage of the tile the
+// producer reads the word, and when every warp has stopped it arms the stage without copies (mbar_arrive, no transaction
+// bytes): the ring's sequence of stages and phases is unchanged, only the TMA traffic goes.  A read that misses a bit costs one
+// box that nobody samples; a set bit is always true, so results never depend on timing.  Slots: the producer runs at most
+// n_stages - 1 stages ahead of the slowest consumer, i.e. at most 1 + (n_stages - 1) / N tiles ahead (3 for N = 1 and a
+// 3-stage ring), so a slot is not reset while a consumer of its previous tile could still write it.
+constexpr int kStopSlots = 4;
+constexpr uint32_t kAllConsumers = (1u << kConsWarps) - 1u;
+static_assert(kStages <= kStopSlots, "stop-word slots must cover the producer's lead");
+__device__ unsigned long long g_early_stop_skipped;   // test hook: stages armed without copies (gmpi_debug_fwd_early_stop_stats)
+
+// consumer warps of a tile at row py0 without a row inside an image of H rows (they only keep the ring going)
+__device__ __forceinline__ uint32_t idle_consumer_warps(int py0, int H) {
+    const int live = (H - py0 + kPairs - 1) / kPairs;
+    return live >= kConsWarps ? 0u : kAllConsumers & ~((1u << live) - 1u);
+}
+
+template <bool kAlignCorners, class Ring, bool kFact, bool kES = false>
 __device__ __forceinline__ void staged_producer(const RenderParams& p, const TmaMaps& maps, float* s_buf, StageMeta* s_meta,
                                             uint64_t* s_full, uint64_t* s_empty, const TileWalk* s_walk, int lane,
-                                            int n_stages = Ring::kRingStages) {
+                                            int n_stages = Ring::kRingStages, uint32_t* s_stop = nullptr) {
     constexpr bool kReverse = Ring::kReverse;
     constexpr int kStride = Ring::kStride;      // floats per ring stage
     constexpr int kTileH = Ring::kTileRows, kStages = Ring::kRingStages, kMaxBH = Ring::kBoxMaxH, kStageFloats = Ring::kPlaneFloats;
@@ -337,10 +362,12 @@ __device__ __forceinline__ void staged_producer(const RenderParams& p, const Tma
     }
     int p_stage = 0;
     uint32_t p_phase = 0;
+    uint32_t n_skipped = 0;      // kES: stages armed without copies
     TileXY txy;
     for (int j = 0; s_walk->at(j, txy); ++j) {
         const int v = txy.v, px0 = txy.px0, py0 = txy.py0;
         const int m = __ldg(p.view2mpi + v);
+        uint32_t* const stop_word = kES ? s_stop + (j & (kStopSlots - 1)) : nullptr;
         float ev[3], zd[3];
         load_eye_z(p, v, ev, zd);
         // the four corner pixels of the tile (replicated over the warp), clamped into the image
@@ -378,6 +405,16 @@ __device__ __forceinline__ void staged_producer(const RenderParams& p, const Tma
             const int rows = n_ops * kRowsPerOp;
             if (Ring::kSleepPolls) mbar_wait_sleep(&s_empty[s], ph ^ 1);
             else mbar_wait(&s_empty[s], ph ^ 1);
+            bool skip = false;
+            if constexpr (kES) {
+                if (ii == 0) {
+                    if (lane == 0) *stop_word = idle_consumer_warps(py0, p.H);   // published by the full barrier's arrive below
+                } else {
+                    skip = __shfl_sync(0xffffffffu, *(volatile uint32_t*)stop_word, 0) == kAllConsumers;
+                    n_skipped += skip ? 1u : 0u;
+                }
+            }
+            const int n_copy = skip ? 0 : n_ops;
             if (lane == 0) {
                 StageMeta mt;
                 mt.cx = kFloorMagicBits + bx0; mt.cy = kFloorMagicBits + by0;
@@ -390,7 +427,7 @@ __device__ __forceinline__ void staged_producer(const RenderParams& p, const Tma
                 s_meta[s] = mt;
                 // bytes the copies of this stage will deliver (a box counts whole, zero-filled parts included)
                 const uint32_t tx = (uint32_t)((kFact ? kMaxBH : rows) * bw * 16);
-                if (n_ops > 0 || kTBytes) mbar_arrive_expect_tx(&s_full[s], (n_ops > 0 ? tx : 0u) + kTBytes);
+                if (n_copy > 0 || kTBytes) mbar_arrive_expect_tx(&s_full[s], (n_copy > 0 ? tx : 0u) + kTBytes);
                 else mbar_arrive(&s_full[s]);
                 if (kReverse)   // the tile's saved transmittance for this plane rides in the same stage
                     tma_load_3d(s_buf + (size_t)s * kStride + kStageFloats, &maps.t, &s_full[s], px0, py0, v * N + i);
@@ -398,7 +435,7 @@ __device__ __forceinline__ void staged_producer(const RenderParams& p, const Tma
             __syncwarp();
             // Few, tall copies.  UTMALDG takes uniform operands, so the lanes of a warp issue their copies ONE AFTER ANOTHER: with a
             // 4-row copy per lane (9-11 per stage, twice that for the factored MPI) the producer was the bottleneck of its own ring.
-            if (n_ops > 0) {
+            if (n_copy > 0) {
                 float* stage = s_buf + (size_t)s * kStride;
                 if constexpr (kFact) {
                     // factored MPI: the colour box (shared image, or the last plane's own) as two or three copies that tile the
@@ -425,6 +462,9 @@ __device__ __forceinline__ void staged_producer(const RenderParams& p, const Tma
                 }
             }
         }
+    }
+    if constexpr (kES) {
+        if (lane == 0 && n_skipped) atomicAdd(&g_early_stop_skipped, (unsigned long long)n_skipped);
     }
 }
 
@@ -478,10 +518,10 @@ __device__ __forceinline__ void store_tile_pixels(const RenderParams& p, int v, 
     store_pixel(p, v, img, (size_t)py * p.W + px, o[0], o[1], o[2], o[3]);
 }
 
-template <bool kAlignCorners, bool kEmitT, bool kFactored>
-__global__ void __launch_bounds__(kStagedThreads, 1)
-mpi_fwd_staged_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps, const int tiles_x, const int tiles_y,
-                      const int ring_stages) {
+// Body of the staged forward kernels.  kES: early stop (mpi_fwd_early_stop_kernel; s_stop is its stop-word ring, see kStopSlots).
+template <bool kAlignCorners, bool kEmitT, bool kFactored, bool kES>
+__device__ __forceinline__ void fwd_staged_body(const RenderParams& p, const TmaMaps& maps, const int tiles_x, const int ring_stages,
+                                                uint32_t* s_stop) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     float* s_buf = reinterpret_cast<float*>(smem_raw);   // the ring starts the dynamic segment (1024-byte aligned)
     using Ring = typename std::conditional<kFactored, FwdRingWide, FwdRing>::type;
@@ -517,12 +557,13 @@ mpi_fwd_staged_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps
     const size_t img = (size_t)p.H * p.W;
 
     if (warp == kConsWarps) {
-        staged_producer<kAlignCorners, Ring, kFactored>(p, maps, s_buf, s_meta, s_full, s_empty, &s_walk, lane, n_stages);
+        staged_producer<kAlignCorners, Ring, kFactored, kES>(p, maps, s_buf, s_meta, s_full, s_empty, &s_walk, lane, n_stages, s_stop);
     } else {
         // ================================ consumer warps ================================
         // warp w owns rows kPairs*w .. kPairs*w + kPairs-1 of the tile; a lane owns x = lane and lane+32 on each of them
         const bool check_last = (p.options & GMPI_CHECK_LAST_PLANE) != 0;
         const bool minus1_1 = (p.options & GMPI_COLOR_MINUS1_1) != 0;
+        const float tau = kES ? p.early_stop : 0.0f;
         int c_stage = 0;            // ring position of this warp: stage index and mbarrier phase parity
         uint32_t c_phase = 0;
         uint32_t flag = 0;
@@ -575,6 +616,8 @@ mpi_fwd_staged_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps
 #pragma unroll
             for (int P = 0; P < kPairs; ++P) { T[P] = splat(1.f); cr[P] = cg[P] = cb[P] = cws[P] = splat(0.f); }
             PlaneConst pc_next = s_pc[0];
+            bool warp_stopped = false;     // kES: every pixel of this warp has stopped (warp-uniform)
+            uint32_t* const stop_word = kES ? s_stop + (j & (kStopSlots - 1)) : nullptr;
             for (int i = 0; i < N; ++i) {
                 const int s = c_stage;
                 const uint32_t ph = c_phase;
@@ -584,7 +627,7 @@ mpi_fwd_staged_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps
                 CoordPairs cc;
                 // Coordinates before the wait.  (Computing plane i+1's coordinates in the shadow of plane i's tap loads was
                 // measured twice: -3 to -4 %; warps in their arithmetic phase leave the shared-memory pipe to the others.)
-                if (warp_fast) coords_pairs<kAlignCorners>(pcc, rp, ex2, ey2, hsx2, hsy2, fWt, fHt, cc);
+                if (warp_fast && !warp_stopped) coords_pairs<kAlignCorners>(pcc, rp, ex2, ey2, hsx2, hsy2, fWt, fHt, cc);
                 if (kEmitT) {              // training: save T_i (before plane i) for the backward sweep, [V,N,H,W]
                     float* ts = p.transmittance + ((size_t)v * N + i) * img;
 #pragma unroll
@@ -597,17 +640,17 @@ mpi_fwd_staged_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps
                 const StageMeta mt = s_meta[s];
                 const float* sb = s_buf + s * kRingFloats;
                 const int sel = mt.sel;                  // warp-uniform; the producer already folded mode and plane range in
-                bool done = false;
-                if (warp_fast) {
+                bool done = warp_stopped;                // a stopped warp only waits on and releases the stage
+                if (warp_fast && !done) {
                     if (Ring::kWideFact) {               // factored: two widths, both with bank-aligned row pitches
-                        if (sel & (1 << 20)) done = sample_pairs<kWideBW, kAOff>(sb, mt.cx, mt.cy, mt.rows2, cc, T, cr, cg, cb, cws);
-                        else if (sel & (1 << 17)) done = sample_pairs<64, kAOff>(sb, mt.cx, mt.cy, mt.rows2, cc, T, cr, cg, cb, cws);
+                        if (sel & (1 << 20)) done = sample_pairs<kWideBW, kAOff, kES>(sb, mt.cx, mt.cy, mt.rows2, cc, T, cr, cg, cb, cws, tau);
+                        else if (sel & (1 << 17)) done = sample_pairs<64, kAOff, kES>(sb, mt.cx, mt.cy, mt.rows2, cc, T, cr, cg, cb, cws, tau);
                     } else {                             // most frequent classes first (FFHQ poses: 72 > 64 > 80 >> 56, 88)
-                        if (sel & (1 << 18)) done = sample_pairs<72, kAOff>(sb, mt.cx, mt.cy, mt.rows2, cc, T, cr, cg, cb, cws);
-                        else if (sel & (1 << 17)) done = sample_pairs<64, kAOff>(sb, mt.cx, mt.cy, mt.rows2, cc, T, cr, cg, cb, cws);
-                        else if (sel & (1 << 19)) done = sample_pairs<80, kAOff>(sb, mt.cx, mt.cy, mt.rows2, cc, T, cr, cg, cb, cws);
-                        else if (sel & (1 << 16)) done = sample_pairs<56, kAOff>(sb, mt.cx, mt.cy, mt.rows2, cc, T, cr, cg, cb, cws);
-                        else if (sel & (1 << 20)) done = sample_pairs<88, kAOff>(sb, mt.cx, mt.cy, mt.rows2, cc, T, cr, cg, cb, cws);
+                        if (sel & (1 << 18)) done = sample_pairs<72, kAOff, kES>(sb, mt.cx, mt.cy, mt.rows2, cc, T, cr, cg, cb, cws, tau);
+                        else if (sel & (1 << 17)) done = sample_pairs<64, kAOff, kES>(sb, mt.cx, mt.cy, mt.rows2, cc, T, cr, cg, cb, cws, tau);
+                        else if (sel & (1 << 19)) done = sample_pairs<80, kAOff, kES>(sb, mt.cx, mt.cy, mt.rows2, cc, T, cr, cg, cb, cws, tau);
+                        else if (sel & (1 << 16)) done = sample_pairs<56, kAOff, kES>(sb, mt.cx, mt.cy, mt.rows2, cc, T, cr, cg, cb, cws, tau);
+                        else if (sel & (1 << 20)) done = sample_pairs<88, kAOff, kES>(sb, mt.cx, mt.cy, mt.rows2, cc, T, cr, cg, cb, cws, tau);
                     }
                 }
                 if (!done) {
@@ -623,6 +666,7 @@ mpi_fwd_staged_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps
                     float* cwss = reinterpret_cast<float*>(cws);
 #pragma unroll
                     for (int q = 0; q < kPix; ++q) {
+                        if (kES && fabsf(Ts[q]) <= tau) continue;   // stopped pixel: adds nothing
                         RayConst rg = rc[q];
                         rg.fast = false;            // rare path: plain IEEE divisions, no per-plane range checks in the hot loop
                         const TexCoord tc = plane_coord<kAlignCorners>(pcc, rg, hsx, hsy, fWt, fHt);
@@ -654,6 +698,15 @@ mpi_fwd_staged_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps
                         Ts[q] -= w;
                     }
                 }
+                if constexpr (kES) {
+                    if (!warp_stopped) {           // one vote per plane; the bit is published by the arrive below
+                        bool st = true;
+#pragma unroll
+                        for (int P = 0; P < kPairs; ++P) st = st && fabsf(T[P].x) <= tau && fabsf(T[P].y) <= tau;
+                        warp_stopped = __all_sync(0xffffffffu, st);
+                        if (warp_stopped && i + 1 < N && lane_ == 0) atomicOr(stop_word, 1u << warp);
+                    }
+                }
                 __syncwarp();
                 mbar_arrive_if(&s_empty[s], lane_ == 0);    // predicated, no branch
             }
@@ -682,6 +735,23 @@ mpi_fwd_staged_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps
         }
         if (flag) atomicOr(p.flags, flag);
     }
+}
+
+template <bool kAlignCorners, bool kEmitT, bool kFactored>
+__global__ void __launch_bounds__(kStagedThreads, 1)
+mpi_fwd_staged_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps, const int tiles_x, const int tiles_y,
+                      const int ring_stages) {
+    fwd_staged_body<kAlignCorners, kEmitT, kFactored, false>(p, maps, tiles_x, ring_stages, nullptr);
+}
+
+// GMPI_EARLY_STOP: the same kernel with the per-pixel early stop (forward only: no transmittance output), a kernel of its own so
+// that the default one keeps its machine code.
+template <bool kAlignCorners, bool kFactored>
+__global__ void __launch_bounds__(kStagedThreads, 1)
+mpi_fwd_early_stop_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps, const int tiles_x, const int tiles_y,
+                          const int ring_stages) {
+    __shared__ uint32_t s_stop[kStopSlots];
+    fwd_staged_body<kAlignCorners, false, kFactored, true>(p, maps, tiles_x, ring_stages, s_stop);
 }
 
 }  // namespace gmpi

@@ -5,6 +5,7 @@
 #include <cuda_runtime.h>
 #include <stdarg.h>
 #include <stdint.h>
+#include <math.h>
 #include <stdio.h>
 #include <string.h>
 
@@ -48,9 +49,10 @@ static int fail(int code, const char* fmt, ...) {
 constexpr int kFwdTileW = 32;
 constexpr int kFwdTileH = 8;
 
-template <bool kAlignCorners>
-__global__ void __launch_bounds__(kFwdTileW* kFwdTileH)
-mpi_fwd_direct_kernel(const RenderParams p) {
+// kES: GMPI_EARLY_STOP, a pixel composites no further plane once |T| <= p.early_stop (mpi_fwd_direct_early_stop_kernel).
+// (p by value: with a reference ptxas allocates the default kernel's registers differently.)
+template <bool kAlignCorners, bool kES>
+__device__ __forceinline__ void fwd_direct_body(const RenderParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     PlaneConst* s_pc = reinterpret_cast<PlaneConst*>(smem_raw);
 
@@ -82,18 +84,19 @@ mpi_fwd_direct_kernel(const RenderParams p) {
         const float hsx = 0.5f * (float)(Wt - 1), hsy = 0.5f * (float)(Ht - 1);
         const size_t tex = (size_t)Ht * Wt;
         const bool check_last = (p.options & GMPI_CHECK_LAST_PLANE) != 0;
+        const float tau = kES ? p.early_stop : 0.0f;
 
         float T = 1.0f, cr = 0.0f, cg = 0.0f, cb = 0.0f, cws = 0.0f;
 #pragma unroll 2
         for (int i = 0; i < p.N; ++i) {
             const PlaneConst pc = s_pc[i];
             const PlaneChans plane = plane_chans(p, m, i, tex);
-            if (p.transmittance) p.transmittance[((size_t)v * p.N + i) * img + pix] = T;   // training: T_i for the backward sweep
+            if (!kES && p.transmittance) p.transmittance[((size_t)v * p.N + i) * img + pix] = T;   // training: T_i for the backward sweep
             const TexCoord tc = plane_coord<kAlignCorners>(pc, rc, hsx, hsy, fWt, fHt);
             if (check_last && i == p.N - 1) {
                 if (!(tc.u >= -1.0f && tc.u <= 1.0f && tc.v >= -1.0f && tc.v <= 1.0f)) flag |= GMPI_FLAG_LAST_PLANE_OOB;
             }
-            if (coord_hits(tc.ix, tc.iy, fWt, fHt)) {
+            if (coord_hits(tc.ix, tc.iy, fWt, fHt) && !(kES && fabsf(T) <= tau)) {
                 const Taps t = make_taps(tc.ix, tc.iy, Ht, Wt);
                 const float r = tap4(plane.c[0], t);
                 const float g = tap4(plane.c[1], t);
@@ -116,6 +119,18 @@ mpi_fwd_direct_kernel(const RenderParams p) {
         store_pixel(p, v, img, pix, cr, cg, cb, dep);
     }
     if (flag) atomicOr(p.flags, flag);
+}
+
+template <bool kAlignCorners>
+__global__ void __launch_bounds__(kFwdTileW* kFwdTileH)
+mpi_fwd_direct_kernel(const RenderParams p) {
+    fwd_direct_body<kAlignCorners, false>(p);
+}
+
+template <bool kAlignCorners>
+__global__ void __launch_bounds__(kFwdTileW* kFwdTileH)
+mpi_fwd_direct_early_stop_kernel(const RenderParams p) {
+    fwd_direct_body<kAlignCorners, true>(p);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -333,6 +348,13 @@ static std::atomic<int> g_fwd_stages{0};    // expanded staged forward's ring de
 
 // Argument checks shared by every entry point.  `bwd`: gradients instead of outputs.
 static int check_params(const RenderParams& p, bool bwd) {
+    if (p.options & GMPI_EARLY_STOP) {
+        if (bwd) return fail(GMPI_ERR_UNSUPPORTED, "GMPI_EARLY_STOP is forward-only: the backward needs every plane's samples");
+        if (p.transmittance)
+            return fail(GMPI_ERR_UNSUPPORTED, "GMPI_EARLY_STOP cannot be combined with the training forward (transmittance)");
+        if (!(p.early_stop >= 0.0f && p.early_stop < 1.0f))
+            return fail(GMPI_ERR_INVALID_ARGUMENT, "early_stop = %g must be in [0, 1) (gmpi_render_desc.early_stop)", (double)p.early_stop);
+    }
     const bool factored = p.alpha != nullptr || p.rgb != nullptr;
     if (factored ? (!p.alpha || !p.rgb || p.rgba) : !p.rgba)
         return fail(GMPI_ERR_INVALID_ARGUMENT, "null input pointer (MPI: pass rgba, or rgb + alpha)");
@@ -416,11 +438,23 @@ static int device_l2_bytes(int* l2) {
     return GMPI_OK;
 }
 
-template <bool AC, bool EMIT, bool FAC>
-static cudaError_t launch_fwd_staged(const RenderParams& p, const TmaMaps& maps, int grid, int tiles_x, int tiles_y, int stages,
-                                     cudaStream_t st) {
-    auto kernel = mpi_fwd_staged_kernel<AC, EMIT, FAC>;
-    const size_t smem = FAC ? kStagedSmemWide : (size_t)stages * kStageFloats * 4 + (size_t)kMaxPlanesStaged * 32;
+// Test hook state of the last early-stop launch: the device counter of stages armed without copies is zeroed on the launch's stream,
+// and the number of (tile, plane) stages it walks is kept here (gmpi_debug_fwd_early_stop_stats).
+static std::atomic<unsigned long long> g_es_total{0};
+
+static int reset_early_stop_stats(unsigned long long total, cudaStream_t st) {
+    void* counter = nullptr;
+    GMPI_CUDA_OK(cudaGetSymbolAddress(&counter, g_early_stop_skipped));
+    GMPI_CUDA_OK(cudaMemsetAsync(counter, 0, sizeof(unsigned long long), st));
+    g_es_total.store(total, std::memory_order_relaxed);
+    return GMPI_OK;
+}
+
+// kernel: an instantiation of mpi_fwd_staged_kernel or mpi_fwd_early_stop_kernel; fac: its kFactored
+template <class Kernel>
+static cudaError_t launch_fwd_staged(Kernel kernel, bool fac, const RenderParams& p, const TmaMaps& maps, int grid, int tiles_x,
+                                     int tiles_y, int stages, cudaStream_t st) {
+    const size_t smem = fac ? kStagedSmemWide : (size_t)stages * kStageFloats * 4 + (size_t)kMaxPlanesStaged * 32;
     cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     kernel<<<grid, kStagedThreads, smem, st>>>(p, maps, tiles_x, tiles_y, stages);
@@ -447,6 +481,7 @@ static int launch_fwd(RenderParams p, cudaStream_t st) {
     // symmetric-memory allocations (256-byte aligned bases; frame slabs are multiples of 16 bytes when W % 4 == 0).
     if (p.W % 4 == 0 && !p.video_rgb && (p.n_peers > 0 || (aligned16(p.color) && aligned16(p.depth)))) p.options |= kOptVec4Stores;
     const bool ac = (p.options & GMPI_ALIGN_CORNERS) != 0, emit = p.transmittance != nullptr, fac = p.alpha != nullptr;
+    const bool es = (p.options & GMPI_EARLY_STOP) != 0;
     if (staged_eligible(p.V, p.N, p.Ht, p.Wt, p.H, p.W) && mpi_aligned(p) && (size_t)p.M * p.N < ((size_t)1 << 31)) {
         TmaMaps maps;
         if (encode_mpi_maps(maps, p, kMaxBH, FwdRingWide::kColourCopyRows, fac) != 0) {
@@ -461,16 +496,22 @@ static int launch_fwd(RenderParams p, cudaStream_t st) {
             const long n_tiles = (long)tiles_x * tiles_y * p.V;
             const int grid = (int)(n_tiles < sms ? n_tiles : sms);
             cudaError_t e;
-            if (fac) {
-                if (ac && emit) e = launch_fwd_staged<true, true, true>(p, maps, grid, tiles_x, tiles_y, stages, st);
-                else if (ac) e = launch_fwd_staged<true, false, true>(p, maps, grid, tiles_x, tiles_y, stages, st);
-                else if (emit) e = launch_fwd_staged<false, true, true>(p, maps, grid, tiles_x, tiles_y, stages, st);
-                else e = launch_fwd_staged<false, false, true>(p, maps, grid, tiles_x, tiles_y, stages, st);
+            if (es) {        // (never with emit: check_params)
+                if ((rc = reset_early_stop_stats((unsigned long long)n_tiles * p.N, st)) != 0) return rc;
+                if (fac) e = ac ? launch_fwd_staged(mpi_fwd_early_stop_kernel<true, true>, fac, p, maps, grid, tiles_x, tiles_y, stages, st)
+                                : launch_fwd_staged(mpi_fwd_early_stop_kernel<false, true>, fac, p, maps, grid, tiles_x, tiles_y, stages, st);
+                else e = ac ? launch_fwd_staged(mpi_fwd_early_stop_kernel<true, false>, fac, p, maps, grid, tiles_x, tiles_y, stages, st)
+                            : launch_fwd_staged(mpi_fwd_early_stop_kernel<false, false>, fac, p, maps, grid, tiles_x, tiles_y, stages, st);
+            } else if (fac) {
+                if (ac && emit) e = launch_fwd_staged(mpi_fwd_staged_kernel<true, true, true>, fac, p, maps, grid, tiles_x, tiles_y, stages, st);
+                else if (ac) e = launch_fwd_staged(mpi_fwd_staged_kernel<true, false, true>, fac, p, maps, grid, tiles_x, tiles_y, stages, st);
+                else if (emit) e = launch_fwd_staged(mpi_fwd_staged_kernel<false, true, true>, fac, p, maps, grid, tiles_x, tiles_y, stages, st);
+                else e = launch_fwd_staged(mpi_fwd_staged_kernel<false, false, true>, fac, p, maps, grid, tiles_x, tiles_y, stages, st);
             } else {
-                if (ac && emit) e = launch_fwd_staged<true, true, false>(p, maps, grid, tiles_x, tiles_y, stages, st);
-                else if (ac) e = launch_fwd_staged<true, false, false>(p, maps, grid, tiles_x, tiles_y, stages, st);
-                else if (emit) e = launch_fwd_staged<false, true, false>(p, maps, grid, tiles_x, tiles_y, stages, st);
-                else e = launch_fwd_staged<false, false, false>(p, maps, grid, tiles_x, tiles_y, stages, st);
+                if (ac && emit) e = launch_fwd_staged(mpi_fwd_staged_kernel<true, true, false>, fac, p, maps, grid, tiles_x, tiles_y, stages, st);
+                else if (ac) e = launch_fwd_staged(mpi_fwd_staged_kernel<true, false, false>, fac, p, maps, grid, tiles_x, tiles_y, stages, st);
+                else if (emit) e = launch_fwd_staged(mpi_fwd_staged_kernel<false, true, false>, fac, p, maps, grid, tiles_x, tiles_y, stages, st);
+                else e = launch_fwd_staged(mpi_fwd_staged_kernel<false, false, false>, fac, p, maps, grid, tiles_x, tiles_y, stages, st);
             }
             GMPI_CUDA_OK(e);
             GMPI_CUDA_OK(cudaGetLastError());
@@ -484,15 +525,11 @@ static int launch_fwd(RenderParams p, cudaStream_t st) {
     dim3 grid((p.W + kFwdTileW - 1) / kFwdTileW, (p.H + kFwdTileH - 1) / kFwdTileH, p.V);
     if (grid.y > 65535) return fail(GMPI_ERR_UNSUPPORTED, "image height %d too large", p.H);
     if (p.V > 65535) return fail(GMPI_ERR_UNSUPPORTED, "V=%d views exceed one launch of the direct kernel (65535); split the batch", p.V);
-    if (ac) {
-        if (smem > 48 * 1024)
-            GMPI_CUDA_OK(cudaFuncSetAttribute(mpi_fwd_direct_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        mpi_fwd_direct_kernel<true><<<grid, block, smem, st>>>(p);
-    } else {
-        if (smem > 48 * 1024)
-            GMPI_CUDA_OK(cudaFuncSetAttribute(mpi_fwd_direct_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        mpi_fwd_direct_kernel<false><<<grid, block, smem, st>>>(p);
-    }
+    if (es && (rc = reset_early_stop_stats(0, st)) != 0) return rc;    // the direct kernel loads per pixel: no stages to skip
+    void (*kernel)(const RenderParams) = es ? (ac ? mpi_fwd_direct_early_stop_kernel<true> : mpi_fwd_direct_early_stop_kernel<false>)
+                                            : (ac ? mpi_fwd_direct_kernel<true> : mpi_fwd_direct_kernel<false>);
+    if (smem > 48 * 1024) GMPI_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kernel<<<grid, block, smem, st>>>(p);
     GMPI_CUDA_OK(cudaGetLastError());
     return GMPI_OK;
 }
@@ -592,14 +629,19 @@ static RenderParams params_from_desc(const gmpi_render_desc* d) {
     p.M = d->M; p.V = d->V; p.N = d->N; p.Ht = d->Ht; p.Wt = d->Wt; p.H = d->H; p.W = d->W;
     p.view_group = d->view_group;
     p.options = d->options & 0xffffu;      // the upper bits are internal
+    // a descriptor of the previous size (GMPI_RENDER_DESC_V2_BYTES) ends before early_stop: check_desc refused GMPI_EARLY_STOP there
+    p.early_stop = d->struct_bytes == sizeof(gmpi_render_desc) ? d->early_stop : 0.0f;
     return p;
 }
 
 static int check_desc(const gmpi_render_desc* d) {
     if (!d) return fail(GMPI_ERR_INVALID_ARGUMENT, "null descriptor");
-    if (d->struct_bytes != sizeof(gmpi_render_desc))
-        return fail(GMPI_ERR_INVALID_ARGUMENT, "gmpi_render_desc.struct_bytes = %u, this library expects %zu (ABI %d)", d->struct_bytes,
-                    sizeof(gmpi_render_desc), GMPI_ABI_VERSION);
+    if (d->struct_bytes != sizeof(gmpi_render_desc) && d->struct_bytes != GMPI_RENDER_DESC_V2_BYTES)
+        return fail(GMPI_ERR_INVALID_ARGUMENT, "gmpi_render_desc.struct_bytes = %u, this library expects %zu or %zu (ABI %d)", d->struct_bytes,
+                    sizeof(gmpi_render_desc), (size_t)GMPI_RENDER_DESC_V2_BYTES, GMPI_ABI_VERSION);
+    if (d->struct_bytes != sizeof(gmpi_render_desc) && (d->options & GMPI_EARLY_STOP))
+        return fail(GMPI_ERR_INVALID_ARGUMENT, "GMPI_EARLY_STOP needs struct_bytes = %zu (a descriptor with the early_stop field)",
+                    sizeof(gmpi_render_desc));
     return GMPI_OK;
 }
 
@@ -610,6 +652,7 @@ static RenderParams params_classic(const float* rgba, const int32_t* view2mpi, c
     p.M = M; p.V = V; p.N = N; p.Ht = Ht; p.Wt = Wt; p.H = H; p.W = W;
     p.options = options & 0xffffu;
     p.view_group = 1;
+    p.early_stop = (options & GMPI_EARLY_STOP) ? NAN : 0.0f;   // the threshold is a descriptor field: check_params refuses the bit here
     return p;
 }
 
@@ -629,6 +672,14 @@ int gmpi_debug_set_fwd_stages(int stages) {
     if (stages != 0 && stages != kStreamStages && stages != kStages)
         return fail(GMPI_ERR_INVALID_ARGUMENT, "stages must be 0 (auto), %d or %d", kStreamStages, kStages);
     g_fwd_stages.store(stages, std::memory_order_relaxed);
+    return GMPI_OK;
+}
+
+int gmpi_debug_fwd_early_stop_stats(unsigned long long* skipped, unsigned long long* total) {
+    if (!skipped || !total) return fail(GMPI_ERR_INVALID_ARGUMENT, "null pointer");
+    GMPI_CUDA_OK(cudaDeviceSynchronize());
+    GMPI_CUDA_OK(cudaMemcpyFromSymbol(skipped, g_early_stop_skipped, sizeof(unsigned long long)));
+    *total = g_es_total.load(std::memory_order_relaxed);
     return GMPI_OK;
 }
 

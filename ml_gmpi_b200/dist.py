@@ -103,7 +103,9 @@ class FrameGather:
         return self._bufs[self._done]
 
     def render(self, rgba, dhw, view2mpi, ray_dir, eye, z_dir, flags, *, align_corners=True, check_last_plane=False,
-               color_minus1_1=False):
+               color_minus1_1=False, early_stop=None):
+        """early_stop: early ray termination threshold in [0, 1), as in render_frames (None: off)."""
+        import ctypes
         from . import _lib
         lib = _lib.load()
         M, N, _, Ht, Wt = rgba.shape
@@ -113,13 +115,13 @@ class FrameGather:
             assert t.is_cuda and t.dtype == torch.float32 and t.is_contiguous(), f"{name} must be a contiguous fp32 CUDA tensor"
         assert view2mpi.dtype == torch.int32 and view2mpi.is_contiguous() and flags.dtype == torch.int32
         options = (_lib.OPT_ALIGN_CORNERS if align_corners else 0) | (_lib.OPT_CHECK_LAST_PLANE if check_last_plane else 0) \
-            | (_lib.OPT_COLOR_MINUS1_1 if color_minus1_1 else 0)
+            | (_lib.OPT_COLOR_MINUS1_1 if color_minus1_1 else 0) | (_lib.OPT_EARLY_STOP if early_stop is not None else 0)
         with torch.cuda.device(rgba.device):
-            _lib.check(lib.gmpi_mpi_render_fwd_gather(
-                rgba.data_ptr(), view2mpi.data_ptr(), dhw.data_ptr(), ray_dir.data_ptr(), eye.data_ptr(), z_dir.data_ptr(),
-                self._peer_ptrs[self._next].data_ptr(), int(self._peer_ptrs[self._next].numel()), self.rank * self.frames_per_rank,
-                flags.data_ptr(),
-                M, V, N, Ht, Wt, self.H, self.W, options, torch.cuda.current_stream(rgba.device).cuda_stream))
+            d = _lib.make_desc(options=options, M=M, V=V, N=N, Ht=Ht, Wt=Wt, H=self.H, W=self.W, rgba=rgba, view2mpi=view2mpi, dhw=dhw,
+                               ray_dir=ray_dir, eye=eye, z_dir=z_dir, peer_frames=self._peer_ptrs[self._next],
+                               n_peers=int(self._peer_ptrs[self._next].numel()), frame_offset=self.rank * self.frames_per_rank,
+                               flags=flags, stream=torch.cuda.current_stream(rgba.device).cuda_stream, early_stop=early_stop)
+            _lib.check(lib.gmpi_mpi_render_fwd_ex(ctypes.byref(d)))
 
     def finish(self):
         """Barrier across ranks on the current stream: after it, every rank's `frames` holds all ranks' frames."""

@@ -36,7 +36,7 @@ class _RenderFn(torch.autograd.Function):
     The MPI is either expanded (`rgba`) or factored (`rgb`, `alpha`, optional `bg_rgb`); the unused form is None."""
 
     @staticmethod
-    def forward(ctx, rgba, rgb, alpha, bg_rgb, dhw, view2mpi, ray_dir, eye, z_dir, options, flags, view_group):
+    def forward(ctx, rgba, rgb, alpha, bg_rgb, dhw, view2mpi, ray_dir, eye, z_dir, options, flags, view_group, early_stop):
         lib = _lib.load()
         factored = rgba is None
         ref = alpha if factored else rgba
@@ -54,7 +54,8 @@ class _RenderFn(torch.autograd.Function):
         with torch.cuda.device(dev):
             d = _lib.make_desc(options=options, M=M, V=V, N=N, Ht=Ht, Wt=Wt, H=H, W=W, view_group=view_group, rgba=rgba, rgb=rgb,
                                alpha=alpha, bg_rgb=bg_rgb, view2mpi=view2mpi, dhw=dhw, ray_dir=ray_dir, eye=eye, z_dir=z_dir,
-                               color=color, depth=depth, transmittance=trans, flags=flags, stream=_stream_ptr(dev))
+                               color=color, depth=depth, transmittance=trans, flags=flags, stream=_stream_ptr(dev),
+                               early_stop=early_stop)
             _lib.check(lib.gmpi_mpi_render_fwd_ex(ctypes.byref(d)))
         ctx.save_for_backward(rgba, rgb, alpha, bg_rgb, dhw, view2mpi, ray_dir, eye, z_dir, trans)
         ctx.options, ctx.view_group = options, view_group
@@ -65,7 +66,7 @@ class _RenderFn(torch.autograd.Function):
     @torch.autograd.function.once_differentiable     # raw kernels: a double backward (create_graph=True) must raise, not
     def backward(ctx, g_color, g_depth):             # silently treat the result as constant (the reference's R1 only differentiates D)
         rgba, rgb, alpha, bg_rgb, dhw, view2mpi, ray_dir, eye, z_dir, trans = ctx.saved_tensors
-        none = (None,) * 12
+        none = (None,) * 13
         if not any(ctx.needs_input_grad[:4]):
             return none
         lib = _lib.load()
@@ -94,7 +95,7 @@ class _RenderFn(torch.autograd.Function):
                                ray_dir=ray_dir, eye=eye, z_dir=z_dir, transmittance=trans, g_color=g_color, g_depth=g_depth,
                                g_rgba=g_rgba, g_rgb=g_rgb, g_bg_rgb=g_bg, g_alpha=g_alpha, stream=_stream_ptr(dev))
             _lib.check(lib.gmpi_mpi_render_bwd_ex(ctypes.byref(d)))
-        return (g_rgba, g_rgb, g_alpha, g_bg) + (None,) * 8
+        return (g_rgba, g_rgb, g_alpha, g_bg) + (None,) * 9
 
 
 _warned_direct = set()
@@ -115,33 +116,47 @@ def _warn_if_direct(ref, V, H, W):
                       f"kernels, several times slower than the TMA-staged path: {reasons}", RuntimeWarning, stacklevel=3)
 
 
-def _options(align_corners, check_last_plane, color_minus1_1, u8_round=False):
+def _options(align_corners, check_last_plane, color_minus1_1, u8_round=False, early_stop=None):
     return (_lib.OPT_ALIGN_CORNERS if align_corners else 0) | (_lib.OPT_CHECK_LAST_PLANE if check_last_plane else 0) \
-        | (_lib.OPT_COLOR_MINUS1_1 if color_minus1_1 else 0) | (_lib.OPT_U8_ROUND_HALF_UP if u8_round else 0)
+        | (_lib.OPT_COLOR_MINUS1_1 if color_minus1_1 else 0) | (_lib.OPT_U8_ROUND_HALF_UP if u8_round else 0) \
+        | (_lib.OPT_EARLY_STOP if early_stop is not None else 0)
+
+
+def _check_early_stop_without_grad(early_stop, *inputs):
+    """early_stop drops the planes behind opaque content, which the backward needs: refuse it where autograd would record."""
+    if early_stop is not None and torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in inputs):
+        raise RuntimeError("ml_gmpi_b200: early_stop is forward-only (it skips the planes the backward needs); render under "
+                           "torch.no_grad() or from inputs that do not require grad")
 
 
 def render_views(rgba, dhw, view2mpi, ray_dir, eye, z_dir, *, align_corners=True, check_last_plane=False,
-                 color_minus1_1=False, flags: Optional[torch.Tensor] = None, view_group: int = 1):
+                 color_minus1_1=False, flags: Optional[torch.Tensor] = None, view_group: int = 1, early_stop: Optional[float] = None):
     """Functional form on packed tensors (no list handling, no host sync).
     rgba [M,N,4,Ht,Wt], dhw [M,N,3], view2mpi [V] int32, ray_dir [V,3,H,W], eye/z_dir [V,3].
     Returns (color [V,3,H,W], depth [V,1,H,W]); `flags` (uint32 tensor of 1, int32 storage) is OR-ed into.
-    view_group > 1: every view_group consecutive views share one MPI (tile-order hint: L2 reuse, see the C header)."""
+    view_group > 1: every view_group consecutive views share one MPI (tile-order hint: L2 reuse, see the C header).
+    early_stop = tau in [0, 1): a pixel composites no further plane once its transmittance |T| <= tau (each colour channel moves by
+    at most tau, 2 tau in [-1,1]; see gmpi_render_desc.early_stop).  Forward only: refused when an input requires grad."""
+    _check_early_stop_without_grad(early_stop, rgba)
     if not rgba.is_cuda:
         raise RuntimeError("ml_gmpi_b200 renders on CUDA devices only (no CPU fallback); got a CPU tensor")
     if flags is None:
         flags = torch.zeros(1, dtype=torch.int32, device=rgba.device)
     _warn_if_direct(rgba, ray_dir.shape[0], ray_dir.shape[2], ray_dir.shape[3])
     return _RenderFn.apply(_as_f32c(rgba), None, None, None, _as_f32c(dhw), view2mpi, _as_f32c(ray_dir), _as_f32c(eye), _as_f32c(z_dir),
-                           _options(align_corners, check_last_plane, color_minus1_1), flags, int(view_group))
+                           _options(align_corners, check_last_plane, color_minus1_1, early_stop=early_stop), flags, int(view_group),
+                           early_stop)
 
 
 def render_views_factored(rgb, alpha, dhw, view2mpi, ray_dir, eye, z_dir, *, bg_rgb=None, align_corners=True,
-                          check_last_plane=False, color_minus1_1=False, flags: Optional[torch.Tensor] = None, view_group: int = 1):
+                          check_last_plane=False, color_minus1_1=False, flags: Optional[torch.Tensor] = None, view_group: int = 1,
+                          early_stop: Optional[float] = None):
     """The same render from the generator's FACTORED output (networks_cond_on_pos_enc.py:950-975,984): one colour image
     rgb [M,3,Ht,Wt] shared by all planes (bg_rgb [M,3,Ht,Wt]: the last plane's own colour under torgba_sep_background) and
     alpha [M,N,1,Ht,Wt] -- what the reference expands to [M,N,4,Ht,Wt] (and copies per view, train.py:553-558,733-738) before
     rendering.  Output identical to render_views on the expanded stack, 4x fewer HBM bytes; differentiable w.r.t. rgb, alpha
-    and bg_rgb (d/d rgb is the sum over the planes that share it)."""
+    and bg_rgb (d/d rgb is the sum over the planes that share it).  early_stop: as in render_views (forward only)."""
+    _check_early_stop_without_grad(early_stop, rgb, alpha, bg_rgb)
     if not alpha.is_cuda:
         raise RuntimeError("ml_gmpi_b200 renders on CUDA devices only (no CPU fallback); got a CPU tensor")
     assert rgb.ndim == 4 and rgb.shape[1] == 3 and alpha.ndim == 5 and alpha.shape[2] == 1 and rgb.shape[0] == alpha.shape[0] \
@@ -151,8 +166,9 @@ def render_views_factored(rgb, alpha, dhw, view2mpi, ray_dir, eye, z_dir, *, bg_
         flags = torch.zeros(1, dtype=torch.int32, device=alpha.device)
     _warn_if_direct(alpha, ray_dir.shape[0], ray_dir.shape[2], ray_dir.shape[3])
     return _RenderFn.apply(None, _as_f32c(rgb), _as_f32c(alpha), None if bg_rgb is None else _as_f32c(bg_rgb), _as_f32c(dhw), view2mpi,
-                           _as_f32c(ray_dir), _as_f32c(eye), _as_f32c(z_dir), _options(align_corners, check_last_plane, color_minus1_1),
-                           flags, int(view_group))
+                           _as_f32c(ray_dir), _as_f32c(eye), _as_f32c(z_dir),
+                           _options(align_corners, check_last_plane, color_minus1_1, early_stop=early_stop), flags, int(view_group),
+                           early_stop)
 
 
 def expand_factored(rgb, alpha, bg_rgb=None):
@@ -167,11 +183,14 @@ def expand_factored(rgb, alpha, bg_rgb=None):
 
 def render_frames(*, dhw, view2mpi, rgba=None, rgb=None, alpha=None, bg_rgb=None, ray_dir=None, eye=None, z_dir=None, cam=None,
                   align_corners=True, check_last_plane=False, video: Optional[dict] = None, u8_round=False,
-                  flags: Optional[torch.Tensor] = None, view_group: int = 1, H: Optional[int] = None, W: Optional[int] = None):
+                  flags: Optional[torch.Tensor] = None, view_group: int = 1, H: Optional[int] = None, W: Optional[int] = None,
+                  early_stop: Optional[float] = None):
     """Inference-only render with the opt-in fast paths of the C ABI (no autograd):
       cam [V,16]     rays generated in the kernel from the pinhole camera (see camera.cam_params) instead of ray_dir/eye/z_dir;
       video={"near": ray_start, "far": ray_end, "depth": True}   uint8 HWC frames as render_video.py:118-126 builds them:
                      returns (rgb_u8 [V,H,W,3], depth_u8 [V,H,W,1] or None); otherwise (color in [-1,1], depth) fp32.
+      early_stop=tau in [0, 1)   early ray termination: a pixel composites no further plane once its transmittance |T| <= tau
+                     (colour in [-1,1] moves by at most 2 tau per channel, a uint8 code by at most one; see render_views).
     """
     ref = alpha if rgba is None else rgba
     if not ref.is_cuda:
@@ -202,10 +221,10 @@ def render_frames(*, dhw, view2mpi, rgba=None, rgb=None, alpha=None, bg_rgb=None
         depth = torch.empty((V, 1, H, W), device=dev, dtype=torch.float32)
     keep = [_as_f32c(t) if t is not None else None for t in (rgba, rgb, alpha, bg_rgb, dhw)]
     with torch.cuda.device(dev):
-        d = _lib.make_desc(options=_options(align_corners, check_last_plane, True, u8_round), M=M, V=V, N=N, Ht=Ht, Wt=Wt, H=H, W=W,
+        d = _lib.make_desc(options=_options(align_corners, check_last_plane, True, u8_round, early_stop), M=M, V=V, N=N, Ht=Ht, Wt=Wt, H=H, W=W,
                            view_group=int(view_group), depth_near=near, depth_range=rng, rgba=keep[0], rgb=keep[1], alpha=keep[2],
                            bg_rgb=keep[3], view2mpi=view2mpi, dhw=keep[4], ray_dir=ray_dir, eye=eye, z_dir=z_dir, cam=cam, color=color,
-                           depth=depth, video_rgb=v_rgb, video_depth=v_depth, flags=flags, stream=_stream_ptr(dev))
+                           depth=depth, video_rgb=v_rgb, video_depth=v_depth, flags=flags, stream=_stream_ptr(dev), early_stop=early_stop)
         _lib.check(lib.gmpi_mpi_render_fwd_ex(ctypes.byref(d)))
     return (v_rgb, v_depth) if video is not None else (color, depth)
 

@@ -35,7 +35,12 @@ def sweep_angles(n_views: int = 100, horizontal: bool = True, mean: float = 0.0)
     return [float(a) + mean for a in np.linspace(half, -half, n_views).tolist()]
 
 
-def _default_video_render(rgba, dhw, c2w, img_size, fov_deg, near, far, fast_rays, factored):
+def _early_stop_kw(early_stop):
+    """early_stop reaches a render_fn only when it is set, so that custom render functions without the keyword keep working."""
+    return {} if early_stop is None else {"early_stop": early_stop}
+
+
+def _default_video_render(rgba, dhw, c2w, img_size, fov_deg, near, far, fast_rays, factored, early_stop=None):
     from .mpi import render_frames
     dev = dhw.device
     V = c2w.shape[0]
@@ -44,18 +49,20 @@ def _default_video_render(rgba, dhw, c2w, img_size, fov_deg, near, far, fast_ray
     if fast_rays:
         cam = cam_params(c2w.to(dev), focal_from_fov(fov_deg, img_size), img_size, img_size)
         return render_frames(dhw=dhw, view2mpi=v2m, cam=cam, H=img_size, W=img_size, video={"near": near, "far": far},
-                             check_last_plane=True, view_group=V, **kw)
+                             check_last_plane=True, view_group=V, early_stop=early_stop, **kw)
     ray_dir, eye, z_dir = PinholeCamera.from_fov(fov_deg, img_size, img_size).generate_rays(c2w.to(dev))
     return render_frames(dhw=dhw, view2mpi=v2m, ray_dir=ray_dir, eye=eye, z_dir=z_dir, video={"near": near, "far": far},
-                         check_last_plane=True, view_group=V, **kw)
+                         check_last_plane=True, view_group=V, early_stop=early_stop, **kw)
 
 
 def render_video_frames(mpi_rgba: Optional[torch.Tensor], dhw: torch.Tensor, angles: Sequence[float], *, img_size: int, fov_deg: float,
                         ray_start: float, ray_end: float, sphere_center, sphere_r: float, horizontal: bool = True,
                         other_angle: float = 0.0, fast_rays: bool = False, factored: Optional[Tuple] = None,
-                        rank: int = 0, world: int = 1, gather: bool = True, render_fn: Optional[Callable] = None):
+                        rank: int = 0, world: int = 1, gather: bool = True, render_fn: Optional[Callable] = None,
+                        early_stop: Optional[float] = None):
     """All `angles` (yaw sweep if `horizontal`, else pitch sweep; the other angle fixed) of ONE MPI ([1,N,4,T,T], or
-    factored=(rgb [1,3,T,T], alpha [1,N,1,T,T], bg_rgb or None)) as uint8 frames.
+    factored=(rgb [1,3,T,T], alpha [1,N,1,T,T], bg_rgb or None)) as uint8 frames.  early_stop: early ray termination threshold
+    (render_frames; None: off).
     Returns (img [V,H,W,3] uint8, depth [V,H,W,1] uint8) as CPU tensors: all V views when `gather` (every rank), else this rank's
     slice [lo, hi) of shard_range(V, rank, world)."""
     V = len(angles)
@@ -66,7 +73,7 @@ def render_video_frames(mpi_rgba: Optional[torch.Tensor], dhw: torch.Tensor, ang
     c2w = sphere_poses(yaws, pitches, sphere_center, sphere_r)
     fn = render_fn or _default_video_render
     if hi > lo:
-        img, depth = fn(mpi_rgba, dhw, c2w, img_size, fov_deg, ray_start, ray_end, fast_rays, factored)
+        img, depth = fn(mpi_rgba, dhw, c2w, img_size, fov_deg, ray_start, ray_end, fast_rays, factored, **_early_stop_kw(early_stop))
     else:
         dev = dhw.device
         img = torch.empty((0, img_size, img_size, 3), dtype=torch.uint8, device=dev)
@@ -89,7 +96,7 @@ def fid_image_indices(num_imgs: int, rank: int, world: int) -> List[int]:
     return list(range(rank, num_imgs, world))
 
 
-def _default_fid_render(renderer, batch_mpi, img_size, yaws, pitches):
+def _default_fid_render(renderer, batch_mpi, img_size, yaws, pitches, early_stop=None):
     from .mpi import render_frames
     dev = batch_mpi.device
     B = batch_mpi.shape[0]
@@ -98,18 +105,21 @@ def _default_fid_render(renderer, batch_mpi, img_size, yaws, pitches):
     ray_dir, eye, z_dir = cam.generate_rays(c2w)
     dhw = renderer.static_mpi_plane_dhws.to(dev).reshape(1, -1, 3).expand(B, -1, -1).contiguous()
     img, _ = render_frames(rgba=batch_mpi, dhw=dhw, view2mpi=torch.arange(B, dtype=torch.int32, device=dev), ray_dir=ray_dir, eye=eye,
-                           z_dir=z_dir, video={"near": 0.0, "far": 1.0, "depth": False}, u8_round=True, check_last_plane=True)
+                           z_dir=z_dir, video={"near": 0.0, "far": 1.0, "depth": False}, u8_round=True, check_last_plane=True,
+                           early_stop=early_stop)
     return img
 
 
 def dump_fid_images(renderer, mpi_source: Callable[[int], torch.Tensor], num_imgs: int, rank: int, world: int, img_size: int,
                     output_dir: Optional[str] = None, writer: Optional[Callable[[int, np.ndarray], None]] = None,
                     h_mean: float = 0.0, h_std: float = 0.289, v_mean: float = 0.0, v_std: float = 0.127,
-                    generator: Optional[torch.Generator] = None, render_fn: Optional[Callable] = None) -> List[int]:
+                    generator: Optional[torch.Generator] = None, render_fn: Optional[Callable] = None,
+                    early_stop: Optional[float] = None) -> List[int]:
     """Rank `rank`'s share of `num_imgs` images: for every call k, `mpi_source(k)` returns a batch [B,N,4,T,T] of MPIs; each is
     rendered from one random pose (truncated Gaussian, as MPIRenderer.render samples it) and converted to uint8 with
     save_image's rounding.  Images are numbered rank, rank + world, ... (the reference's strided file names) and handed to
-    `writer(index, hwc_uint8)` or written to output_dir/{index:05d}.png.  Returns the indices written."""
+    `writer(index, hwc_uint8)` or written to output_dir/{index:05d}.png.  Returns the indices written.  early_stop: early ray
+    termination threshold (render_frames; None: off)."""
     todo = fid_image_indices(num_imgs, rank, world)
     fn = render_fn or _default_fid_render
     done, k = [], 0
@@ -118,7 +128,7 @@ def dump_fid_images(renderer, mpi_source: Callable[[int], torch.Tensor], num_img
         k += 1
         B = batch.shape[0]
         yaws, pitches = sample_yaw_pitch(B, h_mean, h_std, v_mean, v_std, 2, "truncated_gaussian", True, generator=generator)
-        imgs = fn(renderer, batch, img_size, yaws, pitches).cpu().numpy()
+        imgs = fn(renderer, batch, img_size, yaws, pitches, **_early_stop_kw(early_stop)).cpu().numpy()
         for img in imgs:
             if len(done) == len(todo):
                 break
@@ -139,7 +149,7 @@ def to_uint8_truncating(img_m11: torch.Tensor) -> torch.Tensor:
     return (torch.clamp((img_m11 + 1) / 2.0, 0.0, 1.0) * 255).to(torch.uint8)
 
 
-def _default_eval_render(renderer, batch_mpi, n_imgs, img_size, yaws, pitches):
+def _default_eval_render(renderer, batch_mpi, n_imgs, img_size, yaws, pitches, early_stop=None):
     from .mpi import render_frames
     dev = batch_mpi.device
     B = batch_mpi.shape[0]
@@ -148,20 +158,21 @@ def _default_eval_render(renderer, batch_mpi, n_imgs, img_size, yaws, pitches):
     dhw = renderer.static_mpi_plane_dhws.to(dev).reshape(1, -1, 3).expand(B, -1, -1).contiguous()
     view2mpi = torch.arange(B, dtype=torch.int32, device=dev).repeat_interleave(n_imgs)
     return render_frames(rgba=batch_mpi, dhw=dhw, view2mpi=view2mpi, ray_dir=ray_dir, eye=eye, z_dir=z_dir, check_last_plane=True,
-                         view_group=n_imgs)                              # (colour in [-1,1] [V,3,H,W], depth [V,1,H,W])
+                         view_group=n_imgs, early_stop=early_stop)                              # (colour in [-1,1] [V,3,H,W], depth [V,1,H,W])
 
 
 def render_eval_views(renderer, batch_mpi: torch.Tensor, n_imgs: int, img_size: int, *, generator: Optional[torch.Generator] = None,
-                      render_fn: Optional[Callable] = None):
+                      render_fn: Optional[Callable] = None, early_stop: Optional[float] = None):
     """batch_mpi [B,N,4,T,T] -> (img uint8 [B*n_imgs,H,W,3], depth fp32 [B*n_imgs,H,W,1], angles fp32 [B*n_imgs,2] = (pitch,
     yaw)) as numpy arrays, views MPI-major (the n_imgs views of MPI 0 first) like the reference's expand.  Poses are drawn
-    as MPIRenderer.render draws them for a batch of B*n_imgs (same generator consumption: mpi_renderer.py:418-434)."""
+    as MPIRenderer.render draws them for a batch of B*n_imgs (same generator consumption: mpi_renderer.py:418-434).
+    early_stop: early ray termination threshold (render_frames; None: off)."""
     B = batch_mpi.shape[0]
     V = B * int(n_imgs)
     yaws, pitches = sample_yaw_pitch(V, renderer.horizontal_mean, renderer.horizontal_std, renderer.vertical_mean, renderer.vertical_std,
                                      renderer.cam_pose_n_truncated_stds, renderer.cam_sample_method, True, generator=generator)
     fn = render_fn or _default_eval_render
-    img, depth = fn(renderer, batch_mpi, int(n_imgs), img_size, yaws, pitches)
+    img, depth = fn(renderer, batch_mpi, int(n_imgs), img_size, yaws, pitches, **_early_stop_kw(early_stop))
     assert img.shape[0] == V and depth.shape[0] == V, f"{img.shape}, {depth.shape}, {V}"
     img_u8 = to_uint8_truncating(img.permute(0, 2, 3, 1)).cpu().numpy()
     angles = torch.cat([pitches, yaws], dim=-1).numpy()                 # mpi_renderer.py:464

@@ -60,3 +60,34 @@ def make_case(*, n_planes, tex, img, n_mpi, views_per_mpi=1, seed=1234, device="
     dhw = ffhq_dhw(n_planes).to(device).unsqueeze(0).expand(n_mpi, -1, -1).contiguous()
     v2m = torch.arange(n_mpi, dtype=torch.int32, device=device).repeat_interleave(views_per_mpi)
     return Case(t, dhw, v2m, ray_dir, eye, z_dir, c2w, yaws, pitches)
+
+
+def head_alpha(n_planes: int, tex: int, device="cpu") -> torch.Tensor:
+    """[N,T,T] alpha of a structured synthetic MPI: a transparent volume with an opaque ellipsoidal "head" (semi-axes 0.8 x 0.95
+    of the texture, about 60 % of the frame) whose front surface crosses K = max(2, N // 16) planes around the middle, plus the
+    alpha == 1 last plane of a GMPI MPI (networks_cond_on_pos_enc.py:1307-1310).  Plane c0 + k is opaque where the surface lies in
+    front of or on it (a disc that widens with depth), so pixels stop at different planes and the rim (partial bilinear alpha)
+    stays transparent until the last plane.  A trained MPI has not been measured against it."""
+    K = max(2, n_planes // 16)
+    c0 = max(0, n_planes // 2 - K // 2)
+    ax = torch.linspace(-1.0, 1.0, tex, device=device)
+    y, x = torch.meshgrid(ax, ax, indexing="ij")
+    r2 = (x / 0.8) ** 2 + (y / 0.95) ** 2
+    depth = (1.0 - torch.sqrt(torch.clamp(1.0 - r2, min=0.0))) * K      # front surface, in planes behind c0
+    alpha = torch.zeros((n_planes, tex, tex), device=device)
+    for k in range(K):
+        if c0 + k < n_planes:
+            alpha[c0 + k] = ((r2 < 1.0) & (depth < k + 1)).float()
+    alpha[-1] = 1.0
+    return alpha
+
+
+def make_head_case(*, n_planes, tex, img, n_mpi, views_per_mpi=1, seed=1234, device="cpu", yaws=None, pitches=None) -> Case:
+    """make_case with random colours and head_alpha's alpha (tools/early_stop_bench.py and the early-stop tests)."""
+    case = make_case(n_planes=n_planes, tex=tex, img=img, n_mpi=n_mpi, views_per_mpi=views_per_mpi, seed=seed, device=device,
+                     yaws=yaws, pitches=pitches, rgba=False)
+    gen = torch.Generator(device=device).manual_seed(seed)
+    rgba = torch.rand((n_mpi, n_planes, 4, tex, tex), generator=gen, device=device, dtype=torch.float32)
+    rgba[:, :, 3] = head_alpha(n_planes, tex, device)
+    case.rgba = rgba
+    return case
