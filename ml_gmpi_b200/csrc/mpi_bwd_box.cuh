@@ -158,8 +158,6 @@ __device__ __forceinline__ void fix2(f2 vF, f2 w, int& ia, int& ib) {
     ib = ((__float_as_int(t1.y) - kMagicHiBits) << kFixSplit) + (__float_as_int(t2.y) - kFloorMagicBits);
 }
 
-// Fast body: four pixels (two packed pairs) from a staged box of compile-time width BW, contributions into the gradient box.
-// Returns false (nothing sampled, R unchanged) if any footprint is not inside the box.
 // One (pair, channel) of the scatter: the four bilinear contributions of two pixels into the gradient box.
 template <int PITCH, bool kTwoStep>
 __device__ __forceinline__ void scatter_channel(int* __restrict__ ga, int* __restrict__ gq, f2 vF, const f2 (&w)[4]) {
@@ -181,51 +179,21 @@ __device__ __forceinline__ void scatter_channel(int* __restrict__ ga, int* __res
 // Fast body: four pixels (two packed pairs) from a staged box of compile-time width BW: sample, form the gradients, add the 64
 // fixed-point contributions to the gradient box `gb` (same layout as the staged box).  Returns false (nothing sampled, R
 // unchanged, nothing added) if any footprint is not inside the box.
-// AOFF as in sample_pairs: 0 = expanded stage, > 0 = factored (colour box [row][3][BW], alpha box [row][BW] at AOFF).
+// AOFF as in BoxTaps: 0 = expanded stage, > 0 = factored (colour box [row][3][BW], alpha box [row][BW] at AOFF).
 // Each pair is scattered as soon as it is formed: keeping both pairs' weights and values alive until a later scatter phase costs
 // ~36 registers and spills.
 template <int BW, int AOFF = 0>
 __device__ __forceinline__ bool bwd_box_pairs(const float* __restrict__ sb, int* __restrict__ gb, int cx, int cy, int rows2, const CoordPairs& c,
                                               const f2 (&T)[kPairs], const GradPairs& G, f2 (&R)[kPairs], f2 Fs, f2 Fs_rgb,
                                               uint64_t* g_empty_bar, uint32_t g_empty_parity) {
-    constexpr int RP = AOFF ? 3 * BW : 4 * BW, AP = AOFF ? BW : 4 * BW, A0 = AOFF ? AOFF : 3 * BW;
-    const f2 m1 = splat(-1.0f), one = splat(1.0f);
-    const f2 magic = splat(kFloorMagic), nmagic = splat(-kFloorMagic);
-    f2 fx0[kPairs], fy0[kPairs];
-    int idx[kPix], jdx[kPix];
-    bool inbox = true;
+    using Box = BoxTaps<BW, AOFF>;
+    const f2 m1 = splat(-1.0f);
+    Box bt;
+    if (!bt.locate(cx, cy, rows2, c)) return false;
 #pragma unroll
     for (int P = 0; P < kPairs; ++P) {
-        const f2 tx = add2_rm(c.ix[P], magic), ty = add2_rm(c.iy[P], magic);
-        fx0[P] = add2(tx, nmagic);
-        fy0[P] = add2(ty, nmagic);
-        const int rxa = __float_as_int(tx.x) - cx, rxb = __float_as_int(tx.y) - cx;
-        const int rya = __float_as_int(ty.x) - cy, ryb = __float_as_int(ty.y) - cy;
-        inbox = inbox && (unsigned)rxa <= (unsigned)(BW - 2) && (unsigned)rxb <= (unsigned)(BW - 2) &&
-                (unsigned)rya <= (unsigned)rows2 && (unsigned)ryb <= (unsigned)rows2;
-        idx[2 * P] = rya * RP + rxa;
-        idx[2 * P + 1] = ryb * RP + rxb;
-        if (AOFF) { jdx[2 * P] = rya * AP + rxa + A0; jdx[2 * P + 1] = ryb * AP + rxb + A0; }     // separate alpha box
-    }
-    if (!__all_sync(0xffffffffu, inbox)) return false;   // warp-uniform
-#pragma unroll
-    for (int P = 0; P < kPairs; ++P) {
-        const f2 wx1 = fma2(fx0[P], m1, c.ix[P]), wy1 = fma2(fy0[P], m1, c.iy[P]);
-        const f2 wy0 = fma2(wy1, m1, one);
-        f2 w[4];
-        w[3] = mul2(wx1, wy1); w[2] = fma2(w[3], m1, wy1); w[1] = fma2(w[3], m1, wx1); w[0] = fma2(w[1], m1, wy0);
-        const float* ta = sb + idx[2 * P];
-        const float* tb = sb + idx[2 * P + 1];
-#define GMPI_TAP(ch)                                                                                           \
-    fma2(make_float2(ta[RP + ch * BW + 1], tb[RP + ch * BW + 1]), w[3],                                        \
-         fma2(make_float2(ta[RP + ch * BW], tb[RP + ch * BW]), w[2],                                           \
-              fma2(make_float2(ta[ch * BW + 1], tb[ch * BW + 1]), w[1], mul2(make_float2(ta[ch * BW], tb[ch * BW]), w[0]))))
-        const f2 r = GMPI_TAP(0), g = GMPI_TAP(1), b = GMPI_TAP(2);
-#undef GMPI_TAP
-        const float* aa = AOFF ? sb + jdx[2 * P] : ta + A0;
-        const float* ab = AOFF ? sb + jdx[2 * P + 1] : tb + A0;
-        const f2 a = fma2(make_float2(aa[AP + 1], ab[AP + 1]), w[3],
-                          fma2(make_float2(aa[AP], ab[AP]), w[2], fma2(make_float2(aa[1], ab[1]), w[1], mul2(make_float2(aa[0], ab[0]), w[0]))));
+        f2 w[4], r, g, b, a;
+        bt.sample(sb, c, P, w, r, g, b, a);
         const f2 q = fma2(G.g0[P], r, fma2(G.g1[P], g, fma2(G.g2[P], b, mul2(G.gs[P], c.sc[P]))));
         const f2 d = fma2(R[P], m1, q);                 // q - R
         const f2 wT = mul2(a, T[P]);
@@ -234,12 +202,12 @@ __device__ __forceinline__ bool bwd_box_pairs(const float* __restrict__ sb, int*
         // The gradient box is needed only from here on: the flushers get the first pair's sampling time to finish emptying it.
         if (P == 0) mbar_wait(g_empty_bar, g_empty_parity);
         const f2 wF = mul2(wT, Fs_rgb);                 // exact (power of two)
-        int* ga = gb + idx[2 * P];
-        int* gq = gb + idx[2 * P + 1];
-        scatter_channel<RP, false>(ga, gq, mul2(G.g0[P], wF), w);
-        scatter_channel<RP, false>(ga + BW, gq + BW, mul2(G.g1[P], wF), w);
-        scatter_channel<RP, false>(ga + 2 * BW, gq + 2 * BW, mul2(G.g2[P], wF), w);
-        scatter_channel<AP, true>(AOFF ? gb + jdx[2 * P] : ga + A0, AOFF ? gb + jdx[2 * P + 1] : gq + A0, mul2(mul2(T[P], d), Fs), w);   // dL/d alpha
+        int* ga = gb + bt.ia[P];
+        int* gq = gb + bt.ib[P];
+        scatter_channel<Box::RP, false>(ga, gq, mul2(G.g0[P], wF), w);
+        scatter_channel<Box::RP, false>(ga + BW, gq + BW, mul2(G.g1[P], wF), w);
+        scatter_channel<Box::RP, false>(ga + 2 * BW, gq + 2 * BW, mul2(G.g2[P], wF), w);
+        scatter_channel<Box::AP, true>(AOFF ? gb + bt.ja[P] : ga + Box::A0, AOFF ? gb + bt.jb[P] : gq + Box::A0, mul2(mul2(T[P], d), Fs), w);   // dL/d alpha
     }
     return true;
 }
@@ -287,8 +255,6 @@ __device__ __forceinline__ void flush_box(int* __restrict__ gb, const GradMeta& 
         }
     }
 }
-
-__device__ __forceinline__ void bwd_consumer_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kBwdConsThreads) : "memory"); }
 
 template <bool kAlignCorners, bool kFactored>
 __global__ void __launch_bounds__(kBwdThreads, 1)
@@ -376,9 +342,9 @@ mpi_bwd_box_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps, c
             const float ev[3] = {__ldg(e), __ldg(e + 1), __ldg(e + 2)};
             const float zd[3] = {__ldg(p.z_dir + 3 * v), __ldg(p.z_dir + 3 * v + 1), __ldg(p.z_dir + 3 * v + 2)};
             if (v != v_table) {          // (view, plane) constants, once per view and CTA
-                bwd_consumer_bar_sync();
+                consumer_bar_sync<kBwdConsThreads>();
                 if (threadIdx.x == 0) s_zmax = 0u;
-                bwd_consumer_bar_sync();
+                consumer_bar_sync<kBwdConsThreads>();
                 float zm = 0.0f;
                 for (int i = threadIdx.x; i < N; i += kBwdConsThreads) {
                     const PlaneConst pc = make_plane_const(p.dhw + ((size_t)m * N + i) * 3, ev[2]);
@@ -386,7 +352,7 @@ mpi_bwd_box_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps, c
                     zm = fmaxf(zm, fabsf(pc.z_diff));
                 }
                 atomicMax(&s_zmax, __float_as_uint(zm));
-                bwd_consumer_bar_sync();
+                consumer_bar_sync<kBwdConsThreads>();
                 v_table = v;
             }
             // ---- per-pixel inputs (clamped into the image; the tile overhang carries zero upstream gradient) ----
@@ -425,7 +391,7 @@ mpi_bwd_box_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps, c
                 }
                 if (lane == 0) { atomicMax(&s_qmax[slot], __float_as_uint(qmax)); atomicMax(&s_gmax[slot], __float_as_uint(gmax)); }
                 if (threadIdx.x == 0) s_qmax[(j + 1) % 3] = s_gmax[(j + 1) % 3] = 0u;   // next tile's slots: their last readers passed the previous tile's barrier
-                bwd_consumer_bar_sync();
+                consumer_bar_sync<kBwdConsThreads>();
                 qmax = __uint_as_float(s_qmax[slot]);
                 gmax = __uint_as_float(s_gmax[slot]);
             }
@@ -442,12 +408,9 @@ mpi_bwd_box_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps, c
             const float inv_scale_rgb = __uint_as_float((unsigned)(127 - kFixBitsRgb + e_rgb) << 23);
 
             const bool idle = py0 + kPairs * warp >= p.H;      // warp-uniform: no row of this warp is inside the image
+            pack_ray_pairs(rc, rp);
 #pragma unroll
             for (int P = 0; P < kPairs; ++P) {
-                rp.rx2[P] = make_float2(rc[2 * P].rx2, rc[2 * P + 1].rx2);
-                rp.ry2[P] = make_float2(rc[2 * P].ry2, rc[2 * P + 1].ry2);
-                rp.nrz[P] = make_float2(-rc[2 * P].rz, -rc[2 * P + 1].rz);
-                rp.yrz[P] = make_float2(rc[2 * P].yrz, rc[2 * P + 1].yrz);
                 G.g0[P] = make_float2(gq[2 * P][0], gq[2 * P + 1][0]);
                 G.g1[P] = make_float2(gq[2 * P][1], gq[2 * P + 1][1]);
                 G.g2[P] = make_float2(gq[2 * P][2], gq[2 * P + 1][2]);

@@ -141,8 +141,6 @@ __device__ __forceinline__ uint8_t depth_to_u8(float depth, float d_near, float 
 }
 
 // Store one finished pixel: plain outputs, or the same frame slot of every rank's gather buffer (NVLink peer stores).
-__device__ __forceinline__ uint8_t color_to_u8(float img_m11, bool round_half_up);
-__device__ __forceinline__ uint8_t depth_to_u8(float depth, float d_near, float d_range);
 __device__ __forceinline__ void store_pixel(const RenderParams& p, int v, size_t img, size_t pix, float c0, float c1, float c2, float dep) {
     if (p.video_rgb) {        // uint8 HWC frame (render_video.py:118-126)
         const bool up = (p.options & GMPI_U8_ROUND_HALF_UP) != 0;

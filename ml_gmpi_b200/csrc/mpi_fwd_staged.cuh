@@ -26,7 +26,7 @@ constexpr int kConsThreads = kConsWarps * 32, kStagedThreads = kConsThreads + 32
 constexpr int kStages = 3, kStreamStages = 2;
 constexpr int kRowsPerOp = 4;
 constexpr int kMaxBW = 88;
-constexpr int kMaxBH = (((kTileH * 5) / 4 + 6 + kRowsPerOp - 1) / kRowsPerOp) * kRowsPerOp;   // footprint rows at scale 1.25 + taps/slack, whole chunks                 // largest staged footprint (texels)
+constexpr int kMaxBH = (((kTileH * 5) / 4 + 6 + kRowsPerOp - 1) / kRowsPerOp) * kRowsPerOp;   // footprint rows at scale 1.25 + taps/slack, whole chunks
 // Box widths are compile-time classes (multiples of 8: row pitch 4*bw = 0 mod 32 banks) so that the consumers'
 // sixteen taps are LDS [reg + immediate]; the producer picks the narrowest class that covers the footprint.
 constexpr int kMinBW = 56, kBWStep = 8;
@@ -40,6 +40,9 @@ constexpr int kWideBW = 96;
 constexpr int kWideStageFloats = kWideBW * kMaxBH * 4;
 constexpr size_t kStagedSmemWide = (size_t)kStages * kWideStageFloats * 4 + (size_t)kMaxPlanesStaged * 32;
 static_assert(kStagedSmemWide + 1024 <= 227 * 1024, "wide factored ring must fit one SM");
+
+// Box width of class k (tensor-map slot k).  In the factored forward's ring (wide) slot 4 holds kWideBW and slot 1 the 64-wide boxes.
+__host__ __device__ constexpr int class_width(int k, bool wide = false) { return wide && k == kNumMaps - 1 ? kWideBW : kMinBW + k * kBWStep; }
 
 struct TmaMaps {
     CUtensorMap m[kNumMaps];      // expanded rgba [M*N][4][Ht][Wt] as (x, channel, y, plane), box {bw, 4, 4 rows, 1}
@@ -92,6 +95,15 @@ struct RayPairs {
     f2 rx2[kPairs], ry2[kPairs];   // 2*ray_x, 2*ray_y
     f2 nrz[kPairs], yrz[kPairs];   // -ray_z, RN(1/ray_z)
 };
+__device__ __forceinline__ void pack_ray_pairs(const RayConst (&rc)[kPix], RayPairs& rp) {
+#pragma unroll
+    for (int P = 0; P < kPairs; ++P) {
+        rp.rx2[P] = make_float2(rc[2 * P].rx2, rc[2 * P + 1].rx2);
+        rp.ry2[P] = make_float2(rc[2 * P].ry2, rc[2 * P + 1].ry2);
+        rp.nrz[P] = make_float2(-rc[2 * P].rz, -rc[2 * P + 1].rz);
+        rp.yrz[P] = make_float2(rc[2 * P].yrz, rc[2 * P + 1].yrz);
+    }
+}
 struct CoordPairs {
     f2 ix[kPairs], iy[kPairs], sc[kPairs];
 };
@@ -126,59 +138,75 @@ __device__ __forceinline__ void coords_pairs(const PlaneConst& pc, const RayPair
     }
 }
 
+// The bilinear footprints of a thread's two pixel pairs in a staged box of compile-time width BW, shared by the forward's and
+// the backward's fast bodies.  AOFF == 0: expanded stage [row][4 channels][BW].  AOFF > 0 (factored MPI): colour box [row][3][BW]
+// at the stage base and the alpha box [row][BW] AOFF floats further on.  The backward's gradient box has the stage's layout, so
+// the same indices address it.
+template <int BW, int AOFF>
+struct BoxTaps {
+    static constexpr int RP = AOFF ? 3 * BW : 4 * BW;       // colour row pitch
+    static constexpr int AP = AOFF ? BW : 4 * BW;           // alpha row pitch
+    static constexpr int A0 = AOFF ? AOFF : 3 * BW;         // alpha offset from the colour index (factored: separate box)
+    f2 fx0[kPairs], fy0[kPairs];                            // floor of the coordinates, as floats
+    int ia[kPairs], ib[kPairs];                             // colour index of the north-west taps of pixels .x and .y of pair P
+    int ja[kPairs], jb[kPairs];                             // factored: alpha index (separate box)
+
+    // Floors and indices of every footprint.  Returns the warp's vote that all of them lie inside the box (warp-uniform, so the
+    // caller's fallback needs no reconvergence scaffolding).
+    __device__ __forceinline__ bool locate(int cx, int cy, int rows2, const CoordPairs& c) {
+        const f2 magic = splat(kFloorMagic), nmagic = splat(-kFloorMagic);
+        bool inbox = true;
+#pragma unroll
+        for (int P = 0; P < kPairs; ++P) {
+            const f2 tx = add2_rm(c.ix[P], magic), ty = add2_rm(c.iy[P], magic);         // floor without the XU pipe
+            fx0[P] = add2(tx, nmagic);                                    // floor as float (exact)
+            fy0[P] = add2(ty, nmagic);
+            const int rxa = __float_as_int(tx.x) - cx, rxb = __float_as_int(tx.y) - cx;   // floor - box origin, as integers
+            const int rya = __float_as_int(ty.x) - cy, ryb = __float_as_int(ty.y) - cy;
+            inbox = inbox && (unsigned)rxa <= (unsigned)(BW - 2) && (unsigned)rxb <= (unsigned)(BW - 2) &&
+                    (unsigned)rya <= (unsigned)rows2 && (unsigned)ryb <= (unsigned)rows2;
+            ia[P] = rya * RP + rxa;                                       // [row][channel][x], compile-time pitch
+            ib[P] = ryb * RP + rxb;
+            if (AOFF) { ja[P] = rya * AP + rxa + A0; jb[P] = ryb * AP + rxb + A0; }
+        }
+        return __all_sync(0xffffffffu, inbox);
+    }
+    // one channel of pair P: the four taps of a box with row pitch PITCH at ta / tb, weighted
+    template <int PITCH>
+    static __device__ __forceinline__ f2 tap2(const float* ta, const float* tb, const f2 (&w)[4]) {
+        return fma2(make_float2(ta[PITCH + 1], tb[PITCH + 1]), w[3],
+                    fma2(make_float2(ta[PITCH], tb[PITCH]), w[2], fma2(make_float2(ta[1], tb[1]), w[1], mul2(make_float2(ta[0], tb[0]), w[0]))));
+    }
+    // bilinear weights w = (w00, w01, w10, w11) and the four channels of pair P from the staged box sb
+    __device__ __forceinline__ void sample(const float* __restrict__ sb, const CoordPairs& c, int P, f2 (&w)[4], f2& r, f2& g, f2& b,
+                                           f2& a) const {
+        const f2 m1 = splat(-1.0f), one = splat(1.0f);
+        const f2 wx1 = fma2(fx0[P], m1, c.ix[P]), wy1 = fma2(fy0[P], m1, c.iy[P]);   // fractional parts (exact)
+        const f2 wy0 = fma2(wy1, m1, one);
+        w[3] = mul2(wx1, wy1); w[2] = fma2(w[3], m1, wy1); w[1] = fma2(w[3], m1, wx1); w[0] = fma2(w[1], m1, wy0);
+        const float* ta = sb + ia[P];
+        const float* tb = sb + ib[P];
+        r = tap2<RP>(ta, tb, w);
+        g = tap2<RP>(ta + BW, tb + BW, w);
+        b = tap2<RP>(ta + 2 * BW, tb + 2 * BW, w);
+        a = AOFF ? tap2<AP>(sb + ja[P], sb + jb[P], w) : tap2<AP>(ta + A0, tb + A0, w);
+    }
+};
+
 // Sample + composite the four pixels from a staged box of compile-time width BW.  Returns false (and changes nothing)
-// if any of the four footprints is not inside the box.
-// AOFF == 0: expanded stage [row][4 channels][BW].  AOFF > 0 (factored MPI): colour box [row][3][BW] at the stage base and
-// the alpha box [row][BW] AOFF floats further on.
+// if any of the four footprints is not inside the box.  AOFF as in BoxTaps.
 // kES (early stop): a pixel whose |T| <= tau adds nothing; its weight is selected to 0, so its T stays where it stopped.
 template <int BW, int AOFF = 0, bool kES = false>
 __device__ __forceinline__ bool sample_pairs(const float* __restrict__ sb, int cx, int cy, int rows2, const CoordPairs& c,
                                              f2 (&T)[kPairs], f2 (&cr)[kPairs], f2 (&cg)[kPairs], f2 (&cb)[kPairs], f2 (&cws)[kPairs],
                                              float tau = 0.0f) {
-    constexpr int RP = AOFF ? 3 * BW : 4 * BW;       // colour row pitch
-    constexpr int AP = AOFF ? BW : 4 * BW;           // alpha row pitch
-    constexpr int A0 = AOFF ? AOFF : 3 * BW;         // alpha offset from the colour index (factored: separate box)
-    const f2 m1 = splat(-1.0f), one = splat(1.0f);
-    f2 fx0[kPairs], fy0[kPairs];
-    int ia[kPairs], ib[kPairs], ja[kPairs], jb[kPairs];
-    bool inbox = true;
-    const f2 magic = splat(kFloorMagic), nmagic = splat(-kFloorMagic);
+    const f2 m1 = splat(-1.0f);
+    BoxTaps<BW, AOFF> bt;
+    if (!bt.locate(cx, cy, rows2, c)) return false;
 #pragma unroll
     for (int P = 0; P < kPairs; ++P) {
-        const f2 tx = add2_rm(c.ix[P], magic), ty = add2_rm(c.iy[P], magic);         // floor without the XU pipe
-        fx0[P] = add2(tx, nmagic);                                    // floor as float (exact)
-        fy0[P] = add2(ty, nmagic);
-        const int rxa = __float_as_int(tx.x) - cx, rxb = __float_as_int(tx.y) - cx;   // floor - box origin, as integers
-        const int rya = __float_as_int(ty.x) - cy, ryb = __float_as_int(ty.y) - cy;
-        inbox = inbox && (unsigned)rxa <= (unsigned)(BW - 2) && (unsigned)rxb <= (unsigned)(BW - 2) &&
-                (unsigned)rya <= (unsigned)rows2 && (unsigned)ryb <= (unsigned)rows2;
-        ia[P] = rya * RP + rxa;                                       // [row][channel][x], compile-time pitch
-        ib[P] = ryb * RP + rxb;
-        if (AOFF) { ja[P] = rya * AP + rxa + A0; jb[P] = ryb * AP + rxb + A0; }   // alpha taps (separate box)
-    }
-    if (!__all_sync(0xffffffffu, inbox)) return false;   // warp-uniform, so the caller's fallback needs no reconvergence scaffolding
-#pragma unroll
-    for (int P = 0; P < kPairs; ++P) {
-        const f2 wx1 = fma2(fx0[P], m1, c.ix[P]), wy1 = fma2(fy0[P], m1, c.iy[P]);   // fractional parts (exact)
-        const f2 wy0 = fma2(wy1, m1, one);
-        const f2 w11 = mul2(wx1, wy1), w10 = fma2(w11, m1, wy1), w01 = fma2(w11, m1, wx1), w00 = fma2(w01, m1, wy0);
-        const float* ta = sb + ia[P];
-        const float* tb = sb + ib[P];
-#define GMPI_TAP(ch)                                                                                           \
-    fma2(make_float2(ta[RP + ch * BW + 1], tb[RP + ch * BW + 1]), w11,                                         \
-         fma2(make_float2(ta[RP + ch * BW], tb[RP + ch * BW]), w10,                                            \
-              fma2(make_float2(ta[ch * BW + 1], tb[ch * BW + 1]), w01, mul2(make_float2(ta[ch * BW], tb[ch * BW]), w00))))
-        const f2 r = GMPI_TAP(0), g = GMPI_TAP(1), b = GMPI_TAP(2);
-        f2 a;
-        if (AOFF == 0) {
-            a = GMPI_TAP(3);
-        } else {
-            const float* aa = sb + ja[P];
-            const float* ab = sb + jb[P];
-            a = fma2(make_float2(aa[AP + 1], ab[AP + 1]), w11,
-                     fma2(make_float2(aa[AP], ab[AP]), w10, fma2(make_float2(aa[1], ab[1]), w01, mul2(make_float2(aa[0], ab[0]), w00))));
-        }
-#undef GMPI_TAP
+        f2 wb[4], r, g, b, a;
+        bt.sample(sb, c, P, wb, r, g, b, a);
         f2 w = mul2(a, T[P]);                           // mpi.py:423
         if (kES) {
             if (fabsf(T[P].x) <= tau) w.x = 0.0f;
@@ -214,7 +242,9 @@ __device__ __forceinline__ float4 sample_plane_any(const RenderParams& p, const 
     return sample_plane_direct(plane, p.Ht, p.Wt, ix, iy);
 }
 
-__device__ __forceinline__ void consumer_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kConsThreads) : "memory"); }
+// named barrier 1 over the kThreads consumer threads of a kernel
+template <int kThreads>
+__device__ __forceinline__ void consumer_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kThreads) : "memory"); }
 
 // Tile order of the persistent grid (producer and consumers walk the same sequence): every full-height tile of every view
 // first, round-robin over the CTAs; then the partial bottom-row tiles (H % kTileH valid rows), dealt only to the CTAs that
@@ -285,9 +315,6 @@ __device__ __forceinline__ void consumer_idle_tile(uint64_t* s_full, uint64_t* s
     }
 }
 
-// Producer warp, shared by the forward (front-to-back) and backward (back-to-front) kernels: for every (tile, plane) of
-// this CTA, estimate the tile's texel footprint from its four corner rays, pick the narrowest box class, publish the stage
-// header and issue the TMA copies.
 // Ring geometry of a kernel: tile height, ring depth, the largest staged box and what a stage holds.
 struct FwdRing {          // the expanded forward's ring
     static constexpr int kTileRows = kTileH, kRingStages = kStages, kBoxMaxH = kMaxBH;
@@ -312,10 +339,7 @@ struct FwdRingWide {      // the factored forward's ring: 64- or 96-wide boxes (
     // of 128 (TMA destination alignment): any r for bw = 64 / 96.
     static constexpr int kColourCopyRows = kMaxBH / 2;
 };
-// factored MPI: the colour box [row][3][bw] starts the stage, the alpha box [row][bw] follows after 3/4 of the stage
 
-// kFact: factored MPI (compile time: a run-time test of p.alpha in this loop cost the forward 1 %, the producer's per-stage latency
-// being on the critical path of a shallow ring).
 // The expanded forward's copies of one stage: the footprint's n_chunks 4-row chunks as the binary digits of n_chunks.  Lane 0..3
 // owns the digit 8, 4, 2, 1: returns the copy's height in chunks (0: this lane issues nothing) and, in `before`, the chunks
 // covered by the taller copies, i.e. where this copy starts.  (Host-evaluable: gmpi_debug_copy_plan, tests/test_tile_walk.py.)
@@ -344,13 +368,18 @@ __device__ __forceinline__ uint32_t idle_consumer_warps(int py0, int H) {
     return live >= kConsWarps ? 0u : kAllConsumers & ~((1u << live) - 1u);
 }
 
+// Producer warp, shared by the forward (front-to-back) and backward (back-to-front) kernels: for every (tile, plane) of
+// this CTA, estimate the tile's texel footprint from its four corner rays, pick the narrowest box class, publish the stage
+// header and issue the TMA copies.
+// kFact: factored MPI (compile time: a run-time test of p.alpha in this loop cost the forward 1 %, the producer's per-stage latency
+// being on the critical path of a shallow ring).
 template <bool kAlignCorners, class Ring, bool kFact, bool kES = false>
 __device__ __forceinline__ void staged_producer(const RenderParams& p, const TmaMaps& maps, float* s_buf, StageMeta* s_meta,
                                             uint64_t* s_full, uint64_t* s_empty, const TileWalk* s_walk, int lane,
                                             int n_stages = Ring::kRingStages, uint32_t* s_stop = nullptr) {
     constexpr bool kReverse = Ring::kReverse;
     constexpr int kStride = Ring::kStride;      // floats per ring stage
-    constexpr int kTileH = Ring::kTileRows, kStages = Ring::kRingStages, kMaxBH = Ring::kBoxMaxH, kStageFloats = Ring::kPlaneFloats;
+    constexpr int kTileH = Ring::kTileRows, kMaxBH = Ring::kBoxMaxH, kStageFloats = Ring::kPlaneFloats;
     constexpr uint32_t kTBytes = kReverse ? (uint32_t)(kTileW * kTileH * 4) : 0u;
     const int Ht = p.Ht, Wt = p.Wt, N = p.N;
     const float fWt = (float)Wt, fHt = (float)Ht;
@@ -400,7 +429,7 @@ __device__ __forceinline__ void staged_producer(const RenderParams& p, const Tma
             else if (bx0 > Wt - 1 || bx0 + need_w - 1 < 0 || by0 > Ht - 1 || by0 + need_h - 1 < 0) mode = 1;
             // width class k (tensor-map slot, one-hot bit 16 + k of the header); wide rings: slot 1 = 64, slot 4 = kWideBW
             const int k = mode != 0 ? 0 : kWide ? (need_w <= 64 ? 1 : 4) : max(0, (need_w - kMinBW + kBWStep - 1) / kBWStep);
-            const int bw = (kWide && k == 4) ? kWideBW : kMinBW + k * kBWStep;
+            const int bw = class_width(k, kWide);
             const int n_ops = mode == 0 ? (need_h + kRowsPerOp - 1) / kRowsPerOp : 0;
             const int rows = n_ops * kRowsPerOp;
             if (Ring::kSleepPolls) mbar_wait_sleep(&s_empty[s], ph ^ 1);
@@ -438,9 +467,10 @@ __device__ __forceinline__ void staged_producer(const RenderParams& p, const Tma
             if (n_copy > 0) {
                 float* stage = s_buf + (size_t)s * kStride;
                 if constexpr (kFact) {
-                    // factored MPI: the colour box (shared image, or the last plane's own) as two or three copies that tile the
-                    // ring's box height, the alpha box as one copy of the full height.  Rows beyond the footprint are fetched and never
-                    // read: the colour image is shared by all planes and comes from L2, alpha is a quarter of the bytes.
+                    // factored MPI: the colour box [row][3][bw] (shared image, or the last plane's own) starts the stage, as two or
+                    // three copies that tile the ring's box height; the alpha box [row][bw] follows after 3/4 of the stage, as one copy
+                    // of the full height.  Rows beyond the footprint are fetched and never read: the colour image is shared by all
+                    // planes and comes from L2, alpha is a quarter of the bytes.
                     constexpr int kCR = Ring::kColourCopyRows;      // (a copy's destination must be 128-byte aligned, see the rings)
                     static_assert(kMaxBH % kCR == 0, "colour copies tile the box");
                     const CUtensorMap* cmap = (p.bg_rgb && i == N - 1) ? &maps.bg[k] : &maps.rgb[k];
@@ -484,12 +514,6 @@ __device__ __forceinline__ void quad_transpose(float (&a)[4], int lane) {
     }
 }
 
-// Epilogue of one consumer warp: rows py, py + 1 of the tile, 64 pixels each; out[q] = (R, G, B, depth) of pixel
-// (px0 + lane + 32 (q & 1), py + (q >> 1)).  Three destinations:
-//   * uint8 video frames (HWC colour + normalised depth, render_video.py:118-126) when video_rgb is set;
-//   * float4 stores after a quad transpose (lane k of a quad ends up with channel k of four consecutive x): 4 x STG.128 per
-//     thread instead of 16 x STG.32 -- and 4 per peer in the fused all-gather, or 4 in total through a multicast address;
-//   * the scalar store_pixel path for odd widths / unaligned outputs.
 // Epilogue of one consumer warp, one pixel set at a time: o = (R, G, B, depth) of pixel (pxb + lane, py) of view v; all 32 lanes
 // call this (the quad transpose shuffles).  Destinations:
 //   * float4 stores after a quad transpose (lane k of a quad ends up with channel k of four consecutive x): 4 x STG.128 per
@@ -581,9 +605,9 @@ __device__ __forceinline__ void fwd_staged_body(const RenderParams& p, const Tma
             float ev[3], zd[3];
             load_eye_z(p, v, ev, zd);
             if (v != v_table) {          // (view, plane) constants, once per view and CTA
-                consumer_bar_sync();     // everyone is done with the previous view's table
+                consumer_bar_sync<kConsThreads>();     // everyone is done with the previous view's table
                 for (int i = threadIdx.x; i < N; i += kConsThreads) s_pc[i] = make_plane_const(p.dhw + ((size_t)m * N + i) * 3, ev[2]);
-                consumer_bar_sync();
+                consumer_bar_sync<kConsThreads>();
                 v_table = v;
             }
             if (py0 + kPairs * warp >= p.H) {      // warp-uniform: no row of this warp is inside the image
@@ -601,13 +625,7 @@ __device__ __forceinline__ void fwd_staged_body(const RenderParams& p, const Tma
                 rc[q] = make_ray_const(qx, qy, qz, ev, zd);
                 rays_fast = rays_fast && rc[q].fast && fabsf(rc[q].rx2) <= 0x1p40f && fabsf(rc[q].ry2) <= 0x1p40f;
             }
-#pragma unroll
-            for (int P = 0; P < kPairs; ++P) {
-                rp.rx2[P] = make_float2(rc[2 * P].rx2, rc[2 * P + 1].rx2);
-                rp.ry2[P] = make_float2(rc[2 * P].ry2, rc[2 * P + 1].ry2);
-                rp.nrz[P] = make_float2(-rc[2 * P].rz, -rc[2 * P + 1].rz);
-                rp.yrz[P] = make_float2(rc[2 * P].yrz, rc[2 * P + 1].yrz);
-            }
+            pack_ray_pairs(rc, rp);
             const f2 ex2 = splat(rc[0].ex2), ey2 = splat(rc[0].ey2), hsx2 = splat(hsx), hsy2 = splat(hsy);
             // warp-uniform: every ray of this warp is in the range where the reciprocal+FMA division is exact and no
             // coordinate can be NaN, so the per-plane body needs no per-pixel range checks

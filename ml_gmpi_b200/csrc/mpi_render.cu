@@ -285,7 +285,8 @@ __global__ void mpi_debug_coords_kernel(const int32_t* view2mpi, const float* dh
     }
 }
 
-// Test hook for the pixel-pair coordinate path of the staged kernel: pixels 2k, 2k+1 of a row form a pair.
+// Test hook for the pixel-pair coordinate path of the staged kernel: pixels 2k, 2k+1 of a row form a pair (both of the staged
+// kernel's pairs per thread hold it).
 template <bool kAlignCorners>
 __global__ void mpi_debug_coords_packed_kernel(const int32_t* view2mpi, const float* dhw, const float* ray_dir,
                                                const float* eye, float* out, int V, int N, int Ht, int Wt, int H, int W) {
@@ -297,16 +298,13 @@ __global__ void mpi_debug_coords_packed_kernel(const int32_t* view2mpi, const fl
     const float* e = eye + 3 * v;
     const float ev[3] = {e[0], e[1], e[2]};
     const float zd[3] = {0.f, 0.f, 1.f};
-    RayConst rc[2];
-    for (int k = 0; k < 2; ++k) {
-        const float* rd = ray_dir + (size_t)v * 3 * img + pair * 2 + k;
-        rc[k] = make_ray_const(rd[0], rd[img], rd[2 * img], ev, zd);
+    RayConst rc[kPix];
+    for (int q = 0; q < kPix; ++q) {
+        const float* rd = ray_dir + (size_t)v * 3 * img + pair * 2 + (q & 1);
+        rc[q] = make_ray_const(rd[0], rd[img], rd[2 * img], ev, zd);
     }
     RayPairs rp;
-    for (int P = 0; P < 2; ++P) {
-        rp.rx2[P] = make_float2(rc[0].rx2, rc[1].rx2); rp.ry2[P] = make_float2(rc[0].ry2, rc[1].ry2);
-        rp.nrz[P] = make_float2(-rc[0].rz, -rc[1].rz); rp.yrz[P] = make_float2(rc[0].yrz, rc[1].yrz);
-    }
+    pack_ray_pairs(rc, rp);
     const float hsx = 0.5f * (float)(Wt - 1), hsy = 0.5f * (float)(Ht - 1);
     for (int i = 0; i < N; ++i) {
         const PlaneConst pc = make_plane_const(dhw + ((size_t)m * N + i) * 3, ev[2]);
@@ -401,7 +399,7 @@ static bool mpi_aligned(const RenderParams& p) {
 // wide: the factored forward's ring (FwdRingWide) -- slot 4 holds the kWideBW-wide boxes, slot 1 the 64-wide ones, the rest unused.
 static int encode_mpi_maps(TmaMaps& maps, const RenderParams& p, int box_h, int colour_rows, bool wide = false) {
     for (int k = 0; k < kNumMaps; ++k) {
-        const int bw = (wide && k == kNumMaps - 1) ? kWideBW : kMinBW + k * kBWStep;
+        const int bw = class_width(k, wide);
         if (p.alpha) {
             if (encode_color_map(&maps.rgb[k], p.rgb, (uint64_t)p.M, p.Ht, p.Wt, bw, colour_rows) != 0) return -1;
             if (p.bg_rgb && encode_color_map(&maps.bg[k], p.bg_rgb, (uint64_t)p.M, p.Ht, p.Wt, bw, colour_rows) != 0) return -1;
@@ -450,9 +448,24 @@ static int reset_early_stop_stats(unsigned long long total, cudaStream_t st) {
     return GMPI_OK;
 }
 
-// kernel: an instantiation of mpi_fwd_staged_kernel or mpi_fwd_early_stop_kernel; fac: its kFactored
-template <class Kernel>
-static cudaError_t launch_fwd_staged(Kernel kernel, bool fac, const RenderParams& p, const TmaMaps& maps, int grid, int tiles_x,
+// The staged forward's instantiations: mpi_fwd_staged_kernel [align_corners][emit][factored] and the early-stop kernel
+// [align_corners][factored] (never with emit: check_params refuses it).
+using StagedFwdKernel = void (*)(const RenderParams, const TmaMaps, const int, const int, const int);
+static constexpr StagedFwdKernel kFwdStagedKernels[2][2][2] = {
+    {{mpi_fwd_staged_kernel<false, false, false>, mpi_fwd_staged_kernel<false, false, true>},
+     {mpi_fwd_staged_kernel<false, true, false>, mpi_fwd_staged_kernel<false, true, true>}},
+    {{mpi_fwd_staged_kernel<true, false, false>, mpi_fwd_staged_kernel<true, false, true>},
+     {mpi_fwd_staged_kernel<true, true, false>, mpi_fwd_staged_kernel<true, true, true>}}};
+static constexpr StagedFwdKernel kFwdEarlyStopKernels[2][2] = {
+    {mpi_fwd_early_stop_kernel<false, false>, mpi_fwd_early_stop_kernel<false, true>},
+    {mpi_fwd_early_stop_kernel<true, false>, mpi_fwd_early_stop_kernel<true, true>}};
+// the direct forward [early_stop][align_corners]
+static constexpr void (*kFwdDirectKernels[2][2])(const RenderParams) = {
+    {mpi_fwd_direct_kernel<false>, mpi_fwd_direct_kernel<true>},
+    {mpi_fwd_direct_early_stop_kernel<false>, mpi_fwd_direct_early_stop_kernel<true>}};
+
+// fac: the kernel's kFactored
+static cudaError_t launch_fwd_staged(StagedFwdKernel kernel, bool fac, const RenderParams& p, const TmaMaps& maps, int grid, int tiles_x,
                                      int tiles_y, int stages, cudaStream_t st) {
     const size_t smem = fac ? kStagedSmemWide : (size_t)stages * kStageFloats * 4 + (size_t)kMaxPlanesStaged * 32;
     cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -495,24 +508,9 @@ static int launch_fwd(RenderParams p, cudaStream_t st) {
             const int tiles_x = (p.W + kTileW - 1) / kTileW, tiles_y = (p.H + kTileH - 1) / kTileH;
             const long n_tiles = (long)tiles_x * tiles_y * p.V;
             const int grid = (int)(n_tiles < sms ? n_tiles : sms);
-            cudaError_t e;
-            if (es) {        // (never with emit: check_params)
-                if ((rc = reset_early_stop_stats((unsigned long long)n_tiles * p.N, st)) != 0) return rc;
-                if (fac) e = ac ? launch_fwd_staged(mpi_fwd_early_stop_kernel<true, true>, fac, p, maps, grid, tiles_x, tiles_y, stages, st)
-                                : launch_fwd_staged(mpi_fwd_early_stop_kernel<false, true>, fac, p, maps, grid, tiles_x, tiles_y, stages, st);
-                else e = ac ? launch_fwd_staged(mpi_fwd_early_stop_kernel<true, false>, fac, p, maps, grid, tiles_x, tiles_y, stages, st)
-                            : launch_fwd_staged(mpi_fwd_early_stop_kernel<false, false>, fac, p, maps, grid, tiles_x, tiles_y, stages, st);
-            } else if (fac) {
-                if (ac && emit) e = launch_fwd_staged(mpi_fwd_staged_kernel<true, true, true>, fac, p, maps, grid, tiles_x, tiles_y, stages, st);
-                else if (ac) e = launch_fwd_staged(mpi_fwd_staged_kernel<true, false, true>, fac, p, maps, grid, tiles_x, tiles_y, stages, st);
-                else if (emit) e = launch_fwd_staged(mpi_fwd_staged_kernel<false, true, true>, fac, p, maps, grid, tiles_x, tiles_y, stages, st);
-                else e = launch_fwd_staged(mpi_fwd_staged_kernel<false, false, true>, fac, p, maps, grid, tiles_x, tiles_y, stages, st);
-            } else {
-                if (ac && emit) e = launch_fwd_staged(mpi_fwd_staged_kernel<true, true, false>, fac, p, maps, grid, tiles_x, tiles_y, stages, st);
-                else if (ac) e = launch_fwd_staged(mpi_fwd_staged_kernel<true, false, false>, fac, p, maps, grid, tiles_x, tiles_y, stages, st);
-                else if (emit) e = launch_fwd_staged(mpi_fwd_staged_kernel<false, true, false>, fac, p, maps, grid, tiles_x, tiles_y, stages, st);
-                else e = launch_fwd_staged(mpi_fwd_staged_kernel<false, false, false>, fac, p, maps, grid, tiles_x, tiles_y, stages, st);
-            }
+            if (es && (rc = reset_early_stop_stats((unsigned long long)n_tiles * p.N, st)) != 0) return rc;
+            const StagedFwdKernel kernel = es ? kFwdEarlyStopKernels[ac][fac] : kFwdStagedKernels[ac][emit][fac];
+            cudaError_t e = launch_fwd_staged(kernel, fac, p, maps, grid, tiles_x, tiles_y, stages, st);
             GMPI_CUDA_OK(e);
             GMPI_CUDA_OK(cudaGetLastError());
             return GMPI_OK;
@@ -526,8 +524,7 @@ static int launch_fwd(RenderParams p, cudaStream_t st) {
     if (grid.y > 65535) return fail(GMPI_ERR_UNSUPPORTED, "image height %d too large", p.H);
     if (p.V > 65535) return fail(GMPI_ERR_UNSUPPORTED, "V=%d views exceed one launch of the direct kernel (65535); split the batch", p.V);
     if (es && (rc = reset_early_stop_stats(0, st)) != 0) return rc;    // the direct kernel loads per pixel: no stages to skip
-    void (*kernel)(const RenderParams) = es ? (ac ? mpi_fwd_direct_early_stop_kernel<true> : mpi_fwd_direct_early_stop_kernel<false>)
-                                            : (ac ? mpi_fwd_direct_kernel<true> : mpi_fwd_direct_kernel<false>);
+    void (*kernel)(const RenderParams) = kFwdDirectKernels[es][ac];
     if (smem > 48 * 1024) GMPI_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     kernel<<<grid, block, smem, st>>>(p);
     GMPI_CUDA_OK(cudaGetLastError());
@@ -567,20 +564,18 @@ static int launch_bwd_direct(RenderParams p, cudaStream_t st, bool zero) {
     dim3 grid((p.W + tile_w - 1) / tile_w, (p.H + tile_h - 1) / tile_h, p.V);
     if (grid.y > 65535) return fail(GMPI_ERR_UNSUPPORTED, "image height %d too large", p.H);
     if (p.V > 65535) return fail(GMPI_ERR_UNSUPPORTED, "V=%d views exceed one launch of the direct kernel (65535); split the batch", p.V);
-    if (p.options & GMPI_ALIGN_CORNERS) {
-        GMPI_CUDA_OK(cudaFuncSetAttribute(mpi_bwd_direct_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        mpi_bwd_direct_kernel<true><<<grid, block, smem, st>>>(p, tile_w, tile_h);
-    } else {
-        GMPI_CUDA_OK(cudaFuncSetAttribute(mpi_bwd_direct_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        mpi_bwd_direct_kernel<false><<<grid, block, smem, st>>>(p, tile_w, tile_h);
-    }
+    void (*kernel)(const RenderParams, const int, const int) =
+        (p.options & GMPI_ALIGN_CORNERS) ? mpi_bwd_direct_kernel<true> : mpi_bwd_direct_kernel<false>;
+    GMPI_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    kernel<<<grid, block, smem, st>>>(p, tile_w, tile_h);
     GMPI_CUDA_OK(cudaGetLastError());
     return GMPI_OK;
 }
 
-template <bool AC, bool FAC>
-static cudaError_t launch_bwd_box(const RenderParams& p, const TmaMaps& maps, int grid, int tiles_x, int tiles_y, cudaStream_t st) {
-    auto kernel = mpi_bwd_box_kernel<AC, FAC>;
+using BwdBoxKernel = void (*)(const RenderParams, const TmaMaps, const int, const int);
+
+static cudaError_t launch_bwd_box(BwdBoxKernel kernel, const RenderParams& p, const TmaMaps& maps, int grid, int tiles_x, int tiles_y,
+                                  cudaStream_t st) {
     cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBwdSmem);
     if (e != cudaSuccess) return e;
     kernel<<<grid, kBwdThreads, kBwdSmem, st>>>(p, maps, tiles_x, tiles_y);
@@ -610,9 +605,10 @@ static int launch_bwd(RenderParams p, cudaStream_t st) {
     const int grid = (int)(n_tiles < sms ? n_tiles : sms);
     const bool ac = (p.options & GMPI_ALIGN_CORNERS) != 0;
     if ((p.options & GMPI_ZERO_GRAD) && (rc = zero_grads(p, st)) != 0) return rc;
-    cudaError_t e;
-    if (fac) e = ac ? launch_bwd_box<true, true>(p, maps, grid, tiles_x, tiles_y, st) : launch_bwd_box<false, true>(p, maps, grid, tiles_x, tiles_y, st);
-    else e = ac ? launch_bwd_box<true, false>(p, maps, grid, tiles_x, tiles_y, st) : launch_bwd_box<false, false>(p, maps, grid, tiles_x, tiles_y, st);
+    // (not a table: instantiating the four kernels in table order changes the machine code ptxas gives the expanded ones)
+    const BwdBoxKernel kernel = fac ? (ac ? mpi_bwd_box_kernel<true, true> : mpi_bwd_box_kernel<false, true>)
+                                    : (ac ? mpi_bwd_box_kernel<true, false> : mpi_bwd_box_kernel<false, false>);
+    cudaError_t e = launch_bwd_box(kernel, p, maps, grid, tiles_x, tiles_y, st);
     GMPI_CUDA_OK(e);
     GMPI_CUDA_OK(cudaGetLastError());
     return GMPI_OK;
@@ -830,10 +826,8 @@ int gmpi_debug_plane_coords(const int32_t* view2mpi, const float* dhw, const flo
     cudaStream_t st = (cudaStream_t)stream;
     const size_t img = (size_t)H * W;
     dim3 grid((unsigned)((img + 255) / 256), V);
-    if (options & GMPI_ALIGN_CORNERS)
-        mpi_debug_coords_kernel<true><<<grid, 256, 0, st>>>(view2mpi, dhw, ray_dir, eye, out, V, N, Ht, Wt, H, W);
-    else
-        mpi_debug_coords_kernel<false><<<grid, 256, 0, st>>>(view2mpi, dhw, ray_dir, eye, out, V, N, Ht, Wt, H, W);
+    const auto kernel = (options & GMPI_ALIGN_CORNERS) ? mpi_debug_coords_kernel<true> : mpi_debug_coords_kernel<false>;
+    kernel<<<grid, 256, 0, st>>>(view2mpi, dhw, ray_dir, eye, out, V, N, Ht, Wt, H, W);
     GMPI_CUDA_OK(cudaGetLastError());
     return GMPI_OK;
 }
@@ -845,10 +839,8 @@ int gmpi_debug_plane_coords_packed(const int32_t* view2mpi, const float* dhw, co
     cudaStream_t st = (cudaStream_t)stream;
     const size_t pairs = (size_t)H * W / 2;
     dim3 grid((unsigned)((pairs + 255) / 256), V);
-    if (options & GMPI_ALIGN_CORNERS)
-        mpi_debug_coords_packed_kernel<true><<<grid, 256, 0, st>>>(view2mpi, dhw, ray_dir, eye, out, V, N, Ht, Wt, H, W);
-    else
-        mpi_debug_coords_packed_kernel<false><<<grid, 256, 0, st>>>(view2mpi, dhw, ray_dir, eye, out, V, N, Ht, Wt, H, W);
+    const auto kernel = (options & GMPI_ALIGN_CORNERS) ? mpi_debug_coords_packed_kernel<true> : mpi_debug_coords_packed_kernel<false>;
+    kernel<<<grid, 256, 0, st>>>(view2mpi, dhw, ray_dir, eye, out, V, N, Ht, Wt, H, W);
     GMPI_CUDA_OK(cudaGetLastError());
     return GMPI_OK;
 }

@@ -107,6 +107,7 @@ class FrameGather:
         """early_stop: early ray termination threshold in [0, 1), as in render_frames (None: off)."""
         import ctypes
         from . import _lib
+        from .mpi import _options
         lib = _lib.load()
         M, N, _, Ht, Wt = rgba.shape
         V = ray_dir.shape[0]
@@ -114,8 +115,7 @@ class FrameGather:
         for name, t in (("rgba", rgba), ("dhw", dhw), ("ray_dir", ray_dir), ("eye", eye), ("z_dir", z_dir)):   # raw pointers below
             assert t.is_cuda and t.dtype == torch.float32 and t.is_contiguous(), f"{name} must be a contiguous fp32 CUDA tensor"
         assert view2mpi.dtype == torch.int32 and view2mpi.is_contiguous() and flags.dtype == torch.int32
-        options = (_lib.OPT_ALIGN_CORNERS if align_corners else 0) | (_lib.OPT_CHECK_LAST_PLANE if check_last_plane else 0) \
-            | (_lib.OPT_COLOR_MINUS1_1 if color_minus1_1 else 0) | (_lib.OPT_EARLY_STOP if early_stop is not None else 0)
+        options = _options(align_corners, check_last_plane, color_minus1_1, early_stop=early_stop)
         with torch.cuda.device(rgba.device):
             d = _lib.make_desc(options=options, M=M, V=V, N=N, Ht=Ht, Wt=Wt, H=self.H, W=self.W, rgba=rgba, view2mpi=view2mpi, dhw=dhw,
                                ray_dir=ray_dir, eye=eye, z_dir=z_dir, peer_frames=self._peer_ptrs[self._next],

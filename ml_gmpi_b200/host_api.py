@@ -5,6 +5,7 @@ import numpy as np
 import torch
 
 from . import _lib
+from .mpi import _options
 
 
 def render_host(rgba: torch.Tensor, dhw: torch.Tensor, view2mpi: torch.Tensor, ray_dir: torch.Tensor, eye: torch.Tensor,
@@ -23,8 +24,7 @@ def render_host(rgba: torch.Tensor, dhw: torch.Tensor, view2mpi: torch.Tensor, r
     if out_depth is None:
         out_depth = torch.empty((V, 1, H, W), dtype=torch.float32).pin_memory()
     flags = np.zeros(1, np.uint32)
-    options = (_lib.OPT_ALIGN_CORNERS if align_corners else 0) | (_lib.OPT_CHECK_LAST_PLANE if check_last_plane else 0) \
-        | (_lib.OPT_COLOR_MINUS1_1 if color_minus1_1 else 0)
+    options = _options(align_corners, check_last_plane, color_minus1_1)
     _lib.check(lib.gmpi_mpi_render_fwd_host(rgba.data_ptr(), view2mpi.data_ptr(), dhw.data_ptr(), ray_dir.data_ptr(),
                                             eye.data_ptr(), z_dir.data_ptr(), out_color.data_ptr(), out_depth.data_ptr(),
                                             flags.ctypes.data, M, V, N, Ht, Wt, H, W, options, int(device)))
