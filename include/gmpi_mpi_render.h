@@ -61,6 +61,7 @@ extern "C" {
 #define GMPI_U8_ROUND_HALF_UP 16u       /* uint8 epilogue: clamp, x*255+0.5 (torchvision save_image, fid_evaluation.py:125-130)
                                           instead of numpy's truncating astype (render_video.py:119-126) */
 #define GMPI_EARLY_STOP 32u            /* forward only: early ray termination at gmpi_render_desc.early_stop (see there) */
+#define GMPI_MPI_F16 64u               /* forward only: the descriptor's MPI tensors are IEEE binary16 (see gmpi_render_desc) */
 
 int gmpi_abi_version(void);
 const char* gmpi_last_error(void);
@@ -226,11 +227,27 @@ typedef struct gmpi_render_desc {
  */
 #define GMPI_RENDER_DESC_V2_BYTES offsetof(gmpi_render_desc, early_stop)
 
+/*
+ * GMPI_MPI_F16 (off by default): every MPI tensor of the call -- rgba, or rgb + alpha (+ bg_rgb) -- is IEEE binary16, with the
+ * layouts above; the descriptor's float pointers are read as pointers to halves.  Every other input and every output keeps its type.
+ * An fp16 value converts to fp32 exactly and the kernels convert each texel tap before the unchanged fp32 arithmetic, so the output
+ * is bitwise equal to the same call on the fp32 upcast of the MPI (on the same kernel variant and ring depth), at half the MPI bytes
+ * read from HBM -- and, through gmpi_mpi_render_host_ex, uploaded.  The staged kernels need Wt % 8 == 0 and 16-byte aligned MPI
+ * bases (gmpi_mpi_render_fwd_plan_ex); other shapes take the direct kernels.  Accepted by gmpi_mpi_render_fwd_ex and
+ * gmpi_mpi_render_host_ex only: a descriptor that also sets transmittance, gmpi_mpi_render_bwd_ex and every classic entry point
+ * return GMPI_ERR_UNSUPPORTED.
+ */
+
 /* cudaMemsetAsync(ptr, 0, bytes) on `stream`, for callers that accumulate into their own buffers (no GMPI_ZERO_GRAD).  Note that a
  * memset cannot overlap the staged kernels, on whatever stream (they own every SM: measured, tools/zero_overlap_probe.py). */
 int gmpi_mpi_zero_async(void* ptr, size_t bytes, void* stream);
 
 int gmpi_mpi_render_fwd_ex(const gmpi_render_desc* desc);
+/* gmpi_mpi_render_fwd_plan for the forward a descriptor describes (sizes, options, MPI pointers; the other fields are not read).  It sees
+ * GMPI_MPI_F16: an fp16 MPI needs Wt % 8 == 0 for the staged kernels (GMPI_WHY_TEX_WIDTH otherwise).  Every non-NULL MPI pointer
+ * (rgba, rgb, alpha, bg_rgb) must be 16-byte aligned (GMPI_WHY_ALIGNMENT); NULL ones are not checked.  Returns the plan, or a
+ * negative GMPI_ERR_* code for a bad descriptor. */
+int gmpi_mpi_render_fwd_plan_ex(const gmpi_render_desc* desc, uint32_t* why);
 int gmpi_mpi_render_bwd_ex(const gmpi_render_desc* desc);
 /* Host-buffer form (end-to-end entry point, see gmpi_mpi_render_fwd_host): all pointers of *desc are HOST memory, `stream` is
  * ignored, *flags receives the flag word.  Forward only; supports the factored MPI, cam and the video outputs. */
@@ -265,6 +282,8 @@ int gmpi_mpi_apply_shading_bwd(const float* rgba, const float* shade, const floa
  */
 int gmpi_mpi_check_range(const float* rgba, int M, int N, int Ht, int Wt, uint32_t* flags,
                          void* stream);
+/* The same check of an fp16 rgba [M,N,4,Ht,Wt]: sets the flags gmpi_mpi_check_range sets on its fp32 upcast (NaN included). */
+int gmpi_mpi_check_range_f16(const void* rgba, int M, int N, int Ht, int Wt, uint32_t* flags, void* stream);
 
 /*
  * Host-buffer forward (end-to-end entry point): all pointers are HOST memory (pinned memory

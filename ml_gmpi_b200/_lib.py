@@ -29,10 +29,12 @@ EXPORTS = [
     "gmpi_mpi_render_fwd_plan", "gmpi_mpi_render_fwd_ex", "gmpi_mpi_render_bwd_ex", "gmpi_mpi_render_host_ex",
     "gmpi_debug_tile_walk_ex", "gmpi_debug_cam_rays", "gmpi_debug_set_fwd_stages", "gmpi_debug_fwd_ring_stages",
     "gmpi_debug_fwd_early_stop_stats", "gmpi_mpi_zero_async", "gmpi_mpi_alpha_depth_fwd", "gmpi_mpi_alpha_depth_bwd", "gmpi_mpi_apply_shading_fwd", "gmpi_mpi_apply_shading_bwd",
+    "gmpi_mpi_render_fwd_plan_ex", "gmpi_mpi_check_range_f16",
 ]
 
 OPT_U8_ROUND_HALF_UP = 16
 OPT_EARLY_STOP = 32
+OPT_MPI_F16 = 64
 
 
 class RenderDesc(ctypes.Structure):
@@ -102,6 +104,8 @@ def load():
     lib.gmpi_mpi_render_bwd.argtypes = [vp] * 9 + [i] * 7 + [u32, vp]
     lib.gmpi_mpi_check_range.restype = i
     lib.gmpi_mpi_check_range.argtypes = [vp, i, i, i, i, vp, vp]
+    lib.gmpi_mpi_check_range_f16.restype = i
+    lib.gmpi_mpi_check_range_f16.argtypes = [vp, i, i, i, i, vp, vp]
     lib.gmpi_mpi_render_fwd_host.restype = i
     lib.gmpi_mpi_render_fwd_host.argtypes = [vp] * 9 + [i] * 7 + [u32, i]
     lib.gmpi_mpi_release_host_cache.restype = i
@@ -144,6 +148,8 @@ def load():
     lib.gmpi_mpi_apply_shading_bwd.argtypes = [vp, vp, vp, vp, vp, i, i, i, i, vp]
     lib.gmpi_mpi_render_host_ex.restype = i
     lib.gmpi_mpi_render_host_ex.argtypes = [ctypes.POINTER(RenderDesc), i]
+    lib.gmpi_mpi_render_fwd_plan_ex.restype = i
+    lib.gmpi_mpi_render_fwd_plan_ex.argtypes = [ctypes.POINTER(RenderDesc), vp]
     if lib.gmpi_abi_version() != ABI_VERSION:
         raise GmpiLibraryError(f"ABI mismatch: library {lib.gmpi_abi_version()} != binding {ABI_VERSION}; rebuild")
     _lib = lib

@@ -4,6 +4,7 @@
 // (gmpi/core/mpi.py:74-90 + ATen grid_sampler_unnormalize) because the texel coordinate is
 // amplified by (texture size x texel gradient): see DESIGN.md "Coordinates".
 #pragma once
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <type_traits>
@@ -55,16 +56,24 @@ struct RenderParams {
 };
 static_assert(sizeof(RenderParams) == 248, "RenderParams layout (kernel parameter offsets)");
 
-// The four channel slabs (Ht*Wt floats each) of one (MPI, plane): expanded rgba or the generator's factored form.
-struct PlaneChans { const float* c[4]; };
-__device__ __forceinline__ PlaneChans plane_chans(const RenderParams& p, int m, int i, size_t tex) {
-    PlaneChans pc;
+// MPI element types: fp32, or IEEE binary16 under GMPI_MPI_F16 (the MPI pointers of RenderParams then point at halves).  Every
+// tap is converted to fp32 (exactly) before the fp32 arithmetic, so an fp16 MPI renders bit for bit like its fp32 upcast.
+__device__ __forceinline__ float to_f32(float x) { return x; }
+__device__ __forceinline__ float to_f32(__half x) { return __half2float(x); }
+
+// The four channel slabs (Ht*Wt elements each) of one (MPI, plane): expanded rgba or the generator's factored form.
+template <class E = float>
+struct PlaneChansT { const E* c[4]; };
+using PlaneChans = PlaneChansT<float>;
+template <class E = float>
+__device__ __forceinline__ PlaneChansT<E> plane_chans(const RenderParams& p, int m, int i, size_t tex) {
+    PlaneChansT<E> pc;
     if (p.alpha) {
-        const float* rgb = ((p.bg_rgb && i == p.N - 1) ? p.bg_rgb : p.rgb) + (size_t)m * 3 * tex;
+        const E* rgb = reinterpret_cast<const E*>((p.bg_rgb && i == p.N - 1) ? p.bg_rgb : p.rgb) + (size_t)m * 3 * tex;
         pc.c[0] = rgb; pc.c[1] = rgb + tex; pc.c[2] = rgb + 2 * tex;
-        pc.c[3] = p.alpha + ((size_t)m * p.N + i) * tex;
+        pc.c[3] = reinterpret_cast<const E*>(p.alpha) + ((size_t)m * p.N + i) * tex;
     } else {
-        const float* b = p.rgba + ((size_t)m * p.N + i) * 4 * tex;
+        const E* b = reinterpret_cast<const E*>(p.rgba) + ((size_t)m * p.N + i) * 4 * tex;
         pc.c[0] = b; pc.c[1] = b + tex; pc.c[2] = b + 2 * tex; pc.c[3] = b + 3 * tex;
     }
     return pc;
@@ -298,8 +307,9 @@ __device__ __forceinline__ bool coord_hits(float ix, float iy, float fWt, float 
     return ix > -1.0f && ix < fWt && iy > -1.0f && iy < fHt;   // false for NaN
 }
 
-__device__ __forceinline__ float tap4(const float* __restrict__ ch, const Taps& t) {
-    const float a = __ldg(ch + t.o00), b = __ldg(ch + t.o01), c = __ldg(ch + t.o10), d = __ldg(ch + t.o11);
+template <class E>
+__device__ __forceinline__ float tap4(const E* __restrict__ ch, const Taps& t) {
+    const float a = to_f32(__ldg(ch + t.o00)), b = to_f32(__ldg(ch + t.o01)), c = to_f32(__ldg(ch + t.o10)), d = to_f32(__ldg(ch + t.o11));
     return fmaf(d, t.w11, fmaf(c, t.w10, fmaf(b, t.w01, a * t.w00)));
 }
 

@@ -43,6 +43,13 @@ static_assert(kStagedSmemWide + 1024 <= 227 * 1024, "wide factored ring must fit
 
 // Box width of class k (tensor-map slot k).  In the factored forward's ring (wide) slot 4 holds kWideBW and slot 1 the 64-wide boxes.
 __host__ __device__ constexpr int class_width(int k, bool wide = false) { return wide && k == kNumMaps - 1 ? kWideBW : kMinBW + k * kBWStep; }
+// Width of the box staged for class width bw, element type E.  fp16 boxes (GMPI_MPI_F16) start at a multiple of 8 texels (16 bytes),
+// up to 4 texels west of the fp32 origin (a multiple of 4), so they are wider than their class: bw + 8 in the expanded ring; 96 and
+// 128 for the factored ring's 64 and 96 (a colour copy of kColourCopyRows rows lands at a multiple of 132 bw bytes, which must be
+// 128-byte aligned: bw % 32 == 0).  Class, mode and the in-box vote stay those of the fp32 box, so an fp16 MPI takes the fast and
+// the generic body exactly where its fp32 upcast does; only the addresses use the wider box.
+template <class E>
+__host__ __device__ constexpr int staged_width(int bw, bool wide) { return sizeof(E) == 2 ? bw + (wide ? 32 : 8) : bw; }
 
 struct TmaMaps {
     CUtensorMap m[kNumMaps];      // expanded rgba [M*N][4][Ht][Wt] as (x, channel, y, plane), box {bw, 4, 4 rows, 1}
@@ -141,12 +148,13 @@ __device__ __forceinline__ void coords_pairs(const PlaneConst& pc, const RayPair
 // The bilinear footprints of a thread's two pixel pairs in a staged box of compile-time width BW, shared by the forward's and
 // the backward's fast bodies.  AOFF == 0: expanded stage [row][4 channels][BW].  AOFF > 0 (factored MPI): colour box [row][3][BW]
 // at the stage base and the alpha box [row][BW] AOFF floats further on.  The backward's gradient box has the stage's layout, so
-// the same indices address it.
-template <int BW, int AOFF>
+// the same indices address it.  E: the element type of the box (fp16 boxes under GMPI_MPI_F16: each tap is converted to fp32).
+template <int BW, int AOFF, class E = float>
 struct BoxTaps {
-    static constexpr int RP = AOFF ? 3 * BW : 4 * BW;       // colour row pitch
-    static constexpr int AP = AOFF ? BW : 4 * BW;           // alpha row pitch
-    static constexpr int A0 = AOFF ? AOFF : 3 * BW;         // alpha offset from the colour index (factored: separate box)
+    static constexpr int SW = staged_width<E>(BW, AOFF != 0);   // staged box width (BW: the box the vote tests)
+    static constexpr int RP = AOFF ? 3 * SW : 4 * SW;       // colour row pitch
+    static constexpr int AP = AOFF ? SW : 4 * SW;           // alpha row pitch
+    static constexpr int A0 = AOFF ? AOFF : 3 * SW;         // alpha offset from the colour index (factored: separate box)
     f2 fx0[kPairs], fy0[kPairs];                            // floor of the coordinates, as floats
     int ia[kPairs], ib[kPairs];                             // colour index of the north-west taps of pixels .x and .y of pair P
     int ja[kPairs], jb[kPairs];                             // factored: alpha index (separate box)
@@ -173,22 +181,23 @@ struct BoxTaps {
     }
     // one channel of pair P: the four taps of a box with row pitch PITCH at ta / tb, weighted
     template <int PITCH>
-    static __device__ __forceinline__ f2 tap2(const float* ta, const float* tb, const f2 (&w)[4]) {
-        return fma2(make_float2(ta[PITCH + 1], tb[PITCH + 1]), w[3],
-                    fma2(make_float2(ta[PITCH], tb[PITCH]), w[2], fma2(make_float2(ta[1], tb[1]), w[1], mul2(make_float2(ta[0], tb[0]), w[0]))));
+    static __device__ __forceinline__ f2 tap2(const E* ta, const E* tb, const f2 (&w)[4]) {
+        return fma2(make_float2(to_f32(ta[PITCH + 1]), to_f32(tb[PITCH + 1])), w[3],
+                    fma2(make_float2(to_f32(ta[PITCH]), to_f32(tb[PITCH])), w[2],
+                         fma2(make_float2(to_f32(ta[1]), to_f32(tb[1])), w[1], mul2(make_float2(to_f32(ta[0]), to_f32(tb[0])), w[0]))));
     }
     // bilinear weights w = (w00, w01, w10, w11) and the four channels of pair P from the staged box sb
-    __device__ __forceinline__ void sample(const float* __restrict__ sb, const CoordPairs& c, int P, f2 (&w)[4], f2& r, f2& g, f2& b,
+    __device__ __forceinline__ void sample(const E* __restrict__ sb, const CoordPairs& c, int P, f2 (&w)[4], f2& r, f2& g, f2& b,
                                            f2& a) const {
         const f2 m1 = splat(-1.0f), one = splat(1.0f);
         const f2 wx1 = fma2(fx0[P], m1, c.ix[P]), wy1 = fma2(fy0[P], m1, c.iy[P]);   // fractional parts (exact)
         const f2 wy0 = fma2(wy1, m1, one);
         w[3] = mul2(wx1, wy1); w[2] = fma2(w[3], m1, wy1); w[1] = fma2(w[3], m1, wx1); w[0] = fma2(w[1], m1, wy0);
-        const float* ta = sb + ia[P];
-        const float* tb = sb + ib[P];
+        const E* ta = sb + ia[P];
+        const E* tb = sb + ib[P];
         r = tap2<RP>(ta, tb, w);
-        g = tap2<RP>(ta + BW, tb + BW, w);
-        b = tap2<RP>(ta + 2 * BW, tb + 2 * BW, w);
+        g = tap2<RP>(ta + SW, tb + SW, w);
+        b = tap2<RP>(ta + 2 * SW, tb + 2 * SW, w);
         a = AOFF ? tap2<AP>(sb + ja[P], sb + jb[P], w) : tap2<AP>(ta + A0, tb + A0, w);
     }
 };
@@ -196,12 +205,12 @@ struct BoxTaps {
 // Sample + composite the four pixels from a staged box of compile-time width BW.  Returns false (and changes nothing)
 // if any of the four footprints is not inside the box.  AOFF as in BoxTaps.
 // kES (early stop): a pixel whose |T| <= tau adds nothing; its weight is selected to 0, so its T stays where it stopped.
-template <int BW, int AOFF = 0, bool kES = false>
-__device__ __forceinline__ bool sample_pairs(const float* __restrict__ sb, int cx, int cy, int rows2, const CoordPairs& c,
+template <int BW, int AOFF = 0, bool kES = false, class E = float>
+__device__ __forceinline__ bool sample_pairs(const E* __restrict__ sb, int cx, int cy, int rows2, const CoordPairs& c,
                                              f2 (&T)[kPairs], f2 (&cr)[kPairs], f2 (&cg)[kPairs], f2 (&cb)[kPairs], f2 (&cws)[kPairs],
                                              float tau = 0.0f) {
     const f2 m1 = splat(-1.0f);
-    BoxTaps<BW, AOFF> bt;
+    BoxTaps<BW, AOFF, E> bt;
     if (!bt.locate(cx, cy, rows2, c)) return false;
 #pragma unroll
     for (int P = 0; P < kPairs; ++P) {
@@ -235,10 +244,20 @@ __device__ __noinline__ float4 sample_chans_direct(const PlaneChans pl, int Ht, 
     const Taps tp = make_taps(ix, iy, Ht, Wt);
     return make_float4(tap4(pl.c[0], tp), tap4(pl.c[1], tp), tap4(pl.c[2], tp), tap4(pl.c[3], tp));
 }
+// the same from an fp16 MPI (overloads, so that the fp32 functions keep their symbols)
+__device__ __noinline__ float4 sample_plane_direct(const __half* __restrict__ plane, int Ht, int Wt, float ix, float iy) {
+    const size_t tex = (size_t)Ht * Wt;
+    const Taps tp = make_taps(ix, iy, Ht, Wt);
+    return make_float4(tap4(plane, tp), tap4(plane + tex, tp), tap4(plane + 2 * tex, tp), tap4(plane + 3 * tex, tp));
+}
+__device__ __noinline__ float4 sample_chans_direct(const PlaneChansT<__half> pl, int Ht, int Wt, float ix, float iy) {
+    const Taps tp = make_taps(ix, iy, Ht, Wt);
+    return make_float4(tap4(pl.c[0], tp), tap4(pl.c[1], tp), tap4(pl.c[2], tp), tap4(pl.c[3], tp));
+}
 // generic-path sample of plane i of MPI m: the instantiation decides which form crosses the call
-template <bool kFactored>
-__device__ __forceinline__ float4 sample_plane_any(const RenderParams& p, const float* plane, int m, int i, size_t tex, float ix, float iy) {
-    if (kFactored) return sample_chans_direct(plane_chans(p, m, i, tex), p.Ht, p.Wt, ix, iy);
+template <bool kFactored, class E>
+__device__ __forceinline__ float4 sample_plane_any(const RenderParams& p, const E* plane, int m, int i, size_t tex, float ix, float iy) {
+    if (kFactored) return sample_chans_direct(plane_chans<E>(p, m, i, tex), p.Ht, p.Wt, ix, iy);
     return sample_plane_direct(plane, p.Ht, p.Wt, ix, iy);
 }
 
@@ -339,6 +358,13 @@ struct FwdRingWide {      // the factored forward's ring: 64- or 96-wide boxes (
     // of 128 (TMA destination alignment): any r for bw = 64 / 96.
     static constexpr int kColourCopyRows = kMaxBH / 2;
 };
+// GMPI_MPI_F16: the same rings with stages of the wider fp16 boxes (staged_width), in elements
+struct FwdRingF16 : FwdRing {
+    static constexpr int kPlaneFloats = (kMaxBW + 8) * kMaxBH * 4, kStride = kPlaneFloats;
+};
+struct FwdRingWideF16 : FwdRingWide {
+    static constexpr int kPlaneFloats = (kWideBW + 32) * kMaxBH * 4, kStride = kPlaneFloats;
+};
 
 // The expanded forward's copies of one stage: the footprint's n_chunks 4-row chunks as the binary digits of n_chunks.  Lane 0..3
 // owns the digit 8, 4, 2, 1: returns the copy's height in chunks (0: this lane issues nothing) and, in `before`, the chunks
@@ -373,8 +399,9 @@ __device__ __forceinline__ uint32_t idle_consumer_warps(int py0, int H) {
 // header and issue the TMA copies.
 // kFact: factored MPI (compile time: a run-time test of p.alpha in this loop cost the forward 1 %, the producer's per-stage latency
 // being on the critical path of a shallow ring).
-template <bool kAlignCorners, class Ring, bool kFact, bool kES = false>
-__device__ __forceinline__ void staged_producer(const RenderParams& p, const TmaMaps& maps, float* s_buf, StageMeta* s_meta,
+// E: the MPI's element type (the ring holds boxes of it).
+template <bool kAlignCorners, class Ring, bool kFact, bool kES = false, class E = float>
+__device__ __forceinline__ void staged_producer(const RenderParams& p, const TmaMaps& maps, E* s_buf, StageMeta* s_meta,
                                             uint64_t* s_full, uint64_t* s_empty, const TileWalk* s_walk, int lane,
                                             int n_stages = Ring::kRingStages, uint32_t* s_stop = nullptr) {
     constexpr bool kReverse = Ring::kReverse;
@@ -419,7 +446,8 @@ __device__ __forceinline__ void staged_producer(const RenderParams& p, const Tma
             const int fx = finite ? (int)floorf(tc.ix) : 0, fy = finite ? (int)floorf(tc.iy) : 0;
             const int xmin = __reduce_min_sync(0xffffffffu, fx), xmax = __reduce_max_sync(0xffffffffu, fx);
             const int ymin = __reduce_min_sync(0xffffffffu, fy), ymax = __reduce_max_sync(0xffffffffu, fy);
-            // TMA needs a 16-byte aligned start in the innermost dimension: the box origin is a multiple of 4 texels
+            // TMA needs a 16-byte aligned start in the innermost dimension: the box origin is a multiple of 4 texels (fp16: the staged
+            // box starts at bxs, a multiple of 8, see staged_width)
             const int bx0 = ((xmin - 1) >> 2) << 2, by0 = ymin - 1;
             const int need_w = xmax - bx0 + 3, need_h = ymax - ymin + 4;      // +1 east/south tap, +-1 slack
             int mode = 0;
@@ -430,6 +458,7 @@ __device__ __forceinline__ void staged_producer(const RenderParams& p, const Tma
             // width class k (tensor-map slot, one-hot bit 16 + k of the header); wide rings: slot 1 = 64, slot 4 = kWideBW
             const int k = mode != 0 ? 0 : kWide ? (need_w <= 64 ? 1 : 4) : max(0, (need_w - kMinBW + kBWStep - 1) / kBWStep);
             const int bw = class_width(k, kWide);
+            const int bxs = sizeof(E) == 2 ? (bx0 & ~7) : bx0, sw = staged_width<E>(bw, kWide);   // staged box: origin, width
             const int n_ops = mode == 0 ? (need_h + kRowsPerOp - 1) / kRowsPerOp : 0;
             const int rows = n_ops * kRowsPerOp;
             if (Ring::kSleepPolls) mbar_wait_sleep(&s_empty[s], ph ^ 1);
@@ -448,14 +477,14 @@ __device__ __forceinline__ void staged_producer(const RenderParams& p, const Tma
                 StageMeta mt;
                 mt.cx = kFloorMagicBits + bx0; mt.cy = kFloorMagicBits + by0;
                 mt.rows2 = rows - 2;
-                mt.sel = bw | (mode << 8) | ((mode == 0 && pc.fast != 0.0f ? (1 << k) : kSelSlow) << 16);
+                mt.sel = bw | (mode << 8) | ((mode == 0 && pc.fast != 0.0f ? (1 << k) : kSelSlow) << 16) | ((bx0 - bxs) << 10);
                 if constexpr (kReverse) {   // backward: a footprint too magnified for the int32 gradient box (BwdRing::kMagLimit)
                     const int ext_x = min(px0 + kTileW - 1, p.W - 1) - px0, ext_y = min(py0 + kTileH - 1, p.H - 1) - py0;
                     if (Ring::kMagLimit * (xmax - xmin - 1) < ext_x || Ring::kMagLimit * (ymax - ymin - 1) < ext_y) mt.sel &= 0xffff;
                 }
                 s_meta[s] = mt;
                 // bytes the copies of this stage will deliver (a box counts whole, zero-filled parts included)
-                const uint32_t tx = (uint32_t)((kFact ? kMaxBH : rows) * bw * 16);
+                const uint32_t tx = (uint32_t)((kFact ? kMaxBH : rows) * sw * (int)(4 * sizeof(E)));
                 if (n_copy > 0 || kTBytes) mbar_arrive_expect_tx(&s_full[s], (n_copy > 0 ? tx : 0u) + kTBytes);
                 else mbar_arrive(&s_full[s]);
                 if (kReverse)   // the tile's saved transmittance for this plane rides in the same stage
@@ -465,7 +494,7 @@ __device__ __forceinline__ void staged_producer(const RenderParams& p, const Tma
             // Few, tall copies.  UTMALDG takes uniform operands, so the lanes of a warp issue their copies ONE AFTER ANOTHER: with a
             // 4-row copy per lane (9-11 per stage, twice that for the factored MPI) the producer was the bottleneck of its own ring.
             if (n_copy > 0) {
-                float* stage = s_buf + (size_t)s * kStride;
+                E* stage = s_buf + (size_t)s * kStride;
                 if constexpr (kFact) {
                     // factored MPI: the colour box [row][3][bw] (shared image, or the last plane's own) starts the stage, as two or
                     // three copies that tile the ring's box height; the alpha box [row][bw] follows after 3/4 of the stage, as one copy
@@ -474,12 +503,12 @@ __device__ __forceinline__ void staged_producer(const RenderParams& p, const Tma
                     constexpr int kCR = Ring::kColourCopyRows;      // (a copy's destination must be 128-byte aligned, see the rings)
                     static_assert(kMaxBH % kCR == 0, "colour copies tile the box");
                     const CUtensorMap* cmap = (p.bg_rgb && i == N - 1) ? &maps.bg[k] : &maps.rgb[k];
-                    if (lane < kMaxBH / kCR) tma_load_4d(stage + (size_t)lane * kCR * 3 * bw, cmap, &s_full[s], bx0, 0, by0 + lane * kCR, m);
-                    if (lane == 31) tma_load_3d(stage + (kStageFloats / 4) * 3, &maps.a[k], &s_full[s], bx0, by0, m * N + i);
+                    if (lane < kMaxBH / kCR) tma_load_4d(stage + (size_t)lane * kCR * 3 * sw, cmap, &s_full[s], bxs, 0, by0 + lane * kCR, m);
+                    if (lane == 31) tma_load_3d(stage + (kStageFloats / 4) * 3, &maps.a[k], &s_full[s], bxs, by0, m * N + i);
                 } else if (!Ring::kBinaryCopies) {
                     // expanded MPI, backward: one 4-row copy per lane (measured: taller copies make its 2-stage ring 0.5 % slower)
                     if (lane < n_ops)
-                        tma_load_4d(stage + (size_t)lane * kRowsPerOp * 4 * bw, &maps.m[k], &s_full[s], bx0, 0, by0 + lane * kRowsPerOp, m * N + i);
+                        tma_load_4d(stage + (size_t)lane * kRowsPerOp * 4 * sw, &maps.m[k], &s_full[s], bxs, 0, by0 + lane * kRowsPerOp, m * N + i);
                 } else if (lane < 4) {
                     // expanded MPI, forward (HBM-bound: no over-fetch): the n_ops 4-row chunks go out as the binary digits of n_ops,
                     // one copy of 32, 16, 8 and 4 rows each where the digit is set -- at most three copies for up to 44 rows (-1.1 %)
@@ -487,7 +516,7 @@ __device__ __forceinline__ void staged_producer(const RenderParams& p, const Tma
                     const int h = binary_copy_of_lane(n_ops, lane, before);
                     if (h) {
                         const CUtensorMap* mp = h == 8 ? &maps.m32[k] : h == 4 ? &maps.m16[k] : h == 2 ? &maps.m8[k] : &maps.m[k];
-                        tma_load_4d(stage + (size_t)before * kRowsPerOp * 4 * bw, mp, &s_full[s], bx0, 0, by0 + before * kRowsPerOp, m * N + i);
+                        tma_load_4d(stage + (size_t)before * kRowsPerOp * 4 * sw, mp, &s_full[s], bxs, 0, by0 + before * kRowsPerOp, m * N + i);
                     }
                 }
             }
@@ -543,17 +572,20 @@ __device__ __forceinline__ void store_tile_pixels(const RenderParams& p, int v, 
 }
 
 // Body of the staged forward kernels.  kES: early stop (mpi_fwd_early_stop_kernel; s_stop is its stop-word ring, see kStopSlots).
-template <bool kAlignCorners, bool kEmitT, bool kFactored, bool kES>
+// E: the MPI's element type (__half: GMPI_MPI_F16, the ring's boxes are fp16, each stage half the bytes).
+template <bool kAlignCorners, bool kEmitT, bool kFactored, bool kES, class E = float>
 __device__ __forceinline__ void fwd_staged_body(const RenderParams& p, const TmaMaps& maps, const int tiles_x, const int ring_stages,
                                                 uint32_t* s_stop) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
-    float* s_buf = reinterpret_cast<float*>(smem_raw);   // the ring starts the dynamic segment (1024-byte aligned)
-    using Ring = typename std::conditional<kFactored, FwdRingWide, FwdRing>::type;
+    E* s_buf = reinterpret_cast<E*>(smem_raw);   // the ring starts the dynamic segment (1024-byte aligned)
+    constexpr bool kHalf = sizeof(E) == 2;
+    using Ring = typename std::conditional<kFactored, typename std::conditional<kHalf, FwdRingWideF16, FwdRingWide>::type,
+                                           typename std::conditional<kHalf, FwdRingF16, FwdRing>::type>::type;
     constexpr int kStages = Ring::kRingStages;              // ring stages allocated; the expanded MPI uses ring_stages of them
     const int n_stages = kFactored ? kStages : ring_stages;
     constexpr int kRingFloats = Ring::kPlaneFloats;         // floats per ring stage
     constexpr int kAOff = kFactored ? 3 * (kRingFloats / 4) : 0;      // factored: alpha box behind the colour box
-    PlaneConst* s_pc = reinterpret_cast<PlaneConst*>(smem_raw + (size_t)n_stages * kRingFloats * 4);   // [N] of the current view
+    PlaneConst* s_pc = reinterpret_cast<PlaneConst*>(smem_raw + (size_t)n_stages * kRingFloats * sizeof(E));   // [N] of the current view
     __shared__ StageMeta s_meta[kStages];
     __shared__ __align__(8) uint64_t s_full[kStages], s_empty[kStages];
     __shared__ TileWalk s_walk;
@@ -581,7 +613,7 @@ __device__ __forceinline__ void fwd_staged_body(const RenderParams& p, const Tma
     const size_t img = (size_t)p.H * p.W;
 
     if (warp == kConsWarps) {
-        staged_producer<kAlignCorners, Ring, kFactored, kES>(p, maps, s_buf, s_meta, s_full, s_empty, &s_walk, lane, n_stages, s_stop);
+        staged_producer<kAlignCorners, Ring, kFactored, kES, E>(p, maps, s_buf, s_meta, s_full, s_empty, &s_walk, lane, n_stages, s_stop);
     } else {
         // ================================ consumer warps ================================
         // warp w owns rows kPairs*w .. kPairs*w + kPairs-1 of the tile; a lane owns x = lane and lane+32 on each of them
@@ -656,27 +688,27 @@ __device__ __forceinline__ void fwd_staged_body(const RenderParams& p, const Tma
                 }
                 mbar_wait(&s_full[s], ph);
                 const StageMeta mt = s_meta[s];
-                const float* sb = s_buf + s * kRingFloats;
+                const E* sb = s_buf + s * kRingFloats + (kHalf ? (mt.sel >> 10) & 7 : 0);   // fp16: the fp32 box's origin in the stage
                 const int sel = mt.sel;                  // warp-uniform; the producer already folded mode and plane range in
                 bool done = warp_stopped;                // a stopped warp only waits on and releases the stage
                 if (warp_fast && !done) {
                     if (Ring::kWideFact) {               // factored: two widths, both with bank-aligned row pitches
-                        if (sel & (1 << 20)) done = sample_pairs<kWideBW, kAOff, kES>(sb, mt.cx, mt.cy, mt.rows2, cc, T, cr, cg, cb, cws, tau);
-                        else if (sel & (1 << 17)) done = sample_pairs<64, kAOff, kES>(sb, mt.cx, mt.cy, mt.rows2, cc, T, cr, cg, cb, cws, tau);
+                        if (sel & (1 << 20)) done = sample_pairs<kWideBW, kAOff, kES, E>(sb, mt.cx, mt.cy, mt.rows2, cc, T, cr, cg, cb, cws, tau);
+                        else if (sel & (1 << 17)) done = sample_pairs<64, kAOff, kES, E>(sb, mt.cx, mt.cy, mt.rows2, cc, T, cr, cg, cb, cws, tau);
                     } else {                             // most frequent classes first (FFHQ poses: 72 > 64 > 80 >> 56, 88)
-                        if (sel & (1 << 18)) done = sample_pairs<72, kAOff, kES>(sb, mt.cx, mt.cy, mt.rows2, cc, T, cr, cg, cb, cws, tau);
-                        else if (sel & (1 << 17)) done = sample_pairs<64, kAOff, kES>(sb, mt.cx, mt.cy, mt.rows2, cc, T, cr, cg, cb, cws, tau);
-                        else if (sel & (1 << 19)) done = sample_pairs<80, kAOff, kES>(sb, mt.cx, mt.cy, mt.rows2, cc, T, cr, cg, cb, cws, tau);
-                        else if (sel & (1 << 16)) done = sample_pairs<56, kAOff, kES>(sb, mt.cx, mt.cy, mt.rows2, cc, T, cr, cg, cb, cws, tau);
-                        else if (sel & (1 << 20)) done = sample_pairs<88, kAOff, kES>(sb, mt.cx, mt.cy, mt.rows2, cc, T, cr, cg, cb, cws, tau);
+                        if (sel & (1 << 18)) done = sample_pairs<72, kAOff, kES, E>(sb, mt.cx, mt.cy, mt.rows2, cc, T, cr, cg, cb, cws, tau);
+                        else if (sel & (1 << 17)) done = sample_pairs<64, kAOff, kES, E>(sb, mt.cx, mt.cy, mt.rows2, cc, T, cr, cg, cb, cws, tau);
+                        else if (sel & (1 << 19)) done = sample_pairs<80, kAOff, kES, E>(sb, mt.cx, mt.cy, mt.rows2, cc, T, cr, cg, cb, cws, tau);
+                        else if (sel & (1 << 16)) done = sample_pairs<56, kAOff, kES, E>(sb, mt.cx, mt.cy, mt.rows2, cc, T, cr, cg, cb, cws, tau);
+                        else if (sel & (1 << 20)) done = sample_pairs<88, kAOff, kES, E>(sb, mt.cx, mt.cy, mt.rows2, cc, T, cr, cg, cb, cws, tau);
                     }
                 }
                 if (!done) {
                     // ---- generic body: per-pixel range / box checks, direct sampling when not staged ----
-                    const int bw = mt.sel & 0xff, mode = (mt.sel >> 8) & 3, bw4 = 4 * bw;
+                    const int bw = mt.sel & 0xff, mode = (mt.sel >> 8) & 3, bws = staged_width<E>(bw, false), bw4 = 4 * bws;
                     const float fbw2 = (float)(bw - 2), fbh2 = (float)mt.rows2;
                     const float fbx0 = (float)(mt.cx - kFloorMagicBits), fby0 = (float)(mt.cy - kFloorMagicBits);
-                    const float* plane = kFactored ? nullptr : p.rgba + ((size_t)m * N + i) * 4 * tex;
+                    const E* plane = kFactored ? nullptr : reinterpret_cast<const E*>(p.rgba) + ((size_t)m * N + i) * 4 * tex;
                     float* Ts = reinterpret_cast<float*>(T);
                     float* crs = reinterpret_cast<float*>(cr);
                     float* cgs = reinterpret_cast<float*>(cg);
@@ -695,15 +727,17 @@ __device__ __forceinline__ void fwd_staged_body(const RenderParams& p, const Tma
                             const float wx1 = tc.ix - fx, wy1 = tc.iy - fy;
                             const float wx0 = 1.0f - wx1, wy0 = 1.0f - wy1;
                             const float w00 = wx0 * wy0, w01 = wx1 * wy0, w10 = wx0 * wy1, w11 = wx1 * wy1;
-                            const float* t0 = sb + ((int)ryy * bw4 + (int)rxx);
-                            const float* t1 = t0 + bw4;
-                            r = fmaf(t1[1], w11, fmaf(t1[0], w10, fmaf(t0[1], w01, t0[0] * w00)));
-                            g = fmaf(t1[bw + 1], w11, fmaf(t1[bw], w10, fmaf(t0[bw + 1], w01, t0[bw] * w00)));
-                            b = fmaf(t1[2 * bw + 1], w11, fmaf(t1[2 * bw], w10, fmaf(t0[2 * bw + 1], w01, t0[2 * bw] * w00)));
-                            a = fmaf(t1[3 * bw + 1], w11, fmaf(t1[3 * bw], w10, fmaf(t0[3 * bw + 1], w01, t0[3 * bw] * w00)));
+                            const E* t0 = sb + ((int)ryy * bw4 + (int)rxx);
+                            const E* t1 = t0 + bw4;
+                            r = fmaf(to_f32(t1[1]), w11, fmaf(to_f32(t1[0]), w10, fmaf(to_f32(t0[1]), w01, to_f32(t0[0]) * w00)));
+                            g = fmaf(to_f32(t1[bws + 1]), w11, fmaf(to_f32(t1[bws]), w10, fmaf(to_f32(t0[bws + 1]), w01, to_f32(t0[bws]) * w00)));
+                            b = fmaf(to_f32(t1[2 * bws + 1]), w11,
+                                     fmaf(to_f32(t1[2 * bws]), w10, fmaf(to_f32(t0[2 * bws + 1]), w01, to_f32(t0[2 * bws]) * w00)));
+                            a = fmaf(to_f32(t1[3 * bws + 1]), w11,
+                                     fmaf(to_f32(t1[3 * bws]), w10, fmaf(to_f32(t0[3 * bws + 1]), w01, to_f32(t0[3 * bws]) * w00)));
                         } else if (coord_hits(tc.ix, tc.iy, fWt, fHt)) {   // mode 1 ("nothing under the tile") is only the
                             // producer's corner-ray estimate: every pixel is still tested on its own
-                            const float4 sv = sample_plane_any<kFactored>(p, plane, m, i, tex, tc.ix, tc.iy);
+                            const float4 sv = sample_plane_any<kFactored, E>(p, plane, m, i, tex, tc.ix, tc.iy);
                             r = sv.x; g = sv.y; b = sv.z; a = sv.w;
                         } else {
                             continue;   // no texel under this ray on this plane: contributes exactly nothing
@@ -770,6 +804,22 @@ mpi_fwd_early_stop_kernel(const RenderParams p, const __grid_constant__ TmaMaps 
                           const int ring_stages) {
     __shared__ uint32_t s_stop[kStopSlots];
     fwd_staged_body<kAlignCorners, false, kFactored, true>(p, maps, tiles_x, ring_stages, s_stop);
+}
+
+// GMPI_MPI_F16: the forward-only kernels above on an fp16 MPI (no training instantiation: the backward reads fp32).  Kernels of their
+// own, so that the fp32 ones keep their machine code.
+template <bool kAlignCorners, bool kFactored>
+__global__ void __launch_bounds__(kStagedThreads, 1)
+mpi_fwd_staged_f16_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps, const int tiles_x, const int tiles_y,
+                          const int ring_stages) {
+    fwd_staged_body<kAlignCorners, false, kFactored, false, __half>(p, maps, tiles_x, ring_stages, nullptr);
+}
+template <bool kAlignCorners, bool kFactored>
+__global__ void __launch_bounds__(kStagedThreads, 1)
+mpi_fwd_early_stop_f16_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps, const int tiles_x, const int tiles_y,
+                              const int ring_stages) {
+    __shared__ uint32_t s_stop[kStopSlots];
+    fwd_staged_body<kAlignCorners, false, kFactored, true, __half>(p, maps, tiles_x, ring_stages, s_stop);
 }
 
 }  // namespace gmpi

@@ -50,8 +50,8 @@ constexpr int kFwdTileW = 32;
 constexpr int kFwdTileH = 8;
 
 // kES: GMPI_EARLY_STOP, a pixel composites no further plane once |T| <= p.early_stop (mpi_fwd_direct_early_stop_kernel).
-// (p by value: with a reference ptxas allocates the default kernel's registers differently.)
-template <bool kAlignCorners, bool kES>
+// (p by value: with a reference ptxas allocates the default kernel's registers differently.)  E: the MPI's element type.
+template <bool kAlignCorners, bool kES, class E = float>
 __device__ __forceinline__ void fwd_direct_body(const RenderParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     PlaneConst* s_pc = reinterpret_cast<PlaneConst*>(smem_raw);
@@ -90,7 +90,7 @@ __device__ __forceinline__ void fwd_direct_body(const RenderParams p) {
 #pragma unroll 2
         for (int i = 0; i < p.N; ++i) {
             const PlaneConst pc = s_pc[i];
-            const PlaneChans plane = plane_chans(p, m, i, tex);
+            const PlaneChansT<E> plane = plane_chans<E>(p, m, i, tex);
             if (!kES && p.transmittance) p.transmittance[((size_t)v * p.N + i) * img + pix] = T;   // training: T_i for the backward sweep
             const TexCoord tc = plane_coord<kAlignCorners>(pc, rc, hsx, hsy, fWt, fHt);
             if (check_last && i == p.N - 1) {
@@ -131,6 +131,19 @@ template <bool kAlignCorners>
 __global__ void __launch_bounds__(kFwdTileW* kFwdTileH)
 mpi_fwd_direct_early_stop_kernel(const RenderParams p) {
     fwd_direct_body<kAlignCorners, true>(p);
+}
+
+// GMPI_MPI_F16: the direct forward kernels on an fp16 MPI (kernels of their own: the fp32 ones keep their machine code)
+template <bool kAlignCorners>
+__global__ void __launch_bounds__(kFwdTileW* kFwdTileH)
+mpi_fwd_direct_f16_kernel(const RenderParams p) {
+    fwd_direct_body<kAlignCorners, false, __half>(p);
+}
+
+template <bool kAlignCorners>
+__global__ void __launch_bounds__(kFwdTileW* kFwdTileH)
+mpi_fwd_direct_early_stop_f16_kernel(const RenderParams p) {
+    fwd_direct_body<kAlignCorners, true, __half>(p);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -260,6 +273,37 @@ __global__ void mpi_check_range_scalar_kernel(const float* __restrict__ rgba, si
     if (flag) atomicOr(flags, flag);
 }
 
+// The same check of an fp16 MPI, with the flags the fp32 check sets on its upcast: a half is inside [0,1] iff its bit pattern is
+// <= 0x3c00 (1.0) or it is -0.0; negatives, values above 1, infinities and NaN have larger patterns, as their upcasts do in fp32.
+__device__ __forceinline__ bool out_of_unit_f16(uint32_t b) { return b > 0x3c00u && b != 0x8000u; }
+
+__global__ void __launch_bounds__(256)
+mpi_check_range_f16_kernel(const uint4* __restrict__ rgba8, size_t n_slabs, size_t slab8, uint32_t* flags) {
+    // one slab = one (mpi, plane, channel) image of slab8 groups of eight halves; channel = slab % 4
+    uint32_t flag = 0;
+    const size_t total = n_slabs * slab8;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const uint4 x = __ldcs(rgba8 + i);
+        const uint32_t w[4] = {x.x, x.y, x.z, x.w};
+        bool out = false;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) out = out || out_of_unit_f16(w[k] & 0xffffu) || out_of_unit_f16(w[k] >> 16);
+        if (out) flag |= (((i / slab8) & 3) == 3) ? (GMPI_FLAG_ALPHA_RANGE | GMPI_FLAG_RGBA_RANGE) : GMPI_FLAG_RGBA_RANGE;
+    }
+    flag = __reduce_or_sync(0xffffffffu, flag);
+    if (flag && (threadIdx.x & 31) == 0) atomicOr(flags, flag);
+}
+
+__global__ void mpi_check_range_f16_scalar_kernel(const unsigned short* __restrict__ rgba, size_t n_slabs, size_t slab, uint32_t* flags) {
+    uint32_t flag = 0;
+    const size_t total = n_slabs * slab;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        if (out_of_unit_f16(__ldcs(rgba + i)))
+            flag |= (((i / slab) & 3) == 3) ? (GMPI_FLAG_ALPHA_RANGE | GMPI_FLAG_RGBA_RANGE) : GMPI_FLAG_RGBA_RANGE;
+    }
+    if (flag) atomicOr(flags, flag);
+}
+
 // ------------------------------------------------------------------------------------------
 // Test hook: texel coordinates.
 // ------------------------------------------------------------------------------------------
@@ -346,6 +390,11 @@ static std::atomic<int> g_fwd_stages{0};    // expanded staged forward's ring de
 
 // Argument checks shared by every entry point.  `bwd`: gradients instead of outputs.
 static int check_params(const RenderParams& p, bool bwd) {
+    if (p.options & GMPI_MPI_F16) {
+        if (bwd) return fail(GMPI_ERR_UNSUPPORTED, "GMPI_MPI_F16 is forward-only: the backward reads and writes fp32 MPIs");
+        if (p.transmittance)
+            return fail(GMPI_ERR_UNSUPPORTED, "GMPI_MPI_F16 cannot be combined with the training forward (transmittance)");
+    }
     if (p.options & GMPI_EARLY_STOP) {
         if (bwd) return fail(GMPI_ERR_UNSUPPORTED, "GMPI_EARLY_STOP is forward-only: the backward needs every plane's samples");
         if (p.transmittance)
@@ -374,13 +423,13 @@ static int check_params(const RenderParams& p, bool bwd) {
     return GMPI_OK;
 }
 
-// staged needs 16-byte row strides for the tensor map and enough tiles to fill the persistent grid; `why` receives the
-// GMPI_WHY_* bits of every reason the TMA-staged kernel is NOT used (0 = staged)
-static bool staged_eligible(int V, int N, int Ht, int Wt, int H, int W, uint32_t* why = nullptr) {
+// staged needs 16-byte row strides for the tensor map (Wt % 4 == 0 in fp32, Wt % 8 == 0 in fp16) and enough tiles to fill the
+// persistent grid; `why` receives the GMPI_WHY_* bits of every reason the TMA-staged kernel is NOT used (0 = staged)
+static bool staged_eligible(int V, int N, int Ht, int Wt, int H, int W, uint32_t* why = nullptr, bool f16 = false) {
     (void)Ht;
     uint32_t w = 0;
     if (N > kMaxPlanesStaged) w |= GMPI_WHY_MANY_PLANES;
-    if (Wt % 4 != 0) w |= GMPI_WHY_TEX_WIDTH;
+    if (Wt % (f16 ? 8 : 4) != 0) w |= GMPI_WHY_TEX_WIDTH;
     const int forced = g_fwd_variant.load(std::memory_order_relaxed);
     if (forced == 1) w |= GMPI_WHY_FORCED;
     const long tiles = (long)((W + kTileW - 1) / kTileW) * ((H + kTileH - 1) / kTileH) * V;
@@ -397,17 +446,20 @@ static bool mpi_aligned(const RenderParams& p) {
 // Tensor maps of the MPI (expanded or factored) for the five box-width classes.  Returns 0 on success.
 // box_h, colour_rows: the ring's box height and kColourCopyRows (factored: colour copies of colour_rows rows, one alpha copy of box_h).
 // wide: the factored forward's ring (FwdRingWide) -- slot 4 holds the kWideBW-wide boxes, slot 1 the 64-wide ones, the rest unused.
+// The element type is the MPI's: fp16 under GMPI_MPI_F16, else fp32.
 static int encode_mpi_maps(TmaMaps& maps, const RenderParams& p, int box_h, int colour_rows, bool wide = false) {
+    const bool f16 = (p.options & GMPI_MPI_F16) != 0;
+    const MapElem el = f16 ? kMapF16 : kMapF32;
     for (int k = 0; k < kNumMaps; ++k) {
-        const int bw = class_width(k, wide);
+        const int bw = f16 ? staged_width<__half>(class_width(k, wide), wide) : class_width(k, wide);
         if (p.alpha) {
-            if (encode_color_map(&maps.rgb[k], p.rgb, (uint64_t)p.M, p.Ht, p.Wt, bw, colour_rows) != 0) return -1;
-            if (p.bg_rgb && encode_color_map(&maps.bg[k], p.bg_rgb, (uint64_t)p.M, p.Ht, p.Wt, bw, colour_rows) != 0) return -1;
-            if (encode_slab_map(&maps.a[k], p.alpha, (uint64_t)p.M * p.N, p.Ht, p.Wt, bw, box_h, 1) != 0) return -1;
+            if (encode_color_map(&maps.rgb[k], p.rgb, el, (uint64_t)p.M, p.Ht, p.Wt, bw, colour_rows) != 0) return -1;
+            if (p.bg_rgb && encode_color_map(&maps.bg[k], p.bg_rgb, el, (uint64_t)p.M, p.Ht, p.Wt, bw, colour_rows) != 0) return -1;
+            if (encode_slab_map(&maps.a[k], p.alpha, el, (uint64_t)p.M * p.N, p.Ht, p.Wt, bw, box_h, 1) != 0) return -1;
         } else {
             CUtensorMap* const by_rows[4] = {&maps.m[k], &maps.m8[k], &maps.m16[k], &maps.m32[k]};
             for (int b = 0; b < 4; ++b)
-                if (encode_plane_map(by_rows[b], p.rgba, (uint64_t)p.M * p.N, p.Ht, p.Wt, bw, kRowsPerOp << b) != 0) return -1;
+                if (encode_plane_map(by_rows[b], p.rgba, el, (uint64_t)p.M * p.N, p.Ht, p.Wt, bw, kRowsPerOp << b) != 0) return -1;
         }
     }
     return 0;
@@ -463,11 +515,22 @@ static constexpr StagedFwdKernel kFwdEarlyStopKernels[2][2] = {
 static constexpr void (*kFwdDirectKernels[2][2])(const RenderParams) = {
     {mpi_fwd_direct_kernel<false>, mpi_fwd_direct_kernel<true>},
     {mpi_fwd_direct_early_stop_kernel<false>, mpi_fwd_direct_early_stop_kernel<true>}};
+// GMPI_MPI_F16: the staged and early-stop forward [early_stop][align_corners][factored], the direct forward [early_stop][align_corners]
+static constexpr StagedFwdKernel kFwdStagedF16Kernels[2][2][2] = {
+    {{mpi_fwd_staged_f16_kernel<false, false>, mpi_fwd_staged_f16_kernel<false, true>},
+     {mpi_fwd_staged_f16_kernel<true, false>, mpi_fwd_staged_f16_kernel<true, true>}},
+    {{mpi_fwd_early_stop_f16_kernel<false, false>, mpi_fwd_early_stop_f16_kernel<false, true>},
+     {mpi_fwd_early_stop_f16_kernel<true, false>, mpi_fwd_early_stop_f16_kernel<true, true>}}};
+static constexpr void (*kFwdDirectF16Kernels[2][2])(const RenderParams) = {
+    {mpi_fwd_direct_f16_kernel<false>, mpi_fwd_direct_f16_kernel<true>},
+    {mpi_fwd_direct_early_stop_f16_kernel<false>, mpi_fwd_direct_early_stop_f16_kernel<true>}};
 
-// fac: the kernel's kFactored
+// fac: the kernel's kFactored; f16: its MPI is fp16 (the rings of FwdRingF16 / FwdRingWideF16)
 static cudaError_t launch_fwd_staged(StagedFwdKernel kernel, bool fac, const RenderParams& p, const TmaMaps& maps, int grid, int tiles_x,
-                                     int tiles_y, int stages, cudaStream_t st) {
-    const size_t smem = fac ? kStagedSmemWide : (size_t)stages * kStageFloats * 4 + (size_t)kMaxPlanesStaged * 32;
+                                     int tiles_y, int stages, cudaStream_t st, bool f16 = false) {
+    const size_t ring = f16 ? (size_t)(fac ? kStages * FwdRingWideF16::kPlaneFloats : stages * FwdRingF16::kPlaneFloats) * 2
+                            : (size_t)(fac ? kStages * kWideStageFloats : stages * kStageFloats) * 4;
+    const size_t smem = ring + (size_t)kMaxPlanesStaged * 32;
     cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     kernel<<<grid, kStagedThreads, smem, st>>>(p, maps, tiles_x, tiles_y, stages);
@@ -494,8 +557,8 @@ static int launch_fwd(RenderParams p, cudaStream_t st) {
     // symmetric-memory allocations (256-byte aligned bases; frame slabs are multiples of 16 bytes when W % 4 == 0).
     if (p.W % 4 == 0 && !p.video_rgb && (p.n_peers > 0 || (aligned16(p.color) && aligned16(p.depth)))) p.options |= kOptVec4Stores;
     const bool ac = (p.options & GMPI_ALIGN_CORNERS) != 0, emit = p.transmittance != nullptr, fac = p.alpha != nullptr;
-    const bool es = (p.options & GMPI_EARLY_STOP) != 0;
-    if (staged_eligible(p.V, p.N, p.Ht, p.Wt, p.H, p.W) && mpi_aligned(p) && (size_t)p.M * p.N < ((size_t)1 << 31)) {
+    const bool es = (p.options & GMPI_EARLY_STOP) != 0, f16 = (p.options & GMPI_MPI_F16) != 0;
+    if (staged_eligible(p.V, p.N, p.Ht, p.Wt, p.H, p.W, nullptr, f16) && mpi_aligned(p) && (size_t)p.M * p.N < ((size_t)1 << 31)) {
         TmaMaps maps;
         if (encode_mpi_maps(maps, p, kMaxBH, FwdRingWide::kColourCopyRows, fac) != 0) {
             if (g_fwd_variant.load(std::memory_order_relaxed) == 2) return fail(GMPI_ERR_CUDA, "cuTensorMapEncodeTiled failed");
@@ -509,8 +572,8 @@ static int launch_fwd(RenderParams p, cudaStream_t st) {
             const long n_tiles = (long)tiles_x * tiles_y * p.V;
             const int grid = (int)(n_tiles < sms ? n_tiles : sms);
             if (es && (rc = reset_early_stop_stats((unsigned long long)n_tiles * p.N, st)) != 0) return rc;
-            const StagedFwdKernel kernel = es ? kFwdEarlyStopKernels[ac][fac] : kFwdStagedKernels[ac][emit][fac];
-            cudaError_t e = launch_fwd_staged(kernel, fac, p, maps, grid, tiles_x, tiles_y, stages, st);
+            const StagedFwdKernel kernel = f16 ? kFwdStagedF16Kernels[es][ac][fac] : es ? kFwdEarlyStopKernels[ac][fac] : kFwdStagedKernels[ac][emit][fac];
+            cudaError_t e = launch_fwd_staged(kernel, fac, p, maps, grid, tiles_x, tiles_y, stages, st, f16);
             GMPI_CUDA_OK(e);
             GMPI_CUDA_OK(cudaGetLastError());
             return GMPI_OK;
@@ -524,7 +587,7 @@ static int launch_fwd(RenderParams p, cudaStream_t st) {
     if (grid.y > 65535) return fail(GMPI_ERR_UNSUPPORTED, "image height %d too large", p.H);
     if (p.V > 65535) return fail(GMPI_ERR_UNSUPPORTED, "V=%d views exceed one launch of the direct kernel (65535); split the batch", p.V);
     if (es && (rc = reset_early_stop_stats(0, st)) != 0) return rc;    // the direct kernel loads per pixel: no stages to skip
-    void (*kernel)(const RenderParams) = kFwdDirectKernels[es][ac];
+    void (*kernel)(const RenderParams) = f16 ? kFwdDirectF16Kernels[es][ac] : kFwdDirectKernels[es][ac];
     if (smem > 48 * 1024) GMPI_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     kernel<<<grid, block, smem, st>>>(p);
     GMPI_CUDA_OK(cudaGetLastError());
@@ -596,7 +659,7 @@ static int launch_bwd(RenderParams p, cudaStream_t st) {
     if (p.view_group < 1) p.view_group = 1;
     TmaMaps maps;
     if (encode_mpi_maps(maps, p, kBwdMaxBH, BwdRing::kColourCopyRows) != 0) return fail(GMPI_ERR_CUDA, "cuTensorMapEncodeTiled failed");
-    if (encode_slab_map(&maps.t, p.transmittance, (uint64_t)p.V * p.N, p.H, p.W, kTileW, kBwdTileH, 1) != 0)
+    if (encode_slab_map(&maps.t, p.transmittance, kMapF32, (uint64_t)p.V * p.N, p.H, p.W, kTileW, kBwdTileH, 1) != 0)
         return fail(GMPI_ERR_CUDA, "cuTensorMapEncodeTiled (transmittance) failed");
     int sms = 0;
     if ((rc = device_sms(&sms)) != 0) return rc;
@@ -638,6 +701,13 @@ static int check_desc(const gmpi_render_desc* d) {
     if (d->struct_bytes != sizeof(gmpi_render_desc) && (d->options & GMPI_EARLY_STOP))
         return fail(GMPI_ERR_INVALID_ARGUMENT, "GMPI_EARLY_STOP needs struct_bytes = %zu (a descriptor with the early_stop field)",
                     sizeof(gmpi_render_desc));
+    return GMPI_OK;
+}
+
+// The classic entry points take fp32 MPIs only (their pointers are typed float*): GMPI_MPI_F16 needs a descriptor.
+static int refuse_f16_classic(uint32_t options) {
+    if (options & GMPI_MPI_F16)
+        return fail(GMPI_ERR_UNSUPPORTED, "GMPI_MPI_F16 is accepted by gmpi_mpi_render_fwd_ex and gmpi_mpi_render_host_ex only");
     return GMPI_OK;
 }
 
@@ -732,6 +802,18 @@ int gmpi_mpi_render_fwd_plan(int V, int N, int Ht, int Wt, int H, int W, const v
     return w == 0 ? GMPI_PLAN_STAGED : GMPI_PLAN_DIRECT;
 }
 
+int gmpi_mpi_render_fwd_plan_ex(const gmpi_render_desc* d, uint32_t* why) {
+    int rc = check_desc(d);
+    if (rc) return -rc;
+    const bool f16 = (d->options & GMPI_MPI_F16) != 0;
+    uint32_t w = 0;
+    staged_eligible(d->V, d->N, d->Ht, d->Wt, d->H, d->W, &w, f16);
+    for (const float* t : {d->rgba, d->rgb, d->alpha, d->bg_rgb})
+        if (t && !aligned16(t)) w |= GMPI_WHY_ALIGNMENT;
+    if (why) *why = w;
+    return w == 0 ? GMPI_PLAN_STAGED : GMPI_PLAN_DIRECT;
+}
+
 const char* gmpi_mpi_render_fwd_variant(int N, int Ht, int Wt, int H, int W) {
     return staged_eligible(1 << 20, N, Ht, Wt, H, W) ? "fwd_staged_tma_64x30" : "fwd_direct_32x8";
 }
@@ -739,6 +821,7 @@ const char* gmpi_mpi_render_fwd_variant(int N, int Ht, int Wt, int H, int W) {
 int gmpi_mpi_render_fwd(const float* rgba, const int32_t* view2mpi, const float* dhw, const float* ray_dir,
                         const float* eye, const float* z_dir, float* color, float* depth, uint32_t* flags, int M,
                         int V, int N, int Ht, int Wt, int H, int W, uint32_t options, void* stream) {
+    if (int rc = refuse_f16_classic(options)) return rc;
     RenderParams p = params_classic(rgba, view2mpi, dhw, ray_dir, eye, z_dir, M, V, N, Ht, Wt, H, W, options);
     p.color = color; p.depth = depth; p.flags = flags;
     return launch_fwd(p, (cudaStream_t)stream);
@@ -748,6 +831,7 @@ int gmpi_mpi_render_fwd_train(const float* rgba, const int32_t* view2mpi, const 
                               const float* eye, const float* z_dir, float* color, float* depth, float* transmittance,
                               uint32_t* flags, int M, int V, int N, int Ht, int Wt, int H, int W, uint32_t options,
                               void* stream) {
+    if (int rc = refuse_f16_classic(options)) return rc;
     if (!transmittance) return fail(GMPI_ERR_INVALID_ARGUMENT, "null transmittance buffer");
     RenderParams p = params_classic(rgba, view2mpi, dhw, ray_dir, eye, z_dir, M, V, N, Ht, Wt, H, W, options);
     p.color = color; p.depth = depth; p.flags = flags; p.transmittance = transmittance;
@@ -758,6 +842,7 @@ int gmpi_mpi_render_fwd_gather(const float* rgba, const int32_t* view2mpi, const
                                const float* eye, const float* z_dir, float* const* peer_frames, int n_peers,
                                int frame_offset, uint32_t* flags, int M, int V, int N, int Ht, int Wt, int H, int W,
                                uint32_t options, void* stream) {
+    if (int rc = refuse_f16_classic(options)) return rc;
     if (n_peers < 1) return fail(GMPI_ERR_INVALID_ARGUMENT, "n_peers must be >= 1");
     RenderParams p = params_classic(rgba, view2mpi, dhw, ray_dir, eye, z_dir, M, V, N, Ht, Wt, H, W, options);
     p.flags = flags; p.peer_frames = peer_frames; p.n_peers = n_peers; p.frame_offset = frame_offset;
@@ -768,6 +853,7 @@ int gmpi_mpi_render_bwd(const float* rgba, const int32_t* view2mpi, const float*
                         const float* eye, const float* z_dir, const float* g_color, const float* g_depth,
                         float* g_rgba, int M, int V, int N, int Ht, int Wt, int H, int W, uint32_t options,
                         void* stream) {
+    if (int rc = refuse_f16_classic(options)) return rc;
     RenderParams p = params_classic(rgba, view2mpi, dhw, ray_dir, eye, z_dir, M, V, N, Ht, Wt, H, W, options);
     p.g_color = g_color; p.g_depth = g_depth; p.g_rgba = g_rgba;
     return launch_bwd(p, (cudaStream_t)stream);
@@ -777,6 +863,7 @@ int gmpi_mpi_render_bwd_saved(const float* rgba, const int32_t* view2mpi, const 
                               const float* eye, const float* z_dir, const float* transmittance, const float* g_color,
                               const float* g_depth, float* g_rgba, int M, int V, int N, int Ht, int Wt, int H, int W,
                               uint32_t options, void* stream) {
+    if (int rc = refuse_f16_classic(options)) return rc;
     if (!transmittance) return fail(GMPI_ERR_INVALID_ARGUMENT, "null gradient / transmittance pointer");
     RenderParams p = params_classic(rgba, view2mpi, dhw, ray_dir, eye, z_dir, M, V, N, Ht, Wt, H, W, options);
     p.g_color = g_color; p.g_depth = g_depth; p.g_rgba = g_rgba; p.transmittance = const_cast<float*>(transmittance);
@@ -814,6 +901,24 @@ int gmpi_mpi_check_range(const float* rgba, int M, int N, int Ht, int Wt, uint32
         mpi_check_range_kernel<<<grid, 256, 0, st>>>(reinterpret_cast<const float4*>(rgba), n_slabs, slab / 4, flags);
     } else {
         mpi_check_range_scalar_kernel<<<grid, 256, 0, st>>>(rgba, n_slabs, slab, flags);
+    }
+    GMPI_CUDA_OK(cudaGetLastError());
+    return GMPI_OK;
+}
+
+int gmpi_mpi_check_range_f16(const void* rgba, int M, int N, int Ht, int Wt, uint32_t* flags, void* stream) {
+    if (!rgba || !flags) return fail(GMPI_ERR_INVALID_ARGUMENT, "null pointer");
+    if (M < 1 || N < 1 || Ht < 1 || Wt < 1) return fail(GMPI_ERR_INVALID_ARGUMENT, "bad sizes");
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t slab = (size_t)Ht * Wt, n_slabs = (size_t)M * N * 4;
+    int sms = 132;
+    int rc = device_sms(&sms);
+    if (rc) return rc;
+    const int grid = sms * 8;
+    if (slab % 8 == 0 && ((uintptr_t)rgba & 15) == 0) {
+        mpi_check_range_f16_kernel<<<grid, 256, 0, st>>>(reinterpret_cast<const uint4*>(rgba), n_slabs, slab / 8, flags);
+    } else {
+        mpi_check_range_f16_scalar_kernel<<<grid, 256, 0, st>>>(reinterpret_cast<const unsigned short*>(rgba), n_slabs, slab, flags);
     }
     GMPI_CUDA_OK(cudaGetLastError());
     return GMPI_OK;
@@ -977,8 +1082,10 @@ static int host_render_locked(HostCache& c, const RenderParams& h, uint32_t* fla
     const size_t tex = (size_t)h.Ht * h.Wt, img = (size_t)H * W;
     const bool fac = h.alpha != nullptr, video = h.video_rgb != nullptr;
     // one slot = one MPI: expanded [N,4,tex], or factored rgb [3,tex] | bg [3,tex] | alpha [N,tex]
+    // (offsets in MPI elements: fp16 under GMPI_MPI_F16, else fp32)
+    const size_t esz = (h.options & GMPI_MPI_F16) ? 2 : 4;
     const size_t o_bg = 3 * tex, o_alpha = h.bg_rgb ? 6 * tex : 3 * tex;
-    const size_t mpi_bytes = sizeof(float) * (fac ? o_alpha + (size_t)N * tex : (size_t)N * 4 * tex);
+    const size_t mpi_bytes = esz * (fac ? o_alpha + (size_t)N * tex : (size_t)N * 4 * tex);
     auto up = [](size_t x) { return (x + 255) & ~(size_t)255; };
     const size_t o_dhw = 0, o_ray = o_dhw + up(sizeof(float) * (size_t)M * N * 3),
                  o_eye = o_ray + up(h.cam ? sizeof(float) * (size_t)V * 16 : sizeof(float) * (size_t)V * 3 * img),
@@ -1030,21 +1137,23 @@ static int host_render_locked(HostCache& c, const RenderParams& h, uint32_t* fla
         while (v1 < V && h.view2mpi[v1] == m) ++v1;
         if (v1 == v0) continue;
         if (used[slot]) GMPI_CUDA_OK(cudaStreamWaitEvent(s_copy, c.ev_free[slot], 0));
-        float* d_mpi = c.mpi[slot];
+        char* d_mpi = reinterpret_cast<char*>(c.mpi[slot]);
+        auto src = [esz](const float* base, size_t elems) { return reinterpret_cast<const char*>(base) + esz * elems; };
         if (fac) {
-            GMPI_CUDA_OK(cudaMemcpyAsync(d_mpi, h.rgb + (size_t)m * 3 * tex, sizeof(float) * 3 * tex, cudaMemcpyHostToDevice, s_copy));
+            GMPI_CUDA_OK(cudaMemcpyAsync(d_mpi, src(h.rgb, (size_t)m * 3 * tex), esz * 3 * tex, cudaMemcpyHostToDevice, s_copy));
             if (h.bg_rgb)
-                GMPI_CUDA_OK(cudaMemcpyAsync(d_mpi + o_bg, h.bg_rgb + (size_t)m * 3 * tex, sizeof(float) * 3 * tex, cudaMemcpyHostToDevice, s_copy));
-            GMPI_CUDA_OK(cudaMemcpyAsync(d_mpi + o_alpha, h.alpha + (size_t)m * N * tex, sizeof(float) * (size_t)N * tex, cudaMemcpyHostToDevice, s_copy));
+                GMPI_CUDA_OK(cudaMemcpyAsync(d_mpi + esz * o_bg, src(h.bg_rgb, (size_t)m * 3 * tex), esz * 3 * tex, cudaMemcpyHostToDevice, s_copy));
+            GMPI_CUDA_OK(cudaMemcpyAsync(d_mpi + esz * o_alpha, src(h.alpha, (size_t)m * N * tex), esz * (size_t)N * tex, cudaMemcpyHostToDevice, s_copy));
         } else {
-            GMPI_CUDA_OK(cudaMemcpyAsync(d_mpi, h.rgba + (size_t)m * N * 4 * tex, mpi_bytes, cudaMemcpyHostToDevice, s_copy));
+            GMPI_CUDA_OK(cudaMemcpyAsync(d_mpi, src(h.rgba, (size_t)m * N * 4 * tex), mpi_bytes, cudaMemcpyHostToDevice, s_copy));
         }
         GMPI_CUDA_OK(cudaEventRecord(c.ev_in[slot], s_copy));
         GMPI_CUDA_OK(cudaStreamWaitEvent(s_run, c.ev_in[slot], 0));
         RenderParams p = h;
         p.M = 1; p.V = v1 - v0;
-        if (fac) { p.rgb = d_mpi; p.bg_rgb = h.bg_rgb ? d_mpi + o_bg : nullptr; p.alpha = d_mpi + o_alpha; p.rgba = nullptr; }
-        else p.rgba = d_mpi;
+        const auto at = [d_mpi, esz](size_t elems) { return reinterpret_cast<const float*>(d_mpi + esz * elems); };
+        if (fac) { p.rgb = at(0); p.bg_rgb = h.bg_rgb ? at(o_bg) : nullptr; p.alpha = at(o_alpha); p.rgba = nullptr; }
+        else p.rgba = at(0);
         p.view2mpi = d_v2m; p.dhw = d_dhw + (size_t)m * N * 3;
         // mpi.py:70 compares every plane distance with the eye of the CALL's view 0, not of this launch's first view
         if (h.cam) { p.cam = d_ray + (size_t)v0 * 16; p.eye0 = d_ray + 13; p.ray_dir = p.eye = p.z_dir = nullptr; }
@@ -1110,6 +1219,7 @@ static int host_render(const RenderParams& h, uint32_t* flags_out, int device) {
 int gmpi_mpi_render_fwd_host(const float* rgba, const int32_t* view2mpi, const float* dhw, const float* ray_dir,
                              const float* eye, const float* z_dir, float* color, float* depth, uint32_t* flags_out,
                              int M, int V, int N, int Ht, int Wt, int H, int W, uint32_t options, int device) {
+    if (int rc = refuse_f16_classic(options)) return rc;
     RenderParams h = params_classic(rgba, view2mpi, dhw, ray_dir, eye, z_dir, M, V, N, Ht, Wt, H, W, options);
     h.color = color; h.depth = depth;
     return host_render(h, flags_out, device);

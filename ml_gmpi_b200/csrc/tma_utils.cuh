@@ -66,7 +66,7 @@ __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* map) {
 }
 
 // ---------------------------------------------------------------------------------------------------
-// host: tensor map over rgba viewed as [M*N*4 slabs][Ht][Wt] fp32, box {bw, bh, bc}
+// host: tensor map over rgba viewed as [M*N*4 slabs][Ht][Wt], box {bw, bh, bc}
 // ---------------------------------------------------------------------------------------------------
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -85,43 +85,50 @@ inline EncodeTiledFn get_encode_fn() {
     return fn;
 }
 
-// Returns 0 on success.  Requires Wt % 4 == 0 (16-byte row stride) and a 16-byte aligned base.
-inline int encode_slab_map(CUtensorMap* out, const float* base, uint64_t n_slabs, int Ht, int Wt, int bw, int bh, int bc) {
+// Element type of a tensor map: its CUtensorMapDataType and size in bytes (fp32, or the fp16 MPI of GMPI_MPI_F16).
+struct MapElem {
+    CUtensorMapDataType type;
+    cuuint64_t bytes;
+};
+constexpr MapElem kMapF32 = {CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4}, kMapF16 = {CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2};
+
+// Returns 0 on success.  Requires 16-byte row strides (Wt % 4 == 0 in fp32, Wt % 8 == 0 in fp16) and a 16-byte aligned base.
+inline int encode_slab_map(CUtensorMap* out, const void* base, MapElem el, uint64_t n_slabs, int Ht, int Wt, int bw, int bh, int bc) {
     EncodeTiledFn fn = get_encode_fn();
     if (!fn) return -1;
     cuuint64_t dims[3] = {(cuuint64_t)Wt, (cuuint64_t)Ht, (cuuint64_t)n_slabs};
-    cuuint64_t strides[2] = {(cuuint64_t)Wt * 4, (cuuint64_t)Wt * Ht * 4};
+    cuuint64_t strides[2] = {(cuuint64_t)Wt * el.bytes, (cuuint64_t)Wt * Ht * el.bytes};
     cuuint32_t box[3] = {(cuuint32_t)bw, (cuuint32_t)bh, (cuuint32_t)bc};
     cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, (void*)base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+    CUresult r = fn(out, el.type, 3, (void*)base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                     CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     return r == CUDA_SUCCESS ? 0 : (int)r;
 }
 
 // Tensor map over rgba [M*N planes][4 ch][Ht][Wt] with the dimensions ordered (x, channel, y, plane) so that a box
 // {bw, 4, rows, 1} lands in shared memory as [row][channel][x]: rows stay linear however many row-chunks are issued.
-inline int encode_plane_map(CUtensorMap* out, const float* base, uint64_t n_planes, int Ht, int Wt, int bw, int rows) {
+inline int encode_plane_map(CUtensorMap* out, const void* base, MapElem el, uint64_t n_planes, int Ht, int Wt, int bw, int rows) {
     EncodeTiledFn fn = get_encode_fn();
     if (!fn) return -1;
     cuuint64_t dims[4] = {(cuuint64_t)Wt, 4, (cuuint64_t)Ht, (cuuint64_t)n_planes};
-    cuuint64_t strides[3] = {(cuuint64_t)Wt * Ht * 4, (cuuint64_t)Wt * 4, (cuuint64_t)Wt * Ht * 16};
+    cuuint64_t strides[3] = {(cuuint64_t)Wt * Ht * el.bytes, (cuuint64_t)Wt * el.bytes, (cuuint64_t)Wt * Ht * 4 * el.bytes};
     cuuint32_t box[4] = {(cuuint32_t)bw, 4, (cuuint32_t)rows, 1};
     cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void*)base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+    CUresult r = fn(out, el.type, 4, (void*)base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                     CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     return r == CUDA_SUCCESS ? 0 : (int)r;
 }
 
 // Tensor map over a shared colour image rgb [M][3 ch][Ht][Wt] (factored MPI) with the dimensions ordered (x, channel, y, mpi):
 // a box {bw, 3, rows, 1} lands in shared memory as [row][channel][x].
-inline int encode_color_map(CUtensorMap* out, const float* base, uint64_t n_mpi, int Ht, int Wt, int bw, int rows) {
+inline int encode_color_map(CUtensorMap* out, const void* base, MapElem el, uint64_t n_mpi, int Ht, int Wt, int bw, int rows) {
     EncodeTiledFn fn = get_encode_fn();
     if (!fn) return -1;
     cuuint64_t dims[4] = {(cuuint64_t)Wt, 3, (cuuint64_t)Ht, (cuuint64_t)n_mpi};
-    cuuint64_t strides[3] = {(cuuint64_t)Wt * Ht * 4, (cuuint64_t)Wt * 4, (cuuint64_t)Wt * Ht * 12};
+    cuuint64_t strides[3] = {(cuuint64_t)Wt * Ht * el.bytes, (cuuint64_t)Wt * el.bytes, (cuuint64_t)Wt * Ht * 3 * el.bytes};
     cuuint32_t box[4] = {(cuuint32_t)bw, 3, (cuuint32_t)rows, 1};
     cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void*)base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+    CUresult r = fn(out, el.type, 4, (void*)base, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                     CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     return r == CUDA_SUCCESS ? 0 : (int)r;
 }

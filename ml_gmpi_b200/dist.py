@@ -104,18 +104,25 @@ class FrameGather:
 
     def render(self, rgba, dhw, view2mpi, ray_dir, eye, z_dir, flags, *, align_corners=True, check_last_plane=False,
                color_minus1_1=False, early_stop=None):
-        """early_stop: early ray termination threshold in [0, 1), as in render_frames (None: off)."""
+        """early_stop: early ray termination threshold in [0, 1), as in render_frames (None: off).  An fp16 rgba renders natively
+        where render_frames would (GMPI_MPI_F16), else from its fp32 upcast."""
         import ctypes
         from . import _lib
-        from .mpi import _options
+        from .mpi import _half_mpi, _options
         lib = _lib.load()
         M, N, _, Ht, Wt = rgba.shape
         V = ray_dir.shape[0]
         assert V <= self.frames_per_rank and ray_dir.shape[2:] == (self.H, self.W)
-        for name, t in (("rgba", rgba), ("dhw", dhw), ("ray_dir", ray_dir), ("eye", eye), ("z_dir", z_dir)):   # raw pointers below
-            assert t.is_cuda and t.dtype == torch.float32 and t.is_contiguous(), f"{name} must be a contiguous fp32 CUDA tensor"
-        assert view2mpi.dtype == torch.int32 and view2mpi.is_contiguous() and flags.dtype == torch.int32
         options = _options(align_corners, check_last_plane, color_minus1_1, early_stop=early_stop)
+        if rgba.dtype == torch.float16:
+            half = _half_mpi([rgba, None, None, None], V, self.H, self.W, options)
+            rgba, options = (half[0], options | _lib.OPT_MPI_F16) if half is not None else (rgba.float().contiguous(), options)
+        mpi_dtype = torch.float16 if options & _lib.OPT_MPI_F16 else torch.float32
+        f32 = torch.float32
+        for name, t, dtype in (("rgba", rgba, mpi_dtype), ("dhw", dhw, f32), ("ray_dir", ray_dir, f32), ("eye", eye, f32),
+                               ("z_dir", z_dir, f32)):   # raw pointers below
+            assert t.is_cuda and t.dtype == dtype and t.is_contiguous(), f"{name} must be a contiguous {dtype} CUDA tensor"
+        assert view2mpi.dtype == torch.int32 and view2mpi.is_contiguous() and flags.dtype == torch.int32
         with torch.cuda.device(rgba.device):
             d = _lib.make_desc(options=options, M=M, V=V, N=N, Ht=Ht, Wt=Wt, H=self.H, W=self.W, rgba=rgba, view2mpi=view2mpi, dhw=dhw,
                                ray_dir=ray_dir, eye=eye, z_dir=z_dir, peer_frames=self._peer_ptrs[self._next],

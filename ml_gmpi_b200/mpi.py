@@ -98,6 +98,29 @@ class _RenderFn(torch.autograd.Function):
         return (g_rgba, g_rgb, g_alpha, g_bg) + (None,) * 9
 
 
+def _half_mpi(mpi, V, H, W, options):
+    """The MPI tensors `mpi` = [rgba, rgb, alpha, bg_rgb] (None where absent) as contiguous fp16 when the call renders them natively
+    (GMPI_MPI_F16), else None (the call upcasts them to fp32, as it always did).  Native when every MPI tensor is torch.float16,
+    autograd does not record for them (the backward is fp32), and the fp16 MPI gets the kernel plan its fp32 upcast would get (the
+    staged kernels need Wt % 8 == 0 and 16-byte aligned bases in fp16): the output is then bitwise the upcast's."""
+    ts = [t for t in mpi if t is not None]
+    if not all(t.dtype == torch.float16 for t in ts):
+        return None
+    if torch.is_grad_enabled() and any(t.requires_grad for t in ts):
+        return None
+    # detached: under no_grad an fp16 tensor may still carry requires_grad, and the native path has no backward
+    half = [None if t is None else t.detach().contiguous() for t in mpi]
+    rgba, rgb, alpha, bg_rgb = half
+    ref = alpha if rgba is None else rgba
+    lib = _lib.load()
+    sizes = dict(M=ref.shape[0], V=V, N=ref.shape[1], Ht=ref.shape[-2], Wt=ref.shape[-1], H=H, W=W)
+    plans = []
+    for opt, ptrs in ((options, {}), (options | _lib.OPT_MPI_F16, dict(rgba=rgba, rgb=rgb, alpha=alpha, bg_rgb=bg_rgb))):
+        d = _lib.make_desc(options=opt, **sizes, **ptrs)
+        plans.append(lib.gmpi_mpi_render_fwd_plan_ex(ctypes.byref(d), None))
+    return half if plans[0] == plans[1] else None
+
+
 _warned_direct = set()
 
 
@@ -142,10 +165,16 @@ def render_views(rgba, dhw, view2mpi, ray_dir, eye, z_dir, *, align_corners=True
         raise RuntimeError("ml_gmpi_b200 renders on CUDA devices only (no CPU fallback); got a CPU tensor")
     if flags is None:
         flags = torch.zeros(1, dtype=torch.int32, device=rgba.device)
-    _warn_if_direct(rgba, ray_dir.shape[0], ray_dir.shape[2], ray_dir.shape[3])
-    return _RenderFn.apply(_as_f32c(rgba), None, None, None, _as_f32c(dhw), view2mpi, _as_f32c(ray_dir), _as_f32c(eye), _as_f32c(z_dir),
-                           _options(align_corners, check_last_plane, color_minus1_1, early_stop=early_stop), flags, int(view_group),
-                           early_stop)
+    V, _, H, W = ray_dir.shape
+    _warn_if_direct(rgba, V, H, W)
+    options = _options(align_corners, check_last_plane, color_minus1_1, early_stop=early_stop)
+    half = _half_mpi([rgba, None, None, None], V, H, W, options)
+    if half is not None:
+        rgba, options = half[0], options | _lib.OPT_MPI_F16
+    else:
+        rgba = _as_f32c(rgba)
+    return _RenderFn.apply(rgba, None, None, None, _as_f32c(dhw), view2mpi, _as_f32c(ray_dir), _as_f32c(eye), _as_f32c(z_dir),
+                           options, flags, int(view_group), early_stop)
 
 
 def render_views_factored(rgb, alpha, dhw, view2mpi, ray_dir, eye, z_dir, *, bg_rgb=None, align_corners=True,
@@ -164,11 +193,17 @@ def render_views_factored(rgb, alpha, dhw, view2mpi, ray_dir, eye, z_dir, *, bg_
     assert bg_rgb is None or bg_rgb.shape == rgb.shape, f"bg_rgb must have rgb's shape, got {bg_rgb.shape}"
     if flags is None:
         flags = torch.zeros(1, dtype=torch.int32, device=alpha.device)
-    _warn_if_direct(alpha, ray_dir.shape[0], ray_dir.shape[2], ray_dir.shape[3])
-    return _RenderFn.apply(None, _as_f32c(rgb), _as_f32c(alpha), None if bg_rgb is None else _as_f32c(bg_rgb), _as_f32c(dhw), view2mpi,
-                           _as_f32c(ray_dir), _as_f32c(eye), _as_f32c(z_dir),
-                           _options(align_corners, check_last_plane, color_minus1_1, early_stop=early_stop), flags, int(view_group),
-                           early_stop)
+    V, _, H, W = ray_dir.shape
+    _warn_if_direct(alpha, V, H, W)
+    options = _options(align_corners, check_last_plane, color_minus1_1, early_stop=early_stop)
+    half = _half_mpi([None, rgb, alpha, bg_rgb], V, H, W, options)
+    if half is not None:
+        _, rgb, alpha, bg_rgb = half
+        options |= _lib.OPT_MPI_F16
+    else:
+        rgb, alpha, bg_rgb = _as_f32c(rgb), _as_f32c(alpha), None if bg_rgb is None else _as_f32c(bg_rgb)
+    return _RenderFn.apply(None, rgb, alpha, bg_rgb, _as_f32c(dhw), view2mpi, _as_f32c(ray_dir), _as_f32c(eye), _as_f32c(z_dir),
+                           options, flags, int(view_group), early_stop)
 
 
 def expand_factored(rgb, alpha, bg_rgb=None):
@@ -219,9 +254,13 @@ def render_frames(*, dhw, view2mpi, rgba=None, rgb=None, alpha=None, bg_rgb=None
     else:
         color = torch.empty((V, 3, H, W), device=dev, dtype=torch.float32)
         depth = torch.empty((V, 1, H, W), device=dev, dtype=torch.float32)
-    keep = [_as_f32c(t) if t is not None else None for t in (rgba, rgb, alpha, bg_rgb, dhw)]
+    options = _options(align_corners, check_last_plane, True, u8_round, early_stop)
+    half = _half_mpi([rgba, rgb, alpha, bg_rgb], V, H, W, options)
+    if half is not None:
+        options |= _lib.OPT_MPI_F16
+    keep = (half if half is not None else [_as_f32c(t) if t is not None else None for t in (rgba, rgb, alpha, bg_rgb)]) + [_as_f32c(dhw)]
     with torch.cuda.device(dev):
-        d = _lib.make_desc(options=_options(align_corners, check_last_plane, True, u8_round, early_stop), M=M, V=V, N=N, Ht=Ht, Wt=Wt, H=H, W=W,
+        d = _lib.make_desc(options=options, M=M, V=V, N=N, Ht=Ht, Wt=Wt, H=H, W=W,
                            view_group=int(view_group), depth_near=near, depth_range=rng, rgba=keep[0], rgb=keep[1], alpha=keep[2],
                            bg_rgb=keep[3], view2mpi=view2mpi, dhw=keep[4], ray_dir=ray_dir, eye=eye, z_dir=z_dir, cam=cam, color=color,
                            depth=depth, video_rgb=v_rgb, video_depth=v_depth, flags=flags, stream=_stream_ptr(dev), early_stop=early_stop)
@@ -230,11 +269,13 @@ def render_frames(*, dhw, view2mpi, rgba=None, rgb=None, alpha=None, bg_rgb=None
 
 
 def check_range(rgba: torch.Tensor, flags: torch.Tensor) -> None:
-    """One streaming pass: RGBA/alpha in [0,1] (mpi_renderer.py:447-449, mpi.py:185-187) -> flag bits."""
+    """One streaming pass: RGBA/alpha in [0,1] (mpi_renderer.py:447-449, mpi.py:185-187) -> flag bits.  rgba is contiguous fp32, or
+    contiguous fp16 (the flags of the fp32 check on its upcast)."""
     lib = _lib.load()
     M, N, _, Ht, Wt = rgba.shape
+    check = lib.gmpi_mpi_check_range_f16 if rgba.dtype == torch.float16 else lib.gmpi_mpi_check_range
     with torch.cuda.device(rgba.device):
-        _lib.check(lib.gmpi_mpi_check_range(rgba.data_ptr(), M, N, Ht, Wt, flags.data_ptr(), _stream_ptr(rgba.device)))
+        _lib.check(check(rgba.data_ptr(), M, N, Ht, Wt, flags.data_ptr(), _stream_ptr(rgba.device)))
 
 
 class MPI(nn.Module):
@@ -309,7 +350,8 @@ class MPI(nn.Module):
             raise RuntimeError("ml_gmpi_b200.MPI renders on CUDA devices only (no CPU fallback); got a CPU tensor")
         dev = batch_rgba.device
         view2mpi, ray_dir, eye, z_dir = self.pack_views(batch_ray_dir, batch_eye_pos, batch_z_dir, dev)
-        rgba = _as_f32c(batch_rgba)
+        # an fp16 MPI stays fp16: render_views renders it natively where it can (and upcasts it where it cannot)
+        rgba = batch_rgba.contiguous() if batch_rgba.dtype == torch.float16 else _as_f32c(batch_rgba)
         flags = torch.zeros(1, dtype=torch.int32, device=dev)
         if self.validate == "full":
             check_range(rgba.detach(), flags)
