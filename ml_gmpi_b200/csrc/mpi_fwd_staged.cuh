@@ -35,7 +35,8 @@ constexpr int kMaxPlanesStaged = 512;   // plane-constant table: 32 B per plane 
 constexpr int kStageFloats = kMaxBW * kMaxBH * 4;
 // Factored forward: box widths 64 and 96 only.  Its boxes are [row][3][bw] (colour) and [row][bw] (alpha): row pitches of 3 bw and
 // bw words, and only a pitch that is a multiple of the 32 banks keeps a warp whose 32 taps straddle two texture rows (any rotated
-// view) at one wavefront per LDS -- the expanded box [row][4][bw] has that for every bw % 8 == 0.
+// view) at one wavefront per LDS -- the expanded box [row][4][bw] has that for every bw % 8 == 0.  The 96-wide box holds footprints
+// 65..kMaxBW texels wide: wider ones take the generic body, as in the expanded ring (see staged_producer).
 constexpr int kWideBW = 96;
 constexpr int kWideStageFloats = kWideBW * kMaxBH * 4;
 constexpr size_t kStagedSmemWide = (size_t)kStages * kWideStageFloats * 4 + (size_t)kMaxPlanesStaged * 32;
@@ -452,8 +453,11 @@ __device__ __forceinline__ void staged_producer(const RenderParams& p, const Tma
             const int need_w = xmax - bx0 + 3, need_h = ymax - ymin + 4;      // +1 east/south tap, +-1 slack
             int mode = 0;
             constexpr bool kWide = kFact && Ring::kWideFact;
-            constexpr int kBoxMaxW = kWide ? kWideBW : kMaxBW;
-            if (!all_finite || need_w > kBoxMaxW || ((need_h + kRowsPerOp - 1) / kRowsPerOp) * kRowsPerOp > kMaxBH) mode = 2;   // would not fit a ring stage
+            // Footprints wider than kMaxBW take the generic body in every ring, the factored forward's 96-wide boxes included: the fast
+            // body forms its bilinear weights as w10 = wy1 - wx1 wy1 (FMAs), the generic body as (1 - wx1) wy1, which differ in the
+            // last bit, so a footprint 89..96 texels wide staged here but not in the expanded ring would break the factored render's
+            // bitwise equality with the expanded one.
+            if (!all_finite || need_w > kMaxBW || ((need_h + kRowsPerOp - 1) / kRowsPerOp) * kRowsPerOp > kMaxBH) mode = 2;   // would not fit a ring stage
             else if (bx0 > Wt - 1 || bx0 + need_w - 1 < 0 || by0 > Ht - 1 || by0 + need_h - 1 < 0) mode = 1;
             // width class k (tensor-map slot, one-hot bit 16 + k of the header); wide rings: slot 1 = 64, slot 4 = kWideBW
             const int k = mode != 0 ? 0 : kWide ? (need_w <= 64 ? 1 : 4) : max(0, (need_w - kMinBW + kBWStep - 1) / kBWStep);

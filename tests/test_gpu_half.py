@@ -333,7 +333,8 @@ def _limit_footprints(c, lo, hi):
 @pytest.mark.parametrize("stages", ["staged2", "staged3"])
 @pytest.mark.parametrize("factored", [False, True])
 def test_fp16_at_the_widest_box_classes(factored, stages):
-    """Footprints at the widest class (expanded: width need 85..88, class 88; factored: 93..96, class 96) whose fp16 box starts 4
+    """Footprints at the widest class (width need 85..88: class 88 expanded, class 96 factored; the factored case also has footprints
+    93..96, which take the generic body) whose fp16 box starts 4
     texels west of the fp32 one: the fp16 kernel stages a wider box and decides fast / generic body exactly as fp32 does, so the
     render stays bitwise the upcast's."""
     c = _limit_case(factored)
