@@ -73,7 +73,9 @@ mpi_alpha_depth_bwd_kernel(AlphaView a, const float* __restrict__ plane_d, const
     }
 }
 
-__device__ __forceinline__ float clip01(float x) { return fminf(fmaxf(x, 0.0f), 1.0f); }
+// torch.clip(x, 0, 1): a NaN stays NaN (fmaxf alone returns 0 for it, which would hide a diverging colour in the shaded MPI);
+// every other value takes the same fminf(fmaxf) as torch's clamp, so the result is bit for bit torch's.
+__device__ __forceinline__ float clip01(float x) { return isnan(x) ? x : fminf(fmaxf(x, 0.0f), 1.0f); }
 
 // out[m,i,c] = clip(rgba[m,i,c] * shade[m], 0, 1) for c < 3, out[m,i,3] = rgba[m,i,3]   (light_renderer.py:190-199)
 // grid: (tex4 blocks, N, M); one thread = four texels of one plane, all four channels.

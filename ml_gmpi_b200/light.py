@@ -10,6 +10,8 @@ ka/kd growth.  What moves to CUDA (csrc/mpi_light.cuh, through the C ABI):
 The Gaussian blur, the point cloud, the normals and the Lambertian term act on [B,H,W] images (1/N of the MPI) and stay
 torch ops -- plumbing on small tensors.  With the generator's FACTORED output the shading step is a [B,3,H,W] product:
 `shade_factored` returns the shaded colour image and the renderer consumes (rgb, alpha) directly (render_views_factored).
+Both kernels stream four texels per thread; a texture whose Ht*Wt is not a multiple of 4 takes the reference's fp32 torch
+expressions instead (the C ABI refuses such sizes).
 
 No CPU path: tensors must live on a CUDA device.
 """
@@ -29,6 +31,13 @@ def _stream_ptr(device):
     return torch.cuda.current_stream(device).cuda_stream
 
 
+def _streamable(t: torch.Tensor) -> torch.Tensor:
+    """t as a contiguous fp32 tensor whose base is 16-byte aligned, as the float4 kernels read it: t itself when it already is,
+    else a copy (a contiguous view that starts mid-allocation, e.g. one float in, is copied too)."""
+    t = t.float().contiguous()
+    return t if t.data_ptr() % 16 == 0 else t.clone()
+
+
 def _alpha_view(mpi_alpha: torch.Tensor):
     """(tensor to keep alive, base pointer, mpi_stride, plane_stride) of an alpha stack [B,N,1,H,W]: a contiguous tensor, or the
     channel-3 view of a contiguous [B,N,4,H,W] stack (no copy)."""
@@ -37,18 +46,18 @@ def _alpha_view(mpi_alpha: torch.Tensor):
     if mpi_alpha.dtype == torch.float32 and st[-1] == 1 and st[-2] == W and st[1] % 4 == 0 and st[0] % 4 == 0 and \
             mpi_alpha.data_ptr() % 16 == 0 and (H * W) % 4 == 0:
         return mpi_alpha, mpi_alpha.data_ptr(), st[0], st[1]
-    c = mpi_alpha.float().contiguous()
+    c = _streamable(mpi_alpha)
     return c, c.data_ptr(), N * H * W, H * W
 
 
 class _AlphaDepthFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, mpi_alpha, plane_ds):
+    def forward(ctx, mpi_alpha, plane_ds, save_t):
         lib = _lib.load()
         B, N, _, H, W = mpi_alpha.shape
         keep, ptr, ms, ps = _alpha_view(mpi_alpha)
         depth = torch.empty((B, 1, H, W), device=mpi_alpha.device, dtype=torch.float32)
-        trans = torch.empty((B, N, H, W), device=mpi_alpha.device, dtype=torch.float32) if ctx.needs_input_grad[0] else None
+        trans = torch.empty((B, N, H, W), device=mpi_alpha.device, dtype=torch.float32) if save_t else None
         with torch.cuda.device(mpi_alpha.device):
             _lib.check(lib.gmpi_mpi_alpha_depth_fwd(ptr, ms, ps, plane_ds.data_ptr(), depth.data_ptr(),
                                                     None if trans is None else trans.data_ptr(), B, N, H, W,
@@ -62,7 +71,7 @@ class _AlphaDepthFn(torch.autograd.Function):
     def backward(ctx, g_depth):
         keep, plane_ds, trans = ctx.saved_tensors
         if trans is None:
-            return None, None
+            return None, None, None
         lib = _lib.load()
         B, N, H, W = trans.shape
         ms, ps = ctx.view
@@ -72,7 +81,7 @@ class _AlphaDepthFn(torch.autograd.Function):
             _lib.check(lib.gmpi_mpi_alpha_depth_bwd(keep.data_ptr() if keep.is_contiguous() else keep.data_ptr(), ms, ps,
                                                     plane_ds.data_ptr(), trans.data_ptr(), g.data_ptr(), g_alpha.data_ptr(),
                                                     N * H * W, H * W, B, N, H, W, _stream_ptr(trans.device)))
-        return g_alpha, None
+        return g_alpha, None, None
 
 
 class _ApplyShadingFn(torch.autograd.Function):
@@ -105,8 +114,16 @@ def alpha_depth(mpi_alpha: torch.Tensor, plane_ds: torch.Tensor) -> torch.Tensor
     if not mpi_alpha.is_cuda:
         raise RuntimeError("ml_gmpi_b200 runs on CUDA devices only (no CPU fallback); got a CPU tensor")
     pd = plane_ds.reshape(-1).to(device=mpi_alpha.device, dtype=torch.float32).contiguous()
-    assert pd.numel() == mpi_alpha.shape[1], f"{mpi_alpha.shape}, {plane_ds.shape}"
-    return _AlphaDepthFn.apply(mpi_alpha, pd)
+    B, N, _, H, W = mpi_alpha.shape
+    assert pd.numel() == N, f"{mpi_alpha.shape}, {plane_ds.shape}"
+    if (H * W) % 4:
+        # the kernel streams four texels per thread; other texel counts take the reference's fp32 expression and its autograd
+        a = mpi_alpha.float()[:, :, 0]
+        s = (1.0 - a) + 1e-10
+        trans = torch.cumprod(torch.cat((torch.ones_like(s[:, :1]), s[:, :-1]), dim=1), dim=1)
+        return (a * trans * pd.view(1, N, 1, 1)).sum(1, keepdim=True)
+    # T (4 B per texel-plane) is only needed by a backward, and grad mode is always off inside Function.forward: decide here
+    return _AlphaDepthFn.apply(mpi_alpha, pd, torch.is_grad_enabled() and mpi_alpha.requires_grad)
 
 
 def apply_shading(batch_mpi: torch.Tensor, shading: torch.Tensor) -> torch.Tensor:
@@ -114,8 +131,13 @@ def apply_shading(batch_mpi: torch.Tensor, shading: torch.Tensor) -> torch.Tenso
     if not batch_mpi.is_cuda:
         raise RuntimeError("ml_gmpi_b200 runs on CUDA devices only (no CPU fallback); got a CPU tensor")
     B, N, C, H, W = batch_mpi.shape
-    assert C == 4 and (H * W) % 4 == 0, f"{batch_mpi.shape}"
-    return _ApplyShadingFn.apply(batch_mpi.float().contiguous(), shading.reshape(B, 1, H, W).float().contiguous())
+    assert C == 4, f"{batch_mpi.shape}"
+    if (H * W) % 4:
+        # as in alpha_depth: texel counts the float4 kernel cannot stream take the reference's fp32 expression.  split (not two
+        # slices) so that d rgb is g * shade as the kernel writes it: slices would add a zero-filled alpha gradient, turning -0 into +0
+        rgb, alpha = batch_mpi.float().split((3, 1), dim=2)
+        return torch.cat((torch.clip(rgb * shading.reshape(B, 1, 1, H, W).float(), min=0.0, max=1.0), alpha), dim=2)
+    return _ApplyShadingFn.apply(_streamable(batch_mpi), _streamable(shading.reshape(B, 1, H, W)))
 
 
 def gaussian_blur(img: torch.Tensor, ksize: int, sigma: float) -> torch.Tensor:

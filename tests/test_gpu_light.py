@@ -77,6 +77,26 @@ def test_factored_shading_equals_shading_the_expanded_stack():
         assert rel_err(shaded_rgb.cpu().numpy(), full[:, i, :3].cpu().numpy()) <= 1e-6
 
 
+def test_factored_and_expanded_shading_keep_nan_at_the_same_texels():
+    """A NaN colour (a diverging generator) stays NaN through the fused shading, as it does through shade_factored's torch.clip:
+    the two paths agree on where the NaNs are and on every other value."""
+    gd = load_golden("light_2x6x32")
+    d = dev()
+    t = lambda a: torch.from_numpy(a).to(d)
+    rgb, alpha = t(gd["mpi"][:, 0, :3]).contiguous(), t(gd["mpi"][:, :, 3:]).contiguous()
+    rgb[0, 1, 3, 5] = float("nan")
+    rgb[1, :, 10, 20] = float("nan")
+    rgb[1, 2, 0, 0] = float("inf")
+    kw = dict(given_yaws=torch.from_numpy(gd["light_yaws"]).reshape(-1, 1), given_pitches=torch.from_numpy(gd["light_pitches"]).reshape(-1, 1))
+    shaded_rgb = make_lr().shade_factored(rgb, alpha, t(gd["dhw"]), t(gd["xyz"]), **kw)
+    full = make_lr().render(expand_factored(rgb, alpha), t(gd["dhw"]), t(gd["xyz"]), **kw)
+    nan = torch.isnan(shaded_rgb)
+    assert int(nan.sum()) == 4
+    for i in range(alpha.shape[1]):
+        assert torch.equal(torch.isnan(full[:, i, :3]), nan)
+        assert rel_err(shaded_rgb[~nan].cpu().numpy(), full[:, i, :3][~nan].cpu().numpy()) <= 1e-6
+
+
 def test_apply_shading_full_size_stream():
     """One 32-plane 512^2 batch: the fused pass equals the three torch ops it replaces, bit for bit."""
     d = dev()
