@@ -107,6 +107,9 @@ int gmpi_mpi_render_fwd(const float* rgba, const int32_t* view2mpi, const float*
  * one per rank, peer-mapped over NVLink (e.g. torch symmetric memory, cudaIpc).  The stores are posted writes that overlap
  * the remaining compute; the caller makes them visible with a barrier across ranks after the kernel.  Replaces the
  * render + ncclAllGather pair; the reference has no counterpart (its renderer is single-GPU, gloo barriers only).
+ * Preconditions the library cannot check, because the pointer array is in device memory:
+ *   - every peer_frames[r] base is 16-byte aligned (the epilogue stores float4s when W % 4 == 0);
+ *   - every buffer holds F >= frame_offset + V frames.
  */
 int gmpi_mpi_render_fwd_gather(const float* rgba, const int32_t* view2mpi, const float* dhw,
                                const float* ray_dir, const float* eye, const float* z_dir,

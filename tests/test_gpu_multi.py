@@ -24,29 +24,30 @@ def _worker(rank, world, port, q):
     try:
         import ml_gmpi_b200 as g
         from ml_gmpi_b200 import synth, dist as gdist
-        B, N, R = 3, 12, 128
-        case = synth.make_case(n_planes=N, tex=R, img=R, n_mpi=B, seed=100 + rank, device=dev)
         flags = torch.zeros(1, dtype=torch.int32, device=dev)
-        color, depth = g.render_views(case.rgba, case.dhw, case.view2mpi, case.ray_dir, case.eye, case.z_dir, color_minus1_1=True)
-        ref = gdist.all_gather_frames(gdist.pack_frames(color, depth))              # NCCL path
-        # NVLS multicast variant (one store per quad, the switch replicates), when the fabric has it
-        mc_ok = None
-        try:
-            fgm = gdist.FrameGather(B, R, R, dev, multicast=True)
-        except RuntimeError:
-            fgm = None
-        if fgm is not None:
-            fgm.render(case.rgba, case.dhw, case.view2mpi, case.ray_dir, case.eye, case.z_dir, flags, color_minus1_1=True)
-            fgm.finish()
+        ok, maxdiff, mc_ok = True, 0.0, None
+        # 3 views of 128^2 (30 tiles of 64x30: the direct kernel) and 4 views of 256^2 (144 tiles: the staged kernel)
+        for B, N, R in ((4, 12, 256), (3, 12, 128)):
+            case = synth.make_case(n_planes=N, tex=R, img=R, n_mpi=B, seed=100 + rank, device=dev)
+            color, depth = g.render_views(case.rgba, case.dhw, case.view2mpi, case.ray_dir, case.eye, case.z_dir, color_minus1_1=True)
+            ref = gdist.all_gather_frames(gdist.pack_frames(color, depth))          # NCCL path
+            # NVLS multicast variant (one store per quad, the switch replicates), when the fabric has it
+            try:
+                fgm = gdist.FrameGather(B, R, R, dev, multicast=True)
+            except RuntimeError:
+                fgm = None
+            if fgm is not None:
+                fgm.render(case.rgba, case.dhw, case.view2mpi, case.ray_dir, case.eye, case.z_dir, flags, color_minus1_1=True)
+                fgm.finish()
+                torch.cuda.synchronize(dev)
+                mc_ok = bool(torch.equal(fgm.frames, ref)) and mc_ok is not False
+            fg = gdist.FrameGather(B, R, R, dev, multicast=False)
+            for _ in range(2):                                                      # twice: buffers are reused
+                fg.render(case.rgba, case.dhw, case.view2mpi, case.ray_dir, case.eye, case.z_dir, flags, color_minus1_1=True)
+                fg.finish()
             torch.cuda.synchronize(dev)
-            mc_ok = bool(torch.equal(fgm.frames, ref))
-        fg = gdist.FrameGather(B, R, R, dev, multicast=False)
-        for _ in range(2):                                                          # twice: buffers are reused
-            fg.render(case.rgba, case.dhw, case.view2mpi, case.ray_dir, case.eye, case.z_dir, flags, color_minus1_1=True)
-            fg.finish()
-        torch.cuda.synchronize(dev)
-        ok = bool(torch.equal(fg.frames, ref))
-        maxdiff = float((fg.frames - ref).abs().max())
+            ok = ok and bool(torch.equal(fg.frames, ref))
+            maxdiff = max(maxdiff, float((fg.frames - ref).abs().max()))
         # write-after-read across iterations (ADVICE r1): DIFFERENT data every step, ranks deliberately skewed, and a reader
         # of step k's frames still in flight on the render stream while the peers already run step k+1
         cases = [case, synth.make_case(n_planes=N, tex=R, img=R, n_mpi=B, seed=500 + rank, device=dev)]
