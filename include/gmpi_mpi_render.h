@@ -70,18 +70,23 @@ const char* gmpi_last_error(void);
 const char* gmpi_mpi_render_fwd_variant(int N, int Ht, int Wt, int H, int W);
 
 /*
- * Which forward/backward kernels a call with these shapes launches: GMPI_PLAN_STAGED (persistent TMA-staged kernels, the fast
- * path) or GMPI_PLAN_DIRECT (one thread per pixel, any shape, several times slower).  *why (nullable) receives the GMPI_WHY_*
- * bits of every reason the staged path is not taken, so a caller can surface the performance cliff instead of finding it in a
- * profile.  rgba may be NULL (alignment unknown: not checked).
+ * Which FORWARD kernels a call with these shapes launches, for one fp32 MPI rgba [1,N,4,Ht,Wt]: GMPI_PLAN_STAGED (persistent
+ * TMA-staged kernels, the fast path) or GMPI_PLAN_DIRECT (one thread per pixel, any shape, several times slower).  *why (nullable)
+ * receives the GMPI_WHY_* bits of every reason the staged path is not taken, so a caller can surface the performance cliff
+ * instead of finding it in a profile.  rgba may be NULL (alignment unknown: not checked).  gmpi_mpi_render_fwd_plan_ex answers
+ * for a whole descriptor (M MPIs, factored, fp16).  The early-stop and training forwards get the same plan as the plain one.  The
+ * plan assumes the MPI's tensor maps encode; if cuTensorMapEncodeTiled refuses them, the forward takes the direct kernels (or
+ * fails, under gmpi_debug_set_fwd_variant(2)).  The
+ * backward has conditions of its own (gmpi_mpi_render_bwd_saved).
  */
 #define GMPI_PLAN_DIRECT 1
 #define GMPI_PLAN_STAGED 2
-#define GMPI_WHY_TEX_WIDTH 1u    /* Wt % 4 != 0: rows are not 16-byte multiples, no tensor map                     */
+#define GMPI_WHY_TEX_WIDTH 1u    /* Wt % 4 != 0 (fp16: Wt % 8): rows are not 16-byte multiples, no tensor map         */
 #define GMPI_WHY_FEW_TILES 2u    /* fewer than 120 tiles of 64x30 pixels over all views: the persistent grid would idle */
-#define GMPI_WHY_MANY_PLANES 4u  /* N > 512: the per-view plane-constant table does not fit next to the ring        */
-#define GMPI_WHY_ALIGNMENT 8u    /* rgba base not 16-byte aligned                                                   */
-#define GMPI_WHY_FORCED 16u      /* gmpi_debug_set_fwd_variant(1)                                                    */
+#define GMPI_WHY_MANY_PLANES 4u  /* N > 512: the per-view plane-constant table does not fit next to the ring, or
+                                    M*N >= 2^31 planes over all MPIs                                                    */
+#define GMPI_WHY_ALIGNMENT 8u    /* an MPI base (rgba, rgb, alpha or bg_rgb) not 16-byte aligned                        */
+#define GMPI_WHY_FORCED 16u      /* gmpi_debug_set_fwd_variant(1)                                                        */
 int gmpi_mpi_render_fwd_plan(int V, int N, int Ht, int Wt, int H, int W, const void* rgba, uint32_t* why);
 
 /*
@@ -134,7 +139,10 @@ int gmpi_mpi_render_bwd(const float* rgba, const int32_t* view2mpi, const float*
  * Training pair.  gmpi_mpi_render_fwd_train = gmpi_mpi_render_fwd that additionally saves the transmittance in front of
  * every plane, transmittance [V,N,H,W] (T_i = prod_{j<i}(1 - alpha_j), mpi.py:421-423) -- what torch autograd keeps alive as
  * `weights`/`cumprod` tensors, here 4 bytes per (pixel, plane).  gmpi_mpi_render_bwd_saved consumes it: one staged
- * back-to-front sweep instead of the two-pass kernel (falls back to gmpi_mpi_render_bwd for shapes the staged path skips).
+ * back-to-front sweep instead of the two-pass kernel.  That staged box backward runs when the forward plan of the same call is
+ * GMPI_PLAN_STAGED (gmpi_mpi_render_fwd_plan) and also W % 4 == 0, V*N < 2^31 and the gradient and transmittance bases are
+ * 16-byte aligned; otherwise the call runs gmpi_mpi_render_bwd's two-pass kernel.  The same holds for gmpi_mpi_render_bwd_ex with
+ * a transmittance (its plan: gmpi_mpi_render_fwd_plan_ex).
  */
 int gmpi_mpi_render_fwd_train(const float* rgba, const int32_t* view2mpi, const float* dhw,
                               const float* ray_dir, const float* eye, const float* z_dir,
@@ -246,9 +254,10 @@ typedef struct gmpi_render_desc {
 int gmpi_mpi_zero_async(void* ptr, size_t bytes, void* stream);
 
 int gmpi_mpi_render_fwd_ex(const gmpi_render_desc* desc);
-/* gmpi_mpi_render_fwd_plan for the forward a descriptor describes (sizes, options, MPI pointers; the other fields are not read).  It sees
- * GMPI_MPI_F16: an fp16 MPI needs Wt % 8 == 0 for the staged kernels (GMPI_WHY_TEX_WIDTH otherwise).  Every non-NULL MPI pointer
- * (rgba, rgb, alpha, bg_rgb) must be 16-byte aligned (GMPI_WHY_ALIGNMENT); NULL ones are not checked.  Returns the plan, or a
+/* gmpi_mpi_render_fwd_plan for the forward a descriptor describes (sizes, options, MPI pointers; the other fields are not read):
+ * the plan gmpi_mpi_render_fwd_ex launches with.  It sees GMPI_MPI_F16: an fp16 MPI needs Wt % 8 == 0
+ * for the staged kernels (GMPI_WHY_TEX_WIDTH otherwise).  The MPI's pointers (rgba, or rgb + alpha + bg_rgb) must be 16-byte
+ * aligned (GMPI_WHY_ALIGNMENT); NULL ones are not checked.  Forward only, like gmpi_mpi_render_fwd_plan.  Returns the plan, or a
  * negative GMPI_ERR_* code for a bad descriptor. */
 int gmpi_mpi_render_fwd_plan_ex(const gmpi_render_desc* desc, uint32_t* why);
 int gmpi_mpi_render_bwd_ex(const gmpi_render_desc* desc);

@@ -18,8 +18,9 @@ OPT_COLOR_MINUS1_1 = 4
 OPT_ZERO_GRAD = 8
 
 PLAN_DIRECT, PLAN_STAGED = 1, 2
-WHY = {1: "texture width is not a multiple of 4", 2: "fewer than 120 tiles of 64x30 pixels", 4: "more than 512 planes",
-       8: "rgba base pointer not 16-byte aligned", 16: "direct kernel forced by gmpi_debug_set_fwd_variant"}
+WHY = {1: "texture width is not a multiple of 4 (8 in fp16)", 2: "fewer than 120 tiles of 64x30 pixels",
+       4: "more than 512 planes, or 2^31 planes over all MPIs", 8: "an MPI base pointer is not 16-byte aligned",
+       16: "direct kernel forced by gmpi_debug_set_fwd_variant"}
 
 ABI_VERSION = 2
 
@@ -159,3 +160,12 @@ def load():
 def check(rc: int):
     if rc != GMPI_OK:
         raise GmpiLibraryError(f"gmpi error {rc}: {load().gmpi_last_error().decode()}")
+
+
+def fwd_plan(desc: RenderDesc):
+    """(plan, why) of the forward `desc` describes (gmpi_mpi_render_fwd_plan_ex): PLAN_STAGED or PLAN_DIRECT, and the WHY bits."""
+    why = ctypes.c_uint32(0)
+    plan = load().gmpi_mpi_render_fwd_plan_ex(ctypes.byref(desc), ctypes.byref(why))
+    if plan < 0:
+        check(-plan)
+    return plan, why.value

@@ -423,24 +423,23 @@ static int check_params(const RenderParams& p, bool bwd) {
     return GMPI_OK;
 }
 
-// staged needs 16-byte row strides for the tensor map (Wt % 4 == 0 in fp32, Wt % 8 == 0 in fp16) and enough tiles to fill the
-// persistent grid; `why` receives the GMPI_WHY_* bits of every reason the TMA-staged kernel is NOT used (0 = staged)
-static bool staged_eligible(int V, int N, int Ht, int Wt, int H, int W, uint32_t* why = nullptr, bool f16 = false) {
-    (void)Ht;
+static bool aligned16(const void* a) { return ((uintptr_t)a & 15) == 0; }
+
+// The GMPI_WHY_* bits of every reason the TMA-staged forward is not launched for p (0 = staged): the one decision behind
+// launch_fwd, launch_bwd and the plan queries.  The tensor maps need 16-byte row strides (Wt % 4 == 0 in fp32, Wt % 8 == 0 in
+// fp16) and 16-byte aligned MPI bases (NULL counts as aligned); the plane-constant table holds kMaxPlanesStaged planes, and the
+// M*N planes of all MPIs stay below 2^31; the persistent grid needs enough tiles.  Reads the sizes, the fp16 bit, the MPI
+// pointers and the variant override, nothing else: the early-stop and training instantiations get the plain forward's plan.
+static uint32_t fwd_why(const RenderParams& p) {
     uint32_t w = 0;
-    if (N > kMaxPlanesStaged) w |= GMPI_WHY_MANY_PLANES;
-    if (Wt % (f16 ? 8 : 4) != 0) w |= GMPI_WHY_TEX_WIDTH;
+    if (p.N > kMaxPlanesStaged || (size_t)p.M * p.N >= ((size_t)1 << 31)) w |= GMPI_WHY_MANY_PLANES;
+    if (p.Wt % ((p.options & GMPI_MPI_F16) ? 8 : 4) != 0) w |= GMPI_WHY_TEX_WIDTH;
+    if (!(p.alpha ? aligned16(p.rgb) && aligned16(p.alpha) && aligned16(p.bg_rgb) : aligned16(p.rgba))) w |= GMPI_WHY_ALIGNMENT;
     const int forced = g_fwd_variant.load(std::memory_order_relaxed);
     if (forced == 1) w |= GMPI_WHY_FORCED;
-    const long tiles = (long)((W + kTileW - 1) / kTileW) * ((H + kTileH - 1) / kTileH) * V;
+    const long tiles = (long)((p.W + kTileW - 1) / kTileW) * ((p.H + kTileH - 1) / kTileH) * p.V;
     if (forced != 2 && tiles < 120) w |= GMPI_WHY_FEW_TILES;
-    if (why) *why = w;
-    return w == 0;
-}
-
-static bool aligned16(const void* a) { return ((uintptr_t)a & 15) == 0; }
-static bool mpi_aligned(const RenderParams& p) {
-    return p.alpha ? aligned16(p.rgb) && aligned16(p.alpha) && (!p.bg_rgb || aligned16(p.bg_rgb)) : aligned16(p.rgba);
+    return w;
 }
 
 // Tensor maps of the MPI (expanded or factored) for the five box-width classes.  Returns 0 on success.
@@ -558,7 +557,7 @@ static int launch_fwd(RenderParams p, cudaStream_t st) {
     if (p.W % 4 == 0 && !p.video_rgb && (p.n_peers > 0 || (aligned16(p.color) && aligned16(p.depth)))) p.options |= kOptVec4Stores;
     const bool ac = (p.options & GMPI_ALIGN_CORNERS) != 0, emit = p.transmittance != nullptr, fac = p.alpha != nullptr;
     const bool es = (p.options & GMPI_EARLY_STOP) != 0, f16 = (p.options & GMPI_MPI_F16) != 0;
-    if (staged_eligible(p.V, p.N, p.Ht, p.Wt, p.H, p.W, nullptr, f16) && mpi_aligned(p) && (size_t)p.M * p.N < ((size_t)1 << 31)) {
+    if (fwd_why(p) == 0) {
         TmaMaps maps;
         if (encode_mpi_maps(maps, p, kMaxBH, FwdRingWide::kColourCopyRows, fac) != 0) {
             if (g_fwd_variant.load(std::memory_order_relaxed) == 2) return fail(GMPI_ERR_CUDA, "cuTensorMapEncodeTiled failed");
@@ -645,14 +644,15 @@ static cudaError_t launch_bwd_box(BwdBoxKernel kernel, const RenderParams& p, co
     return cudaSuccess;
 }
 
-// Backward: the staged box kernel when the forward saved the transmittance and the shapes allow, else the direct kernel.
+// Backward: the staged box kernel when the forward saved the transmittance, the staged forward would be launched (fwd_why) and
+// the backward's own conditions hold (16-byte aligned gradient and transmittance bases, W % 4 == 0, V*N < 2^31), else the direct kernel.
 static int launch_bwd(RenderParams p, cudaStream_t st) {
     int rc = check_params(p, true);
     if (rc) return rc;
     const bool fac = p.alpha != nullptr;
     const bool grads_aligned = fac ? aligned16(p.g_rgb) && aligned16(p.g_alpha) && (!p.g_bg_rgb || aligned16(p.g_bg_rgb)) : aligned16(p.g_rgba);
-    if (!(p.transmittance && staged_eligible(p.V, p.N, p.Ht, p.Wt, p.H, p.W) && mpi_aligned(p) && grads_aligned &&
-          (size_t)p.M * p.N < ((size_t)1 << 31) && p.W % 4 == 0 && aligned16(p.transmittance) && (size_t)p.V * p.N < ((size_t)1 << 31)))
+    if (!(p.transmittance && fwd_why(p) == 0 && grads_aligned && p.W % 4 == 0 && aligned16(p.transmittance) &&
+          (size_t)p.V * p.N < ((size_t)1 << 31)))
         return launch_bwd_direct(p, st, true);
     if (p.V == 0) return (p.options & GMPI_ZERO_GRAD) ? zero_grads(p, st) : GMPI_OK;
     p.eye0 = p.eye;
@@ -720,6 +720,12 @@ static RenderParams params_classic(const float* rgba, const int32_t* view2mpi, c
     p.view_group = 1;
     p.early_stop = (options & GMPI_EARLY_STOP) ? NAN : 0.0f;   // the threshold is a descriptor field: check_params refuses the bit here
     return p;
+}
+
+static int fwd_plan(const RenderParams& p, uint32_t* why) {
+    const uint32_t w = fwd_why(p);
+    if (why) *why = w;
+    return w == 0 ? GMPI_PLAN_STAGED : GMPI_PLAN_DIRECT;
 }
 
 extern "C" {
@@ -795,27 +801,18 @@ int gmpi_debug_tile_walk(int H, int W, int V, int grid, int cta, int* out_v_px0_
 }
 
 int gmpi_mpi_render_fwd_plan(int V, int N, int Ht, int Wt, int H, int W, const void* rgba, uint32_t* why) {
-    uint32_t w = 0;
-    staged_eligible(V, N, Ht, Wt, H, W, &w);
-    if (rgba && ((uintptr_t)rgba & 15) != 0) w |= GMPI_WHY_ALIGNMENT;
-    if (why) *why = w;
-    return w == 0 ? GMPI_PLAN_STAGED : GMPI_PLAN_DIRECT;
+    return fwd_plan(params_classic(static_cast<const float*>(rgba), nullptr, nullptr, nullptr, nullptr, nullptr, 1, V, N, Ht, Wt, H, W, 0), why);
 }
 
 int gmpi_mpi_render_fwd_plan_ex(const gmpi_render_desc* d, uint32_t* why) {
     int rc = check_desc(d);
     if (rc) return -rc;
-    const bool f16 = (d->options & GMPI_MPI_F16) != 0;
-    uint32_t w = 0;
-    staged_eligible(d->V, d->N, d->Ht, d->Wt, d->H, d->W, &w, f16);
-    for (const float* t : {d->rgba, d->rgb, d->alpha, d->bg_rgb})
-        if (t && !aligned16(t)) w |= GMPI_WHY_ALIGNMENT;
-    if (why) *why = w;
-    return w == 0 ? GMPI_PLAN_STAGED : GMPI_PLAN_DIRECT;
+    return fwd_plan(params_from_desc(d), why);
 }
 
 const char* gmpi_mpi_render_fwd_variant(int N, int Ht, int Wt, int H, int W) {
-    return staged_eligible(1 << 20, N, Ht, Wt, H, W) ? "fwd_staged_tma_64x30" : "fwd_direct_32x8";
+    const RenderParams p = params_classic(nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 1, 1 << 20, N, Ht, Wt, H, W, 0);
+    return fwd_why(p) == 0 ? "fwd_staged_tma_64x30" : "fwd_direct_32x8";
 }
 
 int gmpi_mpi_render_fwd(const float* rgba, const int32_t* view2mpi, const float* dhw, const float* ray_dir,

@@ -108,15 +108,14 @@ class FrameGather:
         where render_frames would (GMPI_MPI_F16), else from its fp32 upcast."""
         import ctypes
         from . import _lib
-        from .mpi import _half_mpi, _options
+        from .mpi import _launch_mpi, _options
         lib = _lib.load()
         M, N, _, Ht, Wt = rgba.shape
         V = ray_dir.shape[0]
         assert V <= self.frames_per_rank and ray_dir.shape[2:] == (self.H, self.W)
         options = _options(align_corners, check_last_plane, color_minus1_1, early_stop=early_stop)
-        if rgba.dtype == torch.float16:
-            half = _half_mpi([rgba, None, None, None], V, self.H, self.W, options)
-            rgba, options = (half[0], options | _lib.OPT_MPI_F16) if half is not None else (rgba.float().contiguous(), options)
+        if rgba.dtype == torch.float16:     # any other MPI is rendered as passed (asserted below)
+            (rgba, _, _, _), options = _launch_mpi([rgba, None, None, None], V, self.H, self.W, options)
         mpi_dtype = torch.float16 if options & _lib.OPT_MPI_F16 else torch.float32
         f32 = torch.float32
         for name, t, dtype in (("rgba", rgba, mpi_dtype), ("dhw", dhw, f32), ("ray_dir", ray_dir, f32), ("eye", eye, f32),

@@ -98,6 +98,15 @@ class _RenderFn(torch.autograd.Function):
         return (g_rgba, g_rgb, g_alpha, g_bg) + (None,) * 9
 
 
+def _mpi_desc(mpi, V, H, W, options):
+    """Descriptor of what the forward plan reads (sizes, options, MPI pointers) for the MPI tensors `mpi` = [rgba, rgb, alpha, bg_rgb]
+    rendered from V views of H x W pixels."""
+    rgba, rgb, alpha, bg_rgb = mpi
+    ref = alpha if rgba is None else rgba
+    return _lib.make_desc(options=options, M=ref.shape[0], V=V, N=ref.shape[1], Ht=ref.shape[-2], Wt=ref.shape[-1], H=H, W=W,
+                          rgba=rgba, rgb=rgb, alpha=alpha, bg_rgb=bg_rgb)
+
+
 def _half_mpi(mpi, V, H, W, options):
     """The MPI tensors `mpi` = [rgba, rgb, alpha, bg_rgb] (None where absent) as contiguous fp16 when the call renders them natively
     (GMPI_MPI_F16), else None (the call upcasts them to fp32, as it always did).  Native when every MPI tensor is torch.float16,
@@ -110,33 +119,36 @@ def _half_mpi(mpi, V, H, W, options):
         return None
     # detached: under no_grad an fp16 tensor may still carry requires_grad, and the native path has no backward
     half = [None if t is None else t.detach().contiguous() for t in mpi]
-    rgba, rgb, alpha, bg_rgb = half
-    ref = alpha if rgba is None else rgba
-    lib = _lib.load()
-    sizes = dict(M=ref.shape[0], V=V, N=ref.shape[1], Ht=ref.shape[-2], Wt=ref.shape[-1], H=H, W=W)
-    plans = []
-    for opt, ptrs in ((options, {}), (options | _lib.OPT_MPI_F16, dict(rgba=rgba, rgb=rgb, alpha=alpha, bg_rgb=bg_rgb))):
-        d = _lib.make_desc(options=opt, **sizes, **ptrs)
-        plans.append(lib.gmpi_mpi_render_fwd_plan_ex(ctypes.byref(d), None))
-    return half if plans[0] == plans[1] else None
+    upcast = _mpi_desc(half, V, H, W, options)
+    upcast.rgba = upcast.rgb = upcast.alpha = upcast.bg_rgb = None     # the upcast is a fresh, aligned allocation
+    return half if _lib.fwd_plan(upcast)[0] == _lib.fwd_plan(_mpi_desc(half, V, H, W, options | _lib.OPT_MPI_F16))[0] else None
+
+
+def _launch_mpi(mpi, V, H, W, options):
+    """The MPI tensors `mpi` = [rgba, rgb, alpha, bg_rgb] (None where absent) as the forward reads them, and its options: contiguous
+    fp16 with GMPI_MPI_F16 where _half_mpi renders them natively, else contiguous fp32."""
+    half = _half_mpi(mpi, V, H, W, options)
+    if half is not None:
+        return half, options | _lib.OPT_MPI_F16
+    return [None if t is None else _as_f32c(t) for t in mpi], options
 
 
 _warned_direct = set()
 
 
-def _warn_if_direct(ref, V, H, W):
-    """Surface the direct-kernel performance cliff (several times slower than the TMA-staged kernels) once per shape."""
-    N, (Ht, Wt) = ref.shape[1], ref.shape[-2:]
-    key = (V, N, Ht, Wt, H, W, ref.data_ptr() & 15)
+def _warn_if_direct(d):
+    """Surface the direct-kernel performance cliff (several times slower than the TMA-staged kernels) of the forward descriptor `d`
+    is about to launch, once per shape, MPI dtype and MPI base alignment."""
+    key = (d.M, d.V, d.N, d.Ht, d.Wt, d.H, d.W, d.options & _lib.OPT_MPI_F16) + \
+        tuple((p or 0) & 15 for p in (d.rgba, d.rgb, d.alpha, d.bg_rgb))
     if key in _warned_direct:
         return
     _warned_direct.add(key)
-    why = ctypes.c_uint32(0)
-    if _lib.load().gmpi_mpi_render_fwd_plan(V, N, Ht, Wt, H, W, ref.data_ptr(), ctypes.byref(why)) == _lib.PLAN_DIRECT \
-            and (why.value & ~2 or V * N * H * W >= 1 << 26):      # "few tiles" only matters when the problem is not tiny
-        reasons = "; ".join(t for b, t in _lib.WHY.items() if why.value & b)
-        warnings.warn(f"ml_gmpi_b200: rendering V={V} N={N} tex={Ht}x{Wt} img={H}x{W} with the direct (one thread per pixel) "
-                      f"kernels, several times slower than the TMA-staged path: {reasons}", RuntimeWarning, stacklevel=3)
+    plan, why = _lib.fwd_plan(d)
+    if plan == _lib.PLAN_DIRECT and (why & ~2 or d.V * d.N * d.H * d.W >= 1 << 26):   # "few tiles" only matters when the problem is not tiny
+        reasons = "; ".join(t for b, t in _lib.WHY.items() if why & b)
+        warnings.warn(f"ml_gmpi_b200: rendering V={d.V} N={d.N} tex={d.Ht}x{d.Wt} img={d.H}x{d.W} with the direct (one thread per "
+                      f"pixel) kernels, several times slower than the TMA-staged path: {reasons}", RuntimeWarning, stacklevel=3)
 
 
 def _options(align_corners, check_last_plane, color_minus1_1, u8_round=False, early_stop=None):
@@ -166,14 +178,10 @@ def render_views(rgba, dhw, view2mpi, ray_dir, eye, z_dir, *, align_corners=True
     if flags is None:
         flags = torch.zeros(1, dtype=torch.int32, device=rgba.device)
     V, _, H, W = ray_dir.shape
-    _warn_if_direct(rgba, V, H, W)
-    options = _options(align_corners, check_last_plane, color_minus1_1, early_stop=early_stop)
-    half = _half_mpi([rgba, None, None, None], V, H, W, options)
-    if half is not None:
-        rgba, options = half[0], options | _lib.OPT_MPI_F16
-    else:
-        rgba = _as_f32c(rgba)
-    return _RenderFn.apply(rgba, None, None, None, _as_f32c(dhw), view2mpi, _as_f32c(ray_dir), _as_f32c(eye), _as_f32c(z_dir),
+    mpi, options = _launch_mpi([rgba, None, None, None], V, H, W,
+                               _options(align_corners, check_last_plane, color_minus1_1, early_stop=early_stop))
+    _warn_if_direct(_mpi_desc(mpi, V, H, W, options))
+    return _RenderFn.apply(*mpi, _as_f32c(dhw), view2mpi, _as_f32c(ray_dir), _as_f32c(eye), _as_f32c(z_dir),
                            options, flags, int(view_group), early_stop)
 
 
@@ -194,15 +202,10 @@ def render_views_factored(rgb, alpha, dhw, view2mpi, ray_dir, eye, z_dir, *, bg_
     if flags is None:
         flags = torch.zeros(1, dtype=torch.int32, device=alpha.device)
     V, _, H, W = ray_dir.shape
-    _warn_if_direct(alpha, V, H, W)
-    options = _options(align_corners, check_last_plane, color_minus1_1, early_stop=early_stop)
-    half = _half_mpi([None, rgb, alpha, bg_rgb], V, H, W, options)
-    if half is not None:
-        _, rgb, alpha, bg_rgb = half
-        options |= _lib.OPT_MPI_F16
-    else:
-        rgb, alpha, bg_rgb = _as_f32c(rgb), _as_f32c(alpha), None if bg_rgb is None else _as_f32c(bg_rgb)
-    return _RenderFn.apply(None, rgb, alpha, bg_rgb, _as_f32c(dhw), view2mpi, _as_f32c(ray_dir), _as_f32c(eye), _as_f32c(z_dir),
+    mpi, options = _launch_mpi([None, rgb, alpha, bg_rgb], V, H, W,
+                               _options(align_corners, check_last_plane, color_minus1_1, early_stop=early_stop))
+    _warn_if_direct(_mpi_desc(mpi, V, H, W, options))
+    return _RenderFn.apply(*mpi, _as_f32c(dhw), view2mpi, _as_f32c(ray_dir), _as_f32c(eye), _as_f32c(z_dir),
                            options, flags, int(view_group), early_stop)
 
 
@@ -254,15 +257,12 @@ def render_frames(*, dhw, view2mpi, rgba=None, rgb=None, alpha=None, bg_rgb=None
     else:
         color = torch.empty((V, 3, H, W), device=dev, dtype=torch.float32)
         depth = torch.empty((V, 1, H, W), device=dev, dtype=torch.float32)
-    options = _options(align_corners, check_last_plane, True, u8_round, early_stop)
-    half = _half_mpi([rgba, rgb, alpha, bg_rgb], V, H, W, options)
-    if half is not None:
-        options |= _lib.OPT_MPI_F16
-    keep = (half if half is not None else [_as_f32c(t) if t is not None else None for t in (rgba, rgb, alpha, bg_rgb)]) + [_as_f32c(dhw)]
+    mpi, options = _launch_mpi([rgba, rgb, alpha, bg_rgb], V, H, W, _options(align_corners, check_last_plane, True, u8_round, early_stop))
+    dhw = _as_f32c(dhw)
     with torch.cuda.device(dev):
         d = _lib.make_desc(options=options, M=M, V=V, N=N, Ht=Ht, Wt=Wt, H=H, W=W,
-                           view_group=int(view_group), depth_near=near, depth_range=rng, rgba=keep[0], rgb=keep[1], alpha=keep[2],
-                           bg_rgb=keep[3], view2mpi=view2mpi, dhw=keep[4], ray_dir=ray_dir, eye=eye, z_dir=z_dir, cam=cam, color=color,
+                           view_group=int(view_group), depth_near=near, depth_range=rng, rgba=mpi[0], rgb=mpi[1], alpha=mpi[2],
+                           bg_rgb=mpi[3], view2mpi=view2mpi, dhw=dhw, ray_dir=ray_dir, eye=eye, z_dir=z_dir, cam=cam, color=color,
                            depth=depth, video_rgb=v_rgb, video_depth=v_depth, flags=flags, stream=_stream_ptr(dev), early_stop=early_stop)
         _lib.check(lib.gmpi_mpi_render_fwd_ex(ctypes.byref(d)))
     return (v_rgb, v_depth) if video is not None else (color, depth)

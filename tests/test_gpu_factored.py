@@ -43,7 +43,7 @@ import ml_gmpi_b200 as g
 from ml_gmpi_b200 import _lib, synth
 from conftest import MPI_CASES, load_golden, rel_err
 from test_gpu_early_stop import set_variant
-from test_gpu_half import _limit_footprints, plan
+from test_gpu_half import _limit_footprints
 from test_gpu_bwd_limits import _expanded_grad, _factored_grads, _one_tile_per_mpi_case
 
 pytestmark = pytest.mark.gpu
@@ -347,7 +347,7 @@ def fwd_plan(c, mpi, view_group=1):
     V, _, H, W = c["ray_dir"].shape
     M, N, _, Ht, Wt = c["alpha"].shape
     desc = _lib.make_desc(options=0, M=M, V=V, N=N, Ht=Ht, Wt=Wt, H=H, W=W, view_group=view_group, rgb=mpi[0], alpha=mpi[1], bg_rgb=mpi[2])
-    p, why = plan(desc)
+    p, why = _lib.fwd_plan(desc)
     return ("staged" if p == _lib.PLAN_STAGED else "direct"), why
 
 

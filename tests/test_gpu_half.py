@@ -77,13 +77,6 @@ def _desc(c, m, half, tau=None, cam=None, u8_round=False, view_group=None):
     return desc, keep
 
 
-def plan(desc):
-    why = ctypes.c_uint32(0)
-    p = _lib.load().gmpi_mpi_render_fwd_plan_ex(ctypes.byref(desc), ctypes.byref(why))
-    assert p > 0
-    return p, why.value
-
-
 def run(c, half, **kw):
     """(outputs..., flags) of one gmpi_mpi_render_fwd_ex call, as numpy."""
     mkw = {k: kw.pop(k) for k in ("bg", "misalign") if k in kw}
@@ -105,7 +98,7 @@ def run_pair(c, variant, **kw):
     h = run(c, True, **kw)
     mkw = {k: kw[k] for k in ("bg", "misalign") if k in kw}
     desc, _ = _desc(c, _mpi(c, True, **mkw), True, **{k: v for k, v in kw.items() if k not in mkw})
-    fell_back = variant != "direct" and plan(desc)[0] == _lib.PLAN_DIRECT
+    fell_back = variant != "direct" and _lib.fwd_plan(desc)[0] == _lib.PLAN_DIRECT
     if fell_back:
         set_variant("direct")
     try:
@@ -146,18 +139,18 @@ def test_unaligned_and_narrow_fp16_fall_back_to_the_direct_kernel():
     try:
         c = case("small")
         desc, _ = _desc(c, _mpi(c, True, misalign=True), True)
-        assert plan(desc) == (_lib.PLAN_DIRECT, 8)
+        assert _lib.fwd_plan(desc) == (_lib.PLAN_DIRECT, 8)
         desc32, _ = _desc(c, _mpi(c, False), False)
-        assert plan(desc32) == (_lib.PLAN_STAGED, 0)
+        assert _lib.fwd_plan(desc32) == (_lib.PLAN_STAGED, 0)
         for tau in (None, 1e-3):
             h, f, fell_back = run_pair(c, "staged3", misalign=True, tau=tau)
             assert fell_back
             assert_bitwise(h, f, ("misaligned", tau))
         n = case("partial_acfalse_nonsquare")        # texture 72 x 116: 116 % 8 == 4
         desc, _ = _desc(n, _mpi(n, True), True)
-        assert plan(desc) == (_lib.PLAN_DIRECT, 1)
+        assert _lib.fwd_plan(desc) == (_lib.PLAN_DIRECT, 1)
         desc32, _ = _desc(n, _mpi(n, False), False)
-        assert plan(desc32) == (_lib.PLAN_STAGED, 0)
+        assert _lib.fwd_plan(desc32) == (_lib.PLAN_STAGED, 0)
         h, f, fell_back = run_pair(n, "staged3")
         assert fell_back
         assert_bitwise(h, f, "Wt % 8")

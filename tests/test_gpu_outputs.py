@@ -87,10 +87,8 @@ def _sentinel(n):
 
 
 def _plan(desc):
-    why = ctypes.c_uint32(0)
-    p = _lib.load().gmpi_mpi_render_fwd_plan_ex(ctypes.byref(desc), ctypes.byref(why))
-    assert p > 0, p
-    return ("staged" if p == _lib.PLAN_STAGED else "direct"), why.value
+    p, why = _lib.fwd_plan(desc)
+    return ("staged" if p == _lib.PLAN_STAGED else "direct"), why
 
 
 def _expect_plan(variant, desc):

@@ -59,9 +59,7 @@ def test_refusals_need_no_gpu(lib):
 
 
 def _plan(lib, half, Wt=1024, **ptrs):
-    why = ctypes.c_uint32(0)
-    d = _lib.make_desc(options=_lib.OPT_MPI_F16 if half else 0, M=4, V=4, N=96, Ht=1024, Wt=Wt, H=1024, W=1024, **ptrs)
-    return lib.gmpi_mpi_render_fwd_plan_ex(ctypes.byref(d), ctypes.byref(why)), why.value
+    return _lib.fwd_plan(_lib.make_desc(options=_lib.OPT_MPI_F16 if half else 0, M=4, V=4, N=96, Ht=1024, Wt=Wt, H=1024, W=1024, **ptrs))
 
 
 def test_plan_query_sees_the_dtype(lib):
@@ -77,7 +75,8 @@ def test_plan_query_sees_the_dtype(lib):
     assert lib.gmpi_mpi_render_fwd_plan(4, 96, 1024, 1020, 1024, 1024, None, ctypes.byref(why)) == _lib.PLAN_STAGED
     d = _lib.make_desc(M=1, V=1, N=1, Ht=8, Wt=8, H=8, W=8)
     d.struct_bytes = 8
-    assert lib.gmpi_mpi_render_fwd_plan_ex(ctypes.byref(d), None) < 0
+    with pytest.raises(_lib.GmpiLibraryError, match="struct_bytes"):
+        _lib.fwd_plan(d)
 
 
 def test_python_dispatch_rule(lib):
