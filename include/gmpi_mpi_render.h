@@ -51,7 +51,8 @@ extern "C" {
 #define GMPI_FLAG_RGBA_RANGE 1u        /* rgba outside [0,1]            mpi_renderer.py:447-449 */
 #define GMPI_FLAG_ALPHA_RANGE 2u       /* alpha outside [0,1]           mpi.py:185-187          */
 #define GMPI_FLAG_LAST_PLANE_OOB 4u    /* |u| or |v| > 1 on last plane  mpi.py:103-109,381-395  */
-#define GMPI_FLAG_PLANE_BEHIND_EYE 8u  /* distance < z_eye[0]           mpi.py:70-72            */
+#define GMPI_FLAG_PLANE_BEHIND_EYE 8u  /* !(distance >= z_eye[0])       mpi.py:70-72            */
+                                       /*   over the planes of the MPIs some view renders; z_eye[0]: view 0's eye */
 
 /* option bits for `options` */
 #define GMPI_ALIGN_CORNERS 1u          /* MPI(align_corners=True), configs/gmpi.yml:74          */

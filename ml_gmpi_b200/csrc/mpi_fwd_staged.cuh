@@ -627,11 +627,6 @@ __device__ __forceinline__ void fwd_staged_body(const RenderParams& p, const Tma
         int c_stage = 0;            // ring position of this warp: stage index and mbarrier phase parity
         uint32_t c_phase = 0;
         uint32_t flag = 0;
-        if (blockIdx.x == 0) {          // mpi.py:70: every plane distance against view 0's eye
-            const float eye0_z = __ldg(p.eye0 + 2);
-            for (int j = threadIdx.x; j < p.M * N; j += kConsThreads)
-                if (!(__ldg(p.dhw + (size_t)j * 3) >= eye0_z)) flag |= GMPI_FLAG_PLANE_BEHIND_EYE;
-        }
         const size_t tex = (size_t)Ht * Wt;
         int v_table = -1;
         TileXY txy;
@@ -642,7 +637,13 @@ __device__ __forceinline__ void fwd_staged_body(const RenderParams& p, const Tma
             load_eye_z(p, v, ev, zd);
             if (v != v_table) {          // (view, plane) constants, once per view and CTA
                 consumer_bar_sync<kConsThreads>();     // everyone is done with the previous view's table
-                for (int i = threadIdx.x; i < N; i += kConsThreads) s_pc[i] = make_plane_const(p.dhw + ((size_t)m * N + i) * 3, ev[2]);
+                // mpi.py:70 compares the distance of every plane the call renders (the MPIs of its views, not all p.M) with view 0's eye
+                const float eye0_z = __ldg(p.eye0 + 2);
+                for (int i = threadIdx.x; i < N; i += kConsThreads) {
+                    const float* dp = p.dhw + ((size_t)m * N + i) * 3;
+                    s_pc[i] = make_plane_const(dp, ev[2]);
+                    if (!(__ldg(dp) >= eye0_z)) flag |= GMPI_FLAG_PLANE_BEHIND_EYE;
+                }
                 consumer_bar_sync<kConsThreads>();
                 v_table = v;
             }

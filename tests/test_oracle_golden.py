@@ -14,6 +14,30 @@ from conftest import MPI_CASES, load_golden, rel_err
 
 TOL = 2e-6
 
+# The flag word each verdict of the reference implies (oracle/make_golden_flags.py): the forward's with the last-plane check, and
+# the range check's.  The forward never sets the range bits; without the last-plane check it never sets LAST_PLANE_OOB.
+FORWARD_FLAGS = {"ok": 0, "alpha": 0, "behind-eye": mpi_oracle.FLAG_PLANE_BEHIND_EYE, "out-of-plane": mpi_oracle.FLAG_LAST_PLANE_OOB}
+RANGE_FLAGS = {"ok": 0, "alpha": mpi_oracle.FLAG_ALPHA_RANGE | mpi_oracle.FLAG_RGBA_RANGE, "behind-eye": 0, "out-of-plane": 0}
+
+
+def load_flag_cases():
+    """[(name, verdict, case)] of tests/golden/flags_edges.npz; a case has rgba, dhw, view2mpi, ray_dir, eye, z_dir, align_corners."""
+    z = load_golden("flags_edges")
+    out = []
+    for name, verdict in zip(z["names"].tolist(), z["verdicts"].tolist()):
+        c = {k: z["pool_%d" % int(z[f"{name}__{k}"])] for k in ("dhw", "view2mpi", "ray_dir", "eye", "z_dir", "align_corners")}
+        r = z[f"{name}__rgba"]
+        c["rgba"] = np.random.default_rng(int(r[0])).random(tuple(z[f"{name}__rgba_shape"].tolist()), dtype=np.float32)
+        if len(r) > 1:
+            c["rgba"][tuple(int(i) for i in r[1:])] = z[f"{name}__rgba_value"]
+        out.append((name, verdict, c))
+    return out
+
+
+FLAG_CASES = load_flag_cases()
+_fz = load_golden("flags_edges")
+FIXTURE_VERDICTS = dict(zip(_fz["fixtures"].tolist(), _fz["fixture_verdicts"].tolist()))
+
 
 @pytest.mark.parametrize("name", MPI_CASES + ["c1_full_256"])
 def test_c_oracle_forward_matches_reference(name):
@@ -24,7 +48,9 @@ def test_c_oracle_forward_matches_reference(name):
     assert rel_err(depth, g["depth"]) <= TOL
     if name == "out_of_plane":
         assert flags & mpi_oracle.FLAG_LAST_PLANE_OOB
-    elif name not in ("nonsquare", "tiny_2mpi_3view_acfalse"):
+    elif name in FIXTURE_VERDICTS:         # the reference's own verdict on the fixture (oracle/make_golden_flags.py)
+        assert flags == FORWARD_FLAGS[FIXTURE_VERDICTS[name]], (flags, FIXTURE_VERDICTS[name])
+    else:
         assert flags == 0
 
 
@@ -126,3 +152,19 @@ def test_edge_cases_c_oracle_and_torch_port(name):
         assert g["view2mpi"].tolist() == [0, 0, 2] and not gr[1].any()          # the view-less MPI gets an exactly zero gradient
     if name == "edge_single_plane":                                             # N = 1: colour = alpha_0 * rgb_0 of the warped plane
         assert g["rgba"].shape[1] == 1 and float(np.max(color)) <= 1.0
+
+
+@pytest.mark.parametrize("name,verdict,case", FLAG_CASES, ids=[n for n, _, _ in FLAG_CASES])
+def test_oracle_flags_are_the_reference_verdict(name, verdict, case):
+    """Crafted cases at the edges of the reference's three data-dependent checks (oracle/make_golden_flags.py): |u| or |v| exactly
+    1 on the last plane and one ulp beyond, a NaN ray, a plane distance equal to view 0's eye z and one ulp below, a plane behind
+    a later view's eye, a plane behind the eye in an MPI no view renders, a NaN distance, alpha of 1 + 2^-23, -0.0, -denormal and
+    NaN.  The oracle's forward (with and without the last-plane check) and range check give exactly the bit the reference's
+    verdict implies, and no other."""
+    c = case
+    args = (c["rgba"], c["view2mpi"], c["dhw"], c["ray_dir"], c["eye"], c["z_dir"])
+    ac = bool(c["align_corners"])
+    assert mpi_oracle.forward(*args, align_corners=ac, check_last_plane=True)[2] == FORWARD_FLAGS[verdict]
+    assert mpi_oracle.forward(*args, align_corners=ac, check_last_plane=False)[2] == \
+        FORWARD_FLAGS[verdict] & ~mpi_oracle.FLAG_LAST_PLANE_OOB
+    assert mpi_oracle.check_range(c["rgba"]) == RANGE_FLAGS[verdict]
