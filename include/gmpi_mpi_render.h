@@ -262,6 +262,29 @@ int gmpi_mpi_render_fwd_ex(const gmpi_render_desc* desc);
  * negative GMPI_ERR_* code for a bad descriptor. */
 int gmpi_mpi_render_fwd_plan_ex(const gmpi_render_desc* desc, uint32_t* why);
 int gmpi_mpi_render_bwd_ex(const gmpi_render_desc* desc);
+
+/*
+ * Deterministic backward (opt-in): gmpi_mpi_render_bwd_ex with bitwise-reproducible gradients.  The same inputs give the same bits
+ * on every call, and so do the views of an MPI permuted together with their rays and upstream gradients.  It takes the same
+ * descriptors and kernel choice as gmpi_mpi_render_bwd_ex (the staged box kernel with a saved transmittance where that call would
+ * use it, the direct kernel otherwise) and refuses what that call refuses.  Every contribution is rounded to a per-call unit
+ * 2^(E - k) and summed exactly in int64 (red.global.add.u64) in `scratch`, so the order of the hardware's additions does not matter:
+ *   E  from the largest upstream gradient of the call (a pre-pass over every pixel of every view; inf/NaN left out), clamped to
+ *      [-100, 128];
+ *   k  = 61 - ceil(log2(H*W)) - ceil(log2(V)) - ceil(log2(planes summed into one element: N for a factored MPI's colour, else 1)),
+ *      so that no element's sum can wrap (GMPI_ERR_UNSUPPORTED below 24 bits).
+ * Each gradient is within (contributions) * 2^(E-k-1) + 2^-24 |gradient| of the exact sum of its contributions, on top of the
+ * staged kernel's per-tile fixed point that gmpi_mpi_render_bwd_ex has too (DESIGN.md section 4.3).  An inf/NaN contribution gives
+ * what an fp32 sum gives: NaN if a NaN or both infinities were added, else that infinity.  Results written with GMPI_ZERO_GRAD,
+ * added into the gradient buffers without it.
+ * scratch: device memory of at least gmpi_mpi_render_bwd_deterministic_scratch_bytes(desc) bytes, 16-byte aligned; zeroed by the
+ * callee on the stream; 8 bytes per gradient element plus half a byte of non-finite bits plus 256.  The callee allocates nothing.
+ * The scratch-size query reads the sizes and which MPI pointers (rgba, or rgb + alpha with or without bg_rgb) are set; it
+ * returns the bytes, or a negative GMPI_ERR_* code.  Neither needs a GPU to refuse a call.
+ */
+long long gmpi_mpi_render_bwd_deterministic_scratch_bytes(const gmpi_render_desc* desc);
+int gmpi_mpi_render_bwd_deterministic_ex(const gmpi_render_desc* desc, void* scratch, size_t scratch_bytes);
+
 /* Host-buffer form (end-to-end entry point, see gmpi_mpi_render_fwd_host): all pointers of *desc are HOST memory, `stream` is
  * ignored, *flags receives the flag word.  Forward only; supports the factored MPI, cam and the video outputs. */
 int gmpi_mpi_render_host_ex(const gmpi_render_desc* desc, int device);

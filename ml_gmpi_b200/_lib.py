@@ -31,6 +31,7 @@ EXPORTS = [
     "gmpi_debug_tile_walk_ex", "gmpi_debug_cam_rays", "gmpi_debug_set_fwd_stages", "gmpi_debug_fwd_ring_stages",
     "gmpi_debug_fwd_early_stop_stats", "gmpi_mpi_zero_async", "gmpi_mpi_alpha_depth_fwd", "gmpi_mpi_alpha_depth_bwd", "gmpi_mpi_apply_shading_fwd", "gmpi_mpi_apply_shading_bwd",
     "gmpi_mpi_render_fwd_plan_ex", "gmpi_mpi_check_range_f16",
+    "gmpi_mpi_render_bwd_deterministic_scratch_bytes", "gmpi_mpi_render_bwd_deterministic_ex",
 ]
 
 OPT_U8_ROUND_HALF_UP = 16
@@ -151,6 +152,10 @@ def load():
     lib.gmpi_mpi_render_host_ex.argtypes = [ctypes.POINTER(RenderDesc), i]
     lib.gmpi_mpi_render_fwd_plan_ex.restype = i
     lib.gmpi_mpi_render_fwd_plan_ex.argtypes = [ctypes.POINTER(RenderDesc), vp]
+    lib.gmpi_mpi_render_bwd_deterministic_scratch_bytes.restype = ll
+    lib.gmpi_mpi_render_bwd_deterministic_scratch_bytes.argtypes = [ctypes.POINTER(RenderDesc)]
+    lib.gmpi_mpi_render_bwd_deterministic_ex.restype = i
+    lib.gmpi_mpi_render_bwd_deterministic_ex.argtypes = [ctypes.POINTER(RenderDesc), vp, ctypes.c_size_t]
     if lib.gmpi_abi_version() != ABI_VERSION:
         raise GmpiLibraryError(f"ABI mismatch: library {lib.gmpi_abi_version()} != binding {ABI_VERSION}; rebuild")
     _lib = lib
@@ -160,6 +165,14 @@ def load():
 def check(rc: int):
     if rc != GMPI_OK:
         raise GmpiLibraryError(f"gmpi error {rc}: {load().gmpi_last_error().decode()}")
+
+
+def deterministic_scratch_bytes(desc: RenderDesc) -> int:
+    """Bytes of scratch gmpi_mpi_render_bwd_deterministic_ex needs for `desc` (raises on a bad descriptor)."""
+    n = load().gmpi_mpi_render_bwd_deterministic_scratch_bytes(ctypes.byref(desc))
+    if n < 0:
+        check(-n)
+    return n
 
 
 def fwd_plan(desc: RenderDesc):

@@ -158,6 +158,92 @@ __device__ __forceinline__ void fix2(f2 vF, f2 w, int& ia, int& ib) {
     ib = ((__float_as_int(t1.y) - kMagicHiBits) << kFixSplit) + (__float_as_int(t2.y) - kFloorMagicBits);
 }
 
+// ---- deterministic backward (gmpi_mpi_render_bwd_deterministic_ex, DESIGN.md section 4.3) ----
+// Every contribution becomes an integer in units of 2^(E - k), one E per call and channel kind (the box kernel's per-tile bound
+// taken over all pixels of all views, mpi_bwd_det_bounds_kernel), and is added with red.global.add.u64 into int64 sums: integer
+// addition is associative, so the sums do not depend on the order the hardware adds in.  An inf/NaN contribution sets a bit of
+// its element instead (1 +inf, 2 -inf, 4 NaN; four bits per element).  mpi_bwd_det_finish_kernel turns both into fp32.
+// The kernels address the sums through the gradient pointers of RenderParams, which point into the scratch viewed as floats:
+// (dst - base) is the element index.
+struct DetAcc {
+    float* base;                 // scratch sums viewed as floats; the g_* pointers of the call's RenderParams point into it
+    unsigned long long* acc;     // [G] int64 sums (two's complement)
+    uint32_t* nf;                // [ceil(G / 8)] non-finite bits
+    uint32_t* bounds;            // [2] bits of the call's qmax and gmax (non-negative floats)
+    int k_a, k_rgb;              // fraction bits of the alpha and colour units (chosen per call on the host: no sum can wrap)
+};
+// The unit 2^ue of one channel kind and 2^-ue as the product of two normal floats (2^-ue itself can be out of float range).
+struct DetUnit {
+    float s0, s1;
+    int ue;
+};
+// Clamp of the call's exponent: every scale constant of the box kernel is a normal float (as per tile)
+__device__ __forceinline__ DetUnit det_unit(float bound, int k) {
+    const int e = max(kMinScaleExp, min(kMaxScaleExp, tile_scale_exponent(bound)));
+    const int sh = k - e, h = sh / 2;
+    DetUnit u;
+    u.s0 = __uint_as_float((unsigned)(127 + h) << 23);
+    u.s1 = __uint_as_float((unsigned)(127 + sh - h) << 23);
+    u.ue = e - k;
+    return u;
+}
+__device__ __forceinline__ void det_add_int(const DetAcc& d, size_t i, long long x) {
+    if (x) asm volatile("red.global.add.u64 [%0], %1;" ::"l"(d.acc + i), "l"(x) : "memory");
+}
+// one fp32 contribution c to the element `dst` points at (a pointer into DetAcc::base)
+__device__ __forceinline__ void det_add(const DetAcc& d, const DetUnit& u, const float* dst, float c) {
+    const size_t i = (size_t)(dst - d.base);
+    if (!(fabsf(c) <= 0x1.fffffep127f)) {
+        const uint32_t bit = c != c ? 4u : c > 0.0f ? 1u : 2u;
+        atomicOr(d.nf + (i >> 3), bit << ((i & 7) * 4));
+        return;
+    }
+    det_add_int(d, i, __float2ll_rn(__fmul_rn(__fmul_rn(c, u.s0), u.s1)));     // exact scaling, one rounding to the unit
+}
+// A tile's fixed-point sum s in units 2^te -> units 2^ue: exact when te >= ue, else rounded to nearest, ties away from zero.
+// (|s 2^(te - ue)| < 2^62 by the choice of k: the shift cannot overflow.)
+__device__ __forceinline__ long long det_rescale(int s, int te, int ue) {
+    const int sh = te - ue;
+    if (sh >= 0) return (long long)((unsigned long long)(long long)s << sh);
+    if (sh < -31) return 0;                                   // |s| <= 2^31: |s| 2^sh < 1/2
+    const long long a = s < 0 ? -(long long)s : (long long)s;
+    const long long q = (a + (1ll << (-sh - 1))) >> -sh;
+    return s < 0 ? -q : q;
+}
+__device__ __noinline__ void scatter_plane_det(const DetAcc& da, const DetUnit& ua, const DetUnit& urgb, float* __restrict__ gplane,
+                                               size_t tex, int Wt, int Ht, int x0, int y0, float v0, float v1, float v2, float v3,
+                                               float w00, float w01, float w10, float w11) {
+    const bool vx0 = (unsigned)x0 < (unsigned)Wt, vx1 = (unsigned)(x0 + 1) < (unsigned)Wt;
+    const bool vy0 = (unsigned)y0 < (unsigned)Ht, vy1 = (unsigned)(y0 + 1) < (unsigned)Ht;
+    float* b0 = gplane + ((long long)y0 * Wt + x0);
+    const float v[4] = {v0, v1, v2, v3};
+#pragma unroll
+    for (int c = 0; c < 4; ++c, b0 += tex) {
+        const DetUnit& u = c == 3 ? ua : urgb;
+        if (vx0 && vy0) det_add(da, u, b0, v[c] * w00);
+        if (vx1 && vy0) det_add(da, u, b0 + 1, v[c] * w01);
+        if (vx0 && vy1) det_add(da, u, b0 + Wt, v[c] * w10);
+        if (vx1 && vy1) det_add(da, u, b0 + Wt + 1, v[c] * w11);
+    }
+}
+__device__ __noinline__ void scatter_pixel_det(const DetAcc& da, const DetUnit& ua, const DetUnit& urgb, const GradChans gch, int Wt,
+                                               int Ht, int x0, int y0, float v0, float v1, float v2, float v3, float w00, float w01,
+                                               float w10, float w11) {
+    const bool vx0 = (unsigned)x0 < (unsigned)Wt, vx1 = (unsigned)(x0 + 1) < (unsigned)Wt;
+    const bool vy0 = (unsigned)y0 < (unsigned)Ht, vy1 = (unsigned)(y0 + 1) < (unsigned)Ht;
+    const long long o = (long long)y0 * Wt + x0;
+    const float v[4] = {v0, v1, v2, v3};
+#pragma unroll
+    for (int c = 0; c < 4; ++c) {
+        const DetUnit& u = c == 3 ? ua : urgb;
+        float* b0 = gch.c[c] + o;
+        if (vx0 && vy0) det_add(da, u, b0, v[c] * w00);
+        if (vx1 && vy0) det_add(da, u, b0 + 1, v[c] * w01);
+        if (vx0 && vy1) det_add(da, u, b0 + Wt, v[c] * w10);
+        if (vx1 && vy1) det_add(da, u, b0 + Wt + 1, v[c] * w11);
+    }
+}
+
 // One (pair, channel) of the scatter: the four bilinear contributions of two pixels into the gradient box.
 template <int PITCH, bool kTwoStep>
 __device__ __forceinline__ void scatter_channel(int* __restrict__ ga, int* __restrict__ gq, f2 vF, const f2 (&w)[4]) {
@@ -213,9 +299,10 @@ __device__ __forceinline__ bool bwd_box_pairs(const float* __restrict__ sb, int*
 }
 
 // Flusher: rows fw, fw + 3, ... of a finished gradient box -> fp32 -> red.global.add.v4.f32, then zero.
-template <int BW, bool FAC>
+// kDet: the box's integer sums go to the deterministic sums instead, converted to the call's units (ue_a, ue_rgb).
+template <int BW, bool FAC, bool kDet = false>
 __device__ __forceinline__ void flush_box(int* __restrict__ gb, const GradMeta& gm, const RenderParams& p, size_t tex, int Ht, int Wt,
-                                          int fw, int lane) {
+                                          int fw, int lane, const DetAcc& da, int ue_a, int ue_rgb) {
     constexpr int Q = BW / 4;      // float4 quads per channel row
     // destination slabs of the four channels
     float* dst[4];
@@ -250,15 +337,25 @@ __device__ __forceinline__ void flush_box(int* __restrict__ gb, const GradMeta& 
             if ((a[k].x | a[k].y | a[k].z | a[k].w) == 0) continue;  // untouched halo (or a row beyond the box): nothing to add or clear
             *reinterpret_cast<int4*>(gb + r * pitch + cell0) = make_int4(0, 0, 0, 0);
             const int ty = gm.by0 + r;
-            if (col_ok && (unsigned)ty < (unsigned)Ht)
+            if constexpr (kDet) {
+                if (col_ok && (unsigned)ty < (unsigned)Ht) {
+                    const int te = (int)((__float_as_uint(sc) >> 23) & 0xffu) - 127, ue = ch < 3 ? ue_rgb : ue_a;   // sc = 2^te
+                    const size_t i = (size_t)(d + (size_t)ty * Wt - da.base);
+                    det_add_int(da, i, det_rescale(a[k].x, te, ue));
+                    det_add_int(da, i + 1, det_rescale(a[k].y, te, ue));
+                    det_add_int(da, i + 2, det_rescale(a[k].z, te, ue));
+                    det_add_int(da, i + 3, det_rescale(a[k].w, te, ue));
+                }
+            } else if (col_ok && (unsigned)ty < (unsigned)Ht)
                 red_add_v4(d + (size_t)ty * Wt, (float)a[k].x * sc, (float)a[k].y * sc, (float)a[k].z * sc, (float)a[k].w * sc);
         }
     }
 }
 
-template <bool kAlignCorners, bool kFactored>
-__global__ void __launch_bounds__(kBwdThreads, 1)
-mpi_bwd_box_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps, const int tiles_x, const int tiles_y) {
+// The box kernel's body; kDet: the deterministic instantiation (flush and generic-body scatter into DetAcc `da`).
+template <bool kAlignCorners, bool kFactored, bool kDet>
+__device__ __forceinline__ void bwd_box_body(const RenderParams p, const TmaMaps& maps, const int tiles_x, const int tiles_y,
+                                             const DetAcc da) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     float* s_buf = reinterpret_cast<float*>(smem_raw);                                          // rgba ring (+ transmittance boxes)
     int* s_grad = reinterpret_cast<int*>(smem_raw + (size_t)kBwdStages * kBwdStride * 4);       // gradient boxes
@@ -299,6 +396,11 @@ mpi_bwd_box_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps, c
     } else if (warp > kBwdConsWarps) {
         // ================================ flushers ================================
         const int fw = warp - kBwdConsWarps - 1;
+        int ue_a = 0, ue_rgb = 0;
+        if constexpr (kDet) {
+            ue_a = det_unit(__uint_as_float(__ldg(da.bounds)), da.k_a).ue;
+            ue_rgb = det_unit(0.5f * __uint_as_float(__ldg(da.bounds + 1)), da.k_rgb).ue;
+        }
         int f_box = 0;
         uint32_t f_phase = 0;
         TileXY txy;
@@ -312,11 +414,11 @@ mpi_bwd_box_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps, c
                 int* gb = s_grad + b * kBwdPlaneFloats;
                 if (gm.rows > 0) {
                     switch (gm.cls) {     // warp-uniform
-                        case 0: flush_box<56, kFactored>(gb, gm, p, tex, Ht, Wt, fw, lane); break;
-                        case 1: flush_box<64, kFactored>(gb, gm, p, tex, Ht, Wt, fw, lane); break;
-                        case 2: flush_box<72, kFactored>(gb, gm, p, tex, Ht, Wt, fw, lane); break;
-                        case 3: flush_box<80, kFactored>(gb, gm, p, tex, Ht, Wt, fw, lane); break;
-                        default: flush_box<88, kFactored>(gb, gm, p, tex, Ht, Wt, fw, lane); break;
+                        case 0: flush_box<56, kFactored, kDet>(gb, gm, p, tex, Ht, Wt, fw, lane, da, ue_a, ue_rgb); break;
+                        case 1: flush_box<64, kFactored, kDet>(gb, gm, p, tex, Ht, Wt, fw, lane, da, ue_a, ue_rgb); break;
+                        case 2: flush_box<72, kFactored, kDet>(gb, gm, p, tex, Ht, Wt, fw, lane, da, ue_a, ue_rgb); break;
+                        case 3: flush_box<80, kFactored, kDet>(gb, gm, p, tex, Ht, Wt, fw, lane, da, ue_a, ue_rgb); break;
+                        default: flush_box<88, kFactored, kDet>(gb, gm, p, tex, Ht, Wt, fw, lane, da, ue_a, ue_rgb); break;
                     }
                 }
                 __syncwarp();
@@ -478,6 +580,11 @@ mpi_bwd_box_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps, c
                     float* gplane = kFactored ? nullptr : p.g_rgba + ((size_t)m * N + i) * 4 * tex;
                     float* Rs = reinterpret_cast<float*>(R);
                     const float* Ts = reinterpret_cast<const float*>(T);
+                    DetUnit ua{}, urgb{};
+                    if constexpr (kDet) {
+                        ua = det_unit(__uint_as_float(__ldg(da.bounds)), da.k_a);
+                        urgb = det_unit(0.5f * __uint_as_float(__ldg(da.bounds + 1)), da.k_rgb);
+                    }
 #pragma unroll
                     for (int q = 0; q < kPix; ++q) {
                         const int qq = (q & 1) + 2 * (q >> 1);      // R / T are stored as pairs: element (P, half) = 2 P + half
@@ -492,7 +599,14 @@ mpi_bwd_box_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps, c
                         const float d = qv - Rs[qq];
                         const float w = sv.w * Ts[qq];
                         Rs[qq] = fmaf(sv.w, d, Rs[qq]);
-                        if (kFactored)
+                        if constexpr (kDet) {
+                            if (kFactored)
+                                scatter_pixel_det(da, ua, urgb, grad_chans(p, m, i, tex), Wt, Ht, (int)fx, (int)fy, gq[q][0] * w,
+                                                  gq[q][1] * w, gq[q][2] * w, Ts[qq] * d, wx0 * wy0, wx1 * wy0, wx0 * wy1, wx1 * wy1);
+                            else
+                                scatter_plane_det(da, ua, urgb, gplane, tex, Wt, Ht, (int)fx, (int)fy, gq[q][0] * w, gq[q][1] * w,
+                                                  gq[q][2] * w, Ts[qq] * d, wx0 * wy0, wx1 * wy0, wx0 * wy1, wx1 * wy1);
+                        } else if (kFactored)
                             scatter_pixel_global(grad_chans(p, m, i, tex), Wt, Ht, (int)fx, (int)fy, gq[q][0] * w, gq[q][1] * w, gq[q][2] * w,
                                                  Ts[qq] * d, wx0 * wy0, wx1 * wy0, wx0 * wy1, wx1 * wy1);
                         else
@@ -503,6 +617,19 @@ mpi_bwd_box_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps, c
             }
         }
     }
+}
+
+template <bool kAlignCorners, bool kFactored>
+__global__ void __launch_bounds__(kBwdThreads, 1)
+mpi_bwd_box_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps, const int tiles_x, const int tiles_y) {
+    bwd_box_body<kAlignCorners, kFactored, false>(p, maps, tiles_x, tiles_y, DetAcc{});
+}
+
+// The deterministic backward's box kernel (a kernel of its own: the default instantiations keep their machine code)
+template <bool kAlignCorners, bool kFactored>
+__global__ void __launch_bounds__(kBwdThreads, 1)
+mpi_bwd_box_det_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps, const int tiles_x, const int tiles_y, const DetAcc da) {
+    bwd_box_body<kAlignCorners, kFactored, true>(p, maps, tiles_x, tiles_y, da);
 }
 
 }  // namespace gmpi

@@ -157,10 +157,10 @@ mpi_fwd_direct_early_stop_f16_kernel(const RenderParams p) {
 //           which equals autograd's  T_i q_i - (sum_{k>i} a_k q_k P_k)/s_i  (cumprod_backward)
 //           without the division by s_i (1e-10 when a_i == 1) and without cancellation.
 //           The four bilinear weights scatter each value with red.global.add.f32.
+// kDet: the deterministic backward's variant, which adds each contribution to the int64 sums of `da` instead (det_add).
 // ------------------------------------------------------------------------------------------
-template <bool kAlignCorners>
-__global__ void __launch_bounds__(128)
-mpi_bwd_direct_kernel(const RenderParams p, const int tile_w, const int tile_h) {
+template <bool kAlignCorners, bool kDet>
+__device__ __forceinline__ void bwd_direct_body(const RenderParams p, const int tile_w, const int tile_h, const DetAcc da) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     PlaneConst* s_pc = reinterpret_cast<PlaneConst*>(smem_raw);
     const int nthreads = tile_w * tile_h;
@@ -196,6 +196,11 @@ mpi_bwd_direct_kernel(const RenderParams p, const int tile_w, const int tile_h) 
     const float G0 = gscale * __ldg(gc), G1 = gscale * __ldg(gc + img), G2 = gscale * __ldg(gc + 2 * img);
     const float Gd = p.g_depth ? __ldg(p.g_depth + (size_t)v * img + pix) : 0.0f;
     const float Gdz = Gd * rc.dz;   // depth_i = scale_i * dz
+    DetUnit ua{}, urgb{};
+    if constexpr (kDet) {
+        ua = det_unit(__uint_as_float(__ldg(da.bounds)), da.k_a);
+        urgb = det_unit(0.5f * __uint_as_float(__ldg(da.bounds + 1)), da.k_rgb);
+    }
 
     // pass A
     float T = 1.0f;
@@ -228,11 +233,105 @@ mpi_bwd_direct_kernel(const RenderParams p, const int tile_w, const int tile_h) 
 #pragma unroll
         for (int c = 0; c < 4; ++c) {
             float* gch = gp.c[c];
-            if (t.w00 != 0.0f) atomicAdd(gch + t.o00, gv[c] * t.w00);
-            if (t.w01 != 0.0f) atomicAdd(gch + t.o01, gv[c] * t.w01);
-            if (t.w10 != 0.0f) atomicAdd(gch + t.o10, gv[c] * t.w10);
-            if (t.w11 != 0.0f) atomicAdd(gch + t.o11, gv[c] * t.w11);
+            if constexpr (kDet) {
+                const DetUnit& u = c == 3 ? ua : urgb;
+                if (t.w00 != 0.0f) det_add(da, u, gch + t.o00, gv[c] * t.w00);
+                if (t.w01 != 0.0f) det_add(da, u, gch + t.o01, gv[c] * t.w01);
+                if (t.w10 != 0.0f) det_add(da, u, gch + t.o10, gv[c] * t.w10);
+                if (t.w11 != 0.0f) det_add(da, u, gch + t.o11, gv[c] * t.w11);
+            } else {
+                if (t.w00 != 0.0f) atomicAdd(gch + t.o00, gv[c] * t.w00);
+                if (t.w01 != 0.0f) atomicAdd(gch + t.o01, gv[c] * t.w01);
+                if (t.w10 != 0.0f) atomicAdd(gch + t.o10, gv[c] * t.w10);
+                if (t.w11 != 0.0f) atomicAdd(gch + t.o11, gv[c] * t.w11);
+            }
         }
+    }
+}
+
+template <bool kAlignCorners>
+__global__ void __launch_bounds__(128)
+mpi_bwd_direct_kernel(const RenderParams p, const int tile_w, const int tile_h) {
+    bwd_direct_body<kAlignCorners, false>(p, tile_w, tile_h, DetAcc{});
+}
+
+template <bool kAlignCorners>
+__global__ void __launch_bounds__(128)
+mpi_bwd_direct_det_kernel(const RenderParams p, const int tile_w, const int tile_h, const DetAcc da) {
+    bwd_direct_body<kAlignCorners, true>(p, tile_w, tile_h, da);
+}
+
+// ------------------------------------------------------------------------------------------
+// Deterministic backward: the call's scale pre-pass and the finish pass (see DetAcc in mpi_bwd_box.cuh).
+// ------------------------------------------------------------------------------------------
+// bounds[0] = max over every pixel of every view of the box kernel's per-pixel alpha bound |G_r| + |G_g| + |G_b| + |G_d dz| *
+// max_i |z_diff_i| / |ray_z| (the same float operations as the tile bound of bwd_box_body, so no tile's exponent exceeds the
+// call's); bounds[1] = max |G_c|.  Pixels with an inf/NaN upstream gradient are left out of bounds[0] and non-finite
+// components out of bounds[1]: their contributions go to the non-finite bits.  Integer atomicMax on the bits of non-negative
+// floats: independent of order.  Grid (pixel blocks, min(V, 65535)) of 256 threads; block row y takes views y, y + gridDim.y, ...
+__global__ void __launch_bounds__(256)
+mpi_bwd_det_bounds_kernel(const RenderParams p, uint32_t* __restrict__ bounds) {
+    __shared__ unsigned s_zmax;
+    const size_t img = (size_t)p.H * p.W, pix = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const float gscale = (p.options & GMPI_COLOR_MINUS1_1) ? 2.0f : 1.0f;
+    float qmax = 0.0f, gmax = 0.0f;
+    for (int v = blockIdx.y; v < p.V; v += gridDim.y) {
+        const int m = __ldg(p.view2mpi + v);
+        const float ev[3] = {__ldg(p.eye + 3 * v), __ldg(p.eye + 3 * v + 1), __ldg(p.eye + 3 * v + 2)};
+        const float zd[3] = {__ldg(p.z_dir + 3 * v), __ldg(p.z_dir + 3 * v + 1), __ldg(p.z_dir + 3 * v + 2)};
+        __syncthreads();
+        if (threadIdx.x == 0) s_zmax = 0u;
+        __syncthreads();
+        float zm = 0.0f;
+        for (int i = threadIdx.x; i < p.N; i += blockDim.x)
+            zm = fmaxf(zm, fabsf(make_plane_const(p.dhw + ((size_t)m * p.N + i) * 3, ev[2]).z_diff));
+        atomicMax(&s_zmax, __float_as_uint(zm));
+        __syncthreads();
+        const float zmax = __uint_as_float(s_zmax);
+        if (pix < img) {
+            const float* rd = p.ray_dir + (size_t)v * 3 * img + pix;
+            const RayConst rc = make_ray_const(__ldg(rd), __ldg(rd + img), __ldg(rd + 2 * img), ev, zd);
+            const float* gc = p.g_color + (size_t)v * 3 * img + pix;
+            const float g0 = gscale * __ldg(gc), g1 = gscale * __ldg(gc + img), g2 = gscale * __ldg(gc + 2 * img);
+            const float g3 = p.g_depth ? __ldg(p.g_depth + (size_t)v * img + pix) * rc.dz : 0.0f;
+            const float ga = fabsf(g0) + fabsf(g1) + fabsf(g2), gd = fabsf(g3);
+            if (ga + gd <= 0x1.fffffep127f) qmax = fmaxf(qmax, ga + gd * (zmax * fabsf(rc.yrz)));   // NaN (0 * inf) is dropped
+            const auto fin = [](float x) { return fabsf(x) <= 0x1.fffffep127f ? fabsf(x) : 0.0f; };
+            gmax = fmaxf(gmax, fmaxf(fin(g0), fmaxf(fin(g1), fin(g2))));
+        }
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+        qmax = fmaxf(qmax, __shfl_xor_sync(0xffffffffu, qmax, o));
+        gmax = fmaxf(gmax, __shfl_xor_sync(0xffffffffu, gmax, o));
+    }
+    if ((threadIdx.x & 31) == 0) {
+        if (qmax > 0.0f) atomicMax(bounds, __float_as_uint(qmax));
+        if (gmax > 0.0f) atomicMax(bounds + 1, __float_as_uint(gmax));
+    }
+}
+
+// The finish pass: element i of the sums (layout: g_rgba, or g_rgb | g_alpha | g_bg_rgb) -> fp32, written (`zero`) or added into
+// the caller's gradient.  Non-finite bits give what an fp32 sum of the contributions gives: NaN if a NaN or both infinities were
+// added, else the infinity.  seg1 / seg2: first elements of g_alpha and g_bg_rgb in the sums (factored; G otherwise).
+__global__ void __launch_bounds__(256)
+mpi_bwd_det_finish_kernel(const DetAcc da, float* __restrict__ g0, float* __restrict__ g1, float* __restrict__ g2, size_t G, size_t seg1,
+                          size_t seg2, size_t tex, bool factored, bool zero) {
+    const DetUnit ua = det_unit(__uint_as_float(__ldg(da.bounds)), da.k_a);
+    const DetUnit urgb = det_unit(0.5f * __uint_as_float(__ldg(da.bounds + 1)), da.k_rgb);
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < G; i += (size_t)gridDim.x * blockDim.x) {
+        const bool alpha = factored ? (i >= seg1 && i < seg2) : (i / tex) % 4 == 3;
+        const uint32_t nf = (__ldcs(da.nf + (i >> 3)) >> ((i & 7) * 4)) & 7u;
+        float x;
+        if (nf) {
+            x = (nf & 4u) || nf == 3u ? __int_as_float(0x7fffffff) : nf == 1u ? INFINITY : -INFINITY;
+        } else {
+            // RN to fp32, then an exact power-of-two scale in two normal steps (a result below the normal range rounds once more)
+            const int ue = alpha ? ua.ue : urgb.ue, h = ue / 2;
+            x = __ll2float_rn((long long)__ldcs(da.acc + i));
+            x = __fmul_rn(__fmul_rn(x, __uint_as_float((unsigned)(127 + h) << 23)), __uint_as_float((unsigned)(127 + ue - h) << 23));
+        }
+        float* dst = i < seg1 ? g0 + i : i < seg2 ? g1 + (i - seg1) : g2 + (i - seg2);
+        *dst = zero ? x : *dst + x;
     }
 }
 
@@ -605,8 +704,8 @@ static int zero_grads(const RenderParams& p, cudaStream_t st) {
     return GMPI_OK;
 }
 
-// Two-pass direct backward (any shape, no saved state).
-static int launch_bwd_direct(RenderParams p, cudaStream_t st, bool zero) {
+// Two-pass direct backward (any shape, no saved state).  da: the deterministic variant, adding into da's sums.
+static int launch_bwd_direct(RenderParams p, cudaStream_t st, bool zero, const DetAcc* da = nullptr) {
     if (zero && (p.options & GMPI_ZERO_GRAD)) {
         int rc = zero_grads(p, st);
         if (rc) return rc;
@@ -626,6 +725,14 @@ static int launch_bwd_direct(RenderParams p, cudaStream_t st, bool zero) {
     dim3 grid((p.W + tile_w - 1) / tile_w, (p.H + tile_h - 1) / tile_h, p.V);
     if (grid.y > 65535) return fail(GMPI_ERR_UNSUPPORTED, "image height %d too large", p.H);
     if (p.V > 65535) return fail(GMPI_ERR_UNSUPPORTED, "V=%d views exceed one launch of the direct kernel (65535); split the batch", p.V);
+    if (da) {
+        void (*kernel)(const RenderParams, const int, const int, const DetAcc) =
+            (p.options & GMPI_ALIGN_CORNERS) ? mpi_bwd_direct_det_kernel<true> : mpi_bwd_direct_det_kernel<false>;
+        GMPI_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        kernel<<<grid, block, smem, st>>>(p, tile_w, tile_h, *da);
+        GMPI_CUDA_OK(cudaGetLastError());
+        return GMPI_OK;
+    }
     void (*kernel)(const RenderParams, const int, const int) =
         (p.options & GMPI_ALIGN_CORNERS) ? mpi_bwd_direct_kernel<true> : mpi_bwd_direct_kernel<false>;
     GMPI_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -644,16 +751,19 @@ static cudaError_t launch_bwd_box(BwdBoxKernel kernel, const RenderParams& p, co
     return cudaSuccess;
 }
 
-// Backward: the staged box kernel when the forward saved the transmittance, the staged forward would be launched (fwd_why) and
-// the backward's own conditions hold (16-byte aligned gradient and transmittance bases, W % 4 == 0, V*N < 2^31), else the direct kernel.
-static int launch_bwd(RenderParams p, cudaStream_t st) {
-    int rc = check_params(p, true);
-    if (rc) return rc;
+// Backward kernel choice: the staged box kernel when the forward saved the transmittance, the staged forward would be launched
+// (fwd_why) and the backward's own conditions hold (16-byte aligned gradient and transmittance bases, W % 4 == 0, V*N < 2^31), else
+// the direct kernel.  The deterministic backward makes the same choice from the caller's descriptor.
+static bool bwd_uses_box(const RenderParams& p) {
     const bool fac = p.alpha != nullptr;
     const bool grads_aligned = fac ? aligned16(p.g_rgb) && aligned16(p.g_alpha) && (!p.g_bg_rgb || aligned16(p.g_bg_rgb)) : aligned16(p.g_rgba);
-    if (!(p.transmittance && fwd_why(p) == 0 && grads_aligned && p.W % 4 == 0 && aligned16(p.transmittance) &&
-          (size_t)p.V * p.N < ((size_t)1 << 31)))
-        return launch_bwd_direct(p, st, true);
+    return p.transmittance && fwd_why(p) == 0 && grads_aligned && p.W % 4 == 0 && aligned16(p.transmittance) &&
+           (size_t)p.V * p.N < ((size_t)1 << 31);
+}
+
+// The box backward of a checked call.  da: the deterministic variant (its sums were zeroed by the caller; no GMPI_ZERO_GRAD here).
+static int launch_bwd_box(RenderParams p, cudaStream_t st, const DetAcc* da) {
+    int rc = GMPI_OK;
     if (p.V == 0) return (p.options & GMPI_ZERO_GRAD) ? zero_grads(p, st) : GMPI_OK;
     p.eye0 = p.eye;
     if (p.view_group < 1) p.view_group = 1;
@@ -666,13 +776,117 @@ static int launch_bwd(RenderParams p, cudaStream_t st) {
     const int tiles_x = (p.W + kTileW - 1) / kTileW, tiles_y = (p.H + kBwdTileH - 1) / kBwdTileH;
     const long n_tiles = (long)tiles_x * tiles_y * p.V;
     const int grid = (int)(n_tiles < sms ? n_tiles : sms);
-    const bool ac = (p.options & GMPI_ALIGN_CORNERS) != 0;
+    const bool ac = (p.options & GMPI_ALIGN_CORNERS) != 0, fac = p.alpha != nullptr;
+    if (da) {
+        const auto kernel = fac ? (ac ? mpi_bwd_box_det_kernel<true, true> : mpi_bwd_box_det_kernel<false, true>)
+                                : (ac ? mpi_bwd_box_det_kernel<true, false> : mpi_bwd_box_det_kernel<false, false>);
+        GMPI_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBwdSmem));
+        kernel<<<grid, kBwdThreads, kBwdSmem, st>>>(p, maps, tiles_x, tiles_y, *da);
+        GMPI_CUDA_OK(cudaGetLastError());
+        return GMPI_OK;
+    }
     if ((p.options & GMPI_ZERO_GRAD) && (rc = zero_grads(p, st)) != 0) return rc;
     // (not a table: instantiating the four kernels in table order changes the machine code ptxas gives the expanded ones)
     const BwdBoxKernel kernel = fac ? (ac ? mpi_bwd_box_kernel<true, true> : mpi_bwd_box_kernel<false, true>)
                                     : (ac ? mpi_bwd_box_kernel<true, false> : mpi_bwd_box_kernel<false, false>);
     cudaError_t e = launch_bwd_box(kernel, p, maps, grid, tiles_x, tiles_y, st);
     GMPI_CUDA_OK(e);
+    GMPI_CUDA_OK(cudaGetLastError());
+    return GMPI_OK;
+}
+
+static int launch_bwd(RenderParams p, cudaStream_t st) {
+    int rc = check_params(p, true);
+    if (rc) return rc;
+    return bwd_uses_box(p) ? launch_bwd_box(p, st, nullptr) : launch_bwd_direct(p, st, true);
+}
+
+// ---- deterministic backward (DetAcc, DESIGN.md section 4.3) ----
+// Scratch: a 256-byte header (the pre-pass's two bounds), the int64 sums of the G gradient elements (in the order g_rgba, or
+// g_rgb | g_alpha | g_bg_rgb), then four non-finite bits per element.
+struct DetLayout {
+    size_t G, seg1, seg2, nf_off, bytes;     // seg1, seg2: first elements of g_alpha and g_bg_rgb (factored; G otherwise)
+};
+constexpr size_t kDetHeaderBytes = 256;
+constexpr int kDetMinFixBits = 24;
+
+static int det_layout(const RenderParams& p, DetLayout& L) {
+    if (p.M < 1 || p.V < 0 || p.N < 1 || p.Ht < 1 || p.Wt < 1 || p.H < 1 || p.W < 1)
+        return fail(GMPI_ERR_INVALID_ARGUMENT, "bad sizes M=%d V=%d N=%d Ht=%d Wt=%d H=%d W=%d", p.M, p.V, p.N, p.Ht, p.Wt, p.H, p.W);
+    const double tex = (double)p.Ht * p.Wt, M = p.M, N = p.N;
+    const double G = p.alpha ? M * 3 * tex + M * N * tex + (p.bg_rgb ? M * 3 * tex : 0.0) : M * N * 4 * tex;
+    if (G * 9 > 0x1p62) return fail(GMPI_ERR_UNSUPPORTED, "%.0f gradient elements exceed the deterministic scratch's range", G);
+    const size_t t = (size_t)p.Ht * p.Wt;
+    if (p.alpha) {
+        L.seg1 = (size_t)p.M * 3 * t;
+        L.seg2 = L.seg1 + (size_t)p.M * p.N * t;
+        L.G = L.seg2 + (p.bg_rgb ? (size_t)p.M * 3 * t : 0);
+    } else {
+        L.G = L.seg1 = L.seg2 = (size_t)p.M * p.N * 4 * t;
+    }
+    L.nf_off = kDetHeaderBytes + 8 * L.G;
+    L.bytes = L.nf_off + 4 * ((L.G + 7) / 8);
+    return GMPI_OK;
+}
+
+static int ceil_log2(unsigned long long x) {
+    int b = 0;
+    while (b < 63 && (1ull << b) < x) ++b;
+    return b;
+}
+// Fraction bits k of the unit 2^(E - k) for elements that sum `planes` planes: one (view, plane) adds at most H*W taps of bilinear
+// weight <= 1 to an element, and V bounds the views of one MPI (view2mpi is device memory).  With C = H*W*V*planes taps of
+// |c| <= 2^E w each, a sum is below 2^(k+1) C <= 2^62 in units of 2^(E - k) (DESIGN.md section 4.3): it cannot wrap int64.
+static int det_fix_bits(const RenderParams& p, int planes) {
+    return 61 - ceil_log2((unsigned long long)p.H * p.W) - ceil_log2((unsigned long long)p.V) - ceil_log2((unsigned long long)planes);
+}
+
+static int launch_bwd_deterministic(RenderParams p, void* scratch, size_t scratch_bytes, cudaStream_t st) {
+    int rc = check_params(p, true);
+    if (rc) return rc;
+    DetLayout L;
+    if ((rc = det_layout(p, L)) != 0) return rc;
+    if (!scratch) return fail(GMPI_ERR_INVALID_ARGUMENT, "null scratch pointer (gmpi_mpi_render_bwd_deterministic_scratch_bytes gives its size)");
+    if (!aligned16(scratch)) return fail(GMPI_ERR_INVALID_ARGUMENT, "the scratch must be 16-byte aligned");
+    if (scratch_bytes < L.bytes)
+        return fail(GMPI_ERR_INVALID_ARGUMENT, "scratch of %zu bytes is smaller than the %zu bytes this call needs", scratch_bytes, L.bytes);
+    const bool fac = p.alpha != nullptr;
+    const int k_a = det_fix_bits(p, 1), k_rgb = det_fix_bits(p, fac ? p.N : 1);
+    if (k_rgb < kDetMinFixBits)
+        return fail(GMPI_ERR_UNSUPPORTED, "V=%d views of %dx%d pixels leave %d fraction bits for exact int64 sums (at least %d needed)", p.V,
+                    p.H, p.W, k_rgb, kDetMinFixBits);
+    if (p.V == 0) return (p.options & GMPI_ZERO_GRAD) ? zero_grads(p, st) : GMPI_OK;
+    const bool box = bwd_uses_box(p);
+    char* s = static_cast<char*>(scratch);
+    DetAcc da;
+    da.bounds = reinterpret_cast<uint32_t*>(s);
+    da.acc = reinterpret_cast<unsigned long long*>(s + kDetHeaderBytes);
+    da.base = reinterpret_cast<float*>(da.acc);
+    da.nf = reinterpret_cast<uint32_t*>(s + L.nf_off);
+    da.k_a = k_a;
+    da.k_rgb = k_rgb;
+    // the kernels' gradient pointers address the sums (DetAcc); the finish pass writes the caller's
+    RenderParams q = p;
+    if (fac) {
+        q.g_rgb = da.base;
+        q.g_alpha = da.base + L.seg1;
+        q.g_bg_rgb = p.g_bg_rgb ? da.base + L.seg2 : nullptr;
+    } else {
+        q.g_rgba = da.base;
+    }
+    q.options &= ~GMPI_ZERO_GRAD;
+    GMPI_CUDA_OK(cudaMemsetAsync(scratch, 0, L.bytes, st));
+    q.eye0 = q.eye;
+    if (q.view_group < 1) q.view_group = 1;
+    dim3 bgrid((unsigned)(((size_t)p.H * p.W + 255) / 256), (unsigned)(p.V < 65535 ? p.V : 65535));
+    mpi_bwd_det_bounds_kernel<<<bgrid, 256, 0, st>>>(q, da.bounds);
+    GMPI_CUDA_OK(cudaGetLastError());
+    rc = box ? launch_bwd_box(q, st, &da) : launch_bwd_direct(q, st, false, &da);
+    if (rc) return rc;
+    int sms = 0;
+    if ((rc = device_sms(&sms)) != 0) return rc;
+    mpi_bwd_det_finish_kernel<<<sms * 8, 256, 0, st>>>(da, fac ? p.g_rgb : p.g_rgba, p.g_alpha, p.g_bg_rgb, L.G, L.seg1, L.seg2,
+                                                      (size_t)p.Ht * p.Wt, fac, (p.options & GMPI_ZERO_GRAD) != 0);
     GMPI_CUDA_OK(cudaGetLastError());
     return GMPI_OK;
 }
@@ -883,6 +1097,20 @@ int gmpi_mpi_render_bwd_ex(const gmpi_render_desc* d) {
     int rc = check_desc(d);
     if (rc) return rc;
     return launch_bwd(params_from_desc(d), (cudaStream_t)d->stream);
+}
+
+long long gmpi_mpi_render_bwd_deterministic_scratch_bytes(const gmpi_render_desc* d) {
+    int rc = check_desc(d);
+    if (rc) return -rc;
+    DetLayout L;
+    if ((rc = det_layout(params_from_desc(d), L)) != 0) return -rc;
+    return (long long)L.bytes;
+}
+
+int gmpi_mpi_render_bwd_deterministic_ex(const gmpi_render_desc* d, void* scratch, size_t scratch_bytes) {
+    int rc = check_desc(d);
+    if (rc) return rc;
+    return launch_bwd_deterministic(params_from_desc(d), scratch, scratch_bytes, (cudaStream_t)d->stream);
 }
 
 int gmpi_mpi_check_range(const float* rgba, int M, int N, int Ht, int Wt, uint32_t* flags, void* stream) {

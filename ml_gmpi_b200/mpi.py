@@ -36,7 +36,8 @@ class _RenderFn(torch.autograd.Function):
     The MPI is either expanded (`rgba`) or factored (`rgb`, `alpha`, optional `bg_rgb`); the unused form is None."""
 
     @staticmethod
-    def forward(ctx, rgba, rgb, alpha, bg_rgb, dhw, view2mpi, ray_dir, eye, z_dir, options, flags, view_group, early_stop):
+    def forward(ctx, rgba, rgb, alpha, bg_rgb, dhw, view2mpi, ray_dir, eye, z_dir, options, flags, view_group, early_stop,
+                deterministic):
         lib = _lib.load()
         factored = rgba is None
         ref = alpha if factored else rgba
@@ -59,6 +60,8 @@ class _RenderFn(torch.autograd.Function):
             _lib.check(lib.gmpi_mpi_render_fwd_ex(ctypes.byref(d)))
         ctx.save_for_backward(rgba, rgb, alpha, bg_rgb, dhw, view2mpi, ray_dir, eye, z_dir, trans)
         ctx.options, ctx.view_group = options, view_group
+        # None: torch's global switch, read now (the backward may run on an autograd thread, after the caller changed it)
+        ctx.deterministic = torch.are_deterministic_algorithms_enabled() if deterministic is None else bool(deterministic)
         ctx.set_materialize_grads(False)
         return color, depth
 
@@ -66,7 +69,7 @@ class _RenderFn(torch.autograd.Function):
     @torch.autograd.function.once_differentiable     # raw kernels: a double backward (create_graph=True) must raise, not
     def backward(ctx, g_color, g_depth):             # silently treat the result as constant (the reference's R1 only differentiates D)
         rgba, rgb, alpha, bg_rgb, dhw, view2mpi, ray_dir, eye, z_dir, trans = ctx.saved_tensors
-        none = (None,) * 13
+        none = (None,) * 14
         if not any(ctx.needs_input_grad[:4]):
             return none
         lib = _lib.load()
@@ -94,8 +97,14 @@ class _RenderFn(torch.autograd.Function):
                                view_group=ctx.view_group, rgba=rgba, rgb=rgb, alpha=alpha, bg_rgb=bg_rgb, view2mpi=view2mpi, dhw=dhw,
                                ray_dir=ray_dir, eye=eye, z_dir=z_dir, transmittance=trans, g_color=g_color, g_depth=g_depth,
                                g_rgba=g_rgba, g_rgb=g_rgb, g_bg_rgb=g_bg, g_alpha=g_alpha, stream=_stream_ptr(dev))
-            _lib.check(lib.gmpi_mpi_render_bwd_ex(ctypes.byref(d)))
-        return (g_rgba, g_rgb, g_alpha, g_bg) + (None,) * 9
+            if ctx.deterministic:
+                # bitwise-reproducible gradients from exact int64 sums (8 B of scratch per gradient element)
+                nbytes = _lib.deterministic_scratch_bytes(d)
+                scratch = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+                _lib.check(lib.gmpi_mpi_render_bwd_deterministic_ex(ctypes.byref(d), scratch.data_ptr(), nbytes))
+            else:
+                _lib.check(lib.gmpi_mpi_render_bwd_ex(ctypes.byref(d)))
+        return (g_rgba, g_rgb, g_alpha, g_bg) + (None,) * 10
 
 
 def _mpi_desc(mpi, V, H, W, options):
@@ -165,13 +174,16 @@ def _check_early_stop_without_grad(early_stop, *inputs):
 
 
 def render_views(rgba, dhw, view2mpi, ray_dir, eye, z_dir, *, align_corners=True, check_last_plane=False,
-                 color_minus1_1=False, flags: Optional[torch.Tensor] = None, view_group: int = 1, early_stop: Optional[float] = None):
+                 color_minus1_1=False, flags: Optional[torch.Tensor] = None, view_group: int = 1, early_stop: Optional[float] = None,
+                 deterministic: Optional[bool] = None):
     """Functional form on packed tensors (no list handling, no host sync).
     rgba [M,N,4,Ht,Wt], dhw [M,N,3], view2mpi [V] int32, ray_dir [V,3,H,W], eye/z_dir [V,3].
     Returns (color [V,3,H,W], depth [V,1,H,W]); `flags` (uint32 tensor of 1, int32 storage) is OR-ed into.
     view_group > 1: every view_group consecutive views share one MPI (tile-order hint: L2 reuse, see the C header).
     early_stop = tau in [0, 1): a pixel composites no further plane once its transmittance |T| <= tau (each colour channel moves by
-    at most tau, 2 tau in [-1,1]; see gmpi_render_desc.early_stop).  Forward only: refused when an input requires grad."""
+    at most tau, 2 tau in [-1,1]; see gmpi_render_desc.early_stop).  Forward only: refused when an input requires grad.
+    deterministic: the backward returns bitwise-reproducible gradients (exact int64 sums in a scratch of 8 B per gradient element,
+    gmpi_mpi_render_bwd_deterministic_ex); None follows torch.are_deterministic_algorithms_enabled() at the time of this call."""
     _check_early_stop_without_grad(early_stop, rgba)
     if not rgba.is_cuda:
         raise RuntimeError("ml_gmpi_b200 renders on CUDA devices only (no CPU fallback); got a CPU tensor")
@@ -182,17 +194,17 @@ def render_views(rgba, dhw, view2mpi, ray_dir, eye, z_dir, *, align_corners=True
                                _options(align_corners, check_last_plane, color_minus1_1, early_stop=early_stop))
     _warn_if_direct(_mpi_desc(mpi, V, H, W, options))
     return _RenderFn.apply(*mpi, _as_f32c(dhw), view2mpi, _as_f32c(ray_dir), _as_f32c(eye), _as_f32c(z_dir),
-                           options, flags, int(view_group), early_stop)
+                           options, flags, int(view_group), early_stop, deterministic)
 
 
 def render_views_factored(rgb, alpha, dhw, view2mpi, ray_dir, eye, z_dir, *, bg_rgb=None, align_corners=True,
                           check_last_plane=False, color_minus1_1=False, flags: Optional[torch.Tensor] = None, view_group: int = 1,
-                          early_stop: Optional[float] = None):
+                          early_stop: Optional[float] = None, deterministic: Optional[bool] = None):
     """The same render from the generator's FACTORED output (networks_cond_on_pos_enc.py:950-975,984): one colour image
     rgb [M,3,Ht,Wt] shared by all planes (bg_rgb [M,3,Ht,Wt]: the last plane's own colour under torgba_sep_background) and
     alpha [M,N,1,Ht,Wt] -- what the reference expands to [M,N,4,Ht,Wt] (and copies per view, train.py:553-558,733-738) before
     rendering.  Output identical to render_views on the expanded stack, 4x fewer HBM bytes; differentiable w.r.t. rgb, alpha
-    and bg_rgb (d/d rgb is the sum over the planes that share it).  early_stop: as in render_views (forward only)."""
+    and bg_rgb (d/d rgb is the sum over the planes that share it).  early_stop, deterministic: as in render_views."""
     _check_early_stop_without_grad(early_stop, rgb, alpha, bg_rgb)
     if not alpha.is_cuda:
         raise RuntimeError("ml_gmpi_b200 renders on CUDA devices only (no CPU fallback); got a CPU tensor")
@@ -206,7 +218,7 @@ def render_views_factored(rgb, alpha, dhw, view2mpi, ray_dir, eye, z_dir, *, bg_
                                _options(align_corners, check_last_plane, color_minus1_1, early_stop=early_stop))
     _warn_if_direct(_mpi_desc(mpi, V, H, W, options))
     return _RenderFn.apply(*mpi, _as_f32c(dhw), view2mpi, _as_f32c(ray_dir), _as_f32c(eye), _as_f32c(z_dir),
-                           options, flags, int(view_group), early_stop)
+                           options, flags, int(view_group), early_stop, deterministic)
 
 
 def expand_factored(rgb, alpha, bg_rgb=None):
@@ -286,13 +298,16 @@ class MPI(nn.Module):
          "defer" the geometric flags are still computed inside the render kernel (free) but nothing
                  is scanned or synced; read them later with `.raise_if_flagged()`;
          "off"   like "defer" without the last-plane check.
+    `deterministic`: bitwise-reproducible gradients w.r.t. batch_rgba (see render_views); None (default) follows
+    torch.use_deterministic_algorithms at each forward.
     """
 
-    def __init__(self, align_corners=True, validate: str = "full"):
+    def __init__(self, align_corners=True, validate: str = "full", deterministic: Optional[bool] = None):
         super().__init__()
         assert validate in ("full", "defer", "off"), validate
         self._align_corners = align_corners
         self.validate = validate
+        self.deterministic = deterministic
         self._flags = None
         self._flag_ctx = None
 
@@ -358,7 +373,7 @@ class MPI(nn.Module):
         color, depth = render_views(rgba, batch_dhw.to(dev), view2mpi, ray_dir.to(dev), eye.to(dev), z_dir.to(dev),
                                     align_corners=self._align_corners,
                                     check_last_plane=bool(assert_not_out_of_last_plane) and self.validate != "off",
-                                    flags=flags, view_group=self.view_group_of(batch_ray_dir))
+                                    flags=flags, view_group=self.view_group_of(batch_ray_dir), deterministic=self.deterministic)
         self._flags = flags
         self._flag_ctx = (batch_dhw, eye, c2w_mat, sphere_c)
         if self.validate == "full":
