@@ -285,6 +285,29 @@ int gmpi_mpi_render_bwd_ex(const gmpi_render_desc* desc);
 long long gmpi_mpi_render_bwd_deterministic_scratch_bytes(const gmpi_render_desc* desc);
 int gmpi_mpi_render_bwd_deterministic_ex(const gmpi_render_desc* desc, void* scratch, size_t scratch_bytes);
 
+/*
+ * Opt-in empty-space skipping (forward only).  A texel of plane i of MPI m is EMPTY when its alpha is +0.0 (bit pattern 0; -0.0 and
+ * NaN count as occupied) and its three colour values are finite (factored MPI: the shared rgb texel, or bg_rgb's on the last plane).
+ * The occupancy map holds one bit per 8 x 8 texel block of every (MPI, plane), set when a texel of the block is not empty: per plane
+ * ceil(Ht/8) rows of ceil(ceil(Wt/8)/32) 32-bit words, bit b of word w = block column 32 w + b; planes in the order m * N + i.
+ *
+ * gmpi_mpi_occupancy_bytes: the map's size for desc (its sizes and MPI pointers: rgba, or rgb + alpha), or a negative GMPI_ERR_*.
+ * gmpi_mpi_build_occupancy: fills the map (device memory, 4-byte aligned, at least the size above) from desc's MPI (fp32, or fp16
+ *   under GMPI_MPI_F16) on desc->stream.  For an expanded MPI with desc->flags set it also ORs in the GMPI_FLAG_RGBA_RANGE |
+ *   GMPI_FLAG_ALPHA_RANGE bits that gmpi_mpi_check_range(_f16) would set, from the same pass.
+ * gmpi_mpi_render_fwd_skip_ex: gmpi_mpi_render_fwd_ex, except that the TMA-staged forward arms a (tile, plane) stage without
+ *   loading it when every texel under its box is empty, and composites nothing where its taps fall in that box.  Compositing such a
+ *   box adds fma(+0, finite, x) == x to colour and depth and leaves T alone, so colour, depth, uint8 frames and flags are bitwise
+ *   those of gmpi_mpi_render_fwd_ex whenever no accumulator is -0.0 and T is finite in front of a skipped stage (DESIGN.md section
+ *   4.1: true for every MPI inside the range check's [0, 1]).  The direct kernel takes the request and skips nothing.  Composes with
+ *   the factored MPI, GMPI_MPI_F16, GMPI_EARLY_STOP, cam, view_group, the video outputs and the fused gather; refuses a descriptor
+ *   with transmittance and a map smaller than gmpi_mpi_occupancy_bytes.  The map must describe the MPI as it is now: the callee
+ *   cannot tell a stale map.  None of the three needs a GPU to refuse a call.
+ */
+long long gmpi_mpi_occupancy_bytes(const gmpi_render_desc* desc);
+int gmpi_mpi_build_occupancy(const gmpi_render_desc* desc, void* occ, size_t bytes);
+int gmpi_mpi_render_fwd_skip_ex(const gmpi_render_desc* desc, const void* occ, size_t bytes);
+
 /* Host-buffer form (end-to-end entry point, see gmpi_mpi_render_fwd_host): all pointers of *desc are HOST memory, `stream` is
  * ignored, *flags receives the flag word.  Forward only; supports the factored MPI, cam and the video outputs. */
 int gmpi_mpi_render_host_ex(const gmpi_render_desc* desc, int device);
@@ -357,6 +380,15 @@ int gmpi_debug_set_fwd_stages(int stages);
 /* Test hook: the last GMPI_EARLY_STOP launch on this device (synchronises the device): *skipped = the (tile, plane) stages the
  * staged kernel armed without loading their box, *total = the stages it walked (tiles x N; 0 when the direct kernel ran). */
 int gmpi_debug_fwd_early_stop_stats(unsigned long long* skipped, unsigned long long* total);
+
+/* Test hook: the last gmpi_mpi_render_fwd_skip_ex launch on this device (synchronises the device): *skipped = the (tile, plane)
+ * stages the staged kernel armed empty, *total = the stages it walked (0 when the direct kernel ran). */
+int gmpi_debug_fwd_skip_stats(unsigned long long* skipped, unsigned long long* total);
+
+/* Test hook (host only): the staged producer's box-versus-map test on one plane's map (host memory, the layout of
+ * gmpi_mpi_build_occupancy): 1 when a block under the texels [bx0, bx0 + bw) x [by0, by0 + rows) inside the Ht x Wt texture is
+ * occupied, 0 when the box is empty, a negative GMPI_ERR_* code on bad arguments. */
+int gmpi_debug_box_occupied(const uint32_t* plane_map, int Ht, int Wt, int bx0, int by0, int bw, int rows);
 
 /* Test hook: the ring depth (2 or 3) the expanded staged forward picks on the current device for M MPIs, V views, N planes of
  * Ht x Wt texels and view_group (gmpi_render_desc.view_group); a negative GMPI_ERR_* code on bad arguments. */

@@ -32,6 +32,8 @@ EXPORTS = [
     "gmpi_debug_fwd_early_stop_stats", "gmpi_mpi_zero_async", "gmpi_mpi_alpha_depth_fwd", "gmpi_mpi_alpha_depth_bwd", "gmpi_mpi_apply_shading_fwd", "gmpi_mpi_apply_shading_bwd",
     "gmpi_mpi_render_fwd_plan_ex", "gmpi_mpi_check_range_f16",
     "gmpi_mpi_render_bwd_deterministic_scratch_bytes", "gmpi_mpi_render_bwd_deterministic_ex",
+    "gmpi_mpi_occupancy_bytes", "gmpi_mpi_build_occupancy", "gmpi_mpi_render_fwd_skip_ex", "gmpi_debug_fwd_skip_stats",
+    "gmpi_debug_box_occupied",
 ]
 
 OPT_U8_ROUND_HALF_UP = 16
@@ -156,6 +158,15 @@ def load():
     lib.gmpi_mpi_render_bwd_deterministic_scratch_bytes.argtypes = [ctypes.POINTER(RenderDesc)]
     lib.gmpi_mpi_render_bwd_deterministic_ex.restype = i
     lib.gmpi_mpi_render_bwd_deterministic_ex.argtypes = [ctypes.POINTER(RenderDesc), vp, ctypes.c_size_t]
+    lib.gmpi_mpi_occupancy_bytes.restype = ll
+    lib.gmpi_mpi_occupancy_bytes.argtypes = [ctypes.POINTER(RenderDesc)]
+    for fn in (lib.gmpi_mpi_build_occupancy, lib.gmpi_mpi_render_fwd_skip_ex):
+        fn.restype = i
+        fn.argtypes = [ctypes.POINTER(RenderDesc), vp, ctypes.c_size_t]
+    lib.gmpi_debug_fwd_skip_stats.restype = i
+    lib.gmpi_debug_fwd_skip_stats.argtypes = [vp, vp]
+    lib.gmpi_debug_box_occupied.restype = i
+    lib.gmpi_debug_box_occupied.argtypes = [vp] + [i] * 6
     if lib.gmpi_abi_version() != ABI_VERSION:
         raise GmpiLibraryError(f"ABI mismatch: library {lib.gmpi_abi_version()} != binding {ABI_VERSION}; rebuild")
     _lib = lib
@@ -170,6 +181,14 @@ def check(rc: int):
 def deterministic_scratch_bytes(desc: RenderDesc) -> int:
     """Bytes of scratch gmpi_mpi_render_bwd_deterministic_ex needs for `desc` (raises on a bad descriptor)."""
     n = load().gmpi_mpi_render_bwd_deterministic_scratch_bytes(ctypes.byref(desc))
+    if n < 0:
+        check(-n)
+    return n
+
+
+def occupancy_bytes(desc: RenderDesc) -> int:
+    """Bytes of the occupancy map of the MPI `desc` describes (gmpi_mpi_occupancy_bytes; raises on a bad descriptor)."""
+    n = load().gmpi_mpi_occupancy_bytes(ctypes.byref(desc))
     if n < 0:
         check(-n)
     return n

@@ -389,6 +389,59 @@ constexpr uint32_t kAllConsumers = (1u << kConsWarps) - 1u;
 static_assert(kStages <= kStopSlots, "stop-word slots must cover the producer's lead");
 __device__ unsigned long long g_early_stop_skipped;   // test hook: stages armed without copies (gmpi_debug_fwd_early_stop_stats)
 
+// Empty-space skipping (kSkip, forward only, the kernels of mpi_skip.cu).  The occupancy map has one bit per kOccB x kOccB texel
+// block of every (MPI, plane), set when a texel of the block is not empty: alpha is not +0 (bit pattern 0), or a colour value is
+// not finite.  A plane's map is `rows` block rows of `words` 32-bit words (bit b of word w: block column 32 w + b).  Compositing a
+// box whose texels are all empty adds fma(+0, finite, x) == x to every sum and leaves T alone, so the producer arms such a stage
+// without copies and marks it kSelEmpty; consumers composite nothing where their taps fall in the box (DESIGN.md section 4.1).
+constexpr int kOccB = 8;
+constexpr int kSelEmpty = 1 << 24;      // StageMeta::sel: the stage's box is empty and was not loaded
+struct OccMap {
+    const uint32_t* bits;           // [M*N][rows][words]
+    int words, rows;
+    unsigned long long* skipped;    // stats: stages armed empty (gmpi_debug_fwd_skip_stats)
+};
+__host__ __device__ __forceinline__ int occ_words(int Wt) { return ((Wt + kOccB - 1) / kOccB + 31) / 32; }
+__host__ __device__ __forceinline__ int occ_rows(int Ht) { return (Ht + kOccB - 1) / kOccB; }
+
+// Lane `lane`'s part of the box-versus-map test: the OR of the map bits of one plane under the texels [bx0, bx0 + bw) x
+// [by0, by0 + rows) that lie inside the texture (TMA zero-fills the rest).  The (block row, word) pairs under the box are dealt to
+// lanes lane, lane + 32, ... (a staged box covers at most 7 block rows of 2 words).  The box is empty iff no lane returns a bit.
+// (Host-evaluable: gmpi_debug_box_occupied, tests/test_skip_empty.py.)
+__host__ __device__ __forceinline__ uint32_t occ_box_bits(const uint32_t* plane, int Ht, int Wt, int words, int bx0, int by0, int bw,
+                                                          int rows, int lane) {
+    const int x0 = max(bx0, 0), x1 = min(bx0 + bw - 1, Wt - 1), y0 = max(by0, 0), y1 = min(by0 + rows - 1, Ht - 1);
+    if (x0 > x1 || y0 > y1) return 0u;
+    const int c0 = x0 / kOccB, c1 = x1 / kOccB, r0 = y0 / kOccB, r1 = y1 / kOccB;
+    const int w0 = c0 >> 5, nw = (c1 >> 5) - w0 + 1, n = (r1 - r0 + 1) * nw;
+    uint32_t acc = 0u;
+    for (int l = lane; l < n; l += 32) {
+        const int r = r0 + l / nw, w = w0 + l % nw;
+        const int lo = max(c0 - 32 * w, 0), hi = min(c1 - 32 * w, 31);
+#ifdef __CUDA_ARCH__
+        const uint32_t word = __ldg(plane + (size_t)r * words + w);
+#else
+        const uint32_t word = plane[(size_t)r * words + w];
+#endif
+        acc |= word & (0xffffffffu >> (31 - hi)) & (0xffffffffu << lo);
+    }
+    return acc;
+}
+
+// The fast body's in-box vote (BoxTaps::locate) for a stage the producer marked empty: every footprint of the warp has its north-west
+// tap at 0 <= rx <= bw2, 0 <= ry <= rows2 relative to the box.
+__device__ __forceinline__ bool box_vote(int cx, int cy, int bw2, int rows2, const CoordPairs& c) {
+    const f2 magic = splat(kFloorMagic);
+    bool inbox = true;
+#pragma unroll
+    for (int P = 0; P < kPairs; ++P) {
+        const f2 tx = add2_rm(c.ix[P], magic), ty = add2_rm(c.iy[P], magic);
+        inbox = inbox && (unsigned)(__float_as_int(tx.x) - cx) <= (unsigned)bw2 && (unsigned)(__float_as_int(tx.y) - cx) <= (unsigned)bw2 &&
+                (unsigned)(__float_as_int(ty.x) - cy) <= (unsigned)rows2 && (unsigned)(__float_as_int(ty.y) - cy) <= (unsigned)rows2;
+    }
+    return __all_sync(0xffffffffu, inbox);
+}
+
 // consumer warps of a tile at row py0 without a row inside an image of H rows (they only keep the ring going)
 __device__ __forceinline__ uint32_t idle_consumer_warps(int py0, int H) {
     const int live = (H - py0 + kPairs - 1) / kPairs;
@@ -401,10 +454,11 @@ __device__ __forceinline__ uint32_t idle_consumer_warps(int py0, int H) {
 // kFact: factored MPI (compile time: a run-time test of p.alpha in this loop cost the forward 1 %, the producer's per-stage latency
 // being on the critical path of a shallow ring).
 // E: the MPI's element type (the ring holds boxes of it).
-template <bool kAlignCorners, class Ring, bool kFact, bool kES = false, class E = float>
+// kSkip: empty-space skipping against the occupancy map `occ` (forward only, see OccMap).
+template <bool kAlignCorners, class Ring, bool kFact, bool kES = false, class E = float, bool kSkip = false>
 __device__ __forceinline__ void staged_producer(const RenderParams& p, const TmaMaps& maps, E* s_buf, StageMeta* s_meta,
                                             uint64_t* s_full, uint64_t* s_empty, const TileWalk* s_walk, int lane,
-                                            int n_stages = Ring::kRingStages, uint32_t* s_stop = nullptr) {
+                                            int n_stages = Ring::kRingStages, uint32_t* s_stop = nullptr, OccMap occ = OccMap{}) {
     constexpr bool kReverse = Ring::kReverse;
     constexpr int kStride = Ring::kStride;      // floats per ring stage
     constexpr int kTileH = Ring::kTileRows, kMaxBH = Ring::kBoxMaxH, kStageFloats = Ring::kPlaneFloats;
@@ -420,6 +474,7 @@ __device__ __forceinline__ void staged_producer(const RenderParams& p, const Tma
     int p_stage = 0;
     uint32_t p_phase = 0;
     uint32_t n_skipped = 0;      // kES: stages armed without copies
+    uint32_t n_empty = 0;        // kSkip: stages armed empty
     TileXY txy;
     for (int j = 0; s_walk->at(j, txy); ++j) {
         const int v = txy.v, px0 = txy.px0, py0 = txy.py0;
@@ -465,8 +520,20 @@ __device__ __forceinline__ void staged_producer(const RenderParams& p, const Tma
             const int bxs = sizeof(E) == 2 ? (bx0 & ~7) : bx0, sw = staged_width<E>(bw, kWide);   // staged box: origin, width
             const int n_ops = mode == 0 ? (need_h + kRowsPerOp - 1) / kRowsPerOp : 0;
             const int rows = n_ops * kRowsPerOp;
+            // kSkip: only a stage that takes the fast body (mode 0, plane constants in the exact range) may be skipped.  The test covers
+            // the whole box the consumers' in-box test accepts (class width bw, not need_w).  Its map loads are issued before the wait
+            // for a free stage and voted on after it, so that their latency hides behind the wait.  (Probing one plane ahead, which
+            // repeats the box computation, made the producer slower still: DESIGN.md section 4.1.)
+            const bool testable = kSkip && mode == 0 && pc.fast != 0.0f;
+            uint32_t occ_bits = 0u;
+            if (testable) occ_bits = occ_box_bits(occ.bits + ((size_t)m * N + i) * occ.rows * occ.words, Ht, Wt, occ.words, bx0, by0, bw, rows, lane);
             if (Ring::kSleepPolls) mbar_wait_sleep(&s_empty[s], ph ^ 1);
             else mbar_wait(&s_empty[s], ph ^ 1);
+            bool empty = false;
+            if constexpr (kSkip) {
+                empty = testable && !__any_sync(0xffffffffu, occ_bits != 0u);
+                n_empty += empty ? 1u : 0u;
+            }
             bool skip = false;
             if constexpr (kES) {
                 if (ii == 0) {
@@ -476,12 +543,13 @@ __device__ __forceinline__ void staged_producer(const RenderParams& p, const Tma
                     n_skipped += skip ? 1u : 0u;
                 }
             }
-            const int n_copy = skip ? 0 : n_ops;
+            const int n_copy = skip || empty ? 0 : n_ops;
             if (lane == 0) {
                 StageMeta mt;
                 mt.cx = kFloorMagicBits + bx0; mt.cy = kFloorMagicBits + by0;
                 mt.rows2 = rows - 2;
                 mt.sel = bw | (mode << 8) | ((mode == 0 && pc.fast != 0.0f ? (1 << k) : kSelSlow) << 16) | ((bx0 - bxs) << 10);
+                if (kSkip && empty) mt.sel |= kSelEmpty;
                 if constexpr (kReverse) {   // backward: a footprint too magnified for the int32 gradient box (BwdRing::kMagLimit)
                     const int ext_x = min(px0 + kTileW - 1, p.W - 1) - px0, ext_y = min(py0 + kTileH - 1, p.H - 1) - py0;
                     if (Ring::kMagLimit * (xmax - xmin - 1) < ext_x || Ring::kMagLimit * (ymax - ymin - 1) < ext_y) mt.sel &= 0xffff;
@@ -528,6 +596,9 @@ __device__ __forceinline__ void staged_producer(const RenderParams& p, const Tma
     }
     if constexpr (kES) {
         if (lane == 0 && n_skipped) atomicAdd(&g_early_stop_skipped, (unsigned long long)n_skipped);
+    }
+    if constexpr (kSkip) {
+        if (lane == 0 && n_empty) atomicAdd(occ.skipped, (unsigned long long)n_empty);
     }
 }
 
@@ -577,9 +648,10 @@ __device__ __forceinline__ void store_tile_pixels(const RenderParams& p, int v, 
 
 // Body of the staged forward kernels.  kES: early stop (mpi_fwd_early_stop_kernel; s_stop is its stop-word ring, see kStopSlots).
 // E: the MPI's element type (__half: GMPI_MPI_F16, the ring's boxes are fp16, each stage half the bytes).
-template <bool kAlignCorners, bool kEmitT, bool kFactored, bool kES, class E = float>
+// kSkip: empty-space skipping against `occ` (the kernels of mpi_skip.cu; forward only).
+template <bool kAlignCorners, bool kEmitT, bool kFactored, bool kES, class E = float, bool kSkip = false>
 __device__ __forceinline__ void fwd_staged_body(const RenderParams& p, const TmaMaps& maps, const int tiles_x, const int ring_stages,
-                                                uint32_t* s_stop) {
+                                                uint32_t* s_stop, OccMap occ = OccMap{}) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     E* s_buf = reinterpret_cast<E*>(smem_raw);   // the ring starts the dynamic segment (1024-byte aligned)
     constexpr bool kHalf = sizeof(E) == 2;
@@ -617,7 +689,8 @@ __device__ __forceinline__ void fwd_staged_body(const RenderParams& p, const Tma
     const size_t img = (size_t)p.H * p.W;
 
     if (warp == kConsWarps) {
-        staged_producer<kAlignCorners, Ring, kFactored, kES, E>(p, maps, s_buf, s_meta, s_full, s_empty, &s_walk, lane, n_stages, s_stop);
+        staged_producer<kAlignCorners, Ring, kFactored, kES, E, kSkip>(p, maps, s_buf, s_meta, s_full, s_empty, &s_walk, lane, n_stages,
+                                                                        s_stop, occ);
     } else {
         // ================================ consumer warps ================================
         // warp w owns rows kPairs*w .. kPairs*w + kPairs-1 of the tile; a lane owns x = lane and lane+32 on each of them
@@ -697,7 +770,9 @@ __device__ __forceinline__ void fwd_staged_body(const RenderParams& p, const Tma
                 const int sel = mt.sel;                  // warp-uniform; the producer already folded mode and plane range in
                 bool done = warp_stopped;                // a stopped warp only waits on and releases the stage
                 if (warp_fast && !done) {
-                    if (Ring::kWideFact) {               // factored: two widths, both with bank-aligned row pitches
+                    if (kSkip && (sel & kSelEmpty)) {    // empty box, not loaded: done when every tap of the warp falls in it
+                        done = box_vote(mt.cx, mt.cy, (sel & 0xff) - 2, mt.rows2, cc);
+                    } else if (Ring::kWideFact) {        // factored: two widths, both with bank-aligned row pitches
                         if (sel & (1 << 20)) done = sample_pairs<kWideBW, kAOff, kES, E>(sb, mt.cx, mt.cy, mt.rows2, cc, T, cr, cg, cb, cws, tau);
                         else if (sel & (1 << 17)) done = sample_pairs<64, kAOff, kES, E>(sb, mt.cx, mt.cy, mt.rows2, cc, T, cr, cg, cb, cws, tau);
                     } else {                             // most frequent classes first (FFHQ poses: 72 > 64 > 80 >> 56, 88)
@@ -728,6 +803,9 @@ __device__ __forceinline__ void fwd_staged_body(const RenderParams& p, const Tma
                         const float fx = floorf(tc.ix), fy = floorf(tc.iy);
                         const float rxx = fx - fbx0, ryy = fy - fby0;
                         float r, g, b, a;
+                        if (kSkip && (mt.sel & kSelEmpty) && rxx >= 0.0f && rxx <= fbw2 && ryy >= 0.0f && ryy <= fbh2) {
+                            continue;   // taps in the empty box: contributes exactly nothing
+                        }
                         if (!kFactored && mode == 0 && rxx >= 0.0f && rxx <= fbw2 && ryy >= 0.0f && ryy <= fbh2) {
                             const float wx1 = tc.ix - fx, wy1 = tc.iy - fy;
                             const float wx0 = 1.0f - wx1, wy0 = 1.0f - wy1;

@@ -3,6 +3,7 @@
 // Replaces gmpi/core/mpi.py MPI.forward (:308-436) + homography (:26-153) and their autograd.
 // DESIGN.md describes the data layout, each kernel and its roofline.
 #include <cuda_runtime.h>
+#include <dlfcn.h>
 #include <stdarg.h>
 #include <stdint.h>
 #include <math.h>
@@ -11,6 +12,7 @@
 
 #include <atomic>
 #include <mutex>
+#include <string>
 
 #include "../../include/gmpi_mpi_render.h"
 #include "mpi_common.cuh"
@@ -623,20 +625,97 @@ static constexpr void (*kFwdDirectF16Kernels[2][2])(const RenderParams) = {
     {mpi_fwd_direct_f16_kernel<false>, mpi_fwd_direct_f16_kernel<true>},
     {mpi_fwd_direct_early_stop_f16_kernel<false>, mpi_fwd_direct_early_stop_f16_kernel<true>}};
 
-// fac: the kernel's kFactored; f16: its MPI is fp16 (the rings of FwdRingF16 / FwdRingWideF16)
-static cudaError_t launch_fwd_staged(StagedFwdKernel kernel, bool fac, const RenderParams& p, const TmaMaps& maps, int grid, int tiles_x,
-                                     int tiles_y, int stages, cudaStream_t st, bool f16 = false) {
+// Dynamic shared memory of a staged forward kernel: its ring and the plane-constant table.  fac: the kernel's kFactored; f16: its MPI
+// is fp16 (the rings of FwdRingF16 / FwdRingWideF16)
+static size_t fwd_staged_smem(bool fac, int stages, bool f16) {
     const size_t ring = f16 ? (size_t)(fac ? kStages * FwdRingWideF16::kPlaneFloats : stages * FwdRingF16::kPlaneFloats) * 2
                             : (size_t)(fac ? kStages * kWideStageFloats : stages * kStageFloats) * 4;
-    const size_t smem = ring + (size_t)kMaxPlanesStaged * 32;
+    return ring + (size_t)kMaxPlanesStaged * 32;
+}
+
+static cudaError_t launch_fwd_staged(StagedFwdKernel kernel, bool fac, const RenderParams& p, const TmaMaps& maps, int grid, int tiles_x,
+                                     int tiles_y, int stages, cudaStream_t st, bool f16 = false) {
+    const size_t smem = fwd_staged_smem(fac, stages, f16);
     cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     kernel<<<grid, kStagedThreads, smem, st>>>(p, maps, tiles_x, tiles_y, stages);
     return cudaSuccess;
 }
 
-// Forward launch for a filled RenderParams.
-static int launch_fwd(RenderParams p, cudaStream_t st) {
+// ---- opt-in empty-space skipping: the kernels of mpi_skip.cu live in a module of their own, libgmpi_mpi_render_skip.fatbin next to
+// this library, so that this library's kernels keep their machine code.  Loaded on first use (a context-independent library: the
+// runtime loads it into each device's context when a kernel of it first runs there).
+struct SkipModule {
+    cudaLibrary_t lib = nullptr;
+    cudaKernel_t fwd[2][2][2][2];           // [f16][align_corners][factored][early_stop]
+    cudaKernel_t occ_exp[2], occ_fac[2];    // [f16]
+};
+static SkipModule g_skip;
+static std::mutex g_skip_mutex;
+static std::atomic<unsigned long long> g_skip_total{0};    // stages the last skipping launch walked (gmpi_debug_fwd_skip_stats)
+
+static int skip_module(const SkipModule** out) {
+    std::lock_guard<std::mutex> lock(g_skip_mutex);
+    if (!g_skip.lib) {
+        Dl_info info;
+        if (!dladdr(reinterpret_cast<void*>(&gmpi_abi_version), &info) || !info.dli_fname)
+            return fail(GMPI_ERR_CUDA, "cannot locate the library file (dladdr)");
+        std::string path(info.dli_fname);
+        path = path.substr(0, path.find_last_of('/') + 1) + "libgmpi_mpi_render_skip.fatbin";
+        SkipModule m;
+        const cudaError_t e = cudaLibraryLoadFromFile(&m.lib, path.c_str(), nullptr, nullptr, 0, nullptr, nullptr, 0);
+        if (e != cudaSuccess) return fail(GMPI_ERR_CUDA, "loading %s failed: %s", path.c_str(), cudaGetErrorString(e));
+        char name[64];
+        for (int h = 0; h < 2; ++h) {
+            for (int a = 0; a < 2; ++a)
+                for (int x = 0; x < 2; ++x)
+                    for (int s = 0; s < 2; ++s) {
+                        snprintf(name, sizeof(name), "gmpi_fwd_skip_a%d_x%d_e%d_%s", a, x, s, h ? "f16" : "f32");
+                        GMPI_CUDA_OK(cudaLibraryGetKernel(&m.fwd[h][a][x][s], m.lib, name));
+                    }
+            GMPI_CUDA_OK(cudaLibraryGetKernel(&m.occ_exp[h], m.lib, h ? "gmpi_occ_expanded_f16" : "gmpi_occ_expanded_f32"));
+            GMPI_CUDA_OK(cudaLibraryGetKernel(&m.occ_fac[h], m.lib, h ? "gmpi_occ_factored_f16" : "gmpi_occ_factored_f32"));
+        }
+        g_skip = m;
+    }
+    *out = &g_skip;
+    return GMPI_OK;
+}
+
+// The module's stage counter on the current device, zeroed on st; `total` stages walked (0: the direct kernel, which skips nothing).
+static int reset_skip_stats(const SkipModule* sm, unsigned long long total, cudaStream_t st, unsigned long long** counter) {
+    size_t bytes = 0;
+    GMPI_CUDA_OK(cudaLibraryGetGlobal(reinterpret_cast<void**>(counter), &bytes, sm->lib, "gmpi_skip_empty_stages"));
+    GMPI_CUDA_OK(cudaMemsetAsync(*counter, 0, sizeof(unsigned long long), st));
+    g_skip_total.store(total, std::memory_order_relaxed);
+    return GMPI_OK;
+}
+
+// Occupancy map: M*N planes of occ_rows(Ht) block rows of occ_words(Wt) words.  Checks what the map's size and build read.
+static int occ_bytes(const RenderParams& p, size_t* bytes) {
+    const bool factored = p.alpha != nullptr || p.rgb != nullptr;
+    if (factored ? (!p.alpha || !p.rgb || p.rgba) : !p.rgba)
+        return fail(GMPI_ERR_INVALID_ARGUMENT, "null input pointer (MPI: pass rgba, or rgb + alpha)");
+    if (p.M < 1 || p.N < 1 || p.Ht < 1 || p.Wt < 1)
+        return fail(GMPI_ERR_INVALID_ARGUMENT, "bad sizes M=%d N=%d Ht=%d Wt=%d", p.M, p.N, p.Ht, p.Wt);
+    if ((size_t)p.Ht * p.Wt > (size_t)0x7fffffff)
+        return fail(GMPI_ERR_UNSUPPORTED, "texture of %dx%d texels exceeds 2^31 elements per channel", p.Ht, p.Wt);
+    *bytes = (size_t)p.M * p.N * occ_rows(p.Ht) * occ_words(p.Wt) * sizeof(uint32_t);
+    return GMPI_OK;
+}
+
+static int check_occ_arg(const RenderParams& p, const void* occ, size_t bytes) {
+    size_t need = 0;
+    int rc = occ_bytes(p, &need);
+    if (rc) return rc;
+    if (!occ) return fail(GMPI_ERR_INVALID_ARGUMENT, "null occupancy map (gmpi_mpi_occupancy_bytes gives its size)");
+    if ((uintptr_t)occ & 3) return fail(GMPI_ERR_INVALID_ARGUMENT, "the occupancy map must be 4-byte aligned");
+    if (bytes < need) return fail(GMPI_ERR_INVALID_ARGUMENT, "occupancy map of %zu bytes is smaller than the %zu bytes of this MPI", bytes, need);
+    return GMPI_OK;
+}
+
+// Forward launch for a filled RenderParams.  occ: empty-space skipping against this occupancy map (checked by the caller).
+static int launch_fwd(RenderParams p, cudaStream_t st, const uint32_t* occ = nullptr) {
     int rc = check_params(p, false);
     if (rc) return rc;
     if (!p.flags) return fail(GMPI_ERR_INVALID_ARGUMENT, "null flags pointer");
@@ -670,6 +749,20 @@ static int launch_fwd(RenderParams p, cudaStream_t st) {
             const long n_tiles = (long)tiles_x * tiles_y * p.V;
             const int grid = (int)(n_tiles < sms ? n_tiles : sms);
             if (es && (rc = reset_early_stop_stats((unsigned long long)n_tiles * p.N, st)) != 0) return rc;
+            if (occ) {
+                const SkipModule* sm = nullptr;
+                OccMap om{occ, occ_words(p.Wt), occ_rows(p.Ht), nullptr};
+                if ((rc = skip_module(&sm)) != 0 || (rc = reset_skip_stats(sm, (unsigned long long)n_tiles * p.N, st, &om.skipped)) != 0)
+                    return rc;
+                const void* kernel = sm->fwd[f16][ac][fac][es];
+                const size_t smem = fwd_staged_smem(fac, stages, f16);
+                GMPI_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+                cudaLaunchConfig_t cfg = {};
+                cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kStagedThreads); cfg.dynamicSmemBytes = smem; cfg.stream = st;
+                void* args[] = {&p, &maps, (void*)&tiles_x, (void*)&tiles_y, (void*)&stages, &om};
+                GMPI_CUDA_OK(cudaLaunchKernelExC(&cfg, kernel, args));
+                return GMPI_OK;
+            }
             const StagedFwdKernel kernel = f16 ? kFwdStagedF16Kernels[es][ac][fac] : es ? kFwdEarlyStopKernels[ac][fac] : kFwdStagedKernels[ac][emit][fac];
             cudaError_t e = launch_fwd_staged(kernel, fac, p, maps, grid, tiles_x, tiles_y, stages, st, f16);
             GMPI_CUDA_OK(e);
@@ -685,6 +778,11 @@ static int launch_fwd(RenderParams p, cudaStream_t st) {
     if (grid.y > 65535) return fail(GMPI_ERR_UNSUPPORTED, "image height %d too large", p.H);
     if (p.V > 65535) return fail(GMPI_ERR_UNSUPPORTED, "V=%d views exceed one launch of the direct kernel (65535); split the batch", p.V);
     if (es && (rc = reset_early_stop_stats(0, st)) != 0) return rc;    // the direct kernel loads per pixel: no stages to skip
+    if (occ) {     // nor empty ones: the direct kernel takes the request and composites every plane, which gives the same output
+        const SkipModule* sm = nullptr;
+        unsigned long long* counter = nullptr;
+        if ((rc = skip_module(&sm)) != 0 || (rc = reset_skip_stats(sm, 0, st, &counter)) != 0) return rc;
+    }
     void (*kernel)(const RenderParams) = f16 ? kFwdDirectF16Kernels[es][ac] : kFwdDirectKernels[es][ac];
     if (smem > 48 * 1024) GMPI_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     kernel<<<grid, block, smem, st>>>(p);
@@ -1111,6 +1209,81 @@ int gmpi_mpi_render_bwd_deterministic_ex(const gmpi_render_desc* d, void* scratc
     int rc = check_desc(d);
     if (rc) return rc;
     return launch_bwd_deterministic(params_from_desc(d), scratch, scratch_bytes, (cudaStream_t)d->stream);
+}
+
+long long gmpi_mpi_occupancy_bytes(const gmpi_render_desc* d) {
+    int rc = check_desc(d);
+    if (rc) return -rc;
+    size_t bytes = 0;
+    if ((rc = occ_bytes(params_from_desc(d), &bytes)) != 0) return -rc;
+    return (long long)bytes;
+}
+
+int gmpi_mpi_build_occupancy(const gmpi_render_desc* d, void* occ, size_t bytes) {
+    int rc = check_desc(d);
+    if (rc) return rc;
+    const RenderParams p = params_from_desc(d);
+    if ((rc = check_occ_arg(p, occ, bytes)) != 0) return rc;
+    const int words = occ_words(p.Wt), rows = occ_rows(p.Ht);
+    if (rows > 65535) return fail(GMPI_ERR_UNSUPPORTED, "Ht=%d exceeds the occupancy build's grid (%d texel rows)", p.Ht, 65535 * kOccB);
+    const SkipModule* sm = nullptr;
+    if ((rc = skip_module(&sm)) != 0) return rc;
+    const bool f16 = (p.options & GMPI_MPI_F16) != 0;
+    const int M = p.M, N = p.N, Ht = p.Ht, Wt = p.Wt;
+    cudaLaunchConfig_t cfg = {};
+    cfg.blockDim = dim3(32 * kOccB);
+    cfg.stream = (cudaStream_t)d->stream;
+    uint32_t* map = static_cast<uint32_t*>(occ);
+    if (p.alpha) {
+        cfg.gridDim = dim3(words, rows, M < 65535 ? M : 65535);
+        const void *rgb = p.rgb, *bg = p.bg_rgb, *alpha = p.alpha;
+        void* args[] = {&rgb, &bg, &alpha, &map, (void*)&M, (void*)&N, (void*)&Ht, (void*)&Wt, (void*)&words, (void*)&rows};
+        GMPI_CUDA_OK(cudaLaunchKernelExC(&cfg, sm->occ_fac[f16], args));
+    } else {
+        const long long P = (long long)M * N;
+        if (P > 0x7fffffffLL) return fail(GMPI_ERR_UNSUPPORTED, "%lld planes exceed the occupancy build (2^31)", P);
+        const int planes = (int)P;
+        cfg.gridDim = dim3(words, rows, planes < 65535 ? planes : 65535);
+        const void* rgba = p.rgba;
+        uint32_t* flags = p.flags;      // the range check's bits, from the same loads
+        void* args[] = {&rgba, &map, &flags, (void*)&planes, (void*)&Ht, (void*)&Wt, (void*)&words, (void*)&rows};
+        GMPI_CUDA_OK(cudaLaunchKernelExC(&cfg, sm->occ_exp[f16], args));
+    }
+    return GMPI_OK;
+}
+
+int gmpi_mpi_render_fwd_skip_ex(const gmpi_render_desc* d, const void* occ, size_t bytes) {
+    int rc = check_desc(d);
+    if (rc) return rc;
+    const RenderParams p = params_from_desc(d);
+    if ((rc = check_params(p, false)) != 0) return rc;
+    if (p.transmittance)
+        return fail(GMPI_ERR_UNSUPPORTED, "empty-space skipping is forward-only: it cannot be combined with the training forward (transmittance)");
+    if ((rc = check_occ_arg(p, occ, bytes)) != 0) return rc;
+    return launch_fwd(p, (cudaStream_t)d->stream, static_cast<const uint32_t*>(occ));
+}
+
+int gmpi_debug_fwd_skip_stats(unsigned long long* skipped, unsigned long long* total) {
+    if (!skipped || !total) return fail(GMPI_ERR_INVALID_ARGUMENT, "null pointer");
+    const SkipModule* sm = nullptr;
+    int rc = skip_module(&sm);
+    if (rc) return rc;
+    void* counter = nullptr;
+    size_t bytes = 0;
+    GMPI_CUDA_OK(cudaDeviceSynchronize());
+    GMPI_CUDA_OK(cudaLibraryGetGlobal(&counter, &bytes, sm->lib, "gmpi_skip_empty_stages"));
+    GMPI_CUDA_OK(cudaMemcpy(skipped, counter, sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+    *total = g_skip_total.load(std::memory_order_relaxed);
+    return GMPI_OK;
+}
+
+// Host evaluation of the producer's box-versus-map test (same code, occ_box_bits, over the 32 lanes of the warp).
+int gmpi_debug_box_occupied(const uint32_t* plane_map, int Ht, int Wt, int bx0, int by0, int bw, int rows) {
+    if (!plane_map || Ht < 1 || Wt < 1 || bw < 1 || rows < 1)
+        return -fail(GMPI_ERR_INVALID_ARGUMENT, "gmpi_debug_box_occupied: bad argument");
+    uint32_t any = 0;
+    for (int lane = 0; lane < 32; ++lane) any |= occ_box_bits(plane_map, Ht, Wt, occ_words(Wt), bx0, by0, bw, rows, lane);
+    return any != 0;
 }
 
 int gmpi_mpi_check_range(const float* rgba, int M, int N, int Ht, int Wt, uint32_t* flags, void* stream) {

@@ -1,0 +1,156 @@
+// Opt-in empty-space skipping of the staged forward (gmpi_mpi_build_occupancy, gmpi_mpi_render_fwd_skip_ex): the occupancy-map
+// build and the staged forward kernels with kSkip.  Compiled into a module of its own (libgmpi_mpi_render_skip.fatbin) that
+// mpi_render.cu loads on first use, so that the main library's kernels and their machine code stay exactly as they are.
+// Kernel names are extern "C" so that the loader can look them up.  DESIGN.md section 4.1 has the exactness argument.
+#include <cuda_runtime.h>
+#include <cuda_fp16.h>
+#include <stdint.h>
+
+#include "../../include/gmpi_mpi_render.h"
+#include "mpi_common.cuh"
+#include "mpi_fwd_staged.cuh"
+
+namespace gmpi {
+
+// Texel tests on bit patterns: U = uint32_t (fp32 MPI) or uint16_t (fp16 MPI).
+//   occupied alpha   any pattern but +0 (-0.0 and NaN count as occupied)
+//   non-finite       exponent all ones (inf, NaN)
+//   out_of_unit      the range check's test (mpi_check_range_kernel / _f16): outside [0,1] and not -0.0, NaN included
+template <class U> struct Bits;
+template <> struct Bits<uint32_t> {
+    static __device__ __forceinline__ bool nonfinite(uint32_t b) { return (b & 0x7f800000u) == 0x7f800000u; }
+    static __device__ __forceinline__ bool out_of_unit(uint32_t b) { return b > 0x3f800000u && b != 0x80000000u; }
+};
+template <> struct Bits<uint16_t> {
+    static __device__ __forceinline__ bool nonfinite(uint32_t b) { return (b & 0x7c00u) == 0x7c00u; }
+    static __device__ __forceinline__ bool out_of_unit(uint32_t b) { return b > 0x3c00u && b != 0x8000u; }
+};
+
+constexpr int kOccThreads = 32 * kOccB;     // one block row of 256 texel columns = one map word per CTA and plane
+
+// The 256 threads' verdicts (texel column threadIdx.x of this word is occupied) -> the map word: each warp holds 4 blocks of 8 columns.
+__device__ __forceinline__ void store_occ_word(bool occupied, uint32_t* dst, uint32_t* s_w) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint32_t b = __ballot_sync(0xffffffffu, occupied);
+    const uint32_t nib = ((b & 0xffu) ? 1u : 0u) | ((b & 0xff00u) ? 2u : 0u) | ((b & 0xff0000u) ? 4u : 0u) | ((b & 0xff000000u) ? 8u : 0u);
+    if (lane == 0) s_w[warp] = nib << (4 * warp);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        uint32_t w = 0;
+#pragma unroll
+        for (int k = 0; k < kOccThreads / 32; ++k) w |= s_w[k];
+        *dst = w;
+    }
+    __syncthreads();
+}
+
+// Expanded MPI [P = M*N][4][Ht][Wt]: grid (words, block rows, planes in steps of gridDim.z).  flags != NULL: also the range-check bits
+// gmpi_mpi_check_range(_f16) sets, from the same loads.
+template <class U>
+__device__ __forceinline__ void occ_expanded(const U* __restrict__ rgba, uint32_t* __restrict__ occ, uint32_t* flags, int P, int Ht,
+                                             int Wt, int words, int rows) {
+    __shared__ uint32_t s_w[kOccThreads / 32];
+    const size_t tex = (size_t)Ht * Wt;
+    const int x = blockIdx.x * kOccThreads + threadIdx.x, y0 = blockIdx.y * kOccB;
+    uint32_t flag = 0;
+    for (int pl = blockIdx.z; pl < P; pl += gridDim.z) {
+        bool occupied = false;
+        if (x < Wt) {
+            const U* base = rgba + (size_t)pl * 4 * tex + x;
+            for (int y = y0; y < y0 + kOccB && y < Ht; ++y) {
+                const size_t o = (size_t)y * Wt;
+                const uint32_t c0 = __ldcs(base + o), c1 = __ldcs(base + tex + o), c2 = __ldcs(base + 2 * tex + o), a = __ldcs(base + 3 * tex + o);
+                occupied = occupied || a != 0u || Bits<U>::nonfinite(c0) || Bits<U>::nonfinite(c1) || Bits<U>::nonfinite(c2);
+                if (Bits<U>::out_of_unit(c0) || Bits<U>::out_of_unit(c1) || Bits<U>::out_of_unit(c2)) flag |= GMPI_FLAG_RGBA_RANGE;
+                if (Bits<U>::out_of_unit(a)) flag |= GMPI_FLAG_RGBA_RANGE | GMPI_FLAG_ALPHA_RANGE;
+            }
+        }
+        store_occ_word(occupied, occ + ((size_t)pl * rows + blockIdx.y) * words + blockIdx.x, s_w);
+    }
+    if (flags) {
+        flag = __reduce_or_sync(0xffffffffu, flag);
+        if (flag && (threadIdx.x & 31) == 0) atomicOr(flags, flag);
+    }
+}
+
+// Factored MPI: colour rgb [M][3][Ht][Wt] shared by the planes (bg [M][3][Ht][Wt]: the last plane's own, nullable), alpha
+// [M][N][Ht][Wt].  Grid (words, block rows, MPIs in steps of gridDim.z).  The colour's finiteness is read once per MPI (an 8-bit row
+// mask per thread) and applied to every plane; per plane only alpha is read.
+template <class U>
+__device__ __forceinline__ void occ_factored(const U* __restrict__ rgb, const U* __restrict__ bg, const U* __restrict__ alpha,
+                                             uint32_t* __restrict__ occ, int M, int N, int Ht, int Wt, int words, int rows) {
+    __shared__ uint32_t s_w[kOccThreads / 32];
+    const size_t tex = (size_t)Ht * Wt;
+    const int x = blockIdx.x * kOccThreads + threadIdx.x, y0 = blockIdx.y * kOccB;
+    for (int m = blockIdx.z; m < M; m += gridDim.z) {
+        uint32_t nf_rgb = 0, nf_bg = 0;     // bit r: a colour value of texel row y0 + r is not finite
+        if (x < Wt) {
+            for (int r = 0; r < kOccB && y0 + r < Ht; ++r) {
+                const size_t o = (size_t)m * 3 * tex + (size_t)(y0 + r) * Wt + x;
+                if (Bits<U>::nonfinite(__ldg(rgb + o)) || Bits<U>::nonfinite(__ldg(rgb + o + tex)) || Bits<U>::nonfinite(__ldg(rgb + o + 2 * tex)))
+                    nf_rgb |= 1u << r;
+                if (bg && (Bits<U>::nonfinite(__ldg(bg + o)) || Bits<U>::nonfinite(__ldg(bg + o + tex)) || Bits<U>::nonfinite(__ldg(bg + o + 2 * tex))))
+                    nf_bg |= 1u << r;
+            }
+        }
+        for (int i = 0; i < N; ++i) {
+            bool occupied = false;
+            if (x < Wt) {
+                occupied = ((bg && i == N - 1) ? nf_bg : nf_rgb) != 0u;
+                const U* a = alpha + ((size_t)m * N + i) * tex + x;
+                for (int y = y0; y < y0 + kOccB && y < Ht; ++y) occupied = occupied || __ldcs(a + (size_t)y * Wt) != 0u;
+            }
+            store_occ_word(occupied, occ + (((size_t)m * N + i) * rows + blockIdx.y) * words + blockIdx.x, s_w);
+        }
+    }
+}
+
+template <bool kAlignCorners, bool kFactored, bool kES, class E>
+__device__ __forceinline__ void fwd_skip(const RenderParams& p, const TmaMaps& maps, int tiles_x, int ring_stages, const OccMap& occ) {
+    __shared__ uint32_t s_stop[kStopSlots];
+    fwd_staged_body<kAlignCorners, false, kFactored, kES, E, true>(p, maps, tiles_x, ring_stages, kES ? s_stop : nullptr, occ);
+}
+
+}  // namespace gmpi
+
+using namespace gmpi;
+
+extern "C" {
+
+__global__ void __launch_bounds__(kOccThreads)
+gmpi_occ_expanded_f32(const uint32_t* rgba, uint32_t* occ, uint32_t* flags, int P, int Ht, int Wt, int words, int rows) {
+    occ_expanded<uint32_t>(rgba, occ, flags, P, Ht, Wt, words, rows);
+}
+__global__ void __launch_bounds__(kOccThreads)
+gmpi_occ_expanded_f16(const uint16_t* rgba, uint32_t* occ, uint32_t* flags, int P, int Ht, int Wt, int words, int rows) {
+    occ_expanded<uint16_t>(rgba, occ, flags, P, Ht, Wt, words, rows);
+}
+__global__ void __launch_bounds__(kOccThreads)
+gmpi_occ_factored_f32(const uint32_t* rgb, const uint32_t* bg, const uint32_t* alpha, uint32_t* occ, int M, int N, int Ht, int Wt,
+                      int words, int rows) {
+    occ_factored<uint32_t>(rgb, bg, alpha, occ, M, N, Ht, Wt, words, rows);
+}
+__global__ void __launch_bounds__(kOccThreads)
+gmpi_occ_factored_f16(const uint16_t* rgb, const uint16_t* bg, const uint16_t* alpha, uint32_t* occ, int M, int N, int Ht, int Wt,
+                      int words, int rows) {
+    occ_factored<uint16_t>(rgb, bg, alpha, occ, M, N, Ht, Wt, words, rows);
+}
+
+// The staged forward with skipping: gmpi_fwd_skip_a{align_corners}_x{factored}_e{early stop}_{f32|f16} (forward only, no kEmitT).
+#define GMPI_FWD_SKIP(AC, FAC, ES, TAG, E)                                                                                        \
+    __global__ void __launch_bounds__(kStagedThreads, 1)                                                                          \
+    gmpi_fwd_skip_a##AC##_x##FAC##_e##ES##_##TAG(const RenderParams p, const __grid_constant__ TmaMaps maps, const int tiles_x,   \
+                                                 const int tiles_y, const int ring_stages, const OccMap occ) {                    \
+        fwd_skip<AC, FAC, ES, E>(p, maps, tiles_x, ring_stages, occ);                                                             \
+    }
+#define GMPI_FWD_SKIP_ES(AC, FAC, TAG, E) GMPI_FWD_SKIP(AC, FAC, 0, TAG, E) GMPI_FWD_SKIP(AC, FAC, 1, TAG, E)
+#define GMPI_FWD_SKIP_FAC(AC, TAG, E) GMPI_FWD_SKIP_ES(AC, 0, TAG, E) GMPI_FWD_SKIP_ES(AC, 1, TAG, E)
+GMPI_FWD_SKIP_FAC(0, f32, float)
+GMPI_FWD_SKIP_FAC(1, f32, float)
+GMPI_FWD_SKIP_FAC(0, f16, __half)
+GMPI_FWD_SKIP_FAC(1, f16, __half)
+
+// stages the last skipping launch armed empty (gmpi_debug_fwd_skip_stats)
+__device__ unsigned long long gmpi_skip_empty_stages;
+
+}  // extern "C"

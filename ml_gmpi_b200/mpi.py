@@ -37,7 +37,7 @@ class _RenderFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, rgba, rgb, alpha, bg_rgb, dhw, view2mpi, ray_dir, eye, z_dir, options, flags, view_group, early_stop,
-                deterministic):
+                deterministic, occ=None):
         lib = _lib.load()
         factored = rgba is None
         ref = alpha if factored else rgba
@@ -57,7 +57,10 @@ class _RenderFn(torch.autograd.Function):
                                alpha=alpha, bg_rgb=bg_rgb, view2mpi=view2mpi, dhw=dhw, ray_dir=ray_dir, eye=eye, z_dir=z_dir,
                                color=color, depth=depth, transmittance=trans, flags=flags, stream=_stream_ptr(dev),
                                early_stop=early_stop)
-            _lib.check(lib.gmpi_mpi_render_fwd_ex(ctypes.byref(d)))
+            if occ is not None:
+                _lib.check(lib.gmpi_mpi_render_fwd_skip_ex(ctypes.byref(d), occ.data_ptr(), occ.nbytes))
+            else:
+                _lib.check(lib.gmpi_mpi_render_fwd_ex(ctypes.byref(d)))
         ctx.save_for_backward(rgba, rgb, alpha, bg_rgb, dhw, view2mpi, ray_dir, eye, z_dir, trans)
         ctx.options, ctx.view_group = options, view_group
         # None: torch's global switch, read now (the backward may run on an autograd thread, after the caller changed it)
@@ -69,7 +72,7 @@ class _RenderFn(torch.autograd.Function):
     @torch.autograd.function.once_differentiable     # raw kernels: a double backward (create_graph=True) must raise, not
     def backward(ctx, g_color, g_depth):             # silently treat the result as constant (the reference's R1 only differentiates D)
         rgba, rgb, alpha, bg_rgb, dhw, view2mpi, ray_dir, eye, z_dir, trans = ctx.saved_tensors
-        none = (None,) * 14
+        none = (None,) * 15
         if not any(ctx.needs_input_grad[:4]):
             return none
         lib = _lib.load()
@@ -104,7 +107,7 @@ class _RenderFn(torch.autograd.Function):
                 _lib.check(lib.gmpi_mpi_render_bwd_deterministic_ex(ctypes.byref(d), scratch.data_ptr(), nbytes))
             else:
                 _lib.check(lib.gmpi_mpi_render_bwd_ex(ctypes.byref(d)))
-        return (g_rgba, g_rgb, g_alpha, g_bg) + (None,) * 10
+        return (g_rgba, g_rgb, g_alpha, g_bg) + (None,) * 11
 
 
 def _mpi_desc(mpi, V, H, W, options):
@@ -173,9 +176,75 @@ def _check_early_stop_without_grad(early_stop, *inputs):
                            "torch.no_grad() or from inputs that do not require grad")
 
 
+class Occupancy:
+    """The occupancy map of one MPI stack (build_occupancy): one bit per 8 x 8 texel block of every (MPI, plane), set when a texel of
+    the block is not empty (alpha not +0, or a colour value not finite; gmpi_mpi_build_occupancy).  It remembers the tensors it was
+    built from (data pointer, shape, dtype and autograd version counter) and raises when a render hands it other tensors, or the
+    same ones after an in-place change: a stale map would skip texels that are no longer empty."""
+
+    def __init__(self, occ: torch.Tensor, nbytes: int, mpi):
+        self.occ, self.nbytes = occ, nbytes
+        self._stamp = self._stamp_of(mpi)
+
+    @staticmethod
+    def _stamp_of(mpi):
+        return tuple(None if t is None else (t.data_ptr(), tuple(t.shape), t.dtype, t._version) for t in mpi)
+
+    def data_ptr(self) -> int:
+        return self.occ.data_ptr()
+
+    def check(self, mpi):
+        if self._stamp_of(mpi) != self._stamp:
+            raise RuntimeError("ml_gmpi_b200: this Occupancy was built from other MPI tensors, or they were changed in place since; "
+                               "build it again (build_occupancy)")
+
+
+def build_occupancy(*, rgba=None, rgb=None, alpha=None, bg_rgb=None, flags: Optional[torch.Tensor] = None) -> Occupancy:
+    """The occupancy map of an expanded MPI rgba [M,N,4,Ht,Wt], or of a factored one (rgb [M,3,Ht,Wt], alpha [M,N,1,Ht,Wt], bg_rgb),
+    fp32 or fp16, for render_views / render_views_factored / render_frames(skip_empty=...).  One streaming pass over the MPI (the
+    factored MPI's colour is read once, its alpha per plane).  `flags` (expanded MPI): also OR in the range-check bits check_range
+    sets, from the same pass."""
+    mpi = [rgba, rgb, alpha, bg_rgb]
+    ref = alpha if rgba is None else rgba
+    if not ref.is_cuda:
+        raise RuntimeError("ml_gmpi_b200 renders on CUDA devices only (no CPU fallback); got a CPU tensor")
+    ts = [t for t in mpi if t is not None]
+    half = all(t.dtype == torch.float16 for t in ts)     # the map of an fp16 MPI is the map of its fp32 upcast
+    launch = [None if t is None else (t.detach().contiguous() if half else _as_f32c(t.detach())) for t in mpi]
+    d = _mpi_desc(launch, 1, 1, 1, _lib.OPT_MPI_F16 if half else 0)
+    n = _lib.occupancy_bytes(d)
+    dev = ref.device
+    occ = torch.empty((n + 3) // 4, dtype=torch.int32, device=dev)
+    with torch.cuda.device(dev):
+        d.flags = flags.data_ptr() if flags is not None else None
+        d.stream = _stream_ptr(dev)
+        _lib.check(_lib.load().gmpi_mpi_build_occupancy(ctypes.byref(d), occ.data_ptr(), n))
+    return Occupancy(occ, n, mpi)
+
+
+def _occupancy_for(skip_empty, mpi) -> Optional[Occupancy]:
+    """skip_empty of a render: False -> None; True -> a map built for this call; an Occupancy -> itself, if it describes `mpi`."""
+    if skip_empty is False or skip_empty is None:
+        return None
+    if skip_empty is True:
+        return build_occupancy(rgba=mpi[0], rgb=mpi[1], alpha=mpi[2], bg_rgb=mpi[3])
+    if not isinstance(skip_empty, Occupancy):
+        raise TypeError(f"skip_empty must be a bool or an Occupancy, got {type(skip_empty).__name__}")
+    skip_empty.check(mpi)
+    return skip_empty
+
+
+def _check_skip_without_grad(skip_empty, *inputs):
+    """The training forward saves the transmittance for the backward, which needs every plane: skip_empty is forward-only."""
+    if skip_empty is not False and skip_empty is not None and torch.is_grad_enabled() and \
+            any(t is not None and t.requires_grad for t in inputs):
+        raise RuntimeError("ml_gmpi_b200: skip_empty is forward-only; render under torch.no_grad() or from inputs that do not "
+                           "require grad")
+
+
 def render_views(rgba, dhw, view2mpi, ray_dir, eye, z_dir, *, align_corners=True, check_last_plane=False,
                  color_minus1_1=False, flags: Optional[torch.Tensor] = None, view_group: int = 1, early_stop: Optional[float] = None,
-                 deterministic: Optional[bool] = None):
+                 deterministic: Optional[bool] = None, skip_empty: Union[bool, Occupancy] = False):
     """Functional form on packed tensors (no list handling, no host sync).
     rgba [M,N,4,Ht,Wt], dhw [M,N,3], view2mpi [V] int32, ray_dir [V,3,H,W], eye/z_dir [V,3].
     Returns (color [V,3,H,W], depth [V,1,H,W]); `flags` (uint32 tensor of 1, int32 storage) is OR-ed into.
@@ -183,29 +252,36 @@ def render_views(rgba, dhw, view2mpi, ray_dir, eye, z_dir, *, align_corners=True
     early_stop = tau in [0, 1): a pixel composites no further plane once its transmittance |T| <= tau (each colour channel moves by
     at most tau, 2 tau in [-1,1]; see gmpi_render_desc.early_stop).  Forward only: refused when an input requires grad.
     deterministic: the backward returns bitwise-reproducible gradients (exact int64 sums in a scratch of 8 B per gradient element,
-    gmpi_mpi_render_bwd_deterministic_ex); None follows torch.are_deterministic_algorithms_enabled() at the time of this call."""
+    gmpi_mpi_render_bwd_deterministic_ex); None follows torch.are_deterministic_algorithms_enabled() at the time of this call.
+    skip_empty: empty-space skipping (gmpi_mpi_render_fwd_skip_ex): the staged kernel does not load or composite the (tile, plane)
+    boxes whose texels all have alpha +0 and finite colour; bitwise the same output.  True builds the map for this call
+    (build_occupancy, one pass over the MPI); an Occupancy is reused.  Forward only: refused when an input requires grad."""
     _check_early_stop_without_grad(early_stop, rgba)
+    _check_skip_without_grad(skip_empty, rgba)
     if not rgba.is_cuda:
         raise RuntimeError("ml_gmpi_b200 renders on CUDA devices only (no CPU fallback); got a CPU tensor")
     if flags is None:
         flags = torch.zeros(1, dtype=torch.int32, device=rgba.device)
+    occ = _occupancy_for(skip_empty, [rgba, None, None, None])
     V, _, H, W = ray_dir.shape
     mpi, options = _launch_mpi([rgba, None, None, None], V, H, W,
                                _options(align_corners, check_last_plane, color_minus1_1, early_stop=early_stop))
     _warn_if_direct(_mpi_desc(mpi, V, H, W, options))
     return _RenderFn.apply(*mpi, _as_f32c(dhw), view2mpi, _as_f32c(ray_dir), _as_f32c(eye), _as_f32c(z_dir),
-                           options, flags, int(view_group), early_stop, deterministic)
+                           options, flags, int(view_group), early_stop, deterministic, occ)
 
 
 def render_views_factored(rgb, alpha, dhw, view2mpi, ray_dir, eye, z_dir, *, bg_rgb=None, align_corners=True,
                           check_last_plane=False, color_minus1_1=False, flags: Optional[torch.Tensor] = None, view_group: int = 1,
-                          early_stop: Optional[float] = None, deterministic: Optional[bool] = None):
+                          early_stop: Optional[float] = None, deterministic: Optional[bool] = None,
+                          skip_empty: Union[bool, Occupancy] = False):
     """The same render from the generator's FACTORED output (networks_cond_on_pos_enc.py:950-975,984): one colour image
     rgb [M,3,Ht,Wt] shared by all planes (bg_rgb [M,3,Ht,Wt]: the last plane's own colour under torgba_sep_background) and
     alpha [M,N,1,Ht,Wt] -- what the reference expands to [M,N,4,Ht,Wt] (and copies per view, train.py:553-558,733-738) before
     rendering.  Output identical to render_views on the expanded stack, 4x fewer HBM bytes; differentiable w.r.t. rgb, alpha
-    and bg_rgb (d/d rgb is the sum over the planes that share it).  early_stop, deterministic: as in render_views."""
+    and bg_rgb (d/d rgb is the sum over the planes that share it).  early_stop, deterministic, skip_empty: as in render_views."""
     _check_early_stop_without_grad(early_stop, rgb, alpha, bg_rgb)
+    _check_skip_without_grad(skip_empty, rgb, alpha, bg_rgb)
     if not alpha.is_cuda:
         raise RuntimeError("ml_gmpi_b200 renders on CUDA devices only (no CPU fallback); got a CPU tensor")
     assert rgb.ndim == 4 and rgb.shape[1] == 3 and alpha.ndim == 5 and alpha.shape[2] == 1 and rgb.shape[0] == alpha.shape[0] \
@@ -213,12 +289,13 @@ def render_views_factored(rgb, alpha, dhw, view2mpi, ray_dir, eye, z_dir, *, bg_
     assert bg_rgb is None or bg_rgb.shape == rgb.shape, f"bg_rgb must have rgb's shape, got {bg_rgb.shape}"
     if flags is None:
         flags = torch.zeros(1, dtype=torch.int32, device=alpha.device)
+    occ = _occupancy_for(skip_empty, [None, rgb, alpha, bg_rgb])
     V, _, H, W = ray_dir.shape
     mpi, options = _launch_mpi([None, rgb, alpha, bg_rgb], V, H, W,
                                _options(align_corners, check_last_plane, color_minus1_1, early_stop=early_stop))
     _warn_if_direct(_mpi_desc(mpi, V, H, W, options))
     return _RenderFn.apply(*mpi, _as_f32c(dhw), view2mpi, _as_f32c(ray_dir), _as_f32c(eye), _as_f32c(z_dir),
-                           options, flags, int(view_group), early_stop, deterministic)
+                           options, flags, int(view_group), early_stop, deterministic, occ)
 
 
 def expand_factored(rgb, alpha, bg_rgb=None):
@@ -234,8 +311,9 @@ def expand_factored(rgb, alpha, bg_rgb=None):
 def render_frames(*, dhw, view2mpi, rgba=None, rgb=None, alpha=None, bg_rgb=None, ray_dir=None, eye=None, z_dir=None, cam=None,
                   align_corners=True, check_last_plane=False, video: Optional[dict] = None, u8_round=False,
                   flags: Optional[torch.Tensor] = None, view_group: int = 1, H: Optional[int] = None, W: Optional[int] = None,
-                  early_stop: Optional[float] = None):
+                  early_stop: Optional[float] = None, skip_empty: Union[bool, Occupancy] = False):
     """Inference-only render with the opt-in fast paths of the C ABI (no autograd):
+      skip_empty=True or an Occupancy   empty-space skipping, bitwise the same frames (see render_views).
       cam [V,16]     rays generated in the kernel from the pinhole camera (see camera.cam_params) instead of ray_dir/eye/z_dir;
       video={"near": ray_start, "far": ray_end, "depth": True}   uint8 HWC frames as render_video.py:118-126 builds them:
                      returns (rgb_u8 [V,H,W,3], depth_u8 [V,H,W,1] or None); otherwise (color in [-1,1], depth) fp32.
@@ -269,6 +347,7 @@ def render_frames(*, dhw, view2mpi, rgba=None, rgb=None, alpha=None, bg_rgb=None
     else:
         color = torch.empty((V, 3, H, W), device=dev, dtype=torch.float32)
         depth = torch.empty((V, 1, H, W), device=dev, dtype=torch.float32)
+    occ = _occupancy_for(skip_empty, [rgba, rgb, alpha, bg_rgb])
     mpi, options = _launch_mpi([rgba, rgb, alpha, bg_rgb], V, H, W, _options(align_corners, check_last_plane, True, u8_round, early_stop))
     dhw = _as_f32c(dhw)
     with torch.cuda.device(dev):
@@ -276,7 +355,10 @@ def render_frames(*, dhw, view2mpi, rgba=None, rgb=None, alpha=None, bg_rgb=None
                            view_group=int(view_group), depth_near=near, depth_range=rng, rgba=mpi[0], rgb=mpi[1], alpha=mpi[2],
                            bg_rgb=mpi[3], view2mpi=view2mpi, dhw=dhw, ray_dir=ray_dir, eye=eye, z_dir=z_dir, cam=cam, color=color,
                            depth=depth, video_rgb=v_rgb, video_depth=v_depth, flags=flags, stream=_stream_ptr(dev), early_stop=early_stop)
-        _lib.check(lib.gmpi_mpi_render_fwd_ex(ctypes.byref(d)))
+        if occ is not None:
+            _lib.check(lib.gmpi_mpi_render_fwd_skip_ex(ctypes.byref(d), occ.data_ptr(), occ.nbytes))
+        else:
+            _lib.check(lib.gmpi_mpi_render_fwd_ex(ctypes.byref(d)))
     return (v_rgb, v_depth) if video is not None else (color, depth)
 
 
@@ -300,14 +382,17 @@ class MPI(nn.Module):
          "off"   like "defer" without the last-plane check.
     `deterministic`: bitwise-reproducible gradients w.r.t. batch_rgba (see render_views); None (default) follows
     torch.use_deterministic_algorithms at each forward.
+    `skip_empty`: empty-space skipping (render_views(skip_empty=...)), forward only: refused when batch_rgba requires grad under
+    autograd.  With validate="full" the occupancy map comes from the range check's pass; the flags and messages are unchanged.
     """
 
-    def __init__(self, align_corners=True, validate: str = "full", deterministic: Optional[bool] = None):
+    def __init__(self, align_corners=True, validate: str = "full", deterministic: Optional[bool] = None, skip_empty: bool = False):
         super().__init__()
         assert validate in ("full", "defer", "off"), validate
         self._align_corners = align_corners
         self.validate = validate
         self.deterministic = deterministic
+        self.skip_empty = bool(skip_empty)
         self._flags = None
         self._flag_ctx = None
 
@@ -368,12 +453,17 @@ class MPI(nn.Module):
         # an fp16 MPI stays fp16: render_views renders it natively where it can (and upcasts it where it cannot)
         rgba = batch_rgba.contiguous() if batch_rgba.dtype == torch.float16 else _as_f32c(batch_rgba)
         flags = torch.zeros(1, dtype=torch.int32, device=dev)
-        if self.validate == "full":
+        occ = False
+        if self.skip_empty:
+            _check_skip_without_grad(True, batch_rgba)
+            occ = build_occupancy(rgba=rgba, flags=flags if self.validate == "full" else None)
+        elif self.validate == "full":
             check_range(rgba.detach(), flags)
         color, depth = render_views(rgba, batch_dhw.to(dev), view2mpi, ray_dir.to(dev), eye.to(dev), z_dir.to(dev),
                                     align_corners=self._align_corners,
                                     check_last_plane=bool(assert_not_out_of_last_plane) and self.validate != "off",
-                                    flags=flags, view_group=self.view_group_of(batch_ray_dir), deterministic=self.deterministic)
+                                    flags=flags, view_group=self.view_group_of(batch_ray_dir), deterministic=self.deterministic,
+                                    skip_empty=occ)
         self._flags = flags
         self._flag_ctx = (batch_dhw, eye, c2w_mat, sphere_c)
         if self.validate == "full":

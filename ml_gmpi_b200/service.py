@@ -35,12 +35,13 @@ def sweep_angles(n_views: int = 100, horizontal: bool = True, mean: float = 0.0)
     return [float(a) + mean for a in np.linspace(half, -half, n_views).tolist()]
 
 
-def _early_stop_kw(early_stop):
-    """early_stop reaches a render_fn only when it is set, so that custom render functions without the keyword keep working."""
-    return {} if early_stop is None else {"early_stop": early_stop}
+def _early_stop_kw(early_stop, skip_empty=False):
+    """early_stop and skip_empty reach a render_fn only when they are set, so that custom render functions without the keywords keep
+    working."""
+    return ({} if early_stop is None else {"early_stop": early_stop}) | ({"skip_empty": True} if skip_empty else {})
 
 
-def _default_video_render(rgba, dhw, c2w, img_size, fov_deg, near, far, fast_rays, factored, early_stop=None):
+def _default_video_render(rgba, dhw, c2w, img_size, fov_deg, near, far, fast_rays, factored, early_stop=None, skip_empty=False):
     from .mpi import render_frames
     dev = dhw.device
     V = c2w.shape[0]
@@ -49,20 +50,21 @@ def _default_video_render(rgba, dhw, c2w, img_size, fov_deg, near, far, fast_ray
     if fast_rays:
         cam = cam_params(c2w.to(dev), focal_from_fov(fov_deg, img_size), img_size, img_size)
         return render_frames(dhw=dhw, view2mpi=v2m, cam=cam, H=img_size, W=img_size, video={"near": near, "far": far},
-                             check_last_plane=True, view_group=V, early_stop=early_stop, **kw)
+                             check_last_plane=True, view_group=V, early_stop=early_stop, skip_empty=skip_empty, **kw)
     ray_dir, eye, z_dir = PinholeCamera.from_fov(fov_deg, img_size, img_size).generate_rays(c2w.to(dev))
     return render_frames(dhw=dhw, view2mpi=v2m, ray_dir=ray_dir, eye=eye, z_dir=z_dir, video={"near": near, "far": far},
-                         check_last_plane=True, view_group=V, early_stop=early_stop, **kw)
+                         check_last_plane=True, view_group=V, early_stop=early_stop, skip_empty=skip_empty, **kw)
 
 
 def render_video_frames(mpi_rgba: Optional[torch.Tensor], dhw: torch.Tensor, angles: Sequence[float], *, img_size: int, fov_deg: float,
                         ray_start: float, ray_end: float, sphere_center, sphere_r: float, horizontal: bool = True,
                         other_angle: float = 0.0, fast_rays: bool = False, factored: Optional[Tuple] = None,
                         rank: int = 0, world: int = 1, gather: bool = True, render_fn: Optional[Callable] = None,
-                        early_stop: Optional[float] = None):
+                        early_stop: Optional[float] = None, skip_empty: bool = False):
     """All `angles` (yaw sweep if `horizontal`, else pitch sweep; the other angle fixed) of ONE MPI ([1,N,4,T,T], or
     factored=(rgb [1,3,T,T], alpha [1,N,1,T,T], bg_rgb or None)) as uint8 frames.  early_stop: early ray termination threshold
-    (render_frames; None: off).
+    (render_frames; None: off).  skip_empty: empty-space skipping with one occupancy map for all views (render_frames; bitwise the
+    same frames).
     Returns (img [V,H,W,3] uint8, depth [V,H,W,1] uint8) as CPU tensors: all V views when `gather` (every rank), else this rank's
     slice [lo, hi) of shard_range(V, rank, world)."""
     V = len(angles)
@@ -73,7 +75,7 @@ def render_video_frames(mpi_rgba: Optional[torch.Tensor], dhw: torch.Tensor, ang
     c2w = sphere_poses(yaws, pitches, sphere_center, sphere_r)
     fn = render_fn or _default_video_render
     if hi > lo:
-        img, depth = fn(mpi_rgba, dhw, c2w, img_size, fov_deg, ray_start, ray_end, fast_rays, factored, **_early_stop_kw(early_stop))
+        img, depth = fn(mpi_rgba, dhw, c2w, img_size, fov_deg, ray_start, ray_end, fast_rays, factored, **_early_stop_kw(early_stop, skip_empty))
     else:
         dev = dhw.device
         img = torch.empty((0, img_size, img_size, 3), dtype=torch.uint8, device=dev)
@@ -149,7 +151,7 @@ def to_uint8_truncating(img_m11: torch.Tensor) -> torch.Tensor:
     return (torch.clamp((img_m11 + 1) / 2.0, 0.0, 1.0) * 255).to(torch.uint8)
 
 
-def _default_eval_render(renderer, batch_mpi, n_imgs, img_size, yaws, pitches, early_stop=None):
+def _default_eval_render(renderer, batch_mpi, n_imgs, img_size, yaws, pitches, early_stop=None, skip_empty=False):
     from .mpi import render_frames
     dev = batch_mpi.device
     B = batch_mpi.shape[0]
@@ -158,21 +160,22 @@ def _default_eval_render(renderer, batch_mpi, n_imgs, img_size, yaws, pitches, e
     dhw = renderer.static_mpi_plane_dhws.to(dev).reshape(1, -1, 3).expand(B, -1, -1).contiguous()
     view2mpi = torch.arange(B, dtype=torch.int32, device=dev).repeat_interleave(n_imgs)
     return render_frames(rgba=batch_mpi, dhw=dhw, view2mpi=view2mpi, ray_dir=ray_dir, eye=eye, z_dir=z_dir, check_last_plane=True,
-                         view_group=n_imgs, early_stop=early_stop)                              # (colour in [-1,1] [V,3,H,W], depth [V,1,H,W])
+                         view_group=n_imgs, early_stop=early_stop, skip_empty=skip_empty)                              # (colour in [-1,1] [V,3,H,W], depth [V,1,H,W])
 
 
 def render_eval_views(renderer, batch_mpi: torch.Tensor, n_imgs: int, img_size: int, *, generator: Optional[torch.Generator] = None,
-                      render_fn: Optional[Callable] = None, early_stop: Optional[float] = None):
+                      render_fn: Optional[Callable] = None, early_stop: Optional[float] = None, skip_empty: bool = False):
     """batch_mpi [B,N,4,T,T] -> (img uint8 [B*n_imgs,H,W,3], depth fp32 [B*n_imgs,H,W,1], angles fp32 [B*n_imgs,2] = (pitch,
     yaw)) as numpy arrays, views MPI-major (the n_imgs views of MPI 0 first) like the reference's expand.  Poses are drawn
     as MPIRenderer.render draws them for a batch of B*n_imgs (same generator consumption: mpi_renderer.py:418-434).
-    early_stop: early ray termination threshold (render_frames; None: off)."""
+    early_stop: early ray termination threshold (render_frames; None: off).  skip_empty: empty-space skipping with one occupancy map
+    for the n_imgs views of each MPI (render_frames; bitwise the same output)."""
     B = batch_mpi.shape[0]
     V = B * int(n_imgs)
     yaws, pitches = sample_yaw_pitch(V, renderer.horizontal_mean, renderer.horizontal_std, renderer.vertical_mean, renderer.vertical_std,
                                      renderer.cam_pose_n_truncated_stds, renderer.cam_sample_method, True, generator=generator)
     fn = render_fn or _default_eval_render
-    img, depth = fn(renderer, batch_mpi, int(n_imgs), img_size, yaws, pitches, **_early_stop_kw(early_stop))
+    img, depth = fn(renderer, batch_mpi, int(n_imgs), img_size, yaws, pitches, **_early_stop_kw(early_stop, skip_empty))
     assert img.shape[0] == V and depth.shape[0] == V, f"{img.shape}, {depth.shape}, {V}"
     img_u8 = to_uint8_truncating(img.permute(0, 2, 3, 1)).cpu().numpy()
     angles = torch.cat([pitches, yaws], dim=-1).numpy()                 # mpi_renderer.py:464
