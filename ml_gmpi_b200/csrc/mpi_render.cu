@@ -489,6 +489,26 @@ using namespace gmpi;
 static std::atomic<int> g_fwd_variant{0};   // 0 auto, 1 direct, 2 staged (test hook; relaxed atomic: any thread may set it)
 static std::atomic<int> g_fwd_stages{0};    // expanded staged forward's ring depth: 0 auto (fwd_ring_stages), 2 or 3 (test hook)
 
+// An MPI is factored (rgb + alpha [+ bg_rgb]) or expanded (rgba).
+static bool factored(const RenderParams& p) { return p.alpha != nullptr; }
+
+static int check_mpi_form(const RenderParams& p) {
+    if (factored(p) ? !p.rgb || p.rgba : !p.rgba || p.rgb)
+        return fail(GMPI_ERR_INVALID_ARGUMENT, "null input pointer (MPI: pass rgba, or rgb + alpha)");
+    return GMPI_OK;
+}
+
+// The sizes of the MPIs, and with `views` those of the views too.  `texels`: the texels of one channel must also stay below 2^31.
+static int check_sizes(const RenderParams& p, bool views, bool texels) {
+    if (views && (p.M < 1 || p.V < 0 || p.N < 1 || p.Ht < 1 || p.Wt < 1 || p.H < 1 || p.W < 1))
+        return fail(GMPI_ERR_INVALID_ARGUMENT, "bad sizes M=%d V=%d N=%d Ht=%d Wt=%d H=%d W=%d", p.M, p.V, p.N, p.Ht, p.Wt, p.H, p.W);
+    if (p.M < 1 || p.N < 1 || p.Ht < 1 || p.Wt < 1)
+        return fail(GMPI_ERR_INVALID_ARGUMENT, "bad sizes M=%d N=%d Ht=%d Wt=%d", p.M, p.N, p.Ht, p.Wt);
+    if (texels && (size_t)p.Ht * p.Wt > (size_t)0x7fffffff)
+        return fail(GMPI_ERR_UNSUPPORTED, "texture of %dx%d texels exceeds 2^31 elements per channel", p.Ht, p.Wt);
+    return GMPI_OK;
+}
+
 // Argument checks shared by every entry point.  `bwd`: gradients instead of outputs.
 static int check_params(const RenderParams& p, bool bwd) {
     if (p.options & GMPI_MPI_F16) {
@@ -503,22 +523,18 @@ static int check_params(const RenderParams& p, bool bwd) {
         if (!(p.early_stop >= 0.0f && p.early_stop < 1.0f))
             return fail(GMPI_ERR_INVALID_ARGUMENT, "early_stop = %g must be in [0, 1) (gmpi_render_desc.early_stop)", (double)p.early_stop);
     }
-    const bool factored = p.alpha != nullptr || p.rgb != nullptr;
-    if (factored ? (!p.alpha || !p.rgb || p.rgba) : !p.rgba)
-        return fail(GMPI_ERR_INVALID_ARGUMENT, "null input pointer (MPI: pass rgba, or rgb + alpha)");
+    int rc = check_mpi_form(p);
+    if (rc) return rc;
     if (!p.view2mpi || !p.dhw) return fail(GMPI_ERR_INVALID_ARGUMENT, "null input pointer");
     if (!p.cam && (!p.ray_dir || !p.eye || !p.z_dir))
         return fail(GMPI_ERR_INVALID_ARGUMENT, "null input pointer (camera: pass ray_dir + eye + z_dir, or cam)");
-    if (p.M < 1 || p.V < 0 || p.N < 1 || p.Ht < 1 || p.Wt < 1 || p.H < 1 || p.W < 1)
-        return fail(GMPI_ERR_INVALID_ARGUMENT, "bad sizes M=%d V=%d N=%d Ht=%d Wt=%d H=%d W=%d", p.M, p.V, p.N, p.Ht, p.Wt, p.H, p.W);
-    if ((size_t)p.Ht * p.Wt > (size_t)0x7fffffff)
-        return fail(GMPI_ERR_UNSUPPORTED, "texture of %dx%d texels exceeds 2^31 elements per channel", p.Ht, p.Wt);
+    if ((rc = check_sizes(p, true, true)) != 0) return rc;
     if (p.view_group < 0 || (p.view_group > 1 && p.V % p.view_group != 0))
         return fail(GMPI_ERR_INVALID_ARGUMENT, "view_group=%d does not divide V=%d", p.view_group, p.V);
     if (bwd) {
         if (p.cam) return fail(GMPI_ERR_UNSUPPORTED, "the backward needs the reference's ray tensors (cam is forward-only)");
         if (!p.g_color) return fail(GMPI_ERR_INVALID_ARGUMENT, "null gradient pointer");
-        if (factored ? (!p.g_rgb || !p.g_alpha || (p.bg_rgb && !p.g_bg_rgb) || p.g_rgba) : !p.g_rgba)
+        if (factored(p) ? (!p.g_rgb || !p.g_alpha || (p.bg_rgb && !p.g_bg_rgb) || p.g_rgba) : !p.g_rgba)
             return fail(GMPI_ERR_INVALID_ARGUMENT, "null gradient pointer (pass g_rgba, or g_rgb + g_alpha [+ g_bg_rgb])");
     }
     return GMPI_OK;
@@ -535,7 +551,7 @@ static uint32_t fwd_why(const RenderParams& p) {
     uint32_t w = 0;
     if (p.N > kMaxPlanesStaged || (size_t)p.M * p.N >= ((size_t)1 << 31)) w |= GMPI_WHY_MANY_PLANES;
     if (p.Wt % ((p.options & GMPI_MPI_F16) ? 8 : 4) != 0) w |= GMPI_WHY_TEX_WIDTH;
-    if (!(p.alpha ? aligned16(p.rgb) && aligned16(p.alpha) && aligned16(p.bg_rgb) : aligned16(p.rgba))) w |= GMPI_WHY_ALIGNMENT;
+    if (!(factored(p) ? aligned16(p.rgb) && aligned16(p.alpha) && aligned16(p.bg_rgb) : aligned16(p.rgba))) w |= GMPI_WHY_ALIGNMENT;
     const int forced = g_fwd_variant.load(std::memory_order_relaxed);
     if (forced == 1) w |= GMPI_WHY_FORCED;
     const long tiles = (long)((p.W + kTileW - 1) / kTileW) * ((p.H + kTileH - 1) / kTileH) * p.V;
@@ -552,7 +568,7 @@ static int encode_mpi_maps(TmaMaps& maps, const RenderParams& p, int box_h, int 
     const MapElem el = f16 ? kMapF16 : kMapF32;
     for (int k = 0; k < kNumMaps; ++k) {
         const int bw = f16 ? staged_width<__half>(class_width(k, wide), wide) : class_width(k, wide);
-        if (p.alpha) {
+        if (factored(p)) {
             if (encode_color_map(&maps.rgb[k], p.rgb, el, (uint64_t)p.M, p.Ht, p.Wt, bw, colour_rows) != 0) return -1;
             if (p.bg_rgb && encode_color_map(&maps.bg[k], p.bg_rgb, el, (uint64_t)p.M, p.Ht, p.Wt, bw, colour_rows) != 0) return -1;
             if (encode_slab_map(&maps.a[k], p.alpha, el, (uint64_t)p.M * p.N, p.Ht, p.Wt, bw, box_h, 1) != 0) return -1;
@@ -565,10 +581,10 @@ static int encode_mpi_maps(TmaMaps& maps, const RenderParams& p, int box_h, int 
     return 0;
 }
 
-static int device_sms(int* sms) {
+static int device_attr(cudaDeviceAttr attr, int* value) {
     int dev = 0;
     GMPI_CUDA_OK(cudaGetDevice(&dev));
-    GMPI_CUDA_OK(cudaDeviceGetAttribute(sms, cudaDevAttrMultiProcessorCount, dev));
+    GMPI_CUDA_OK(cudaDeviceGetAttribute(value, attr, dev));
     return GMPI_OK;
 }
 
@@ -581,49 +597,104 @@ static int fwd_ring_stages(const RenderParams& p, int l2_bytes) {
     return shared_mpi || fits_l2 ? kStages : kStreamStages;
 }
 
-static int device_l2_bytes(int* l2) {
-    int dev = 0;
-    GMPI_CUDA_OK(cudaGetDevice(&dev));
-    GMPI_CUDA_OK(cudaDeviceGetAttribute(l2, cudaDevAttrL2CacheSize, dev));
+// What picks a render kernel: the bits of its variant.  kKeyStaged: a persistent TMA kernel (the staged forward, the box backward).
+// The direct forward's key has no kKeyFac and no kKeyEmit, and the direct backward's no kKeyFac: those kernels read both at run time.
+enum : uint32_t { kKeyAC = 1, kKeyFac = 2, kKeyEmit = 4, kKeyES = 8, kKeyF16 = 16, kKeyStaged = 32, kKeyBwd = 64, kKeyDet = 128 };
+
+// Every statically built render kernel by its key.  This switch is the first reference to each kernel, so its cases give the order
+// the kernels are instantiated in, and ptxas gives some kernels other machine code when that order changes (the expanded box
+// backward's, when the four box kernels are listed by [align_corners][factored]).  Do not reorder the cases: the recorded SASS
+// digests (tests/golden/sass_digests.json) check the machine code.  A key without a kernel gives nullptr, which the launch refuses.
+static const void* render_kernel(uint32_t key) {
+    switch (key) {
+    case kKeyStaged: return (const void*)mpi_fwd_staged_kernel<false, false, false>;
+    case kKeyStaged | kKeyFac: return (const void*)mpi_fwd_staged_kernel<false, false, true>;
+    case kKeyStaged | kKeyEmit: return (const void*)mpi_fwd_staged_kernel<false, true, false>;
+    case kKeyStaged | kKeyEmit | kKeyFac: return (const void*)mpi_fwd_staged_kernel<false, true, true>;
+    case kKeyStaged | kKeyAC: return (const void*)mpi_fwd_staged_kernel<true, false, false>;
+    case kKeyStaged | kKeyAC | kKeyFac: return (const void*)mpi_fwd_staged_kernel<true, false, true>;
+    case kKeyStaged | kKeyAC | kKeyEmit: return (const void*)mpi_fwd_staged_kernel<true, true, false>;
+    case kKeyStaged | kKeyAC | kKeyEmit | kKeyFac: return (const void*)mpi_fwd_staged_kernel<true, true, true>;
+    case kKeyStaged | kKeyES: return (const void*)mpi_fwd_early_stop_kernel<false, false>;
+    case kKeyStaged | kKeyES | kKeyFac: return (const void*)mpi_fwd_early_stop_kernel<false, true>;
+    case kKeyStaged | kKeyES | kKeyAC: return (const void*)mpi_fwd_early_stop_kernel<true, false>;
+    case kKeyStaged | kKeyES | kKeyAC | kKeyFac: return (const void*)mpi_fwd_early_stop_kernel<true, true>;
+    case 0: return (const void*)mpi_fwd_direct_kernel<false>;
+    case kKeyAC: return (const void*)mpi_fwd_direct_kernel<true>;
+    case kKeyES: return (const void*)mpi_fwd_direct_early_stop_kernel<false>;
+    case kKeyES | kKeyAC: return (const void*)mpi_fwd_direct_early_stop_kernel<true>;
+    case kKeyF16 | kKeyStaged: return (const void*)mpi_fwd_staged_f16_kernel<false, false>;
+    case kKeyF16 | kKeyStaged | kKeyFac: return (const void*)mpi_fwd_staged_f16_kernel<false, true>;
+    case kKeyF16 | kKeyStaged | kKeyAC: return (const void*)mpi_fwd_staged_f16_kernel<true, false>;
+    case kKeyF16 | kKeyStaged | kKeyAC | kKeyFac: return (const void*)mpi_fwd_staged_f16_kernel<true, true>;
+    case kKeyF16 | kKeyStaged | kKeyES: return (const void*)mpi_fwd_early_stop_f16_kernel<false, false>;
+    case kKeyF16 | kKeyStaged | kKeyES | kKeyFac: return (const void*)mpi_fwd_early_stop_f16_kernel<false, true>;
+    case kKeyF16 | kKeyStaged | kKeyES | kKeyAC: return (const void*)mpi_fwd_early_stop_f16_kernel<true, false>;
+    case kKeyF16 | kKeyStaged | kKeyES | kKeyAC | kKeyFac: return (const void*)mpi_fwd_early_stop_f16_kernel<true, true>;
+    case kKeyF16: return (const void*)mpi_fwd_direct_f16_kernel<false>;
+    case kKeyF16 | kKeyAC: return (const void*)mpi_fwd_direct_f16_kernel<true>;
+    case kKeyF16 | kKeyES: return (const void*)mpi_fwd_direct_early_stop_f16_kernel<false>;
+    case kKeyF16 | kKeyES | kKeyAC: return (const void*)mpi_fwd_direct_early_stop_f16_kernel<true>;
+    case kKeyBwd | kKeyDet | kKeyAC: return (const void*)mpi_bwd_direct_det_kernel<true>;
+    case kKeyBwd | kKeyDet: return (const void*)mpi_bwd_direct_det_kernel<false>;
+    case kKeyBwd | kKeyAC: return (const void*)mpi_bwd_direct_kernel<true>;
+    case kKeyBwd: return (const void*)mpi_bwd_direct_kernel<false>;
+    case kKeyBwd | kKeyDet | kKeyStaged | kKeyAC | kKeyFac: return (const void*)mpi_bwd_box_det_kernel<true, true>;
+    case kKeyBwd | kKeyDet | kKeyStaged | kKeyFac: return (const void*)mpi_bwd_box_det_kernel<false, true>;
+    case kKeyBwd | kKeyDet | kKeyStaged | kKeyAC: return (const void*)mpi_bwd_box_det_kernel<true, false>;
+    case kKeyBwd | kKeyDet | kKeyStaged: return (const void*)mpi_bwd_box_det_kernel<false, false>;
+    case kKeyBwd | kKeyStaged | kKeyAC | kKeyFac: return (const void*)mpi_bwd_box_kernel<true, true>;
+    case kKeyBwd | kKeyStaged | kKeyFac: return (const void*)mpi_bwd_box_kernel<false, true>;
+    case kKeyBwd | kKeyStaged | kKeyAC: return (const void*)mpi_bwd_box_kernel<true, false>;
+    case kKeyBwd | kKeyStaged: return (const void*)mpi_bwd_box_kernel<false, false>;
+    }
+    return nullptr;
+}
+
+// Everything one render-kernel launch needs.  The arguments point into this object, so it is built in place and never copied.
+struct Launch {
+    const void* kernel = nullptr;    // a static kernel (render_kernel) or a kernel of the skipping module
+    dim3 grid, block;
+    size_t smem = 0;
+    long tiles = 0;                  // the tiles of all views a persistent kernel walks (0: a direct kernel)
+    RenderParams p;                  // the first argument of every render kernel
+    TmaMaps maps;
+    int ints[3] = {};                // a persistent kernel's tiles_x, tiles_y and ring stages; the direct backward's tile_w, tile_h
+    OccMap om;
+    DetAcc da;
+    void* args[6] = {&p};
+    int n_args = 1;
+    // the set-up every render launch shares: the call's view-0 eye (the host entry point sets its own) and one view per group
+    explicit Launch(const RenderParams& q) : p(q) {
+        if (!p.eye0) p.eye0 = p.cam ? p.cam + 13 : p.eye;
+        if (p.view_group < 1) p.view_group = 1;
+    }
+    Launch(const Launch&) = delete;
+    void arg(void* a) { args[n_args++] = a; }
+};
+
+static int launch(Launch& l, cudaStream_t st) {
+    if (l.smem > 48 * 1024) GMPI_CUDA_OK(cudaFuncSetAttribute(l.kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)l.smem));
+    cudaLaunchConfig_t cfg = {l.grid, l.block, l.smem, st, nullptr, 0};
+    GMPI_CUDA_OK(cudaLaunchKernelExC(&cfg, l.kernel, l.args));
     return GMPI_OK;
 }
 
-// Test hook state of the last early-stop launch: the device counter of stages armed without copies is zeroed on the launch's stream,
-// and the number of (tile, plane) stages it walks is kept here (gmpi_debug_fwd_early_stop_stats).
-static std::atomic<unsigned long long> g_es_total{0};
-
-static int reset_early_stop_stats(unsigned long long total, cudaStream_t st) {
-    void* counter = nullptr;
-    GMPI_CUDA_OK(cudaGetSymbolAddress(&counter, g_early_stop_skipped));
-    GMPI_CUDA_OK(cudaMemsetAsync(counter, 0, sizeof(unsigned long long), st));
-    g_es_total.store(total, std::memory_order_relaxed);
+// The persistent grid of the staged forward and the box backward: tiles of kTileW x tile_h pixels in every view, at most one CTA
+// per SM.  Also adds the arguments both kernels take after p: maps, tiles_x, tiles_y.
+static int persistent_grid(Launch& l, int tile_h) {
+    const RenderParams& p = l.p;
+    int sms = 0;
+    if (int rc = device_attr(cudaDevAttrMultiProcessorCount, &sms)) return rc;
+    l.ints[0] = (p.W + kTileW - 1) / kTileW;
+    l.ints[1] = (p.H + tile_h - 1) / tile_h;
+    l.tiles = (long)l.ints[0] * l.ints[1] * p.V;
+    l.grid = dim3((unsigned)(l.tiles < sms ? l.tiles : sms));
+    l.arg(&l.maps);
+    l.arg(&l.ints[0]);
+    l.arg(&l.ints[1]);
     return GMPI_OK;
 }
-
-// The staged forward's instantiations: mpi_fwd_staged_kernel [align_corners][emit][factored] and the early-stop kernel
-// [align_corners][factored] (never with emit: check_params refuses it).
-using StagedFwdKernel = void (*)(const RenderParams, const TmaMaps, const int, const int, const int);
-static constexpr StagedFwdKernel kFwdStagedKernels[2][2][2] = {
-    {{mpi_fwd_staged_kernel<false, false, false>, mpi_fwd_staged_kernel<false, false, true>},
-     {mpi_fwd_staged_kernel<false, true, false>, mpi_fwd_staged_kernel<false, true, true>}},
-    {{mpi_fwd_staged_kernel<true, false, false>, mpi_fwd_staged_kernel<true, false, true>},
-     {mpi_fwd_staged_kernel<true, true, false>, mpi_fwd_staged_kernel<true, true, true>}}};
-static constexpr StagedFwdKernel kFwdEarlyStopKernels[2][2] = {
-    {mpi_fwd_early_stop_kernel<false, false>, mpi_fwd_early_stop_kernel<false, true>},
-    {mpi_fwd_early_stop_kernel<true, false>, mpi_fwd_early_stop_kernel<true, true>}};
-// the direct forward [early_stop][align_corners]
-static constexpr void (*kFwdDirectKernels[2][2])(const RenderParams) = {
-    {mpi_fwd_direct_kernel<false>, mpi_fwd_direct_kernel<true>},
-    {mpi_fwd_direct_early_stop_kernel<false>, mpi_fwd_direct_early_stop_kernel<true>}};
-// GMPI_MPI_F16: the staged and early-stop forward [early_stop][align_corners][factored], the direct forward [early_stop][align_corners]
-static constexpr StagedFwdKernel kFwdStagedF16Kernels[2][2][2] = {
-    {{mpi_fwd_staged_f16_kernel<false, false>, mpi_fwd_staged_f16_kernel<false, true>},
-     {mpi_fwd_staged_f16_kernel<true, false>, mpi_fwd_staged_f16_kernel<true, true>}},
-    {{mpi_fwd_early_stop_f16_kernel<false, false>, mpi_fwd_early_stop_f16_kernel<false, true>},
-     {mpi_fwd_early_stop_f16_kernel<true, false>, mpi_fwd_early_stop_f16_kernel<true, true>}}};
-static constexpr void (*kFwdDirectF16Kernels[2][2])(const RenderParams) = {
-    {mpi_fwd_direct_f16_kernel<false>, mpi_fwd_direct_f16_kernel<true>},
-    {mpi_fwd_direct_early_stop_f16_kernel<false>, mpi_fwd_direct_early_stop_f16_kernel<true>}};
 
 // Dynamic shared memory of a staged forward kernel: its ring and the plane-constant table.  fac: the kernel's kFactored; f16: its MPI
 // is fp16 (the rings of FwdRingF16 / FwdRingWideF16)
@@ -631,15 +702,6 @@ static size_t fwd_staged_smem(bool fac, int stages, bool f16) {
     const size_t ring = f16 ? (size_t)(fac ? kStages * FwdRingWideF16::kPlaneFloats : stages * FwdRingF16::kPlaneFloats) * 2
                             : (size_t)(fac ? kStages * kWideStageFloats : stages * kStageFloats) * 4;
     return ring + (size_t)kMaxPlanesStaged * 32;
-}
-
-static cudaError_t launch_fwd_staged(StagedFwdKernel kernel, bool fac, const RenderParams& p, const TmaMaps& maps, int grid, int tiles_x,
-                                     int tiles_y, int stages, cudaStream_t st, bool f16 = false) {
-    const size_t smem = fwd_staged_smem(fac, stages, f16);
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    kernel<<<grid, kStagedThreads, smem, st>>>(p, maps, tiles_x, tiles_y, stages);
-    return cudaSuccess;
 }
 
 // ---- opt-in empty-space skipping: the kernels of mpi_skip.cu live in a module of their own, libgmpi_mpi_render_skip.fatbin next to
@@ -652,7 +714,6 @@ struct SkipModule {
 };
 static SkipModule g_skip;
 static std::mutex g_skip_mutex;
-static std::atomic<unsigned long long> g_skip_total{0};    // stages the last skipping launch walked (gmpi_debug_fwd_skip_stats)
 
 static int skip_module(const SkipModule** out) {
     std::lock_guard<std::mutex> lock(g_skip_mutex);
@@ -682,24 +743,46 @@ static int skip_module(const SkipModule** out) {
     return GMPI_OK;
 }
 
-// The module's stage counter on the current device, zeroed on st; `total` stages walked (0: the direct kernel, which skips nothing).
-static int reset_skip_stats(const SkipModule* sm, unsigned long long total, cudaStream_t st, unsigned long long** counter) {
+// The stage counters of the test hooks gmpi_debug_fwd_early_stop_stats and gmpi_debug_fwd_skip_stats: on the device, the stages
+// the last early-stop or skipping launch armed without copies (zeroed on its stream); here, the (tile, plane) stages it walked.
+enum StageStats { kEarlyStopStats, kSkipStats };
+static std::atomic<unsigned long long> g_stages_walked[2];
+
+// The device counter on the current device (the skipping module's is a global of that module).
+static int stage_counter(StageStats s, unsigned long long** counter) {
+    if (s == kEarlyStopStats) {
+        GMPI_CUDA_OK(cudaGetSymbolAddress(reinterpret_cast<void**>(counter), g_early_stop_skipped));
+        return GMPI_OK;
+    }
+    const SkipModule* sm = nullptr;
+    if (int rc = skip_module(&sm)) return rc;
     size_t bytes = 0;
     GMPI_CUDA_OK(cudaLibraryGetGlobal(reinterpret_cast<void**>(counter), &bytes, sm->lib, "gmpi_skip_empty_stages"));
-    GMPI_CUDA_OK(cudaMemsetAsync(*counter, 0, sizeof(unsigned long long), st));
-    g_skip_total.store(total, std::memory_order_relaxed);
+    return GMPI_OK;
+}
+
+static int reset_stage_stats(StageStats s, unsigned long long walked, cudaStream_t st) {
+    unsigned long long* counter = nullptr;
+    if (int rc = stage_counter(s, &counter)) return rc;
+    GMPI_CUDA_OK(cudaMemsetAsync(counter, 0, sizeof(unsigned long long), st));
+    g_stages_walked[s].store(walked, std::memory_order_relaxed);
+    return GMPI_OK;
+}
+
+static int read_stage_stats(StageStats s, unsigned long long* skipped, unsigned long long* walked) {
+    if (!skipped || !walked) return fail(GMPI_ERR_INVALID_ARGUMENT, "null pointer");
+    unsigned long long* counter = nullptr;
+    if (int rc = stage_counter(s, &counter)) return rc;
+    GMPI_CUDA_OK(cudaDeviceSynchronize());
+    GMPI_CUDA_OK(cudaMemcpy(skipped, counter, sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+    *walked = g_stages_walked[s].load(std::memory_order_relaxed);
     return GMPI_OK;
 }
 
 // Occupancy map: M*N planes of occ_rows(Ht) block rows of occ_words(Wt) words.  Checks what the map's size and build read.
 static int occ_bytes(const RenderParams& p, size_t* bytes) {
-    const bool factored = p.alpha != nullptr || p.rgb != nullptr;
-    if (factored ? (!p.alpha || !p.rgb || p.rgba) : !p.rgba)
-        return fail(GMPI_ERR_INVALID_ARGUMENT, "null input pointer (MPI: pass rgba, or rgb + alpha)");
-    if (p.M < 1 || p.N < 1 || p.Ht < 1 || p.Wt < 1)
-        return fail(GMPI_ERR_INVALID_ARGUMENT, "bad sizes M=%d N=%d Ht=%d Wt=%d", p.M, p.N, p.Ht, p.Wt);
-    if ((size_t)p.Ht * p.Wt > (size_t)0x7fffffff)
-        return fail(GMPI_ERR_UNSUPPORTED, "texture of %dx%d texels exceeds 2^31 elements per channel", p.Ht, p.Wt);
+    int rc = check_mpi_form(p);
+    if (rc || (rc = check_sizes(p, false, true)) != 0) return rc;
     *bytes = (size_t)p.M * p.N * occ_rows(p.Ht) * occ_words(p.Wt) * sizeof(uint32_t);
     return GMPI_OK;
 }
@@ -711,6 +794,48 @@ static int check_occ_arg(const RenderParams& p, const void* occ, size_t bytes) {
     if (!occ) return fail(GMPI_ERR_INVALID_ARGUMENT, "null occupancy map (gmpi_mpi_occupancy_bytes gives its size)");
     if ((uintptr_t)occ & 3) return fail(GMPI_ERR_INVALID_ARGUMENT, "the occupancy map must be 4-byte aligned");
     if (bytes < need) return fail(GMPI_ERR_INVALID_ARGUMENT, "occupancy map of %zu bytes is smaller than the %zu bytes of this MPI", bytes, need);
+    return GMPI_OK;
+}
+
+// The forward kernel of a checked call with V > 0, with its launch.  occ: empty-space skipping against this map.  The staged
+// kernel when fwd_why(p) == 0 and its tensor maps encode, else the direct kernel; a forced staged variant fails instead.
+static int fwd_launch(Launch& l, const uint32_t* occ) {
+    const RenderParams& p = l.p;
+    const bool ac = (p.options & GMPI_ALIGN_CORNERS) != 0, fac = factored(p), es = (p.options & GMPI_EARLY_STOP) != 0;
+    const bool f16 = (p.options & GMPI_MPI_F16) != 0;
+    const uint32_t key = (ac ? kKeyAC : 0) | (es ? kKeyES : 0) | (f16 ? kKeyF16 : 0);
+    int rc = GMPI_OK;
+    if (fwd_why(p) == 0) {
+        if (encode_mpi_maps(l.maps, p, kMaxBH, FwdRingWide::kColourCopyRows, fac) == 0) {
+            int l2 = 0;
+            if ((rc = persistent_grid(l, kTileH)) != 0) return rc;
+            if ((rc = device_attr(cudaDevAttrL2CacheSize, &l2)) != 0) return rc;
+            const int forced_stages = g_fwd_stages.load(std::memory_order_relaxed);
+            l.ints[2] = forced_stages ? forced_stages : fwd_ring_stages(p, l2);
+            l.block = dim3(kStagedThreads);
+            l.smem = fwd_staged_smem(fac, l.ints[2], f16);
+            l.arg(&l.ints[2]);
+            if (!occ) {
+                l.kernel = render_kernel(key | kKeyStaged | (fac ? kKeyFac : 0) | (p.transmittance ? kKeyEmit : 0));
+                return GMPI_OK;
+            }
+            const SkipModule* sm = nullptr;
+            if ((rc = skip_module(&sm)) != 0) return rc;
+            l.kernel = sm->fwd[f16][ac][fac][es];
+            l.om = OccMap{occ, occ_words(p.Wt), occ_rows(p.Ht), nullptr};
+            l.arg(&l.om);
+            return stage_counter(kSkipStats, &l.om.skipped);
+        }
+        if (g_fwd_variant.load(std::memory_order_relaxed) == 2) return fail(GMPI_ERR_CUDA, "cuTensorMapEncodeTiled failed");
+    }
+    l.p.options &= ~kOptVec4Stores;      // the direct kernel stores pixel by pixel
+    l.smem = sizeof(PlaneConst) * (size_t)p.N;
+    if (l.smem > 200 * 1024) return fail(GMPI_ERR_UNSUPPORTED, "N=%d planes exceed the shared-memory plane table", p.N);
+    l.block = dim3(kFwdTileW, kFwdTileH);
+    l.grid = dim3((p.W + kFwdTileW - 1) / kFwdTileW, (p.H + kFwdTileH - 1) / kFwdTileH, p.V);
+    if (l.grid.y > 65535) return fail(GMPI_ERR_UNSUPPORTED, "image height %d too large", p.H);
+    if (p.V > 65535) return fail(GMPI_ERR_UNSUPPORTED, "V=%d views exceed one launch of the direct kernel (65535); split the batch", p.V);
+    l.kernel = render_kernel(key);
     return GMPI_OK;
 }
 
@@ -728,66 +853,16 @@ static int launch_fwd(RenderParams p, cudaStream_t st, const uint32_t* occ = nul
         return fail(GMPI_ERR_INVALID_ARGUMENT, "null output pointer");
     }
     if (p.V == 0) return GMPI_OK;
-    if (!p.eye0) p.eye0 = p.cam ? p.cam + 13 : p.eye;
-    if (p.view_group < 1) p.view_group = 1;
     // float4 epilogue stores: whole quads of x stay inside a row and every destination is 16-byte aligned.  Peer buffers are
     // symmetric-memory allocations (256-byte aligned bases; frame slabs are multiples of 16 bytes when W % 4 == 0).
     if (p.W % 4 == 0 && !p.video_rgb && (p.n_peers > 0 || (aligned16(p.color) && aligned16(p.depth)))) p.options |= kOptVec4Stores;
-    const bool ac = (p.options & GMPI_ALIGN_CORNERS) != 0, emit = p.transmittance != nullptr, fac = p.alpha != nullptr;
-    const bool es = (p.options & GMPI_EARLY_STOP) != 0, f16 = (p.options & GMPI_MPI_F16) != 0;
-    if (fwd_why(p) == 0) {
-        TmaMaps maps;
-        if (encode_mpi_maps(maps, p, kMaxBH, FwdRingWide::kColourCopyRows, fac) != 0) {
-            if (g_fwd_variant.load(std::memory_order_relaxed) == 2) return fail(GMPI_ERR_CUDA, "cuTensorMapEncodeTiled failed");
-        } else {
-            int sms = 0, l2 = 0;
-            if ((rc = device_sms(&sms)) != 0) return rc;
-            if ((rc = device_l2_bytes(&l2)) != 0) return rc;
-            const int forced_stages = g_fwd_stages.load(std::memory_order_relaxed);
-            const int stages = forced_stages ? forced_stages : fwd_ring_stages(p, l2);
-            const int tiles_x = (p.W + kTileW - 1) / kTileW, tiles_y = (p.H + kTileH - 1) / kTileH;
-            const long n_tiles = (long)tiles_x * tiles_y * p.V;
-            const int grid = (int)(n_tiles < sms ? n_tiles : sms);
-            if (es && (rc = reset_early_stop_stats((unsigned long long)n_tiles * p.N, st)) != 0) return rc;
-            if (occ) {
-                const SkipModule* sm = nullptr;
-                OccMap om{occ, occ_words(p.Wt), occ_rows(p.Ht), nullptr};
-                if ((rc = skip_module(&sm)) != 0 || (rc = reset_skip_stats(sm, (unsigned long long)n_tiles * p.N, st, &om.skipped)) != 0)
-                    return rc;
-                const void* kernel = sm->fwd[f16][ac][fac][es];
-                const size_t smem = fwd_staged_smem(fac, stages, f16);
-                GMPI_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-                cudaLaunchConfig_t cfg = {};
-                cfg.gridDim = dim3(grid); cfg.blockDim = dim3(kStagedThreads); cfg.dynamicSmemBytes = smem; cfg.stream = st;
-                void* args[] = {&p, &maps, (void*)&tiles_x, (void*)&tiles_y, (void*)&stages, &om};
-                GMPI_CUDA_OK(cudaLaunchKernelExC(&cfg, kernel, args));
-                return GMPI_OK;
-            }
-            const StagedFwdKernel kernel = f16 ? kFwdStagedF16Kernels[es][ac][fac] : es ? kFwdEarlyStopKernels[ac][fac] : kFwdStagedKernels[ac][emit][fac];
-            cudaError_t e = launch_fwd_staged(kernel, fac, p, maps, grid, tiles_x, tiles_y, stages, st, f16);
-            GMPI_CUDA_OK(e);
-            GMPI_CUDA_OK(cudaGetLastError());
-            return GMPI_OK;
-        }
-    }
-    p.options &= ~kOptVec4Stores;      // the direct kernel stores pixel by pixel
-    const size_t smem = sizeof(PlaneConst) * (size_t)p.N;
-    if (smem > 200 * 1024) return fail(GMPI_ERR_UNSUPPORTED, "N=%d planes exceed the shared-memory plane table", p.N);
-    dim3 block(kFwdTileW, kFwdTileH);
-    dim3 grid((p.W + kFwdTileW - 1) / kFwdTileW, (p.H + kFwdTileH - 1) / kFwdTileH, p.V);
-    if (grid.y > 65535) return fail(GMPI_ERR_UNSUPPORTED, "image height %d too large", p.H);
-    if (p.V > 65535) return fail(GMPI_ERR_UNSUPPORTED, "V=%d views exceed one launch of the direct kernel (65535); split the batch", p.V);
-    if (es && (rc = reset_early_stop_stats(0, st)) != 0) return rc;    // the direct kernel loads per pixel: no stages to skip
-    if (occ) {     // nor empty ones: the direct kernel takes the request and composites every plane, which gives the same output
-        const SkipModule* sm = nullptr;
-        unsigned long long* counter = nullptr;
-        if ((rc = skip_module(&sm)) != 0 || (rc = reset_skip_stats(sm, 0, st, &counter)) != 0) return rc;
-    }
-    void (*kernel)(const RenderParams) = f16 ? kFwdDirectF16Kernels[es][ac] : kFwdDirectKernels[es][ac];
-    if (smem > 48 * 1024) GMPI_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kernel<<<grid, block, smem, st>>>(p);
-    GMPI_CUDA_OK(cudaGetLastError());
-    return GMPI_OK;
+    Launch l(p);
+    if ((rc = fwd_launch(l, occ)) != 0) return rc;
+    // the direct kernel walks no stages: it loads per pixel, and composites every plane (which gives a skipping call's output)
+    const unsigned long long walked = (unsigned long long)l.tiles * p.N;
+    if ((p.options & GMPI_EARLY_STOP) && (rc = reset_stage_stats(kEarlyStopStats, walked, st)) != 0) return rc;
+    if (occ && (rc = reset_stage_stats(kSkipStats, walked, st)) != 0) return rc;
+    return launch(l, st);
 }
 
 static int zero_grads(const RenderParams& p, cudaStream_t st) {
@@ -802,101 +877,60 @@ static int zero_grads(const RenderParams& p, cudaStream_t st) {
     return GMPI_OK;
 }
 
-// Two-pass direct backward (any shape, no saved state).  da: the deterministic variant, adding into da's sums.
-static int launch_bwd_direct(RenderParams p, cudaStream_t st, bool zero, const DetAcc* da = nullptr) {
-    if (zero && (p.options & GMPI_ZERO_GRAD)) {
-        int rc = zero_grads(p, st);
-        if (rc) return rc;
-    }
-    if (p.V == 0) return GMPI_OK;
-    p.eye0 = p.eye;
-    if (p.view_group < 1) p.view_group = 1;
-    // tile: as many threads (<=128) as the per-thread transmittance stash allows
-    int tile_w = 32, tile_h = 4;
-    size_t smem = 0;
-    for (;; tile_h >>= 1) {
-        if (tile_h == 0) return fail(GMPI_ERR_UNSUPPORTED, "N=%d planes exceed the backward stash (227 KB / 32 threads)", p.N);
-        smem = sizeof(PlaneConst) * (size_t)p.N + sizeof(float) * (size_t)p.N * tile_w * tile_h;
-        if (smem <= 227 * 1024) break;
-    }
-    dim3 block(tile_w, tile_h);
-    dim3 grid((p.W + tile_w - 1) / tile_w, (p.H + tile_h - 1) / tile_h, p.V);
-    if (grid.y > 65535) return fail(GMPI_ERR_UNSUPPORTED, "image height %d too large", p.H);
-    if (p.V > 65535) return fail(GMPI_ERR_UNSUPPORTED, "V=%d views exceed one launch of the direct kernel (65535); split the batch", p.V);
-    if (da) {
-        void (*kernel)(const RenderParams, const int, const int, const DetAcc) =
-            (p.options & GMPI_ALIGN_CORNERS) ? mpi_bwd_direct_det_kernel<true> : mpi_bwd_direct_det_kernel<false>;
-        GMPI_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        kernel<<<grid, block, smem, st>>>(p, tile_w, tile_h, *da);
-        GMPI_CUDA_OK(cudaGetLastError());
-        return GMPI_OK;
-    }
-    void (*kernel)(const RenderParams, const int, const int) =
-        (p.options & GMPI_ALIGN_CORNERS) ? mpi_bwd_direct_kernel<true> : mpi_bwd_direct_kernel<false>;
-    GMPI_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kernel<<<grid, block, smem, st>>>(p, tile_w, tile_h);
-    GMPI_CUDA_OK(cudaGetLastError());
-    return GMPI_OK;
-}
-
-using BwdBoxKernel = void (*)(const RenderParams, const TmaMaps, const int, const int);
-
-static cudaError_t launch_bwd_box(BwdBoxKernel kernel, const RenderParams& p, const TmaMaps& maps, int grid, int tiles_x, int tiles_y,
-                                  cudaStream_t st) {
-    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBwdSmem);
-    if (e != cudaSuccess) return e;
-    kernel<<<grid, kBwdThreads, kBwdSmem, st>>>(p, maps, tiles_x, tiles_y);
-    return cudaSuccess;
-}
-
 // Backward kernel choice: the staged box kernel when the forward saved the transmittance, the staged forward would be launched
 // (fwd_why) and the backward's own conditions hold (16-byte aligned gradient and transmittance bases, W % 4 == 0, V*N < 2^31), else
 // the direct kernel.  The deterministic backward makes the same choice from the caller's descriptor.
 static bool bwd_uses_box(const RenderParams& p) {
-    const bool fac = p.alpha != nullptr;
+    const bool fac = factored(p);
     const bool grads_aligned = fac ? aligned16(p.g_rgb) && aligned16(p.g_alpha) && (!p.g_bg_rgb || aligned16(p.g_bg_rgb)) : aligned16(p.g_rgba);
     return p.transmittance && fwd_why(p) == 0 && grads_aligned && p.W % 4 == 0 && aligned16(p.transmittance) &&
            (size_t)p.V * p.N < ((size_t)1 << 31);
 }
 
-// The box backward of a checked call.  da: the deterministic variant (its sums were zeroed by the caller; no GMPI_ZERO_GRAD here).
-static int launch_bwd_box(RenderParams p, cudaStream_t st, const DetAcc* da) {
-    int rc = GMPI_OK;
-    if (p.V == 0) return (p.options & GMPI_ZERO_GRAD) ? zero_grads(p, st) : GMPI_OK;
-    p.eye0 = p.eye;
-    if (p.view_group < 1) p.view_group = 1;
-    TmaMaps maps;
-    if (encode_mpi_maps(maps, p, kBwdMaxBH, BwdRing::kColourCopyRows) != 0) return fail(GMPI_ERR_CUDA, "cuTensorMapEncodeTiled failed");
-    if (encode_slab_map(&maps.t, p.transmittance, kMapF32, (uint64_t)p.V * p.N, p.H, p.W, kTileW, kBwdTileH, 1) != 0)
-        return fail(GMPI_ERR_CUDA, "cuTensorMapEncodeTiled (transmittance) failed");
-    int sms = 0;
-    if ((rc = device_sms(&sms)) != 0) return rc;
-    const int tiles_x = (p.W + kTileW - 1) / kTileW, tiles_y = (p.H + kBwdTileH - 1) / kBwdTileH;
-    const long n_tiles = (long)tiles_x * tiles_y * p.V;
-    const int grid = (int)(n_tiles < sms ? n_tiles : sms);
-    const bool ac = (p.options & GMPI_ALIGN_CORNERS) != 0, fac = p.alpha != nullptr;
-    if (da) {
-        const auto kernel = fac ? (ac ? mpi_bwd_box_det_kernel<true, true> : mpi_bwd_box_det_kernel<false, true>)
-                                : (ac ? mpi_bwd_box_det_kernel<true, false> : mpi_bwd_box_det_kernel<false, false>);
-        GMPI_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBwdSmem));
-        kernel<<<grid, kBwdThreads, kBwdSmem, st>>>(p, maps, tiles_x, tiles_y, *da);
-        GMPI_CUDA_OK(cudaGetLastError());
-        return GMPI_OK;
+// The backward kernel of a checked call with V > 0, with its launch: the box kernel when `box` (bwd_uses_box), else the two-pass
+// direct kernel (any shape, no saved state).  det: the deterministic variant, adding into the sums of l.da.
+static int bwd_launch(Launch& l, bool box, bool det) {
+    const RenderParams& p = l.p;
+    uint32_t key = kKeyBwd | (det ? kKeyDet : 0) | ((p.options & GMPI_ALIGN_CORNERS) ? kKeyAC : 0);
+    if (box) {
+        if (encode_mpi_maps(l.maps, p, kBwdMaxBH, BwdRing::kColourCopyRows) != 0) return fail(GMPI_ERR_CUDA, "cuTensorMapEncodeTiled failed");
+        if (encode_slab_map(&l.maps.t, p.transmittance, kMapF32, (uint64_t)p.V * p.N, p.H, p.W, kTileW, kBwdTileH, 1) != 0)
+            return fail(GMPI_ERR_CUDA, "cuTensorMapEncodeTiled (transmittance) failed");
+        if (int rc = persistent_grid(l, kBwdTileH)) return rc;
+        l.block = dim3(kBwdThreads);
+        l.smem = kBwdSmem;
+        key |= kKeyStaged | (factored(p) ? kKeyFac : 0);
+    } else {
+        // tile: as many threads (<=128) as the per-thread transmittance stash allows
+        int tile_w = 32, tile_h = 4;
+        for (;; tile_h >>= 1) {
+            if (tile_h == 0) return fail(GMPI_ERR_UNSUPPORTED, "N=%d planes exceed the backward stash (227 KB / 32 threads)", p.N);
+            l.smem = sizeof(PlaneConst) * (size_t)p.N + sizeof(float) * (size_t)p.N * tile_w * tile_h;
+            if (l.smem <= 227 * 1024) break;
+        }
+        l.block = dim3(tile_w, tile_h);
+        l.grid = dim3((p.W + tile_w - 1) / tile_w, (p.H + tile_h - 1) / tile_h, p.V);
+        if (l.grid.y > 65535) return fail(GMPI_ERR_UNSUPPORTED, "image height %d too large", p.H);
+        if (p.V > 65535) return fail(GMPI_ERR_UNSUPPORTED, "V=%d views exceed one launch of the direct kernel (65535); split the batch", p.V);
+        l.ints[0] = tile_w;
+        l.ints[1] = tile_h;
+        l.arg(&l.ints[0]);
+        l.arg(&l.ints[1]);
     }
-    if ((p.options & GMPI_ZERO_GRAD) && (rc = zero_grads(p, st)) != 0) return rc;
-    // (not a table: instantiating the four kernels in table order changes the machine code ptxas gives the expanded ones)
-    const BwdBoxKernel kernel = fac ? (ac ? mpi_bwd_box_kernel<true, true> : mpi_bwd_box_kernel<false, true>)
-                                    : (ac ? mpi_bwd_box_kernel<true, false> : mpi_bwd_box_kernel<false, false>);
-    cudaError_t e = launch_bwd_box(kernel, p, maps, grid, tiles_x, tiles_y, st);
-    GMPI_CUDA_OK(e);
-    GMPI_CUDA_OK(cudaGetLastError());
+    if (det) l.arg(&l.da);
+    l.kernel = render_kernel(key);
     return GMPI_OK;
 }
 
 static int launch_bwd(RenderParams p, cudaStream_t st) {
     int rc = check_params(p, true);
     if (rc) return rc;
-    return bwd_uses_box(p) ? launch_bwd_box(p, st, nullptr) : launch_bwd_direct(p, st, true);
+    const bool zero = (p.options & GMPI_ZERO_GRAD) != 0;
+    if (p.V == 0) return zero ? zero_grads(p, st) : GMPI_OK;
+    Launch l(p);
+    if ((rc = bwd_launch(l, bwd_uses_box(p), false)) != 0) return rc;
+    if (zero && (rc = zero_grads(p, st)) != 0) return rc;
+    return launch(l, st);
 }
 
 // ---- deterministic backward (DetAcc, DESIGN.md section 4.3) ----
@@ -909,13 +943,12 @@ constexpr size_t kDetHeaderBytes = 256;
 constexpr int kDetMinFixBits = 24;
 
 static int det_layout(const RenderParams& p, DetLayout& L) {
-    if (p.M < 1 || p.V < 0 || p.N < 1 || p.Ht < 1 || p.Wt < 1 || p.H < 1 || p.W < 1)
-        return fail(GMPI_ERR_INVALID_ARGUMENT, "bad sizes M=%d V=%d N=%d Ht=%d Wt=%d H=%d W=%d", p.M, p.V, p.N, p.Ht, p.Wt, p.H, p.W);
+    if (int rc = check_sizes(p, true, false)) return rc;
     const double tex = (double)p.Ht * p.Wt, M = p.M, N = p.N;
-    const double G = p.alpha ? M * 3 * tex + M * N * tex + (p.bg_rgb ? M * 3 * tex : 0.0) : M * N * 4 * tex;
+    const double G = factored(p) ? M * 3 * tex + M * N * tex + (p.bg_rgb ? M * 3 * tex : 0.0) : M * N * 4 * tex;
     if (G * 9 > 0x1p62) return fail(GMPI_ERR_UNSUPPORTED, "%.0f gradient elements exceed the deterministic scratch's range", G);
     const size_t t = (size_t)p.Ht * p.Wt;
-    if (p.alpha) {
+    if (factored(p)) {
         L.seg1 = (size_t)p.M * 3 * t;
         L.seg2 = L.seg1 + (size_t)p.M * p.N * t;
         L.G = L.seg2 + (p.bg_rgb ? (size_t)p.M * 3 * t : 0);
@@ -948,15 +981,15 @@ static int launch_bwd_deterministic(RenderParams p, void* scratch, size_t scratc
     if (!aligned16(scratch)) return fail(GMPI_ERR_INVALID_ARGUMENT, "the scratch must be 16-byte aligned");
     if (scratch_bytes < L.bytes)
         return fail(GMPI_ERR_INVALID_ARGUMENT, "scratch of %zu bytes is smaller than the %zu bytes this call needs", scratch_bytes, L.bytes);
-    const bool fac = p.alpha != nullptr;
+    const bool fac = factored(p);
     const int k_a = det_fix_bits(p, 1), k_rgb = det_fix_bits(p, fac ? p.N : 1);
     if (k_rgb < kDetMinFixBits)
         return fail(GMPI_ERR_UNSUPPORTED, "V=%d views of %dx%d pixels leave %d fraction bits for exact int64 sums (at least %d needed)", p.V,
                     p.H, p.W, k_rgb, kDetMinFixBits);
     if (p.V == 0) return (p.options & GMPI_ZERO_GRAD) ? zero_grads(p, st) : GMPI_OK;
-    const bool box = bwd_uses_box(p);
+    Launch l(p);
+    DetAcc& da = l.da;
     char* s = static_cast<char*>(scratch);
-    DetAcc da;
     da.bounds = reinterpret_cast<uint32_t*>(s);
     da.acc = reinterpret_cast<unsigned long long*>(s + kDetHeaderBytes);
     da.base = reinterpret_cast<float*>(da.acc);
@@ -964,25 +997,21 @@ static int launch_bwd_deterministic(RenderParams p, void* scratch, size_t scratc
     da.k_a = k_a;
     da.k_rgb = k_rgb;
     // the kernels' gradient pointers address the sums (DetAcc); the finish pass writes the caller's
-    RenderParams q = p;
     if (fac) {
-        q.g_rgb = da.base;
-        q.g_alpha = da.base + L.seg1;
-        q.g_bg_rgb = p.g_bg_rgb ? da.base + L.seg2 : nullptr;
+        l.p.g_rgb = da.base;
+        l.p.g_alpha = da.base + L.seg1;
+        l.p.g_bg_rgb = p.g_bg_rgb ? da.base + L.seg2 : nullptr;
     } else {
-        q.g_rgba = da.base;
+        l.p.g_rgba = da.base;
     }
-    q.options &= ~GMPI_ZERO_GRAD;
+    if ((rc = bwd_launch(l, bwd_uses_box(p), true)) != 0) return rc;
     GMPI_CUDA_OK(cudaMemsetAsync(scratch, 0, L.bytes, st));
-    q.eye0 = q.eye;
-    if (q.view_group < 1) q.view_group = 1;
     dim3 bgrid((unsigned)(((size_t)p.H * p.W + 255) / 256), (unsigned)(p.V < 65535 ? p.V : 65535));
-    mpi_bwd_det_bounds_kernel<<<bgrid, 256, 0, st>>>(q, da.bounds);
+    mpi_bwd_det_bounds_kernel<<<bgrid, 256, 0, st>>>(l.p, da.bounds);
     GMPI_CUDA_OK(cudaGetLastError());
-    rc = box ? launch_bwd_box(q, st, &da) : launch_bwd_direct(q, st, false, &da);
-    if (rc) return rc;
+    if ((rc = launch(l, st)) != 0) return rc;
     int sms = 0;
-    if ((rc = device_sms(&sms)) != 0) return rc;
+    if ((rc = device_attr(cudaDevAttrMultiProcessorCount, &sms)) != 0) return rc;
     mpi_bwd_det_finish_kernel<<<sms * 8, 256, 0, st>>>(da, fac ? p.g_rgb : p.g_rgba, p.g_alpha, p.g_bg_rgb, L.G, L.seg1, L.seg2,
                                                       (size_t)p.Ht * p.Wt, fac, (p.options & GMPI_ZERO_GRAD) != 0);
     GMPI_CUDA_OK(cudaGetLastError());
@@ -1060,11 +1089,7 @@ int gmpi_debug_set_fwd_stages(int stages) {
 }
 
 int gmpi_debug_fwd_early_stop_stats(unsigned long long* skipped, unsigned long long* total) {
-    if (!skipped || !total) return fail(GMPI_ERR_INVALID_ARGUMENT, "null pointer");
-    GMPI_CUDA_OK(cudaDeviceSynchronize());
-    GMPI_CUDA_OK(cudaMemcpyFromSymbol(skipped, g_early_stop_skipped, sizeof(unsigned long long)));
-    *total = g_es_total.load(std::memory_order_relaxed);
-    return GMPI_OK;
+    return read_stage_stats(kEarlyStopStats, skipped, total);
 }
 
 int gmpi_debug_fwd_ring_stages(int M, int V, int N, int Ht, int Wt, int view_group) {
@@ -1073,7 +1098,7 @@ int gmpi_debug_fwd_ring_stages(int M, int V, int N, int Ht, int Wt, int view_gro
     RenderParams p{};
     p.M = M; p.V = V; p.N = N; p.Ht = Ht; p.Wt = Wt;
     p.view_group = view_group < 1 ? 1 : view_group;
-    int l2 = 0, rc = device_l2_bytes(&l2);
+    int l2 = 0, rc = device_attr(cudaDevAttrL2CacheSize, &l2);
     if (rc) return -rc;
     return fwd_ring_stages(p, l2);
 }
@@ -1234,7 +1259,7 @@ int gmpi_mpi_build_occupancy(const gmpi_render_desc* d, void* occ, size_t bytes)
     cfg.blockDim = dim3(32 * kOccB);
     cfg.stream = (cudaStream_t)d->stream;
     uint32_t* map = static_cast<uint32_t*>(occ);
-    if (p.alpha) {
+    if (factored(p)) {
         cfg.gridDim = dim3(words, rows, M < 65535 ? M : 65535);
         const void *rgb = p.rgb, *bg = p.bg_rgb, *alpha = p.alpha;
         void* args[] = {&rgb, &bg, &alpha, &map, (void*)&M, (void*)&N, (void*)&Ht, (void*)&Wt, (void*)&words, (void*)&rows};
@@ -1264,17 +1289,7 @@ int gmpi_mpi_render_fwd_skip_ex(const gmpi_render_desc* d, const void* occ, size
 }
 
 int gmpi_debug_fwd_skip_stats(unsigned long long* skipped, unsigned long long* total) {
-    if (!skipped || !total) return fail(GMPI_ERR_INVALID_ARGUMENT, "null pointer");
-    const SkipModule* sm = nullptr;
-    int rc = skip_module(&sm);
-    if (rc) return rc;
-    void* counter = nullptr;
-    size_t bytes = 0;
-    GMPI_CUDA_OK(cudaDeviceSynchronize());
-    GMPI_CUDA_OK(cudaLibraryGetGlobal(&counter, &bytes, sm->lib, "gmpi_skip_empty_stages"));
-    GMPI_CUDA_OK(cudaMemcpy(skipped, counter, sizeof(unsigned long long), cudaMemcpyDeviceToHost));
-    *total = g_skip_total.load(std::memory_order_relaxed);
-    return GMPI_OK;
+    return read_stage_stats(kSkipStats, skipped, total);
 }
 
 // Host evaluation of the producer's box-versus-map test (same code, occ_box_bits, over the 32 lanes of the warp).
@@ -1292,7 +1307,7 @@ int gmpi_mpi_check_range(const float* rgba, int M, int N, int Ht, int Wt, uint32
     cudaStream_t st = (cudaStream_t)stream;
     const size_t slab = (size_t)Ht * Wt, n_slabs = (size_t)M * N * 4;
     int sms = 132;
-    int rc = device_sms(&sms);
+    int rc = device_attr(cudaDevAttrMultiProcessorCount, &sms);
     if (rc) return rc;
     const int grid = sms * 8;
     if (slab % 4 == 0 && ((uintptr_t)rgba & 15) == 0) {
@@ -1310,7 +1325,7 @@ int gmpi_mpi_check_range_f16(const void* rgba, int M, int N, int Ht, int Wt, uin
     cudaStream_t st = (cudaStream_t)stream;
     const size_t slab = (size_t)Ht * Wt, n_slabs = (size_t)M * N * 4;
     int sms = 132;
-    int rc = device_sms(&sms);
+    int rc = device_attr(cudaDevAttrMultiProcessorCount, &sms);
     if (rc) return rc;
     const int grid = sms * 8;
     if (slab % 8 == 0 && ((uintptr_t)rgba & 15) == 0) {
@@ -1478,7 +1493,7 @@ static int host_render_locked(HostCache& c, const RenderParams& h, uint32_t* fla
     int rc = GMPI_OK;
     const int M = h.M, V = h.V, N = h.N, H = h.H, W = h.W;
     const size_t tex = (size_t)h.Ht * h.Wt, img = (size_t)H * W;
-    const bool fac = h.alpha != nullptr, video = h.video_rgb != nullptr;
+    const bool fac = factored(h), video = h.video_rgb != nullptr;
     // one slot = one MPI: expanded [N,4,tex], or factored rgb [3,tex] | bg [3,tex] | alpha [N,tex]
     // (offsets in MPI elements: fp16 under GMPI_MPI_F16, else fp32)
     const size_t esz = (h.options & GMPI_MPI_F16) ? 2 : 4;
