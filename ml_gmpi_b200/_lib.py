@@ -24,18 +24,6 @@ WHY = {1: "texture width is not a multiple of 4 (8 in fp16)", 2: "fewer than 120
 
 ABI_VERSION = 2
 
-EXPORTS = [
-    "gmpi_abi_version", "gmpi_last_error", "gmpi_mpi_render_fwd_variant", "gmpi_mpi_render_fwd",
-    "gmpi_mpi_render_fwd_gather", "gmpi_mpi_render_fwd_train", "gmpi_mpi_render_bwd", "gmpi_mpi_render_bwd_saved", "gmpi_mpi_check_range", "gmpi_mpi_render_fwd_host", "gmpi_mpi_release_host_cache", "gmpi_debug_plane_coords", "gmpi_debug_division", "gmpi_debug_set_fwd_variant", "gmpi_debug_copy_plan", "gmpi_debug_plane_coords_packed", "gmpi_debug_tile_walk",
-    "gmpi_mpi_render_fwd_plan", "gmpi_mpi_render_fwd_ex", "gmpi_mpi_render_bwd_ex", "gmpi_mpi_render_host_ex",
-    "gmpi_debug_tile_walk_ex", "gmpi_debug_cam_rays", "gmpi_debug_set_fwd_stages", "gmpi_debug_fwd_ring_stages",
-    "gmpi_debug_fwd_early_stop_stats", "gmpi_mpi_zero_async", "gmpi_mpi_alpha_depth_fwd", "gmpi_mpi_alpha_depth_bwd", "gmpi_mpi_apply_shading_fwd", "gmpi_mpi_apply_shading_bwd",
-    "gmpi_mpi_render_fwd_plan_ex", "gmpi_mpi_check_range_f16",
-    "gmpi_mpi_render_bwd_deterministic_scratch_bytes", "gmpi_mpi_render_bwd_deterministic_ex",
-    "gmpi_mpi_occupancy_bytes", "gmpi_mpi_build_occupancy", "gmpi_mpi_render_fwd_skip_ex", "gmpi_debug_fwd_skip_stats",
-    "gmpi_debug_box_occupied",
-]
-
 OPT_U8_ROUND_HALF_UP = 16
 OPT_EARLY_STOP = 32
 OPT_MPI_F16 = 64
@@ -55,6 +43,54 @@ class RenderDesc(ctypes.Structure):
 
 # struct_bytes of a descriptor built against the header before early_stop was appended (GMPI_RENDER_DESC_V2_BYTES)
 RENDER_DESC_V2_BYTES = RenderDesc.early_stop.offset
+
+
+_vp, _i, _u32, _ll, _size, _desc = ctypes.c_void_p, ctypes.c_int, ctypes.c_uint32, ctypes.c_longlong, ctypes.c_size_t, \
+    ctypes.POINTER(RenderDesc)
+# {name: (restype, argtypes)} of every function the header declares, in its order
+SIGNATURES = {
+    "gmpi_abi_version": (_i, []),
+    "gmpi_last_error": (ctypes.c_char_p, []),
+    "gmpi_mpi_render_fwd_variant": (ctypes.c_char_p, [_i] * 5),
+    "gmpi_mpi_render_fwd_plan": (_i, [_i] * 6 + [_vp, _vp]),
+    "gmpi_mpi_render_fwd": (_i, [_vp] * 9 + [_i] * 7 + [_u32, _vp]),
+    "gmpi_mpi_render_fwd_gather": (_i, [_vp] * 7 + [_i, _i, _vp] + [_i] * 7 + [_u32, _vp]),
+    "gmpi_mpi_render_bwd": (_i, [_vp] * 9 + [_i] * 7 + [_u32, _vp]),
+    "gmpi_mpi_render_fwd_train": (_i, [_vp] * 10 + [_i] * 7 + [_u32, _vp]),
+    "gmpi_mpi_render_bwd_saved": (_i, [_vp] * 10 + [_i] * 7 + [_u32, _vp]),
+    "gmpi_mpi_zero_async": (_i, [_vp, _size, _vp]),
+    "gmpi_mpi_render_fwd_ex": (_i, [_desc]),
+    "gmpi_mpi_render_fwd_plan_ex": (_i, [_desc, _vp]),
+    "gmpi_mpi_render_bwd_ex": (_i, [_desc]),
+    "gmpi_mpi_render_bwd_deterministic_scratch_bytes": (_ll, [_desc]),
+    "gmpi_mpi_render_bwd_deterministic_ex": (_i, [_desc, _vp, _size]),
+    "gmpi_mpi_occupancy_bytes": (_ll, [_desc]),
+    "gmpi_mpi_build_occupancy": (_i, [_desc, _vp, _size]),
+    "gmpi_mpi_render_fwd_skip_ex": (_i, [_desc, _vp, _size]),
+    "gmpi_mpi_render_host_ex": (_i, [_desc, _i]),
+    "gmpi_mpi_alpha_depth_fwd": (_i, [_vp, _ll, _ll, _vp, _vp, _vp] + [_i] * 4 + [_vp]),
+    "gmpi_mpi_alpha_depth_bwd": (_i, [_vp, _ll, _ll, _vp, _vp, _vp, _vp, _ll, _ll] + [_i] * 4 + [_vp]),
+    "gmpi_mpi_apply_shading_fwd": (_i, [_vp] * 3 + [_i] * 4 + [_vp]),
+    "gmpi_mpi_apply_shading_bwd": (_i, [_vp] * 5 + [_i] * 4 + [_vp]),
+    "gmpi_mpi_check_range": (_i, [_vp] + [_i] * 4 + [_vp, _vp]),
+    "gmpi_mpi_check_range_f16": (_i, [_vp] + [_i] * 4 + [_vp, _vp]),
+    "gmpi_mpi_render_fwd_host": (_i, [_vp] * 9 + [_i] * 7 + [_u32, _i]),
+    "gmpi_mpi_release_host_cache": (_i, []),
+    "gmpi_debug_plane_coords": (_i, [_vp] * 5 + [_i] * 6 + [_u32, _vp]),
+    "gmpi_debug_plane_coords_packed": (_i, [_vp] * 5 + [_i] * 6 + [_u32, _vp]),
+    "gmpi_debug_set_fwd_variant": (_i, [_i]),
+    "gmpi_debug_set_fwd_stages": (_i, [_i]),
+    "gmpi_debug_fwd_early_stop_stats": (_i, [_vp, _vp]),
+    "gmpi_debug_fwd_skip_stats": (_i, [_vp, _vp]),
+    "gmpi_debug_box_occupied": (_i, [_vp] + [_i] * 6),
+    "gmpi_debug_fwd_ring_stages": (_i, [_i] * 6),
+    "gmpi_debug_copy_plan": (_i, [_i, _vp, _i]),
+    "gmpi_debug_tile_walk_ex": (_i, [_i] * 7 + [_vp, _i]),
+    "gmpi_debug_cam_rays": (_i, [_vp, _vp, _i, _i, _i, _vp]),
+    "gmpi_debug_tile_walk": (_i, [_i] * 5 + [_vp, _i]),
+    "gmpi_debug_division": (_i, [_vp] * 4 + [_size, _vp]),
+}
+EXPORTS = sorted(SIGNATURES)
 
 
 def make_desc(**kw) -> RenderDesc:
@@ -87,86 +123,9 @@ def load():
             f"{path} is missing: the CUDA (sm_90a) renderer is not built. Run "
             "`python -c 'import __graft_entry__ as g; g.build()'` (needs nvcc). There is no CPU fallback.")
     lib = ctypes.CDLL(path)
-    vp, i, u32 = ctypes.c_void_p, ctypes.c_int, ctypes.c_uint32
-    lib.gmpi_abi_version.restype = i
-    lib.gmpi_abi_version.argtypes = []
-    lib.gmpi_last_error.restype = ctypes.c_char_p
-    lib.gmpi_last_error.argtypes = []
-    lib.gmpi_mpi_render_fwd_variant.restype = ctypes.c_char_p
-    lib.gmpi_mpi_render_fwd_variant.argtypes = [i] * 5
-    lib.gmpi_mpi_render_fwd_plan.restype = i
-    lib.gmpi_mpi_render_fwd_plan.argtypes = [i] * 6 + [vp, vp]
-    lib.gmpi_mpi_render_fwd.restype = i
-    lib.gmpi_mpi_render_fwd.argtypes = [vp] * 9 + [i] * 7 + [u32, vp]
-    lib.gmpi_mpi_render_fwd_gather.restype = i
-    lib.gmpi_mpi_render_fwd_gather.argtypes = [vp] * 7 + [i, i, vp] + [i] * 7 + [u32, vp]
-    lib.gmpi_mpi_render_fwd_train.restype = i
-    lib.gmpi_mpi_render_fwd_train.argtypes = [vp] * 10 + [i] * 7 + [u32, vp]
-    lib.gmpi_mpi_render_bwd_saved.restype = i
-    lib.gmpi_mpi_render_bwd_saved.argtypes = [vp] * 10 + [i] * 7 + [u32, vp]
-    lib.gmpi_mpi_render_bwd.restype = i
-    lib.gmpi_mpi_render_bwd.argtypes = [vp] * 9 + [i] * 7 + [u32, vp]
-    lib.gmpi_mpi_check_range.restype = i
-    lib.gmpi_mpi_check_range.argtypes = [vp, i, i, i, i, vp, vp]
-    lib.gmpi_mpi_check_range_f16.restype = i
-    lib.gmpi_mpi_check_range_f16.argtypes = [vp, i, i, i, i, vp, vp]
-    lib.gmpi_mpi_render_fwd_host.restype = i
-    lib.gmpi_mpi_render_fwd_host.argtypes = [vp] * 9 + [i] * 7 + [u32, i]
-    lib.gmpi_mpi_release_host_cache.restype = i
-    lib.gmpi_mpi_release_host_cache.argtypes = []
-    lib.gmpi_debug_plane_coords.restype = i
-    lib.gmpi_debug_plane_coords.argtypes = [vp] * 5 + [i] * 6 + [u32, vp]
-    lib.gmpi_debug_plane_coords_packed.restype = i
-    lib.gmpi_debug_plane_coords_packed.argtypes = [vp] * 5 + [i] * 6 + [u32, vp]
-    lib.gmpi_debug_division.restype = i
-    lib.gmpi_debug_division.argtypes = [vp, vp, vp, vp, ctypes.c_size_t, vp]
-    lib.gmpi_debug_set_fwd_variant.restype = i
-    lib.gmpi_debug_set_fwd_variant.argtypes = [i]
-    lib.gmpi_debug_set_fwd_stages.restype = i
-    lib.gmpi_debug_set_fwd_stages.argtypes = [i]
-    lib.gmpi_debug_fwd_early_stop_stats.restype = i
-    lib.gmpi_debug_fwd_early_stop_stats.argtypes = [vp, vp]
-    lib.gmpi_debug_fwd_ring_stages.restype = i
-    lib.gmpi_debug_fwd_ring_stages.argtypes = [i] * 6
-    lib.gmpi_debug_copy_plan.restype = i
-    lib.gmpi_debug_copy_plan.argtypes = [i, vp, i]
-    lib.gmpi_debug_tile_walk.restype = i
-    lib.gmpi_debug_tile_walk.argtypes = [i, i, i, i, i, vp, i]
-    lib.gmpi_debug_tile_walk_ex.restype = i
-    lib.gmpi_debug_tile_walk_ex.argtypes = [i, i, i, i, i, i, i, vp, i]
-    lib.gmpi_debug_cam_rays.restype = i
-    lib.gmpi_debug_cam_rays.argtypes = [vp, vp, i, i, i, vp]
-    for fn in (lib.gmpi_mpi_render_fwd_ex, lib.gmpi_mpi_render_bwd_ex):
-        fn.restype = i
-        fn.argtypes = [ctypes.POINTER(RenderDesc)]
-    lib.gmpi_mpi_zero_async.restype = i
-    lib.gmpi_mpi_zero_async.argtypes = [vp, ctypes.c_size_t, vp]
-    ll = ctypes.c_longlong
-    lib.gmpi_mpi_alpha_depth_fwd.restype = i
-    lib.gmpi_mpi_alpha_depth_fwd.argtypes = [vp, ll, ll, vp, vp, vp, i, i, i, i, vp]
-    lib.gmpi_mpi_alpha_depth_bwd.restype = i
-    lib.gmpi_mpi_alpha_depth_bwd.argtypes = [vp, ll, ll, vp, vp, vp, vp, ll, ll, i, i, i, i, vp]
-    lib.gmpi_mpi_apply_shading_fwd.restype = i
-    lib.gmpi_mpi_apply_shading_fwd.argtypes = [vp, vp, vp, i, i, i, i, vp]
-    lib.gmpi_mpi_apply_shading_bwd.restype = i
-    lib.gmpi_mpi_apply_shading_bwd.argtypes = [vp, vp, vp, vp, vp, i, i, i, i, vp]
-    lib.gmpi_mpi_render_host_ex.restype = i
-    lib.gmpi_mpi_render_host_ex.argtypes = [ctypes.POINTER(RenderDesc), i]
-    lib.gmpi_mpi_render_fwd_plan_ex.restype = i
-    lib.gmpi_mpi_render_fwd_plan_ex.argtypes = [ctypes.POINTER(RenderDesc), vp]
-    lib.gmpi_mpi_render_bwd_deterministic_scratch_bytes.restype = ll
-    lib.gmpi_mpi_render_bwd_deterministic_scratch_bytes.argtypes = [ctypes.POINTER(RenderDesc)]
-    lib.gmpi_mpi_render_bwd_deterministic_ex.restype = i
-    lib.gmpi_mpi_render_bwd_deterministic_ex.argtypes = [ctypes.POINTER(RenderDesc), vp, ctypes.c_size_t]
-    lib.gmpi_mpi_occupancy_bytes.restype = ll
-    lib.gmpi_mpi_occupancy_bytes.argtypes = [ctypes.POINTER(RenderDesc)]
-    for fn in (lib.gmpi_mpi_build_occupancy, lib.gmpi_mpi_render_fwd_skip_ex):
-        fn.restype = i
-        fn.argtypes = [ctypes.POINTER(RenderDesc), vp, ctypes.c_size_t]
-    lib.gmpi_debug_fwd_skip_stats.restype = i
-    lib.gmpi_debug_fwd_skip_stats.argtypes = [vp, vp]
-    lib.gmpi_debug_box_occupied.restype = i
-    lib.gmpi_debug_box_occupied.argtypes = [vp] + [i] * 6
+    for name, (restype, argtypes) in SIGNATURES.items():
+        fn = getattr(lib, name)
+        fn.restype, fn.argtypes = restype, argtypes
     if lib.gmpi_abi_version() != ABI_VERSION:
         raise GmpiLibraryError(f"ABI mismatch: library {lib.gmpi_abi_version()} != binding {ABI_VERSION}; rebuild")
     _lib = lib

@@ -106,13 +106,11 @@ class FrameGather:
                color_minus1_1=False, early_stop=None):
         """early_stop: early ray termination threshold in [0, 1), as in render_frames (None: off).  An fp16 rgba renders natively
         where render_frames would (GMPI_MPI_F16), else from its fp32 upcast."""
-        import ctypes
         from . import _lib
-        from .mpi import _launch_mpi, _options
-        lib = _lib.load()
-        M, N, _, Ht, Wt = rgba.shape
+        from .mpi import _launch_mpi, _mpi_desc, _options, _render_fwd
+        _lib.load()                     # a missing library is reported before the arguments are checked
         V = ray_dir.shape[0]
-        assert V <= self.frames_per_rank and ray_dir.shape[2:] == (self.H, self.W)
+        assert rgba.ndim == 5 and V <= self.frames_per_rank and ray_dir.shape[2:] == (self.H, self.W)
         options = _options(align_corners, check_last_plane, color_minus1_1, early_stop=early_stop)
         if rgba.dtype == torch.float16:     # any other MPI is rendered as passed (asserted below)
             (rgba, _, _, _), options = _launch_mpi([rgba, None, None, None], V, self.H, self.W, options)
@@ -122,12 +120,10 @@ class FrameGather:
                                ("z_dir", z_dir, f32)):   # raw pointers below
             assert t.is_cuda and t.dtype == dtype and t.is_contiguous(), f"{name} must be a contiguous {dtype} CUDA tensor"
         assert view2mpi.dtype == torch.int32 and view2mpi.is_contiguous() and flags.dtype == torch.int32
-        with torch.cuda.device(rgba.device):
-            d = _lib.make_desc(options=options, M=M, V=V, N=N, Ht=Ht, Wt=Wt, H=self.H, W=self.W, rgba=rgba, view2mpi=view2mpi, dhw=dhw,
-                               ray_dir=ray_dir, eye=eye, z_dir=z_dir, peer_frames=self._peer_ptrs[self._next],
-                               n_peers=int(self._peer_ptrs[self._next].numel()), frame_offset=self.rank * self.frames_per_rank,
-                               flags=flags, stream=torch.cuda.current_stream(rgba.device).cuda_stream, early_stop=early_stop)
-            _lib.check(lib.gmpi_mpi_render_fwd_ex(ctypes.byref(d)))
+        peers = self._peer_ptrs[self._next]
+        _render_fwd(_mpi_desc([rgba, None, None, None], V, self.H, self.W, options, view2mpi=view2mpi, dhw=dhw, ray_dir=ray_dir,
+                              eye=eye, z_dir=z_dir, peer_frames=peers, n_peers=int(peers.numel()),
+                              frame_offset=self.rank * self.frames_per_rank, flags=flags, early_stop=early_stop), None, rgba.device)
 
     def finish(self):
         """Barrier across ranks on the current stream: after it, every rank's `frames` holds all ranks' frames."""

@@ -23,12 +23,9 @@ import torch.nn.functional as F
 
 from . import _lib
 from .camera import sample_yaw_pitch, sphere_poses
+from .mpi import _require_cuda, _stream_ptr
 
 EPS = 1e-8          # light_renderer.py:8
-
-
-def _stream_ptr(device):
-    return torch.cuda.current_stream(device).cuda_stream
 
 
 def _streamable(t: torch.Tensor) -> torch.Tensor:
@@ -111,8 +108,7 @@ class _ApplyShadingFn(torch.autograd.Function):
 
 def alpha_depth(mpi_alpha: torch.Tensor, plane_ds: torch.Tensor) -> torch.Tensor:
     """LightRenderer.compute_depth (light_renderer.py:82-100): [B,N,1,H,W] alpha, [N] plane distances -> [B,1,H,W]."""
-    if not mpi_alpha.is_cuda:
-        raise RuntimeError("ml_gmpi_b200 runs on CUDA devices only (no CPU fallback); got a CPU tensor")
+    _require_cuda(mpi_alpha, "ml_gmpi_b200 runs")
     pd = plane_ds.reshape(-1).to(device=mpi_alpha.device, dtype=torch.float32).contiguous()
     B, N, _, H, W = mpi_alpha.shape
     assert pd.numel() == N, f"{mpi_alpha.shape}, {plane_ds.shape}"
@@ -128,8 +124,7 @@ def alpha_depth(mpi_alpha: torch.Tensor, plane_ds: torch.Tensor) -> torch.Tensor
 
 def apply_shading(batch_mpi: torch.Tensor, shading: torch.Tensor) -> torch.Tensor:
     """clip(rgb * shading, 0, 1) on the colour channels, alpha unchanged (light_renderer.py:190-199): [B,N,4,H,W] x [B,1,H,W]."""
-    if not batch_mpi.is_cuda:
-        raise RuntimeError("ml_gmpi_b200 runs on CUDA devices only (no CPU fallback); got a CPU tensor")
+    _require_cuda(batch_mpi, "ml_gmpi_b200 runs")
     B, N, C, H, W = batch_mpi.shape
     assert C == 4, f"{batch_mpi.shape}"
     if (H * W) % 4:

@@ -25,6 +25,15 @@ def _stream_ptr(device):
     return torch.cuda.current_stream(device).cuda_stream
 
 
+def _require_cuda(t: torch.Tensor, who: str = "ml_gmpi_b200 renders"):
+    if not t.is_cuda:
+        raise RuntimeError(f"{who} on CUDA devices only (no CPU fallback); got a CPU tensor")
+
+
+def _zero_flags(device) -> torch.Tensor:
+    return torch.zeros(1, dtype=torch.int32, device=device)
+
+
 def _as_f32c(t: torch.Tensor) -> torch.Tensor:
     if t.dtype != torch.float32:
         t = t.float()
@@ -38,12 +47,9 @@ class _RenderFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, rgba, rgb, alpha, bg_rgb, dhw, view2mpi, ray_dir, eye, z_dir, options, flags, view_group, early_stop,
                 deterministic, occ=None):
-        lib = _lib.load()
-        factored = rgba is None
-        ref = alpha if factored else rgba
-        M, N = ref.shape[0], ref.shape[1]
-        Ht, Wt = ref.shape[-2:]
+        mpi = [rgba, rgb, alpha, bg_rgb]
         V, _, H, W = ray_dir.shape
+        ref = _mpi_ref(mpi)
         dev = ref.device
         color = torch.empty((V, 3, H, W), device=dev, dtype=torch.float32)
         depth = torch.empty((V, 1, H, W), device=dev, dtype=torch.float32)
@@ -51,16 +57,10 @@ class _RenderFn(torch.autograd.Function):
         # backward is ONE staged back-to-front sweep (torch autograd keeps ~30 such tensors alive for the reference)
         trans = None
         if any(ctx.needs_input_grad[:4]):
-            trans = torch.empty((V, N, H, W), device=dev, dtype=torch.float32)
-        with torch.cuda.device(dev):
-            d = _lib.make_desc(options=options, M=M, V=V, N=N, Ht=Ht, Wt=Wt, H=H, W=W, view_group=view_group, rgba=rgba, rgb=rgb,
-                               alpha=alpha, bg_rgb=bg_rgb, view2mpi=view2mpi, dhw=dhw, ray_dir=ray_dir, eye=eye, z_dir=z_dir,
-                               color=color, depth=depth, transmittance=trans, flags=flags, stream=_stream_ptr(dev),
-                               early_stop=early_stop)
-            if occ is not None:
-                _lib.check(lib.gmpi_mpi_render_fwd_skip_ex(ctypes.byref(d), occ.data_ptr(), occ.nbytes))
-            else:
-                _lib.check(lib.gmpi_mpi_render_fwd_ex(ctypes.byref(d)))
+            trans = torch.empty((V, ref.shape[1], H, W), device=dev, dtype=torch.float32)
+        _render_fwd(_mpi_desc(mpi, V, H, W, options, view_group=view_group, view2mpi=view2mpi, dhw=dhw, ray_dir=ray_dir, eye=eye,
+                              z_dir=z_dir, color=color, depth=depth, transmittance=trans, flags=flags, early_stop=early_stop),
+                    occ, dev)
         ctx.save_for_backward(rgba, rgb, alpha, bg_rgb, dhw, view2mpi, ray_dir, eye, z_dir, trans)
         ctx.options, ctx.view_group = options, view_group
         # None: torch's global switch, read now (the backward may run on an autograd thread, after the caller changed it)
@@ -76,19 +76,16 @@ class _RenderFn(torch.autograd.Function):
         if not any(ctx.needs_input_grad[:4]):
             return none
         lib = _lib.load()
-        factored = rgba is None
-        ref = alpha if factored else rgba
-        M, N = ref.shape[0], ref.shape[1]
-        Ht, Wt = ref.shape[-2:]
+        mpi = [rgba, rgb, alpha, bg_rgb]
         V, _, H, W = ray_dir.shape
-        dev = ref.device
+        dev = _mpi_ref(mpi).device
         if g_color is None:
             g_color = torch.zeros((V, 3, H, W), device=dev, dtype=torch.float32)
         g_color = _as_f32c(g_color)
         g_depth = _as_f32c(g_depth) if g_depth is not None else None
         # GMPI_ZERO_GRAD: the callee zeroes the buffers on the stream.  (Zeroing them on a side stream during the forward, as an
         # earlier version did, buys nothing: a memset cannot overlap the persistent kernels -- tools/zero_overlap_probe.py.)
-        if factored:
+        if rgba is None:
             g_rgba = None
             g_rgb, g_alpha = torch.empty_like(rgb), torch.empty_like(alpha)
             g_bg = torch.empty_like(bg_rgb) if bg_rgb is not None else None
@@ -96,10 +93,9 @@ class _RenderFn(torch.autograd.Function):
             g_rgb = g_alpha = g_bg = None
             g_rgba = torch.empty_like(rgba)
         with torch.cuda.device(dev):   # autograd worker threads do not inherit the device
-            d = _lib.make_desc(options=ctx.options | _lib.OPT_ZERO_GRAD, M=M, V=V, N=N, Ht=Ht, Wt=Wt, H=H, W=W,
-                               view_group=ctx.view_group, rgba=rgba, rgb=rgb, alpha=alpha, bg_rgb=bg_rgb, view2mpi=view2mpi, dhw=dhw,
-                               ray_dir=ray_dir, eye=eye, z_dir=z_dir, transmittance=trans, g_color=g_color, g_depth=g_depth,
-                               g_rgba=g_rgba, g_rgb=g_rgb, g_bg_rgb=g_bg, g_alpha=g_alpha, stream=_stream_ptr(dev))
+            d = _mpi_desc(mpi, V, H, W, ctx.options | _lib.OPT_ZERO_GRAD, view_group=ctx.view_group, view2mpi=view2mpi, dhw=dhw,
+                          ray_dir=ray_dir, eye=eye, z_dir=z_dir, transmittance=trans, g_color=g_color, g_depth=g_depth,
+                          g_rgba=g_rgba, g_rgb=g_rgb, g_bg_rgb=g_bg, g_alpha=g_alpha, stream=_stream_ptr(dev))
             if ctx.deterministic:
                 # bitwise-reproducible gradients from exact int64 sums (8 B of scratch per gradient element)
                 nbytes = _lib.deterministic_scratch_bytes(d)
@@ -110,13 +106,30 @@ class _RenderFn(torch.autograd.Function):
         return (g_rgba, g_rgb, g_alpha, g_bg) + (None,) * 11
 
 
-def _mpi_desc(mpi, V, H, W, options):
-    """Descriptor of what the forward plan reads (sizes, options, MPI pointers) for the MPI tensors `mpi` = [rgba, rgb, alpha, bg_rgb]
-    rendered from V views of H x W pixels."""
-    rgba, rgb, alpha, bg_rgb = mpi
-    ref = alpha if rgba is None else rgba
+def _mpi_ref(mpi) -> torch.Tensor:
+    """The tensor of `mpi` = [rgba, rgb, alpha, bg_rgb] whose shape [M,N,_,Ht,Wt] and device a render takes: rgba, or the alpha of a
+    factored MPI."""
+    rgba, _, alpha, _ = mpi
+    return alpha if rgba is None else rgba
+
+
+def _mpi_desc(mpi, V, H, W, options, **fields):
+    """Descriptor of a render of the MPI tensors `mpi` = [rgba, rgb, alpha, bg_rgb] (None where absent) from V views of H x W pixels:
+    sizes, options and MPI pointers, plus the other descriptor `fields` (tensors or values, see _lib.make_desc)."""
+    ref = _mpi_ref(mpi)
     return _lib.make_desc(options=options, M=ref.shape[0], V=V, N=ref.shape[1], Ht=ref.shape[-2], Wt=ref.shape[-1], H=H, W=W,
-                          rgba=rgba, rgb=rgb, alpha=alpha, bg_rgb=bg_rgb)
+                          rgba=mpi[0], rgb=mpi[1], alpha=mpi[2], bg_rgb=mpi[3], **fields)
+
+
+def _render_fwd(d, occ: Optional["Occupancy"], device):
+    """Launch the forward `d` describes on `device`'s current stream; with an Occupancy `occ`, with empty-space skipping."""
+    lib = _lib.load()
+    with torch.cuda.device(device):
+        d.stream = _stream_ptr(device)
+        if occ is not None:
+            _lib.check(lib.gmpi_mpi_render_fwd_skip_ex(ctypes.byref(d), occ.data_ptr(), occ.nbytes))
+        else:
+            _lib.check(lib.gmpi_mpi_render_fwd_ex(ctypes.byref(d)))
 
 
 def _half_mpi(mpi, V, H, W, options):
@@ -160,7 +173,7 @@ def _warn_if_direct(d):
     if plan == _lib.PLAN_DIRECT and (why & ~2 or d.V * d.N * d.H * d.W >= 1 << 26):   # "few tiles" only matters when the problem is not tiny
         reasons = "; ".join(t for b, t in _lib.WHY.items() if why & b)
         warnings.warn(f"ml_gmpi_b200: rendering V={d.V} N={d.N} tex={d.Ht}x{d.Wt} img={d.H}x{d.W} with the direct (one thread per "
-                      f"pixel) kernels, several times slower than the TMA-staged path: {reasons}", RuntimeWarning, stacklevel=3)
+                      f"pixel) kernels, several times slower than the TMA-staged path: {reasons}", RuntimeWarning, stacklevel=4)
 
 
 def _options(align_corners, check_last_plane, color_minus1_1, u8_round=False, early_stop=None):
@@ -169,11 +182,13 @@ def _options(align_corners, check_last_plane, color_minus1_1, u8_round=False, ea
         | (_lib.OPT_EARLY_STOP if early_stop is not None else 0)
 
 
-def _check_early_stop_without_grad(early_stop, *inputs):
-    """early_stop drops the planes behind opaque content, which the backward needs: refuse it where autograd would record."""
-    if early_stop is not None and torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in inputs):
-        raise RuntimeError("ml_gmpi_b200: early_stop is forward-only (it skips the planes the backward needs); render under "
-                           "torch.no_grad() or from inputs that do not require grad")
+def _check_forward_only(option: str, is_set: bool, *inputs):
+    """The backward needs every plane: early_stop drops the planes behind opaque content, and skip_empty the empty ones whose
+    transmittance the training forward saves.  Refuse a set `option` where autograd would record."""
+    if is_set and torch.is_grad_enabled() and any(t is not None and t.requires_grad for t in inputs):
+        why = " (it skips the planes the backward needs)" if option == "early_stop" else ""
+        raise RuntimeError(f"ml_gmpi_b200: {option} is forward-only{why}; render under torch.no_grad() or from inputs that do not "
+                           "require grad")
 
 
 class Occupancy:
@@ -205,9 +220,8 @@ def build_occupancy(*, rgba=None, rgb=None, alpha=None, bg_rgb=None, flags: Opti
     factored MPI's colour is read once, its alpha per plane).  `flags` (expanded MPI): also OR in the range-check bits check_range
     sets, from the same pass."""
     mpi = [rgba, rgb, alpha, bg_rgb]
-    ref = alpha if rgba is None else rgba
-    if not ref.is_cuda:
-        raise RuntimeError("ml_gmpi_b200 renders on CUDA devices only (no CPU fallback); got a CPU tensor")
+    ref = _mpi_ref(mpi)
+    _require_cuda(ref)
     ts = [t for t in mpi if t is not None]
     half = all(t.dtype == torch.float16 for t in ts)     # the map of an fp16 MPI is the map of its fp32 upcast
     launch = [None if t is None else (t.detach().contiguous() if half else _as_f32c(t.detach())) for t in mpi]
@@ -234,14 +248,6 @@ def _occupancy_for(skip_empty, mpi) -> Optional[Occupancy]:
     return skip_empty
 
 
-def _check_skip_without_grad(skip_empty, *inputs):
-    """The training forward saves the transmittance for the backward, which needs every plane: skip_empty is forward-only."""
-    if skip_empty is not False and skip_empty is not None and torch.is_grad_enabled() and \
-            any(t is not None and t.requires_grad for t in inputs):
-        raise RuntimeError("ml_gmpi_b200: skip_empty is forward-only; render under torch.no_grad() or from inputs that do not "
-                           "require grad")
-
-
 def render_views(rgba, dhw, view2mpi, ray_dir, eye, z_dir, *, align_corners=True, check_last_plane=False,
                  color_minus1_1=False, flags: Optional[torch.Tensor] = None, view_group: int = 1, early_stop: Optional[float] = None,
                  deterministic: Optional[bool] = None, skip_empty: Union[bool, Occupancy] = False):
@@ -256,19 +262,8 @@ def render_views(rgba, dhw, view2mpi, ray_dir, eye, z_dir, *, align_corners=True
     skip_empty: empty-space skipping (gmpi_mpi_render_fwd_skip_ex): the staged kernel does not load or composite the (tile, plane)
     boxes whose texels all have alpha +0 and finite colour; bitwise the same output.  True builds the map for this call
     (build_occupancy, one pass over the MPI); an Occupancy is reused.  Forward only: refused when an input requires grad."""
-    _check_early_stop_without_grad(early_stop, rgba)
-    _check_skip_without_grad(skip_empty, rgba)
-    if not rgba.is_cuda:
-        raise RuntimeError("ml_gmpi_b200 renders on CUDA devices only (no CPU fallback); got a CPU tensor")
-    if flags is None:
-        flags = torch.zeros(1, dtype=torch.int32, device=rgba.device)
-    occ = _occupancy_for(skip_empty, [rgba, None, None, None])
-    V, _, H, W = ray_dir.shape
-    mpi, options = _launch_mpi([rgba, None, None, None], V, H, W,
-                               _options(align_corners, check_last_plane, color_minus1_1, early_stop=early_stop))
-    _warn_if_direct(_mpi_desc(mpi, V, H, W, options))
-    return _RenderFn.apply(*mpi, _as_f32c(dhw), view2mpi, _as_f32c(ray_dir), _as_f32c(eye), _as_f32c(z_dir),
-                           options, flags, int(view_group), early_stop, deterministic, occ)
+    return _render_views([rgba, None, None, None], dhw, view2mpi, ray_dir, eye, z_dir, align_corners, check_last_plane, color_minus1_1,
+                         flags, view_group, early_stop, deterministic, skip_empty)
 
 
 def render_views_factored(rgb, alpha, dhw, view2mpi, ray_dir, eye, z_dir, *, bg_rgb=None, align_corners=True,
@@ -280,19 +275,27 @@ def render_views_factored(rgb, alpha, dhw, view2mpi, ray_dir, eye, z_dir, *, bg_
     alpha [M,N,1,Ht,Wt] -- what the reference expands to [M,N,4,Ht,Wt] (and copies per view, train.py:553-558,733-738) before
     rendering.  Output identical to render_views on the expanded stack, 4x fewer HBM bytes; differentiable w.r.t. rgb, alpha
     and bg_rgb (d/d rgb is the sum over the planes that share it).  early_stop, deterministic, skip_empty: as in render_views."""
-    _check_early_stop_without_grad(early_stop, rgb, alpha, bg_rgb)
-    _check_skip_without_grad(skip_empty, rgb, alpha, bg_rgb)
-    if not alpha.is_cuda:
-        raise RuntimeError("ml_gmpi_b200 renders on CUDA devices only (no CPU fallback); got a CPU tensor")
-    assert rgb.ndim == 4 and rgb.shape[1] == 3 and alpha.ndim == 5 and alpha.shape[2] == 1 and rgb.shape[0] == alpha.shape[0] \
-        and rgb.shape[-2:] == alpha.shape[-2:], f"expected rgb [M,3,Ht,Wt] and alpha [M,N,1,Ht,Wt], got {rgb.shape}, {alpha.shape}"
-    assert bg_rgb is None or bg_rgb.shape == rgb.shape, f"bg_rgb must have rgb's shape, got {bg_rgb.shape}"
+    return _render_views([None, rgb, alpha, bg_rgb], dhw, view2mpi, ray_dir, eye, z_dir, align_corners, check_last_plane, color_minus1_1,
+                         flags, view_group, early_stop, deterministic, skip_empty)
+
+
+def _render_views(mpi, dhw, view2mpi, ray_dir, eye, z_dir, align_corners, check_last_plane, color_minus1_1, flags, view_group,
+                  early_stop, deterministic, skip_empty):
+    """render_views of the MPI tensors `mpi` = [rgba, rgb, alpha, bg_rgb] (None where absent), and render_views_factored."""
+    _check_forward_only("early_stop", early_stop is not None, *mpi)
+    _check_forward_only("skip_empty", skip_empty is not False and skip_empty is not None, *mpi)
+    ref = _mpi_ref(mpi)
+    _require_cuda(ref)
+    rgba, rgb, alpha, bg_rgb = mpi
+    if rgba is None:
+        assert rgb.ndim == 4 and rgb.shape[1] == 3 and alpha.ndim == 5 and alpha.shape[2] == 1 and rgb.shape[0] == alpha.shape[0] \
+            and rgb.shape[-2:] == alpha.shape[-2:], f"expected rgb [M,3,Ht,Wt] and alpha [M,N,1,Ht,Wt], got {rgb.shape}, {alpha.shape}"
+        assert bg_rgb is None or bg_rgb.shape == rgb.shape, f"bg_rgb must have rgb's shape, got {bg_rgb.shape}"
     if flags is None:
-        flags = torch.zeros(1, dtype=torch.int32, device=alpha.device)
-    occ = _occupancy_for(skip_empty, [None, rgb, alpha, bg_rgb])
+        flags = _zero_flags(ref.device)
+    occ = _occupancy_for(skip_empty, mpi)
     V, _, H, W = ray_dir.shape
-    mpi, options = _launch_mpi([None, rgb, alpha, bg_rgb], V, H, W,
-                               _options(align_corners, check_last_plane, color_minus1_1, early_stop=early_stop))
+    mpi, options = _launch_mpi(mpi, V, H, W, _options(align_corners, check_last_plane, color_minus1_1, early_stop=early_stop))
     _warn_if_direct(_mpi_desc(mpi, V, H, W, options))
     return _RenderFn.apply(*mpi, _as_f32c(dhw), view2mpi, _as_f32c(ray_dir), _as_f32c(eye), _as_f32c(z_dir),
                            options, flags, int(view_group), early_stop, deterministic, occ)
@@ -320,13 +323,11 @@ def render_frames(*, dhw, view2mpi, rgba=None, rgb=None, alpha=None, bg_rgb=None
       early_stop=tau in [0, 1)   early ray termination: a pixel composites no further plane once its transmittance |T| <= tau
                      (colour in [-1,1] moves by at most 2 tau per channel, a uint8 code by at most one; see render_views).
     """
-    ref = alpha if rgba is None else rgba
-    if not ref.is_cuda:
-        raise RuntimeError("ml_gmpi_b200 renders on CUDA devices only (no CPU fallback); got a CPU tensor")
-    lib = _lib.load()
+    mpi = [rgba, rgb, alpha, bg_rgb]
+    ref = _mpi_ref(mpi)
+    _require_cuda(ref)
+    _lib.load()                     # a missing library is reported before the arguments are checked
     dev = ref.device
-    M, N = ref.shape[0], ref.shape[1]
-    Ht, Wt = ref.shape[-2:]
     if cam is not None:
         V = cam.shape[0]
         assert H is not None and W is not None, "pass H and W with cam"
@@ -335,7 +336,7 @@ def render_frames(*, dhw, view2mpi, rgba=None, rgb=None, alpha=None, bg_rgb=None
         V, _, H, W = ray_dir.shape
         ray_dir, eye, z_dir = _as_f32c(ray_dir), _as_f32c(eye), _as_f32c(z_dir)
     if flags is None:
-        flags = torch.zeros(1, dtype=torch.int32, device=dev)
+        flags = _zero_flags(dev)
     color = depth = v_rgb = v_depth = None
     near = rng = 0.0
     if video is not None:
@@ -347,18 +348,11 @@ def render_frames(*, dhw, view2mpi, rgba=None, rgb=None, alpha=None, bg_rgb=None
     else:
         color = torch.empty((V, 3, H, W), device=dev, dtype=torch.float32)
         depth = torch.empty((V, 1, H, W), device=dev, dtype=torch.float32)
-    occ = _occupancy_for(skip_empty, [rgba, rgb, alpha, bg_rgb])
-    mpi, options = _launch_mpi([rgba, rgb, alpha, bg_rgb], V, H, W, _options(align_corners, check_last_plane, True, u8_round, early_stop))
-    dhw = _as_f32c(dhw)
-    with torch.cuda.device(dev):
-        d = _lib.make_desc(options=options, M=M, V=V, N=N, Ht=Ht, Wt=Wt, H=H, W=W,
-                           view_group=int(view_group), depth_near=near, depth_range=rng, rgba=mpi[0], rgb=mpi[1], alpha=mpi[2],
-                           bg_rgb=mpi[3], view2mpi=view2mpi, dhw=dhw, ray_dir=ray_dir, eye=eye, z_dir=z_dir, cam=cam, color=color,
-                           depth=depth, video_rgb=v_rgb, video_depth=v_depth, flags=flags, stream=_stream_ptr(dev), early_stop=early_stop)
-        if occ is not None:
-            _lib.check(lib.gmpi_mpi_render_fwd_skip_ex(ctypes.byref(d), occ.data_ptr(), occ.nbytes))
-        else:
-            _lib.check(lib.gmpi_mpi_render_fwd_ex(ctypes.byref(d)))
+    occ = _occupancy_for(skip_empty, mpi)
+    mpi, options = _launch_mpi(mpi, V, H, W, _options(align_corners, check_last_plane, True, u8_round, early_stop))
+    _render_fwd(_mpi_desc(mpi, V, H, W, options, view_group=int(view_group), depth_near=near, depth_range=rng, view2mpi=view2mpi,
+                          dhw=_as_f32c(dhw), ray_dir=ray_dir, eye=eye, z_dir=z_dir, cam=cam, color=color, depth=depth, video_rgb=v_rgb,
+                          video_depth=v_depth, flags=flags, early_stop=early_stop), occ, dev)
     return (v_rgb, v_depth) if video is not None else (color, depth)
 
 
@@ -446,16 +440,15 @@ class MPI(nn.Module):
                 c2w_mat: torch.Tensor = None, sphere_c: np.ndarray = None):
         self.check_shapes(batch_rgba=batch_rgba, batch_dhw=batch_dhw, batch_ray_dir=batch_ray_dir,
                           batch_eye_pos=batch_eye_pos, batch_z_dir=batch_z_dir, separate_background=separate_background)
-        if not batch_rgba.is_cuda:
-            raise RuntimeError("ml_gmpi_b200.MPI renders on CUDA devices only (no CPU fallback); got a CPU tensor")
+        _require_cuda(batch_rgba, "ml_gmpi_b200.MPI renders")
         dev = batch_rgba.device
         view2mpi, ray_dir, eye, z_dir = self.pack_views(batch_ray_dir, batch_eye_pos, batch_z_dir, dev)
         # an fp16 MPI stays fp16: render_views renders it natively where it can (and upcasts it where it cannot)
         rgba = batch_rgba.contiguous() if batch_rgba.dtype == torch.float16 else _as_f32c(batch_rgba)
-        flags = torch.zeros(1, dtype=torch.int32, device=dev)
+        flags = _zero_flags(dev)
         occ = False
         if self.skip_empty:
-            _check_skip_without_grad(True, batch_rgba)
+            _check_forward_only("skip_empty", True, batch_rgba)
             occ = build_occupancy(rgba=rgba, flags=flags if self.validate == "full" else None)
         elif self.validate == "full":
             check_range(rgba.detach(), flags)

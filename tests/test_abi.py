@@ -24,12 +24,45 @@ def declared_symbols():
     return sorted(set(re.findall(r"\b(gmpi_[a-z0-9_]+)\s*\(", hdr)))
 
 
+C_TYPES = {"int": ctypes.c_int, "uint32_t": ctypes.c_uint32, "size_t": ctypes.c_size_t, "long long": ctypes.c_longlong}
+
+
+def _ctype(decl):
+    """The ctypes type of a C parameter or return declaration (its name, if any, dropped)."""
+    if "*" in decl:
+        if "gmpi_render_desc" in decl:
+            return ctypes.POINTER(_lib.RenderDesc)
+        return ctypes.c_char_p if re.match(r"(const\s+)?char\s*\*$", decl) else ctypes.c_void_p
+    return C_TYPES[decl if decl in C_TYPES else decl.rsplit(" ", 1)[0]]
+
+
+def declared_prototypes():
+    """{name: (return declaration, [parameter declarations])} of every function the header declares."""
+    hdr = open(os.path.join(ROOT, "include", "gmpi_mpi_render.h")).read()
+    hdr = re.sub(r"/\*.*?\*/", "", hdr, flags=re.S)
+    out = {}
+    for ret, name, params in re.findall(r"^([a-z][a-z ]*?\**)\s*(gmpi_[a-z0-9_]+)\s*\(([^)]*)\)\s*;", hdr, re.M):
+        params = " ".join(params.split())
+        out[name] = (ret.strip(), [] if params == "void" else [p.strip() for p in params.split(",")])
+    return out
+
+
 def test_header_symbols_are_exported(lib):
     syms = declared_symbols()
     assert "gmpi_mpi_render_fwd" in syms and "gmpi_mpi_render_bwd" in syms
     for s in syms:
         assert hasattr(lib, s), f"{s} declared in the header but not exported"
     assert sorted(_lib.EXPORTS) == syms
+    # every exported function has a signature that matches its prototype: ctypes' defaults (an int return, int arguments) would
+    # cut 64-bit pointers short
+    protos = declared_prototypes()
+    assert list(_lib.SIGNATURES) == list(protos)              # the header's order
+    for name, (restype, argtypes) in _lib.SIGNATURES.items():
+        ret, params = protos[name]
+        assert restype is _ctype(ret), (name, ret)
+        assert len(argtypes) == len(params), (name, params)
+        for i, (t, p) in enumerate(zip(argtypes, params)):
+            assert t is _ctype(p), (name, i, p)
 
 
 def test_abi_version_and_constants(lib):
