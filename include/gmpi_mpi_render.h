@@ -63,6 +63,7 @@ extern "C" {
                                           instead of numpy's truncating astype (render_video.py:119-126) */
 #define GMPI_EARLY_STOP 32u            /* forward only: early ray termination at gmpi_render_desc.early_stop (see there) */
 #define GMPI_MPI_F16 64u               /* forward only: the descriptor's MPI tensors are IEEE binary16 (see gmpi_render_desc) */
+#define GMPI_MPI_U8 128u               /* forward only: the descriptor's rgba is uint8, code b = b / 255 (see gmpi_render_desc) */
 
 int gmpi_abi_version(void);
 const char* gmpi_last_error(void);
@@ -82,7 +83,7 @@ const char* gmpi_mpi_render_fwd_variant(int N, int Ht, int Wt, int H, int W);
  */
 #define GMPI_PLAN_DIRECT 1
 #define GMPI_PLAN_STAGED 2
-#define GMPI_WHY_TEX_WIDTH 1u    /* Wt % 4 != 0 (fp16: Wt % 8): rows are not 16-byte multiples, no tensor map         */
+#define GMPI_WHY_TEX_WIDTH 1u    /* Wt % 4 != 0 (fp16: Wt % 8, uint8: Wt % 16): rows are not 16-byte multiples, no tensor map */
 #define GMPI_WHY_FEW_TILES 2u    /* fewer than 120 tiles of 64x30 pixels over all views: the persistent grid would idle */
 #define GMPI_WHY_MANY_PLANES 4u  /* N > 512: the per-view plane-constant table does not fit next to the ring, or
                                     M*N >= 2^31 planes over all MPIs                                                    */
@@ -248,6 +249,17 @@ typedef struct gmpi_render_desc {
  * bases (gmpi_mpi_render_fwd_plan_ex); other shapes take the direct kernels.  Accepted by gmpi_mpi_render_fwd_ex and
  * gmpi_mpi_render_host_ex only: a descriptor that also sets transmittance, gmpi_mpi_render_bwd_ex and every classic entry point
  * return GMPI_ERR_UNSUPPORTED.
+ *
+ * GMPI_MPI_U8 (off by default): rgba is uint8 [M,N,4,Ht,Wt] (the planar layout of RGBA8 plane images after the reference's permute,
+ * mpi_utils.py:336-337); the descriptor's rgba pointer is read as a pointer to bytes and code b stands for b / 255 rounded to nearest
+ * in fp32.  The kernels convert each texel tap exactly before the unchanged fp32 arithmetic, so the output (colour, depth, uint8
+ * frames, flags) is bitwise equal to the same call on the fp32 tensor rgba / 255 (on the same kernel variant and ring depth), at a
+ * quarter of the fp32 MPI's bytes read from HBM -- and, through gmpi_mpi_render_host_ex, uploaded.  The staged kernels need
+ * Wt % 16 == 0 and a 16-byte aligned rgba (gmpi_mpi_render_fwd_plan_ex); other shapes take the direct kernels.  Accepted by
+ * gmpi_mpi_render_fwd_ex, gmpi_mpi_render_fwd_skip_ex, gmpi_mpi_render_host_ex, gmpi_mpi_render_fwd_plan_ex, gmpi_mpi_occupancy_bytes
+ * and gmpi_mpi_build_occupancy; composes with GMPI_EARLY_STOP, cam, view_group, the video outputs and the fused gather.  Together
+ * with GMPI_MPI_F16: GMPI_ERR_INVALID_ARGUMENT.  GMPI_ERR_UNSUPPORTED for a factored MPI (rgb / alpha / bg_rgb set), a descriptor
+ * that sets transmittance, the backward calls, the deterministic scratch query and every classic entry point.
  */
 
 /* cudaMemsetAsync(ptr, 0, bytes) on `stream`, for callers that accumulate into their own buffers (no GMPI_ZERO_GRAD).  Note that a
@@ -256,8 +268,8 @@ int gmpi_mpi_zero_async(void* ptr, size_t bytes, void* stream);
 
 int gmpi_mpi_render_fwd_ex(const gmpi_render_desc* desc);
 /* gmpi_mpi_render_fwd_plan for the forward a descriptor describes (sizes, options, MPI pointers; the other fields are not read):
- * the plan gmpi_mpi_render_fwd_ex launches with.  It sees GMPI_MPI_F16: an fp16 MPI needs Wt % 8 == 0
- * for the staged kernels (GMPI_WHY_TEX_WIDTH otherwise).  The MPI's pointers (rgba, or rgb + alpha + bg_rgb) must be 16-byte
+ * the plan gmpi_mpi_render_fwd_ex launches with.  It sees GMPI_MPI_F16 and GMPI_MPI_U8: an fp16 MPI needs Wt % 8 == 0 and a
+ * uint8 MPI Wt % 16 == 0 for the staged kernels (GMPI_WHY_TEX_WIDTH otherwise).  The MPI's pointers (rgba, or rgb + alpha + bg_rgb) must be 16-byte
  * aligned (GMPI_WHY_ALIGNMENT); NULL ones are not checked.  Forward only, like gmpi_mpi_render_fwd_plan.  Returns the plan, or a
  * negative GMPI_ERR_* code for a bad descriptor. */
 int gmpi_mpi_render_fwd_plan_ex(const gmpi_render_desc* desc, uint32_t* why);
@@ -292,16 +304,17 @@ int gmpi_mpi_render_bwd_deterministic_ex(const gmpi_render_desc* desc, void* scr
  * ceil(Ht/8) rows of ceil(ceil(Wt/8)/32) 32-bit words, bit b of word w = block column 32 w + b; planes in the order m * N + i.
  *
  * gmpi_mpi_occupancy_bytes: the map's size for desc (its sizes and MPI pointers: rgba, or rgb + alpha), or a negative GMPI_ERR_*.
- * gmpi_mpi_build_occupancy: fills the map (device memory, 4-byte aligned, at least the size above) from desc's MPI (fp32, or fp16
- *   under GMPI_MPI_F16) on desc->stream.  For an expanded MPI with desc->flags set it also ORs in the GMPI_FLAG_RGBA_RANGE |
- *   GMPI_FLAG_ALPHA_RANGE bits that gmpi_mpi_check_range(_f16) would set, from the same pass.
+ * gmpi_mpi_build_occupancy: fills the map (device memory, 4-byte aligned, at least the size above) from desc's MPI (fp32, fp16
+ *   under GMPI_MPI_F16, or uint8 under GMPI_MPI_U8: empty iff the alpha byte is 0) on desc->stream.  For an fp32 or fp16 expanded
+ *   MPI with desc->flags set it also ORs in the GMPI_FLAG_RGBA_RANGE | GMPI_FLAG_ALPHA_RANGE bits that gmpi_mpi_check_range(_f16)
+ *   would set, from the same pass (a uint8 MPI is always inside [0, 1]: its build does not read the flags).
  * gmpi_mpi_render_fwd_skip_ex: gmpi_mpi_render_fwd_ex, except that the TMA-staged forward arms a (tile, plane) stage without
  *   loading it when every texel under its box is empty, and composites nothing where its taps fall in that box.  Compositing such a
  *   box adds fma(+0, finite, x) == x to colour and depth and leaves T alone, so colour, depth, uint8 frames and flags are bitwise
  *   those of gmpi_mpi_render_fwd_ex whenever no accumulator is -0.0 and T is finite in front of a skipped stage (DESIGN.md section
  *   4.1: true for every MPI inside the range check's [0, 1]).  The direct kernel takes the request and skips nothing.  Composes with
- *   the factored MPI, GMPI_MPI_F16, GMPI_EARLY_STOP, cam, view_group, the video outputs and the fused gather; refuses a descriptor
- *   with transmittance and a map smaller than gmpi_mpi_occupancy_bytes.  The map must describe the MPI as it is now: the callee
+ *   the factored MPI, GMPI_MPI_F16, GMPI_MPI_U8, GMPI_EARLY_STOP, cam, view_group, the video outputs and the fused gather; refuses a
+ *   descriptor with transmittance and a map smaller than gmpi_mpi_occupancy_bytes.  The map must describe the MPI as it is now: the callee
  *   cannot tell a stale map.  None of the three needs a GPU to refuse a call.
  */
 long long gmpi_mpi_occupancy_bytes(const gmpi_render_desc* desc);
@@ -389,6 +402,11 @@ int gmpi_debug_fwd_skip_stats(unsigned long long* skipped, unsigned long long* t
  * gmpi_mpi_build_occupancy): 1 when a block under the texels [bx0, bx0 + bw) x [by0, by0 + rows) inside the Ht x Wt texture is
  * occupied, 0 when the box is empty, a negative GMPI_ERR_* code on bad arguments. */
 int gmpi_debug_box_occupied(const uint32_t* plane_map, int Ht, int Wt, int bx0, int by0, int bw, int rows);
+
+/* Test hooks of the GMPI_MPI_U8 conversion: out[b] = the fp32 value of code b for the 256 codes.  _host: the host build, out is host
+ * memory (no GPU work); without the suffix: the device build (a kernel of the uint8 module), out is device memory, on `stream`. */
+int gmpi_debug_u8_codes_host(float* out);
+int gmpi_debug_u8_codes(float* out, void* stream);
 
 /* Test hook: the ring depth (2 or 3) the expanded staged forward picks on the current device for M MPIs, V views, N planes of
  * Ht x Wt texels and view_group (gmpi_render_desc.view_group); a negative GMPI_ERR_* code on bad arguments. */

@@ -3,7 +3,7 @@
 from . import _lib  # noqa: F401
 from ._build import build_library  # noqa: F401
 from .mpi import (MPI, MPIOutOfPlaneError, Occupancy, build_occupancy, check_range, expand_factored, render_frames,  # noqa: F401
-                  render_views, render_views_factored)
+                  render_views, render_views_factored, unorm8_to_float)
 
 __all__ = ["MPI", "MPIOutOfPlaneError", "render_views", "render_views_factored", "render_frames", "expand_factored", "check_range",
-           "build_library", "build_occupancy", "Occupancy"]
+           "build_library", "build_occupancy", "Occupancy", "unorm8_to_float"]

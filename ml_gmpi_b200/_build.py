@@ -9,9 +9,13 @@ LIB_PATH = os.path.join(PKG_DIR, "libgmpi_mpi_render.so")
 # the empty-space skipping kernels: a module of their own, loaded by the library on first use (the library's kernels keep their
 # machine code)
 SKIP_PATH = os.path.join(PKG_DIR, "libgmpi_mpi_render_skip.fatbin")
+# the uint8-MPI kernels (GMPI_MPI_U8): likewise a module of their own
+U8_PATH = os.path.join(PKG_DIR, "libgmpi_mpi_render_u8.fatbin")
 SOURCES = ["mpi_render.cu"]
 SKIP_SOURCES = ["mpi_skip.cu"]
-HEADERS = ["mpi_common.cuh", "mpi_fwd_staged.cuh", "mpi_bwd_box.cuh", "tma_utils.cuh", os.path.join("..", "..", "include", "gmpi_mpi_render.h")]
+U8_SOURCES = ["mpi_u8.cu"]
+HEADERS = ["mpi_common.cuh", "mpi_fwd_staged.cuh", "mpi_fwd_direct.cuh", "mpi_bwd_box.cuh", "tma_utils.cuh",
+           os.path.join("..", "..", "include", "gmpi_mpi_render.h")]
 ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-diag-suppress", "1886"]
 NVCC_FLAGS = ARCH_FLAGS + ["-shared", "-Xcompiler", "-fPIC"]
 
@@ -40,9 +44,10 @@ def _nvcc(args, verbose):
 
 
 def build_library(force: bool = False, verbose: bool = False) -> str:
-    """Builds the library and the skipping module next to it; returns the library's path."""
-    if force or is_stale(SKIP_PATH):
-        _nvcc(ARCH_FLAGS + ["-fatbin", "-o", SKIP_PATH] + SKIP_SOURCES, verbose)
+    """Builds the library and the skipping and uint8 modules next to it; returns the library's path."""
+    for path, sources in ((SKIP_PATH, SKIP_SOURCES), (U8_PATH, U8_SOURCES)):
+        if force or is_stale(path):
+            _nvcc(ARCH_FLAGS + ["-fatbin", "-o", path] + sources, verbose)
     if force or is_stale(LIB_PATH):
         _nvcc(NVCC_FLAGS + ["-o", LIB_PATH] + SOURCES, verbose)
     return LIB_PATH

@@ -18,7 +18,7 @@ OPT_COLOR_MINUS1_1 = 4
 OPT_ZERO_GRAD = 8
 
 PLAN_DIRECT, PLAN_STAGED = 1, 2
-WHY = {1: "texture width is not a multiple of 4 (8 in fp16)", 2: "fewer than 120 tiles of 64x30 pixels",
+WHY = {1: "texture width is not a multiple of 4 (8 in fp16, 16 in uint8)", 2: "fewer than 120 tiles of 64x30 pixels",
        4: "more than 512 planes, or 2^31 planes over all MPIs", 8: "an MPI base pointer is not 16-byte aligned",
        16: "direct kernel forced by gmpi_debug_set_fwd_variant"}
 
@@ -27,6 +27,7 @@ ABI_VERSION = 2
 OPT_U8_ROUND_HALF_UP = 16
 OPT_EARLY_STOP = 32
 OPT_MPI_F16 = 64
+OPT_MPI_U8 = 128
 
 
 class RenderDesc(ctypes.Structure):
@@ -83,6 +84,8 @@ SIGNATURES = {
     "gmpi_debug_fwd_early_stop_stats": (_i, [_vp, _vp]),
     "gmpi_debug_fwd_skip_stats": (_i, [_vp, _vp]),
     "gmpi_debug_box_occupied": (_i, [_vp] + [_i] * 6),
+    "gmpi_debug_u8_codes_host": (_i, [_vp]),
+    "gmpi_debug_u8_codes": (_i, [_vp, _vp]),
     "gmpi_debug_fwd_ring_stages": (_i, [_i] * 6),
     "gmpi_debug_copy_plan": (_i, [_i, _vp, _i]),
     "gmpi_debug_tile_walk_ex": (_i, [_i] * 7 + [_vp, _i]),

@@ -60,6 +60,22 @@ static_assert(sizeof(RenderParams) == 248, "RenderParams layout (kernel paramete
 // tap is converted to fp32 (exactly) before the fp32 arithmetic, so an fp16 MPI renders bit for bit like its fp32 upcast.
 __device__ __forceinline__ float to_f32(float x) { return x; }
 __device__ __forceinline__ float to_f32(__half x) { return __half2float(x); }
+// GMPI_MPI_U8: the 8-bit code b stands for b / 255 rounded to nearest in fp32 (the reference's astype(np.float32) / 255.0,
+// mpi_utils.py:336-337).  b * RN(1/255) is not that for 126 of the 256 codes; the quotient is exact with Markstein's correction
+// (q0 = b y, r = b - 255 q0 exactly in an FMA, q = RN(q0 + r y), y = RN(1/255); checked for every code on the host and on the
+// device, tests/test_unorm8.py).  On the device b becomes a float without the XU pipe: the bits 0x4b0000bb are 2^23 + b.
+__host__ __device__ __forceinline__ float to_f32(uint8_t b) {
+    constexpr float y = 0x1.010102p-8f;     // RN(1/255)
+#ifdef __CUDA_ARCH__
+    const float x = __fadd_rn(__uint_as_float(0x4b000000u | b), -8388608.0f);
+    const float q0 = __fmul_rn(x, y);
+    return __fmaf_rn(__fmaf_rn(-q0, 255.0f, x), y, q0);
+#else
+    const float x = (float)b;
+    const float q0 = x * y;
+    return fmaf(fmaf(-q0, 255.0f, x), y, q0);
+#endif
+}
 
 // The four channel slabs (Ht*Wt elements each) of one (MPI, plane): expanded rgba or the generator's factored form.
 template <class E = float>

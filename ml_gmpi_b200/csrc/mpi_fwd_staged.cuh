@@ -49,8 +49,15 @@ __host__ __device__ constexpr int class_width(int k, bool wide = false) { return
 // 128 for the factored ring's 64 and 96 (a colour copy of kColourCopyRows rows lands at a multiple of 132 bw bytes, which must be
 // 128-byte aligned: bw % 32 == 0).  Class, mode and the in-box vote stay those of the fp32 box, so an fp16 MPI takes the fast and
 // the generic body exactly where its fp32 upcast does; only the addresses use the wider box.
+// uint8 boxes (GMPI_MPI_U8, expanded ring only) start at a multiple of 16 texels (16 bytes), up to 12 texels west of the fp32 origin,
+// and are 16-byte multiples wide that cover the class box after that shift: 80, 80, 96, 96, 112 for the classes 56 .. 88.
 template <class E>
-__host__ __device__ constexpr int staged_width(int bw, bool wide) { return sizeof(E) == 2 ? bw + (wide ? 32 : 8) : bw; }
+__host__ __device__ constexpr int staged_width(int bw, bool wide) {
+    return sizeof(E) == 1 ? (bw + 12 + 15) & ~15 : sizeof(E) == 2 ? bw + (wide ? 32 : 8) : bw;
+}
+// Offset of the fp32 box's origin from the staged box's: 0 in fp32, 0 or 4 in fp16, 0..12 in uint8 (StageMeta::sel bits 10-13).
+template <class E>
+__host__ __device__ constexpr int staged_origin(int bx0) { return sizeof(E) == 1 ? bx0 & ~15 : sizeof(E) == 2 ? bx0 & ~7 : bx0; }
 
 struct TmaMaps {
     CUtensorMap m[kNumMaps];      // expanded rgba [M*N][4][Ht][Wt] as (x, channel, y, plane), box {bw, 4, 4 rows, 1}
@@ -255,6 +262,19 @@ __device__ __noinline__ float4 sample_chans_direct(const PlaneChansT<__half> pl,
     const Taps tp = make_taps(ix, iy, Ht, Wt);
     return make_float4(tap4(pl.c[0], tp), tap4(pl.c[1], tp), tap4(pl.c[2], tp), tap4(pl.c[3], tp));
 }
+// any other element type (uint8_t, GMPI_MPI_U8): templates, instantiated only by the kernels that use them (mpi_u8.cu); the overloads
+// above stay the exact matches for fp32 and fp16
+template <class E>
+__device__ __noinline__ float4 sample_plane_direct(const E* __restrict__ plane, int Ht, int Wt, float ix, float iy) {
+    const size_t tex = (size_t)Ht * Wt;
+    const Taps tp = make_taps(ix, iy, Ht, Wt);
+    return make_float4(tap4(plane, tp), tap4(plane + tex, tp), tap4(plane + 2 * tex, tp), tap4(plane + 3 * tex, tp));
+}
+template <class E>
+__device__ __noinline__ float4 sample_chans_direct(const PlaneChansT<E> pl, int Ht, int Wt, float ix, float iy) {
+    const Taps tp = make_taps(ix, iy, Ht, Wt);
+    return make_float4(tap4(pl.c[0], tp), tap4(pl.c[1], tp), tap4(pl.c[2], tp), tap4(pl.c[3], tp));
+}
 // generic-path sample of plane i of MPI m: the instantiation decides which form crosses the call
 template <bool kFactored, class E>
 __device__ __forceinline__ float4 sample_plane_any(const RenderParams& p, const E* plane, int m, int i, size_t tex, float ix, float iy) {
@@ -366,6 +386,12 @@ struct FwdRingF16 : FwdRing {
 struct FwdRingWideF16 : FwdRingWide {
     static constexpr int kPlaneFloats = (kWideBW + 32) * kMaxBH * 4, kStride = kPlaneFloats;
 };
+// GMPI_MPI_U8 (expanded MPI only): stages of the widest uint8 box, 19712 bytes (a multiple of 128: every stage and every 4-row copy,
+// at 16 * staged width bytes per chunk, lands 128-byte aligned)
+struct FwdRingU8 : FwdRing {
+    static constexpr int kPlaneFloats = staged_width<uint8_t>(kMaxBW, false) * kMaxBH * 4, kStride = kPlaneFloats;
+};
+static_assert(FwdRingU8::kPlaneFloats % 128 == 0, "uint8 ring stages stay 128-byte aligned");
 
 // The expanded forward's copies of one stage: the footprint's n_chunks 4-row chunks as the binary digits of n_chunks.  Lane 0..3
 // owns the digit 8, 4, 2, 1: returns the copy's height in chunks (0: this lane issues nothing) and, in `before`, the chunks
@@ -403,6 +429,25 @@ struct OccMap {
 };
 __host__ __device__ __forceinline__ int occ_words(int Wt) { return ((Wt + kOccB - 1) / kOccB + 31) / 32; }
 __host__ __device__ __forceinline__ int occ_rows(int Ht) { return (Ht + kOccB - 1) / kOccB; }
+
+// The map builds (mpi_skip.cu, mpi_u8.cu): one CTA row of kOccThreads threads = 256 texel columns = one map word per plane.
+constexpr int kOccThreads = 32 * kOccB;
+
+// The 256 threads' verdicts (texel column threadIdx.x of this word is occupied) -> the map word: each warp holds 4 blocks of 8 columns.
+__device__ __forceinline__ void store_occ_word(bool occupied, uint32_t* dst, uint32_t* s_w) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const uint32_t b = __ballot_sync(0xffffffffu, occupied);
+    const uint32_t nib = ((b & 0xffu) ? 1u : 0u) | ((b & 0xff00u) ? 2u : 0u) | ((b & 0xff0000u) ? 4u : 0u) | ((b & 0xff000000u) ? 8u : 0u);
+    if (lane == 0) s_w[warp] = nib << (4 * warp);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        uint32_t w = 0;
+#pragma unroll
+        for (int k = 0; k < kOccThreads / 32; ++k) w |= s_w[k];
+        *dst = w;
+    }
+    __syncthreads();
+}
 
 // Lane `lane`'s part of the box-versus-map test: the OR of the map bits of one plane under the texels [bx0, bx0 + bw) x
 // [by0, by0 + rows) that lie inside the texture (TMA zero-fills the rest).  The (block row, word) pairs under the box are dealt to
@@ -503,7 +548,7 @@ __device__ __forceinline__ void staged_producer(const RenderParams& p, const Tma
             const int xmin = __reduce_min_sync(0xffffffffu, fx), xmax = __reduce_max_sync(0xffffffffu, fx);
             const int ymin = __reduce_min_sync(0xffffffffu, fy), ymax = __reduce_max_sync(0xffffffffu, fy);
             // TMA needs a 16-byte aligned start in the innermost dimension: the box origin is a multiple of 4 texels (fp16: the staged
-            // box starts at bxs, a multiple of 8, see staged_width)
+            // box starts at bxs, a multiple of 8, uint8: of 16, see staged_width)
             const int bx0 = ((xmin - 1) >> 2) << 2, by0 = ymin - 1;
             const int need_w = xmax - bx0 + 3, need_h = ymax - ymin + 4;      // +1 east/south tap, +-1 slack
             int mode = 0;
@@ -517,7 +562,7 @@ __device__ __forceinline__ void staged_producer(const RenderParams& p, const Tma
             // width class k (tensor-map slot, one-hot bit 16 + k of the header); wide rings: slot 1 = 64, slot 4 = kWideBW
             const int k = mode != 0 ? 0 : kWide ? (need_w <= 64 ? 1 : 4) : max(0, (need_w - kMinBW + kBWStep - 1) / kBWStep);
             const int bw = class_width(k, kWide);
-            const int bxs = sizeof(E) == 2 ? (bx0 & ~7) : bx0, sw = staged_width<E>(bw, kWide);   // staged box: origin, width
+            const int bxs = staged_origin<E>(bx0), sw = staged_width<E>(bw, kWide);   // staged box: origin, width
             const int n_ops = mode == 0 ? (need_h + kRowsPerOp - 1) / kRowsPerOp : 0;
             const int rows = n_ops * kRowsPerOp;
             // kSkip: only a stage that takes the fast body (mode 0, plane constants in the exact range) may be skipped.  The test covers
@@ -654,9 +699,11 @@ __device__ __forceinline__ void fwd_staged_body(const RenderParams& p, const Tma
                                                 uint32_t* s_stop, OccMap occ = OccMap{}) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     E* s_buf = reinterpret_cast<E*>(smem_raw);   // the ring starts the dynamic segment (1024-byte aligned)
-    constexpr bool kHalf = sizeof(E) == 2;
+    constexpr bool kHalf = sizeof(E) == 2, kU8 = sizeof(E) == 1;
     using Ring = typename std::conditional<kFactored, typename std::conditional<kHalf, FwdRingWideF16, FwdRingWide>::type,
-                                           typename std::conditional<kHalf, FwdRingF16, FwdRing>::type>::type;
+                                           typename std::conditional<kHalf, FwdRingF16,
+                                                                     typename std::conditional<kU8, FwdRingU8, FwdRing>::type>::type>::type;
+    static_assert(!(kU8 && kFactored), "uint8 MPIs are expanded");
     constexpr int kStages = Ring::kRingStages;              // ring stages allocated; the expanded MPI uses ring_stages of them
     const int n_stages = kFactored ? kStages : ring_stages;
     constexpr int kRingFloats = Ring::kPlaneFloats;         // floats per ring stage
@@ -766,7 +813,8 @@ __device__ __forceinline__ void fwd_staged_body(const RenderParams& p, const Tma
                 }
                 mbar_wait(&s_full[s], ph);
                 const StageMeta mt = s_meta[s];
-                const E* sb = s_buf + s * kRingFloats + (kHalf ? (mt.sel >> 10) & 7 : 0);   // fp16: the fp32 box's origin in the stage
+                // fp16, uint8: the fp32 box's origin in the stage
+                const E* sb = s_buf + s * kRingFloats + (kU8 ? (mt.sel >> 10) & 15 : kHalf ? (mt.sel >> 10) & 7 : 0);
                 const int sel = mt.sel;                  // warp-uniform; the producer already folded mode and plane range in
                 bool done = warp_stopped;                // a stopped warp only waits on and releases the stage
                 if (warp_fast && !done) {

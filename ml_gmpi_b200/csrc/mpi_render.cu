@@ -19,6 +19,7 @@
 #include "mpi_fwd_staged.cuh"
 #include "mpi_bwd_box.cuh"
 #include "mpi_light.cuh"
+#include "mpi_fwd_direct.cuh"
 
 namespace gmpi {
 
@@ -44,85 +45,8 @@ static int fail(int code, const char* fmt, ...) {
     } while (0)
 
 // ------------------------------------------------------------------------------------------
-// Forward, direct-gather variant: one thread = one output pixel, a warp = 32 consecutive x.
-// Taps are read straight from global memory through L1 (per channel a warp touches one or two
-// 128-byte lines per tap row).  Works for every shape; the TMA-staged variant is the fast path.
+// Forward, direct-gather variant (fwd_direct_body, mpi_fwd_direct.cuh).
 // ------------------------------------------------------------------------------------------
-constexpr int kFwdTileW = 32;
-constexpr int kFwdTileH = 8;
-
-// kES: GMPI_EARLY_STOP, a pixel composites no further plane once |T| <= p.early_stop (mpi_fwd_direct_early_stop_kernel).
-// (p by value: with a reference ptxas allocates the default kernel's registers differently.)  E: the MPI's element type.
-template <bool kAlignCorners, bool kES, class E = float>
-__device__ __forceinline__ void fwd_direct_body(const RenderParams p) {
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    PlaneConst* s_pc = reinterpret_cast<PlaneConst*>(smem_raw);
-
-    const int v = blockIdx.z;
-    const int m = __ldg(p.view2mpi + v);
-    const int tid = threadIdx.y * kFwdTileW + threadIdx.x;
-    float ev[3], zd[3];
-    load_eye_z(p, v, ev, zd);
-    const float eye0_z = __ldg(p.eye0 + 2);  // mpi.py:70 compares every distance with view 0's eye
-    uint32_t flag = 0;
-    for (int i = tid; i < p.N; i += kFwdTileW * kFwdTileH) {
-        const float* dp = p.dhw + ((size_t)m * p.N + i) * 3;
-        s_pc[i] = make_plane_const(dp, ev[2]);
-        if (!(__ldg(dp) >= eye0_z)) flag |= GMPI_FLAG_PLANE_BEHIND_EYE;
-    }
-    __syncthreads();
-
-    const int px = blockIdx.x * kFwdTileW + threadIdx.x;
-    const int py = blockIdx.y * kFwdTileH + threadIdx.y;
-    if (px < p.W && py < p.H) {
-        const size_t img = (size_t)p.H * p.W;
-        const size_t pix = (size_t)py * p.W + px;
-        float qx, qy, qz;
-        load_ray(p, v, px, py, img, qx, qy, qz);
-        const RayConst rc = make_ray_const(qx, qy, qz, ev, zd);
-
-        const int Ht = p.Ht, Wt = p.Wt;
-        const float fWt = (float)Wt, fHt = (float)Ht;
-        const float hsx = 0.5f * (float)(Wt - 1), hsy = 0.5f * (float)(Ht - 1);
-        const size_t tex = (size_t)Ht * Wt;
-        const bool check_last = (p.options & GMPI_CHECK_LAST_PLANE) != 0;
-        const float tau = kES ? p.early_stop : 0.0f;
-
-        float T = 1.0f, cr = 0.0f, cg = 0.0f, cb = 0.0f, cws = 0.0f;
-#pragma unroll 2
-        for (int i = 0; i < p.N; ++i) {
-            const PlaneConst pc = s_pc[i];
-            const PlaneChansT<E> plane = plane_chans<E>(p, m, i, tex);
-            if (!kES && p.transmittance) p.transmittance[((size_t)v * p.N + i) * img + pix] = T;   // training: T_i for the backward sweep
-            const TexCoord tc = plane_coord<kAlignCorners>(pc, rc, hsx, hsy, fWt, fHt);
-            if (check_last && i == p.N - 1) {
-                if (!(tc.u >= -1.0f && tc.u <= 1.0f && tc.v >= -1.0f && tc.v <= 1.0f)) flag |= GMPI_FLAG_LAST_PLANE_OOB;
-            }
-            if (coord_hits(tc.ix, tc.iy, fWt, fHt) && !(kES && fabsf(T) <= tau)) {
-                const Taps t = make_taps(tc.ix, tc.iy, Ht, Wt);
-                const float r = tap4(plane.c[0], t);
-                const float g = tap4(plane.c[1], t);
-                const float b = tap4(plane.c[2], t);
-                const float a = tap4(plane.c[3], t);
-                const float w = a * T;                                   // mpi.py:423
-                cr = fmaf(w, r, cr);                                     // mpi.py:430
-                cg = fmaf(w, g, cg);
-                cb = fmaf(w, b, cb);
-                cws = fmaf(w, tc.scale, cws);                            // depth_i = scale * (ray.z_dir), :150
-                T *= (1.0f - a) + 1e-10f;                                // mpi.py:421
-            }
-        }
-        const float dep = cws * rc.dz;
-        if (p.options & GMPI_COLOR_MINUS1_1) {                           // mpi_renderer.py:467
-            cr = fmaf(2.0f, cr, -1.0f);
-            cg = fmaf(2.0f, cg, -1.0f);
-            cb = fmaf(2.0f, cb, -1.0f);
-        }
-        store_pixel(p, v, img, pix, cr, cg, cb, dep);
-    }
-    if (flag) atomicOr(p.flags, flag);
-}
-
 template <bool kAlignCorners>
 __global__ void __launch_bounds__(kFwdTileW* kFwdTileH)
 mpi_fwd_direct_kernel(const RenderParams p) {
@@ -509,8 +433,20 @@ static int check_sizes(const RenderParams& p, bool views, bool texels) {
     return GMPI_OK;
 }
 
+// GMPI_MPI_U8: an expanded MPI, not fp16 as well.  `bwd`: a backward call, which reads and writes fp32 MPIs.
+static int check_u8(const RenderParams& p, bool bwd) {
+    if (!(p.options & GMPI_MPI_U8)) return GMPI_OK;
+    if (p.options & GMPI_MPI_F16) return fail(GMPI_ERR_INVALID_ARGUMENT, "GMPI_MPI_U8 and GMPI_MPI_F16 are exclusive");
+    if (bwd) return fail(GMPI_ERR_UNSUPPORTED, "GMPI_MPI_U8 is forward-only: the backward reads and writes fp32 MPIs");
+    if (p.rgb || p.alpha || p.bg_rgb) return fail(GMPI_ERR_UNSUPPORTED, "GMPI_MPI_U8 takes an expanded MPI (rgba), not a factored one");
+    if (p.transmittance)
+        return fail(GMPI_ERR_UNSUPPORTED, "GMPI_MPI_U8 cannot be combined with the training forward (transmittance)");
+    return GMPI_OK;
+}
+
 // Argument checks shared by every entry point.  `bwd`: gradients instead of outputs.
 static int check_params(const RenderParams& p, bool bwd) {
+    if (int rc = check_u8(p, bwd)) return rc;
     if (p.options & GMPI_MPI_F16) {
         if (bwd) return fail(GMPI_ERR_UNSUPPORTED, "GMPI_MPI_F16 is forward-only: the backward reads and writes fp32 MPIs");
         if (p.transmittance)
@@ -544,13 +480,14 @@ static bool aligned16(const void* a) { return ((uintptr_t)a & 15) == 0; }
 
 // The GMPI_WHY_* bits of every reason the TMA-staged forward is not launched for p (0 = staged): the one decision behind
 // launch_fwd, launch_bwd and the plan queries.  The tensor maps need 16-byte row strides (Wt % 4 == 0 in fp32, Wt % 8 == 0 in
-// fp16) and 16-byte aligned MPI bases (NULL counts as aligned); the plane-constant table holds kMaxPlanesStaged planes, and the
-// M*N planes of all MPIs stay below 2^31; the persistent grid needs enough tiles.  Reads the sizes, the fp16 bit, the MPI
-// pointers and the variant override, nothing else: the early-stop and training instantiations get the plain forward's plan.
+// fp16, Wt % 16 == 0 in uint8) and 16-byte aligned MPI bases (NULL counts as aligned); the plane-constant table holds
+// kMaxPlanesStaged planes, and the M*N planes of all MPIs stay below 2^31; the persistent grid needs enough tiles.  Reads the sizes,
+// the fp16 and uint8 bits, the MPI pointers and the variant override, nothing else: the early-stop and training instantiations get
+// the plain forward's plan.
 static uint32_t fwd_why(const RenderParams& p) {
     uint32_t w = 0;
     if (p.N > kMaxPlanesStaged || (size_t)p.M * p.N >= ((size_t)1 << 31)) w |= GMPI_WHY_MANY_PLANES;
-    if (p.Wt % ((p.options & GMPI_MPI_F16) ? 8 : 4) != 0) w |= GMPI_WHY_TEX_WIDTH;
+    if (p.Wt % ((p.options & GMPI_MPI_U8) ? 16 : (p.options & GMPI_MPI_F16) ? 8 : 4) != 0) w |= GMPI_WHY_TEX_WIDTH;
     if (!(factored(p) ? aligned16(p.rgb) && aligned16(p.alpha) && aligned16(p.bg_rgb) : aligned16(p.rgba))) w |= GMPI_WHY_ALIGNMENT;
     const int forced = g_fwd_variant.load(std::memory_order_relaxed);
     if (forced == 1) w |= GMPI_WHY_FORCED;
@@ -564,10 +501,12 @@ static uint32_t fwd_why(const RenderParams& p) {
 // wide: the factored forward's ring (FwdRingWide) -- slot 4 holds the kWideBW-wide boxes, slot 1 the 64-wide ones, the rest unused.
 // The element type is the MPI's: fp16 under GMPI_MPI_F16, else fp32.
 static int encode_mpi_maps(TmaMaps& maps, const RenderParams& p, int box_h, int colour_rows, bool wide = false) {
-    const bool f16 = (p.options & GMPI_MPI_F16) != 0;
-    const MapElem el = f16 ? kMapF16 : kMapF32;
+    const bool f16 = (p.options & GMPI_MPI_F16) != 0, u8 = (p.options & GMPI_MPI_U8) != 0;
+    const MapElem el = u8 ? kMapU8 : f16 ? kMapF16 : kMapF32;
     for (int k = 0; k < kNumMaps; ++k) {
-        const int bw = f16 ? staged_width<__half>(class_width(k, wide), wide) : class_width(k, wide);
+        const int bw = u8    ? staged_width<uint8_t>(class_width(k, wide), wide)
+                       : f16 ? staged_width<__half>(class_width(k, wide), wide)
+                             : class_width(k, wide);
         if (factored(p)) {
             if (encode_color_map(&maps.rgb[k], p.rgb, el, (uint64_t)p.M, p.Ht, p.Wt, bw, colour_rows) != 0) return -1;
             if (p.bg_rgb && encode_color_map(&maps.bg[k], p.bg_rgb, el, (uint64_t)p.M, p.Ht, p.Wt, bw, colour_rows) != 0) return -1;
@@ -696,83 +635,130 @@ static int persistent_grid(Launch& l, int tile_h) {
     return GMPI_OK;
 }
 
-// Dynamic shared memory of a staged forward kernel: its ring and the plane-constant table.  fac: the kernel's kFactored; f16: its MPI
-// is fp16 (the rings of FwdRingF16 / FwdRingWideF16)
-static size_t fwd_staged_smem(bool fac, int stages, bool f16) {
-    const size_t ring = f16 ? (size_t)(fac ? kStages * FwdRingWideF16::kPlaneFloats : stages * FwdRingF16::kPlaneFloats) * 2
-                            : (size_t)(fac ? kStages * kWideStageFloats : stages * kStageFloats) * 4;
+// Dynamic shared memory of a staged forward kernel: its ring and the plane-constant table.  fac: the kernel's kFactored; f16, u8: its
+// MPI is fp16 (the rings of FwdRingF16 / FwdRingWideF16) or uint8 (FwdRingU8, expanded only)
+static size_t fwd_staged_smem(bool fac, int stages, bool f16, bool u8) {
+    const size_t ring = u8    ? (size_t)stages * FwdRingU8::kPlaneFloats
+                        : f16 ? (size_t)(fac ? kStages * FwdRingWideF16::kPlaneFloats : stages * FwdRingF16::kPlaneFloats) * 2
+                              : (size_t)(fac ? kStages * kWideStageFloats : stages * kStageFloats) * 4;
     return ring + (size_t)kMaxPlanesStaged * 32;
 }
 
-// ---- opt-in empty-space skipping: the kernels of mpi_skip.cu live in a module of their own, libgmpi_mpi_render_skip.fatbin next to
-// this library, so that this library's kernels keep their machine code.  Loaded on first use (a context-independent library: the
-// runtime loads it into each device's context when a kernel of it first runs there).
+// ---- kernel modules next to this library: the kernels of opt-in features that live in a module of their own, so that this
+// library's kernels keep their machine code.  Each is loaded on first use (a context-independent library: the runtime loads it into
+// each device's context when a kernel of it first runs there).
+//   libgmpi_mpi_render_skip.fatbin   empty-space skipping (mpi_skip.cu)
+//   libgmpi_mpi_render_u8.fatbin     uint8 MPIs, GMPI_MPI_U8 (mpi_u8.cu)
 struct SkipModule {
-    cudaLibrary_t lib = nullptr;
     cudaKernel_t fwd[2][2][2][2];           // [f16][align_corners][factored][early_stop]
     cudaKernel_t occ_exp[2], occ_fac[2];    // [f16]
+    static int get(cudaLibrary_t lib, SkipModule& m);
 };
-static SkipModule g_skip;
-static std::mutex g_skip_mutex;
+struct U8Module {
+    cudaKernel_t staged[2][2][2];           // [skip][align_corners][early_stop]
+    cudaKernel_t direct[2][2];              // [align_corners][early_stop]
+    cudaKernel_t occ, codes;
+    static int get(cudaLibrary_t lib, U8Module& m);
+};
+template <class K>
+struct Module {
+    const char* file;
+    cudaLibrary_t lib = nullptr;
+    K k;
+    std::mutex mutex;
+};
+static Module<SkipModule> g_skip{"libgmpi_mpi_render_skip.fatbin"};
+static Module<U8Module> g_u8{"libgmpi_mpi_render_u8.fatbin"};
 
-static int skip_module(const SkipModule** out) {
-    std::lock_guard<std::mutex> lock(g_skip_mutex);
-    if (!g_skip.lib) {
+static int get_kernel(cudaLibrary_t lib, cudaKernel_t* k, const char* fmt, ...) {
+    char name[64];
+    va_list ap;
+    va_start(ap, fmt);
+    vsnprintf(name, sizeof(name), fmt, ap);
+    va_end(ap);
+    GMPI_CUDA_OK(cudaLibraryGetKernel(k, lib, name));
+    return GMPI_OK;
+}
+
+int SkipModule::get(cudaLibrary_t lib, SkipModule& m) {
+    for (int h = 0; h < 2; ++h) {
+        for (int a = 0; a < 2; ++a)
+            for (int x = 0; x < 2; ++x)
+                for (int s = 0; s < 2; ++s)
+                    if (int rc = get_kernel(lib, &m.fwd[h][a][x][s], "gmpi_fwd_skip_a%d_x%d_e%d_%s", a, x, s, h ? "f16" : "f32")) return rc;
+        if (int rc = get_kernel(lib, &m.occ_exp[h], "gmpi_occ_expanded_%s", h ? "f16" : "f32")) return rc;
+        if (int rc = get_kernel(lib, &m.occ_fac[h], "gmpi_occ_factored_%s", h ? "f16" : "f32")) return rc;
+    }
+    return GMPI_OK;
+}
+
+int U8Module::get(cudaLibrary_t lib, U8Module& m) {
+    for (int a = 0; a < 2; ++a)
+        for (int s = 0; s < 2; ++s) {
+            if (int rc = get_kernel(lib, &m.staged[0][a][s], "gmpi_fwd_u8_a%d_e%d", a, s)) return rc;
+            if (int rc = get_kernel(lib, &m.staged[1][a][s], "gmpi_fwd_u8_skip_a%d_e%d", a, s)) return rc;
+            if (int rc = get_kernel(lib, &m.direct[a][s], "gmpi_fwd_direct_u8_a%d_e%d", a, s)) return rc;
+        }
+    if (int rc = get_kernel(lib, &m.occ, "gmpi_occ_expanded_u8")) return rc;
+    return get_kernel(lib, &m.codes, "gmpi_u8_codes");
+}
+
+// The module's library and kernels, loaded on the first call.
+template <class K>
+static int load_module(Module<K>& mod, const K** kernels, cudaLibrary_t* lib = nullptr) {
+    std::lock_guard<std::mutex> lock(mod.mutex);
+    if (!mod.lib) {
         Dl_info info;
         if (!dladdr(reinterpret_cast<void*>(&gmpi_abi_version), &info) || !info.dli_fname)
             return fail(GMPI_ERR_CUDA, "cannot locate the library file (dladdr)");
         std::string path(info.dli_fname);
-        path = path.substr(0, path.find_last_of('/') + 1) + "libgmpi_mpi_render_skip.fatbin";
-        SkipModule m;
-        const cudaError_t e = cudaLibraryLoadFromFile(&m.lib, path.c_str(), nullptr, nullptr, 0, nullptr, nullptr, 0);
+        path = path.substr(0, path.find_last_of('/') + 1) + mod.file;
+        cudaLibrary_t l = nullptr;
+        const cudaError_t e = cudaLibraryLoadFromFile(&l, path.c_str(), nullptr, nullptr, 0, nullptr, nullptr, 0);
         if (e != cudaSuccess) return fail(GMPI_ERR_CUDA, "loading %s failed: %s", path.c_str(), cudaGetErrorString(e));
-        char name[64];
-        for (int h = 0; h < 2; ++h) {
-            for (int a = 0; a < 2; ++a)
-                for (int x = 0; x < 2; ++x)
-                    for (int s = 0; s < 2; ++s) {
-                        snprintf(name, sizeof(name), "gmpi_fwd_skip_a%d_x%d_e%d_%s", a, x, s, h ? "f16" : "f32");
-                        GMPI_CUDA_OK(cudaLibraryGetKernel(&m.fwd[h][a][x][s], m.lib, name));
-                    }
-            GMPI_CUDA_OK(cudaLibraryGetKernel(&m.occ_exp[h], m.lib, h ? "gmpi_occ_expanded_f16" : "gmpi_occ_expanded_f32"));
-            GMPI_CUDA_OK(cudaLibraryGetKernel(&m.occ_fac[h], m.lib, h ? "gmpi_occ_factored_f16" : "gmpi_occ_factored_f32"));
-        }
-        g_skip = m;
+        if (int rc = K::get(l, mod.k)) return rc;
+        mod.lib = l;
     }
-    *out = &g_skip;
+    if (kernels) *kernels = &mod.k;
+    if (lib) *lib = mod.lib;
     return GMPI_OK;
 }
 
 // The stage counters of the test hooks gmpi_debug_fwd_early_stop_stats and gmpi_debug_fwd_skip_stats: on the device, the stages
-// the last early-stop or skipping launch armed without copies (zeroed on its stream); here, the (tile, plane) stages it walked.
+// the last early-stop or skipping launch armed without copies (zeroed on its stream); here, the (tile, plane) stages it walked and
+// whether a kernel of the uint8 module ran it (that module has counters of its own).
 enum StageStats { kEarlyStopStats, kSkipStats };
 static std::atomic<unsigned long long> g_stages_walked[2];
+static std::atomic<bool> g_stages_u8[2];
 
-// The device counter on the current device (the skipping module's is a global of that module).
-static int stage_counter(StageStats s, unsigned long long** counter) {
-    if (s == kEarlyStopStats) {
+// The device counter on the current device: a global of this library or of the module whose kernel ran (u8).  The uint8 module's
+// early-stop counter is its own copy of g_early_stop_skipped (mpi_fwd_staged.cuh), found by its mangled name.
+static int stage_counter(StageStats s, bool u8, unsigned long long** counter) {
+    if (s == kEarlyStopStats && !u8) {
         GMPI_CUDA_OK(cudaGetSymbolAddress(reinterpret_cast<void**>(counter), g_early_stop_skipped));
         return GMPI_OK;
     }
-    const SkipModule* sm = nullptr;
-    if (int rc = skip_module(&sm)) return rc;
+    cudaLibrary_t lib = nullptr;
+    if (int rc = u8 ? load_module<U8Module>(g_u8, nullptr, &lib) : load_module<SkipModule>(g_skip, nullptr, &lib)) return rc;
     size_t bytes = 0;
-    GMPI_CUDA_OK(cudaLibraryGetGlobal(reinterpret_cast<void**>(counter), &bytes, sm->lib, "gmpi_skip_empty_stages"));
+    GMPI_CUDA_OK(cudaLibraryGetGlobal(reinterpret_cast<void**>(counter), &bytes, lib,
+                                      s == kEarlyStopStats ? "_ZN4gmpi20g_early_stop_skippedE" : "gmpi_skip_empty_stages"));
     return GMPI_OK;
 }
 
-static int reset_stage_stats(StageStats s, unsigned long long walked, cudaStream_t st) {
+static int reset_stage_stats(StageStats s, bool u8, unsigned long long walked, cudaStream_t st) {
     unsigned long long* counter = nullptr;
-    if (int rc = stage_counter(s, &counter)) return rc;
+    if (int rc = stage_counter(s, u8, &counter)) return rc;
     GMPI_CUDA_OK(cudaMemsetAsync(counter, 0, sizeof(unsigned long long), st));
     g_stages_walked[s].store(walked, std::memory_order_relaxed);
+    g_stages_u8[s].store(u8, std::memory_order_relaxed);
     return GMPI_OK;
 }
 
 static int read_stage_stats(StageStats s, unsigned long long* skipped, unsigned long long* walked) {
     if (!skipped || !walked) return fail(GMPI_ERR_INVALID_ARGUMENT, "null pointer");
     unsigned long long* counter = nullptr;
-    if (int rc = stage_counter(s, &counter)) return rc;
+    if (int rc = stage_counter(s, g_stages_u8[s].load(std::memory_order_relaxed), &counter)) return rc;
     GMPI_CUDA_OK(cudaDeviceSynchronize());
     GMPI_CUDA_OK(cudaMemcpy(skipped, counter, sizeof(unsigned long long), cudaMemcpyDeviceToHost));
     *walked = g_stages_walked[s].load(std::memory_order_relaxed);
@@ -781,7 +767,8 @@ static int read_stage_stats(StageStats s, unsigned long long* skipped, unsigned 
 
 // Occupancy map: M*N planes of occ_rows(Ht) block rows of occ_words(Wt) words.  Checks what the map's size and build read.
 static int occ_bytes(const RenderParams& p, size_t* bytes) {
-    int rc = check_mpi_form(p);
+    int rc = check_u8(p, false);
+    if (rc || (rc = check_mpi_form(p)) != 0) return rc;
     if (rc || (rc = check_sizes(p, false, true)) != 0) return rc;
     *bytes = (size_t)p.M * p.N * occ_rows(p.Ht) * occ_words(p.Wt) * sizeof(uint32_t);
     return GMPI_OK;
@@ -802,9 +789,11 @@ static int check_occ_arg(const RenderParams& p, const void* occ, size_t bytes) {
 static int fwd_launch(Launch& l, const uint32_t* occ) {
     const RenderParams& p = l.p;
     const bool ac = (p.options & GMPI_ALIGN_CORNERS) != 0, fac = factored(p), es = (p.options & GMPI_EARLY_STOP) != 0;
-    const bool f16 = (p.options & GMPI_MPI_F16) != 0;
+    const bool f16 = (p.options & GMPI_MPI_F16) != 0, u8 = (p.options & GMPI_MPI_U8) != 0;
     const uint32_t key = (ac ? kKeyAC : 0) | (es ? kKeyES : 0) | (f16 ? kKeyF16 : 0);
+    const U8Module* um = nullptr;     // u8: every kernel comes from the uint8 module
     int rc = GMPI_OK;
+    if (u8 && (rc = load_module<U8Module>(g_u8, &um)) != 0) return rc;
     if (fwd_why(p) == 0) {
         if (encode_mpi_maps(l.maps, p, kMaxBH, FwdRingWide::kColourCopyRows, fac) == 0) {
             int l2 = 0;
@@ -813,18 +802,22 @@ static int fwd_launch(Launch& l, const uint32_t* occ) {
             const int forced_stages = g_fwd_stages.load(std::memory_order_relaxed);
             l.ints[2] = forced_stages ? forced_stages : fwd_ring_stages(p, l2);
             l.block = dim3(kStagedThreads);
-            l.smem = fwd_staged_smem(fac, l.ints[2], f16);
+            l.smem = fwd_staged_smem(fac, l.ints[2], f16, u8);
             l.arg(&l.ints[2]);
             if (!occ) {
-                l.kernel = render_kernel(key | kKeyStaged | (fac ? kKeyFac : 0) | (p.transmittance ? kKeyEmit : 0));
+                l.kernel = u8 ? um->staged[0][ac][es] : render_kernel(key | kKeyStaged | (fac ? kKeyFac : 0) | (p.transmittance ? kKeyEmit : 0));
                 return GMPI_OK;
             }
-            const SkipModule* sm = nullptr;
-            if ((rc = skip_module(&sm)) != 0) return rc;
-            l.kernel = sm->fwd[f16][ac][fac][es];
+            if (u8) {
+                l.kernel = um->staged[1][ac][es];
+            } else {
+                const SkipModule* sm = nullptr;
+                if ((rc = load_module<SkipModule>(g_skip, &sm)) != 0) return rc;
+                l.kernel = sm->fwd[f16][ac][fac][es];
+            }
             l.om = OccMap{occ, occ_words(p.Wt), occ_rows(p.Ht), nullptr};
             l.arg(&l.om);
-            return stage_counter(kSkipStats, &l.om.skipped);
+            return stage_counter(kSkipStats, u8, &l.om.skipped);
         }
         if (g_fwd_variant.load(std::memory_order_relaxed) == 2) return fail(GMPI_ERR_CUDA, "cuTensorMapEncodeTiled failed");
     }
@@ -835,7 +828,7 @@ static int fwd_launch(Launch& l, const uint32_t* occ) {
     l.grid = dim3((p.W + kFwdTileW - 1) / kFwdTileW, (p.H + kFwdTileH - 1) / kFwdTileH, p.V);
     if (l.grid.y > 65535) return fail(GMPI_ERR_UNSUPPORTED, "image height %d too large", p.H);
     if (p.V > 65535) return fail(GMPI_ERR_UNSUPPORTED, "V=%d views exceed one launch of the direct kernel (65535); split the batch", p.V);
-    l.kernel = render_kernel(key);
+    l.kernel = u8 ? um->direct[ac][es] : render_kernel(key);
     return GMPI_OK;
 }
 
@@ -860,8 +853,9 @@ static int launch_fwd(RenderParams p, cudaStream_t st, const uint32_t* occ = nul
     if ((rc = fwd_launch(l, occ)) != 0) return rc;
     // the direct kernel walks no stages: it loads per pixel, and composites every plane (which gives a skipping call's output)
     const unsigned long long walked = (unsigned long long)l.tiles * p.N;
-    if ((p.options & GMPI_EARLY_STOP) && (rc = reset_stage_stats(kEarlyStopStats, walked, st)) != 0) return rc;
-    if (occ && (rc = reset_stage_stats(kSkipStats, walked, st)) != 0) return rc;
+    const bool u8 = (p.options & GMPI_MPI_U8) != 0;
+    if ((p.options & GMPI_EARLY_STOP) && (rc = reset_stage_stats(kEarlyStopStats, u8, walked, st)) != 0) return rc;
+    if (occ && (rc = reset_stage_stats(kSkipStats, u8, walked, st)) != 0) return rc;
     return launch(l, st);
 }
 
@@ -1045,10 +1039,12 @@ static int check_desc(const gmpi_render_desc* d) {
     return GMPI_OK;
 }
 
-// The classic entry points take fp32 MPIs only (their pointers are typed float*): GMPI_MPI_F16 needs a descriptor.
+// The classic entry points take fp32 MPIs only (their pointers are typed float*): GMPI_MPI_F16 and GMPI_MPI_U8 need a descriptor.
 static int refuse_f16_classic(uint32_t options) {
     if (options & GMPI_MPI_F16)
         return fail(GMPI_ERR_UNSUPPORTED, "GMPI_MPI_F16 is accepted by gmpi_mpi_render_fwd_ex and gmpi_mpi_render_host_ex only");
+    if (options & GMPI_MPI_U8)
+        return fail(GMPI_ERR_UNSUPPORTED, "GMPI_MPI_U8 is accepted by the descriptor forward entry points only");
     return GMPI_OK;
 }
 
@@ -1226,7 +1222,8 @@ long long gmpi_mpi_render_bwd_deterministic_scratch_bytes(const gmpi_render_desc
     int rc = check_desc(d);
     if (rc) return -rc;
     DetLayout L;
-    if ((rc = det_layout(params_from_desc(d), L)) != 0) return -rc;
+    const RenderParams p = params_from_desc(d);
+    if ((rc = check_u8(p, true)) != 0 || (rc = det_layout(p, L)) != 0) return -rc;
     return (long long)L.bytes;
 }
 
@@ -1251,15 +1248,25 @@ int gmpi_mpi_build_occupancy(const gmpi_render_desc* d, void* occ, size_t bytes)
     if ((rc = check_occ_arg(p, occ, bytes)) != 0) return rc;
     const int words = occ_words(p.Wt), rows = occ_rows(p.Ht);
     if (rows > 65535) return fail(GMPI_ERR_UNSUPPORTED, "Ht=%d exceeds the occupancy build's grid (%d texel rows)", p.Ht, 65535 * kOccB);
+    const bool f16 = (p.options & GMPI_MPI_F16) != 0, u8 = (p.options & GMPI_MPI_U8) != 0;
     const SkipModule* sm = nullptr;
-    if ((rc = skip_module(&sm)) != 0) return rc;
-    const bool f16 = (p.options & GMPI_MPI_F16) != 0;
+    const U8Module* um = nullptr;
+    if ((rc = u8 ? load_module<U8Module>(g_u8, &um) : load_module<SkipModule>(g_skip, &sm)) != 0) return rc;
     const int M = p.M, N = p.N, Ht = p.Ht, Wt = p.Wt;
     cudaLaunchConfig_t cfg = {};
     cfg.blockDim = dim3(32 * kOccB);
     cfg.stream = (cudaStream_t)d->stream;
     uint32_t* map = static_cast<uint32_t*>(occ);
-    if (factored(p)) {
+    if (u8) {
+        // every code is inside [0, 1]: no range bits to set, so the flags are not read
+        const long long P = (long long)M * N;
+        if (P > 0x7fffffffLL) return fail(GMPI_ERR_UNSUPPORTED, "%lld planes exceed the occupancy build (2^31)", P);
+        const int planes = (int)P;
+        cfg.gridDim = dim3(words, rows, planes < 65535 ? planes : 65535);
+        const void* rgba = p.rgba;
+        void* args[] = {&rgba, &map, (void*)&planes, (void*)&Ht, (void*)&Wt, (void*)&words, (void*)&rows};
+        GMPI_CUDA_OK(cudaLaunchKernelExC(&cfg, um->occ, args));
+    } else if (factored(p)) {
         cfg.gridDim = dim3(words, rows, M < 65535 ? M : 65535);
         const void *rgb = p.rgb, *bg = p.bg_rgb, *alpha = p.alpha;
         void* args[] = {&rgb, &bg, &alpha, &map, (void*)&M, (void*)&N, (void*)&Ht, (void*)&Wt, (void*)&words, (void*)&rows};
@@ -1299,6 +1306,22 @@ int gmpi_debug_box_occupied(const uint32_t* plane_map, int Ht, int Wt, int bx0, 
     uint32_t any = 0;
     for (int lane = 0; lane < 32; ++lane) any |= occ_box_bits(plane_map, Ht, Wt, occ_words(Wt), bx0, by0, bw, rows, lane);
     return any != 0;
+}
+
+int gmpi_debug_u8_codes_host(float* out) {
+    if (!out) return fail(GMPI_ERR_INVALID_ARGUMENT, "null pointer");
+    for (int b = 0; b < 256; ++b) out[b] = to_f32((uint8_t)b);
+    return GMPI_OK;
+}
+
+int gmpi_debug_u8_codes(float* out, void* stream) {
+    if (!out) return fail(GMPI_ERR_INVALID_ARGUMENT, "null pointer");
+    const U8Module* um = nullptr;
+    if (int rc = load_module<U8Module>(g_u8, &um)) return rc;
+    cudaLaunchConfig_t cfg = {dim3(1), dim3(256), 0, (cudaStream_t)stream, nullptr, 0};
+    void* args[] = {&out};
+    GMPI_CUDA_OK(cudaLaunchKernelExC(&cfg, um->codes, args));
+    return GMPI_OK;
 }
 
 int gmpi_mpi_check_range(const float* rgba, int M, int N, int Ht, int Wt, uint32_t* flags, void* stream) {
@@ -1495,8 +1518,8 @@ static int host_render_locked(HostCache& c, const RenderParams& h, uint32_t* fla
     const size_t tex = (size_t)h.Ht * h.Wt, img = (size_t)H * W;
     const bool fac = factored(h), video = h.video_rgb != nullptr;
     // one slot = one MPI: expanded [N,4,tex], or factored rgb [3,tex] | bg [3,tex] | alpha [N,tex]
-    // (offsets in MPI elements: fp16 under GMPI_MPI_F16, else fp32)
-    const size_t esz = (h.options & GMPI_MPI_F16) ? 2 : 4;
+    // (offsets in MPI elements: fp16 under GMPI_MPI_F16, uint8 under GMPI_MPI_U8, else fp32)
+    const size_t esz = (h.options & GMPI_MPI_U8) ? 1 : (h.options & GMPI_MPI_F16) ? 2 : 4;
     const size_t o_bg = 3 * tex, o_alpha = h.bg_rgb ? 6 * tex : 3 * tex;
     const size_t mpi_bytes = esz * (fac ? o_alpha + (size_t)N * tex : (size_t)N * 4 * tex);
     auto up = [](size_t x) { return (x + 255) & ~(size_t)255; };

@@ -26,24 +26,6 @@ template <> struct Bits<uint16_t> {
     static __device__ __forceinline__ bool out_of_unit(uint32_t b) { return b > 0x3c00u && b != 0x8000u; }
 };
 
-constexpr int kOccThreads = 32 * kOccB;     // one block row of 256 texel columns = one map word per CTA and plane
-
-// The 256 threads' verdicts (texel column threadIdx.x of this word is occupied) -> the map word: each warp holds 4 blocks of 8 columns.
-__device__ __forceinline__ void store_occ_word(bool occupied, uint32_t* dst, uint32_t* s_w) {
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t b = __ballot_sync(0xffffffffu, occupied);
-    const uint32_t nib = ((b & 0xffu) ? 1u : 0u) | ((b & 0xff00u) ? 2u : 0u) | ((b & 0xff0000u) ? 4u : 0u) | ((b & 0xff000000u) ? 8u : 0u);
-    if (lane == 0) s_w[warp] = nib << (4 * warp);
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        uint32_t w = 0;
-#pragma unroll
-        for (int k = 0; k < kOccThreads / 32; ++k) w |= s_w[k];
-        *dst = w;
-    }
-    __syncthreads();
-}
-
 // Expanded MPI [P = M*N][4][Ht][Wt]: grid (words, block rows, planes in steps of gridDim.z).  flags != NULL: also the range-check bits
 // gmpi_mpi_check_range(_f16) sets, from the same loads.
 template <class U>

@@ -149,9 +149,47 @@ def _half_mpi(mpi, V, H, W, options):
     return half if _lib.fwd_plan(upcast)[0] == _lib.fwd_plan(_mpi_desc(half, V, H, W, options | _lib.OPT_MPI_F16))[0] else None
 
 
-def _launch_mpi(mpi, V, H, W, options):
-    """The MPI tensors `mpi` = [rgba, rgb, alpha, bg_rgb] (None where absent) as the forward reads them, and its options: contiguous
-    fp16 with GMPI_MPI_F16 where _half_mpi renders them natively, else contiguous fp32."""
+_unorm8_tables = {}
+
+
+def unorm8_to_float(x: torch.Tensor) -> torch.Tensor:
+    """The fp32 MPI an 8-bit one stands for: code b -> b / 255 rounded to nearest, what the reference's mpi_from_plane_imgs computes
+    (astype(np.float32) / 255.0, mpi_utils.py:336-337) and what GMPI_MPI_U8 renders.  A lookup in the 256-entry table of torch's CPU
+    division, which rounds each quotient once; x.float() / 255 on a CUDA tensor multiplies by RN(1/255) instead, which differs in the
+    last bit for 126 of the 256 codes."""
+    t = _unorm8_tables.get(x.device)
+    if t is None:
+        t = _unorm8_tables[x.device] = (torch.arange(256, dtype=torch.float32) / 255).to(x.device)
+    return t[x.int()]
+
+
+def _check_unorm8(mpi):
+    """unorm8=True takes an expanded torch.uint8 rgba: TypeError for anything else."""
+    if mpi[0] is None or any(t is not None for t in mpi[1:]):
+        raise TypeError("unorm8=True renders an expanded torch.uint8 rgba (code b = b / 255); got a factored MPI")
+    if mpi[0].dtype != torch.uint8:
+        raise TypeError(f"unorm8=True renders an expanded torch.uint8 rgba (code b = b / 255); got rgba of dtype {mpi[0].dtype}")
+
+
+def _unorm8_mpi(mpi, V, H, W, options):
+    """unorm8=True: the uint8 rgba of `mpi` = [rgba, rgb, alpha, bg_rgb] as the forward reads it, and its options.  Native (contiguous
+    uint8 with GMPI_MPI_U8) when the uint8 MPI gets the kernel plan a fresh fp32 allocation of its shape would get (the staged kernels
+    need Wt % 16 == 0 and a 16-byte aligned base in uint8), else its fp32 conversion (unorm8_to_float): the output is bitwise the
+    render of that conversion either way."""
+    _check_unorm8(mpi)
+    u8 = [mpi[0].contiguous(), None, None, None]
+    fp32 = _mpi_desc(u8, V, H, W, options)
+    fp32.rgba = None                     # a fresh, aligned allocation
+    if _lib.fwd_plan(fp32)[0] == _lib.fwd_plan(_mpi_desc(u8, V, H, W, options | _lib.OPT_MPI_U8))[0]:
+        return u8, options | _lib.OPT_MPI_U8
+    return [unorm8_to_float(u8[0]), None, None, None], options
+
+
+def _launch_mpi(mpi, V, H, W, options, unorm8=False):
+    """The MPI tensors `mpi` = [rgba, rgb, alpha, bg_rgb] (None where absent) as the forward reads them, and its options: with unorm8,
+    see _unorm8_mpi; else contiguous fp16 with GMPI_MPI_F16 where _half_mpi renders them natively, else contiguous fp32."""
+    if unorm8:
+        return _unorm8_mpi(mpi, V, H, W, options)
     half = _half_mpi(mpi, V, H, W, options)
     if half is not None:
         return half, options | _lib.OPT_MPI_F16
@@ -164,7 +202,7 @@ _warned_direct = set()
 def _warn_if_direct(d):
     """Surface the direct-kernel performance cliff (several times slower than the TMA-staged kernels) of the forward descriptor `d`
     is about to launch, once per shape, MPI dtype and MPI base alignment."""
-    key = (d.M, d.V, d.N, d.Ht, d.Wt, d.H, d.W, d.options & _lib.OPT_MPI_F16) + \
+    key = (d.M, d.V, d.N, d.Ht, d.Wt, d.H, d.W, d.options & (_lib.OPT_MPI_F16 | _lib.OPT_MPI_U8)) + \
         tuple((p or 0) & 15 for p in (d.rgba, d.rgb, d.alpha, d.bg_rgb))
     if key in _warned_direct:
         return
@@ -214,18 +252,25 @@ class Occupancy:
                                "build it again (build_occupancy)")
 
 
-def build_occupancy(*, rgba=None, rgb=None, alpha=None, bg_rgb=None, flags: Optional[torch.Tensor] = None) -> Occupancy:
+def build_occupancy(*, rgba=None, rgb=None, alpha=None, bg_rgb=None, flags: Optional[torch.Tensor] = None,
+                    unorm8: bool = False) -> Occupancy:
     """The occupancy map of an expanded MPI rgba [M,N,4,Ht,Wt], or of a factored one (rgb [M,3,Ht,Wt], alpha [M,N,1,Ht,Wt], bg_rgb),
     fp32 or fp16, for render_views / render_views_factored / render_frames(skip_empty=...).  One streaming pass over the MPI (the
     factored MPI's colour is read once, its alpha per plane).  `flags` (expanded MPI): also OR in the range-check bits check_range
-    sets, from the same pass."""
+    sets, from the same pass.  unorm8=True: rgba is an 8-bit MPI (render_views(unorm8=True)); the pass reads its alpha bytes only,
+    and every code is inside [0, 1], so there are no range bits to set."""
     mpi = [rgba, rgb, alpha, bg_rgb]
     ref = _mpi_ref(mpi)
     _require_cuda(ref)
     ts = [t for t in mpi if t is not None]
-    half = all(t.dtype == torch.float16 for t in ts)     # the map of an fp16 MPI is the map of its fp32 upcast
-    launch = [None if t is None else (t.detach().contiguous() if half else _as_f32c(t.detach())) for t in mpi]
-    d = _mpi_desc(launch, 1, 1, 1, _lib.OPT_MPI_F16 if half else 0)
+    if unorm8:
+        _check_unorm8(mpi)
+        launch, options = [rgba.detach().contiguous(), None, None, None], _lib.OPT_MPI_U8
+    else:
+        half = all(t.dtype == torch.float16 for t in ts)     # the map of an fp16 MPI is the map of its fp32 upcast
+        launch = [None if t is None else (t.detach().contiguous() if half else _as_f32c(t.detach())) for t in mpi]
+        options = _lib.OPT_MPI_F16 if half else 0
+    d = _mpi_desc(launch, 1, 1, 1, options)
     n = _lib.occupancy_bytes(d)
     dev = ref.device
     occ = torch.empty((n + 3) // 4, dtype=torch.int32, device=dev)
@@ -236,11 +281,13 @@ def build_occupancy(*, rgba=None, rgb=None, alpha=None, bg_rgb=None, flags: Opti
     return Occupancy(occ, n, mpi)
 
 
-def _occupancy_for(skip_empty, mpi) -> Optional[Occupancy]:
+def _occupancy_for(skip_empty, mpi, unorm8=False) -> Optional[Occupancy]:
     """skip_empty of a render: False -> None; True -> a map built for this call; an Occupancy -> itself, if it describes `mpi`."""
     if skip_empty is False or skip_empty is None:
         return None
     if skip_empty is True:
+        if unorm8:
+            return build_occupancy(rgba=mpi[0], unorm8=True)
         return build_occupancy(rgba=mpi[0], rgb=mpi[1], alpha=mpi[2], bg_rgb=mpi[3])
     if not isinstance(skip_empty, Occupancy):
         raise TypeError(f"skip_empty must be a bool or an Occupancy, got {type(skip_empty).__name__}")
@@ -250,7 +297,7 @@ def _occupancy_for(skip_empty, mpi) -> Optional[Occupancy]:
 
 def render_views(rgba, dhw, view2mpi, ray_dir, eye, z_dir, *, align_corners=True, check_last_plane=False,
                  color_minus1_1=False, flags: Optional[torch.Tensor] = None, view_group: int = 1, early_stop: Optional[float] = None,
-                 deterministic: Optional[bool] = None, skip_empty: Union[bool, Occupancy] = False):
+                 deterministic: Optional[bool] = None, skip_empty: Union[bool, Occupancy] = False, unorm8: bool = False):
     """Functional form on packed tensors (no list handling, no host sync).
     rgba [M,N,4,Ht,Wt], dhw [M,N,3], view2mpi [V] int32, ray_dir [V,3,H,W], eye/z_dir [V,3].
     Returns (color [V,3,H,W], depth [V,1,H,W]); `flags` (uint32 tensor of 1, int32 storage) is OR-ed into.
@@ -261,9 +308,13 @@ def render_views(rgba, dhw, view2mpi, ray_dir, eye, z_dir, *, align_corners=True
     gmpi_mpi_render_bwd_deterministic_ex); None follows torch.are_deterministic_algorithms_enabled() at the time of this call.
     skip_empty: empty-space skipping (gmpi_mpi_render_fwd_skip_ex): the staged kernel does not load or composite the (tile, plane)
     boxes whose texels all have alpha +0 and finite colour; bitwise the same output.  True builds the map for this call
-    (build_occupancy, one pass over the MPI); an Occupancy is reused.  Forward only: refused when an input requires grad."""
+    (build_occupancy, one pass over the MPI); an Occupancy is reused.  Forward only: refused when an input requires grad.
+    unorm8=True: rgba is an 8-bit MPI (torch.uint8, TypeError otherwise) whose code b stands for b / 255, the planar RGBA8 plane images
+    of the reference's mpi_from_plane_imgs.  Rendered natively (GMPI_MPI_U8: a quarter of the fp32 bytes, no fp32 copy) where the
+    kernel plan allows, else from its fp32 conversion; the output is bitwise render_views(unorm8_to_float(rgba)) either way.  With
+    unorm8=False a uint8 rgba is upcast without scaling, as before."""
     return _render_views([rgba, None, None, None], dhw, view2mpi, ray_dir, eye, z_dir, align_corners, check_last_plane, color_minus1_1,
-                         flags, view_group, early_stop, deterministic, skip_empty)
+                         flags, view_group, early_stop, deterministic, skip_empty, unorm8)
 
 
 def render_views_factored(rgb, alpha, dhw, view2mpi, ray_dir, eye, z_dir, *, bg_rgb=None, align_corners=True,
@@ -280,7 +331,7 @@ def render_views_factored(rgb, alpha, dhw, view2mpi, ray_dir, eye, z_dir, *, bg_
 
 
 def _render_views(mpi, dhw, view2mpi, ray_dir, eye, z_dir, align_corners, check_last_plane, color_minus1_1, flags, view_group,
-                  early_stop, deterministic, skip_empty):
+                  early_stop, deterministic, skip_empty, unorm8=False):
     """render_views of the MPI tensors `mpi` = [rgba, rgb, alpha, bg_rgb] (None where absent), and render_views_factored."""
     _check_forward_only("early_stop", early_stop is not None, *mpi)
     _check_forward_only("skip_empty", skip_empty is not False and skip_empty is not None, *mpi)
@@ -293,9 +344,11 @@ def _render_views(mpi, dhw, view2mpi, ray_dir, eye, z_dir, align_corners, check_
         assert bg_rgb is None or bg_rgb.shape == rgb.shape, f"bg_rgb must have rgb's shape, got {bg_rgb.shape}"
     if flags is None:
         flags = _zero_flags(ref.device)
-    occ = _occupancy_for(skip_empty, mpi)
     V, _, H, W = ray_dir.shape
-    mpi, options = _launch_mpi(mpi, V, H, W, _options(align_corners, check_last_plane, color_minus1_1, early_stop=early_stop))
+    if unorm8:
+        _check_unorm8(mpi)
+    occ = _occupancy_for(skip_empty, mpi, unorm8)
+    mpi, options = _launch_mpi(mpi, V, H, W, _options(align_corners, check_last_plane, color_minus1_1, early_stop=early_stop), unorm8)
     _warn_if_direct(_mpi_desc(mpi, V, H, W, options))
     return _RenderFn.apply(*mpi, _as_f32c(dhw), view2mpi, _as_f32c(ray_dir), _as_f32c(eye), _as_f32c(z_dir),
                            options, flags, int(view_group), early_stop, deterministic, occ)
@@ -314,8 +367,9 @@ def expand_factored(rgb, alpha, bg_rgb=None):
 def render_frames(*, dhw, view2mpi, rgba=None, rgb=None, alpha=None, bg_rgb=None, ray_dir=None, eye=None, z_dir=None, cam=None,
                   align_corners=True, check_last_plane=False, video: Optional[dict] = None, u8_round=False,
                   flags: Optional[torch.Tensor] = None, view_group: int = 1, H: Optional[int] = None, W: Optional[int] = None,
-                  early_stop: Optional[float] = None, skip_empty: Union[bool, Occupancy] = False):
+                  early_stop: Optional[float] = None, skip_empty: Union[bool, Occupancy] = False, unorm8: bool = False):
     """Inference-only render with the opt-in fast paths of the C ABI (no autograd):
+      unorm8=True    rgba is an 8-bit MPI, code b = b / 255 (see render_views).
       skip_empty=True or an Occupancy   empty-space skipping, bitwise the same frames (see render_views).
       cam [V,16]     rays generated in the kernel from the pinhole camera (see camera.cam_params) instead of ray_dir/eye/z_dir;
       video={"near": ray_start, "far": ray_end, "depth": True}   uint8 HWC frames as render_video.py:118-126 builds them:
@@ -348,8 +402,10 @@ def render_frames(*, dhw, view2mpi, rgba=None, rgb=None, alpha=None, bg_rgb=None
     else:
         color = torch.empty((V, 3, H, W), device=dev, dtype=torch.float32)
         depth = torch.empty((V, 1, H, W), device=dev, dtype=torch.float32)
-    occ = _occupancy_for(skip_empty, mpi)
-    mpi, options = _launch_mpi(mpi, V, H, W, _options(align_corners, check_last_plane, True, u8_round, early_stop))
+    if unorm8:
+        _check_unorm8(mpi)
+    occ = _occupancy_for(skip_empty, mpi, unorm8)
+    mpi, options = _launch_mpi(mpi, V, H, W, _options(align_corners, check_last_plane, True, u8_round, early_stop), unorm8)
     _render_fwd(_mpi_desc(mpi, V, H, W, options, view_group=int(view_group), depth_near=near, depth_range=rng, view2mpi=view2mpi,
                           dhw=_as_f32c(dhw), ray_dir=ray_dir, eye=eye, z_dir=z_dir, cam=cam, color=color, depth=depth, video_rgb=v_rgb,
                           video_depth=v_depth, flags=flags, early_stop=early_stop), occ, dev)
