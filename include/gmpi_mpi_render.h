@@ -404,7 +404,7 @@ int gmpi_debug_fwd_skip_stats(unsigned long long* skipped, unsigned long long* t
 int gmpi_debug_box_occupied(const uint32_t* plane_map, int Ht, int Wt, int bx0, int by0, int bw, int rows);
 
 /* Test hooks of the GMPI_MPI_U8 conversion: out[b] = the fp32 value of code b for the 256 codes.  _host: the host build, out is host
- * memory (no GPU work); without the suffix: the device build (a kernel of the uint8 module), out is device memory, on `stream`. */
+ * memory (no GPU work); without the suffix: the device build (a kernel of mpi_u8.cu), out is device memory, on `stream`. */
 int gmpi_debug_u8_codes_host(float* out);
 int gmpi_debug_u8_codes(float* out, void* stream);
 

@@ -1,4 +1,8 @@
-"""In-tree build of the CUDA library (nvcc, sm_90a only).  The .so is git-ignored: build() makes it."""
+"""In-tree build of the CUDA library (nvcc, sm_90a only).  The .so is git-ignored: build() makes it.
+
+One nvcc call compiles and links the library's three translation units: mpi_render.cu, and the empty-space skipping (mpi_skip.cu)
+and uint8-MPI (mpi_u8.cu) kernels it launches.  Without -rdc each file's device code is compiled on its own, so the kernels of one
+file keep their machine code whatever the others add."""
 import os
 import shutil
 import subprocess
@@ -6,18 +10,11 @@ import subprocess
 PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_PATH = os.path.join(PKG_DIR, "libgmpi_mpi_render.so")
-# the empty-space skipping kernels: a module of their own, loaded by the library on first use (the library's kernels keep their
-# machine code)
-SKIP_PATH = os.path.join(PKG_DIR, "libgmpi_mpi_render_skip.fatbin")
-# the uint8-MPI kernels (GMPI_MPI_U8): likewise a module of their own
-U8_PATH = os.path.join(PKG_DIR, "libgmpi_mpi_render_u8.fatbin")
-SOURCES = ["mpi_render.cu"]
-SKIP_SOURCES = ["mpi_skip.cu"]
-U8_SOURCES = ["mpi_u8.cu"]
-HEADERS = ["mpi_common.cuh", "mpi_fwd_staged.cuh", "mpi_fwd_direct.cuh", "mpi_bwd_box.cuh", "tma_utils.cuh",
+SOURCES = ["mpi_render.cu", "mpi_skip.cu", "mpi_u8.cu"]
+HEADERS = ["mpi_common.cuh", "mpi_fwd_staged.cuh", "mpi_fwd_direct.cuh", "mpi_fwd_units.cuh", "mpi_bwd_box.cuh", "tma_utils.cuh",
            os.path.join("..", "..", "include", "gmpi_mpi_render.h")]
-ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-diag-suppress", "1886"]
-NVCC_FLAGS = ARCH_FLAGS + ["-shared", "-Xcompiler", "-fPIC"]
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-diag-suppress", "1886", "-shared",
+              "-Xcompiler", "-fPIC"]
 
 
 def nvcc_path():
@@ -44,10 +41,7 @@ def _nvcc(args, verbose):
 
 
 def build_library(force: bool = False, verbose: bool = False) -> str:
-    """Builds the library and the skipping and uint8 modules next to it; returns the library's path."""
-    for path, sources in ((SKIP_PATH, SKIP_SOURCES), (U8_PATH, U8_SOURCES)):
-        if force or is_stale(path):
-            _nvcc(ARCH_FLAGS + ["-fatbin", "-o", path] + sources, verbose)
+    """Builds the library; returns its path."""
     if force or is_stale(LIB_PATH):
         _nvcc(NVCC_FLAGS + ["-o", LIB_PATH] + SOURCES, verbose)
     return LIB_PATH

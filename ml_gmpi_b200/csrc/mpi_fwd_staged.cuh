@@ -243,22 +243,30 @@ __device__ __forceinline__ bool sample_pairs(const E* __restrict__ sb, int cx, i
 // Expanded MPI: ONE base pointer crosses the call.  (Passing the four channel pointers of PlaneChans instead -- 8 registers that
 // are live only inside the rare branch -- still shifted the register allocation of the hot loop: -3.8 % frames/s, bisected on
 // the GPU in round 2.  The factored instantiation, which needs them, is a separate template instance.)
-__device__ __noinline__ float4 sample_plane_direct(const float* __restrict__ plane, int Ht, int Wt, float ix, float iy) {
+// Three translation units of the one library define the four non-template overloads.  Their host stubs are static, so that the
+// library links; their device code keeps external linkage, because static device functions change where ptxas places the
+// deterministic box backward's subroutines, and so that kernel's machine code.
+#ifdef __CUDA_ARCH__
+#define GMPI_HOST_STATIC
+#else
+#define GMPI_HOST_STATIC static
+#endif
+GMPI_HOST_STATIC __device__ __noinline__ float4 sample_plane_direct(const float* __restrict__ plane, int Ht, int Wt, float ix, float iy) {
     const size_t tex = (size_t)Ht * Wt;
     const Taps tp = make_taps(ix, iy, Ht, Wt);
     return make_float4(tap4(plane, tp), tap4(plane + tex, tp), tap4(plane + 2 * tex, tp), tap4(plane + 3 * tex, tp));
 }
-__device__ __noinline__ float4 sample_chans_direct(const PlaneChans pl, int Ht, int Wt, float ix, float iy) {
+GMPI_HOST_STATIC __device__ __noinline__ float4 sample_chans_direct(const PlaneChans pl, int Ht, int Wt, float ix, float iy) {
     const Taps tp = make_taps(ix, iy, Ht, Wt);
     return make_float4(tap4(pl.c[0], tp), tap4(pl.c[1], tp), tap4(pl.c[2], tp), tap4(pl.c[3], tp));
 }
 // the same from an fp16 MPI (overloads, so that the fp32 functions keep their symbols)
-__device__ __noinline__ float4 sample_plane_direct(const __half* __restrict__ plane, int Ht, int Wt, float ix, float iy) {
+GMPI_HOST_STATIC __device__ __noinline__ float4 sample_plane_direct(const __half* __restrict__ plane, int Ht, int Wt, float ix, float iy) {
     const size_t tex = (size_t)Ht * Wt;
     const Taps tp = make_taps(ix, iy, Ht, Wt);
     return make_float4(tap4(plane, tp), tap4(plane + tex, tp), tap4(plane + 2 * tex, tp), tap4(plane + 3 * tex, tp));
 }
-__device__ __noinline__ float4 sample_chans_direct(const PlaneChansT<__half> pl, int Ht, int Wt, float ix, float iy) {
+GMPI_HOST_STATIC __device__ __noinline__ float4 sample_chans_direct(const PlaneChansT<__half> pl, int Ht, int Wt, float ix, float iy) {
     const Taps tp = make_taps(ix, iy, Ht, Wt);
     return make_float4(tap4(pl.c[0], tp), tap4(pl.c[1], tp), tap4(pl.c[2], tp), tap4(pl.c[3], tp));
 }

@@ -3,7 +3,6 @@
 // Replaces gmpi/core/mpi.py MPI.forward (:308-436) + homography (:26-153) and their autograd.
 // DESIGN.md describes the data layout, each kernel and its roofline.
 #include <cuda_runtime.h>
-#include <dlfcn.h>
 #include <stdarg.h>
 #include <stdint.h>
 #include <math.h>
@@ -12,7 +11,6 @@
 
 #include <atomic>
 #include <mutex>
-#include <string>
 
 #include "../../include/gmpi_mpi_render.h"
 #include "mpi_common.cuh"
@@ -20,6 +18,7 @@
 #include "mpi_bwd_box.cuh"
 #include "mpi_light.cuh"
 #include "mpi_fwd_direct.cuh"
+#include "mpi_fwd_units.cuh"
 
 namespace gmpi {
 
@@ -538,12 +537,17 @@ static int fwd_ring_stages(const RenderParams& p, int l2_bytes) {
 
 // What picks a render kernel: the bits of its variant.  kKeyStaged: a persistent TMA kernel (the staged forward, the box backward).
 // The direct forward's key has no kKeyFac and no kKeyEmit, and the direct backward's no kKeyFac: those kernels read both at run time.
-enum : uint32_t { kKeyAC = 1, kKeyFac = 2, kKeyEmit = 4, kKeyES = 8, kKeyF16 = 16, kKeyStaged = 32, kKeyBwd = 64, kKeyDet = 128 };
+// kKeySkip: empty-space skipping (the kernels of mpi_skip.cu, or of mpi_u8.cu with kKeyU8).  kKeyU8: a uint8 MPI (mpi_u8.cu).
+enum : uint32_t {
+    kKeyAC = 1, kKeyFac = 2, kKeyEmit = 4, kKeyES = 8, kKeyF16 = 16, kKeyStaged = 32, kKeyBwd = 64, kKeyDet = 128, kKeySkip = 256,
+    kKeyU8 = 512
+};
 
-// Every statically built render kernel by its key.  This switch is the first reference to each kernel, so its cases give the order
-// the kernels are instantiated in, and ptxas gives some kernels other machine code when that order changes (the expanded box
+// Every render kernel by its key.  This switch is the first reference to each kernel template of this file, so its cases give the
+// order the kernels are instantiated in, and ptxas gives some kernels other machine code when that order changes (the expanded box
 // backward's, when the four box kernels are listed by [align_corners][factored]).  Do not reorder the cases: the recorded SASS
-// digests (tests/golden/sass_digests.json) check the machine code.  A key without a kernel gives nullptr, which the launch refuses.
+// digests (tests/golden/sass_digests.json) check the machine code.  The kernels of mpi_skip.cu and mpi_u8.cu come last.  A key
+// without a kernel gives nullptr, which the launch refuses.
 static const void* render_kernel(uint32_t key) {
     switch (key) {
     case kKeyStaged: return (const void*)mpi_fwd_staged_kernel<false, false, false>;
@@ -586,13 +590,41 @@ static const void* render_kernel(uint32_t key) {
     case kKeyBwd | kKeyStaged | kKeyFac: return (const void*)mpi_bwd_box_kernel<false, true>;
     case kKeyBwd | kKeyStaged | kKeyAC: return (const void*)mpi_bwd_box_kernel<true, false>;
     case kKeyBwd | kKeyStaged: return (const void*)mpi_bwd_box_kernel<false, false>;
+    case kKeySkip | kKeyStaged: return (const void*)gmpi_fwd_skip_a0_x0_e0_f32;
+    case kKeySkip | kKeyStaged | kKeyES: return (const void*)gmpi_fwd_skip_a0_x0_e1_f32;
+    case kKeySkip | kKeyStaged | kKeyFac: return (const void*)gmpi_fwd_skip_a0_x1_e0_f32;
+    case kKeySkip | kKeyStaged | kKeyFac | kKeyES: return (const void*)gmpi_fwd_skip_a0_x1_e1_f32;
+    case kKeySkip | kKeyStaged | kKeyAC: return (const void*)gmpi_fwd_skip_a1_x0_e0_f32;
+    case kKeySkip | kKeyStaged | kKeyAC | kKeyES: return (const void*)gmpi_fwd_skip_a1_x0_e1_f32;
+    case kKeySkip | kKeyStaged | kKeyAC | kKeyFac: return (const void*)gmpi_fwd_skip_a1_x1_e0_f32;
+    case kKeySkip | kKeyStaged | kKeyAC | kKeyFac | kKeyES: return (const void*)gmpi_fwd_skip_a1_x1_e1_f32;
+    case kKeySkip | kKeyStaged | kKeyF16: return (const void*)gmpi_fwd_skip_a0_x0_e0_f16;
+    case kKeySkip | kKeyStaged | kKeyF16 | kKeyES: return (const void*)gmpi_fwd_skip_a0_x0_e1_f16;
+    case kKeySkip | kKeyStaged | kKeyF16 | kKeyFac: return (const void*)gmpi_fwd_skip_a0_x1_e0_f16;
+    case kKeySkip | kKeyStaged | kKeyF16 | kKeyFac | kKeyES: return (const void*)gmpi_fwd_skip_a0_x1_e1_f16;
+    case kKeySkip | kKeyStaged | kKeyF16 | kKeyAC: return (const void*)gmpi_fwd_skip_a1_x0_e0_f16;
+    case kKeySkip | kKeyStaged | kKeyF16 | kKeyAC | kKeyES: return (const void*)gmpi_fwd_skip_a1_x0_e1_f16;
+    case kKeySkip | kKeyStaged | kKeyF16 | kKeyAC | kKeyFac: return (const void*)gmpi_fwd_skip_a1_x1_e0_f16;
+    case kKeySkip | kKeyStaged | kKeyF16 | kKeyAC | kKeyFac | kKeyES: return (const void*)gmpi_fwd_skip_a1_x1_e1_f16;
+    case kKeyU8 | kKeyStaged: return (const void*)gmpi_fwd_u8_a0_e0;
+    case kKeyU8 | kKeyStaged | kKeyES: return (const void*)gmpi_fwd_u8_a0_e1;
+    case kKeyU8 | kKeyStaged | kKeyAC: return (const void*)gmpi_fwd_u8_a1_e0;
+    case kKeyU8 | kKeyStaged | kKeyAC | kKeyES: return (const void*)gmpi_fwd_u8_a1_e1;
+    case kKeyU8 | kKeySkip | kKeyStaged: return (const void*)gmpi_fwd_u8_skip_a0_e0;
+    case kKeyU8 | kKeySkip | kKeyStaged | kKeyES: return (const void*)gmpi_fwd_u8_skip_a0_e1;
+    case kKeyU8 | kKeySkip | kKeyStaged | kKeyAC: return (const void*)gmpi_fwd_u8_skip_a1_e0;
+    case kKeyU8 | kKeySkip | kKeyStaged | kKeyAC | kKeyES: return (const void*)gmpi_fwd_u8_skip_a1_e1;
+    case kKeyU8: return (const void*)gmpi_fwd_direct_u8_a0_e0;
+    case kKeyU8 | kKeyES: return (const void*)gmpi_fwd_direct_u8_a0_e1;
+    case kKeyU8 | kKeyAC: return (const void*)gmpi_fwd_direct_u8_a1_e0;
+    case kKeyU8 | kKeyAC | kKeyES: return (const void*)gmpi_fwd_direct_u8_a1_e1;
     }
     return nullptr;
 }
 
 // Everything one render-kernel launch needs.  The arguments point into this object, so it is built in place and never copied.
 struct Launch {
-    const void* kernel = nullptr;    // a static kernel (render_kernel) or a kernel of the skipping module
+    const void* kernel = nullptr;    // render_kernel(key)
     dim3 grid, block;
     size_t smem = 0;
     long tiles = 0;                  // the tiles of all views a persistent kernel walks (0: a direct kernel)
@@ -644,121 +676,43 @@ static size_t fwd_staged_smem(bool fac, int stages, bool f16, bool u8) {
     return ring + (size_t)kMaxPlanesStaged * 32;
 }
 
-// ---- kernel modules next to this library: the kernels of opt-in features that live in a module of their own, so that this
-// library's kernels keep their machine code.  Each is loaded on first use (a context-independent library: the runtime loads it into
-// each device's context when a kernel of it first runs there).
-//   libgmpi_mpi_render_skip.fatbin   empty-space skipping (mpi_skip.cu)
-//   libgmpi_mpi_render_u8.fatbin     uint8 MPIs, GMPI_MPI_U8 (mpi_u8.cu)
-struct SkipModule {
-    cudaKernel_t fwd[2][2][2][2];           // [f16][align_corners][factored][early_stop]
-    cudaKernel_t occ_exp[2], occ_fac[2];    // [f16]
-    static int get(cudaLibrary_t lib, SkipModule& m);
-};
-struct U8Module {
-    cudaKernel_t staged[2][2][2];           // [skip][align_corners][early_stop]
-    cudaKernel_t direct[2][2];              // [align_corners][early_stop]
-    cudaKernel_t occ, codes;
-    static int get(cudaLibrary_t lib, U8Module& m);
-};
-template <class K>
-struct Module {
-    const char* file;
-    cudaLibrary_t lib = nullptr;
-    K k;
-    std::mutex mutex;
-};
-static Module<SkipModule> g_skip{"libgmpi_mpi_render_skip.fatbin"};
-static Module<U8Module> g_u8{"libgmpi_mpi_render_u8.fatbin"};
-
-static int get_kernel(cudaLibrary_t lib, cudaKernel_t* k, const char* fmt, ...) {
-    char name[64];
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(name, sizeof(name), fmt, ap);
-    va_end(ap);
-    GMPI_CUDA_OK(cudaLibraryGetKernel(k, lib, name));
-    return GMPI_OK;
-}
-
-int SkipModule::get(cudaLibrary_t lib, SkipModule& m) {
-    for (int h = 0; h < 2; ++h) {
-        for (int a = 0; a < 2; ++a)
-            for (int x = 0; x < 2; ++x)
-                for (int s = 0; s < 2; ++s)
-                    if (int rc = get_kernel(lib, &m.fwd[h][a][x][s], "gmpi_fwd_skip_a%d_x%d_e%d_%s", a, x, s, h ? "f16" : "f32")) return rc;
-        if (int rc = get_kernel(lib, &m.occ_exp[h], "gmpi_occ_expanded_%s", h ? "f16" : "f32")) return rc;
-        if (int rc = get_kernel(lib, &m.occ_fac[h], "gmpi_occ_factored_%s", h ? "f16" : "f32")) return rc;
-    }
-    return GMPI_OK;
-}
-
-int U8Module::get(cudaLibrary_t lib, U8Module& m) {
-    for (int a = 0; a < 2; ++a)
-        for (int s = 0; s < 2; ++s) {
-            if (int rc = get_kernel(lib, &m.staged[0][a][s], "gmpi_fwd_u8_a%d_e%d", a, s)) return rc;
-            if (int rc = get_kernel(lib, &m.staged[1][a][s], "gmpi_fwd_u8_skip_a%d_e%d", a, s)) return rc;
-            if (int rc = get_kernel(lib, &m.direct[a][s], "gmpi_fwd_direct_u8_a%d_e%d", a, s)) return rc;
-        }
-    if (int rc = get_kernel(lib, &m.occ, "gmpi_occ_expanded_u8")) return rc;
-    return get_kernel(lib, &m.codes, "gmpi_u8_codes");
-}
-
-// The module's library and kernels, loaded on the first call.
-template <class K>
-static int load_module(Module<K>& mod, const K** kernels, cudaLibrary_t* lib = nullptr) {
-    std::lock_guard<std::mutex> lock(mod.mutex);
-    if (!mod.lib) {
-        Dl_info info;
-        if (!dladdr(reinterpret_cast<void*>(&gmpi_abi_version), &info) || !info.dli_fname)
-            return fail(GMPI_ERR_CUDA, "cannot locate the library file (dladdr)");
-        std::string path(info.dli_fname);
-        path = path.substr(0, path.find_last_of('/') + 1) + mod.file;
-        cudaLibrary_t l = nullptr;
-        const cudaError_t e = cudaLibraryLoadFromFile(&l, path.c_str(), nullptr, nullptr, 0, nullptr, nullptr, 0);
-        if (e != cudaSuccess) return fail(GMPI_ERR_CUDA, "loading %s failed: %s", path.c_str(), cudaGetErrorString(e));
-        if (int rc = K::get(l, mod.k)) return rc;
-        mod.lib = l;
-    }
-    if (kernels) *kernels = &mod.k;
-    if (lib) *lib = mod.lib;
-    return GMPI_OK;
-}
-
 // The stage counters of the test hooks gmpi_debug_fwd_early_stop_stats and gmpi_debug_fwd_skip_stats: on the device, the stages
 // the last early-stop or skipping launch armed without copies (zeroed on its stream); here, the (tile, plane) stages it walked and
-// whether a kernel of the uint8 module ran it (that module has counters of its own).
+// which file's kernels it launched.  Each file has its own copy of g_early_stop_skipped (mpi_fwd_staged.cuh); the skipping kernels of
+// mpi_skip.cu and mpi_u8.cu count into their file's gmpi_skip_empty_stages (OccMap::skipped).
 enum StageStats { kEarlyStopStats, kSkipStats };
+enum KernelFile { kRenderFile, kSkipFile, kU8File };     // mpi_render.cu, mpi_skip.cu, mpi_u8.cu
 static std::atomic<unsigned long long> g_stages_walked[2];
-static std::atomic<bool> g_stages_u8[2];
+static std::atomic<int> g_stages_file[2] = {{kRenderFile}, {kSkipFile}};     // before any launch too: mpi_render.cu has no skip counter
 
-// The device counter on the current device: a global of this library or of the module whose kernel ran (u8).  The uint8 module's
-// early-stop counter is its own copy of g_early_stop_skipped (mpi_fwd_staged.cuh), found by its mangled name.
-static int stage_counter(StageStats s, bool u8, unsigned long long** counter) {
-    if (s == kEarlyStopStats && !u8) {
-        GMPI_CUDA_OK(cudaGetSymbolAddress(reinterpret_cast<void**>(counter), g_early_stop_skipped));
-        return GMPI_OK;
-    }
-    cudaLibrary_t lib = nullptr;
-    if (int rc = u8 ? load_module<U8Module>(g_u8, nullptr, &lib) : load_module<SkipModule>(g_skip, nullptr, &lib)) return rc;
-    size_t bytes = 0;
-    GMPI_CUDA_OK(cudaLibraryGetGlobal(reinterpret_cast<void**>(counter), &bytes, lib,
-                                      s == kEarlyStopStats ? "_ZN4gmpi20g_early_stop_skippedE" : "gmpi_skip_empty_stages"));
+// The file of a forward call's staged kernel.  The direct kernels count no stages, so the counters of that file read 0 after them.
+static KernelFile kernel_file(const RenderParams& p, const uint32_t* occ) {
+    return (p.options & GMPI_MPI_U8) ? kU8File : occ ? kSkipFile : kRenderFile;
+}
+
+// The device counter on the current device (mpi_render.cu has no skipping kernels, so no skip counter).
+static int stage_counter(StageStats s, KernelFile file, unsigned long long** counter) {
+    unsigned long long* c[2] = {nullptr, nullptr};
+    if (file == kRenderFile) GMPI_CUDA_OK(cudaGetSymbolAddress(reinterpret_cast<void**>(&c[kEarlyStopStats]), g_early_stop_skipped));
+    if (file == kSkipFile) GMPI_CUDA_OK(skip_stage_counters(&c[kEarlyStopStats], &c[kSkipStats]));
+    if (file == kU8File) GMPI_CUDA_OK(u8_stage_counters(&c[kEarlyStopStats], &c[kSkipStats]));
+    *counter = c[s];
     return GMPI_OK;
 }
 
-static int reset_stage_stats(StageStats s, bool u8, unsigned long long walked, cudaStream_t st) {
+static int reset_stage_stats(StageStats s, KernelFile file, unsigned long long walked, cudaStream_t st) {
     unsigned long long* counter = nullptr;
-    if (int rc = stage_counter(s, u8, &counter)) return rc;
+    if (int rc = stage_counter(s, file, &counter)) return rc;
     GMPI_CUDA_OK(cudaMemsetAsync(counter, 0, sizeof(unsigned long long), st));
     g_stages_walked[s].store(walked, std::memory_order_relaxed);
-    g_stages_u8[s].store(u8, std::memory_order_relaxed);
+    g_stages_file[s].store(file, std::memory_order_relaxed);
     return GMPI_OK;
 }
 
 static int read_stage_stats(StageStats s, unsigned long long* skipped, unsigned long long* walked) {
     if (!skipped || !walked) return fail(GMPI_ERR_INVALID_ARGUMENT, "null pointer");
     unsigned long long* counter = nullptr;
-    if (int rc = stage_counter(s, g_stages_u8[s].load(std::memory_order_relaxed), &counter)) return rc;
+    if (int rc = stage_counter(s, (KernelFile)g_stages_file[s].load(std::memory_order_relaxed), &counter)) return rc;
     GMPI_CUDA_OK(cudaDeviceSynchronize());
     GMPI_CUDA_OK(cudaMemcpy(skipped, counter, sizeof(unsigned long long), cudaMemcpyDeviceToHost));
     *walked = g_stages_walked[s].load(std::memory_order_relaxed);
@@ -788,12 +742,10 @@ static int check_occ_arg(const RenderParams& p, const void* occ, size_t bytes) {
 // kernel when fwd_why(p) == 0 and its tensor maps encode, else the direct kernel; a forced staged variant fails instead.
 static int fwd_launch(Launch& l, const uint32_t* occ) {
     const RenderParams& p = l.p;
-    const bool ac = (p.options & GMPI_ALIGN_CORNERS) != 0, fac = factored(p), es = (p.options & GMPI_EARLY_STOP) != 0;
-    const bool f16 = (p.options & GMPI_MPI_F16) != 0, u8 = (p.options & GMPI_MPI_U8) != 0;
-    const uint32_t key = (ac ? kKeyAC : 0) | (es ? kKeyES : 0) | (f16 ? kKeyF16 : 0);
-    const U8Module* um = nullptr;     // u8: every kernel comes from the uint8 module
+    const bool fac = factored(p), f16 = (p.options & GMPI_MPI_F16) != 0, u8 = (p.options & GMPI_MPI_U8) != 0;
+    uint32_t key = ((p.options & GMPI_ALIGN_CORNERS) ? kKeyAC : 0) | ((p.options & GMPI_EARLY_STOP) ? kKeyES : 0) |
+                   (f16 ? kKeyF16 : 0) | (u8 ? kKeyU8 : 0);
     int rc = GMPI_OK;
-    if (u8 && (rc = load_module<U8Module>(g_u8, &um)) != 0) return rc;
     if (fwd_why(p) == 0) {
         if (encode_mpi_maps(l.maps, p, kMaxBH, FwdRingWide::kColourCopyRows, fac) == 0) {
             int l2 = 0;
@@ -804,20 +756,12 @@ static int fwd_launch(Launch& l, const uint32_t* occ) {
             l.block = dim3(kStagedThreads);
             l.smem = fwd_staged_smem(fac, l.ints[2], f16, u8);
             l.arg(&l.ints[2]);
-            if (!occ) {
-                l.kernel = u8 ? um->staged[0][ac][es] : render_kernel(key | kKeyStaged | (fac ? kKeyFac : 0) | (p.transmittance ? kKeyEmit : 0));
-                return GMPI_OK;
-            }
-            if (u8) {
-                l.kernel = um->staged[1][ac][es];
-            } else {
-                const SkipModule* sm = nullptr;
-                if ((rc = load_module<SkipModule>(g_skip, &sm)) != 0) return rc;
-                l.kernel = sm->fwd[f16][ac][fac][es];
-            }
+            key |= kKeyStaged | (fac ? kKeyFac : 0) | (occ ? kKeySkip : 0) | (p.transmittance ? kKeyEmit : 0);
+            l.kernel = render_kernel(key);
+            if (!occ) return GMPI_OK;
             l.om = OccMap{occ, occ_words(p.Wt), occ_rows(p.Ht), nullptr};
             l.arg(&l.om);
-            return stage_counter(kSkipStats, u8, &l.om.skipped);
+            return stage_counter(kSkipStats, kernel_file(p, occ), &l.om.skipped);
         }
         if (g_fwd_variant.load(std::memory_order_relaxed) == 2) return fail(GMPI_ERR_CUDA, "cuTensorMapEncodeTiled failed");
     }
@@ -828,7 +772,7 @@ static int fwd_launch(Launch& l, const uint32_t* occ) {
     l.grid = dim3((p.W + kFwdTileW - 1) / kFwdTileW, (p.H + kFwdTileH - 1) / kFwdTileH, p.V);
     if (l.grid.y > 65535) return fail(GMPI_ERR_UNSUPPORTED, "image height %d too large", p.H);
     if (p.V > 65535) return fail(GMPI_ERR_UNSUPPORTED, "V=%d views exceed one launch of the direct kernel (65535); split the batch", p.V);
-    l.kernel = u8 ? um->direct[ac][es] : render_kernel(key);
+    l.kernel = render_kernel(key);
     return GMPI_OK;
 }
 
@@ -853,9 +797,9 @@ static int launch_fwd(RenderParams p, cudaStream_t st, const uint32_t* occ = nul
     if ((rc = fwd_launch(l, occ)) != 0) return rc;
     // the direct kernel walks no stages: it loads per pixel, and composites every plane (which gives a skipping call's output)
     const unsigned long long walked = (unsigned long long)l.tiles * p.N;
-    const bool u8 = (p.options & GMPI_MPI_U8) != 0;
-    if ((p.options & GMPI_EARLY_STOP) && (rc = reset_stage_stats(kEarlyStopStats, u8, walked, st)) != 0) return rc;
-    if (occ && (rc = reset_stage_stats(kSkipStats, u8, walked, st)) != 0) return rc;
+    const KernelFile file = kernel_file(p, occ);
+    if ((p.options & GMPI_EARLY_STOP) && (rc = reset_stage_stats(kEarlyStopStats, file, walked, st)) != 0) return rc;
+    if (occ && (rc = reset_stage_stats(kSkipStats, file, walked, st)) != 0) return rc;
     return launch(l, st);
 }
 
@@ -1249,9 +1193,6 @@ int gmpi_mpi_build_occupancy(const gmpi_render_desc* d, void* occ, size_t bytes)
     const int words = occ_words(p.Wt), rows = occ_rows(p.Ht);
     if (rows > 65535) return fail(GMPI_ERR_UNSUPPORTED, "Ht=%d exceeds the occupancy build's grid (%d texel rows)", p.Ht, 65535 * kOccB);
     const bool f16 = (p.options & GMPI_MPI_F16) != 0, u8 = (p.options & GMPI_MPI_U8) != 0;
-    const SkipModule* sm = nullptr;
-    const U8Module* um = nullptr;
-    if ((rc = u8 ? load_module<U8Module>(g_u8, &um) : load_module<SkipModule>(g_skip, &sm)) != 0) return rc;
     const int M = p.M, N = p.N, Ht = p.Ht, Wt = p.Wt;
     cudaLaunchConfig_t cfg = {};
     cfg.blockDim = dim3(32 * kOccB);
@@ -1265,12 +1206,12 @@ int gmpi_mpi_build_occupancy(const gmpi_render_desc* d, void* occ, size_t bytes)
         cfg.gridDim = dim3(words, rows, planes < 65535 ? planes : 65535);
         const void* rgba = p.rgba;
         void* args[] = {&rgba, &map, (void*)&planes, (void*)&Ht, (void*)&Wt, (void*)&words, (void*)&rows};
-        GMPI_CUDA_OK(cudaLaunchKernelExC(&cfg, um->occ, args));
+        GMPI_CUDA_OK(cudaLaunchKernelExC(&cfg, (const void*)gmpi_occ_expanded_u8, args));
     } else if (factored(p)) {
         cfg.gridDim = dim3(words, rows, M < 65535 ? M : 65535);
         const void *rgb = p.rgb, *bg = p.bg_rgb, *alpha = p.alpha;
         void* args[] = {&rgb, &bg, &alpha, &map, (void*)&M, (void*)&N, (void*)&Ht, (void*)&Wt, (void*)&words, (void*)&rows};
-        GMPI_CUDA_OK(cudaLaunchKernelExC(&cfg, sm->occ_fac[f16], args));
+        GMPI_CUDA_OK(cudaLaunchKernelExC(&cfg, f16 ? (const void*)gmpi_occ_factored_f16 : (const void*)gmpi_occ_factored_f32, args));
     } else {
         const long long P = (long long)M * N;
         if (P > 0x7fffffffLL) return fail(GMPI_ERR_UNSUPPORTED, "%lld planes exceed the occupancy build (2^31)", P);
@@ -1279,7 +1220,7 @@ int gmpi_mpi_build_occupancy(const gmpi_render_desc* d, void* occ, size_t bytes)
         const void* rgba = p.rgba;
         uint32_t* flags = p.flags;      // the range check's bits, from the same loads
         void* args[] = {&rgba, &map, &flags, (void*)&planes, (void*)&Ht, (void*)&Wt, (void*)&words, (void*)&rows};
-        GMPI_CUDA_OK(cudaLaunchKernelExC(&cfg, sm->occ_exp[f16], args));
+        GMPI_CUDA_OK(cudaLaunchKernelExC(&cfg, f16 ? (const void*)gmpi_occ_expanded_f16 : (const void*)gmpi_occ_expanded_f32, args));
     }
     return GMPI_OK;
 }
@@ -1316,11 +1257,9 @@ int gmpi_debug_u8_codes_host(float* out) {
 
 int gmpi_debug_u8_codes(float* out, void* stream) {
     if (!out) return fail(GMPI_ERR_INVALID_ARGUMENT, "null pointer");
-    const U8Module* um = nullptr;
-    if (int rc = load_module<U8Module>(g_u8, &um)) return rc;
     cudaLaunchConfig_t cfg = {dim3(1), dim3(256), 0, (cudaStream_t)stream, nullptr, 0};
     void* args[] = {&out};
-    GMPI_CUDA_OK(cudaLaunchKernelExC(&cfg, um->codes, args));
+    GMPI_CUDA_OK(cudaLaunchKernelExC(&cfg, (const void*)gmpi_u8_codes, args));
     return GMPI_OK;
 }
 

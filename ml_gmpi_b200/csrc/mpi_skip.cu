@@ -1,7 +1,6 @@
 // Opt-in empty-space skipping of the staged forward (gmpi_mpi_build_occupancy, gmpi_mpi_render_fwd_skip_ex): the occupancy-map
-// build and the staged forward kernels with kSkip.  Compiled into a module of its own (libgmpi_mpi_render_skip.fatbin) that
-// mpi_render.cu loads on first use, so that the main library's kernels and their machine code stay exactly as they are.
-// Kernel names are extern "C" so that the loader can look them up.  DESIGN.md section 4.1 has the exactness argument.
+// build and the staged forward kernels with kSkip, launched by mpi_render.cu (mpi_fwd_units.cuh declares them).  A translation
+// unit of its own, so that the kernels of mpi_render.cu keep their machine code.  DESIGN.md section 4.1 has the exactness argument.
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
 #include <stdint.h>
@@ -9,6 +8,7 @@
 #include "../../include/gmpi_mpi_render.h"
 #include "mpi_common.cuh"
 #include "mpi_fwd_staged.cuh"
+#include "mpi_fwd_units.cuh"
 
 namespace gmpi {
 
@@ -132,7 +132,12 @@ GMPI_FWD_SKIP_FAC(1, f32, float)
 GMPI_FWD_SKIP_FAC(0, f16, __half)
 GMPI_FWD_SKIP_FAC(1, f16, __half)
 
-// stages the last skipping launch armed empty (gmpi_debug_fwd_skip_stats)
+// stages the last skipping launch armed empty (gmpi_debug_fwd_skip_stats, through OccMap::skipped)
 __device__ unsigned long long gmpi_skip_empty_stages;
 
 }  // extern "C"
+
+cudaError_t gmpi::skip_stage_counters(unsigned long long** early_stop, unsigned long long** empty) {
+    const cudaError_t e = cudaGetSymbolAddress(reinterpret_cast<void**>(early_stop), g_early_stop_skipped);
+    return e != cudaSuccess ? e : cudaGetSymbolAddress(reinterpret_cast<void**>(empty), gmpi_skip_empty_stages);
+}

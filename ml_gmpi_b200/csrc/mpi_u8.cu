@@ -1,7 +1,7 @@
 // 8-bit RGBA MPIs (GMPI_MPI_U8, forward only): the staged forward with and without empty-space skipping, the direct forward and the
-// occupancy-map build on an expanded uint8 rgba [M,N,4,Ht,Wt] whose code b stands for b / 255 (to_f32(uint8_t), exact).  Compiled
-// into a module of its own (libgmpi_mpi_render_u8.fatbin) that mpi_render.cu loads on first use, so that the main library's and the
-// skipping module's kernels keep their machine code.  Kernel names are extern "C" so that the loader can look them up.
+// occupancy-map build on an expanded uint8 rgba [M,N,4,Ht,Wt] whose code b stands for b / 255 (to_f32(uint8_t), exact), launched
+// by mpi_render.cu (mpi_fwd_units.cuh declares them).  A translation unit of its own, so that the kernels of mpi_render.cu and
+// mpi_skip.cu keep their machine code.
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
 #include <stdint.h>
@@ -10,6 +10,7 @@
 #include "mpi_common.cuh"
 #include "mpi_fwd_staged.cuh"
 #include "mpi_fwd_direct.cuh"
+#include "mpi_fwd_units.cuh"
 
 namespace gmpi {
 
@@ -66,8 +67,12 @@ gmpi_occ_expanded_u8(const uint8_t* rgba, uint32_t* occ, int P, int Ht, int Wt, 
 // Test hook (gmpi_debug_u8_codes): out[b] = to_f32(b) for the 256 codes, the device build of the conversion.
 __global__ void gmpi_u8_codes(float* out) { out[threadIdx.x] = to_f32((uint8_t)threadIdx.x); }
 
-// stages the last skipping launch of this module armed empty (gmpi_debug_fwd_skip_stats); its early-stop launches count into this
-// module's own g_early_stop_skipped (mpi_fwd_staged.cuh)
+// stages the last skipping launch of this file's kernels armed empty (gmpi_debug_fwd_skip_stats, through OccMap::skipped)
 __device__ unsigned long long gmpi_skip_empty_stages;
 
 }  // extern "C"
+
+cudaError_t gmpi::u8_stage_counters(unsigned long long** early_stop, unsigned long long** empty) {
+    const cudaError_t e = cudaGetSymbolAddress(reinterpret_cast<void**>(early_stop), g_early_stop_skipped);
+    return e != cudaSuccess ? e : cudaGetSymbolAddress(reinterpret_cast<void**>(empty), gmpi_skip_empty_stages);
+}

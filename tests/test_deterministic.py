@@ -1,15 +1,8 @@
 """CPU-side checks of the deterministic backward (gmpi_mpi_render_bwd_deterministic_ex): the scratch-size query, the refusals
-that need no GPU, the choice of the fixed-point fraction bits k (no int64 sum can wrap), and the machine code of every kernel
-that existed before it (unchanged: the deterministic kernels are instantiations of their own).
-
-    python tests/test_deterministic.py --record-sass   # rewrites tests/golden/sass_digests.json (all but the deterministic kernels)
-"""
+that need no GPU, and the choice of the fixed-point fraction bits k (no int64 sum can wrap).  test_library_build.py checks the
+machine code of its kernels."""
 import ctypes
-import hashlib
-import json
 import os
-import re
-import subprocess
 import sys
 
 import numpy as np
@@ -22,7 +15,6 @@ if ROOT not in sys.path:
 import ml_gmpi_b200 as g  # noqa: E402
 from ml_gmpi_b200 import _lib  # noqa: E402
 
-SASS_DIGESTS = os.path.join(ROOT, "tests", "golden", "sass_digests.json")
 ERR_INVALID, ERR_UNSUPPORTED = 1, 3
 
 
@@ -140,47 +132,3 @@ def test_worst_case_sums_cannot_wrap_int64():
         if fix_bits(H, W, V, P) < 24:
             continue                                # refused by the library
         assert _worst_case_sum(H, W, V, P) < 2 ** 63, (H, W, V, P)
-
-
-# ------------------------------------------------------------------------------------------------------------------------
-# machine code of the kernels that existed before the deterministic backward
-# ------------------------------------------------------------------------------------------------------------------------
-def _nvcc_release():
-    out = subprocess.run([g._build.nvcc_path(), "--version"], capture_output=True, text=True).stdout
-    m = re.search(r"release [0-9.]+, V[0-9.]+", out)
-    return m.group(0) if m else out.strip()
-
-
-def sass_digests(path):
-    """{mangled kernel name: sha256 of its SASS instructions} of a built library (cuobjdump -sass)."""
-    txt = subprocess.run(["cuobjdump", "-sass", path], capture_output=True, text=True, check=True).stdout
-    out = {}
-    for f in re.split(r"\n\s*Function : ", txt)[1:]:
-        name, body = f.split("\n", 1)
-        lines = [l.strip() for l in body.split("\n") if re.match(r"\s+/\*[0-9a-f]{4,}\*/", l)]
-        out[name.strip()] = hashlib.sha256("\n".join(lines).encode()).hexdigest()
-    return out
-
-
-def test_sass_of_the_existing_kernels_is_unchanged():
-    """Every kernel the library had before the deterministic backward keeps its machine code, instruction for instruction (the
-    record was taken from the library without it, by the compiler release it names)."""
-    with open(SASS_DIGESTS) as f:
-        rec = json.load(f)
-    if _nvcc_release() != rec["nvcc"]:
-        pytest.skip(f"machine code recorded with nvcc {rec['nvcc']}, this is {_nvcc_release()}")
-    g.build_library()
-    ours = sass_digests(g._build.LIB_PATH)
-    changed = [n for n, h in rec["kernels"].items() if ours.get(n) != h]
-    assert not changed, changed
-    new = sorted(n for n in ours if n not in rec["kernels"])
-    assert len(new) == 8 and all("_det_" in n for n in new), new
-
-
-if __name__ == "__main__" and "--record-sass" in sys.argv:
-    g.build_library()
-    kernels = {n: h for n, h in sass_digests(g._build.LIB_PATH).items() if "_det_" not in n}
-    with open(SASS_DIGESTS, "w") as f:
-        json.dump({"nvcc": _nvcc_release(), "kernels": kernels}, f, indent=1, sort_keys=True)
-        f.write("\n")
-    print("wrote", SASS_DIGESTS)

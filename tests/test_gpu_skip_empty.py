@@ -267,6 +267,23 @@ def test_stats_random_mpi_skips_nothing_and_head_skips_the_front(staged):
     assert skipped >= total * 12 // 32, (skipped, total)
 
 
+def early_stop_stats():
+    s, t = ctypes.c_ulonglong(0), ctypes.c_ulonglong(0)
+    _lib.check(_lib.load().gmpi_debug_fwd_early_stop_stats(ctypes.byref(s), ctypes.byref(t)))
+    return s.value, t.value
+
+
+@pytest.mark.parametrize("name", ["head", "fp16"])
+def test_stats_of_skip_with_early_stop(staged, name):
+    """A skipping launch with early stop reports the early-stop stages of the kernel that ran: it walked the stages the skip stats
+    count, and armed some but not all of them without copies."""
+    _frames(CASES[name](), True, early_stop=0.05)
+    skipped, total = skip_stats()
+    assert 0 < skipped < total, (skipped, total)
+    es, es_total = early_stop_stats()
+    assert es_total == total and 0 < es < es_total, (es, es_total, total)
+
+
 def test_direct_kernel_skips_nothing():
     set_variant("direct")
     try:

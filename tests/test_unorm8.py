@@ -1,5 +1,5 @@
 """CPU checks of 8-bit RGBA MPIs (GMPI_MPI_U8): the exact conversion of all 256 codes in the host build, the option bit, the refusals
-and plan reasons that need no GPU, the Python dispatch rule, the machine code of the uint8 module (libgmpi_mpi_render_u8.fatbin),
+and plan reasons that need no GPU, the Python dispatch rule, the machine code of the uint8 kernels (mpi_u8.cu),
 and the reference's plane-image conversion recorded in tests/golden/u8_planes.npz."""
 import ctypes
 import os
@@ -145,7 +145,7 @@ def test_python_dispatch_rule(lib):
 
 
 # ------------------------------------------------------------------------------------------------------------------------
-# machine code of the uint8 module
+# machine code of the uint8 kernels
 # ------------------------------------------------------------------------------------------------------------------------
 def _functions(path):
     sass = subprocess.run(["cuobjdump", "-sass", path], capture_output=True, text=True, check=True).stdout
@@ -159,11 +159,12 @@ def _functions(path):
     return funcs, usage
 
 
-def test_u8_module_kernels_and_resources():
+def test_u8_kernels_of_the_library_and_resources():
     """8 staged kernels ([skip][align_corners][early stop]) with TMA loads and 8-bit shared-memory taps, 4 direct kernels, the map
     build and the conversion hook: at most 128 registers, no stack, no local memory, no spills."""
     g.build_library()
-    funcs, usage = _functions(g._build.U8_PATH)
+    funcs, usage = _functions(g._build.LIB_PATH)
+    funcs = {n: b for n, b in funcs.items() if re.fullmatch(r"gmpi_\w*u8\w*", n)}
     staged = sorted(n for n in funcs if re.fullmatch(r"gmpi_fwd_u8_(skip_)?a[01]_e[01]", n))
     direct = sorted(n for n in funcs if re.fullmatch(r"gmpi_fwd_direct_u8_a[01]_e[01]", n))
     assert len(staged) == 8 and len(direct) == 4, sorted(funcs)
