@@ -619,17 +619,19 @@ __device__ __forceinline__ void bwd_box_body(const RenderParams p, const TmaMaps
     }
 }
 
-template <bool kAlignCorners, bool kFactored>
+// The box backward kernels by key (KeyTraits), and the deterministic ones (kKeyDet), which take the DetAcc too.
+template <uint32_t K>
 __global__ void __launch_bounds__(kBwdThreads, 1)
 mpi_bwd_box_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps, const int tiles_x, const int tiles_y) {
-    bwd_box_body<kAlignCorners, kFactored, false>(p, maps, tiles_x, tiles_y, DetAcc{});
+    static_assert((K & ~(kKeyAC | kKeyFac)) == (kKeyBwd | kKeyStaged), "a box backward key");
+    bwd_box_body<KeyTraits<K>::kAlignCorners, KeyTraits<K>::kFactored, false>(p, maps, tiles_x, tiles_y, DetAcc{});
 }
 
-// The deterministic backward's box kernel (a kernel of its own: the default instantiations keep their machine code)
-template <bool kAlignCorners, bool kFactored>
+template <uint32_t K>
 __global__ void __launch_bounds__(kBwdThreads, 1)
 mpi_bwd_box_det_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps, const int tiles_x, const int tiles_y, const DetAcc da) {
-    bwd_box_body<kAlignCorners, kFactored, true>(p, maps, tiles_x, tiles_y, da);
+    static_assert((K & ~(kKeyAC | kKeyFac)) == (kKeyBwd | kKeyStaged | kKeyDet), "a deterministic box backward key");
+    bwd_box_body<KeyTraits<K>::kAlignCorners, KeyTraits<K>::kFactored, true>(p, maps, tiles_x, tiles_y, da);
 }
 
 }  // namespace gmpi

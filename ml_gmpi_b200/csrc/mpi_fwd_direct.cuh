@@ -3,13 +3,14 @@
 // variant is the fast path.  Shared by the library's kernels (mpi_render.cu) and the uint8 kernels (mpi_u8.cu).
 #pragma once
 #include "mpi_common.cuh"
+#include "mpi_kernel_keys.cuh"
 
 namespace gmpi {
 
 constexpr int kFwdTileW = 32;
 constexpr int kFwdTileH = 8;
 
-// kES: GMPI_EARLY_STOP, a pixel composites no further plane once |T| <= p.early_stop (mpi_fwd_direct_early_stop_kernel).
+// kES: GMPI_EARLY_STOP, a pixel composites no further plane once |T| <= p.early_stop.
 // (p by value: with a reference ptxas allocates the default kernel's registers differently.)  E: the MPI's element type.
 template <bool kAlignCorners, bool kES, class E = float>
 __device__ __forceinline__ void fwd_direct_body(const RenderParams p) {
@@ -79,6 +80,14 @@ __device__ __forceinline__ void fwd_direct_body(const RenderParams p) {
         store_pixel(p, v, img, pix, cr, cg, cb, dep);
     }
     if (flag) atomicOr(p.flags, flag);
+}
+
+// The direct forward kernels by key (KeyTraits): fp32, fp16 and uint8 MPIs, early stop.
+template <uint32_t K>
+__global__ void __launch_bounds__(kFwdTileW* kFwdTileH) mpi_fwd_direct_kernel(const RenderParams p) {
+    using T = KeyTraits<K>;
+    static_assert((K & (kKeyStaged | kKeyBwd | kKeySkip | kKeyFac | kKeyEmit)) == 0, "a direct forward key");
+    fwd_direct_body<T::kAlignCorners, T::kES, typename T::Elem>(p);
 }
 
 }  // namespace gmpi

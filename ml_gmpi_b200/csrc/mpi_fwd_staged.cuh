@@ -13,6 +13,7 @@
 #pragma once
 #include "mpi_common.cuh"
 #include "tma_utils.cuh"
+#include "mpi_kernel_keys.cuh"
 
 namespace gmpi {
 
@@ -423,7 +424,7 @@ constexpr uint32_t kAllConsumers = (1u << kConsWarps) - 1u;
 static_assert(kStages <= kStopSlots, "stop-word slots must cover the producer's lead");
 __device__ unsigned long long g_early_stop_skipped;   // test hook: stages armed without copies (gmpi_debug_fwd_early_stop_stats)
 
-// Empty-space skipping (kSkip, forward only, the kernels of mpi_skip.cu).  The occupancy map has one bit per kOccB x kOccB texel
+// Empty-space skipping (kSkip, forward only, mpi_fwd_skip_kernel).  The occupancy map has one bit per kOccB x kOccB texel
 // block of every (MPI, plane), set when a texel of the block is not empty: alpha is not +0 (bit pattern 0), or a colour value is
 // not finite.  A plane's map is `rows` block rows of `words` 32-bit words (bit b of word w: block column 32 w + b).  Compositing a
 // box whose texels are all empty adds fma(+0, finite, x) == x to every sum and leaves T alone, so the producer arms such a stage
@@ -699,9 +700,9 @@ __device__ __forceinline__ void store_tile_pixels(const RenderParams& p, int v, 
     store_pixel(p, v, img, (size_t)py * p.W + px, o[0], o[1], o[2], o[3]);
 }
 
-// Body of the staged forward kernels.  kES: early stop (mpi_fwd_early_stop_kernel; s_stop is its stop-word ring, see kStopSlots).
+// Body of the staged forward kernels.  kES: early stop (kKeyES; s_stop is its stop-word ring, see kStopSlots).
 // E: the MPI's element type (__half: GMPI_MPI_F16, the ring's boxes are fp16, each stage half the bytes).
-// kSkip: empty-space skipping against `occ` (the kernels of mpi_skip.cu; forward only).
+// kSkip: empty-space skipping against `occ` (mpi_fwd_skip_kernel; forward only).
 template <bool kAlignCorners, bool kEmitT, bool kFactored, bool kES, class E = float, bool kSkip = false>
 __device__ __forceinline__ void fwd_staged_body(const RenderParams& p, const TmaMaps& maps, const int tiles_x, const int ring_stages,
                                                 uint32_t* s_stop, OccMap occ = OccMap{}) {
@@ -928,37 +929,35 @@ __device__ __forceinline__ void fwd_staged_body(const RenderParams& p, const Tma
     }
 }
 
-template <bool kAlignCorners, bool kEmitT, bool kFactored>
+// The staged forward kernels by key (KeyTraits), without and with empty-space skipping against `occ` (two templates: the skipping
+// kernels take one more parameter).  An early-stop kernel declares its stop-word ring in kernel scope, ahead of the body's shared
+// variables, where the shared-memory offsets in its machine code come from.
+template <uint32_t K>
 __global__ void __launch_bounds__(kStagedThreads, 1)
 mpi_fwd_staged_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps, const int tiles_x, const int tiles_y,
                       const int ring_stages) {
-    fwd_staged_body<kAlignCorners, kEmitT, kFactored, false>(p, maps, tiles_x, ring_stages, nullptr);
+    using T = KeyTraits<K>;
+    static_assert((K & (kKeyStaged | kKeyBwd | kKeySkip)) == kKeyStaged, "a staged forward key without skipping");
+    if constexpr (T::kES) {
+        __shared__ uint32_t s_stop[kStopSlots];
+        fwd_staged_body<T::kAlignCorners, T::kEmitT, T::kFactored, true, typename T::Elem>(p, maps, tiles_x, ring_stages, s_stop);
+    } else {
+        fwd_staged_body<T::kAlignCorners, T::kEmitT, T::kFactored, false, typename T::Elem>(p, maps, tiles_x, ring_stages, nullptr);
+    }
 }
 
-// GMPI_EARLY_STOP: the same kernel with the per-pixel early stop (forward only: no transmittance output), a kernel of its own so
-// that the default one keeps its machine code.
-template <bool kAlignCorners, bool kFactored>
+template <uint32_t K>
 __global__ void __launch_bounds__(kStagedThreads, 1)
-mpi_fwd_early_stop_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps, const int tiles_x, const int tiles_y,
-                          const int ring_stages) {
-    __shared__ uint32_t s_stop[kStopSlots];
-    fwd_staged_body<kAlignCorners, false, kFactored, true>(p, maps, tiles_x, ring_stages, s_stop);
-}
-
-// GMPI_MPI_F16: the forward-only kernels above on an fp16 MPI (no training instantiation: the backward reads fp32).  Kernels of their
-// own, so that the fp32 ones keep their machine code.
-template <bool kAlignCorners, bool kFactored>
-__global__ void __launch_bounds__(kStagedThreads, 1)
-mpi_fwd_staged_f16_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps, const int tiles_x, const int tiles_y,
-                          const int ring_stages) {
-    fwd_staged_body<kAlignCorners, false, kFactored, false, __half>(p, maps, tiles_x, ring_stages, nullptr);
-}
-template <bool kAlignCorners, bool kFactored>
-__global__ void __launch_bounds__(kStagedThreads, 1)
-mpi_fwd_early_stop_f16_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps, const int tiles_x, const int tiles_y,
-                              const int ring_stages) {
-    __shared__ uint32_t s_stop[kStopSlots];
-    fwd_staged_body<kAlignCorners, false, kFactored, true, __half>(p, maps, tiles_x, ring_stages, s_stop);
+mpi_fwd_skip_kernel(const RenderParams p, const __grid_constant__ TmaMaps maps, const int tiles_x, const int tiles_y,
+                    const int ring_stages, const OccMap occ) {
+    using T = KeyTraits<K>;
+    static_assert((K & (kKeyStaged | kKeyBwd | kKeySkip | kKeyEmit)) == (kKeyStaged | kKeySkip), "a skipping forward key");
+    if constexpr (T::kES) {
+        __shared__ uint32_t s_stop[kStopSlots];
+        fwd_staged_body<T::kAlignCorners, false, T::kFactored, true, typename T::Elem, true>(p, maps, tiles_x, ring_stages, s_stop, occ);
+    } else {
+        fwd_staged_body<T::kAlignCorners, false, T::kFactored, false, typename T::Elem, true>(p, maps, tiles_x, ring_stages, nullptr, occ);
+    }
 }
 
 }  // namespace gmpi

@@ -9,7 +9,9 @@
 #include <stdio.h>
 #include <string.h>
 
+#include <algorithm>
 #include <atomic>
+#include <iterator>
 #include <mutex>
 
 #include "../../include/gmpi_mpi_render.h"
@@ -18,7 +20,7 @@
 #include "mpi_bwd_box.cuh"
 #include "mpi_light.cuh"
 #include "mpi_fwd_direct.cuh"
-#include "mpi_fwd_units.cuh"
+#include "mpi_kernel_keys.cuh"
 
 namespace gmpi {
 
@@ -42,34 +44,6 @@ static int fail(int code, const char* fmt, ...) {
             return fail(GMPI_ERR_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e),    \
                         __FILE__, __LINE__);                                                      \
     } while (0)
-
-// ------------------------------------------------------------------------------------------
-// Forward, direct-gather variant (fwd_direct_body, mpi_fwd_direct.cuh).
-// ------------------------------------------------------------------------------------------
-template <bool kAlignCorners>
-__global__ void __launch_bounds__(kFwdTileW* kFwdTileH)
-mpi_fwd_direct_kernel(const RenderParams p) {
-    fwd_direct_body<kAlignCorners, false>(p);
-}
-
-template <bool kAlignCorners>
-__global__ void __launch_bounds__(kFwdTileW* kFwdTileH)
-mpi_fwd_direct_early_stop_kernel(const RenderParams p) {
-    fwd_direct_body<kAlignCorners, true>(p);
-}
-
-// GMPI_MPI_F16: the direct forward kernels on an fp16 MPI (kernels of their own: the fp32 ones keep their machine code)
-template <bool kAlignCorners>
-__global__ void __launch_bounds__(kFwdTileW* kFwdTileH)
-mpi_fwd_direct_f16_kernel(const RenderParams p) {
-    fwd_direct_body<kAlignCorners, false, __half>(p);
-}
-
-template <bool kAlignCorners>
-__global__ void __launch_bounds__(kFwdTileW* kFwdTileH)
-mpi_fwd_direct_early_stop_f16_kernel(const RenderParams p) {
-    fwd_direct_body<kAlignCorners, true, __half>(p);
-}
 
 // ------------------------------------------------------------------------------------------
 // Backward, direct variant.
@@ -174,16 +148,19 @@ __device__ __forceinline__ void bwd_direct_body(const RenderParams p, const int 
     }
 }
 
-template <bool kAlignCorners>
+// The direct backward kernels by key (KeyTraits), and the deterministic ones (kKeyDet), which take the DetAcc too.
+template <uint32_t K>
 __global__ void __launch_bounds__(128)
 mpi_bwd_direct_kernel(const RenderParams p, const int tile_w, const int tile_h) {
-    bwd_direct_body<kAlignCorners, false>(p, tile_w, tile_h, DetAcc{});
+    static_assert((K & ~kKeyAC) == kKeyBwd, "a direct backward key");
+    bwd_direct_body<KeyTraits<K>::kAlignCorners, false>(p, tile_w, tile_h, DetAcc{});
 }
 
-template <bool kAlignCorners>
+template <uint32_t K>
 __global__ void __launch_bounds__(128)
 mpi_bwd_direct_det_kernel(const RenderParams p, const int tile_w, const int tile_h, const DetAcc da) {
-    bwd_direct_body<kAlignCorners, true>(p, tile_w, tile_h, da);
+    static_assert((K & ~kKeyAC) == (kKeyBwd | kKeyDet), "a deterministic direct backward key");
+    bwd_direct_body<KeyTraits<K>::kAlignCorners, true>(p, tile_w, tile_h, da);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -535,96 +512,76 @@ static int fwd_ring_stages(const RenderParams& p, int l2_bytes) {
     return shared_mpi || fits_l2 ? kStages : kStreamStages;
 }
 
-// What picks a render kernel: the bits of its variant.  kKeyStaged: a persistent TMA kernel (the staged forward, the box backward).
-// The direct forward's key has no kKeyFac and no kKeyEmit, and the direct backward's no kKeyFac: those kernels read both at run time.
-// kKeySkip: empty-space skipping (the kernels of mpi_skip.cu, or of mpi_u8.cu with kKeyU8).  kKeyU8: a uint8 MPI (mpi_u8.cu).
-enum : uint32_t {
-    kKeyAC = 1, kKeyFac = 2, kKeyEmit = 4, kKeyES = 8, kKeyF16 = 16, kKeyStaged = 32, kKeyBwd = 64, kKeyDet = 128, kKeySkip = 256,
-    kKeyU8 = 512
+// The render kernels of this file.  This table is the first reference to each kernel template here, so its order is the order the
+// kernels are instantiated in, and ptxas gives some kernels other machine code when that order changes (the expanded box
+// backward's, when the four box kernels are listed by [align_corners][factored]).  Do not reorder it: the recorded SASS digests
+// (tests/golden/sass_digests.json) check the machine code.
+static const RenderKernel kRenderKernels[] = {
+    {kKeyStaged, mpi_fwd_staged_kernel<kKeyStaged>},
+    {kKeyStaged | kKeyFac, mpi_fwd_staged_kernel<kKeyStaged | kKeyFac>},
+    {kKeyStaged | kKeyEmit, mpi_fwd_staged_kernel<kKeyStaged | kKeyEmit>},
+    {kKeyStaged | kKeyEmit | kKeyFac, mpi_fwd_staged_kernel<kKeyStaged | kKeyEmit | kKeyFac>},
+    {kKeyStaged | kKeyAC, mpi_fwd_staged_kernel<kKeyStaged | kKeyAC>},
+    {kKeyStaged | kKeyAC | kKeyFac, mpi_fwd_staged_kernel<kKeyStaged | kKeyAC | kKeyFac>},
+    {kKeyStaged | kKeyAC | kKeyEmit, mpi_fwd_staged_kernel<kKeyStaged | kKeyAC | kKeyEmit>},
+    {kKeyStaged | kKeyAC | kKeyEmit | kKeyFac, mpi_fwd_staged_kernel<kKeyStaged | kKeyAC | kKeyEmit | kKeyFac>},
+    {kKeyStaged | kKeyES, mpi_fwd_staged_kernel<kKeyStaged | kKeyES>},
+    {kKeyStaged | kKeyES | kKeyFac, mpi_fwd_staged_kernel<kKeyStaged | kKeyES | kKeyFac>},
+    {kKeyStaged | kKeyES | kKeyAC, mpi_fwd_staged_kernel<kKeyStaged | kKeyES | kKeyAC>},
+    {kKeyStaged | kKeyES | kKeyAC | kKeyFac, mpi_fwd_staged_kernel<kKeyStaged | kKeyES | kKeyAC | kKeyFac>},
+    {0, mpi_fwd_direct_kernel<0>},
+    {kKeyAC, mpi_fwd_direct_kernel<kKeyAC>},
+    {kKeyES, mpi_fwd_direct_kernel<kKeyES>},
+    {kKeyES | kKeyAC, mpi_fwd_direct_kernel<kKeyES | kKeyAC>},
+    {kKeyF16 | kKeyStaged, mpi_fwd_staged_kernel<kKeyF16 | kKeyStaged>},
+    {kKeyF16 | kKeyStaged | kKeyFac, mpi_fwd_staged_kernel<kKeyF16 | kKeyStaged | kKeyFac>},
+    {kKeyF16 | kKeyStaged | kKeyAC, mpi_fwd_staged_kernel<kKeyF16 | kKeyStaged | kKeyAC>},
+    {kKeyF16 | kKeyStaged | kKeyAC | kKeyFac, mpi_fwd_staged_kernel<kKeyF16 | kKeyStaged | kKeyAC | kKeyFac>},
+    {kKeyF16 | kKeyStaged | kKeyES, mpi_fwd_staged_kernel<kKeyF16 | kKeyStaged | kKeyES>},
+    {kKeyF16 | kKeyStaged | kKeyES | kKeyFac, mpi_fwd_staged_kernel<kKeyF16 | kKeyStaged | kKeyES | kKeyFac>},
+    {kKeyF16 | kKeyStaged | kKeyES | kKeyAC, mpi_fwd_staged_kernel<kKeyF16 | kKeyStaged | kKeyES | kKeyAC>},
+    {kKeyF16 | kKeyStaged | kKeyES | kKeyAC | kKeyFac, mpi_fwd_staged_kernel<kKeyF16 | kKeyStaged | kKeyES | kKeyAC | kKeyFac>},
+    {kKeyF16, mpi_fwd_direct_kernel<kKeyF16>},
+    {kKeyF16 | kKeyAC, mpi_fwd_direct_kernel<kKeyF16 | kKeyAC>},
+    {kKeyF16 | kKeyES, mpi_fwd_direct_kernel<kKeyF16 | kKeyES>},
+    {kKeyF16 | kKeyES | kKeyAC, mpi_fwd_direct_kernel<kKeyF16 | kKeyES | kKeyAC>},
+    {kKeyBwd | kKeyDet | kKeyAC, mpi_bwd_direct_det_kernel<kKeyBwd | kKeyDet | kKeyAC>},
+    {kKeyBwd | kKeyDet, mpi_bwd_direct_det_kernel<kKeyBwd | kKeyDet>},
+    {kKeyBwd | kKeyAC, mpi_bwd_direct_kernel<kKeyBwd | kKeyAC>},
+    {kKeyBwd, mpi_bwd_direct_kernel<kKeyBwd>},
+    {kKeyBwd | kKeyDet | kKeyStaged | kKeyAC | kKeyFac, mpi_bwd_box_det_kernel<kKeyBwd | kKeyDet | kKeyStaged | kKeyAC | kKeyFac>},
+    {kKeyBwd | kKeyDet | kKeyStaged | kKeyFac, mpi_bwd_box_det_kernel<kKeyBwd | kKeyDet | kKeyStaged | kKeyFac>},
+    {kKeyBwd | kKeyDet | kKeyStaged | kKeyAC, mpi_bwd_box_det_kernel<kKeyBwd | kKeyDet | kKeyStaged | kKeyAC>},
+    {kKeyBwd | kKeyDet | kKeyStaged, mpi_bwd_box_det_kernel<kKeyBwd | kKeyDet | kKeyStaged>},
+    {kKeyBwd | kKeyStaged | kKeyAC | kKeyFac, mpi_bwd_box_kernel<kKeyBwd | kKeyStaged | kKeyAC | kKeyFac>},
+    {kKeyBwd | kKeyStaged | kKeyFac, mpi_bwd_box_kernel<kKeyBwd | kKeyStaged | kKeyFac>},
+    {kKeyBwd | kKeyStaged | kKeyAC, mpi_bwd_box_kernel<kKeyBwd | kKeyStaged | kKeyAC>},
+    {kKeyBwd | kKeyStaged, mpi_bwd_box_kernel<kKeyBwd | kKeyStaged>},
 };
 
-// Every render kernel by its key.  This switch is the first reference to each kernel template of this file, so its cases give the
-// order the kernels are instantiated in, and ptxas gives some kernels other machine code when that order changes (the expanded box
-// backward's, when the four box kernels are listed by [align_corners][factored]).  Do not reorder the cases: the recorded SASS
-// digests (tests/golden/sass_digests.json) check the machine code.  The kernels of mpi_skip.cu and mpi_u8.cu come last.  A key
-// without a kernel gives nullptr, which the launch refuses.
+// mpi_render.cu has no skipping kernels, so no skip counter.
+static cudaError_t render_stage_counters(unsigned long long** early_stop, unsigned long long** empty) {
+    *empty = nullptr;
+    return cudaGetSymbolAddress(reinterpret_cast<void**>(early_stop), g_early_stop_skipped);
+}
+
+const KernelUnit gmpi::render_unit = {std::begin(kRenderKernels), std::end(kRenderKernels), render_stage_counters};
+
+// The translation unit that defines the kernel of `key`.
+static const KernelUnit& key_unit(uint32_t key) {
+    return (key & kKeyU8) ? u8_unit : (key & kKeySkip) ? skip_unit : render_unit;
+}
+
+// Every render kernel by its key.  A key without a kernel gives nullptr, which the launch refuses.
 static const void* render_kernel(uint32_t key) {
-    switch (key) {
-    case kKeyStaged: return (const void*)mpi_fwd_staged_kernel<false, false, false>;
-    case kKeyStaged | kKeyFac: return (const void*)mpi_fwd_staged_kernel<false, false, true>;
-    case kKeyStaged | kKeyEmit: return (const void*)mpi_fwd_staged_kernel<false, true, false>;
-    case kKeyStaged | kKeyEmit | kKeyFac: return (const void*)mpi_fwd_staged_kernel<false, true, true>;
-    case kKeyStaged | kKeyAC: return (const void*)mpi_fwd_staged_kernel<true, false, false>;
-    case kKeyStaged | kKeyAC | kKeyFac: return (const void*)mpi_fwd_staged_kernel<true, false, true>;
-    case kKeyStaged | kKeyAC | kKeyEmit: return (const void*)mpi_fwd_staged_kernel<true, true, false>;
-    case kKeyStaged | kKeyAC | kKeyEmit | kKeyFac: return (const void*)mpi_fwd_staged_kernel<true, true, true>;
-    case kKeyStaged | kKeyES: return (const void*)mpi_fwd_early_stop_kernel<false, false>;
-    case kKeyStaged | kKeyES | kKeyFac: return (const void*)mpi_fwd_early_stop_kernel<false, true>;
-    case kKeyStaged | kKeyES | kKeyAC: return (const void*)mpi_fwd_early_stop_kernel<true, false>;
-    case kKeyStaged | kKeyES | kKeyAC | kKeyFac: return (const void*)mpi_fwd_early_stop_kernel<true, true>;
-    case 0: return (const void*)mpi_fwd_direct_kernel<false>;
-    case kKeyAC: return (const void*)mpi_fwd_direct_kernel<true>;
-    case kKeyES: return (const void*)mpi_fwd_direct_early_stop_kernel<false>;
-    case kKeyES | kKeyAC: return (const void*)mpi_fwd_direct_early_stop_kernel<true>;
-    case kKeyF16 | kKeyStaged: return (const void*)mpi_fwd_staged_f16_kernel<false, false>;
-    case kKeyF16 | kKeyStaged | kKeyFac: return (const void*)mpi_fwd_staged_f16_kernel<false, true>;
-    case kKeyF16 | kKeyStaged | kKeyAC: return (const void*)mpi_fwd_staged_f16_kernel<true, false>;
-    case kKeyF16 | kKeyStaged | kKeyAC | kKeyFac: return (const void*)mpi_fwd_staged_f16_kernel<true, true>;
-    case kKeyF16 | kKeyStaged | kKeyES: return (const void*)mpi_fwd_early_stop_f16_kernel<false, false>;
-    case kKeyF16 | kKeyStaged | kKeyES | kKeyFac: return (const void*)mpi_fwd_early_stop_f16_kernel<false, true>;
-    case kKeyF16 | kKeyStaged | kKeyES | kKeyAC: return (const void*)mpi_fwd_early_stop_f16_kernel<true, false>;
-    case kKeyF16 | kKeyStaged | kKeyES | kKeyAC | kKeyFac: return (const void*)mpi_fwd_early_stop_f16_kernel<true, true>;
-    case kKeyF16: return (const void*)mpi_fwd_direct_f16_kernel<false>;
-    case kKeyF16 | kKeyAC: return (const void*)mpi_fwd_direct_f16_kernel<true>;
-    case kKeyF16 | kKeyES: return (const void*)mpi_fwd_direct_early_stop_f16_kernel<false>;
-    case kKeyF16 | kKeyES | kKeyAC: return (const void*)mpi_fwd_direct_early_stop_f16_kernel<true>;
-    case kKeyBwd | kKeyDet | kKeyAC: return (const void*)mpi_bwd_direct_det_kernel<true>;
-    case kKeyBwd | kKeyDet: return (const void*)mpi_bwd_direct_det_kernel<false>;
-    case kKeyBwd | kKeyAC: return (const void*)mpi_bwd_direct_kernel<true>;
-    case kKeyBwd: return (const void*)mpi_bwd_direct_kernel<false>;
-    case kKeyBwd | kKeyDet | kKeyStaged | kKeyAC | kKeyFac: return (const void*)mpi_bwd_box_det_kernel<true, true>;
-    case kKeyBwd | kKeyDet | kKeyStaged | kKeyFac: return (const void*)mpi_bwd_box_det_kernel<false, true>;
-    case kKeyBwd | kKeyDet | kKeyStaged | kKeyAC: return (const void*)mpi_bwd_box_det_kernel<true, false>;
-    case kKeyBwd | kKeyDet | kKeyStaged: return (const void*)mpi_bwd_box_det_kernel<false, false>;
-    case kKeyBwd | kKeyStaged | kKeyAC | kKeyFac: return (const void*)mpi_bwd_box_kernel<true, true>;
-    case kKeyBwd | kKeyStaged | kKeyFac: return (const void*)mpi_bwd_box_kernel<false, true>;
-    case kKeyBwd | kKeyStaged | kKeyAC: return (const void*)mpi_bwd_box_kernel<true, false>;
-    case kKeyBwd | kKeyStaged: return (const void*)mpi_bwd_box_kernel<false, false>;
-    case kKeySkip | kKeyStaged: return (const void*)gmpi_fwd_skip_a0_x0_e0_f32;
-    case kKeySkip | kKeyStaged | kKeyES: return (const void*)gmpi_fwd_skip_a0_x0_e1_f32;
-    case kKeySkip | kKeyStaged | kKeyFac: return (const void*)gmpi_fwd_skip_a0_x1_e0_f32;
-    case kKeySkip | kKeyStaged | kKeyFac | kKeyES: return (const void*)gmpi_fwd_skip_a0_x1_e1_f32;
-    case kKeySkip | kKeyStaged | kKeyAC: return (const void*)gmpi_fwd_skip_a1_x0_e0_f32;
-    case kKeySkip | kKeyStaged | kKeyAC | kKeyES: return (const void*)gmpi_fwd_skip_a1_x0_e1_f32;
-    case kKeySkip | kKeyStaged | kKeyAC | kKeyFac: return (const void*)gmpi_fwd_skip_a1_x1_e0_f32;
-    case kKeySkip | kKeyStaged | kKeyAC | kKeyFac | kKeyES: return (const void*)gmpi_fwd_skip_a1_x1_e1_f32;
-    case kKeySkip | kKeyStaged | kKeyF16: return (const void*)gmpi_fwd_skip_a0_x0_e0_f16;
-    case kKeySkip | kKeyStaged | kKeyF16 | kKeyES: return (const void*)gmpi_fwd_skip_a0_x0_e1_f16;
-    case kKeySkip | kKeyStaged | kKeyF16 | kKeyFac: return (const void*)gmpi_fwd_skip_a0_x1_e0_f16;
-    case kKeySkip | kKeyStaged | kKeyF16 | kKeyFac | kKeyES: return (const void*)gmpi_fwd_skip_a0_x1_e1_f16;
-    case kKeySkip | kKeyStaged | kKeyF16 | kKeyAC: return (const void*)gmpi_fwd_skip_a1_x0_e0_f16;
-    case kKeySkip | kKeyStaged | kKeyF16 | kKeyAC | kKeyES: return (const void*)gmpi_fwd_skip_a1_x0_e1_f16;
-    case kKeySkip | kKeyStaged | kKeyF16 | kKeyAC | kKeyFac: return (const void*)gmpi_fwd_skip_a1_x1_e0_f16;
-    case kKeySkip | kKeyStaged | kKeyF16 | kKeyAC | kKeyFac | kKeyES: return (const void*)gmpi_fwd_skip_a1_x1_e1_f16;
-    case kKeyU8 | kKeyStaged: return (const void*)gmpi_fwd_u8_a0_e0;
-    case kKeyU8 | kKeyStaged | kKeyES: return (const void*)gmpi_fwd_u8_a0_e1;
-    case kKeyU8 | kKeyStaged | kKeyAC: return (const void*)gmpi_fwd_u8_a1_e0;
-    case kKeyU8 | kKeyStaged | kKeyAC | kKeyES: return (const void*)gmpi_fwd_u8_a1_e1;
-    case kKeyU8 | kKeySkip | kKeyStaged: return (const void*)gmpi_fwd_u8_skip_a0_e0;
-    case kKeyU8 | kKeySkip | kKeyStaged | kKeyES: return (const void*)gmpi_fwd_u8_skip_a0_e1;
-    case kKeyU8 | kKeySkip | kKeyStaged | kKeyAC: return (const void*)gmpi_fwd_u8_skip_a1_e0;
-    case kKeyU8 | kKeySkip | kKeyStaged | kKeyAC | kKeyES: return (const void*)gmpi_fwd_u8_skip_a1_e1;
-    case kKeyU8: return (const void*)gmpi_fwd_direct_u8_a0_e0;
-    case kKeyU8 | kKeyES: return (const void*)gmpi_fwd_direct_u8_a0_e1;
-    case kKeyU8 | kKeyAC: return (const void*)gmpi_fwd_direct_u8_a1_e0;
-    case kKeyU8 | kKeyAC | kKeyES: return (const void*)gmpi_fwd_direct_u8_a1_e1;
-    }
-    return nullptr;
+    const KernelUnit& u = key_unit(key);
+    const RenderKernel* k = std::find_if(u.begin, u.end, [key](const RenderKernel& r) { return r.key == key; });
+    return k == u.end ? nullptr : k->kernel;
 }
 
 // Everything one render-kernel launch needs.  The arguments point into this object, so it is built in place and never copied.
 struct Launch {
-    const void* kernel = nullptr;    // render_kernel(key)
+    uint32_t key = 0;                // the kernel's key (render_kernel)
     dim3 grid, block;
     size_t smem = 0;
     long tiles = 0;                  // the tiles of all views a persistent kernel walks (0: a direct kernel)
@@ -645,9 +602,10 @@ struct Launch {
 };
 
 static int launch(Launch& l, cudaStream_t st) {
-    if (l.smem > 48 * 1024) GMPI_CUDA_OK(cudaFuncSetAttribute(l.kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)l.smem));
+    const void* kernel = render_kernel(l.key);
+    if (l.smem > 48 * 1024) GMPI_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)l.smem));
     cudaLaunchConfig_t cfg = {l.grid, l.block, l.smem, st, nullptr, 0};
-    GMPI_CUDA_OK(cudaLaunchKernelExC(&cfg, l.kernel, l.args));
+    GMPI_CUDA_OK(cudaLaunchKernelExC(&cfg, kernel, l.args));
     return GMPI_OK;
 }
 
@@ -678,43 +636,35 @@ static size_t fwd_staged_smem(bool fac, int stages, bool f16, bool u8) {
 
 // The stage counters of the test hooks gmpi_debug_fwd_early_stop_stats and gmpi_debug_fwd_skip_stats: on the device, the stages
 // the last early-stop or skipping launch armed without copies (zeroed on its stream); here, the (tile, plane) stages it walked and
-// which file's kernels it launched.  Each file has its own copy of g_early_stop_skipped (mpi_fwd_staged.cuh); the skipping kernels of
-// mpi_skip.cu and mpi_u8.cu count into their file's gmpi_skip_empty_stages (OccMap::skipped).
+// the unit whose kernel it launched (KernelUnit::stage_counters).  The direct kernels count no stages: their counters read 0.
 enum StageStats { kEarlyStopStats, kSkipStats };
-enum KernelFile { kRenderFile, kSkipFile, kU8File };     // mpi_render.cu, mpi_skip.cu, mpi_u8.cu
 static std::atomic<unsigned long long> g_stages_walked[2];
-static std::atomic<int> g_stages_file[2] = {{kRenderFile}, {kSkipFile}};     // before any launch too: mpi_render.cu has no skip counter
+static std::atomic<const KernelUnit*> g_stages_unit[2] = {{&render_unit}, {&render_unit}};
 
-// The file of a forward call's staged kernel.  The direct kernels count no stages, so the counters of that file read 0 after them.
-static KernelFile kernel_file(const RenderParams& p, const uint32_t* occ) {
-    return (p.options & GMPI_MPI_U8) ? kU8File : occ ? kSkipFile : kRenderFile;
-}
-
-// The device counter on the current device (mpi_render.cu has no skipping kernels, so no skip counter).
-static int stage_counter(StageStats s, KernelFile file, unsigned long long** counter) {
+// The device counter on the current device; nullptr: the unit has no such counter, which reads 0.
+static int stage_counter(StageStats s, const KernelUnit& unit, unsigned long long** counter) {
     unsigned long long* c[2] = {nullptr, nullptr};
-    if (file == kRenderFile) GMPI_CUDA_OK(cudaGetSymbolAddress(reinterpret_cast<void**>(&c[kEarlyStopStats]), g_early_stop_skipped));
-    if (file == kSkipFile) GMPI_CUDA_OK(skip_stage_counters(&c[kEarlyStopStats], &c[kSkipStats]));
-    if (file == kU8File) GMPI_CUDA_OK(u8_stage_counters(&c[kEarlyStopStats], &c[kSkipStats]));
+    GMPI_CUDA_OK(unit.stage_counters(&c[kEarlyStopStats], &c[kSkipStats]));
     *counter = c[s];
     return GMPI_OK;
 }
 
-static int reset_stage_stats(StageStats s, KernelFile file, unsigned long long walked, cudaStream_t st) {
+static int reset_stage_stats(StageStats s, const KernelUnit& unit, unsigned long long walked, cudaStream_t st) {
     unsigned long long* counter = nullptr;
-    if (int rc = stage_counter(s, file, &counter)) return rc;
-    GMPI_CUDA_OK(cudaMemsetAsync(counter, 0, sizeof(unsigned long long), st));
+    if (int rc = stage_counter(s, unit, &counter)) return rc;
+    if (counter) GMPI_CUDA_OK(cudaMemsetAsync(counter, 0, sizeof(unsigned long long), st));
     g_stages_walked[s].store(walked, std::memory_order_relaxed);
-    g_stages_file[s].store(file, std::memory_order_relaxed);
+    g_stages_unit[s].store(&unit, std::memory_order_relaxed);
     return GMPI_OK;
 }
 
 static int read_stage_stats(StageStats s, unsigned long long* skipped, unsigned long long* walked) {
     if (!skipped || !walked) return fail(GMPI_ERR_INVALID_ARGUMENT, "null pointer");
     unsigned long long* counter = nullptr;
-    if (int rc = stage_counter(s, (KernelFile)g_stages_file[s].load(std::memory_order_relaxed), &counter)) return rc;
+    if (int rc = stage_counter(s, *g_stages_unit[s].load(std::memory_order_relaxed), &counter)) return rc;
     GMPI_CUDA_OK(cudaDeviceSynchronize());
-    GMPI_CUDA_OK(cudaMemcpy(skipped, counter, sizeof(unsigned long long), cudaMemcpyDeviceToHost));
+    *skipped = 0;
+    if (counter) GMPI_CUDA_OK(cudaMemcpy(skipped, counter, sizeof(unsigned long long), cudaMemcpyDeviceToHost));
     *walked = g_stages_walked[s].load(std::memory_order_relaxed);
     return GMPI_OK;
 }
@@ -757,11 +707,11 @@ static int fwd_launch(Launch& l, const uint32_t* occ) {
             l.smem = fwd_staged_smem(fac, l.ints[2], f16, u8);
             l.arg(&l.ints[2]);
             key |= kKeyStaged | (fac ? kKeyFac : 0) | (occ ? kKeySkip : 0) | (p.transmittance ? kKeyEmit : 0);
-            l.kernel = render_kernel(key);
+            l.key = key;
             if (!occ) return GMPI_OK;
             l.om = OccMap{occ, occ_words(p.Wt), occ_rows(p.Ht), nullptr};
             l.arg(&l.om);
-            return stage_counter(kSkipStats, kernel_file(p, occ), &l.om.skipped);
+            return stage_counter(kSkipStats, key_unit(key), &l.om.skipped);
         }
         if (g_fwd_variant.load(std::memory_order_relaxed) == 2) return fail(GMPI_ERR_CUDA, "cuTensorMapEncodeTiled failed");
     }
@@ -772,7 +722,7 @@ static int fwd_launch(Launch& l, const uint32_t* occ) {
     l.grid = dim3((p.W + kFwdTileW - 1) / kFwdTileW, (p.H + kFwdTileH - 1) / kFwdTileH, p.V);
     if (l.grid.y > 65535) return fail(GMPI_ERR_UNSUPPORTED, "image height %d too large", p.H);
     if (p.V > 65535) return fail(GMPI_ERR_UNSUPPORTED, "V=%d views exceed one launch of the direct kernel (65535); split the batch", p.V);
-    l.kernel = render_kernel(key);
+    l.key = key;
     return GMPI_OK;
 }
 
@@ -797,9 +747,9 @@ static int launch_fwd(RenderParams p, cudaStream_t st, const uint32_t* occ = nul
     if ((rc = fwd_launch(l, occ)) != 0) return rc;
     // the direct kernel walks no stages: it loads per pixel, and composites every plane (which gives a skipping call's output)
     const unsigned long long walked = (unsigned long long)l.tiles * p.N;
-    const KernelFile file = kernel_file(p, occ);
-    if ((p.options & GMPI_EARLY_STOP) && (rc = reset_stage_stats(kEarlyStopStats, file, walked, st)) != 0) return rc;
-    if (occ && (rc = reset_stage_stats(kSkipStats, file, walked, st)) != 0) return rc;
+    const KernelUnit& unit = key_unit(l.key);
+    if ((p.options & GMPI_EARLY_STOP) && (rc = reset_stage_stats(kEarlyStopStats, unit, walked, st)) != 0) return rc;
+    if (occ && (rc = reset_stage_stats(kSkipStats, unit, walked, st)) != 0) return rc;
     return launch(l, st);
 }
 
@@ -856,7 +806,7 @@ static int bwd_launch(Launch& l, bool box, bool det) {
         l.arg(&l.ints[1]);
     }
     if (det) l.arg(&l.da);
-    l.kernel = render_kernel(key);
+    l.key = key;
     return GMPI_OK;
 }
 

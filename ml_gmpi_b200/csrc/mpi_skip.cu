@@ -1,14 +1,16 @@
 // Opt-in empty-space skipping of the staged forward (gmpi_mpi_build_occupancy, gmpi_mpi_render_fwd_skip_ex): the occupancy-map
-// build and the staged forward kernels with kSkip, launched by mpi_render.cu (mpi_fwd_units.cuh declares them).  A translation
-// unit of its own, so that the kernels of mpi_render.cu keep their machine code.  DESIGN.md section 4.1 has the exactness argument.
+// builds and the fp32 and fp16 staged forward kernels with kKeySkip, launched by mpi_render.cu (skip_unit, mpi_kernel_keys.cuh).  A
+// translation unit of its own, so that the kernels of mpi_render.cu keep their machine code.  DESIGN.md section 4.1 has the exactness argument.
 #include <cuda_runtime.h>
 #include <cuda_fp16.h>
 #include <stdint.h>
 
+#include <iterator>
+
 #include "../../include/gmpi_mpi_render.h"
 #include "mpi_common.cuh"
 #include "mpi_fwd_staged.cuh"
-#include "mpi_fwd_units.cuh"
+#include "mpi_kernel_keys.cuh"
 
 namespace gmpi {
 
@@ -87,12 +89,6 @@ __device__ __forceinline__ void occ_factored(const U* __restrict__ rgb, const U*
     }
 }
 
-template <bool kAlignCorners, bool kFactored, bool kES, class E>
-__device__ __forceinline__ void fwd_skip(const RenderParams& p, const TmaMaps& maps, int tiles_x, int ring_stages, const OccMap& occ) {
-    __shared__ uint32_t s_stop[kStopSlots];
-    fwd_staged_body<kAlignCorners, false, kFactored, kES, E, true>(p, maps, tiles_x, ring_stages, kES ? s_stop : nullptr, occ);
-}
-
 }  // namespace gmpi
 
 using namespace gmpi;
@@ -118,26 +114,34 @@ gmpi_occ_factored_f16(const uint16_t* rgb, const uint16_t* bg, const uint16_t* a
     occ_factored<uint16_t>(rgb, bg, alpha, occ, M, N, Ht, Wt, words, rows);
 }
 
-// The staged forward with skipping: gmpi_fwd_skip_a{align_corners}_x{factored}_e{early stop}_{f32|f16} (forward only, no kEmitT).
-#define GMPI_FWD_SKIP(AC, FAC, ES, TAG, E)                                                                                        \
-    __global__ void __launch_bounds__(kStagedThreads, 1)                                                                          \
-    gmpi_fwd_skip_a##AC##_x##FAC##_e##ES##_##TAG(const RenderParams p, const __grid_constant__ TmaMaps maps, const int tiles_x,   \
-                                                 const int tiles_y, const int ring_stages, const OccMap occ) {                    \
-        fwd_skip<AC, FAC, ES, E>(p, maps, tiles_x, ring_stages, occ);                                                             \
-    }
-#define GMPI_FWD_SKIP_ES(AC, FAC, TAG, E) GMPI_FWD_SKIP(AC, FAC, 0, TAG, E) GMPI_FWD_SKIP(AC, FAC, 1, TAG, E)
-#define GMPI_FWD_SKIP_FAC(AC, TAG, E) GMPI_FWD_SKIP_ES(AC, 0, TAG, E) GMPI_FWD_SKIP_ES(AC, 1, TAG, E)
-GMPI_FWD_SKIP_FAC(0, f32, float)
-GMPI_FWD_SKIP_FAC(1, f32, float)
-GMPI_FWD_SKIP_FAC(0, f16, __half)
-GMPI_FWD_SKIP_FAC(1, f16, __half)
-
 // stages the last skipping launch armed empty (gmpi_debug_fwd_skip_stats, through OccMap::skipped)
 __device__ unsigned long long gmpi_skip_empty_stages;
 
 }  // extern "C"
 
-cudaError_t gmpi::skip_stage_counters(unsigned long long** early_stop, unsigned long long** empty) {
+// The render kernels of this file, in the order they were first defined here (the order of instantiation can change machine code).
+static const RenderKernel kSkipKernels[] = {
+    {kKeySkip | kKeyStaged, mpi_fwd_skip_kernel<kKeySkip | kKeyStaged>},
+    {kKeySkip | kKeyStaged | kKeyES, mpi_fwd_skip_kernel<kKeySkip | kKeyStaged | kKeyES>},
+    {kKeySkip | kKeyStaged | kKeyFac, mpi_fwd_skip_kernel<kKeySkip | kKeyStaged | kKeyFac>},
+    {kKeySkip | kKeyStaged | kKeyFac | kKeyES, mpi_fwd_skip_kernel<kKeySkip | kKeyStaged | kKeyFac | kKeyES>},
+    {kKeySkip | kKeyStaged | kKeyAC, mpi_fwd_skip_kernel<kKeySkip | kKeyStaged | kKeyAC>},
+    {kKeySkip | kKeyStaged | kKeyAC | kKeyES, mpi_fwd_skip_kernel<kKeySkip | kKeyStaged | kKeyAC | kKeyES>},
+    {kKeySkip | kKeyStaged | kKeyAC | kKeyFac, mpi_fwd_skip_kernel<kKeySkip | kKeyStaged | kKeyAC | kKeyFac>},
+    {kKeySkip | kKeyStaged | kKeyAC | kKeyFac | kKeyES, mpi_fwd_skip_kernel<kKeySkip | kKeyStaged | kKeyAC | kKeyFac | kKeyES>},
+    {kKeySkip | kKeyStaged | kKeyF16, mpi_fwd_skip_kernel<kKeySkip | kKeyStaged | kKeyF16>},
+    {kKeySkip | kKeyStaged | kKeyF16 | kKeyES, mpi_fwd_skip_kernel<kKeySkip | kKeyStaged | kKeyF16 | kKeyES>},
+    {kKeySkip | kKeyStaged | kKeyF16 | kKeyFac, mpi_fwd_skip_kernel<kKeySkip | kKeyStaged | kKeyF16 | kKeyFac>},
+    {kKeySkip | kKeyStaged | kKeyF16 | kKeyFac | kKeyES, mpi_fwd_skip_kernel<kKeySkip | kKeyStaged | kKeyF16 | kKeyFac | kKeyES>},
+    {kKeySkip | kKeyStaged | kKeyF16 | kKeyAC, mpi_fwd_skip_kernel<kKeySkip | kKeyStaged | kKeyF16 | kKeyAC>},
+    {kKeySkip | kKeyStaged | kKeyF16 | kKeyAC | kKeyES, mpi_fwd_skip_kernel<kKeySkip | kKeyStaged | kKeyF16 | kKeyAC | kKeyES>},
+    {kKeySkip | kKeyStaged | kKeyF16 | kKeyAC | kKeyFac, mpi_fwd_skip_kernel<kKeySkip | kKeyStaged | kKeyF16 | kKeyAC | kKeyFac>},
+    {kKeySkip | kKeyStaged | kKeyF16 | kKeyAC | kKeyFac | kKeyES, mpi_fwd_skip_kernel<kKeySkip | kKeyStaged | kKeyF16 | kKeyAC | kKeyFac | kKeyES>},
+};
+
+static cudaError_t skip_stage_counters(unsigned long long** early_stop, unsigned long long** empty) {
     const cudaError_t e = cudaGetSymbolAddress(reinterpret_cast<void**>(early_stop), g_early_stop_skipped);
     return e != cudaSuccess ? e : cudaGetSymbolAddress(reinterpret_cast<void**>(empty), gmpi_skip_empty_stages);
 }
+
+const KernelUnit gmpi::skip_unit = {std::begin(kSkipKernels), std::end(kSkipKernels), skip_stage_counters};

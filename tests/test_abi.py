@@ -173,30 +173,28 @@ def test_descriptor_entry_points_validate_without_gpu(lib):
     assert lib.gmpi_mpi_render_fwd_ex(ctypes.byref(d)) == 1 and b"view_group" in lib.gmpi_last_error()
 
 
-def test_sass_of_the_hot_kernels_is_tma_mbarrier_packed_math():
+def test_sass_of_the_hot_kernel_keys_is_tma_mbarrier_packed_math():
     """The shipped library's staged kernels are what DESIGN.md says they are (checked on the machine code, no GPU needed):
     TMA tensor loads + mbarrier transactions + the pixel-pair arithmetic as scalar FFMA in the forward (sm_90 has no packed
     fp32 instructions), additionally native integer shared atomics
     and vector global reductions in the backward; no local-memory spills in the expanded instantiations."""
     import re
-    import subprocess
+    from test_library_build import KEY_AC, KEY_BWD, KEY_ES, KEY_F16, KEY_FAC, KEY_STAGED, KEY_U8, library_kernels, render_kernels
     g.build_library()
-    txt = subprocess.run(["cuobjdump", "-sass", g._build.LIB_PATH], capture_output=True, text=True).stdout
-    funcs = {}
-    for f in re.split(r"\n\s*Function : ", txt)[1:]:
-        name, body = f.split("\n", 1)
-        funcs[name] = body
-    fwd = [b for n, b in funcs.items() if "mpi_fwd_staged_kernel" in n]
-    bwd = [b for n, b in funcs.items() if "mpi_bwd_box_kernel" in n]
+    kernels = library_kernels()
+    fwd = render_kernels(kernels, "mpi_fwd_staged_kernel", lacks=KEY_ES | KEY_F16 | KEY_U8)
+    bwd = render_kernels(kernels, "mpi_bwd_box_kernel")
     assert len(fwd) == 8 and len(bwd) == 4                       # align_corners x training x factored; align_corners x factored
-    for n, b in ((n, b) for n, b in funcs.items() if "mpi_fwd_staged_kernel" in n):
+    for n, k in fwd.items():
+        b = k.sass
         assert "UTMALDG" in b and "SYNCS.PHASECHK.TRANS64.TRYWAIT" in b and "SYNCS.ARRIVE.TRANS64" in b
         # 2 pairs x 16 taps x 2 loads per tap pair, for each box width: two in the factored ring, five in the expanded one
-        widths = 2 if re.search(r"mpi_fwd_staged_kernelILb[01]ELb[01]ELb1E", n) else 5
+        widths = 2 if k.key & KEY_FAC else 5
         assert len(re.findall(r"\bFFMA\b", b)) > 200 and b.count("LDS") >= 64 * widths and "STG.E.128" in b, n
-    for b in bwd:
+    for k in bwd.values():
+        b = k.sass
         assert "UTMALDG" in b and b.count("ATOMS.ADD") >= 256 and "REDG.E.ADD.F32x4" in b and "ATOMS.CAST" not in b
-    expanded_ac = {n: b for n, b in funcs.items() if "mpi_fwd_staged_kernelILb1ELb0ELb0" in n or "mpi_bwd_box_kernelILb1ELb0E" in n}
+    expanded_ac = {n: k.sass for n, k in {**fwd, **bwd}.items() if k.key in (KEY_STAGED | KEY_AC, KEY_BWD | KEY_STAGED | KEY_AC)}
     assert len(expanded_ac) == 2
     for n, b in expanded_ac.items():                             # the two instantiations the headline bench runs
         local = b.count(" STL") + b.count(" LDL")

@@ -1,7 +1,7 @@
 """The factored MPI (shared colour rgb [M,3,Ht,Wt], optional bg_rgb for the last plane, per-plane alpha [M,N,1,Ht,Wt]) against the
 oracle on the expanded stack, on the direct kernels and on the TMA-staged forward + box backward (run on an H100: pytest -m gpu).
 
-The factored kernels are template instantiations of their own (mpi_fwd_staged_kernel<*,*,true>, mpi_bwd_box_kernel<*,true>) with
+The factored kernels are template instantiations of their own (mpi_fwd_staged_kernel<kKeyFac | ...>, mpi_bwd_box_kernel<kKeyFac | ...>) with
 their own ring and box layout, so every edge the expanded kernels are tested at is repeated here: align_corners=False, non-square
 textures, partial tiles, N = 1 and N = 512, footprints 89..96 texels wide (they fit the factored forward's 96-wide box but take the
 generic body, as in the expanded ring) and wider than 96, non-pinhole and degenerate rays, MPIs without views, views in any order, GMPI_ZERO_GRAD, view_group, unaligned

@@ -27,7 +27,7 @@ B. Saved transmittance [V,N,H,W] against float64.  T64_i = prod_{j<i} (1 - a_j),
    |a - a64| keeps it >= -2^-20.  T is written into a sentinel-filled allocation: every element must be written and the slack
    around it untouched.  test_transmittance_bars_fail_on_wrong_problems shows the bound fails by >= 10x on two wrong problems.
 
-C. The training instantiations (mpi_fwd_staged_kernel<*, true, *>, the direct kernel with transmittance set) differ from the
+C. The training instantiations (mpi_fwd_staged_kernel<kKeyEmit | ...>, the direct kernel with transmittance set) differ from the
    inference ones only by the T stores, so their colour, depth and flags must be the inference kernel's bit for bit, through the
    descriptor and through the classic gmpi_mpi_render_fwd_train.
 

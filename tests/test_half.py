@@ -3,7 +3,6 @@ rule, and the machine code of the fp16 staged kernels."""
 import ctypes
 import os
 import re
-import subprocess
 
 import pytest
 import torch
@@ -12,6 +11,7 @@ import ml_gmpi_b200 as g
 from ml_gmpi_b200 import _lib
 from ml_gmpi_b200.mpi import _half_mpi
 from conftest import ROOT
+from test_library_build import KEY_F16, library_kernels, render_kernels
 
 UNSUPPORTED = 3
 
@@ -102,25 +102,18 @@ def test_python_dispatch_rule(lib):
     assert got is not None and got[0].is_contiguous() and got[0].dtype == torch.float16
 
 
-def test_sass_of_the_fp16_staged_kernels():
+def test_sass_of_the_fp16_staged_kernel_keys():
     """The fp16 staged kernels are TMA + mbarrier kernels like the fp32 ones: 128 registers, no local memory, their taps are
     16-bit shared loads converted to fp32 (checked on the machine code, no GPU needed)."""
     g.build_library()
-    sass = subprocess.run(["cuobjdump", "-sass", g._build.LIB_PATH], capture_output=True, text=True).stdout
-    funcs = {}
-    for f in re.split(r"\n\s*Function : ", sass)[1:]:
-        name, body = f.split("\n", 1)
-        funcs[name.strip()] = body
-    res = subprocess.run(["cuobjdump", "-res-usage", g._build.LIB_PATH], capture_output=True, text=True).stdout
-    usage = dict(re.findall(r"Function (\S+):\s*\n\s*(REG:\d+ STACK:\d+ SHARED:\d+ LOCAL:\d+)", res))
-    kernels = [n for n in funcs if re.search(r"mpi_fwd_(staged|early_stop)_f16_kernel", n)]
-    assert len(kernels) == 8, kernels                  # [early stop][align_corners][factored]; no training instantiation
-    for n in kernels:
-        b = funcs[n]
+    funcs = library_kernels()
+    kernels = render_kernels(funcs, "mpi_fwd_staged_kernel", has=KEY_F16)
+    assert len(kernels) == 8, sorted(kernels)          # [early stop][align_corners][factored]; no training instantiation
+    for n, k in kernels.items():
+        b = k.sass
         assert "UTMALDG" in b and "SYNCS.PHASECHK.TRANS64.TRYWAIT" in b and "SYNCS.ARRIVE.TRANS64" in b, n
         assert "LDS.U16" in b and len(re.findall(r"\bFFMA\b", b)) > 200, n
         assert " STL" not in b and " LDL" not in b, n
-        u = usage[n]
-        assert "REG:128 " in u and "STACK:0 " in u and "LOCAL:0" in u, (n, u)
-    assert len([n for n in funcs if re.search(r"mpi_fwd_direct(_early_stop)?_f16_kernel", n)]) == 4
-    assert any("mpi_check_range_f16_kernel" in n for n in funcs)
+        assert (k.regs, k.stack, k.local) == (128, 0, 0), (n, k.regs, k.stack, k.local)
+    assert len(render_kernels(funcs, "mpi_fwd_direct_kernel", has=KEY_F16)) == 4
+    assert any(k.template == "mpi_check_range_f16_kernel" for k in funcs.values())

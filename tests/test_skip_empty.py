@@ -3,8 +3,6 @@ map-size query, the refusals that need no GPU, the producer's box-versus-map tes
 resources of the skipping kernels (mpi_skip.cu: 128 registers, no spills).  test_library_build.py checks their machine code."""
 import ctypes
 import os
-import re
-import subprocess
 import sys
 
 import numpy as np
@@ -16,6 +14,7 @@ if ROOT not in sys.path:
 
 import ml_gmpi_b200 as g  # noqa: E402
 from ml_gmpi_b200 import _lib  # noqa: E402
+from test_library_build import KEY_U8, library_kernels, render_kernels  # noqa: E402
 
 ERR_INVALID, ERR_UNSUPPORTED = 1, 3
 B = 8
@@ -162,17 +161,11 @@ def test_box_test_refuses_bad_arguments(lib):
 # ------------------------------------------------------------------------------------------------------------------------
 # resources of the skipping kernels
 # ------------------------------------------------------------------------------------------------------------------------
-def _resources(path):
-    """{kernel: (registers, stack bytes, local bytes)} of a built library (cuobjdump -res-usage)."""
-    txt = subprocess.run(["cuobjdump", "-res-usage", path], capture_output=True, text=True, check=True).stdout
-    return {m.group(1): (int(m.group(2)), int(m.group(3)), int(m.group(4)))
-            for m in re.finditer(r"Function (\S+):\s*\n\s*REG:(\d+) STACK:(\d+) SHARED:\d+ LOCAL:(\d+)", txt)}
-
-
-def test_skip_kernels_of_the_library_use_128_registers_without_spills():
+def test_skip_kernel_keys_of_the_library_use_128_registers_without_spills():
     g.build_library()
-    res = _resources(g._build.LIB_PATH)
-    fwd = {n: r for n, r in res.items() if n.startswith("gmpi_fwd_skip_")}
+    kernels = library_kernels()
+    res = {n: (k.regs, k.stack, k.local) for n, k in kernels.items()}
+    fwd = {n: res[n] for n in render_kernels(kernels, "mpi_fwd_skip_kernel", lacks=KEY_U8)}
     occ = {n: r for n, r in res.items() if n.startswith("gmpi_occ_") and not n.endswith("_u8")}
     assert len(fwd) == 16 and set(occ) == {
         "gmpi_occ_expanded_f32", "gmpi_occ_expanded_f16", "gmpi_occ_factored_f32", "gmpi_occ_factored_f16"}, sorted(res)

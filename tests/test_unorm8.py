@@ -4,7 +4,6 @@ and the reference's plane-image conversion recorded in tests/golden/u8_planes.np
 import ctypes
 import os
 import re
-import subprocess
 
 import numpy as np
 import pytest
@@ -14,6 +13,7 @@ import ml_gmpi_b200 as g
 from ml_gmpi_b200 import _lib
 from ml_gmpi_b200.mpi import _check_unorm8, _unorm8_mpi
 from conftest import ROOT
+from test_library_build import KEY_AC, KEY_U8, library_kernels, render_kernels
 
 INVALID, UNSUPPORTED = 1, 3
 U8 = 128
@@ -147,36 +147,24 @@ def test_python_dispatch_rule(lib):
 # ------------------------------------------------------------------------------------------------------------------------
 # machine code of the uint8 kernels
 # ------------------------------------------------------------------------------------------------------------------------
-def _functions(path):
-    sass = subprocess.run(["cuobjdump", "-sass", path], capture_output=True, text=True, check=True).stdout
-    funcs = {}
-    for f in re.split(r"\n\s*Function : ", sass)[1:]:
-        name, body = f.split("\n", 1)
-        funcs[name.strip()] = body
-    res = subprocess.run(["cuobjdump", "-res-usage", path], capture_output=True, text=True, check=True).stdout
-    usage = {m.group(1): (int(m.group(2)), int(m.group(3)), int(m.group(4)))
-             for m in re.finditer(r"Function (\S+):\s*\n\s*REG:(\d+) STACK:(\d+) SHARED:\d+ LOCAL:(\d+)", res)}
-    return funcs, usage
-
-
-def test_u8_kernels_of_the_library_and_resources():
+def test_u8_kernel_keys_of_the_library_and_resources():
     """8 staged kernels ([skip][align_corners][early stop]) with TMA loads and 8-bit shared-memory taps, 4 direct kernels, the map
     build and the conversion hook: at most 128 registers, no stack, no local memory, no spills."""
     g.build_library()
-    funcs, usage = _functions(g._build.LIB_PATH)
-    funcs = {n: b for n, b in funcs.items() if re.fullmatch(r"gmpi_\w*u8\w*", n)}
-    staged = sorted(n for n in funcs if re.fullmatch(r"gmpi_fwd_u8_(skip_)?a[01]_e[01]", n))
-    direct = sorted(n for n in funcs if re.fullmatch(r"gmpi_fwd_direct_u8_a[01]_e[01]", n))
+    funcs = {n: k for n, k in library_kernels().items() if (k.key or 0) & KEY_U8 or "u8" in k.template}
+    staged = {**render_kernels(funcs, "mpi_fwd_staged_kernel"), **render_kernels(funcs, "mpi_fwd_skip_kernel")}
+    direct = render_kernels(funcs, "mpi_fwd_direct_kernel")
     assert len(staged) == 8 and len(direct) == 4, sorted(funcs)
-    assert set(funcs) == set(staged) | set(direct) | {"gmpi_occ_expanded_u8", "gmpi_u8_codes"}, sorted(funcs)
-    for n in staged:
-        b = funcs[n]
+    assert {funcs[n].template for n in set(funcs) - set(staged) - set(direct)} == {"gmpi_occ_expanded_u8", "gmpi_u8_codes"}, sorted(funcs)
+    for n, k in staged.items():
+        b = k.sass
         assert "UTMALDG" in b and "SYNCS.PHASECHK.TRANS64.TRYWAIT" in b and "LDS.U8" in b, n
         assert " STL" not in b and " LDL" not in b, n
-        assert usage[n] == (128, 0, 0), (n, usage[n])
-    for n in funcs:
-        assert usage[n][0] <= 128 and usage[n][1:] == (0, 0), (n, usage[n])
-    assert "LDG.E.U8" in funcs["gmpi_fwd_direct_u8_a1_e0"] or "LDG.E.U8.CONSTANT" in funcs["gmpi_fwd_direct_u8_a1_e0"]
+        assert (k.regs, k.stack, k.local) == (128, 0, 0), (n, k.regs, k.stack, k.local)
+    for n, k in funcs.items():
+        assert k.regs <= 128 and (k.stack, k.local) == (0, 0), (n, k.regs, k.stack, k.local)
+    b = next(k.sass for k in direct.values() if k.key == KEY_U8 | KEY_AC)
+    assert "LDG.E.U8" in b or "LDG.E.U8.CONSTANT" in b
 
 
 # ------------------------------------------------------------------------------------------------------------------------
