@@ -246,9 +246,11 @@ typedef struct gmpi_render_desc {
  * An fp16 value converts to fp32 exactly and the kernels convert each texel tap before the unchanged fp32 arithmetic, so the output
  * is bitwise equal to the same call on the fp32 upcast of the MPI (on the same kernel variant and ring depth), at half the MPI bytes
  * read from HBM -- and, through gmpi_mpi_render_host_ex, uploaded.  The staged kernels need Wt % 8 == 0 and 16-byte aligned MPI
- * bases (gmpi_mpi_render_fwd_plan_ex); other shapes take the direct kernels.  Accepted by gmpi_mpi_render_fwd_ex and
- * gmpi_mpi_render_host_ex only: a descriptor that also sets transmittance, gmpi_mpi_render_bwd_ex and every classic entry point
- * return GMPI_ERR_UNSUPPORTED.
+ * bases (gmpi_mpi_render_fwd_plan_ex); other shapes take the direct kernels.  Accepted by gmpi_mpi_render_fwd_ex,
+ * gmpi_mpi_render_fwd_skip_ex, gmpi_mpi_render_host_ex, gmpi_mpi_render_fwd_plan_ex, gmpi_mpi_occupancy_bytes and
+ * gmpi_mpi_build_occupancy.  GMPI_ERR_UNSUPPORTED for a descriptor that sets transmittance, the backward calls and every classic
+ * entry point.  The deterministic scratch query does not refuse the bit (nor GMPI_EARLY_STOP): it returns the size, and the
+ * deterministic backward refuses the call.
  *
  * GMPI_MPI_U8 (off by default): rgba is uint8 [M,N,4,Ht,Wt] (the planar layout of RGBA8 plane images after the reference's permute,
  * mpi_utils.py:336-337); the descriptor's rgba pointer is read as a pointer to bytes and code b stands for b / 255 rounded to nearest

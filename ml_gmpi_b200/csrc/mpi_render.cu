@@ -392,12 +392,6 @@ static std::atomic<int> g_fwd_stages{0};    // expanded staged forward's ring de
 // An MPI is factored (rgb + alpha [+ bg_rgb]) or expanded (rgba).
 static bool factored(const RenderParams& p) { return p.alpha != nullptr; }
 
-static int check_mpi_form(const RenderParams& p) {
-    if (factored(p) ? !p.rgb || p.rgba : !p.rgba || p.rgb)
-        return fail(GMPI_ERR_INVALID_ARGUMENT, "null input pointer (MPI: pass rgba, or rgb + alpha)");
-    return GMPI_OK;
-}
-
 // The sizes of the MPIs, and with `views` those of the views too.  `texels`: the texels of one channel must also stay below 2^31.
 static int check_sizes(const RenderParams& p, bool views, bool texels) {
     if (views && (p.M < 1 || p.V < 0 || p.N < 1 || p.Ht < 1 || p.Wt < 1 || p.H < 1 || p.W < 1))
@@ -409,38 +403,82 @@ static int check_sizes(const RenderParams& p, bool views, bool texels) {
     return GMPI_OK;
 }
 
-// GMPI_MPI_U8: an expanded MPI, not fp16 as well.  `bwd`: a backward call, which reads and writes fp32 MPIs.
-static int check_u8(const RenderParams& p, bool bwd) {
-    if (!(p.options & GMPI_MPI_U8)) return GMPI_OK;
-    if (p.options & GMPI_MPI_F16) return fail(GMPI_ERR_INVALID_ARGUMENT, "GMPI_MPI_U8 and GMPI_MPI_F16 are exclusive");
-    if (bwd) return fail(GMPI_ERR_UNSUPPORTED, "GMPI_MPI_U8 is forward-only: the backward reads and writes fp32 MPIs");
-    if (p.rgb || p.alpha || p.bg_rgb) return fail(GMPI_ERR_UNSUPPORTED, "GMPI_MPI_U8 takes an expanded MPI (rgba), not a factored one");
-    if (p.transmittance)
-        return fail(GMPI_ERR_UNSUPPORTED, "GMPI_MPI_U8 cannot be combined with the training forward (transmittance)");
+// The forward-only options.  A backward call refuses them, and so does a forward that saves the transmittance for one (the
+// training forward).  Those refusals come from this table, in its order; `why`: why the backward cannot take the option.
+struct ForwardOnly { uint32_t bit; const char *name, *why; };
+static const ForwardOnly kForwardOnly[] = {
+    {GMPI_MPI_F16, "GMPI_MPI_F16", "the backward reads and writes fp32 MPIs"},
+    {GMPI_MPI_U8, "GMPI_MPI_U8", "the backward reads and writes fp32 MPIs"},
+    {GMPI_EARLY_STOP, "GMPI_EARLY_STOP", "the backward needs every plane's samples"},
+};
+
+// The calls check_call knows.  A classic entry point fills a descriptor and is checked as the call it corresponds to.
+enum CallKind {
+    kFwdCall,         // gmpi_mpi_render_fwd_ex; the classic fwd, fwd_train and fwd_gather
+    kSkipCall,        // gmpi_mpi_render_fwd_skip_ex
+    kHostCall,        // gmpi_mpi_render_host_ex (host buffers); the classic fwd_host
+    kBwdCall,         // gmpi_mpi_render_bwd_ex and gmpi_mpi_render_bwd_deterministic_ex; the classic bwd and bwd_saved
+    kOccQueryCall,    // gmpi_mpi_occupancy_bytes
+    kOccBuildCall,    // gmpi_mpi_build_occupancy
+    kScratchCall,     // gmpi_mpi_render_bwd_deterministic_scratch_bytes
+};
+
+struct Call {
+    CallKind kind;
+    bool classic = false;                     // from a classic entry point
+    const char* classic_refusal = nullptr;    // that entry point's own refusal of its arguments (nullptr: none)
+    const void* occ = nullptr; size_t occ_bytes = 0;    // the occupancy map of kSkipCall and kOccBuildCall
+};
+
+// Occupancy map: M*N planes of occ_rows(Ht) block rows of occ_words(Wt) words.
+static size_t occ_map_bytes(const RenderParams& p) { return (size_t)p.M * p.N * occ_rows(p.Ht) * occ_words(p.Wt) * sizeof(uint32_t); }
+
+static int check_occ_map(const RenderParams& p, const Call& c) {
+    if (!c.occ) return fail(GMPI_ERR_INVALID_ARGUMENT, "null occupancy map (gmpi_mpi_occupancy_bytes gives its size)");
+    if ((uintptr_t)c.occ & 3) return fail(GMPI_ERR_INVALID_ARGUMENT, "the occupancy map must be 4-byte aligned");
+    const size_t need = occ_map_bytes(p);
+    if (c.occ_bytes < need)
+        return fail(GMPI_ERR_INVALID_ARGUMENT, "occupancy map of %zu bytes is smaller than the %zu bytes of this MPI", c.occ_bytes, need);
     return GMPI_OK;
 }
 
-// Argument checks shared by every entry point.  `bwd`: gradients instead of outputs.
-static int check_params(const RenderParams& p, bool bwd) {
-    if (int rc = check_u8(p, bwd)) return rc;
-    if (p.options & GMPI_MPI_F16) {
-        if (bwd) return fail(GMPI_ERR_UNSUPPORTED, "GMPI_MPI_F16 is forward-only: the backward reads and writes fp32 MPIs");
-        if (p.transmittance)
-            return fail(GMPI_ERR_UNSUPPORTED, "GMPI_MPI_F16 cannot be combined with the training forward (transmittance)");
+// Every check of a call's RenderParams, and of the occupancy map it reads.  The first refusal wins.
+static int check_call(const RenderParams& p, const Call& c) {
+    // A classic entry point takes no forward-only option.  Its MPI pointer is a float*, so fp16 and uint8 are refused first.  It has
+    // no early_stop field, so GMPI_EARLY_STOP is refused where a descriptor's threshold is checked.
+    for (const ForwardOnly& o : kForwardOnly)
+        if (c.classic && (p.options & o.bit & (GMPI_MPI_F16 | GMPI_MPI_U8)))
+            return fail(GMPI_ERR_UNSUPPORTED, "%s is accepted by the descriptor forward entry points only", o.name);
+    if (c.classic_refusal) return fail(GMPI_ERR_INVALID_ARGUMENT, "%s", c.classic_refusal);
+    // the uint8 MPI's own rules: not fp16 as well (here), and expanded only (after the backward's refusals)
+    if ((p.options & GMPI_MPI_U8) && (p.options & GMPI_MPI_F16))
+        return fail(GMPI_ERR_INVALID_ARGUMENT, "GMPI_MPI_U8 and GMPI_MPI_F16 are exclusive");
+    // Of the forward-only options, the occupancy calls and the scratch query check GMPI_MPI_U8 alone: the scratch query returns a size
+    // for GMPI_MPI_F16 and GMPI_EARLY_STOP, which the deterministic backward refuses.
+    const bool occ = c.kind == kOccQueryCall || c.kind == kOccBuildCall, bwd = c.kind == kBwdCall || c.kind == kScratchCall;
+    const uint32_t opts = p.options & (occ || c.kind == kScratchCall ? GMPI_MPI_U8 : GMPI_MPI_F16 | GMPI_MPI_U8 | GMPI_EARLY_STOP);
+    for (const ForwardOnly& o : kForwardOnly)
+        if (bwd && (opts & o.bit)) return fail(GMPI_ERR_UNSUPPORTED, "%s is forward-only: %s", o.name, o.why);
+    if ((opts & GMPI_MPI_U8) && (p.rgb || p.alpha || p.bg_rgb))
+        return fail(GMPI_ERR_UNSUPPORTED, "GMPI_MPI_U8 takes an expanded MPI (rgba), not a factored one");
+    for (const ForwardOnly& o : kForwardOnly)
+        if ((opts & o.bit) && p.transmittance)
+            return fail(GMPI_ERR_UNSUPPORTED, "%s cannot be combined with the training forward (transmittance)", o.name);
+    if ((opts & GMPI_EARLY_STOP) && c.classic)
+        return fail(GMPI_ERR_INVALID_ARGUMENT, "GMPI_EARLY_STOP needs a descriptor: the classic entry points have no early_stop field");
+    if ((opts & GMPI_EARLY_STOP) && !(p.early_stop >= 0.0f && p.early_stop < 1.0f))
+        return fail(GMPI_ERR_INVALID_ARGUMENT, "early_stop = %g must be in [0, 1) (gmpi_render_desc.early_stop)", (double)p.early_stop);
+    if (c.kind == kScratchCall) return check_sizes(p, true, false);
+    if (factored(p) ? !p.rgb || p.rgba : !p.rgba || p.rgb)
+        return fail(GMPI_ERR_INVALID_ARGUMENT, "null input pointer (MPI: pass rgba, or rgb + alpha)");
+    if (occ) {
+        if (int rc = check_sizes(p, false, true)) return rc;
+        return c.kind == kOccBuildCall ? check_occ_map(p, c) : GMPI_OK;
     }
-    if (p.options & GMPI_EARLY_STOP) {
-        if (bwd) return fail(GMPI_ERR_UNSUPPORTED, "GMPI_EARLY_STOP is forward-only: the backward needs every plane's samples");
-        if (p.transmittance)
-            return fail(GMPI_ERR_UNSUPPORTED, "GMPI_EARLY_STOP cannot be combined with the training forward (transmittance)");
-        if (!(p.early_stop >= 0.0f && p.early_stop < 1.0f))
-            return fail(GMPI_ERR_INVALID_ARGUMENT, "early_stop = %g must be in [0, 1) (gmpi_render_desc.early_stop)", (double)p.early_stop);
-    }
-    int rc = check_mpi_form(p);
-    if (rc) return rc;
     if (!p.view2mpi || !p.dhw) return fail(GMPI_ERR_INVALID_ARGUMENT, "null input pointer");
     if (!p.cam && (!p.ray_dir || !p.eye || !p.z_dir))
         return fail(GMPI_ERR_INVALID_ARGUMENT, "null input pointer (camera: pass ray_dir + eye + z_dir, or cam)");
-    if ((rc = check_sizes(p, true, true)) != 0) return rc;
+    if (int rc = check_sizes(p, true, true)) return rc;
     if (p.view_group < 0 || (p.view_group > 1 && p.V % p.view_group != 0))
         return fail(GMPI_ERR_INVALID_ARGUMENT, "view_group=%d does not divide V=%d", p.view_group, p.V);
     if (bwd) {
@@ -448,6 +486,27 @@ static int check_params(const RenderParams& p, bool bwd) {
         if (!p.g_color) return fail(GMPI_ERR_INVALID_ARGUMENT, "null gradient pointer");
         if (factored(p) ? (!p.g_rgb || !p.g_alpha || (p.bg_rgb && !p.g_bg_rgb) || p.g_rgba) : !p.g_rgba)
             return fail(GMPI_ERR_INVALID_ARGUMENT, "null gradient pointer (pass g_rgba, or g_rgb + g_alpha [+ g_bg_rgb])");
+        return GMPI_OK;
+    }
+    if (c.kind == kSkipCall) {
+        if (p.transmittance)
+            return fail(GMPI_ERR_UNSUPPORTED, "empty-space skipping is forward-only: it cannot be combined with the training forward (transmittance)");
+        if (int rc = check_occ_map(p, c)) return rc;
+    }
+    // the forward's outputs
+    if (c.kind == kHostCall) {
+        if (!p.flags || (!p.video_rgb && (!p.color || !p.depth))) return fail(GMPI_ERR_INVALID_ARGUMENT, "null output pointer");
+        if (p.n_peers > 0 || p.transmittance) return fail(GMPI_ERR_UNSUPPORTED, "the host entry point renders to host buffers only");
+    } else if (!p.flags) {
+        return fail(GMPI_ERR_INVALID_ARGUMENT, "null flags pointer");
+    }
+    if (p.video_rgb) {
+        if (p.n_peers > 0) return fail(GMPI_ERR_INVALID_ARGUMENT, "video outputs and peer frames are exclusive");
+        if (p.video_depth && !(p.depth_range != 0.0f)) return fail(GMPI_ERR_INVALID_ARGUMENT, "depth_range must be non-zero");
+    } else if (p.n_peers > 0) {
+        if (!p.peer_frames || p.frame_offset < 0) return fail(GMPI_ERR_INVALID_ARGUMENT, "bad peer frame buffers");
+    } else if (!p.color || !p.depth) {
+        return fail(GMPI_ERR_INVALID_ARGUMENT, "null output pointer");
     }
     return GMPI_OK;
 }
@@ -669,25 +728,6 @@ static int read_stage_stats(StageStats s, unsigned long long* skipped, unsigned 
     return GMPI_OK;
 }
 
-// Occupancy map: M*N planes of occ_rows(Ht) block rows of occ_words(Wt) words.  Checks what the map's size and build read.
-static int occ_bytes(const RenderParams& p, size_t* bytes) {
-    int rc = check_u8(p, false);
-    if (rc || (rc = check_mpi_form(p)) != 0) return rc;
-    if (rc || (rc = check_sizes(p, false, true)) != 0) return rc;
-    *bytes = (size_t)p.M * p.N * occ_rows(p.Ht) * occ_words(p.Wt) * sizeof(uint32_t);
-    return GMPI_OK;
-}
-
-static int check_occ_arg(const RenderParams& p, const void* occ, size_t bytes) {
-    size_t need = 0;
-    int rc = occ_bytes(p, &need);
-    if (rc) return rc;
-    if (!occ) return fail(GMPI_ERR_INVALID_ARGUMENT, "null occupancy map (gmpi_mpi_occupancy_bytes gives its size)");
-    if ((uintptr_t)occ & 3) return fail(GMPI_ERR_INVALID_ARGUMENT, "the occupancy map must be 4-byte aligned");
-    if (bytes < need) return fail(GMPI_ERR_INVALID_ARGUMENT, "occupancy map of %zu bytes is smaller than the %zu bytes of this MPI", bytes, need);
-    return GMPI_OK;
-}
-
 // The forward kernel of a checked call with V > 0, with its launch.  occ: empty-space skipping against this map.  The staged
 // kernel when fwd_why(p) == 0 and its tensor maps encode, else the direct kernel; a forced staged variant fails instead.
 static int fwd_launch(Launch& l, const uint32_t* occ) {
@@ -726,25 +766,15 @@ static int fwd_launch(Launch& l, const uint32_t* occ) {
     return GMPI_OK;
 }
 
-// Forward launch for a filled RenderParams.  occ: empty-space skipping against this occupancy map (checked by the caller).
+// Forward launch of a checked call (check_call).  occ: empty-space skipping against this occupancy map.
 static int launch_fwd(RenderParams p, cudaStream_t st, const uint32_t* occ = nullptr) {
-    int rc = check_params(p, false);
-    if (rc) return rc;
-    if (!p.flags) return fail(GMPI_ERR_INVALID_ARGUMENT, "null flags pointer");
-    if (p.video_rgb) {
-        if (p.n_peers > 0) return fail(GMPI_ERR_INVALID_ARGUMENT, "video outputs and peer frames are exclusive");
-        if (p.video_depth && !(p.depth_range != 0.0f)) return fail(GMPI_ERR_INVALID_ARGUMENT, "depth_range must be non-zero");
-    } else if (p.n_peers > 0) {
-        if (!p.peer_frames || p.frame_offset < 0) return fail(GMPI_ERR_INVALID_ARGUMENT, "bad peer frame buffers");
-    } else if (!p.color || !p.depth) {
-        return fail(GMPI_ERR_INVALID_ARGUMENT, "null output pointer");
-    }
     if (p.V == 0) return GMPI_OK;
     // float4 epilogue stores: whole quads of x stay inside a row and every destination is 16-byte aligned.  Peer buffers are
     // symmetric-memory allocations (256-byte aligned bases; frame slabs are multiples of 16 bytes when W % 4 == 0).
     if (p.W % 4 == 0 && !p.video_rgb && (p.n_peers > 0 || (aligned16(p.color) && aligned16(p.depth)))) p.options |= kOptVec4Stores;
     Launch l(p);
-    if ((rc = fwd_launch(l, occ)) != 0) return rc;
+    int rc = fwd_launch(l, occ);
+    if (rc) return rc;
     // the direct kernel walks no stages: it loads per pixel, and composites every plane (which gives a skipping call's output)
     const unsigned long long walked = (unsigned long long)l.tiles * p.N;
     const KernelUnit& unit = key_unit(l.key);
@@ -811,12 +841,11 @@ static int bwd_launch(Launch& l, bool box, bool det) {
 }
 
 static int launch_bwd(RenderParams p, cudaStream_t st) {
-    int rc = check_params(p, true);
-    if (rc) return rc;
     const bool zero = (p.options & GMPI_ZERO_GRAD) != 0;
     if (p.V == 0) return zero ? zero_grads(p, st) : GMPI_OK;
     Launch l(p);
-    if ((rc = bwd_launch(l, bwd_uses_box(p), false)) != 0) return rc;
+    int rc = bwd_launch(l, bwd_uses_box(p), false);
+    if (rc) return rc;
     if (zero && (rc = zero_grads(p, st)) != 0) return rc;
     return launch(l, st);
 }
@@ -830,8 +859,8 @@ struct DetLayout {
 constexpr size_t kDetHeaderBytes = 256;
 constexpr int kDetMinFixBits = 24;
 
+// The layout of a call with checked sizes (check_call).
 static int det_layout(const RenderParams& p, DetLayout& L) {
-    if (int rc = check_sizes(p, true, false)) return rc;
     const double tex = (double)p.Ht * p.Wt, M = p.M, N = p.N;
     const double G = factored(p) ? M * 3 * tex + M * N * tex + (p.bg_rgb ? M * 3 * tex : 0.0) : M * N * 4 * tex;
     if (G * 9 > 0x1p62) return fail(GMPI_ERR_UNSUPPORTED, "%.0f gradient elements exceed the deterministic scratch's range", G);
@@ -861,10 +890,9 @@ static int det_fix_bits(const RenderParams& p, int planes) {
 }
 
 static int launch_bwd_deterministic(RenderParams p, void* scratch, size_t scratch_bytes, cudaStream_t st) {
-    int rc = check_params(p, true);
-    if (rc) return rc;
     DetLayout L;
-    if ((rc = det_layout(p, L)) != 0) return rc;
+    int rc = det_layout(p, L);
+    if (rc) return rc;
     if (!scratch) return fail(GMPI_ERR_INVALID_ARGUMENT, "null scratch pointer (gmpi_mpi_render_bwd_deterministic_scratch_bytes gives its size)");
     if (!aligned16(scratch)) return fail(GMPI_ERR_INVALID_ARGUMENT, "the scratch must be 16-byte aligned");
     if (scratch_bytes < L.bytes)
@@ -933,30 +961,47 @@ static int check_desc(const gmpi_render_desc* d) {
     return GMPI_OK;
 }
 
-// The classic entry points take fp32 MPIs only (their pointers are typed float*): GMPI_MPI_F16 and GMPI_MPI_U8 need a descriptor.
-static int refuse_f16_classic(uint32_t options) {
-    if (options & GMPI_MPI_F16)
-        return fail(GMPI_ERR_UNSUPPORTED, "GMPI_MPI_F16 is accepted by gmpi_mpi_render_fwd_ex and gmpi_mpi_render_host_ex only");
-    if (options & GMPI_MPI_U8)
-        return fail(GMPI_ERR_UNSUPPORTED, "GMPI_MPI_U8 is accepted by the descriptor forward entry points only");
-    return GMPI_OK;
+// The RenderParams p of a descriptor call, checked (check_desc, check_call).
+static int check_desc_call(const gmpi_render_desc* d, const Call& c, RenderParams& p) {
+    int rc = check_desc(d);
+    if (rc) return rc;
+    p = params_from_desc(d);
+    return check_call(p, c);
 }
 
-static RenderParams params_classic(const float* rgba, const int32_t* view2mpi, const float* dhw, const float* ray_dir, const float* eye,
-                                   const float* z_dir, int M, int V, int N, int Ht, int Wt, int H, int W, uint32_t options) {
+// The path of gmpi_mpi_render_fwd_ex (kFwdCall) and gmpi_mpi_render_bwd_ex (kBwdCall).
+static int render(const gmpi_render_desc* d, const Call& c) {
     RenderParams p{};
-    p.rgba = rgba; p.view2mpi = view2mpi; p.dhw = dhw; p.ray_dir = ray_dir; p.eye = eye; p.z_dir = z_dir;
-    p.M = M; p.V = V; p.N = N; p.Ht = Ht; p.Wt = Wt; p.H = H; p.W = W;
-    p.options = options & 0xffffu;
-    p.view_group = 1;
-    p.early_stop = (options & GMPI_EARLY_STOP) ? NAN : 0.0f;   // the threshold is a descriptor field: check_params refuses the bit here
-    return p;
+    int rc = check_desc_call(d, c, p);
+    return rc ? rc : c.kind == kBwdCall ? launch_bwd(p, (cudaStream_t)d->stream) : launch_fwd(p, (cudaStream_t)d->stream);
 }
 
-static int fwd_plan(const RenderParams& p, uint32_t* why) {
-    const uint32_t w = fwd_why(p);
-    if (why) *why = w;
-    return w == 0 ? GMPI_PLAN_STAGED : GMPI_PLAN_DIRECT;
+// The descriptor of a classic entry point's arguments: an expanded fp32 MPI and the reference's ray tensors.  The entry point adds
+// its outputs or gradients and takes the path of the descriptor call it corresponds to, checked as a classic call.
+static gmpi_render_desc classic_desc(const float* rgba, const int32_t* view2mpi, const float* dhw, const float* ray_dir, const float* eye,
+                                     const float* z_dir, int M, int V, int N, int Ht, int Wt, int H, int W, uint32_t options, void* stream) {
+    gmpi_render_desc d{};
+    d.struct_bytes = sizeof(gmpi_render_desc); d.options = options; d.view_group = 1; d.stream = stream;
+    d.M = M; d.V = V; d.N = N; d.Ht = Ht; d.Wt = Wt; d.H = H; d.W = W;
+    d.rgba = rgba; d.view2mpi = view2mpi; d.dhw = dhw; d.ray_dir = ray_dir; d.eye = eye; d.z_dir = z_dir;
+    return d;
+}
+
+// The range check of an fp32 or (f16) fp16 rgba: 16-byte loads when every slab is a whole number of them on an aligned base.
+static int check_range(const void* rgba, bool f16, int M, int N, int Ht, int Wt, uint32_t* flags, cudaStream_t st) {
+    if (!rgba || !flags) return fail(GMPI_ERR_INVALID_ARGUMENT, "null pointer");
+    if (M < 1 || N < 1 || Ht < 1 || Wt < 1) return fail(GMPI_ERR_INVALID_ARGUMENT, "bad sizes");
+    const size_t slab = (size_t)Ht * Wt, n_slabs = (size_t)M * N * 4, per_load = f16 ? 8 : 4;
+    int sms = 132;
+    if (int rc = device_attr(cudaDevAttrMultiProcessorCount, &sms)) return rc;
+    const int grid = sms * 8;
+    const bool vec = slab % per_load == 0 && aligned16(rgba);
+    if (f16 && vec) mpi_check_range_f16_kernel<<<grid, 256, 0, st>>>(static_cast<const uint4*>(rgba), n_slabs, slab / 8, flags);
+    else if (f16) mpi_check_range_f16_scalar_kernel<<<grid, 256, 0, st>>>(static_cast<const unsigned short*>(rgba), n_slabs, slab, flags);
+    else if (vec) mpi_check_range_kernel<<<grid, 256, 0, st>>>(static_cast<const float4*>(rgba), n_slabs, slab / 4, flags);
+    else mpi_check_range_scalar_kernel<<<grid, 256, 0, st>>>(static_cast<const float*>(rgba), n_slabs, slab, flags);
+    GMPI_CUDA_OK(cudaGetLastError());
+    return GMPI_OK;
 }
 
 extern "C" {
@@ -1028,70 +1073,65 @@ int gmpi_debug_tile_walk(int H, int W, int V, int grid, int cta, int* out_v_px0_
 }
 
 int gmpi_mpi_render_fwd_plan(int V, int N, int Ht, int Wt, int H, int W, const void* rgba, uint32_t* why) {
-    return fwd_plan(params_classic(static_cast<const float*>(rgba), nullptr, nullptr, nullptr, nullptr, nullptr, 1, V, N, Ht, Wt, H, W, 0), why);
+    const gmpi_render_desc d = classic_desc(static_cast<const float*>(rgba), nullptr, nullptr, nullptr, nullptr, nullptr, 1, V, N, Ht, Wt,
+                                            H, W, 0, nullptr);
+    return gmpi_mpi_render_fwd_plan_ex(&d, why);
 }
 
 int gmpi_mpi_render_fwd_plan_ex(const gmpi_render_desc* d, uint32_t* why) {
     int rc = check_desc(d);
     if (rc) return -rc;
-    return fwd_plan(params_from_desc(d), why);
+    const uint32_t w = fwd_why(params_from_desc(d));
+    if (why) *why = w;
+    return w == 0 ? GMPI_PLAN_STAGED : GMPI_PLAN_DIRECT;
 }
 
 const char* gmpi_mpi_render_fwd_variant(int N, int Ht, int Wt, int H, int W) {
-    const RenderParams p = params_classic(nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 1, 1 << 20, N, Ht, Wt, H, W, 0);
-    return fwd_why(p) == 0 ? "fwd_staged_tma_64x30" : "fwd_direct_32x8";
+    return gmpi_mpi_render_fwd_plan(1 << 20, N, Ht, Wt, H, W, nullptr, nullptr) == GMPI_PLAN_STAGED ? "fwd_staged_tma_64x30" : "fwd_direct_32x8";
 }
 
 int gmpi_mpi_render_fwd(const float* rgba, const int32_t* view2mpi, const float* dhw, const float* ray_dir,
                         const float* eye, const float* z_dir, float* color, float* depth, uint32_t* flags, int M,
                         int V, int N, int Ht, int Wt, int H, int W, uint32_t options, void* stream) {
-    if (int rc = refuse_f16_classic(options)) return rc;
-    RenderParams p = params_classic(rgba, view2mpi, dhw, ray_dir, eye, z_dir, M, V, N, Ht, Wt, H, W, options);
-    p.color = color; p.depth = depth; p.flags = flags;
-    return launch_fwd(p, (cudaStream_t)stream);
+    gmpi_render_desc d = classic_desc(rgba, view2mpi, dhw, ray_dir, eye, z_dir, M, V, N, Ht, Wt, H, W, options, stream);
+    d.color = color; d.depth = depth; d.flags = flags;
+    return render(&d, Call{kFwdCall, true});
 }
 
 int gmpi_mpi_render_fwd_train(const float* rgba, const int32_t* view2mpi, const float* dhw, const float* ray_dir,
                               const float* eye, const float* z_dir, float* color, float* depth, float* transmittance,
                               uint32_t* flags, int M, int V, int N, int Ht, int Wt, int H, int W, uint32_t options,
                               void* stream) {
-    if (int rc = refuse_f16_classic(options)) return rc;
-    if (!transmittance) return fail(GMPI_ERR_INVALID_ARGUMENT, "null transmittance buffer");
-    RenderParams p = params_classic(rgba, view2mpi, dhw, ray_dir, eye, z_dir, M, V, N, Ht, Wt, H, W, options);
-    p.color = color; p.depth = depth; p.flags = flags; p.transmittance = transmittance;
-    return launch_fwd(p, (cudaStream_t)stream);
+    gmpi_render_desc d = classic_desc(rgba, view2mpi, dhw, ray_dir, eye, z_dir, M, V, N, Ht, Wt, H, W, options, stream);
+    d.color = color; d.depth = depth; d.flags = flags; d.transmittance = transmittance;
+    return render(&d, Call{kFwdCall, true, transmittance ? nullptr : "null transmittance buffer"});
 }
 
 int gmpi_mpi_render_fwd_gather(const float* rgba, const int32_t* view2mpi, const float* dhw, const float* ray_dir,
                                const float* eye, const float* z_dir, float* const* peer_frames, int n_peers,
                                int frame_offset, uint32_t* flags, int M, int V, int N, int Ht, int Wt, int H, int W,
                                uint32_t options, void* stream) {
-    if (int rc = refuse_f16_classic(options)) return rc;
-    if (n_peers < 1) return fail(GMPI_ERR_INVALID_ARGUMENT, "n_peers must be >= 1");
-    RenderParams p = params_classic(rgba, view2mpi, dhw, ray_dir, eye, z_dir, M, V, N, Ht, Wt, H, W, options);
-    p.flags = flags; p.peer_frames = peer_frames; p.n_peers = n_peers; p.frame_offset = frame_offset;
-    return launch_fwd(p, (cudaStream_t)stream);
+    gmpi_render_desc d = classic_desc(rgba, view2mpi, dhw, ray_dir, eye, z_dir, M, V, N, Ht, Wt, H, W, options, stream);
+    d.flags = flags; d.peer_frames = peer_frames; d.n_peers = n_peers; d.frame_offset = frame_offset;
+    return render(&d, Call{kFwdCall, true, n_peers < 1 ? "n_peers must be >= 1" : nullptr});
 }
 
 int gmpi_mpi_render_bwd(const float* rgba, const int32_t* view2mpi, const float* dhw, const float* ray_dir,
                         const float* eye, const float* z_dir, const float* g_color, const float* g_depth,
                         float* g_rgba, int M, int V, int N, int Ht, int Wt, int H, int W, uint32_t options,
                         void* stream) {
-    if (int rc = refuse_f16_classic(options)) return rc;
-    RenderParams p = params_classic(rgba, view2mpi, dhw, ray_dir, eye, z_dir, M, V, N, Ht, Wt, H, W, options);
-    p.g_color = g_color; p.g_depth = g_depth; p.g_rgba = g_rgba;
-    return launch_bwd(p, (cudaStream_t)stream);
+    gmpi_render_desc d = classic_desc(rgba, view2mpi, dhw, ray_dir, eye, z_dir, M, V, N, Ht, Wt, H, W, options, stream);
+    d.g_color = g_color; d.g_depth = g_depth; d.g_rgba = g_rgba;
+    return render(&d, Call{kBwdCall, true});
 }
 
 int gmpi_mpi_render_bwd_saved(const float* rgba, const int32_t* view2mpi, const float* dhw, const float* ray_dir,
                               const float* eye, const float* z_dir, const float* transmittance, const float* g_color,
                               const float* g_depth, float* g_rgba, int M, int V, int N, int Ht, int Wt, int H, int W,
                               uint32_t options, void* stream) {
-    if (int rc = refuse_f16_classic(options)) return rc;
-    if (!transmittance) return fail(GMPI_ERR_INVALID_ARGUMENT, "null gradient / transmittance pointer");
-    RenderParams p = params_classic(rgba, view2mpi, dhw, ray_dir, eye, z_dir, M, V, N, Ht, Wt, H, W, options);
-    p.g_color = g_color; p.g_depth = g_depth; p.g_rgba = g_rgba; p.transmittance = const_cast<float*>(transmittance);
-    return launch_bwd(p, (cudaStream_t)stream);
+    gmpi_render_desc d = classic_desc(rgba, view2mpi, dhw, ray_dir, eye, z_dir, M, V, N, Ht, Wt, H, W, options, stream);
+    d.g_color = g_color; d.g_depth = g_depth; d.g_rgba = g_rgba; d.transmittance = const_cast<float*>(transmittance);
+    return render(&d, Call{kBwdCall, true, transmittance ? nullptr : "null gradient / transmittance pointer"});
 }
 
 int gmpi_mpi_zero_async(void* ptr, size_t bytes, void* stream) {
@@ -1100,46 +1140,34 @@ int gmpi_mpi_zero_async(void* ptr, size_t bytes, void* stream) {
     return GMPI_OK;
 }
 
-int gmpi_mpi_render_fwd_ex(const gmpi_render_desc* d) {
-    int rc = check_desc(d);
-    if (rc) return rc;
-    return launch_fwd(params_from_desc(d), (cudaStream_t)d->stream);
-}
+int gmpi_mpi_render_fwd_ex(const gmpi_render_desc* d) { return render(d, Call{kFwdCall}); }
 
-int gmpi_mpi_render_bwd_ex(const gmpi_render_desc* d) {
-    int rc = check_desc(d);
-    if (rc) return rc;
-    return launch_bwd(params_from_desc(d), (cudaStream_t)d->stream);
-}
+int gmpi_mpi_render_bwd_ex(const gmpi_render_desc* d) { return render(d, Call{kBwdCall}); }
 
 long long gmpi_mpi_render_bwd_deterministic_scratch_bytes(const gmpi_render_desc* d) {
-    int rc = check_desc(d);
-    if (rc) return -rc;
+    RenderParams p{};
     DetLayout L;
-    const RenderParams p = params_from_desc(d);
-    if ((rc = check_u8(p, true)) != 0 || (rc = det_layout(p, L)) != 0) return -rc;
+    int rc = check_desc_call(d, Call{kScratchCall}, p);
+    if (rc || (rc = det_layout(p, L)) != 0) return -rc;
     return (long long)L.bytes;
 }
 
 int gmpi_mpi_render_bwd_deterministic_ex(const gmpi_render_desc* d, void* scratch, size_t scratch_bytes) {
-    int rc = check_desc(d);
-    if (rc) return rc;
-    return launch_bwd_deterministic(params_from_desc(d), scratch, scratch_bytes, (cudaStream_t)d->stream);
+    RenderParams p{};
+    int rc = check_desc_call(d, Call{kBwdCall}, p);
+    return rc ? rc : launch_bwd_deterministic(p, scratch, scratch_bytes, (cudaStream_t)d->stream);
 }
 
 long long gmpi_mpi_occupancy_bytes(const gmpi_render_desc* d) {
-    int rc = check_desc(d);
-    if (rc) return -rc;
-    size_t bytes = 0;
-    if ((rc = occ_bytes(params_from_desc(d), &bytes)) != 0) return -rc;
-    return (long long)bytes;
+    RenderParams p{};
+    int rc = check_desc_call(d, Call{kOccQueryCall}, p);
+    return rc ? -rc : (long long)occ_map_bytes(p);
 }
 
 int gmpi_mpi_build_occupancy(const gmpi_render_desc* d, void* occ, size_t bytes) {
-    int rc = check_desc(d);
+    RenderParams p{};
+    int rc = check_desc_call(d, Call{kOccBuildCall, false, nullptr, occ, bytes}, p);
     if (rc) return rc;
-    const RenderParams p = params_from_desc(d);
-    if ((rc = check_occ_arg(p, occ, bytes)) != 0) return rc;
     const int words = occ_words(p.Wt), rows = occ_rows(p.Ht);
     if (rows > 65535) return fail(GMPI_ERR_UNSUPPORTED, "Ht=%d exceeds the occupancy build's grid (%d texel rows)", p.Ht, 65535 * kOccB);
     const bool f16 = (p.options & GMPI_MPI_F16) != 0, u8 = (p.options & GMPI_MPI_U8) != 0;
@@ -1176,14 +1204,9 @@ int gmpi_mpi_build_occupancy(const gmpi_render_desc* d, void* occ, size_t bytes)
 }
 
 int gmpi_mpi_render_fwd_skip_ex(const gmpi_render_desc* d, const void* occ, size_t bytes) {
-    int rc = check_desc(d);
-    if (rc) return rc;
-    const RenderParams p = params_from_desc(d);
-    if ((rc = check_params(p, false)) != 0) return rc;
-    if (p.transmittance)
-        return fail(GMPI_ERR_UNSUPPORTED, "empty-space skipping is forward-only: it cannot be combined with the training forward (transmittance)");
-    if ((rc = check_occ_arg(p, occ, bytes)) != 0) return rc;
-    return launch_fwd(p, (cudaStream_t)d->stream, static_cast<const uint32_t*>(occ));
+    RenderParams p{};
+    int rc = check_desc_call(d, Call{kSkipCall, false, nullptr, occ, bytes}, p);
+    return rc ? rc : launch_fwd(p, (cudaStream_t)d->stream, static_cast<const uint32_t*>(occ));
 }
 
 int gmpi_debug_fwd_skip_stats(unsigned long long* skipped, unsigned long long* total) {
@@ -1214,39 +1237,11 @@ int gmpi_debug_u8_codes(float* out, void* stream) {
 }
 
 int gmpi_mpi_check_range(const float* rgba, int M, int N, int Ht, int Wt, uint32_t* flags, void* stream) {
-    if (!rgba || !flags) return fail(GMPI_ERR_INVALID_ARGUMENT, "null pointer");
-    if (M < 1 || N < 1 || Ht < 1 || Wt < 1) return fail(GMPI_ERR_INVALID_ARGUMENT, "bad sizes");
-    cudaStream_t st = (cudaStream_t)stream;
-    const size_t slab = (size_t)Ht * Wt, n_slabs = (size_t)M * N * 4;
-    int sms = 132;
-    int rc = device_attr(cudaDevAttrMultiProcessorCount, &sms);
-    if (rc) return rc;
-    const int grid = sms * 8;
-    if (slab % 4 == 0 && ((uintptr_t)rgba & 15) == 0) {
-        mpi_check_range_kernel<<<grid, 256, 0, st>>>(reinterpret_cast<const float4*>(rgba), n_slabs, slab / 4, flags);
-    } else {
-        mpi_check_range_scalar_kernel<<<grid, 256, 0, st>>>(rgba, n_slabs, slab, flags);
-    }
-    GMPI_CUDA_OK(cudaGetLastError());
-    return GMPI_OK;
+    return check_range(rgba, false, M, N, Ht, Wt, flags, (cudaStream_t)stream);
 }
 
 int gmpi_mpi_check_range_f16(const void* rgba, int M, int N, int Ht, int Wt, uint32_t* flags, void* stream) {
-    if (!rgba || !flags) return fail(GMPI_ERR_INVALID_ARGUMENT, "null pointer");
-    if (M < 1 || N < 1 || Ht < 1 || Wt < 1) return fail(GMPI_ERR_INVALID_ARGUMENT, "bad sizes");
-    cudaStream_t st = (cudaStream_t)stream;
-    const size_t slab = (size_t)Ht * Wt, n_slabs = (size_t)M * N * 4;
-    int sms = 132;
-    int rc = device_attr(cudaDevAttrMultiProcessorCount, &sms);
-    if (rc) return rc;
-    const int grid = sms * 8;
-    if (slab % 8 == 0 && ((uintptr_t)rgba & 15) == 0) {
-        mpi_check_range_f16_kernel<<<grid, 256, 0, st>>>(reinterpret_cast<const uint4*>(rgba), n_slabs, slab / 8, flags);
-    } else {
-        mpi_check_range_f16_scalar_kernel<<<grid, 256, 0, st>>>(reinterpret_cast<const unsigned short*>(rgba), n_slabs, slab, flags);
-    }
-    GMPI_CUDA_OK(cudaGetLastError());
-    return GMPI_OK;
+    return check_range(rgba, true, M, N, Ht, Wt, flags, (cudaStream_t)stream);
 }
 
 int gmpi_debug_plane_coords(const int32_t* view2mpi, const float* dhw, const float* ray_dir, const float* eye,
@@ -1400,8 +1395,8 @@ int gmpi_mpi_release_host_cache(void) {
     return GMPI_OK;
 }
 
-// `h` holds HOST pointers.  Streams every MPI through a double-buffered device slot and renders its views.
-static int host_render_locked(HostCache& c, const RenderParams& h, uint32_t* flags_out) {
+// `h` holds HOST pointers (a checked call).  Streams every MPI through a double-buffered device slot and renders its views.
+static int host_render_locked(HostCache& c, const RenderParams& h) {
     int rc = GMPI_OK;
     const int M = h.M, V = h.V, N = h.N, H = h.H, W = h.W;
     const size_t tex = (size_t)h.Ht * h.Wt, img = (size_t)H * W;
@@ -1507,18 +1502,17 @@ static int host_render_locked(HostCache& c, const RenderParams& h, uint32_t* fla
         GMPI_CUDA_OK(cudaMemcpyAsync(h.color, base + o_color, sizeof(float) * (size_t)V * 3 * img, cudaMemcpyDeviceToHost, s_run));
         GMPI_CUDA_OK(cudaMemcpyAsync(h.depth, base + o_depth, sizeof(float) * (size_t)V * img, cudaMemcpyDeviceToHost, s_run));
     }
-    GMPI_CUDA_OK(cudaMemcpyAsync(flags_out, d_flags, sizeof(uint32_t), cudaMemcpyDeviceToHost, s_run));
+    GMPI_CUDA_OK(cudaMemcpyAsync(h.flags, d_flags, sizeof(uint32_t), cudaMemcpyDeviceToHost, s_run));
     GMPI_CUDA_OK(cudaStreamSynchronize(s_run));
     GMPI_CUDA_OK(cudaStreamSynchronize(s_copy));
     return GMPI_OK;
 }
 
-static int host_render(const RenderParams& h, uint32_t* flags_out, int device) {
-    int rc = check_params(h, false);
+// The path of gmpi_mpi_render_host_ex: d's pointers are host memory, d->flags receives the flag word.
+static int render_host(const gmpi_render_desc* d, int device, const Call& call) {
+    RenderParams h{};
+    int rc = check_desc_call(d, call, h);
     if (rc) return rc;
-    if (!flags_out) return fail(GMPI_ERR_INVALID_ARGUMENT, "null output pointer");
-    if (h.video_rgb ? false : (!h.color || !h.depth)) return fail(GMPI_ERR_INVALID_ARGUMENT, "null output pointer");
-    if (h.n_peers > 0 || h.transmittance) return fail(GMPI_ERR_UNSUPPORTED, "the host entry point renders to host buffers only");
     if (device < 0 || device >= 64) return fail(GMPI_ERR_INVALID_ARGUMENT, "device %d out of range", device);
     for (int v = 0; v + 1 < h.V; ++v)
         if (h.view2mpi[v] > h.view2mpi[v + 1]) return fail(GMPI_ERR_INVALID_ARGUMENT, "views must be MPI-major (sorted view2mpi)");
@@ -1527,7 +1521,7 @@ static int host_render(const RenderParams& h, uint32_t* flags_out, int device) {
     GMPI_CUDA_OK(cudaSetDevice(device));
     std::lock_guard<std::mutex> lock(g_host_mutex[device]);
     HostCache& c = g_host_cache[device];
-    rc = host_render_locked(c, h, flags_out);
+    rc = host_render_locked(c, h);
     if (rc != GMPI_OK) {
         // An error may have left asynchronous copies reading the caller's host buffers or rendering from the staging slots:
         // drain both streams before returning so that the caller may free its buffers and the next call starts clean.
@@ -1544,16 +1538,11 @@ static int host_render(const RenderParams& h, uint32_t* flags_out, int device) {
 int gmpi_mpi_render_fwd_host(const float* rgba, const int32_t* view2mpi, const float* dhw, const float* ray_dir,
                              const float* eye, const float* z_dir, float* color, float* depth, uint32_t* flags_out,
                              int M, int V, int N, int Ht, int Wt, int H, int W, uint32_t options, int device) {
-    if (int rc = refuse_f16_classic(options)) return rc;
-    RenderParams h = params_classic(rgba, view2mpi, dhw, ray_dir, eye, z_dir, M, V, N, Ht, Wt, H, W, options);
-    h.color = color; h.depth = depth;
-    return host_render(h, flags_out, device);
+    gmpi_render_desc d = classic_desc(rgba, view2mpi, dhw, ray_dir, eye, z_dir, M, V, N, Ht, Wt, H, W, options, nullptr);
+    d.color = color; d.depth = depth; d.flags = flags_out;
+    return render_host(&d, device, Call{kHostCall, true});
 }
 
-int gmpi_mpi_render_host_ex(const gmpi_render_desc* d, int device) {
-    int rc = check_desc(d);
-    if (rc) return rc;
-    return host_render(params_from_desc(d), d->flags, device);
-}
+int gmpi_mpi_render_host_ex(const gmpi_render_desc* d, int device) { return render_host(d, device, Call{kHostCall}); }
 
 }  // extern "C"
