@@ -33,32 +33,52 @@ constexpr int kMaxBH = (((kTileH * 5) / 4 + 6 + kRowsPerOp - 1) / kRowsPerOp) * 
 constexpr int kMinBW = 56, kBWStep = 8;
 constexpr int kNumMaps = (kMaxBW - kMinBW) / kBWStep + 1;
 constexpr int kMaxPlanesStaged = 512;   // plane-constant table: 32 B per plane in shared memory
-constexpr int kStageFloats = kMaxBW * kMaxBH * 4;
 // Factored forward: box widths 64 and 96 only.  Its boxes are [row][3][bw] (colour) and [row][bw] (alpha): row pitches of 3 bw and
 // bw words, and only a pitch that is a multiple of the 32 banks keeps a warp whose 32 taps straddle two texture rows (any rotated
 // view) at one wavefront per LDS -- the expanded box [row][4][bw] has that for every bw % 8 == 0.  The 96-wide box holds footprints
 // 65..kMaxBW texels wide: wider ones take the generic body, as in the expanded ring (see staged_producer).
 constexpr int kWideBW = 96;
-constexpr int kWideStageFloats = kWideBW * kMaxBH * 4;
-constexpr size_t kStagedSmemWide = (size_t)kStages * kWideStageFloats * 4 + (size_t)kMaxPlanesStaged * 32;
-static_assert(kStagedSmemWide + 1024 <= 227 * 1024, "wide factored ring must fit one SM");
 
 // Box width of class k (tensor-map slot k).  In the factored forward's ring (wide) slot 4 holds kWideBW and slot 1 the 64-wide boxes.
 __host__ __device__ constexpr int class_width(int k, bool wide = false) { return wide && k == kNumMaps - 1 ? kWideBW : kMinBW + k * kBWStep; }
-// Width of the box staged for class width bw, element type E.  fp16 boxes (GMPI_MPI_F16) start at a multiple of 8 texels (16 bytes),
-// up to 4 texels west of the fp32 origin (a multiple of 4), so they are wider than their class: bw + 8 in the expanded ring; 96 and
+
+// MPI element types E (KeyTraits::Elem): fp32, fp16 (GMPI_MPI_F16) and uint8 (GMPI_MPI_U8, expanded only), each described once by
+// ElemTraits<E>: ElemBase derives what follows from the element size, each specialisation states the rest.  TMA moves whole 16 bytes,
+// so the tensor maps need Wt % kAlign == 0 and a staged box starts at a multiple of kAlign texels: the producer computes footprint,
+// class, mode and box origin as in fp32 (a multiple of 4 texels), then stages the box at staged_origin(origin), staged_width(class
+// width, factored) wide; StageMeta::sel bits 10-13 carry the offset between the two origins.  Class, mode and the in-box vote stay
+// those of the fp32 box, so an MPI takes the fast and the generic body exactly where its fp32 conversion does.
+template <class E, class B, CUtensorMapDataType kType>
+struct ElemBase {
+    using Elem = E;
+    using Bits = B;                                         // an element's bit pattern
+    static constexpr MapElem kMap = {kType, sizeof(E)};     // tensor-map data type and element bytes
+    static constexpr int kAlign = 16 / sizeof(E);           // texels per 16 bytes
+    // mask of the fp32 box's offset in the staged box: a compile-time 0 in fp32, whose boxes already start 16-byte aligned
+    static constexpr int kOriginMask = kAlign == 4 ? 0 : kAlign - 1;
+    static __host__ __device__ constexpr int staged_origin(int bx0) { return bx0 & ~kOriginMask; }
+};
+template <class E> struct ElemTraits;
+// fp32.  Bit tests, shared by the range check and the occupancy build: non-finite = exponent all ones (inf, NaN); out of unit =
+// outside [0, 1] and not -0.0 (negatives and NaN have larger patterns than 1.0).
+template <> struct ElemTraits<float> : ElemBase<float, uint32_t, CU_TENSOR_MAP_DATA_TYPE_FLOAT32> {
+    static __host__ __device__ constexpr int staged_width(int bw, bool) { return bw; }
+    static __device__ __forceinline__ bool nonfinite(uint32_t b) { return (b & 0x7f800000u) == 0x7f800000u; }
+    static __device__ __forceinline__ bool out_of_unit(uint32_t b) { return b > 0x3f800000u && b != 0x80000000u; }
+};
+// fp16: boxes start 0 or 4 texels west of the fp32 origin, so they are wider than their class: bw + 8 in the expanded ring; 96 and
 // 128 for the factored ring's 64 and 96 (a colour copy of kColourCopyRows rows lands at a multiple of 132 bw bytes, which must be
-// 128-byte aligned: bw % 32 == 0).  Class, mode and the in-box vote stay those of the fp32 box, so an fp16 MPI takes the fast and
-// the generic body exactly where its fp32 upcast does; only the addresses use the wider box.
-// uint8 boxes (GMPI_MPI_U8, expanded ring only) start at a multiple of 16 texels (16 bytes), up to 12 texels west of the fp32 origin,
-// and are 16-byte multiples wide that cover the class box after that shift: 80, 80, 96, 96, 112 for the classes 56 .. 88.
-template <class E>
-__host__ __device__ constexpr int staged_width(int bw, bool wide) {
-    return sizeof(E) == 1 ? (bw + 12 + 15) & ~15 : sizeof(E) == 2 ? bw + (wide ? 32 : 8) : bw;
-}
-// Offset of the fp32 box's origin from the staged box's: 0 in fp32, 0 or 4 in fp16, 0..12 in uint8 (StageMeta::sel bits 10-13).
-template <class E>
-__host__ __device__ constexpr int staged_origin(int bx0) { return sizeof(E) == 1 ? bx0 & ~15 : sizeof(E) == 2 ? bx0 & ~7 : bx0; }
+// 128-byte aligned: bw % 32 == 0).  The bit tests give each half the verdict of its fp32 upcast.
+template <> struct ElemTraits<__half> : ElemBase<__half, uint16_t, CU_TENSOR_MAP_DATA_TYPE_FLOAT16> {
+    static __host__ __device__ constexpr int staged_width(int bw, bool factored) { return bw + (factored ? 32 : 8); }
+    static __device__ __forceinline__ bool nonfinite(uint32_t b) { return (b & 0x7c00u) == 0x7c00u; }
+    static __device__ __forceinline__ bool out_of_unit(uint32_t b) { return b > 0x3c00u && b != 0x8000u; }
+};
+// uint8 (expanded ring only): boxes start 0..12 texels west of the fp32 origin and are the 16-byte multiples that cover the class box
+// after that shift: 80, 80, 96, 96, 112 for the classes 56 .. 88.  No bit tests: every code is finite and inside [0, 1].
+template <> struct ElemTraits<uint8_t> : ElemBase<uint8_t, uint8_t, CU_TENSOR_MAP_DATA_TYPE_UINT8> {
+    static __host__ __device__ constexpr int staged_width(int bw, bool) { return (bw + 12 + 15) & ~15; }
+};
 
 struct TmaMaps {
     CUtensorMap m[kNumMaps];      // expanded rgba [M*N][4][Ht][Wt] as (x, channel, y, plane), box {bw, 4, 4 rows, 1}
@@ -160,7 +180,7 @@ __device__ __forceinline__ void coords_pairs(const PlaneConst& pc, const RayPair
 // the same indices address it.  E: the element type of the box (fp16 boxes under GMPI_MPI_F16: each tap is converted to fp32).
 template <int BW, int AOFF, class E = float>
 struct BoxTaps {
-    static constexpr int SW = staged_width<E>(BW, AOFF != 0);   // staged box width (BW: the box the vote tests)
+    static constexpr int SW = ElemTraits<E>::staged_width(BW, AOFF != 0);   // staged box width (BW: the box the vote tests)
     static constexpr int RP = AOFF ? 3 * SW : 4 * SW;       // colour row pitch
     static constexpr int AP = AOFF ? SW : 4 * SW;           // alpha row pitch
     static constexpr int A0 = AOFF ? AOFF : 3 * SW;         // alpha offset from the colour index (factored: separate box)
@@ -365,42 +385,32 @@ __device__ __forceinline__ void consumer_idle_tile(uint64_t* s_full, uint64_t* s
 }
 
 // Ring geometry of a kernel: tile height, ring depth, the largest staged box and what a stage holds.
-struct FwdRing {          // the expanded forward's ring
+// The staged forward's ring on an MPI of element type E: expanded, or (kFactored) the factored forward's 64- or 96-wide boxes (see
+// kWideBW).  A stage holds the staged box (ElemTraits) of the widest class.
+template <bool kFactored, class E>
+struct FwdRing {
     static constexpr int kTileRows = kTileH, kRingStages = kStages, kBoxMaxH = kMaxBH;
-    static constexpr int kPlaneFloats = kStageFloats;      // floats of one staged plane box
-    static constexpr int kStride = kStageFloats;           // floats per ring stage
+    // elements of one staged plane box, and per ring stage
+    static constexpr int kPlaneFloats = ElemTraits<E>::staged_width(kFactored ? kWideBW : kMaxBW, kFactored) * kMaxBH * 4;
+    static constexpr int kStride = kPlaneFloats;
+    static constexpr size_t kStageBytes = (size_t)kPlaneFloats * sizeof(E);
     static constexpr bool kReverse = false;                // planes front to back; no transmittance box
     // producer sleeps between polls of a full ring (see mbar_wait_sleep).  Measured: sleeping costs the forward 1 % (a shallow
     // ring wants its producer prompt)
     static constexpr bool kSleepPolls = false;
-    static constexpr bool kWideFact = false;
+    static constexpr bool kWideFact = kFactored;
     static constexpr bool kBinaryCopies = true;            // expanded MPI: copies of 32/16/8/4 rows (see staged_producer)
+    // factored MPI: colour box = 2 copies of 22 rows.  A copy lands at row offset r * 3 * bw * sizeof(E) bytes, which must be a
+    // multiple of 128 (TMA destination alignment): any r for the staged widths 64 / 96 in fp32, 96 / 128 in fp16.
+    static constexpr int kColourCopyRows = kMaxBH / 2;
+    static_assert(kStages * kStageBytes + (size_t)kMaxPlanesStaged * 32 + 1024 <= 227 * 1024, "the ring must fit one SM");
 };
 static_assert(kMaxBH % 2 == 0 && kMaxBH / kRowsPerOp < 16, "half-height colour copies; binary digits of the chunk count");
-struct FwdRingWide {      // the factored forward's ring: 64- or 96-wide boxes (see kWideBW)
-    static constexpr int kTileRows = kTileH, kRingStages = kStages, kBoxMaxH = kMaxBH;
-    static constexpr int kPlaneFloats = kWideStageFloats, kStride = kWideStageFloats;
-    static constexpr bool kReverse = false;
-    static constexpr bool kSleepPolls = false;
-    static constexpr bool kWideFact = true;
-    static constexpr bool kBinaryCopies = true;
-    // factored MPI: colour box = 2 copies of 22 rows.  A copy lands at row offset r * 3 * bw * 4 bytes, which must be a multiple
-    // of 128 (TMA destination alignment): any r for bw = 64 / 96.
-    static constexpr int kColourCopyRows = kMaxBH / 2;
-};
-// GMPI_MPI_F16: the same rings with stages of the wider fp16 boxes (staged_width), in elements
-struct FwdRingF16 : FwdRing {
-    static constexpr int kPlaneFloats = (kMaxBW + 8) * kMaxBH * 4, kStride = kPlaneFloats;
-};
-struct FwdRingWideF16 : FwdRingWide {
-    static constexpr int kPlaneFloats = (kWideBW + 32) * kMaxBH * 4, kStride = kPlaneFloats;
-};
-// GMPI_MPI_U8 (expanded MPI only): stages of the widest uint8 box, 19712 bytes (a multiple of 128: every stage and every 4-row copy,
-// at 16 * staged width bytes per chunk, lands 128-byte aligned)
-struct FwdRingU8 : FwdRing {
-    static constexpr int kPlaneFloats = staged_width<uint8_t>(kMaxBW, false) * kMaxBH * 4, kStride = kPlaneFloats;
-};
-static_assert(FwdRingU8::kPlaneFloats % 128 == 0, "uint8 ring stages stay 128-byte aligned");
+static_assert(FwdRing<false, float>::kPlaneFloats == 15488 && FwdRing<true, float>::kPlaneFloats == 16896 &&
+              FwdRing<false, __half>::kPlaneFloats == 16896 && FwdRing<true, __half>::kPlaneFloats == 22528 &&
+              FwdRing<false, uint8_t>::kPlaneFloats == 19712, "the staged forward's ring stages");
+// uint8: a multiple of 128 bytes, so that every stage and every 4-row copy (16 * staged width bytes per chunk) lands 128-byte aligned
+static_assert(FwdRing<false, uint8_t>::kStageBytes % 128 == 0, "uint8 ring stages stay 128-byte aligned");
 
 // The expanded forward's copies of one stage: the footprint's n_chunks 4-row chunks as the binary digits of n_chunks.  Lane 0..3
 // owns the digit 8, 4, 2, 1: returns the copy's height in chunks (0: this lane issues nothing) and, in `before`, the chunks
@@ -557,7 +567,7 @@ __device__ __forceinline__ void staged_producer(const RenderParams& p, const Tma
             const int xmin = __reduce_min_sync(0xffffffffu, fx), xmax = __reduce_max_sync(0xffffffffu, fx);
             const int ymin = __reduce_min_sync(0xffffffffu, fy), ymax = __reduce_max_sync(0xffffffffu, fy);
             // TMA needs a 16-byte aligned start in the innermost dimension: the box origin is a multiple of 4 texels (fp16: the staged
-            // box starts at bxs, a multiple of 8, uint8: of 16, see staged_width)
+            // box starts at bxs, a multiple of 8, uint8: of 16, see ElemTraits)
             const int bx0 = ((xmin - 1) >> 2) << 2, by0 = ymin - 1;
             const int need_w = xmax - bx0 + 3, need_h = ymax - ymin + 4;      // +1 east/south tap, +-1 slack
             int mode = 0;
@@ -571,7 +581,7 @@ __device__ __forceinline__ void staged_producer(const RenderParams& p, const Tma
             // width class k (tensor-map slot, one-hot bit 16 + k of the header); wide rings: slot 1 = 64, slot 4 = kWideBW
             const int k = mode != 0 ? 0 : kWide ? (need_w <= 64 ? 1 : 4) : max(0, (need_w - kMinBW + kBWStep - 1) / kBWStep);
             const int bw = class_width(k, kWide);
-            const int bxs = staged_origin<E>(bx0), sw = staged_width<E>(bw, kWide);   // staged box: origin, width
+            const int bxs = ElemTraits<E>::staged_origin(bx0), sw = ElemTraits<E>::staged_width(bw, kWide);   // staged box: origin, width
             const int n_ops = mode == 0 ? (need_h + kRowsPerOp - 1) / kRowsPerOp : 0;
             const int rows = n_ops * kRowsPerOp;
             // kSkip: only a stage that takes the fast body (mode 0, plane constants in the exact range) may be skipped.  The test covers
@@ -708,11 +718,8 @@ __device__ __forceinline__ void fwd_staged_body(const RenderParams& p, const Tma
                                                 uint32_t* s_stop, OccMap occ = OccMap{}) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     E* s_buf = reinterpret_cast<E*>(smem_raw);   // the ring starts the dynamic segment (1024-byte aligned)
-    constexpr bool kHalf = sizeof(E) == 2, kU8 = sizeof(E) == 1;
-    using Ring = typename std::conditional<kFactored, typename std::conditional<kHalf, FwdRingWideF16, FwdRingWide>::type,
-                                           typename std::conditional<kHalf, FwdRingF16,
-                                                                     typename std::conditional<kU8, FwdRingU8, FwdRing>::type>::type>::type;
-    static_assert(!(kU8 && kFactored), "uint8 MPIs are expanded");
+    using Ring = FwdRing<kFactored, E>;
+    static_assert(!(kFactored && std::is_same<E, uint8_t>::value), "uint8 MPIs are expanded");
     constexpr int kStages = Ring::kRingStages;              // ring stages allocated; the expanded MPI uses ring_stages of them
     const int n_stages = kFactored ? kStages : ring_stages;
     constexpr int kRingFloats = Ring::kPlaneFloats;         // floats per ring stage
@@ -822,8 +829,8 @@ __device__ __forceinline__ void fwd_staged_body(const RenderParams& p, const Tma
                 }
                 mbar_wait(&s_full[s], ph);
                 const StageMeta mt = s_meta[s];
-                // fp16, uint8: the fp32 box's origin in the stage
-                const E* sb = s_buf + s * kRingFloats + (kU8 ? (mt.sel >> 10) & 15 : kHalf ? (mt.sel >> 10) & 7 : 0);
+                // the fp32 box's origin in the stage
+                const E* sb = s_buf + s * kRingFloats + ((mt.sel >> 10) & ElemTraits<E>::kOriginMask);
                 const int sel = mt.sel;                  // warp-uniform; the producer already folded mode and plane range in
                 bool done = warp_stopped;                // a stopped warp only waits on and releases the stage
                 if (warp_fast && !done) {
@@ -842,7 +849,7 @@ __device__ __forceinline__ void fwd_staged_body(const RenderParams& p, const Tma
                 }
                 if (!done) {
                     // ---- generic body: per-pixel range / box checks, direct sampling when not staged ----
-                    const int bw = mt.sel & 0xff, mode = (mt.sel >> 8) & 3, bws = staged_width<E>(bw, false), bw4 = 4 * bws;
+                    const int bw = mt.sel & 0xff, mode = (mt.sel >> 8) & 3, bws = ElemTraits<E>::staged_width(bw, false), bw4 = 4 * bws;
                     const float fbw2 = (float)(bw - 2), fbh2 = (float)mt.rows2;
                     const float fbx0 = (float)(mt.cx - kFloorMagicBits), fby0 = (float)(mt.cy - kFloorMagicBits);
                     const E* plane = kFactored ? nullptr : reinterpret_cast<const E*>(p.rgba) + ((size_t)m * N + i) * 4 * tex;

@@ -238,13 +238,10 @@ mpi_bwd_det_finish_kernel(const DetAcc da, float* __restrict__ g0, float* __rest
 }
 
 // ------------------------------------------------------------------------------------------
-// Range check: one streaming pass over rgba.  A float is inside [0,1] iff its bit pattern,
-// read as unsigned, is <= 0x3f800000 (or it is -0.0); NaN and negatives have larger patterns.
+// Range check: one streaming pass over rgba, testing each element's bit pattern (ElemTraits<E>::out_of_unit).
 // ------------------------------------------------------------------------------------------
-__device__ __forceinline__ bool out_of_unit(float x) {
-    const uint32_t b = __float_as_uint(x);
-    return b > 0x3f800000u && b != 0x80000000u;
-}
+using F32Elem = ElemTraits<float>;
+using F16Elem = ElemTraits<__half>;
 
 __global__ void __launch_bounds__(256)
 mpi_check_range_kernel(const float4* __restrict__ rgba4, size_t n_slabs, size_t slab4, uint32_t* flags) {
@@ -253,7 +250,8 @@ mpi_check_range_kernel(const float4* __restrict__ rgba4, size_t n_slabs, size_t 
     const size_t total = n_slabs * slab4;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
         const float4 x = __ldcs(rgba4 + i);
-        if (out_of_unit(x.x) || out_of_unit(x.y) || out_of_unit(x.z) || out_of_unit(x.w)) {
+        if (F32Elem::out_of_unit(__float_as_uint(x.x)) || F32Elem::out_of_unit(__float_as_uint(x.y)) ||
+            F32Elem::out_of_unit(__float_as_uint(x.z)) || F32Elem::out_of_unit(__float_as_uint(x.w))) {
             const size_t slab = i / slab4;
             flag |= ((slab & 3) == 3) ? (GMPI_FLAG_ALPHA_RANGE | GMPI_FLAG_RGBA_RANGE) : GMPI_FLAG_RGBA_RANGE;
         }
@@ -267,16 +265,14 @@ __global__ void mpi_check_range_scalar_kernel(const float* __restrict__ rgba, si
     uint32_t flag = 0;
     const size_t total = n_slabs * slab;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-        if (out_of_unit(__ldcs(rgba + i))) {
+        if (F32Elem::out_of_unit(__float_as_uint(__ldcs(rgba + i)))) {
             flag |= (((i / slab) & 3) == 3) ? (GMPI_FLAG_ALPHA_RANGE | GMPI_FLAG_RGBA_RANGE) : GMPI_FLAG_RGBA_RANGE;
         }
     }
     if (flag) atomicOr(flags, flag);
 }
 
-// The same check of an fp16 MPI, with the flags the fp32 check sets on its upcast: a half is inside [0,1] iff its bit pattern is
-// <= 0x3c00 (1.0) or it is -0.0; negatives, values above 1, infinities and NaN have larger patterns, as their upcasts do in fp32.
-__device__ __forceinline__ bool out_of_unit_f16(uint32_t b) { return b > 0x3c00u && b != 0x8000u; }
+// The same check of an fp16 MPI, with the flags the fp32 check sets on its upcast.
 
 __global__ void __launch_bounds__(256)
 mpi_check_range_f16_kernel(const uint4* __restrict__ rgba8, size_t n_slabs, size_t slab8, uint32_t* flags) {
@@ -288,7 +284,7 @@ mpi_check_range_f16_kernel(const uint4* __restrict__ rgba8, size_t n_slabs, size
         const uint32_t w[4] = {x.x, x.y, x.z, x.w};
         bool out = false;
 #pragma unroll
-        for (int k = 0; k < 4; ++k) out = out || out_of_unit_f16(w[k] & 0xffffu) || out_of_unit_f16(w[k] >> 16);
+        for (int k = 0; k < 4; ++k) out = out || F16Elem::out_of_unit(w[k] & 0xffffu) || F16Elem::out_of_unit(w[k] >> 16);
         if (out) flag |= (((i / slab8) & 3) == 3) ? (GMPI_FLAG_ALPHA_RANGE | GMPI_FLAG_RGBA_RANGE) : GMPI_FLAG_RGBA_RANGE;
     }
     flag = __reduce_or_sync(0xffffffffu, flag);
@@ -299,7 +295,7 @@ __global__ void mpi_check_range_f16_scalar_kernel(const unsigned short* __restri
     uint32_t flag = 0;
     const size_t total = n_slabs * slab;
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-        if (out_of_unit_f16(__ldcs(rgba + i)))
+        if (F16Elem::out_of_unit(__ldcs(rgba + i)))
             flag |= (((i / slab) & 3) == 3) ? (GMPI_FLAG_ALPHA_RANGE | GMPI_FLAG_RGBA_RANGE) : GMPI_FLAG_RGBA_RANGE;
     }
     if (flag) atomicOr(flags, flag);
@@ -513,16 +509,25 @@ static int check_call(const RenderParams& p, const Call& c) {
 
 static bool aligned16(const void* a) { return ((uintptr_t)a & 15) == 0; }
 
+// The element type E of a checked call's MPI: fp16 under GMPI_MPI_F16, uint8 under GMPI_MPI_U8 (exclusive, check_call), else fp32.
+// Returns f(ElemTraits<E>{}).
+template <class F>
+static auto with_mpi_elem(uint32_t options, F&& f) {
+    if (options & GMPI_MPI_U8) return f(ElemTraits<uint8_t>{});
+    if (options & GMPI_MPI_F16) return f(ElemTraits<__half>{});
+    return f(ElemTraits<float>{});
+}
+
 // The GMPI_WHY_* bits of every reason the TMA-staged forward is not launched for p (0 = staged): the one decision behind
-// launch_fwd, launch_bwd and the plan queries.  The tensor maps need 16-byte row strides (Wt % 4 == 0 in fp32, Wt % 8 == 0 in
-// fp16, Wt % 16 == 0 in uint8) and 16-byte aligned MPI bases (NULL counts as aligned); the plane-constant table holds
+// launch_fwd, launch_bwd and the plan queries.  The tensor maps need 16-byte row strides (Wt % ElemTraits<E>::kAlign == 0: 4 in
+// fp32, 8 in fp16, 16 in uint8) and 16-byte aligned MPI bases (NULL counts as aligned); the plane-constant table holds
 // kMaxPlanesStaged planes, and the M*N planes of all MPIs stay below 2^31; the persistent grid needs enough tiles.  Reads the sizes,
 // the fp16 and uint8 bits, the MPI pointers and the variant override, nothing else: the early-stop and training instantiations get
 // the plain forward's plan.
 static uint32_t fwd_why(const RenderParams& p) {
     uint32_t w = 0;
     if (p.N > kMaxPlanesStaged || (size_t)p.M * p.N >= ((size_t)1 << 31)) w |= GMPI_WHY_MANY_PLANES;
-    if (p.Wt % ((p.options & GMPI_MPI_U8) ? 16 : (p.options & GMPI_MPI_F16) ? 8 : 4) != 0) w |= GMPI_WHY_TEX_WIDTH;
+    if (with_mpi_elem(p.options, [&](auto e) { return p.Wt % decltype(e)::kAlign; }) != 0) w |= GMPI_WHY_TEX_WIDTH;
     if (!(factored(p) ? aligned16(p.rgb) && aligned16(p.alpha) && aligned16(p.bg_rgb) : aligned16(p.rgba))) w |= GMPI_WHY_ALIGNMENT;
     const int forced = g_fwd_variant.load(std::memory_order_relaxed);
     if (forced == 1) w |= GMPI_WHY_FORCED;
@@ -533,15 +538,12 @@ static uint32_t fwd_why(const RenderParams& p) {
 
 // Tensor maps of the MPI (expanded or factored) for the five box-width classes.  Returns 0 on success.
 // box_h, colour_rows: the ring's box height and kColourCopyRows (factored: colour copies of colour_rows rows, one alpha copy of box_h).
-// wide: the factored forward's ring (FwdRingWide) -- slot 4 holds the kWideBW-wide boxes, slot 1 the 64-wide ones, the rest unused.
-// The element type is the MPI's: fp16 under GMPI_MPI_F16, else fp32.
+// wide: the factored forward's ring (FwdRing<true, E>) -- slot 4 holds the kWideBW-wide boxes, slot 1 the 64-wide ones, the rest
+// unused.  The maps are of the MPI's element type, with its staged box widths (ElemTraits).
 static int encode_mpi_maps(TmaMaps& maps, const RenderParams& p, int box_h, int colour_rows, bool wide = false) {
-    const bool f16 = (p.options & GMPI_MPI_F16) != 0, u8 = (p.options & GMPI_MPI_U8) != 0;
-    const MapElem el = u8 ? kMapU8 : f16 ? kMapF16 : kMapF32;
+    const MapElem el = with_mpi_elem(p.options, [](auto e) { return decltype(e)::kMap; });
     for (int k = 0; k < kNumMaps; ++k) {
-        const int bw = u8    ? staged_width<uint8_t>(class_width(k, wide), wide)
-                       : f16 ? staged_width<__half>(class_width(k, wide), wide)
-                             : class_width(k, wide);
+        const int bw = with_mpi_elem(p.options, [&](auto e) { return decltype(e)::staged_width(class_width(k, wide), wide); });
         if (factored(p)) {
             if (encode_color_map(&maps.rgb[k], p.rgb, el, (uint64_t)p.M, p.Ht, p.Wt, bw, colour_rows) != 0) return -1;
             if (p.bg_rgb && encode_color_map(&maps.bg[k], p.bg_rgb, el, (uint64_t)p.M, p.Ht, p.Wt, bw, colour_rows) != 0) return -1;
@@ -684,12 +686,13 @@ static int persistent_grid(Launch& l, int tile_h) {
     return GMPI_OK;
 }
 
-// Dynamic shared memory of a staged forward kernel: its ring and the plane-constant table.  fac: the kernel's kFactored; f16, u8: its
-// MPI is fp16 (the rings of FwdRingF16 / FwdRingWideF16) or uint8 (FwdRingU8, expanded only)
-static size_t fwd_staged_smem(bool fac, int stages, bool f16, bool u8) {
-    const size_t ring = u8    ? (size_t)stages * FwdRingU8::kPlaneFloats
-                        : f16 ? (size_t)(fac ? kStages * FwdRingWideF16::kPlaneFloats : stages * FwdRingF16::kPlaneFloats) * 2
-                              : (size_t)(fac ? kStages * kWideStageFloats : stages * kStageFloats) * 4;
+// Dynamic shared memory of the staged forward kernel of p: its ring (FwdRing of the kernel's kFactored and the MPI's element type;
+// stages of them when expanded, kStages when factored) and the plane-constant table.
+static size_t fwd_staged_smem(const RenderParams& p, int stages) {
+    const size_t ring = with_mpi_elem(p.options, [&](auto e) {
+        using E = typename decltype(e)::Elem;
+        return factored(p) ? kStages * FwdRing<true, E>::kStageBytes : stages * FwdRing<false, E>::kStageBytes;
+    });
     return ring + (size_t)kMaxPlanesStaged * 32;
 }
 
@@ -732,19 +735,19 @@ static int read_stage_stats(StageStats s, unsigned long long* skipped, unsigned 
 // kernel when fwd_why(p) == 0 and its tensor maps encode, else the direct kernel; a forced staged variant fails instead.
 static int fwd_launch(Launch& l, const uint32_t* occ) {
     const RenderParams& p = l.p;
-    const bool fac = factored(p), f16 = (p.options & GMPI_MPI_F16) != 0, u8 = (p.options & GMPI_MPI_U8) != 0;
+    const bool fac = factored(p);
     uint32_t key = ((p.options & GMPI_ALIGN_CORNERS) ? kKeyAC : 0) | ((p.options & GMPI_EARLY_STOP) ? kKeyES : 0) |
-                   (f16 ? kKeyF16 : 0) | (u8 ? kKeyU8 : 0);
+                   ((p.options & GMPI_MPI_F16) ? kKeyF16 : 0) | ((p.options & GMPI_MPI_U8) ? kKeyU8 : 0);
     int rc = GMPI_OK;
     if (fwd_why(p) == 0) {
-        if (encode_mpi_maps(l.maps, p, kMaxBH, FwdRingWide::kColourCopyRows, fac) == 0) {
+        if (encode_mpi_maps(l.maps, p, kMaxBH, FwdRing<true, float>::kColourCopyRows, fac) == 0) {
             int l2 = 0;
             if ((rc = persistent_grid(l, kTileH)) != 0) return rc;
             if ((rc = device_attr(cudaDevAttrL2CacheSize, &l2)) != 0) return rc;
             const int forced_stages = g_fwd_stages.load(std::memory_order_relaxed);
             l.ints[2] = forced_stages ? forced_stages : fwd_ring_stages(p, l2);
             l.block = dim3(kStagedThreads);
-            l.smem = fwd_staged_smem(fac, l.ints[2], f16, u8);
+            l.smem = fwd_staged_smem(p, l.ints[2]);
             l.arg(&l.ints[2]);
             key |= kKeyStaged | (fac ? kKeyFac : 0) | (occ ? kKeySkip : 0) | (p.transmittance ? kKeyEmit : 0);
             l.key = key;
@@ -812,7 +815,7 @@ static int bwd_launch(Launch& l, bool box, bool det) {
     uint32_t key = kKeyBwd | (det ? kKeyDet : 0) | ((p.options & GMPI_ALIGN_CORNERS) ? kKeyAC : 0);
     if (box) {
         if (encode_mpi_maps(l.maps, p, kBwdMaxBH, BwdRing::kColourCopyRows) != 0) return fail(GMPI_ERR_CUDA, "cuTensorMapEncodeTiled failed");
-        if (encode_slab_map(&l.maps.t, p.transmittance, kMapF32, (uint64_t)p.V * p.N, p.H, p.W, kTileW, kBwdTileH, 1) != 0)
+        if (encode_slab_map(&l.maps.t, p.transmittance, ElemTraits<float>::kMap, (uint64_t)p.V * p.N, p.H, p.W, kTileW, kBwdTileH, 1) != 0)
             return fail(GMPI_ERR_CUDA, "cuTensorMapEncodeTiled (transmittance) failed");
         if (int rc = persistent_grid(l, kBwdTileH)) return rc;
         l.block = dim3(kBwdThreads);
@@ -986,6 +989,13 @@ static gmpi_render_desc classic_desc(const float* rgba, const int32_t* view2mpi,
     d.rgba = rgba; d.view2mpi = view2mpi; d.dhw = dhw; d.ray_dir = ray_dir; d.eye = eye; d.z_dir = z_dir;
     return d;
 }
+
+// The occupancy-map build of an MPI (mpi_kernel_keys.cuh) by element type and form, and whether it takes the range check's flags (the
+// expanded fp32 and fp16 builds set them from the same loads; uint8 MPIs are expanded, and every code is inside [0, 1]).
+struct OccBuild { const void* kernel; bool range_flags; };
+static OccBuild occ_build(ElemTraits<float>, bool fac) { return {fac ? (const void*)gmpi_occ_factored_f32 : (const void*)gmpi_occ_expanded_f32, !fac}; }
+static OccBuild occ_build(ElemTraits<__half>, bool fac) { return {fac ? (const void*)gmpi_occ_factored_f16 : (const void*)gmpi_occ_expanded_f16, !fac}; }
+static OccBuild occ_build(ElemTraits<uint8_t>, bool) { return {(const void*)gmpi_occ_expanded_u8, false}; }
 
 // The range check of an fp32 or (f16) fp16 rgba: 16-byte loads when every slab is a whole number of them on an aligned base.
 static int check_range(const void* rgba, bool f16, int M, int N, int Ht, int Wt, uint32_t* flags, cudaStream_t st) {
@@ -1170,35 +1180,27 @@ int gmpi_mpi_build_occupancy(const gmpi_render_desc* d, void* occ, size_t bytes)
     if (rc) return rc;
     const int words = occ_words(p.Wt), rows = occ_rows(p.Ht);
     if (rows > 65535) return fail(GMPI_ERR_UNSUPPORTED, "Ht=%d exceeds the occupancy build's grid (%d texel rows)", p.Ht, 65535 * kOccB);
-    const bool f16 = (p.options & GMPI_MPI_F16) != 0, u8 = (p.options & GMPI_MPI_U8) != 0;
+    const OccBuild build = with_mpi_elem(p.options, [&](auto e) { return occ_build(e, factored(p)); });
     const int M = p.M, N = p.N, Ht = p.Ht, Wt = p.Wt;
     cudaLaunchConfig_t cfg = {};
     cfg.blockDim = dim3(32 * kOccB);
     cfg.stream = (cudaStream_t)d->stream;
     uint32_t* map = static_cast<uint32_t*>(occ);
-    if (u8) {
-        // every code is inside [0, 1]: no range bits to set, so the flags are not read
-        const long long P = (long long)M * N;
-        if (P > 0x7fffffffLL) return fail(GMPI_ERR_UNSUPPORTED, "%lld planes exceed the occupancy build (2^31)", P);
-        const int planes = (int)P;
-        cfg.gridDim = dim3(words, rows, planes < 65535 ? planes : 65535);
-        const void* rgba = p.rgba;
-        void* args[] = {&rgba, &map, (void*)&planes, (void*)&Ht, (void*)&Wt, (void*)&words, (void*)&rows};
-        GMPI_CUDA_OK(cudaLaunchKernelExC(&cfg, (const void*)gmpi_occ_expanded_u8, args));
-    } else if (factored(p)) {
+    if (factored(p)) {
         cfg.gridDim = dim3(words, rows, M < 65535 ? M : 65535);
         const void *rgb = p.rgb, *bg = p.bg_rgb, *alpha = p.alpha;
         void* args[] = {&rgb, &bg, &alpha, &map, (void*)&M, (void*)&N, (void*)&Ht, (void*)&Wt, (void*)&words, (void*)&rows};
-        GMPI_CUDA_OK(cudaLaunchKernelExC(&cfg, f16 ? (const void*)gmpi_occ_factored_f16 : (const void*)gmpi_occ_factored_f32, args));
+        GMPI_CUDA_OK(cudaLaunchKernelExC(&cfg, build.kernel, args));
     } else {
         const long long P = (long long)M * N;
         if (P > 0x7fffffffLL) return fail(GMPI_ERR_UNSUPPORTED, "%lld planes exceed the occupancy build (2^31)", P);
         const int planes = (int)P;
         cfg.gridDim = dim3(words, rows, planes < 65535 ? planes : 65535);
         const void* rgba = p.rgba;
-        uint32_t* flags = p.flags;      // the range check's bits, from the same loads
+        uint32_t* flags = p.flags;
         void* args[] = {&rgba, &map, &flags, (void*)&planes, (void*)&Ht, (void*)&Wt, (void*)&words, (void*)&rows};
-        GMPI_CUDA_OK(cudaLaunchKernelExC(&cfg, f16 ? (const void*)gmpi_occ_expanded_f16 : (const void*)gmpi_occ_expanded_f32, args));
+        void* args_no_flags[] = {&rgba, &map, (void*)&planes, (void*)&Ht, (void*)&Wt, (void*)&words, (void*)&rows};
+        GMPI_CUDA_OK(cudaLaunchKernelExC(&cfg, build.kernel, build.range_flags ? args : args_no_flags));
     }
     return GMPI_OK;
 }
@@ -1402,10 +1404,10 @@ static int host_render_locked(HostCache& c, const RenderParams& h) {
     const size_t tex = (size_t)h.Ht * h.Wt, img = (size_t)H * W;
     const bool fac = factored(h), video = h.video_rgb != nullptr;
     // one slot = one MPI: expanded [N,4,tex], or factored rgb [3,tex] | bg [3,tex] | alpha [N,tex]
-    // (offsets in MPI elements: fp16 under GMPI_MPI_F16, uint8 under GMPI_MPI_U8, else fp32)
-    const size_t esz = (h.options & GMPI_MPI_U8) ? 1 : (h.options & GMPI_MPI_F16) ? 2 : 4;
+    // (offsets in MPI elements, of ebytes bytes each)
+    const size_t ebytes = with_mpi_elem(h.options, [](auto e) { return sizeof(typename decltype(e)::Elem); });
     const size_t o_bg = 3 * tex, o_alpha = h.bg_rgb ? 6 * tex : 3 * tex;
-    const size_t mpi_bytes = esz * (fac ? o_alpha + (size_t)N * tex : (size_t)N * 4 * tex);
+    const size_t mpi_bytes = ebytes * (fac ? o_alpha + (size_t)N * tex : (size_t)N * 4 * tex);
     auto up = [](size_t x) { return (x + 255) & ~(size_t)255; };
     const size_t o_dhw = 0, o_ray = o_dhw + up(sizeof(float) * (size_t)M * N * 3),
                  o_eye = o_ray + up(h.cam ? sizeof(float) * (size_t)V * 16 : sizeof(float) * (size_t)V * 3 * img),
@@ -1458,12 +1460,12 @@ static int host_render_locked(HostCache& c, const RenderParams& h) {
         if (v1 == v0) continue;
         if (used[slot]) GMPI_CUDA_OK(cudaStreamWaitEvent(s_copy, c.ev_free[slot], 0));
         char* d_mpi = reinterpret_cast<char*>(c.mpi[slot]);
-        auto src = [esz](const float* base, size_t elems) { return reinterpret_cast<const char*>(base) + esz * elems; };
+        auto src = [ebytes](const float* base, size_t elems) { return reinterpret_cast<const char*>(base) + ebytes * elems; };
         if (fac) {
-            GMPI_CUDA_OK(cudaMemcpyAsync(d_mpi, src(h.rgb, (size_t)m * 3 * tex), esz * 3 * tex, cudaMemcpyHostToDevice, s_copy));
+            GMPI_CUDA_OK(cudaMemcpyAsync(d_mpi, src(h.rgb, (size_t)m * 3 * tex), ebytes * 3 * tex, cudaMemcpyHostToDevice, s_copy));
             if (h.bg_rgb)
-                GMPI_CUDA_OK(cudaMemcpyAsync(d_mpi + esz * o_bg, src(h.bg_rgb, (size_t)m * 3 * tex), esz * 3 * tex, cudaMemcpyHostToDevice, s_copy));
-            GMPI_CUDA_OK(cudaMemcpyAsync(d_mpi + esz * o_alpha, src(h.alpha, (size_t)m * N * tex), esz * (size_t)N * tex, cudaMemcpyHostToDevice, s_copy));
+                GMPI_CUDA_OK(cudaMemcpyAsync(d_mpi + ebytes * o_bg, src(h.bg_rgb, (size_t)m * 3 * tex), ebytes * 3 * tex, cudaMemcpyHostToDevice, s_copy));
+            GMPI_CUDA_OK(cudaMemcpyAsync(d_mpi + ebytes * o_alpha, src(h.alpha, (size_t)m * N * tex), ebytes * (size_t)N * tex, cudaMemcpyHostToDevice, s_copy));
         } else {
             GMPI_CUDA_OK(cudaMemcpyAsync(d_mpi, src(h.rgba, (size_t)m * N * 4 * tex), mpi_bytes, cudaMemcpyHostToDevice, s_copy));
         }
@@ -1471,7 +1473,7 @@ static int host_render_locked(HostCache& c, const RenderParams& h) {
         GMPI_CUDA_OK(cudaStreamWaitEvent(s_run, c.ev_in[slot], 0));
         RenderParams p = h;
         p.M = 1; p.V = v1 - v0;
-        const auto at = [d_mpi, esz](size_t elems) { return reinterpret_cast<const float*>(d_mpi + esz * elems); };
+        const auto at = [d_mpi, ebytes](size_t elems) { return reinterpret_cast<const float*>(d_mpi + ebytes * elems); };
         if (fac) { p.rgb = at(0); p.bg_rgb = h.bg_rgb ? at(o_bg) : nullptr; p.alpha = at(o_alpha); p.rgba = nullptr; }
         else p.rgba = at(0);
         p.view2mpi = d_v2m; p.dhw = d_dhw + (size_t)m * N * 3;

@@ -14,25 +14,15 @@
 
 namespace gmpi {
 
-// Texel tests on bit patterns: U = uint32_t (fp32 MPI) or uint16_t (fp16 MPI).
-//   occupied alpha   any pattern but +0 (-0.0 and NaN count as occupied)
-//   non-finite       exponent all ones (inf, NaN)
-//   out_of_unit      the range check's test (mpi_check_range_kernel / _f16): outside [0,1] and not -0.0, NaN included
-template <class U> struct Bits;
-template <> struct Bits<uint32_t> {
-    static __device__ __forceinline__ bool nonfinite(uint32_t b) { return (b & 0x7f800000u) == 0x7f800000u; }
-    static __device__ __forceinline__ bool out_of_unit(uint32_t b) { return b > 0x3f800000u && b != 0x80000000u; }
-};
-template <> struct Bits<uint16_t> {
-    static __device__ __forceinline__ bool nonfinite(uint32_t b) { return (b & 0x7c00u) == 0x7c00u; }
-    static __device__ __forceinline__ bool out_of_unit(uint32_t b) { return b > 0x3c00u && b != 0x8000u; }
-};
+// A texel is occupied when its alpha is any bit pattern but +0 (-0.0 and NaN count as occupied) or a colour value is not finite
+// (ElemTraits<E>::nonfinite, on the element's bit pattern U).
 
 // Expanded MPI [P = M*N][4][Ht][Wt]: grid (words, block rows, planes in steps of gridDim.z).  flags != NULL: also the range-check bits
-// gmpi_mpi_check_range(_f16) sets, from the same loads.
-template <class U>
+// gmpi_mpi_check_range(_f16) sets, from the same loads and with its test (ElemTraits<E>::out_of_unit).
+template <class E, class U = typename ElemTraits<E>::Bits>
 __device__ __forceinline__ void occ_expanded(const U* __restrict__ rgba, uint32_t* __restrict__ occ, uint32_t* flags, int P, int Ht,
                                              int Wt, int words, int rows) {
+    using T = ElemTraits<E>;
     __shared__ uint32_t s_w[kOccThreads / 32];
     const size_t tex = (size_t)Ht * Wt;
     const int x = blockIdx.x * kOccThreads + threadIdx.x, y0 = blockIdx.y * kOccB;
@@ -44,9 +34,9 @@ __device__ __forceinline__ void occ_expanded(const U* __restrict__ rgba, uint32_
             for (int y = y0; y < y0 + kOccB && y < Ht; ++y) {
                 const size_t o = (size_t)y * Wt;
                 const uint32_t c0 = __ldcs(base + o), c1 = __ldcs(base + tex + o), c2 = __ldcs(base + 2 * tex + o), a = __ldcs(base + 3 * tex + o);
-                occupied = occupied || a != 0u || Bits<U>::nonfinite(c0) || Bits<U>::nonfinite(c1) || Bits<U>::nonfinite(c2);
-                if (Bits<U>::out_of_unit(c0) || Bits<U>::out_of_unit(c1) || Bits<U>::out_of_unit(c2)) flag |= GMPI_FLAG_RGBA_RANGE;
-                if (Bits<U>::out_of_unit(a)) flag |= GMPI_FLAG_RGBA_RANGE | GMPI_FLAG_ALPHA_RANGE;
+                occupied = occupied || a != 0u || T::nonfinite(c0) || T::nonfinite(c1) || T::nonfinite(c2);
+                if (T::out_of_unit(c0) || T::out_of_unit(c1) || T::out_of_unit(c2)) flag |= GMPI_FLAG_RGBA_RANGE;
+                if (T::out_of_unit(a)) flag |= GMPI_FLAG_RGBA_RANGE | GMPI_FLAG_ALPHA_RANGE;
             }
         }
         store_occ_word(occupied, occ + ((size_t)pl * rows + blockIdx.y) * words + blockIdx.x, s_w);
@@ -60,9 +50,10 @@ __device__ __forceinline__ void occ_expanded(const U* __restrict__ rgba, uint32_
 // Factored MPI: colour rgb [M][3][Ht][Wt] shared by the planes (bg [M][3][Ht][Wt]: the last plane's own, nullable), alpha
 // [M][N][Ht][Wt].  Grid (words, block rows, MPIs in steps of gridDim.z).  The colour's finiteness is read once per MPI (an 8-bit row
 // mask per thread) and applied to every plane; per plane only alpha is read.
-template <class U>
+template <class E, class U = typename ElemTraits<E>::Bits>
 __device__ __forceinline__ void occ_factored(const U* __restrict__ rgb, const U* __restrict__ bg, const U* __restrict__ alpha,
                                              uint32_t* __restrict__ occ, int M, int N, int Ht, int Wt, int words, int rows) {
+    using T = ElemTraits<E>;
     __shared__ uint32_t s_w[kOccThreads / 32];
     const size_t tex = (size_t)Ht * Wt;
     const int x = blockIdx.x * kOccThreads + threadIdx.x, y0 = blockIdx.y * kOccB;
@@ -71,9 +62,9 @@ __device__ __forceinline__ void occ_factored(const U* __restrict__ rgb, const U*
         if (x < Wt) {
             for (int r = 0; r < kOccB && y0 + r < Ht; ++r) {
                 const size_t o = (size_t)m * 3 * tex + (size_t)(y0 + r) * Wt + x;
-                if (Bits<U>::nonfinite(__ldg(rgb + o)) || Bits<U>::nonfinite(__ldg(rgb + o + tex)) || Bits<U>::nonfinite(__ldg(rgb + o + 2 * tex)))
+                if (T::nonfinite(__ldg(rgb + o)) || T::nonfinite(__ldg(rgb + o + tex)) || T::nonfinite(__ldg(rgb + o + 2 * tex)))
                     nf_rgb |= 1u << r;
-                if (bg && (Bits<U>::nonfinite(__ldg(bg + o)) || Bits<U>::nonfinite(__ldg(bg + o + tex)) || Bits<U>::nonfinite(__ldg(bg + o + 2 * tex))))
+                if (bg && (T::nonfinite(__ldg(bg + o)) || T::nonfinite(__ldg(bg + o + tex)) || T::nonfinite(__ldg(bg + o + 2 * tex))))
                     nf_bg |= 1u << r;
             }
         }
@@ -97,21 +88,21 @@ extern "C" {
 
 __global__ void __launch_bounds__(kOccThreads)
 gmpi_occ_expanded_f32(const uint32_t* rgba, uint32_t* occ, uint32_t* flags, int P, int Ht, int Wt, int words, int rows) {
-    occ_expanded<uint32_t>(rgba, occ, flags, P, Ht, Wt, words, rows);
+    occ_expanded<float>(rgba, occ, flags, P, Ht, Wt, words, rows);
 }
 __global__ void __launch_bounds__(kOccThreads)
 gmpi_occ_expanded_f16(const uint16_t* rgba, uint32_t* occ, uint32_t* flags, int P, int Ht, int Wt, int words, int rows) {
-    occ_expanded<uint16_t>(rgba, occ, flags, P, Ht, Wt, words, rows);
+    occ_expanded<__half>(rgba, occ, flags, P, Ht, Wt, words, rows);
 }
 __global__ void __launch_bounds__(kOccThreads)
 gmpi_occ_factored_f32(const uint32_t* rgb, const uint32_t* bg, const uint32_t* alpha, uint32_t* occ, int M, int N, int Ht, int Wt,
                       int words, int rows) {
-    occ_factored<uint32_t>(rgb, bg, alpha, occ, M, N, Ht, Wt, words, rows);
+    occ_factored<float>(rgb, bg, alpha, occ, M, N, Ht, Wt, words, rows);
 }
 __global__ void __launch_bounds__(kOccThreads)
 gmpi_occ_factored_f16(const uint16_t* rgb, const uint16_t* bg, const uint16_t* alpha, uint32_t* occ, int M, int N, int Ht, int Wt,
                       int words, int rows) {
-    occ_factored<uint16_t>(rgb, bg, alpha, occ, M, N, Ht, Wt, words, rows);
+    occ_factored<__half>(rgb, bg, alpha, occ, M, N, Ht, Wt, words, rows);
 }
 
 // stages the last skipping launch armed empty (gmpi_debug_fwd_skip_stats, through OccMap::skipped)

@@ -85,17 +85,13 @@ inline EncodeTiledFn get_encode_fn() {
     return fn;
 }
 
-// Element type of a tensor map: its CUtensorMapDataType and size in bytes (fp32, the fp16 MPI of GMPI_MPI_F16, the uint8 MPI of
-// GMPI_MPI_U8).
+// Element type of a tensor map: its CUtensorMapDataType and size in bytes (the MPI's: ElemTraits<E>::kMap, mpi_fwd_staged.cuh).
 struct MapElem {
     CUtensorMapDataType type;
     cuuint64_t bytes;
 };
-constexpr MapElem kMapF32 = {CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4}, kMapF16 = {CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2},
-                  kMapU8 = {CU_TENSOR_MAP_DATA_TYPE_UINT8, 1};
 
-// Returns 0 on success.  Requires 16-byte row strides (Wt % 4 == 0 in fp32, Wt % 8 == 0 in fp16, Wt % 16 == 0 in uint8) and a
-// 16-byte aligned base.
+// Returns 0 on success.  Requires 16-byte row strides (Wt a multiple of 16 / el.bytes) and a 16-byte aligned base.
 inline int encode_slab_map(CUtensorMap* out, const void* base, MapElem el, uint64_t n_slabs, int Ht, int Wt, int bw, int bh, int bc) {
     EncodeTiledFn fn = get_encode_fn();
     if (!fn) return -1;

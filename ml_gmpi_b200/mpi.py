@@ -132,6 +132,15 @@ def _render_fwd(d, occ: Optional["Occupancy"], device):
             _lib.check(lib.gmpi_mpi_render_fwd_ex(ctypes.byref(d)))
 
 
+def _renders_natively(mpi, V, H, W, options, native):
+    """Whether the MPI tensors `mpi` = [rgba, rgb, alpha, bg_rgb] (None where absent) render natively with the element-type option
+    `native` (OPT_MPI_F16, OPT_MPI_U8): when they get the kernel plan a fresh fp32 allocation of their shape would get, so that the
+    output is bitwise the render of their fp32 conversion."""
+    fp32 = _mpi_desc(mpi, V, H, W, options)
+    fp32.rgba = fp32.rgb = fp32.alpha = fp32.bg_rgb = None     # a fresh, aligned allocation
+    return _lib.fwd_plan(fp32)[0] == _lib.fwd_plan(_mpi_desc(mpi, V, H, W, options | native))[0]
+
+
 def _half_mpi(mpi, V, H, W, options):
     """The MPI tensors `mpi` = [rgba, rgb, alpha, bg_rgb] (None where absent) as contiguous fp16 when the call renders them natively
     (GMPI_MPI_F16), else None (the call upcasts them to fp32, as it always did).  Native when every MPI tensor is torch.float16,
@@ -144,9 +153,7 @@ def _half_mpi(mpi, V, H, W, options):
         return None
     # detached: under no_grad an fp16 tensor may still carry requires_grad, and the native path has no backward
     half = [None if t is None else t.detach().contiguous() for t in mpi]
-    upcast = _mpi_desc(half, V, H, W, options)
-    upcast.rgba = upcast.rgb = upcast.alpha = upcast.bg_rgb = None     # the upcast is a fresh, aligned allocation
-    return half if _lib.fwd_plan(upcast)[0] == _lib.fwd_plan(_mpi_desc(half, V, H, W, options | _lib.OPT_MPI_F16))[0] else None
+    return half if _renders_natively(half, V, H, W, options, _lib.OPT_MPI_F16) else None
 
 
 _unorm8_tables = {}
@@ -178,9 +185,7 @@ def _unorm8_mpi(mpi, V, H, W, options):
     render of that conversion either way."""
     _check_unorm8(mpi)
     u8 = [mpi[0].contiguous(), None, None, None]
-    fp32 = _mpi_desc(u8, V, H, W, options)
-    fp32.rgba = None                     # a fresh, aligned allocation
-    if _lib.fwd_plan(fp32)[0] == _lib.fwd_plan(_mpi_desc(u8, V, H, W, options | _lib.OPT_MPI_U8))[0]:
+    if _renders_natively(u8, V, H, W, options, _lib.OPT_MPI_U8):
         return u8, options | _lib.OPT_MPI_U8
     return [unorm8_to_float(u8[0]), None, None, None], options
 

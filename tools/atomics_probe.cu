@@ -84,7 +84,7 @@ int main() {
     // (3) TMA reduce-add
     CUtensorMap map;
     const int bw = 72, rows = 36;
-    if (encode_plane_map(&map, g, kMapF32, N, H, W, bw, rows) != 0) { printf("encode failed\n"); return 1; }
+    if (encode_plane_map(&map, g, MapElem{CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4}, N, H, W, bw, rows) != 0) { printf("encode failed\n"); return 1; }
     cudaFuncSetAttribute(k_tma_reduce, cudaFuncAttributeMaxDynamicSharedMemorySize, bw * rows * 16);
     k_tma_reduce<<<sms, 128, bw * rows * 16>>>(map, 4, 16, 35, bw, rows);
     cudaEventRecord(e0); k_tma_reduce<<<sms, 128, bw * rows * 16>>>(map, N, 16, 35, bw, rows); cudaEventRecord(e1); cudaEventSynchronize(e1);

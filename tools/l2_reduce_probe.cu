@@ -105,7 +105,7 @@ int main() {
     {
         CUtensorMap map;
         const int bw = 64, rows = 32;
-        if (encode_plane_map(&map, g, kMapF32, N, H, W, bw, rows) != 0) { printf("encode failed\n"); return 1; }
+        if (encode_plane_map(&map, g, MapElem{CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4}, N, H, W, bw, rows) != 0) { printf("encode failed\n"); return 1; }
         cudaFuncSetAttribute(k_tma_reduce, cudaFuncAttributeMaxDynamicSharedMemorySize, bw * rows * 16);
         timeit("P5 TMA reduce-add, disjoint 64x32x4 boxes, every element once",
                [&] { k_tma_reduce<<<sms, 128, bw * rows * 16>>>(map, N, W / bw, H / rows, bw, rows); }, (double)kElems);
@@ -113,7 +113,7 @@ int main() {
     {
         CUtensorMap map;
         const int bw = 72, rows = 36;       // overlapping, as a footprint-fitted gradient box would be (origin step 64x30)
-        if (encode_plane_map(&map, g, kMapF32, N, H, W, bw, rows) != 0) { printf("encode failed\n"); return 1; }
+        if (encode_plane_map(&map, g, MapElem{CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4}, N, H, W, bw, rows) != 0) { printf("encode failed\n"); return 1; }
         cudaFuncSetAttribute(k_tma_reduce, cudaFuncAttributeMaxDynamicSharedMemorySize, bw * rows * 16);
         timeit("P5b TMA reduce-add, 72x36x4 boxes stepping by 72x36 (unaligned rows)",
                [&] { k_tma_reduce<<<sms, 128, bw * rows * 16>>>(map, N, W / bw, H / rows, bw, rows); }, (double)N * (W / bw) * (H / rows) * bw * rows * 4);

@@ -39,8 +39,8 @@ int main(int argc, char** argv) {
     const int bw = (var & 4) ? 64 : 72, rows = 4;
     CUtensorMap map; memset(&map, 0, sizeof(map));
     int rank = (var & 16) ? 4 : ((var & 2) ? 2 : 3), r, bytes;
-    if (rank == 4) { r = encode_plane_map(&map, d, kMapF32, S / 4, Ht, Wt, bw, rows); bytes = bw * 4 * rows * 4; }
-    else if (rank == 3) { r = encode_slab_map(&map, d, kMapF32, S, Ht, Wt, bw, rows, 4); bytes = bw * rows * 4 * 4; }
+    if (rank == 4) { r = encode_plane_map(&map, d, MapElem{CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4}, S / 4, Ht, Wt, bw, rows); bytes = bw * 4 * rows * 4; }
+    else if (rank == 3) { r = encode_slab_map(&map, d, MapElem{CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4}, S, Ht, Wt, bw, rows, 4); bytes = bw * rows * 4 * 4; }
     else {
         EncodeTiledFn fn = get_encode_fn();
         cuuint64_t dims[2] = {(cuuint64_t)Wt, (cuuint64_t)Ht * S}; cuuint64_t strides[1] = {(cuuint64_t)Wt * 4};

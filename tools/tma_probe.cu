@@ -88,7 +88,7 @@ int main(int argc, char** argv) {
         if (only >= 0 && (int)ci != only) continue;
         auto c = cfgs[ci];
         CUtensorMap map;
-        int r = encode_slab_map(&map, d, kMapF32, (uint64_t)N * 4, Ht, Wt, c.bw, c.rc, 4);
+        int r = encode_slab_map(&map, d, MapElem{CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4}, (uint64_t)N * 4, Ht, Wt, c.bw, c.rc, 4);
         if (r) { printf("encode failed %d\n", r); continue; }
         ProbeParams p{N, Ht, Wt, c.tw, c.th, c.bw, ((c.bh + c.rc - 1) / c.rc) * c.rc, c.rc, Wt / c.tw, Ht / c.th, c.lds};
         size_t smem = (size_t)kStages * p.bw * p.bh * 4 * 4;
