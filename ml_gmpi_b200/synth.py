@@ -48,18 +48,35 @@ def make_poses(n_views, img, seed=1234, yaws=None, pitches=None, device="cpu"):
 
 
 def make_case(*, n_planes, tex, img, n_mpi, views_per_mpi=1, seed=1234, device="cpu", last_alpha_one=False,
-              yaws=None, pitches=None, rgba=True) -> Case:
+              yaws=None, pitches=None, rgba=True, alpha="uniform") -> Case:
+    """alpha: "uniform" (U(0, 1) on every plane) or "equal_weight" (equal_weight_alpha, whose last plane is opaque)."""
+    assert alpha in ("uniform", "equal_weight"), alpha
     V = n_mpi * views_per_mpi
     ray_dir, eye, z_dir, c2w, yaws, pitches = make_poses(V, img, seed, yaws, pitches, device)
     gen = torch.Generator(device=device).manual_seed(seed)
     t = None
     if rgba:
         t = torch.rand((n_mpi, n_planes, 4, tex, tex), generator=gen, device=device, dtype=torch.float32)
+        if alpha == "equal_weight":
+            t[:, :, 3] = equal_weight_alpha((n_mpi, n_planes, tex, tex), gen, device)
         if last_alpha_one:
             t[:, -1, 3] = 1.0      # production MPIs: networks_cond_on_pos_enc.py:1307-1310
     dhw = ffhq_dhw(n_planes).to(device).unsqueeze(0).expand(n_mpi, -1, -1).contiguous()
     v2m = torch.arange(n_mpi, dtype=torch.int32, device=device).repeat_interleave(views_per_mpi)
     return Case(t, dhw, v2m, ray_dir, eye, z_dir, c2w, yaws, pitches)
+
+
+def equal_weight_alpha(shape, generator, device="cpu") -> torch.Tensor:
+    """[..., N, Ht, Wt] alpha under which every plane carries weight: U(0, 1) alpha hides the planes past ~25 (transmittance
+    falls as e^-i), so a render or gradient check at 96 planes could not see a kernel error on them.  Plane i gets
+    min(1, u * 2 / (N - i)), u ~ U(0, 1) per texel (E[alpha_i] = 1 / (N - i), hence an expected compositing weight of 1 / N for
+    every plane), and the last plane is opaque, as in a GMPI MPI."""
+    n = shape[-3]
+    u = torch.rand(shape, generator=generator, device=device, dtype=torch.float32)
+    scale = 2.0 / torch.arange(n, 0, -1, device=device, dtype=torch.float32)
+    alpha = torch.clamp(u * scale[:, None, None], max=1.0)
+    alpha[..., -1, :, :] = 1.0
+    return alpha
 
 
 def head_alpha(n_planes: int, tex: int, device="cpu") -> torch.Tensor:

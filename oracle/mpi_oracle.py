@@ -127,6 +127,37 @@ def coords(view2mpi, dhw, ray_dir, eye, Ht, Wt, align_corners=True):
     return out
 
 
+FWD_TILE = (30, 44)    # staged forward: tile rows kTileH, box rows kMaxBH (csrc/mpi_fwd_staged.cuh)
+BWD_TILE = (24, 36)    # box backward: kBwdTileH, kBwdMaxBH (csrc/mpi_bwd_box.cuh)
+
+
+def footprints(view2mpi, dhw, ray_dir, eye, Ht, Wt, align_corners=True, tile=FWD_TILE, wide=False):
+    """The staged producer's box of every (view, tile, plane) stage (staged_producer, csrc/mpi_fwd_staged.cuh), computed as it
+    does from coords() of each 64 x tile[0] pixel tile's four corner pixels (clamped into the image).  -> dict of int64 arrays
+    [V, tiles_y, tiles_x, N]: bx0 (box origin, a multiple of 4), need_w, need_h, mode (0 staged, 1 nothing under the tile, 2 the
+    generic body) and cls (the box width of the class: 56..88 in steps of 8, or 64 / 96 in the factored forward's wide ring;
+    0 where mode != 0).  tile: (tile rows, box rows) of the forward (FWD_TILE) or the backward (BWD_TILE)."""
+    tile_h, max_bh = tile
+    V, _, H, W = ray_dir.shape
+    px, py = np.arange(0, W, 64), np.arange(0, H, tile_h)
+    xs = np.stack([px, np.minimum(px + 63, W - 1)], -1).reshape(-1)
+    ys = np.stack([py, np.minimum(py + tile_h - 1, H - 1)], -1).reshape(-1)
+    corners = np.ascontiguousarray(np.asarray(ray_dir)[:, :, ys][:, :, :, xs])
+    c = coords(view2mpi, dhw, corners, eye, Ht, Wt, align_corners)             # [V, N, 2, 2 tiles_y, 2 tiles_x]
+    N = c.shape[1]
+    c = c.reshape(V, N, 2, len(py), 2, len(px), 2).transpose(0, 3, 5, 1, 2, 4, 6).reshape(V, len(py), len(px), N, 2, 4)
+    ok = np.abs(c) < 1e9                                                         # False for inf and NaN
+    finite = ok.all(axis=(-2, -1))
+    f = np.floor(np.where(ok, c, 0)).astype(np.int64)
+    xmin, xmax, ymin, ymax = f[..., 0, :].min(-1), f[..., 0, :].max(-1), f[..., 1, :].min(-1), f[..., 1, :].max(-1)
+    bx0, by0 = (xmin - 1) // 4 * 4, ymin - 1
+    need_w, need_h = xmax - bx0 + 3, ymax - ymin + 4
+    mode = np.where(~finite | (need_w > 88) | (-(-need_h // 4) * 4 > max_bh), 2,
+                    np.where((bx0 > Wt - 1) | (bx0 + need_w - 1 < 0) | (by0 > Ht - 1) | (by0 + need_h - 1 < 0), 1, 0))
+    cls = np.where(need_w <= 64, 64, 96) if wide else 56 + 8 * np.maximum(0, -(-(need_w - 56) // 8))
+    return dict(bx0=bx0, need_w=need_w, need_h=need_h, mode=mode, cls=np.where(mode == 0, cls, 0))
+
+
 def check_range(rgba):
     M, N, _, Ht, Wt = rgba.shape
     rgba, p = _f(rgba)

@@ -13,6 +13,7 @@ import mpi_oracle
 import ml_gmpi_b200 as g
 from ml_gmpi_b200 import _lib, synth
 from conftest import rel_err
+from test_gpu_parity import each_alpha
 
 pytestmark = pytest.mark.gpu
 EXPECT = 2e-5
@@ -128,14 +129,22 @@ def test_view_order_does_not_change_a_bit(form, variant):
         _bitwise(base, _grads(case, gc, gd, deterministic=True, factored=fac, order=torch.tensor(order, device=d)))
 
 
-def test_full_size_training_shape_is_repeatable(variant):
-    """4 MPIs x 1 view, 96 planes, 1024^2 texture and image (13.7 GB of scratch)."""
+@each_alpha("variant", ["staged", "direct"], indirect=["variant"])
+def test_full_size_training_shape_is_repeatable(variant, alpha):
+    """4 MPIs x 1 view, 96 planes, 1024^2 texture and image (13.7 GB of scratch); the first MPI's gradient (its one view's) against
+    the oracle.  With equal-weight alpha every plane's gradient is far from 0, so repeatability is not met trivially on the back
+    planes."""
     d = dev()
-    case = synth.make_case(n_planes=96, tex=1024, img=1024, n_mpi=4, seed=3, device=d, last_alpha_one=True)
+    case = synth.make_case(n_planes=96, tex=1024, img=1024, n_mpi=4, seed=3, device=d, last_alpha_one=True, alpha=alpha)
     gc, gd = _upstream(4, 1024, 1024, 9, d)
     a = _grads(case, gc, gd, deterministic=True)
     _bitwise(a, _grads(case, gc, gd, deterministic=True))
     e = rel_err(a[0], _grads(case, gc, gd, deterministic=False)[0])
+    assert e <= EXPECT, e
+    v0 = lambda t: n(t[:1])
+    ref = mpi_oracle.backward(v0(case.rgba), v0(case.view2mpi), v0(case.dhw), v0(case.ray_dir), v0(case.eye), v0(case.z_dir),
+                              v0(gc), v0(gd), nthreads=_NT)
+    e = rel_err(a[0][:1], ref)
     assert e <= EXPECT, e
 
 

@@ -79,14 +79,16 @@ def _golden(name):
 
 
 def _synth(geo, M, N, tex_hw, seed, alpha_scale=None, last_one=True, ray=None, depth_grad=True, m11=False, ac=True, visible=False,
-           extra_mpis=0):
+           extra_mpis=0, alpha="uniform"):
     """A synth.make_case geometry (rgba=False) with random factors.  alpha_scale scales the alphas in front of the last plane (visible:
-    the background shows through, T in front of it mostly >= 0.1).  extra_mpis: MPIs that no view looks at."""
+    the background shows through, T in front of it mostly >= 0.1).  extra_mpis: MPIs that no view looks at.  alpha: "uniform"
+    (U(0, 1)) or "equal_weight" (synth.equal_weight_alpha: every plane reaches the render)."""
     ray = geo.ray_dir if ray is None else ray
     gen = torch.Generator().manual_seed(seed)
     Mt = M + extra_mpis
     rgb, bg = torch.rand((Mt, 3) + tex_hw, generator=gen), torch.rand((Mt, 3) + tex_hw, generator=gen)
-    alpha = torch.rand((Mt, N, 1) + tex_hw, generator=gen)
+    alpha = synth.equal_weight_alpha((Mt, N) + tex_hw, gen).unsqueeze(2) if alpha == "equal_weight" else \
+        torch.rand((Mt, N, 1) + tex_hw, generator=gen)
     if alpha_scale is not None:
         alpha[:, :-1] *= alpha_scale
     if last_one:
@@ -166,17 +168,17 @@ def _degenerate():
     return c
 
 
-def _op_bench():
+def _op_bench(alpha="uniform"):
     """bench.py's N1 shape for one view: 96 planes, 1024^2, random alpha (make_factored), colour-only upstream gradient w.r.t.
     2c - 1 (fb_factored)."""
     geo = _mk(n_planes=96, tex=1024, img=1024, n_mpi=1, seed=1234)
-    return _synth(geo, 1, 96, (1024, 1024), 99, last_one=False, depth_grad=False, m11=True)
+    return _synth(geo, 1, 96, (1024, 1024), 99, last_one=False, depth_grad=False, m11=True, alpha=alpha)
 
 
-def _op_views4():
+def _op_views4(alpha="uniform"):
     """One 48-plane 512^2 MPI seen from four views, colour and depth upstream gradients, alpha == 1 last plane."""
     geo = _mk(n_planes=48, tex=512, img=512, n_mpi=1, views_per_mpi=4, seed=21)
-    return _synth(geo, 1, 48, (512, 512), 21)
+    return _synth(geo, 1, 48, (512, 512), 21, alpha=alpha)
 
 
 def _abi(order):
@@ -199,6 +201,9 @@ SYNTH = {
     "degenerate_rays": _degenerate,
     "bench_96x1024": _op_bench,
     "views4_48x512": _op_views4,
+    # the operating points with every plane visible: U(0, 1) alpha hides the planes past ~25 from every bar
+    "bench_96x1024_equal_weight": lambda: _op_bench("equal_weight"),
+    "views4_48x512_equal_weight": lambda: _op_views4("equal_weight"),
     "view_group": lambda: _synth(_mk(n_planes=16, tex=256, img=256, n_mpi=2, views_per_mpi=4, seed=8), 2, 16, (256, 256), 8,
                                  alpha_scale=0.12, visible=True),
     "small": lambda: _synth(_mk(n_planes=12, tex=96, img=128, n_mpi=2, views_per_mpi=2, seed=5), 2, 12, (96, 96), 5,
@@ -209,7 +214,7 @@ SYNTH = {
 }
 GOLDEN = MPI_CASES + ["edge_odd_sizes", "edge_single_plane", "edge_acfalse_nonsquare", "edge_ragged_zero_views"]
 MATRIX = GOLDEN + ["partial_acfalse_nonsquare", "N1", "N512", "band_89_96", "wider_than_96", "shuffled_rays", "corners_off_the_planes",
-                   "degenerate_rays", "bench_96x1024", "views4_48x512"]
+                   "degenerate_rays", "bench_96x1024", "views4_48x512", "bench_96x1024_equal_weight", "views4_48x512_equal_weight"]
 
 
 @functools.lru_cache(maxsize=None)
@@ -393,7 +398,7 @@ def run(name, with_bg, mpi=None, view_group=1):
 # 1. the matrix
 # ------------------------------------------------------------------------------------------------------------------------------
 # with and without bg_rgb, except at the two operating points: the benchmark renders without one, the four-view case with one
-_BGS = {"bench_96x1024": (False,), "views4_48x512": (True,)}
+_BGS = {"bench_96x1024": (False,), "views4_48x512": (True,), "bench_96x1024_equal_weight": (False,), "views4_48x512_equal_weight": (True,)}
 
 
 def _matrix_params():

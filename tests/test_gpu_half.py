@@ -11,6 +11,7 @@ import numpy as np
 import pytest
 import torch
 
+import mpi_oracle
 import ml_gmpi_b200 as g
 from ml_gmpi_b200 import _lib, synth
 from ml_gmpi_b200.camera import cam_params
@@ -300,38 +301,51 @@ def _limit_case(factored):
     return _synth(16, 8, 720, 1, views=3, seed=21, tex_hw=(512, 1024), factored=factored)
 
 
+def footprints(c):
+    """mpi_oracle.footprints of case c's staged forward (the producer's box of every (view, tile, plane) stage)."""
+    M, N, _, Ht, Wt = c["rgba"].shape
+    return mpi_oracle.footprints(c["view2mpi"], c["dhw"], c["ray_dir"], c["eye"], Ht, Wt, c["ac"])
+
+
 def _limit_footprints(c, lo, hi):
-    """(tile, plane) stages whose fp32 box is staged (mode 0) with a width need in [lo, hi] and an origin 4 texels past a multiple
-    of 8, computed as the producer does from the texel coordinates of each tile's four corner pixels (gmpi_debug_plane_coords)."""
-    d = dev()
-    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(d)
-    V, _, H, W = c["ray_dir"].shape
-    N, Ht, Wt = c["rgba"].shape[1], c["rgba"].shape[-2], c["rgba"].shape[-1]
-    out = torch.empty((V, N, 2, H, W), device=d)
-    keep = [t(c[k]) for k in ("view2mpi", "dhw", "ray_dir", "eye")]
-    _lib.check(_lib.load().gmpi_debug_plane_coords(*[k.data_ptr() for k in keep], out.data_ptr(), V, N, Ht, Wt, H, W,
-                                                    _lib.OPT_ALIGN_CORNERS if c["ac"] else 0, None))
-    o = out.cpu().numpy()
-    px, py = np.arange(0, W, 64), np.arange(0, H, 30)
-    cxs, cys = [px, np.minimum(px + 63, W - 1)], [py, np.minimum(py + 29, H - 1)]
-    f = lambda a: np.stack([np.floor(a[:, :, cy][:, :, :, cx]) for cy in cys for cx in cxs], -1).astype(np.int64)
-    fx, fy = f(o[:, :, 0]), f(o[:, :, 1])
-    xmin, xmax, ymin, ymax = fx.min(-1), fx.max(-1), fy.min(-1), fy.max(-1)
-    bx0, by0 = (xmin - 1) // 4 * 4, ymin - 1
-    need_w, need_h = xmax - bx0 + 3, ymax - ymin + 4
-    staged = (-(-need_h // 4) * 4 <= 44) & (bx0 <= Wt - 1) & (bx0 + need_w - 1 >= 0) & (by0 <= Ht - 1) & (by0 + need_h - 1 >= 0)
-    return int((staged & (need_w >= lo) & (need_w <= hi) & (bx0 % 8 == 4)).sum())
+    """(tile, plane) stages whose fp32 box lies under the tile with rows that fit a stage (mode 0, or mode 2 only for a width need
+    above kMaxBW = 88) with a width need in [lo, hi] and an origin 4 texels past a multiple of 8."""
+    f = footprints(c)
+    fits = (f["mode"] != 1) & (-(-f["need_h"] // 4) * 4 <= mpi_oracle.FWD_TILE[1])
+    return int((fits & (f["need_w"] >= lo) & (f["need_w"] <= hi) & (f["bx0"] % 8 == 4)).sum())
+
+
+@functools.lru_cache(maxsize=None)
+def headline_case():
+    """One view of the headline MPI, 96 x 1024^2, with equal-weight alpha (synth.equal_weight_alpha): every plane, the back ones
+    with the widest boxes included, reaches the render, so a back-plane tap the native kernel staged or converted wrongly changes
+    the bits of the output (with U(0, 1) alpha it would be absorbed by the rounding of the accumulator)."""
+    cs = synth.make_case(n_planes=96, tex=1024, img=1024, n_mpi=1, seed=1234, alpha="equal_weight")
+    return dict(rgba=cs.rgba.numpy(), view2mpi=cs.view2mpi.numpy(), dhw=cs.dhw.numpy(), ray_dir=cs.ray_dir.numpy(),
+                eye=cs.eye.numpy(), z_dir=cs.z_dir.numpy(), ac=True)
+
+
+def assert_class_88_behind_plane_25(c):
+    cls = footprints(c)["cls"]
+    assert (cls[..., 25:] == 88).any() and all((cls == k).any() for k in range(56, 96, 8))
 
 
 @pytest.mark.parametrize("stages", ["staged2", "staged3"])
-@pytest.mark.parametrize("factored", [False, True])
+@pytest.mark.parametrize("factored", [pytest.param(False, id="False"), pytest.param(True, id="True"),
+                                      pytest.param("headline", id="headline_96x1024_equal_weight")])
 def test_fp16_at_the_widest_box_classes(factored, stages):
     """Footprints at the widest class (width need 85..88: class 88 expanded, class 96 factored; the factored case also has footprints
     93..96, which take the generic body) whose fp16 box starts 4
     texels west of the fp32 one: the fp16 kernel stages a wider box and decides fast / generic body exactly as fp32 does, so the
-    render stays bitwise the upcast's."""
-    c = _limit_case(factored)
-    assert _limit_footprints(c, 85, 88) > 0 and (not factored or _limit_footprints(c, 93, 96) > 0)
+    render stays bitwise the upcast's.  "headline": the same at 96 x 1024^2 with equal-weight alpha, where every box class occurs on
+    planes that reach the render."""
+    if factored == "headline":
+        c = headline_case()
+        assert_class_88_behind_plane_25(c)
+        factored = False
+    else:
+        c = _limit_case(factored)
+        assert _limit_footprints(c, 85, 88) > 0 and (not factored or _limit_footprints(c, 93, 96) > 0)
     set_variant(stages)
     try:
         for kw in ([{}, dict(bg=False)] if factored else [{}]):

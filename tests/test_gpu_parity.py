@@ -3,6 +3,9 @@
 
 Bars (SURVEY.md section 8c): max|ours-ref| / max|ref| <= 1e-4 for colour, depth and d/d rgba
 (fp32); the texel coordinates (ix, iy) are bit-exact."""
+import functools
+import json
+
 import numpy as np
 import pytest
 import torch
@@ -214,18 +217,61 @@ def _ffhq_case(N, res, V, seed=1234, device=None):
     return synth.make_case(n_planes=N, tex=res, img=res, n_mpi=V, seed=seed, device=device)
 
 
-@pytest.mark.parametrize("N,res,V", [(32, 256, 8), (96, 512, 2), (96, 1024, 1)])
-def test_full_size_against_oracle(N, res, V, fwd_variant_auto):
-    d = dev()
-    case = _ffhq_case(N, res, V, device=d)
+# The full-size cases run on two MPIs: U(0, 1) alpha, and equal-weight alpha (synth.equal_weight_alpha).  Under U(0, 1) alpha the
+# transmittance falls as e^-i and planes past ~25 move the render and its gradient by less than the bar, so only the equal-weight
+# MPI checks the back planes, where the widest box classes occur (tests/test_every_plane_weight.py).
+ALPHAS = ["uniform", "equal_weight"]
+_C4_YAWS = np.linspace(0.5, -0.5, 120).astype(np.float32)[::8]
+FULL = {   # name: synth.make_case arguments
+    "full_32x256": dict(n_planes=32, tex=256, img=256, n_mpi=8, seed=1234),
+    "full_96x512": dict(n_planes=96, tex=512, img=512, n_mpi=2, seed=1234),
+    "full_96x1024": dict(n_planes=96, tex=1024, img=1024, n_mpi=1, seed=1234),
+    "c3": dict(n_planes=96, tex=1024, img=1024, n_mpi=1, seed=1234, last_alpha_one=True),
+    "c5": dict(n_planes=96, tex=512, img=512, n_mpi=4, seed=99, last_alpha_one=True),
+    "four_views": dict(n_planes=48, tex=512, img=512, n_mpi=1, views_per_mpi=4, seed=21, last_alpha_one=True),
+    "c4_video": dict(n_planes=96, tex=512, img=512, n_mpi=1, views_per_mpi=15, seed=1234, yaws=_C4_YAWS, pitches=np.zeros(15, np.float32)),
+}
+
+
+def _full_case(name, alpha):
+    from ml_gmpi_b200 import synth
+    return synth.make_case(**FULL[name], alpha=alpha, device=dev())
+
+
+@functools.lru_cache(maxsize=2)
+def _oracle_forward(name, alpha):
+    """(colour, depth) of every view of a FULL case, once per case for all the kernels a test runs."""
+    case = _full_case(name, alpha)
+    n = lambda t: t.cpu().numpy()
+    rc, rd, _ = mpi_oracle.forward(n(case.rgba), n(case.view2mpi), n(case.dhw), n(case.ray_dir), n(case.eye), n(case.z_dir),
+                                   nthreads=_NT)
+    return rc, rd
+
+
+def each_alpha(argnames, sets, indirect=()):
+    """parametrize(argnames + ",alpha") over sets x ALPHAS.  The U(0, 1) sets keep the ids they had before the equal-weight input
+    was added; the equal-weight ones end in "-equal_weight"."""
+    params = []
+    for alpha in ALPHAS:
+        for vals in sets:
+            vals = vals if isinstance(vals, tuple) else (vals,)
+            ident = "-".join(str(v) for v in vals) + ("" if alpha == "uniform" else "-" + alpha)
+            params.append(pytest.param(*vals, alpha, id=ident))
+    return pytest.mark.parametrize(argnames + ",alpha", params, indirect=list(indirect))
+
+
+@each_alpha("N,res,V", [(32, 256, 8), (96, 512, 2), (96, 1024, 1)])
+def test_full_size_against_oracle(N, res, V, alpha, fwd_variant_auto):
+    """The BASELINE.json shapes, every view."""
+    name = f"full_{N}x{res}"
+    assert FULL[name]["n_mpi"] == V
+    case = _full_case(name, alpha)
     color, depth = g.render_views(case.rgba, case.dhw, case.view2mpi, case.ray_dir, case.eye, case.z_dir,
                                   check_last_plane=True)
-    v = V - 1
-    rc, rd, fl = mpi_oracle.forward(case.rgba[v:v + 1].cpu().numpy(), np.zeros(1, np.int32), case.dhw[v:v + 1].cpu().numpy(),
-                                    case.ray_dir[v:v + 1].cpu().numpy(), case.eye[v:v + 1].cpu().numpy(),
-                                    case.z_dir[v:v + 1].cpu().numpy(), nthreads=32)
-    assert rel_err(color[v:v + 1].cpu().numpy(), rc) <= EXPECT
-    assert rel_err(depth[v:v + 1].cpu().numpy(), rd) <= EXPECT
+    rc, rd = _oracle_forward(name, alpha)
+    for v in range(rc.shape[0]):
+        assert rel_err(color[v].cpu().numpy(), rc[v]) <= EXPECT, v
+        assert rel_err(depth[v].cpu().numpy(), rd[v]) <= EXPECT, v
 
 
 def test_sanity_mode_all_alpha_one_shows_first_plane(fwd_variant):
@@ -335,15 +381,14 @@ def test_renderer_facade_matches_reference_render():
     assert img.shape == (4, 3, 256, 256) and ang.shape == (4, 2)
 
 
-def test_every_view_of_a_batch_matches_the_oracle(fwd_variant):
+@each_alpha("fwd_variant", ["direct", "staged", "staged2", "staged3"], indirect=["fwd_variant"])
+def test_every_view_of_a_batch_matches_the_oracle(fwd_variant, alpha):
     """All views (not just one) of a multi-view batch, including the most oblique pose of the synthetic set, whose tiles on
     the left image border have tall (scale 1.23) and partly out-of-texture footprints."""
-    d = dev()
-    from ml_gmpi_b200 import synth
-    case = synth.make_case(n_planes=32, tex=256, img=256, n_mpi=8, seed=1234, device=d)
+    case = _full_case("full_32x256", alpha)
     color, depth = g.render_views(case.rgba, case.dhw, case.view2mpi, case.ray_dir, case.eye, case.z_dir)
     n = lambda t: t.cpu().numpy()
-    rc, rd, _ = mpi_oracle.forward(n(case.rgba), n(case.view2mpi), n(case.dhw), n(case.ray_dir), n(case.eye), n(case.z_dir), nthreads=32)
+    rc, rd = _oracle_forward("full_32x256", alpha)
     assert rel_err(n(color), rc) <= EXPECT and rel_err(n(depth), rd) <= EXPECT
     # single-plane renders isolate per-plane sampling errors that transmittance would otherwise hide
     for k in (0, 13, 26, 31):
@@ -390,60 +435,107 @@ import os as _os
 _NT = max(1, min(64, (_os.cpu_count() or 8)))
 
 
-def _grad_check(case, with_depth, minus1_1=False, seed=3):
-    d = case.rgba.device
+def _upstream(case, with_depth, seed=3):
+    """The upstream colour and depth gradients of a case's render (randn from a CPU generator, on the case's device)."""
+    V, _, H, W = case.ray_dir.shape
+    gen = torch.Generator().manual_seed(seed)
+    gc = torch.randn((V, 3, H, W), generator=gen).to(case.rgba.device)
+    gdp = torch.randn((V, 1, H, W), generator=gen).to(case.rgba.device) if with_depth else None
+    return gc, gdp
+
+
+def _oracle_grad(case, with_depth, minus1_1=False):
+    """The oracle's d rgba under _upstream's gradients."""
+    gc, gdp = _upstream(case, with_depth)
+    n = lambda t: t.detach().cpu().numpy()
+    return mpi_oracle.backward(n(case.rgba), n(case.view2mpi), n(case.dhw), n(case.ray_dir), n(case.eye), n(case.z_dir),
+                               (2.0 if minus1_1 else 1.0) * n(gc), n(gdp) if with_depth else None, nthreads=_NT)
+
+
+@functools.lru_cache(maxsize=1)
+def _oracle_backward(name, alpha, with_depth, minus1_1=False):
+    """_oracle_grad of a FULL case, once for all the kernels a test runs."""
+    return _oracle_grad(_full_case(name, alpha), with_depth, minus1_1)
+
+
+def _render_and_grad(case, with_depth, minus1_1=False):
+    """(colour, depth, d rgba) of the kernels under _upstream's gradients, as numpy."""
     rgba = case.rgba.clone().requires_grad_(True)
     color, depth = g.render_views(rgba, case.dhw, case.view2mpi, case.ray_dir, case.eye, case.z_dir, color_minus1_1=minus1_1)
-    gen = torch.Generator().manual_seed(seed)
-    gc = torch.randn(color.shape, generator=gen).to(d)
-    gdp = torch.randn(depth.shape, generator=gen).to(d) if with_depth else None
+    gc, gdp = _upstream(case, with_depth)
     loss = (color * gc).sum()
     if with_depth:
         loss = loss + (depth * gdp).sum()
     loss.backward()
     n = lambda t: t.detach().cpu().numpy()
-    ref = mpi_oracle.backward(n(case.rgba), n(case.view2mpi), n(case.dhw), n(case.ray_dir), n(case.eye), n(case.z_dir),
-                              (2.0 if minus1_1 else 1.0) * n(gc), n(gdp) if with_depth else None, nthreads=_NT)
-    ours = n(rgba.grad)
-    del rgba, color, depth, loss
-    return rel_err(ours, ref)
+    return n(color), n(depth), n(rgba.grad)
 
 
-def test_full_size_backward_c3_one_view_96x1024_vs_oracle(fwd_variant_auto):
+def _grad_check(case, with_depth, minus1_1=False):
+    return rel_err(_render_and_grad(case, with_depth, minus1_1)[2], _oracle_grad(case, with_depth, minus1_1))
+
+
+def _full_grad_check(name, alpha, with_depth, minus1_1=False):
+    ours = _render_and_grad(_full_case(name, alpha), with_depth, minus1_1)[2]
+    return rel_err(ours, _oracle_backward(name, alpha, with_depth, minus1_1))
+
+
+_AUTO = ["direct", "staged"]
+
+
+@each_alpha("fwd_variant_auto", _AUTO, indirect=["fwd_variant_auto"])
+def test_full_size_backward_c3_one_view_96x1024_vs_oracle(fwd_variant_auto, alpha):
     """BASELINE configs[2] (FFHQ1024 forward+backward): one 96-plane 1024^2 view, production alpha==1 last plane, colour and
     depth upstream gradients.  (gmpi/core/mpi.py:411-436 autograd; train.py:733-740.)"""
-    from ml_gmpi_b200 import synth
-    case = synth.make_case(n_planes=96, tex=1024, img=1024, n_mpi=1, seed=1234, device=dev(), last_alpha_one=True)
-    assert _grad_check(case, with_depth=True) <= EXPECT
+    assert _full_grad_check("c3", alpha, with_depth=True) <= EXPECT
 
 
-def test_full_size_backward_c5_batch4_96x512_vs_oracle(fwd_variant_auto):
+@each_alpha("fwd_variant_auto", _AUTO, indirect=["fwd_variant_auto"])
+def test_full_size_backward_c5_batch4_96x512_vs_oracle(fwd_variant_auto, alpha):
     """BASELINE configs[4] per-GPU shape: M = V = 4, 96 planes, 512^2, alpha==1 last plane, colour-only upstream gradient w.r.t.
     2c-1 (what train.py:740,779 backpropagates; the depth output is discarded there)."""
-    from ml_gmpi_b200 import synth
-    case = synth.make_case(n_planes=96, tex=512, img=512, n_mpi=4, seed=99, device=dev(), last_alpha_one=True)
-    assert _grad_check(case, with_depth=False, minus1_1=True) <= EXPECT
+    assert _full_grad_check("c5", alpha, with_depth=False, minus1_1=True) <= EXPECT
 
 
-def test_full_size_backward_four_views_share_one_mpi_512_vs_oracle(fwd_variant_auto):
+@each_alpha("fwd_variant_auto", _AUTO, indirect=["fwd_variant_auto"])
+def test_full_size_backward_four_views_share_one_mpi_512_vs_oracle(fwd_variant_auto, alpha):
     """Gradient accumulation over 4 views of ONE MPI at 512^2 (the expand of train.py:733-738, train_helpers.py:181-186)."""
-    from ml_gmpi_b200 import synth
-    case = synth.make_case(n_planes=48, tex=512, img=512, n_mpi=1, views_per_mpi=4, seed=21, device=dev(), last_alpha_one=True)
-    assert _grad_check(case, with_depth=True) <= EXPECT
+    assert _full_grad_check("four_views", alpha, with_depth=True) <= EXPECT
 
 
-def test_full_size_forward_c4_video_every_view_vs_oracle(fwd_variant_auto):
+def test_the_bars_fail_on_a_slightly_wrong_problem():
+    """The kernels' C3 colour and gradient on equal-weight data, checked against the oracle of a slightly wrong problem: plane N/2
+    or N - 2 rolled by one texel, or plane N/2 or N - 2 left out of the gradient.  Each must fail the bar by 10x or more, so the
+    full-size tests above would catch a kernel that mis-sampled, or dropped the gradient of, one plane in the back half."""
+    case = _full_case("c3", "equal_weight")
+    N = case.rgba.shape[1]
+    color, _, grad = _render_and_grad(case, with_depth=True)
+    right_c, _ = _oracle_forward("c3", "equal_weight")
+    right_g = _oracle_backward("c3", "equal_weight", True)
+    assert rel_err(color, right_c) <= EXPECT and rel_err(grad, right_g) <= EXPECT
+    n = lambda t: t.cpu().numpy()
+    geo = (n(case.view2mpi), n(case.dhw), n(case.ray_dir), n(case.eye), n(case.z_dir))
+    ratios = {}
+    for k in (N // 2, N - 2):
+        rolled = n(case.rgba)
+        rolled[:, k] = np.roll(rolled[:, k], 1, axis=-1)
+        ratios[f"plane_{k}_rolled"] = rel_err(color, mpi_oracle.forward(rolled, *geo, nthreads=_NT)[0]) / EXPECT
+        omitted = right_g.copy()
+        omitted[:, k] = 0.0
+        ratios[f"plane_{k}_gradient_omitted"] = rel_err(grad, omitted) / EXPECT
+    print("PARITY_TEETH " + json.dumps({k: float("%.3g" % v) for k, v in ratios.items()}))
+    assert all(v >= 10 for v in ratios.values()), ratios
+
+
+@each_alpha("fwd_variant_auto", _AUTO, indirect=["fwd_variant_auto"])
+def test_full_size_forward_c4_video_every_view_vs_oracle(fwd_variant_auto, alpha):
     """BASELINE configs[3] shape: ONE 96-plane 512^2 MPI, 15 views (one rank's share of the 120) spread over the whole
     yaw = linspace(0.5, -0.5, 120) sweep, pitch 0 (render_video.py:95-107); every view against the oracle."""
-    from ml_gmpi_b200 import synth
-    yaws = np.linspace(0.5, -0.5, 120).astype(np.float32)[::8]
-    assert len(yaws) == 15
-    case = synth.make_case(n_planes=96, tex=512, img=512, n_mpi=1, views_per_mpi=15, seed=1234, device=dev(), yaws=yaws,
-                           pitches=np.zeros(15, np.float32))
+    assert len(_C4_YAWS) == 15
+    case = _full_case("c4_video", alpha)
     color, depth = g.render_views(case.rgba, case.dhw, case.view2mpi, case.ray_dir, case.eye, case.z_dir, check_last_plane=True)
     n = lambda t: t.cpu().numpy()
-    rc, rd, _ = mpi_oracle.forward(n(case.rgba), n(case.view2mpi), n(case.dhw), n(case.ray_dir), n(case.eye), n(case.z_dir),
-                                   nthreads=_NT)
+    rc, rd = _oracle_forward("c4_video", alpha)
     for v in range(15):
         assert rel_err(n(color[v]), rc[v]) <= EXPECT and rel_err(n(depth[v]), rd[v]) <= EXPECT, v
 

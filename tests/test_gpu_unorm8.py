@@ -17,7 +17,7 @@ from ml_gmpi_b200 import _lib, synth
 from ml_gmpi_b200.camera import cam_params
 from conftest import ROOT
 from test_gpu_early_stop import CASES, case, set_variant
-from test_gpu_half import _limit_case
+from test_gpu_half import _limit_case, assert_class_88_behind_plane_25, footprints, headline_case
 
 pytestmark = pytest.mark.gpu
 TAUS = [None, 0.0, 2.0 ** -24, 1e-3]
@@ -195,36 +195,24 @@ def test_host_entry_point_takes_u8_host_buffers(name):
 
 def _shift_footprints(c, lo, hi):
     """{shift: count} of the (tile, plane) stages whose fp32 box is staged (mode 0) with a width need in [lo, hi], by the offset of
-    the fp32 box origin from the multiple of 16 the uint8 box starts at (0, 4, 8, 12), computed as the producer does from the texel
-    coordinates of each tile's four corner pixels (gmpi_debug_plane_coords)."""
-    d = dev()
-    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(d)
-    V, _, H, W = c["ray_dir"].shape
-    N, Ht, Wt = c["rgba"].shape[1], c["rgba"].shape[-2], c["rgba"].shape[-1]
-    out = torch.empty((V, N, 2, H, W), device=d)
-    keep = [t(c[k]) for k in ("view2mpi", "dhw", "ray_dir", "eye")]
-    _lib.check(_lib.load().gmpi_debug_plane_coords(*[k.data_ptr() for k in keep], out.data_ptr(), V, N, Ht, Wt, H, W,
-                                                    _lib.OPT_ALIGN_CORNERS if c["ac"] else 0, None))
-    o = out.cpu().numpy()
-    px, py = np.arange(0, W, 64), np.arange(0, H, 30)
-    cxs, cys = [px, np.minimum(px + 63, W - 1)], [py, np.minimum(py + 29, H - 1)]
-    f = lambda a: np.stack([np.floor(a[:, :, cy][:, :, :, cx]) for cy in cys for cx in cxs], -1).astype(np.int64)
-    fx, fy = f(o[:, :, 0]), f(o[:, :, 1])
-    xmin, xmax, ymin, ymax = fx.min(-1), fx.max(-1), fy.min(-1), fy.max(-1)
-    bx0, by0 = (xmin - 1) // 4 * 4, ymin - 1
-    need_w, need_h = xmax - bx0 + 3, ymax - ymin + 4
-    staged = (-(-need_h // 4) * 4 <= 44) & (bx0 <= Wt - 1) & (bx0 + need_w - 1 >= 0) & (by0 <= Ht - 1) & (by0 + need_h - 1 >= 0)
-    sel = staged & (need_w >= lo) & (need_w <= hi)
-    return {s: int((sel & (bx0 % 16 == s)).sum()) for s in (0, 4, 8, 12)}
+    the fp32 box origin from the multiple of 16 the uint8 box starts at (0, 4, 8, 12)."""
+    f = footprints(c)
+    sel = (f["mode"] == 0) & (f["need_w"] >= lo) & (f["need_w"] <= hi)
+    return {s: int((sel & (f["bx0"] % 16 == s)).sum()) for s in (0, 4, 8, 12)}
 
 
-@pytest.mark.parametrize("stages", ["staged2", "staged3"])
-def test_u8_at_the_widest_box_class_at_every_shift(stages):
+@pytest.mark.parametrize("stages,shape", [pytest.param("staged2", "limit", id="staged2"), pytest.param("staged3", "limit", id="staged3"),
+                                          pytest.param("staged2", "headline", id="staged2-headline_96x1024_equal_weight"),
+                                          pytest.param("staged3", "headline", id="staged3-headline_96x1024_equal_weight")])
+def test_u8_at_the_widest_box_class_at_every_shift(stages, shape):
     """Footprints at the widest class (width need 81..88, class 88) whose fp32 box starts 0, 4, 8 and 12 texels past a multiple of 16:
-    the uint8 kernel stages a 112-wide box from that multiple and decides fast / generic body exactly as fp32 does."""
-    c = _limit_case(False)
+    the uint8 kernel stages a 112-wide box from that multiple and decides fast / generic body exactly as fp32 does.  "headline": 96 x
+    1024^2 with equal-weight alpha, where those footprints lie on planes that reach the render."""
+    c = _limit_case(False) if shape == "limit" else headline_case()
     counts = _shift_footprints(c, 81, 88)
     assert all(n > 0 for n in counts.values()), counts
+    if shape == "headline":
+        assert_class_88_behind_plane_25(c)
     u8 = quantize(c["rgba"])
     set_variant(stages)
     try:
