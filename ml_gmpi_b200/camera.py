@@ -173,10 +173,10 @@ def sphere_poses(yaws: torch.Tensor, pitches: torch.Tensor, sphere_center, spher
     then the translation (cam_utils.py:687-731)."""
     yaws = yaws.reshape(-1, 1).float()
     pitches = pitches.reshape(-1, 1).float()
-    cp = torch.abs(torch.cos(pitches))
-    pos = sphere_r * torch.cat([cp * torch.cos(yaws), cp * torch.sin(yaws), torch.sin(pitches)], 1)     # fp32, like the reference
+    rc = sphere_r * torch.abs(torch.cos(pitches))
+    pos = torch.cat([rc * torch.cos(yaws), rc * torch.sin(yaws), sphere_r * torch.sin(pitches)], 1)    # fp32, in the reference's order
     unit = lambda v: v / torch.norm(v, dim=-1, keepdim=True)
-    fwd = unit(-pos)
+    fwd = unit(unit(-pos))                                            # normalised twice, as the reference does (cam_utils.py:786, :599)
     down0 = torch.tensor([0.0, 0.0, -1.0]).expand_as(fwd)
     right = unit(torch.cross(down0, fwd, dim=-1))
     down = unit(torch.cross(fwd, right, dim=-1))

@@ -64,6 +64,18 @@ FFHQ = dict(  # curriculums.py:109-116, configs/gmpi.yml:74-96
     confined=True,
 )
 
+AFHQCAT = dict(  # curriculums.py:147-154 (fov, ray_start / ray_end, h_stddev / v_stddev), configs/gmpi.yml:98-103 (FOR_AFHQCat)
+    plane_min_d=2.55, plane_max_d=2.8, enlarge_factor=1.001, distance_method="inverse", fov_deg=13.39,
+    sphere_center=(0.0, 0.0, 2.7), sphere_r=2.7, h_mean=0.0, h_std=0.19, v_mean=0.0, v_std=0.15, n_truncated_stds=3,
+    confined=True,
+)
+
+METFACES = dict(  # curriculums.py:185-192, configs/gmpi.yml:105-110 (FOR_MetFaces)
+    plane_min_d=0.95, plane_max_d=1.12, enlarge_factor=1.001, distance_method="inverse", fov_deg=12.6,
+    sphere_center=(0.0, 0.0, 1.0), sphere_r=1.0, h_mean=0.0, h_std=0.339, v_mean=0.0, v_std=0.133, n_truncated_stds=2,
+    confined=True,
+)
+
 
 # ---- texel positions of the planes: what the generator is conditioned on and what LightRenderer shades with --------------------
 # Mirrors MPIRenderer.comput_tex_pixels_3d_coords / comput_tex_pixels_3d_normalized_coords_mpi / get_xyz_single_res(only_z) /
