@@ -10,12 +10,7 @@ import torch
 import ml_gmpi_b200 as g
 from ml_gmpi_b200 import _lib
 from conftest import ROOT
-
-
-@pytest.fixture(scope="module")
-def lib():
-    g.build_library()
-    return _lib.load()
+from testlib import KEY_AC, KEY_BWD, KEY_ES, KEY_F16, KEY_FAC, KEY_STAGED, KEY_U8, lib, library_kernels, render_kernels
 
 
 def declared_symbols():
@@ -179,7 +174,6 @@ def test_sass_of_the_hot_kernel_keys_is_tma_mbarrier_packed_math():
     fp32 instructions), additionally native integer shared atomics
     and vector global reductions in the backward; no local-memory spills in the expanded instantiations."""
     import re
-    from test_library_build import KEY_AC, KEY_BWD, KEY_ES, KEY_F16, KEY_FAC, KEY_STAGED, KEY_U8, library_kernels, render_kernels
     g.build_library()
     kernels = library_kernels()
     fwd = render_kernels(kernels, "mpi_fwd_staged_kernel", lacks=KEY_ES | KEY_F16 | KEY_U8)

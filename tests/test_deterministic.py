@@ -12,16 +12,10 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
-import ml_gmpi_b200 as g  # noqa: E402
 from ml_gmpi_b200 import _lib  # noqa: E402
+from testlib import lib  # noqa: E402
 
 ERR_INVALID, ERR_UNSUPPORTED = 1, 3
-
-
-@pytest.fixture(scope="module")
-def lib():
-    g.build_library()
-    return _lib.load()
 
 
 def _buf():

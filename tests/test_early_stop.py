@@ -12,6 +12,7 @@ import ml_gmpi_b200 as g
 import torch_port
 from ml_gmpi_b200 import _lib, service
 from conftest import MPI_CASES, ROOT, load_golden
+from testlib import lib, max_plane_depth
 
 EDGE_CASES = ["edge_single_plane", "edge_ragged_zero_views", "edge_acfalse_nonsquare", "edge_odd_sizes"]
 
@@ -56,15 +57,6 @@ def _port(gd, early_stop=None):
     return color.numpy(), depth.numpy()
 
 
-def max_plane_depth(gd):
-    """[V,1,H,W]: the largest |z-depth| of a pixel over the planes, (d - e_z) / r_z * (r . z_dir) (mpi.py:74-76,149-151)."""
-    ray, eye, z = gd["ray_dir"].astype(np.float64), gd["eye"].astype(np.float64), gd["z_dir"].astype(np.float64)
-    d = gd["dhw"][gd["view2mpi"], :, 0].astype(np.float64)                      # [V,N]
-    zlen = np.einsum("vchw,vc->vhw", ray, z)
-    t = (d[:, :, None, None] - eye[:, 2, None, None, None]) / ray[:, None, 2]    # [V,N,H,W]
-    return np.max(np.abs(t * zlen[:, None]), axis=1, keepdims=True)
-
-
 @pytest.mark.parametrize("name", MPI_CASES + EDGE_CASES)
 def test_oracle_tau_zero_and_off_are_bitwise_the_torch_port(name):
     """Without tau and at tau = 0 the early-stop oracle is bit for bit oracle/torch_port.render_views (itself bit-identical to
@@ -95,12 +87,6 @@ def test_oracle_early_stop_drops_planes_behind_opaque_content():
     c0, _ = _port(gd)
     c, _ = _port(gd, early_stop=0.05)
     assert np.max(np.abs(c - c0)) > 0.0
-
-
-@pytest.fixture(scope="module")
-def lib():
-    g.build_library()
-    return _lib.load()
 
 
 def test_header_option_bit_and_descriptor_sizes():

@@ -18,15 +18,14 @@ import json
 import os
 import sys
 
-import pytest
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
-import ml_gmpi_b200 as g  # noqa: E402
 from ml_gmpi_b200 import _lib  # noqa: E402
+from testlib import lib  # noqa: E402
 
 RECORD = os.path.join(ROOT, "tests", "golden", "entry_point_codes.json")
 F16, U8, ES = _lib.OPT_MPI_F16, _lib.OPT_MPI_U8, _lib.OPT_EARLY_STOP
@@ -147,12 +146,6 @@ def write_record(cells):
     with open(RECORD, "w") as f:
         f.write('{"cells": ' + json.dumps(names, indent=0) + ',\n"messages": ' + json.dumps(messages, indent=0) + ',\n"entry_points": {\n' +
                 ",\n".join(f"{json.dumps(e)}: {json.dumps(r, separators=(',', ':'))}" for e, r in rows.items()) + "\n}}\n")
-
-
-@pytest.fixture(scope="module")
-def lib():
-    g.build_library()
-    return _lib.load()
 
 
 def test_every_entry_point_answers_every_cell_as_recorded(lib):

@@ -7,6 +7,7 @@ import pytest
 import torch
 
 from conftest import load_golden
+from testlib import reference_signatures
 from ml_gmpi_b200 import geometry
 from ml_gmpi_b200.renderer import MPIRenderer
 
@@ -107,7 +108,6 @@ def test_view_info_from_c2w_mat_matches_reference():
 
 def test_facade_has_every_public_method_of_the_reference_with_its_signature():
     from make_golden_signatures import params
-    from test_interface_matches_reference import reference_signatures
     for name, sig in reference_signatures()["MPIRenderer"].items():
         if name == "__init__":
             continue

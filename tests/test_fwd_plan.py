@@ -12,26 +12,12 @@ import warnings
 import pytest
 import torch
 
-import ml_gmpi_b200 as g
 from ml_gmpi_b200 import _lib, mpi, synth
-from test_gpu_early_stop import set_variant
-from test_gpu_half import _misaligned
+from testlib import assert_bitwise, early_stop_stats, forced_kernel, lib, misaligned
 
 TEX_WIDTH, FEW_TILES, MANY_PLANES, ALIGNMENT, FORCED = 1, 2, 4, 8, 16
 F16 = _lib.OPT_MPI_F16
 SIZES = dict(M=4, V=4, N=96, Ht=1024, Wt=1024, H=1024, W=1024)     # the benchmark's shape: staged
-
-
-@pytest.fixture(scope="module")
-def lib():
-    g.build_library()
-    return _lib.load()
-
-
-@pytest.fixture
-def variant():
-    yield set_variant
-    set_variant("auto")
 
 
 def _why(**kw):
@@ -55,25 +41,25 @@ def test_each_reason_sets_its_bit(lib):
     assert _why(V=1, H=48, W=48, N=600, Wt=1022, rgba=8) == TEX_WIDTH | FEW_TILES | MANY_PLANES | ALIGNMENT
 
 
-def test_forced_variants(lib, variant):
-    variant("direct")
-    assert _why() == FORCED and _why(V=1, H=48, W=48) == FORCED | FEW_TILES
-    variant("staged")
-    assert _why(V=1, H=48, W=48) == 0 and _why(V=1, H=48, W=48, Wt=1022) == TEX_WIDTH and _why(N=513, rgba=8) == MANY_PLANES | ALIGNMENT
+def test_forced_variants(lib):
+    with forced_kernel("direct"):
+        assert _why() == FORCED and _why(V=1, H=48, W=48) == FORCED | FEW_TILES
+    with forced_kernel("staged"):
+        assert _why(V=1, H=48, W=48) == 0 and _why(V=1, H=48, W=48, Wt=1022) == TEX_WIDTH and _why(N=513, rgba=8) == MANY_PLANES | ALIGNMENT
 
 
-def test_the_three_queries_agree_on_fp32_expanded_mpis(lib, variant):
+def test_the_three_queries_agree_on_fp32_expanded_mpis(lib):
     """gmpi_mpi_render_fwd_plan is _plan_ex of one MPI at the given rgba; _variant is _plan_ex of 2^20 views without a pointer."""
     why = ctypes.c_uint32(0)
     for v in ("auto", "direct", "staged"):
-        variant(v)
-        for V, N, Wt, HW, rgba in itertools.product((1, 4), (16, 512, 513), (1020, 1022, 1024), (48, 300, 1024), (None, 8, 16)):
-            plan = lib.gmpi_mpi_render_fwd_plan(V, N, 1024, Wt, HW, HW, rgba, ctypes.byref(why))
-            case = (v, V, N, Wt, HW, rgba)
-            assert (plan, why.value) == _lib.fwd_plan(_lib.make_desc(M=1, V=V, N=N, Ht=1024, Wt=Wt, H=HW, W=HW, rgba=rgba)), case
-            staged = _lib.fwd_plan(_lib.make_desc(M=1, V=1 << 20, N=N, Ht=1024, Wt=Wt, H=HW, W=HW))[0] == _lib.PLAN_STAGED
-            assert lib.gmpi_mpi_render_fwd_variant(N, 1024, Wt, HW, HW).decode() == \
-                ("fwd_staged_tma_64x30" if staged else "fwd_direct_32x8"), case
+        with forced_kernel(v):
+            for V, N, Wt, HW, rgba in itertools.product((1, 4), (16, 512, 513), (1020, 1022, 1024), (48, 300, 1024), (None, 8, 16)):
+                plan = lib.gmpi_mpi_render_fwd_plan(V, N, 1024, Wt, HW, HW, rgba, ctypes.byref(why))
+                case = (v, V, N, Wt, HW, rgba)
+                assert (plan, why.value) == _lib.fwd_plan(_lib.make_desc(M=1, V=V, N=N, Ht=1024, Wt=Wt, H=HW, W=HW, rgba=rgba)), case
+                staged = _lib.fwd_plan(_lib.make_desc(M=1, V=1 << 20, N=N, Ht=1024, Wt=Wt, H=HW, W=HW))[0] == _lib.PLAN_STAGED
+                assert lib.gmpi_mpi_render_fwd_variant(N, 1024, Wt, HW, HW).decode() == \
+                    ("fwd_staged_tma_64x30" if staged else "fwd_direct_32x8"), case
 
 
 def test_warning_sees_every_mpi_tensor(lib, monkeypatch):
@@ -136,7 +122,7 @@ def _render(form, half, N=8, tex=64, Wt=None, img=256, views=2, misalign=None, s
     else:
         m = dict(rgb=rand(2, 3, *hw), alpha=rand(2, N, 1, *hw), bg_rgb=rand(2, 3, *hw) if form == "factored_bg" else None)
     if misalign:
-        m[misalign] = _misaligned(m[misalign])
+        m[misalign] = misaligned(m[misalign], 8)
     V, _, H, W = geo["ray_dir"].shape
     descs, outs = [], []
     for tau in (0.0, None):
@@ -151,19 +137,18 @@ def _render(form, half, N=8, tex=64, Wt=None, img=256, views=2, misalign=None, s
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("form,half,kw,expect_why", LAUNCH_CASES)
-def test_each_launch_takes_the_kernel_its_plan_predicts(form, half, kw, expect_why, lib, variant):
+def test_each_launch_takes_the_kernel_its_plan_predicts(form, half, kw, expect_why, lib):
     assert torch.cuda.is_available(), "GPU tests need a CUDA device"
     kw = dict(kw)
-    variant(kw.pop("variant", "auto"))
-    (es, plain), (out_es, out_plain), keep = _render(form, half, **kw)
-    plan, why = _lib.fwd_plan(es)
-    assert why == expect_why and _lib.fwd_plan(plain) == (plan, why), (plan, why)
-    _lib.check(lib.gmpi_mpi_render_fwd_ex(ctypes.byref(es)))
-    skipped, total = ctypes.c_ulonglong(0), ctypes.c_ulonglong(0)
-    _lib.check(lib.gmpi_debug_fwd_early_stop_stats(ctypes.byref(skipped), ctypes.byref(total)))
-    stages = -(-es.W // 64) * -(-es.H // 30) * es.V * es.N
-    assert total.value == (stages if plan == _lib.PLAN_STAGED else 0), (plan, why, total.value, stages)
-    _lib.check(lib.gmpi_mpi_render_fwd_ex(ctypes.byref(plain)))
-    torch.cuda.synchronize()
+    with forced_kernel(kw.pop("variant", "auto")):
+        (es, plain), (out_es, out_plain), keep = _render(form, half, **kw)
+        plan, why = _lib.fwd_plan(es)
+        assert why == expect_why and _lib.fwd_plan(plain) == (plan, why), (plan, why)
+        _lib.check(lib.gmpi_mpi_render_fwd_ex(ctypes.byref(es)))
+        skipped, total = early_stop_stats()
+        stages = -(-es.W // 64) * -(-es.H // 30) * es.V * es.N
+        assert total == (stages if plan == _lib.PLAN_STAGED else 0), (plan, why, total, stages)
+        _lib.check(lib.gmpi_mpi_render_fwd_ex(ctypes.byref(plain)))
+        torch.cuda.synchronize()
     for k in ("color", "depth", "flags"):
-        assert torch.equal(out_es[k].view(torch.int32), out_plain[k].view(torch.int32)), k
+        assert_bitwise(out_es[k], out_plain[k], k)

@@ -21,6 +21,7 @@ from conftest import GOLDEN     # first: it puts the repository on sys.path when
 import ml_gmpi_b200 as g  # noqa: E402
 from ml_gmpi_b200 import _lib, mpi, synth  # noqa: E402
 from ml_gmpi_b200.camera import cam_params, focal_from_fov  # noqa: E402
+from testlib import dev, misaligned  # noqa: E402
 
 CALLS = os.path.join(GOLDEN, "binding_calls.json")
 
@@ -80,26 +81,13 @@ def _resolve(calls, names):
     return out
 
 
-def _dev():
-    return torch.device("cuda:0")
-
-
 def _geo(views=2, img=256):
     c = synth.make_case(n_planes=8, tex=8, img=img, n_mpi=2, views_per_mpi=views, seed=3, rgba=False)
-    return {k: getattr(c, k).to(_dev()) for k in ("dhw", "view2mpi", "ray_dir", "eye", "z_dir", "c2w")}
+    return {k: getattr(c, k).to(dev()) for k in ("dhw", "view2mpi", "ray_dir", "eye", "z_dir", "c2w")}
 
 
 def _rand(*shape, dtype=torch.float32, seed=1):
-    return torch.rand(shape, generator=torch.Generator().manual_seed(seed)).to(_dev(), dtype)
-
-
-def _misaligned(x):
-    """x's values in a buffer whose base is 8 bytes past a 16-byte boundary."""
-    off = 8 // x.element_size()
-    buf = torch.empty(x.numel() + 2 * off, dtype=x.dtype, device=x.device)
-    y = buf[off:off + x.numel()].view(x.shape)
-    y.copy_(x)
-    return y
+    return torch.rand(shape, generator=torch.Generator().manual_seed(seed)).to(dev(), dtype)
 
 
 def _views(names, **kw):
@@ -134,7 +122,7 @@ def _factored(dtype=torch.float32, bg=True, grad=False, **kw):
 
 def _backward(color, depth):
     gen = torch.Generator().manual_seed(9)
-    gc, gd = torch.randn(color.shape, generator=gen).to(_dev()), torch.randn(depth.shape, generator=gen).to(_dev())
+    gc, gd = torch.randn(color.shape, generator=gen).to(dev()), torch.randn(depth.shape, generator=gen).to(dev())
     ((color * gc).sum() + (depth * gd).sum()).backward()
 
 
@@ -172,7 +160,7 @@ def _frames(cam=False, factored=False, video=None, **kw):
         names.update(rgb=_rand(2, 3, 64, 64, seed=2), alpha=_rand(2, 8, 1, 64, 64, seed=3), bg_rgb=_rand(2, 3, 64, 64, seed=4))
     rays = dict(ray_dir=geo["ray_dir"], eye=geo["eye"], z_dir=geo["z_dir"])
     if cam:
-        names["cam"] = cam_params(geo["c2w"].cpu(), focal_from_fov(12.6, 256), 256, 256).to(_dev())
+        names["cam"] = cam_params(geo["c2w"].cpu(), focal_from_fov(12.6, 256), 256, 256).to(dev())
         rays = dict(cam=names["cam"], H=256, W=256)
 
     def call():
@@ -200,7 +188,7 @@ def _renderer():
     r = MPIRenderer(n_mpi_planes=8, plane_min_d=0.95, plane_max_d=1.12, plan_spatial_enlarge_factor=1.001,
                     plane_distances_sample_method="inverse", cam_fov=12.6, sphere_center_z=1.0, sphere_r=1.0,
                     horizontal_mean=0.0, horizontal_std=0.289, vertical_mean=0.0, vertical_std=0.127,
-                    cam_pose_n_truncated_stds=2, cam_sample_method="truncated_gaussian", device=_dev())
+                    cam_pose_n_truncated_stds=2, cam_sample_method="truncated_gaussian", device=dev())
     r.set_cam(12.6, 128, 128)
     names = dict(rgba=_rand(4, 8, 4, 64, 64))
     yaws, pitches = torch.tensor([[0.1], [-0.1], [0.05], [0.0]]), torch.tensor([[0.05], [0.0], [-0.05], [0.02]])
@@ -216,7 +204,7 @@ CASES = {
     "views_fp16_native": lambda: _expanded(torch.float16),
     "views_fp16_upcast": lambda: _expanded(torch.float16, Wt=68),          # Wt % 8 != 0: the fp16 plan is not the fp32 plan
     "views_fp64": lambda: _expanded(torch.float64),
-    "views_misaligned": lambda: _views(dict(_geo(), rgba=_misaligned(_rand(2, 8, 4, 64, 64)))),
+    "views_misaligned": lambda: _views(dict(_geo(), rgba=misaligned(_rand(2, 8, 4, 64, 64), 8))),
     "views_align_corners_false": lambda: _expanded(align_corners=False),
     "views_check_last_plane": lambda: _expanded(check_last_plane=True),
     "views_color_minus1_1": lambda: _expanded(color_minus1_1=True),

@@ -13,61 +13,24 @@ import torch
 
 import mpi_oracle
 import ml_gmpi_b200 as g
-from ml_gmpi_b200 import _lib, synth
+from ml_gmpi_b200 import synth
 from conftest import rel_err
+from testlib import dev, expanded_grad, factored_grads, forced_kernel, kernel_fixture, one_tile_per_mpi_case
 
 pytestmark = pytest.mark.gpu
 EXPECT = 2e-5
 _NT = max(1, min(64, (os.cpu_count() or 8)))
-
-
-def dev():
-    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
-    return torch.device("cuda:0")
-
-
-def _force(variant):
-    lib = _lib.load()
-    _lib.check(lib.gmpi_debug_set_fwd_variant(variant))
+bwd_variant = kernel_fixture("staged", "direct")
 
 
 @pytest.fixture
 def staged():
     """TMA-staged forward and box backward whatever the number of tiles."""
-    _force(2)
-    yield
-    _force(0)
-
-
-@pytest.fixture(params=["staged", "direct"])
-def bwd_variant(request):
-    _force({"direct": 1, "staged": 2}[request.param])
-    yield request.param
-    _force(0)
+    with forced_kernel("staged"):
+        yield
 
 
 n = lambda t: t.detach().cpu().numpy()
-
-
-def _expanded_grad(rgba, case, gc, gd, ray=None):
-    x = rgba.clone().requires_grad_(True)
-    color, depth = g.render_views(x, case.dhw, case.view2mpi, case.ray_dir if ray is None else ray, case.eye, case.z_dir)
-    loss = (color * gc).sum()
-    if gd is not None:
-        loss = loss + (depth * gd).sum()
-    loss.backward()
-    return n(x.grad)
-
-
-def _factored_grads(rgb, alpha, bg, case, gc, gd, ray=None):
-    r, a, b = (t.clone().requires_grad_(True) for t in (rgb, alpha, bg))
-    color, depth = g.render_views_factored(r, a, case.dhw, case.view2mpi, case.ray_dir if ray is None else ray, case.eye, case.z_dir,
-                                           bg_rgb=b)
-    loss = (color * gc).sum()
-    if gd is not None:
-        loss = loss + (depth * gd).sum()
-    loss.backward()
-    return n(r.grad), n(a.grad), n(b.grad)
 
 
 def _oracle(rgba, case, gc, gd, ray=None):
@@ -126,35 +89,25 @@ def test_magnified_texture_gradient_box_does_not_wrap(tex, pose, loss, staged):
         gc, gd = torch.ones((1, 3, img, img), device=d), torch.ones((1, 1, img, img), device=d)
     ref = _oracle(rgba, case, gc, gd)
     assert float(np.abs(ref).max()) > 0
-    e = rel_err(_expanded_grad(rgba, case, gc, gd), ref)
+    e = rel_err(expanded_grad(rgba, case, gc, gd), ref)
     assert e <= EXPECT, e
     rgba_f = g.expand_factored(rgb, alpha, bg)
-    _check_factored(_factored_grads(rgb, alpha, bg, case, gc, gd), _oracle(rgba_f, case, gc, gd))
+    _check_factored(factored_grads(rgb, alpha, bg, case, gc, gd), _oracle(rgba_f, case, gc, gd))
 
 
 # ------------------------------------------------------------------------------------------------------------------------
 # 2. the tile exponent tracks the gradient exactly
 # ------------------------------------------------------------------------------------------------------------------------
-def _one_tile_per_mpi_case(d):
-    """Two MPIs, one near-frontal view each, of ONE 64 x 24 backward tile (rows 20..43 of a 64^2 pinhole image): every
-    (tile, plane) takes the box, and every texel of g_rgba receives exactly one flush per plane, so the result does not
-    depend on the order of fp32 atomics."""
-    import dataclasses
-    case = synth.make_case(n_planes=6, tex=64, img=64, n_mpi=2, seed=13, device=d, last_alpha_one=True,
-                           yaws=[0.05, -0.08], pitches=[0.02, -0.03])
-    return dataclasses.replace(case, ray_dir=case.ray_dir[:, :, 20:44].contiguous())
-
-
 @pytest.mark.parametrize("k", [-40, -13, 0, 7, 40])
 def test_power_of_two_scaled_upstream_gradient_scales_the_result_bitwise(k, staged):
     d = dev()
-    case = _one_tile_per_mpi_case(d)
+    case = one_tile_per_mpi_case(d)
     gen = torch.Generator().manual_seed(4)
     gc = torch.randn((2, 3, 24, 64), generator=gen).to(d)
     gd = torch.randn((2, 1, 24, 64), generator=gen).to(d)
     s = 2.0 ** k
-    base = _expanded_grad(case.rgba, case, gc, gd)
-    scaled = _expanded_grad(case.rgba, case, gc * s, gd * s)
+    base = expanded_grad(case.rgba, case, gc, gd)
+    scaled = expanded_grad(case.rgba, case, gc * s, gd * s)
     assert np.array_equal(scaled, base * np.float32(s))
     assert rel_err(base, _oracle(case.rgba, case, gc, gd)) <= EXPECT
     # factored: per-plane alpha and the background colour get one flush per texel; the shared colour image sums the planes'
@@ -165,8 +118,8 @@ def test_power_of_two_scaled_upstream_gradient_scales_the_result_bitwise(k, stag
     # colour scale, where the box's error is bounded relative to that scale rather than to the background gradient itself
     alpha[:, :-1] *= 0.3
     alpha[:, -1] = 1.0
-    fb = _factored_grads(rgb, alpha, bg, case, gc, gd)
-    fs = _factored_grads(rgb, alpha, bg, case, gc * s, gd * s)
+    fb = factored_grads(rgb, alpha, bg, case, gc, gd)
+    fs = factored_grads(rgb, alpha, bg, case, gc * s, gd * s)
     assert np.array_equal(fs[1], fb[1] * np.float32(s)) and np.array_equal(fs[2], fb[2] * np.float32(s))
     assert rel_err(fs[0], fb[0] * np.float32(s)) <= 1e-6
     _check_factored(fb, _oracle(g.expand_factored(rgb, alpha, bg), case, gc, gd))
@@ -186,12 +139,12 @@ def test_extreme_upstream_gradient_magnitudes(scale, staged):
     gd = (torch.randn((2, 1, 128, 128), generator=gen) * scale).to(d)
     ref = _oracle(case.rgba, case, gc, gd)
     assert np.isfinite(ref).all() and float(np.abs(ref).max()) > 0
-    e = rel_err(_expanded_grad(case.rgba, case, gc, gd), ref)
+    e = rel_err(expanded_grad(case.rgba, case, gc, gd), ref)
     assert e <= EXPECT, e
     gen = torch.Generator(device=d).manual_seed(9)
     rgb, alpha, bg = (torch.rand(sh, generator=gen, device=d) for sh in ((2, 3, 128, 128), (2, 6, 1, 128, 128), (2, 3, 128, 128)))
     alpha[:, -1] = 1.0
-    _check_factored(_factored_grads(rgb, alpha, bg, case, gc, gd), _oracle(g.expand_factored(rgb, alpha, bg), case, gc, gd))
+    _check_factored(factored_grads(rgb, alpha, bg, case, gc, gd), _oracle(g.expand_factored(rgb, alpha, bg), case, gc, gd))
 
 
 # ------------------------------------------------------------------------------------------------------------------------
@@ -223,11 +176,11 @@ def test_nan_and_inf_upstream_gradients_propagate_like_autograd(bwd_variant):
     gc[0, 0, 30, 40] = float("nan")          # backward tile (px0, py0) = (0, 24)
     gd[0, 0, 100, 100] = float("inf")        # backward tile (64, 96)
     ref = _oracle(case.rgba, case, gc, gd)
-    _check_poisoned(_expanded_grad(case.rgba, case, gc, gd), ref, bwd_variant)
+    _check_poisoned(expanded_grad(case.rgba, case, gc, gd), ref, bwd_variant)
     gen = torch.Generator(device=d).manual_seed(11)
     rgb, alpha, bg = (torch.rand(sh, generator=gen, device=d) for sh in ((1, 3, 128, 128), (1, 6, 1, 128, 128), (1, 3, 128, 128)))
     alpha[:, -1] = 1.0
-    ours = _factored_grads(rgb, alpha, bg, case, gc, gd)
+    ours = factored_grads(rgb, alpha, bg, case, gc, gd)
     refs = _factored_refs(_oracle(g.expand_factored(rgb, alpha, bg), case, gc, gd))
     for o, r, tol in zip(ours, refs, (2 * EXPECT, EXPECT, EXPECT)):      # d rgb: see _check_factored
         _check_poisoned(o, r, bwd_variant, tol)

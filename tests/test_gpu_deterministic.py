@@ -13,7 +13,7 @@ import mpi_oracle
 import ml_gmpi_b200 as g
 from ml_gmpi_b200 import _lib, synth
 from conftest import rel_err
-from test_gpu_parity import each_alpha
+from testlib import assert_bitwise, dev, each_alpha, kernel_fixture
 
 pytestmark = pytest.mark.gpu
 EXPECT = 2e-5
@@ -21,18 +21,7 @@ _NT = max(1, min(64, (os.cpu_count() or 8)))
 n = lambda t: t.detach().cpu().numpy()
 
 
-def dev():
-    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
-    return torch.device("cuda:0")
-
-
-@pytest.fixture(params=["staged", "direct"])
-def variant(request):
-    """Staged forward + box backward (whatever the number of tiles), or the direct kernels."""
-    lib = _lib.load()
-    _lib.check(lib.gmpi_debug_set_fwd_variant({"direct": 1, "staged": 2}[request.param]))
-    yield request.param
-    _lib.check(lib.gmpi_debug_set_fwd_variant(0))
+variant = kernel_fixture("staged", "direct")     # staged forward + box backward (whatever the number of tiles), or the direct kernels
 
 
 def _grads(case, gc, gd, *, deterministic, factored=None, align_corners=True, view_group=1, ray=None, order=None):
@@ -73,11 +62,6 @@ def _factored_mpi(M, N, tex, seed, d):
     return rgb, alpha, bg
 
 
-def _bitwise(a, b):
-    for x, y in zip(a, b):
-        assert x.shape == y.shape and np.array_equal(x.view(np.uint32), y.view(np.uint32))
-
-
 def _check_accuracy(ours, default, ref, factored):
     """Within the oracle's bar (2e-5; the factored colour sums N-1 planes' roundings: twice that), and within the same bar of the
     default backward: the deterministic sums add at most 2^(E-k-1) per contribution and one fp32 rounding to the box kernel's
@@ -111,7 +95,7 @@ def test_repeatable_and_accurate(form, depth, align_corners, variant):
     kw = dict(factored=fac, align_corners=align_corners, view_group=vpm)
     a = _grads(case, gc, gd, deterministic=True, **kw)
     b = _grads(case, gc, gd, deterministic=True, **kw)
-    _bitwise(a, b)
+    assert_bitwise(a, b)
     rgba = case.rgba if fac is None else g.expand_factored(*fac)
     _check_accuracy(a, _grads(case, gc, gd, deterministic=False, **kw), _oracle(rgba, case, gc, gd, align_corners), fac is not None)
 
@@ -126,7 +110,7 @@ def test_view_order_does_not_change_a_bit(form, variant):
     fac = _factored_mpi(M, N, tex, 8, d) if form == "factored" else None
     base = _grads(case, gc, gd, deterministic=True, factored=fac)
     for order in ([2, 0, 1, 5, 3, 4], [4, 5, 3, 1, 2, 0]):
-        _bitwise(base, _grads(case, gc, gd, deterministic=True, factored=fac, order=torch.tensor(order, device=d)))
+        assert_bitwise(base, _grads(case, gc, gd, deterministic=True, factored=fac, order=torch.tensor(order, device=d)))
 
 
 @each_alpha("variant", ["staged", "direct"], indirect=["variant"])
@@ -138,7 +122,7 @@ def test_full_size_training_shape_is_repeatable(variant, alpha):
     case = synth.make_case(n_planes=96, tex=1024, img=1024, n_mpi=4, seed=3, device=d, last_alpha_one=True, alpha=alpha)
     gc, gd = _upstream(4, 1024, 1024, 9, d)
     a = _grads(case, gc, gd, deterministic=True)
-    _bitwise(a, _grads(case, gc, gd, deterministic=True))
+    assert_bitwise(a, _grads(case, gc, gd, deterministic=True))
     e = rel_err(a[0], _grads(case, gc, gd, deterministic=False)[0])
     assert e <= EXPECT, e
     v0 = lambda t: n(t[:1])
@@ -154,7 +138,7 @@ def test_fifteen_views_of_one_mpi_are_repeatable(variant):
     case = synth.make_case(n_planes=96, tex=512, img=512, n_mpi=1, views_per_mpi=15, seed=4, device=d, last_alpha_one=True)
     gc, gd = _upstream(15, 512, 512, 10, d)
     a = _grads(case, gc, gd, deterministic=True, view_group=15)
-    _bitwise(a, _grads(case, gc, gd, deterministic=True, view_group=15))
+    assert_bitwise(a, _grads(case, gc, gd, deterministic=True, view_group=15))
     e = rel_err(a[0], _grads(case, gc, gd, deterministic=False, view_group=15)[0])
     assert e <= EXPECT, e
 
@@ -169,11 +153,11 @@ def test_magnified_texture(tex, variant):
     case = synth.make_case(n_planes=N, tex=tex, img=img, n_mpi=1, seed=3, device=d, yaws=[0.35], pitches=[-0.15], last_alpha_one=True)
     gc, gd = torch.ones((1, 3, img, img), device=d), torch.ones((1, 1, img, img), device=d)
     a = _grads(case, gc, gd, deterministic=True)
-    _bitwise(a, _grads(case, gc, gd, deterministic=True))
+    assert_bitwise(a, _grads(case, gc, gd, deterministic=True))
     _check_accuracy(a, _grads(case, gc, gd, deterministic=False), _oracle(case.rgba, case, gc, gd), False)
     fac = _factored_mpi(1, N, tex, 12, d)
     a = _grads(case, gc, gd, deterministic=True, factored=fac)
-    _bitwise(a, _grads(case, gc, gd, deterministic=True, factored=fac))
+    assert_bitwise(a, _grads(case, gc, gd, deterministic=True, factored=fac))
     _check_accuracy(a, _grads(case, gc, gd, deterministic=False, factored=fac), _oracle(g.expand_factored(*fac), case, gc, gd), True)
 
 
@@ -185,13 +169,13 @@ def test_extreme_upstream_gradient_magnitudes(scale, variant):
     gc = (torch.randn((2, 3, 128, 128), generator=gen) * scale).to(d)
     gd = (torch.randn((2, 1, 128, 128), generator=gen) * scale).to(d)
     a = _grads(case, gc, gd, deterministic=True)
-    _bitwise(a, _grads(case, gc, gd, deterministic=True))
+    assert_bitwise(a, _grads(case, gc, gd, deterministic=True))
     ref = _oracle(case.rgba, case, gc, gd)
     assert np.isfinite(ref).all() and float(np.abs(ref).max()) > 0
     _check_accuracy(a, _grads(case, gc, gd, deterministic=False), ref, False)
     fac = _factored_mpi(2, 6, 128, 9, d)
     a = _grads(case, gc, gd, deterministic=True, factored=fac)
-    _bitwise(a, _grads(case, gc, gd, deterministic=True, factored=fac))
+    assert_bitwise(a, _grads(case, gc, gd, deterministic=True, factored=fac))
     _check_accuracy(a, _grads(case, gc, gd, deterministic=False, factored=fac), _oracle(g.expand_factored(*fac), case, gc, gd), True)
 
 
@@ -213,7 +197,7 @@ def test_non_finite_upstream_gradients(variant):
         b = _grads(case, gc, gd, deterministic=True, factored=f)
         ref = _grads(case, gc, gd, deterministic=False, factored=f)
         for x, y, r in zip(a, b, ref):
-            assert np.array_equal(x.view(np.uint32), y.view(np.uint32))
+            assert_bitwise(x, y)
             bad = ~np.isfinite(r)
             assert bad.any()
             for kind in (np.isnan, np.isposinf, np.isneginf):
@@ -289,7 +273,7 @@ def test_torch_deterministic_switch_selects_the_deterministic_backward(monkeypat
     finally:
         torch.use_deterministic_algorithms(was)
     assert len(calls) == 2
-    _bitwise([a], [b])
+    assert_bitwise([a], [b])
     assert rel_err(a, default) <= EXPECT
     # the constructor's option overrides the switch, in both directions
     _train_step(case, gc, gd, g.MPI(align_corners=True, deterministic=True))

@@ -14,80 +14,12 @@ import torch
 import mpi_oracle
 import ml_gmpi_b200 as g
 from ml_gmpi_b200 import _lib, synth
-from conftest import MPI_CASES, load_golden
-from test_early_stop import max_plane_depth
+from testlib import CASES, assert_bitwise, case, dev, early_stop_stats, forced_kernel, kernel_fixture, max_plane_depth
 
 pytestmark = pytest.mark.gpu
 EXPECT = 2e-5
 TAUS = [2.0 ** -24, 1e-3, 0.05]
-_VARIANTS = {"direct": (1, 0), "staged": (2, 0), "staged2": (2, 2), "staged3": (2, 3)}   # (kernel variant, ring depth)
-
-
-def dev():
-    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
-    return torch.device("cuda:0")
-
-
-def set_variant(name):
-    lib = _lib.load()
-    variant, stages = _VARIANTS.get(name, (0, 0))
-    _lib.check(lib.gmpi_debug_set_fwd_variant(variant))
-    _lib.check(lib.gmpi_debug_set_fwd_stages(stages))
-
-
-@pytest.fixture(params=["direct", "staged2", "staged3"])
-def variant(request):
-    set_variant(request.param)
-    yield request.param
-    set_variant("auto")
-
-
-def _golden(name):
-    gd = load_golden(name)
-    return dict(rgba=gd["rgba"], view2mpi=gd["view2mpi"], dhw=gd["dhw"], ray_dir=gd["ray_dir"], eye=gd["eye"], z_dir=gd["z_dir"],
-                ac=bool(gd["align_corners"]))
-
-
-def _synth(n_planes, tex, img, n_mpi, views=1, seed=0, alpha_scale=None, crop=None, tex_hw=None, ac=True, view_group=1,
-           factored=False, video=False):
-    case = synth.make_case(n_planes=n_planes, tex=tex, img=img, n_mpi=n_mpi, views_per_mpi=views, seed=seed, last_alpha_one=True)
-    rgba = case.rgba
-    if tex_hw is not None:
-        rgba = torch.rand((n_mpi, n_planes, 4) + tex_hw, generator=torch.Generator().manual_seed(seed))
-        rgba[:, -1, 3] = 1.0
-    if alpha_scale is not None:
-        rgba = rgba.clone()
-        rgba[:, :-1, 3] *= alpha_scale
-    ray = case.ray_dir if crop is None else case.ray_dir[:, :, crop[0]:crop[1]].contiguous()
-    c = dict(rgba=rgba.numpy(), view2mpi=case.view2mpi.numpy(), dhw=case.dhw.numpy(), ray_dir=ray.numpy(), eye=case.eye.numpy(),
-             z_dir=case.z_dir.numpy(), ac=ac, view_group=view_group, video=video)
-    if factored:      # one shared colour image, the last plane's own colour, per-plane alpha
-        gen = torch.Generator().manual_seed(seed + 1)
-        rgb, bg = torch.rand((n_mpi, 3) + rgba.shape[-2:], generator=gen), torch.rand((n_mpi, 3) + rgba.shape[-2:], generator=gen)
-        alpha = torch.from_numpy(c["rgba"][:, :, 3:4].copy())
-        c.update(factored=(rgb.numpy(), alpha.numpy(), bg.numpy()), rgba=g.expand_factored(rgb, alpha, bg).numpy())
-    return c
-
-
-SYNTH = {
-    "small": lambda: _synth(16, 64, 96, 2, views=2, seed=1),
-    "view_group3": lambda: _synth(24, 96, 128, 1, views=3, seed=2, view_group=3),
-    "factored": lambda: _synth(24, 96, 128, 2, views=2, seed=3, factored=True),
-    "factored_view_group2": lambda: _synth(12, 64, 96, 1, views=2, seed=4, factored=True, view_group=2),
-    "uint8": lambda: _synth(16, 64, 96, 2, views=2, seed=5, video=True),
-    "N1": lambda: _synth(1, 128, 160, 2, seed=6),
-    "N2": lambda: _synth(2, 128, 160, 2, seed=7),
-    "N512": lambda: _synth(512, 96, 128, 2, seed=8, alpha_scale=0.02),
-    "partial_acfalse_nonsquare": lambda: _synth(10, 8, 136, 2, views=2, seed=9, crop=(18, 118), tex_hw=(72, 116), ac=False),
-}
-
-
-@functools.lru_cache(maxsize=None)
-def case(name):
-    return SYNTH[name]() if name in SYNTH else _golden(name)
-
-
-CASES = MPI_CASES + ["c1_full_256"] + list(SYNTH)
+variant = kernel_fixture("direct", "staged2", "staged3")
 
 
 @functools.lru_cache(maxsize=None)
@@ -112,15 +44,10 @@ def render(name, early_stop=None):
     return a.cpu().numpy(), b.cpu().numpy()
 
 
-def bits(a):
-    return a.view(np.uint32) if a.dtype == np.float32 else a
-
-
 @pytest.mark.parametrize("name", CASES)
 def test_tau_zero_is_bitwise_early_stop_off(name, variant):
     off, zero = render(name), render(name, early_stop=0.0)
-    for x, y in zip(off, zero):
-        assert np.array_equal(bits(x), bits(y)), float(np.max(np.abs(x.astype(np.float64) - y)))
+    assert_bitwise(off, zero, name)
 
 
 def _check_bound(name, got, ref, tau, factor=1.0):
@@ -150,20 +77,11 @@ def test_early_stop_stays_within_its_bound(name, tau, variant):
 @pytest.mark.parametrize("tau", TAUS)
 @pytest.mark.parametrize("name", ["small", "factored", "N512", "partial_acfalse_nonsquare", "c1_full_256", "alpha_one_planes"])
 def test_staged_and_direct_agree_within_twice_the_bound(name, tau):
-    try:
-        set_variant("direct")
+    with forced_kernel("direct"):
         direct = render(name, early_stop=tau)
-        set_variant("staged")           # staged kernel at the ring depth it picks itself
+    with forced_kernel("staged"):           # staged kernel at the ring depth it picks itself
         staged = render(name, early_stop=tau)
-    finally:
-        set_variant("auto")
     _check_bound(name, staged, direct, tau, factor=2.0)
-
-
-def _stats():
-    s, t = ctypes.c_ulonglong(), ctypes.c_ulonglong()
-    _lib.check(_lib.load().gmpi_debug_fwd_early_stop_stats(ctypes.byref(s), ctypes.byref(t)))
-    return s.value, t.value
 
 
 def _stop_planes(c, tau):
@@ -209,19 +127,16 @@ def test_structured_workload_skips_stages_within_the_bound(stages, factored):
         c["rgba"] = g.expand_factored(rgb, torch.from_numpy(c["rgba"][:, :, 3:4].copy())).numpy()
     else:
         mpi = dict(rgba=t(c["rgba"]))
-    set_variant(stages)
-    try:
-        out = {}
+    out = {}
+    with forced_kernel(stages):
         for tau_ in (None, 0.0, tau, 0.05):
             with torch.no_grad():
                 col, dep = g.render_frames(dhw=t(c["dhw"]), view2mpi=t(c["view2mpi"]), ray_dir=t(c["ray_dir"]), eye=t(c["eye"]),
                                            z_dir=t(c["z_dir"]), view_group=V, early_stop=tau_, **mpi)
             out[tau_] = (col.cpu().numpy(), dep.cpu().numpy())
             if tau_ is not None:
-                out[("stats", tau_)] = _stats()
-    finally:
-        set_variant("auto")
-    assert all(np.array_equal(bits(x), bits(y)) for x, y in zip(out[None], out[0.0]))
+                out[("stats", tau_)] = early_stop_stats()
+    assert_bitwise(out[None], out[0.0])
     tiles = -(-R // 64) * -(-R // 30) * V
     assert out[("stats", 0.0)][1] == tiles * N
     for tau_ in (tau, 0.05):      # the producer lags a stopped tile by at most the ring depth; these tiles stop ~N/2 planes early

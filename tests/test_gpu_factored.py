@@ -42,9 +42,8 @@ import mpi_oracle
 import ml_gmpi_b200 as g
 from ml_gmpi_b200 import _lib, synth
 from conftest import MPI_CASES, load_golden, rel_err
-from test_gpu_early_stop import set_variant
-from test_gpu_half import _limit_footprints
-from test_gpu_bwd_limits import _expanded_grad, _factored_grads, _one_tile_per_mpi_case
+from testlib import (assert_bitwise, dev, expanded_grad, factored_grads, forced_kernel, kernel_fixture, limit_footprints, misaligned,
+                     one_tile_per_mpi_case)
 
 pytestmark = pytest.mark.gpu
 EXPECT = 2e-5
@@ -53,18 +52,9 @@ ROUND_RGB = 2.0 ** -(FIX_BITS_RGB - 1)   # largest rounding of one colour contri
 _NT = max(1, min(64, (os.cpu_count() or 8)))
 
 
-def dev():
-    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
-    return torch.device("cuda:0")
-
-
-@pytest.fixture(params=["direct", "staged"])
-def variant(request):
-    """The direct kernels, or the staged forward + box backward forced whatever the number of tiles (the factored ring is always 3
-    deep: gmpi_debug_set_fwd_stages does not apply to it).  Restores the automatic choice."""
-    set_variant(request.param)
-    yield request.param
-    set_variant("auto")
+# The direct kernels, or the staged forward + box backward forced whatever the number of tiles (the factored ring is always 3 deep:
+# the ring depth does not apply to it).
+variant = kernel_fixture("direct", "staged")
 
 
 # ------------------------------------------------------------------------------------------------------------------------------
@@ -124,7 +114,7 @@ def _n512():
 
 
 def _wide(tex_hw, seed):
-    """16 planes of a wide texture at 720^2 from three random poses (test_gpu_half._limit_case): 512 x 1024 gives many footprints 89..96
+    """16 planes of a wide texture at 720^2 from three random poses (testlib.limit_case): 512 x 1024 gives many footprints 89..96
     texels wide, which the factored forward's 96-wide box could hold but which take the generic body in the forward (as in the expanded
     ring: the bodies' bilinear weights differ in the last bit) and in the backward (classes 56..88); 512 x 1536 gives footprints wider
     than 96."""
@@ -344,10 +334,6 @@ def _dev_tensors(c, with_bg):
     return mpi, geo
 
 
-def _same_bits(a, b):
-    return a.shape == b.shape and torch.equal(a.view(torch.int32), b.view(torch.int32))
-
-
 def fwd_plan(c, mpi, view_group=1):
     V, _, H, W = c["ray_dir"].shape
     M, N, _, Ht, Wt = c["alpha"].shape
@@ -367,20 +353,20 @@ def run(name, with_bg, mpi=None, view_group=1):
     flags = lambda: torch.zeros(1, dtype=torch.int32, device=d)
     x = g.expand_factored(*base)
     if any(t is not None and t.data_ptr() % 16 for t in mpi):
-        x = _misaligned(x)                  # the expanded stack takes the direct kernel too
+        x = misaligned(x, 4)                # the expanded stack takes the direct kernel too
     with torch.no_grad():
         ff, fe = flags(), flags()
         cf, df = g.render_views_factored(mpi[0], mpi[1], *geo, bg_rgb=mpi[2], flags=ff, **kw)
         ce, de = g.render_views(x, *geo, flags=fe, **kw)
-    assert _same_bits(cf, ce) and _same_bits(df, de), (name, "forward-only kernel != expanded")
+    assert_bitwise((cf, df), (ce, de), (name, "forward-only kernel != expanded"))
     assert int(ff.item()) == int(fe.item())
     leaves = [None if v is None else v.detach().requires_grad_(True) for v in mpi]
     xe = x.detach().requires_grad_(True)
     ft, fte = flags(), flags()
     col, dep = g.render_views_factored(leaves[0], leaves[1], *geo, bg_rgb=leaves[2], flags=ft, **kw)
     ce2, de2 = g.render_views(xe, *geo, flags=fte, **kw)
-    assert _same_bits(col.detach(), ce2.detach()) and _same_bits(dep.detach(), de2.detach()), (name, "training forward != expanded")
-    assert _same_bits(col.detach(), cf) and _same_bits(dep.detach(), df)
+    assert_bitwise((col, dep), (ce2, de2), (name, "training forward != expanded"))
+    assert_bitwise((col, dep), (cf, df), (name, "training forward != forward-only kernel"))
     del ce2, de2, xe, x
     gc = torch.from_numpy(c["gc"]).to(d)
     loss = (col * gc).sum()
@@ -420,9 +406,9 @@ def test_factored_matches_the_oracle(name, with_bg, variant):
     else:
         assert p == "staged", why
     if name == "band_89_96":
-        assert _limit_footprints(_shim(c), 89, 96) > 0
+        assert limit_footprints(_shim(c), 89, 96) > 0
     if name == "wider_than_96":
-        assert _limit_footprints(_shim(c), 97, 1 << 30) > 0
+        assert limit_footprints(_shim(c), 97, 1 << 30) > 0
     ours = run(name, with_bg)
     if name == "N1" and with_bg:
         assert not ours["g_rgb"].any()              # the one plane is the background: nothing reaches rgb
@@ -430,7 +416,7 @@ def test_factored_matches_the_oracle(name, with_bg, variant):
 
 
 def _shim(c):
-    """c as test_gpu_half._limit_footprints reads it (it takes the sizes from an expanded stack)."""
+    """c as testlib.limit_footprints reads it (it takes the sizes from an expanded stack)."""
     M, N, _, Ht, Wt = c["alpha"].shape
     return dict(c, rgba=np.broadcast_to(np.float32(0), (M, N, 4, Ht, Wt)))
 
@@ -439,12 +425,11 @@ def _shim(c):
 # 2. one integer flush per texel and plane: the factored box backward is bitwise the expanded one
 # ------------------------------------------------------------------------------------------------------------------------------
 def test_one_tile_per_mpi_factored_gradients_are_bitwise_the_expanded_ones():
-    """test_gpu_bwd_limits._one_tile_per_mpi_case: every texel gets exactly one integer flush per plane, so d alpha and d bg of the
+    """testlib.one_tile_per_mpi_case: every texel gets exactly one integer flush per plane, so d alpha and d bg of the
     staged factored backward equal the expanded backward's g_rgba[:, :, 3] and g_rgba[:, -1, :3] bit for bit."""
     d = dev()
-    set_variant("staged")
-    try:
-        geo = _one_tile_per_mpi_case(d)
+    with forced_kernel("staged"):
+        geo = one_tile_per_mpi_case(d)
         gen = torch.Generator().manual_seed(4)
         gc = torch.randn((2, 3, 24, 64), generator=gen).to(d)
         gd = torch.randn((2, 1, 24, 64), generator=gen).to(d)
@@ -452,13 +437,10 @@ def test_one_tile_per_mpi_factored_gradients_are_bitwise_the_expanded_ones():
         rgb, alpha, bg = (torch.rand(sh, generator=gen, device=d) for sh in ((2, 3, 64, 64), (2, 6, 1, 64, 64), (2, 3, 64, 64)))
         alpha[:, :-1] *= 0.3
         alpha[:, -1] = 1.0
-        f_rgb, f_alpha, f_bg = _factored_grads(rgb, alpha, bg, geo, gc, gd)
-        e = _expanded_grad(g.expand_factored(rgb, alpha, bg), geo, gc, gd)
-    finally:
-        set_variant("auto")
-    assert np.array_equal(f_alpha[:, :, 0].view(np.uint32), e[:, :, 3].view(np.uint32)), \
-        float(np.max(np.abs(f_alpha[:, :, 0] - e[:, :, 3])))
-    assert np.array_equal(f_bg.view(np.uint32), e[:, -1, :3].view(np.uint32)), float(np.max(np.abs(f_bg - e[:, -1, :3])))
+        f_rgb, f_alpha, f_bg = factored_grads(rgb, alpha, bg, geo, gc, gd)
+        e = expanded_grad(g.expand_factored(rgb, alpha, bg), geo, gc, gd)
+    assert_bitwise(f_alpha[:, :, 0], e[:, :, 3], "d alpha")
+    assert_bitwise(f_bg, e[:, -1, :3], "d bg_rgb")
     assert rel_err(f_rgb, e[:, :-1, :3].astype(np.float64).sum(1)) <= 1e-6         # fp32 atomics over the planes: order only
 
 
@@ -511,7 +493,7 @@ def test_view_group_changes_no_output_bit_and_no_gradient_beyond_the_bar(variant
     ref = reference(name, True)
     for vg, o in outs.items():
         for k in ("color", "depth"):
-            assert np.array_equal(o[k].view(np.uint32), outs[1][k].view(np.uint32)), (vg, k)
+            assert_bitwise(o[k], outs[1][k], (vg, k))
         check(f"{name}/view_group={vg}/{variant}", o, name, True)
         # and against view_group = 1 with the same bars (the group-1 result as the reference)
         one = dict(ref, **{k: outs[1][k] for k in ("color", "depth", "g_alpha", "g_bg")},
@@ -520,22 +502,13 @@ def test_view_group_changes_no_output_bit_and_no_gradient_beyond_the_bar(variant
         assert all(e[k] <= b[k] for k in b), (vg, e, b)
 
 
-def _misaligned(x):
-    """x's values in a buffer whose base is 4 bytes past a 16-byte boundary."""
-    buf = torch.empty(x.numel() + 4, dtype=x.dtype, device=x.device)
-    y = buf[1:1 + x.numel()].view(x.shape)
-    y.copy_(x)
-    assert y.data_ptr() % 16 == 4
-    return y
-
-
 @pytest.mark.parametrize("which", ["rgb", "alpha", "bg_rgb"])
 def test_one_unaligned_factor_takes_the_direct_kernels(which, variant):
     name = "small"
     c = case(name)
     mpi, _ = _dev_tensors(c, True)
     i = ["rgb", "alpha", "bg_rgb"].index(which)
-    mpi = tuple(_misaligned(t) if j == i else t for j, t in enumerate(mpi))
+    mpi = tuple(misaligned(t, 4) if j == i else t for j, t in enumerate(mpi))
     p, why = fwd_plan(c, mpi)
     assert p == "direct" and why & 8, (p, why)
     check(f"{name}/unaligned_{which}/{variant}", run(name, True, mpi=mpi), name, True, p)
@@ -562,8 +535,7 @@ def test_host_entry_point_with_ray_tensors_is_bitwise_the_device_call(with_bg, v
     df = torch.zeros(1, dtype=torch.int32, device=d)
     _lib.check(lib.gmpi_mpi_render_fwd_ex(ctypes.byref(_lib.make_desc(color=dc, depth=dd, flags=df, **sizes, **t))))
     torch.cuda.synchronize()
-    assert np.array_equal(color.view(np.uint32), dc.cpu().numpy().view(np.uint32))
-    assert np.array_equal(depth.view(np.uint32), dd.cpu().numpy().view(np.uint32))
+    assert_bitwise((color, depth), (dc, dd), "host entry point != device entry point")
     assert int(flags[0]) == int(df.item())
     ref = reference(name, with_bg)
     assert rel_err(color, 2 * ref["color"] - 1) <= EXPECT and rel_err(depth, ref["depth"]) <= EXPECT

@@ -20,27 +20,15 @@ from ml_gmpi_b200 import _lib, synth
 from ml_gmpi_b200.camera import PinholeCamera, cam_params, focal_from_fov
 from ml_gmpi_b200.geometry import FFHQ
 from conftest import rel_err
+from testlib import dev, kernel_fixture, video_reference
 
 pytestmark = pytest.mark.gpu
 EXPECT = 2e-5
 
 
-def dev():
-    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
-    return torch.device("cuda:0")
-
-
-@pytest.fixture(params=["direct", "staged", "staged2", "staged3"])
-def fwd_variant(request):
-    """Direct gather, or the TMA-staged forward at the ring depth it picks itself or forced to a 2- or 3-stage ring (expanded MPI;
-    the factored forward's ring is 3 deep)."""
-    lib = _lib.load()
-    variant, stages = {"direct": (1, 0), "staged": (2, 0), "staged2": (2, 2), "staged3": (2, 3)}[request.param]
-    _lib.check(lib.gmpi_debug_set_fwd_variant(variant))
-    _lib.check(lib.gmpi_debug_set_fwd_stages(stages))
-    yield request.param
-    _lib.check(lib.gmpi_debug_set_fwd_variant(0))
-    _lib.check(lib.gmpi_debug_set_fwd_stages(0))
+# Direct gather, or the TMA-staged forward at the ring depth it picks itself or forced to a 2- or 3-stage ring (expanded MPI; the
+# factored forward's ring is 3 deep).
+fwd_variant = kernel_fixture("direct", "staged", "staged2", "staged3")
 
 
 def factored_case(n_planes, tex, img, n_mpi, views_per_mpi, seed, with_bg):
@@ -117,18 +105,6 @@ def test_view_grouped_tile_order_changes_nothing(fwd_variant):
         assert rel_err(gr.cpu().numpy(), outs[0][2].cpu().numpy()) <= 1e-6      # atomics: summation order only
 
 
-def _video_reference(color_m11, depth, near, far):
-    """gmpi/eval/vis/render_video.py:118-126, verbatim arithmetic on numpy float32 arrays."""
-    img = color_m11.permute(0, 2, 3, 1).cpu().numpy()
-    img = (img + 1) / 2.0
-    img = (img * 255).astype(np.uint8)
-    depth_map = depth.permute(0, 2, 3, 1).cpu().numpy()
-    depth_map = (depth_map - near) / (far - near)
-    depth_map = np.clip(depth_map, 0, 1)
-    depth_map = (depth_map * 255).astype(np.uint8)
-    return img, depth_map
-
-
 def test_video_epilogue_equals_reference_conversion(fwd_variant):
     d = dev()
     case = synth.make_case(n_planes=32, tex=256, img=256, n_mpi=1, views_per_mpi=5, seed=12, device=d, last_alpha_one=True,
@@ -137,7 +113,7 @@ def test_video_epilogue_equals_reference_conversion(fwd_variant):
     c, dp = g.render_views(case.rgba, case.dhw, case.view2mpi, case.ray_dir, case.eye, case.z_dir, color_minus1_1=True)
     u8, d8 = g.render_frames(rgba=case.rgba, dhw=case.dhw, view2mpi=case.view2mpi, ray_dir=case.ray_dir, eye=case.eye, z_dir=case.z_dir,
                              video={"near": near, "far": far}, view_group=5)
-    ref_img, ref_depth = _video_reference(c, dp, near, far)
+    ref_img, ref_depth = video_reference(c, dp, near, far)
     assert u8.shape == (5, 256, 256, 3) and d8.shape == (5, 256, 256, 1)
     assert np.array_equal(u8.cpu().numpy(), ref_img) and np.array_equal(d8.cpu().numpy(), ref_depth)
     assert 20 < int(ref_img.std()) and int(ref_depth.max()) > 100          # the frames are not trivially constant
@@ -226,7 +202,7 @@ def test_video_service_equals_the_per_view_reference_loop():
     for i, a in enumerate(angles):
         im, dm, _, _ = r.render(mpi, I, I, horizontal_mean=a, horizontal_std=0.0, vertical_mean=0.0, vertical_std=0.0,
                                 assert_not_out_of_last_plane=True)
-        ref_img, ref_depth = _video_reference(im, dm, near, far)
+        ref_img, ref_depth = video_reference(im, dm, near, far)
         # The service rotates the camera rays of all its views in ONE batched matmul, the loop one view at a time: cuBLAS may sum
         # the three products in a different order, the rays differ in the last ulp and a white-noise MPI turns that into a grey
         # level on a few pixels.  (With identical rays the frames are identical: test_video_epilogue_equals_reference_conversion.)

@@ -32,32 +32,13 @@ from ml_gmpi_b200 import _lib
 from ml_gmpi_b200.mpi import MPI, MPIOutOfPlaneError
 from ml_gmpi_b200.synth import ffhq_dhw, make_poses
 from ml_gmpi_b200.camera import cam_params
-from test_oracle_golden import FLAG_CASES, FORWARD_FLAGS
+from testlib import FLAG_CASES, FORWARD_FLAGS, dev, forced_kernel, kernel_fixture
 
 gpu = pytest.mark.gpu
 OOB, BEHIND = mpi_oracle.FLAG_LAST_PLANE_OOB, mpi_oracle.FLAG_PLANE_BEHIND_EYE
 OPT_AC, OPT_CHECK, OPT_M11, OPT_ES, OPT_F16 = (_lib.OPT_ALIGN_CORNERS, _lib.OPT_CHECK_LAST_PLANE, _lib.OPT_COLOR_MINUS1_1,
                                                _lib.OPT_EARLY_STOP, _lib.OPT_MPI_F16)
-_VARIANTS = {"auto": (0, 0), "direct": (1, 0), "staged2": (2, 2), "staged3": (2, 3)}
-
-
-def set_variant(name):
-    lib = _lib.load()
-    v, s = _VARIANTS[name]
-    _lib.check(lib.gmpi_debug_set_fwd_variant(v))
-    _lib.check(lib.gmpi_debug_set_fwd_stages(s))
-
-
-@pytest.fixture(params=["direct", "staged2", "staged3"])
-def variant(request):
-    set_variant(request.param)
-    yield request.param
-    set_variant("auto")
-
-
-def dev():
-    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
-    return torch.device("cuda:0")
+variant = kernel_fixture("direct", "staged2", "staged3")
 
 
 # ------------------------------------------------------------------------------------------------------------------------------
@@ -376,8 +357,7 @@ EXCEPTIONS = {"alpha": (AssertionError, "Expected alpha to be within the the ran
 @gpu
 @pytest.mark.parametrize("kernel", ["direct", "staged2"])
 def test_mpi_module_raises_the_reference_exception_for_each_verdict(kernel):
-    set_variant(kernel)
-    try:
+    with forced_kernel(kernel):
         for name, verdict, c in FLAG_CASES:
             full = MPI(align_corners=bool(c["align_corners"]), validate="full")
             if verdict == "ok":
@@ -399,8 +379,6 @@ def test_mpi_module_raises_the_reference_exception_for_each_verdict(kernel):
             off = MPI(align_corners=bool(c["align_corners"]), validate="off")
             _mpi_call(off, c)
             assert off.last_flags() == FORWARD_FLAGS[verdict] & ~OOB, (name, off.last_flags())
-    finally:
-        set_variant("auto")
 
 
 # ------------------------------------------------------------------------------------------------------------------------------

@@ -11,36 +11,15 @@ import numpy as np
 import pytest
 import torch
 
-import mpi_oracle
 import ml_gmpi_b200 as g
 from ml_gmpi_b200 import _lib, synth
 from ml_gmpi_b200.camera import cam_params
-from test_gpu_early_stop import CASES, _synth, case, set_variant
+from testlib import (CASES, assert_bitwise, assert_class_88_behind_plane_25, case, dev, forced_kernel, forward_desc, headline_case,
+                     kernel_fixture, limit_case, limit_footprints, misaligned, native_vs_fp32, render_fwd)
 
 pytestmark = pytest.mark.gpu
 TAUS = [None, 0.0, 2.0 ** -24, 1e-3]
-
-
-def dev():
-    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
-    return torch.device("cuda:0")
-
-
-@pytest.fixture(params=["direct", "staged2", "staged3"])
-def variant(request):
-    set_variant(request.param)
-    yield request.param
-    set_variant("auto")
-
-
-def _misaligned(x):
-    """x's values in a buffer whose base is 8 bytes past a 16-byte boundary."""
-    off = 8 // x.element_size()
-    buf = torch.empty(x.numel() + 2 * off, dtype=x.dtype, device=x.device)
-    y = buf[off:off + x.numel()].view(x.shape)
-    y.copy_(x)
-    assert y.data_ptr() % 16 == 8
-    return y
+variant = kernel_fixture("direct", "staged2", "staged3")
 
 
 def _mpi(c, half, bg=True, misalign=False):
@@ -53,60 +32,13 @@ def _mpi(c, half, bg=True, misalign=False):
     else:
         m = dict(rgba=q(c["rgba"]))
     if misalign:
-        m = {k: None if v is None else _misaligned(v) for k, v in m.items()}
+        m = {k: None if v is None else misaligned(v, 8) for k, v in m.items()}
     return m
 
 
-def _desc(c, m, half, tau=None, cam=None, u8_round=False, view_group=None):
-    d = dev()
-    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(d)
-    ref = m["alpha"] if "alpha" in m else m["rgba"]
-    V, _, H, W = c["ray_dir"].shape
-    out = {}
-    if c.get("video"):
-        out = dict(video_rgb=torch.empty((V, H, W, 3), dtype=torch.uint8, device=d),
-                   video_depth=torch.empty((V, H, W, 1), dtype=torch.uint8, device=d), depth_near=0.9, depth_range=np.float32(0.3).item())
-    else:
-        out = dict(color=torch.empty((V, 3, H, W), device=d), depth=torch.empty((V, 1, H, W), device=d))
-    rays = dict(cam=cam) if cam is not None else dict(ray_dir=t(c["ray_dir"]), eye=t(c["eye"]), z_dir=t(c["z_dir"]))
-    opts = (_lib.OPT_ALIGN_CORNERS if c["ac"] else 0) | _lib.OPT_COLOR_MINUS1_1 | (_lib.OPT_U8_ROUND_HALF_UP if u8_round else 0) \
-        | (_lib.OPT_EARLY_STOP if tau is not None else 0) | (_lib.OPT_MPI_F16 if half else 0)
-    flags = torch.zeros(1, dtype=torch.int32, device=d)
-    keep = dict(view2mpi=t(c["view2mpi"]), dhw=t(c["dhw"]), flags=flags, **rays, **out, **m)
-    desc = _lib.make_desc(options=opts, M=ref.shape[0], V=V, N=ref.shape[1], Ht=ref.shape[-2], Wt=ref.shape[-1], H=H, W=W,
-                          view_group=c.get("view_group", 1) if view_group is None else view_group, early_stop=tau, **keep)
-    return desc, keep
-
-
-def run(c, half, **kw):
-    """(outputs..., flags) of one gmpi_mpi_render_fwd_ex call, as numpy."""
-    mkw = {k: kw.pop(k) for k in ("bg", "misalign") if k in kw}
-    desc, keep = _desc(c, _mpi(c, half, **mkw), half, **kw)
-    _lib.check(_lib.load().gmpi_mpi_render_fwd_ex(ctypes.byref(desc)))
-    torch.cuda.synchronize()
-    names = ("video_rgb", "video_depth") if "video_rgb" in keep else ("color", "depth")
-    return tuple(keep[n].cpu().numpy() for n in names) + (keep["flags"].cpu().numpy(),)
-
-
-def assert_bitwise(a, b, what):
-    for x, y in zip(a, b):
-        assert x.dtype == y.dtype and np.array_equal(x.view(np.uint8), y.view(np.uint8)), \
-            (what, float(np.max(np.abs(x.astype(np.float64) - y))))
-
-
-def run_pair(c, variant, **kw):
+def run_pair(c, variant, bg=True, misalign=False, **kw):
     """fp16 render and the fp32 render of the upcast, on the kernel the fp16 call gets under `variant`."""
-    h = run(c, True, **kw)
-    mkw = {k: kw[k] for k in ("bg", "misalign") if k in kw}
-    desc, _ = _desc(c, _mpi(c, True, **mkw), True, **{k: v for k, v in kw.items() if k not in mkw})
-    fell_back = variant != "direct" and _lib.fwd_plan(desc)[0] == _lib.PLAN_DIRECT
-    if fell_back:
-        set_variant("direct")
-    try:
-        f = run(c, False, **kw)
-    finally:
-        set_variant(variant)
-    return h, f, fell_back
+    return native_vs_fp32(c, _mpi(c, True, bg, misalign), _mpi(c, False, bg, misalign), variant, **kw)
 
 
 @pytest.mark.parametrize("name", CASES)
@@ -136,30 +68,27 @@ def test_fp16_render_with_cam_rays(name, variant):
 def test_unaligned_and_narrow_fp16_fall_back_to_the_direct_kernel():
     """An fp16 base 8 bytes off a 16-byte boundary, or Wt % 8 != 0 (with Wt % 4 == 0): the plan query says why, the call runs
     the direct kernel, and the output is bitwise the direct kernel's on the upcast (the staged kernel would differ in the last bits)."""
-    set_variant("staged3")
-    try:
+    with forced_kernel("staged3"):
         c = case("small")
-        desc, _ = _desc(c, _mpi(c, True, misalign=True), True)
+        desc, _ = forward_desc(c, _mpi(c, True, misalign=True))
         assert _lib.fwd_plan(desc) == (_lib.PLAN_DIRECT, 8)
-        desc32, _ = _desc(c, _mpi(c, False), False)
+        desc32, _ = forward_desc(c, _mpi(c, False))
         assert _lib.fwd_plan(desc32) == (_lib.PLAN_STAGED, 0)
         for tau in (None, 1e-3):
             h, f, fell_back = run_pair(c, "staged3", misalign=True, tau=tau)
             assert fell_back
             assert_bitwise(h, f, ("misaligned", tau))
         n = case("partial_acfalse_nonsquare")        # texture 72 x 116: 116 % 8 == 4
-        desc, _ = _desc(n, _mpi(n, True), True)
+        desc, _ = forward_desc(n, _mpi(n, True))
         assert _lib.fwd_plan(desc) == (_lib.PLAN_DIRECT, 1)
-        desc32, _ = _desc(n, _mpi(n, False), False)
+        desc32, _ = forward_desc(n, _mpi(n, False))
         assert _lib.fwd_plan(desc32) == (_lib.PLAN_STAGED, 0)
         h, f, fell_back = run_pair(n, "staged3")
         assert fell_back
         assert_bitwise(h, f, "Wt % 8")
-        set_variant("direct")
-        h32 = run(n, False)
-        assert_bitwise(h, h32, "Wt % 8 vs the direct kernel on the upcast")
-    finally:
-        set_variant("auto")
+    with forced_kernel("direct"):
+        h32 = render_fwd(n, _mpi(n, False))
+    assert_bitwise(h, h32, "Wt % 8 vs the direct kernel on the upcast")
 
 
 @pytest.mark.parametrize("name", ["small", "factored", "uint8"])
@@ -188,7 +117,7 @@ def test_host_entry_point_takes_fp16_host_buffers(name):
         _lib.check(lib.gmpi_mpi_render_host_ex(ctypes.byref(d), 0))
         outs.append(tuple(o.values()) + (flags.view(np.int32),))
     assert_bitwise(outs[0], outs[1], name)
-    assert_bitwise(outs[0], run(c, True, view_group=1), (name, "device entry point"))
+    assert_bitwise(outs[0], render_fwd(c, _mpi(c, True), view_group=1), (name, "device entry point"))
 
 
 def test_range_flags_match_the_fp32_check_of_the_upcast():
@@ -232,15 +161,15 @@ def test_render_views_passes_fp16_natively_without_an_fp32_copy():
         peak = torch.cuda.max_memory_allocated() - base
     outputs = sum(t.numel() * t.element_size() for t in out)
     assert peak <= outputs + (1 << 20), (peak, outputs, x16.numel() * 4)       # no fp32 copy of the MPI (8 MB here)
-    assert_bitwise([t.cpu().numpy() for t in out], [t.cpu().numpy() for t in ref], "render_views")
+    assert_bitwise(out, ref, "render_views")
     f = dict(rgb=x16[:, 0, :3].contiguous(), alpha=x16[:, :, 3:4].contiguous())
     with torch.no_grad():
         a = g.render_views_factored(f["rgb"], f["alpha"], *args)
         b = g.render_views_factored(f["rgb"].float(), f["alpha"].float(), *args)
         v = g.render_frames(rgba=x16, dhw=c.dhw, view2mpi=c.view2mpi, ray_dir=c.ray_dir, eye=c.eye, z_dir=c.z_dir, early_stop=1e-3)
         w = g.render_frames(rgba=x16.float(), dhw=c.dhw, view2mpi=c.view2mpi, ray_dir=c.ray_dir, eye=c.eye, z_dir=c.z_dir, early_stop=1e-3)
-    assert_bitwise([t.cpu().numpy() for t in a], [t.cpu().numpy() for t in b], "render_views_factored")
-    assert_bitwise([t.cpu().numpy() for t in v], [t.cpu().numpy() for t in w], "render_frames")
+    assert_bitwise(a, b, "render_views_factored")
+    assert_bitwise(v, w, "render_frames")
 
 
 def test_mpi_forward_on_fp16_matches_the_upcast():
@@ -253,7 +182,7 @@ def test_mpi_forward_on_fp16_matches_the_upcast():
     with torch.no_grad():
         a = g.MPI(validate="full")(**kw(x16))
         b = g.MPI(validate="full")(**kw(x16.float()))
-    assert_bitwise([t.cpu().numpy() for t in a], [t.cpu().numpy() for t in b], "MPI.forward")
+    assert_bitwise(a, b, "MPI.forward")
     bad = x16.clone()
     bad[0, 3, 3, 5, 5] = -0.25
     with torch.no_grad(), pytest.raises(AssertionError, match="alpha"):
@@ -272,14 +201,15 @@ def test_fp16_that_requires_grad_takes_the_upcast_path():
         outs.append([color.detach().cpu().numpy(), depth.detach().cpu().numpy()])
         grads.append(x.grad.cpu().numpy())
     assert_bitwise(outs[0], outs[1], "output")
-    assert grads[0].dtype == np.float16 and np.array_equal(grads[0].view(np.uint16), grads[1].view(np.uint16))
+    assert grads[0].dtype == np.float16
+    assert_bitwise(grads[0], grads[1], "gradient")
 
 
 def test_fp16_refusals_on_device_buffers():
     """Refused with GMPI_ERR_UNSUPPORTED: together with a transmittance output, on the backward, on the classic entry points."""
     c = case("small")
     lib = _lib.load()
-    desc, keep = _desc(c, _mpi(c, True), True)
+    desc, keep = forward_desc(c, _mpi(c, True))
     V, _, H, W = c["ray_dir"].shape
     trans = torch.empty((V, c["rgba"].shape[1], H, W), device=dev())
     desc.transmittance = trans.data_ptr()
@@ -292,42 +222,6 @@ def test_fp16_refusals_on_device_buffers():
     p = [keep[k].data_ptr() for k in ("rgba", "view2mpi", "dhw", "ray_dir", "eye", "z_dir", "color", "depth", "flags")]
     assert lib.gmpi_mpi_render_fwd(*p, M, V, N, Ht, Wt, H, W, _lib.OPT_MPI_F16, None) == 3
     torch.cuda.synchronize()
-
-
-@functools.lru_cache(maxsize=None)
-def _limit_case(factored):
-    """A 512 x 1024 texture seen at 720^2 from three random poses: 1.4 texels per pixel across a tile (64 pixels), 0.7 down it.
-    Many (tile, plane) footprints need the widest box classes, at origins where the fp16 box starts 4 texels further west."""
-    return _synth(16, 8, 720, 1, views=3, seed=21, tex_hw=(512, 1024), factored=factored)
-
-
-def footprints(c):
-    """mpi_oracle.footprints of case c's staged forward (the producer's box of every (view, tile, plane) stage)."""
-    M, N, _, Ht, Wt = c["rgba"].shape
-    return mpi_oracle.footprints(c["view2mpi"], c["dhw"], c["ray_dir"], c["eye"], Ht, Wt, c["ac"])
-
-
-def _limit_footprints(c, lo, hi):
-    """(tile, plane) stages whose fp32 box lies under the tile with rows that fit a stage (mode 0, or mode 2 only for a width need
-    above kMaxBW = 88) with a width need in [lo, hi] and an origin 4 texels past a multiple of 8."""
-    f = footprints(c)
-    fits = (f["mode"] != 1) & (-(-f["need_h"] // 4) * 4 <= mpi_oracle.FWD_TILE[1])
-    return int((fits & (f["need_w"] >= lo) & (f["need_w"] <= hi) & (f["bx0"] % 8 == 4)).sum())
-
-
-@functools.lru_cache(maxsize=None)
-def headline_case():
-    """One view of the headline MPI, 96 x 1024^2, with equal-weight alpha (synth.equal_weight_alpha): every plane, the back ones
-    with the widest boxes included, reaches the render, so a back-plane tap the native kernel staged or converted wrongly changes
-    the bits of the output (with U(0, 1) alpha it would be absorbed by the rounding of the accumulator)."""
-    cs = synth.make_case(n_planes=96, tex=1024, img=1024, n_mpi=1, seed=1234, alpha="equal_weight")
-    return dict(rgba=cs.rgba.numpy(), view2mpi=cs.view2mpi.numpy(), dhw=cs.dhw.numpy(), ray_dir=cs.ray_dir.numpy(),
-                eye=cs.eye.numpy(), z_dir=cs.z_dir.numpy(), ac=True)
-
-
-def assert_class_88_behind_plane_25(c):
-    cls = footprints(c)["cls"]
-    assert (cls[..., 25:] == 88).any() and all((cls == k).any() for k in range(56, 96, 8))
 
 
 @pytest.mark.parametrize("stages", ["staged2", "staged3"])
@@ -344,17 +238,14 @@ def test_fp16_at_the_widest_box_classes(factored, stages):
         assert_class_88_behind_plane_25(c)
         factored = False
     else:
-        c = _limit_case(factored)
-        assert _limit_footprints(c, 85, 88) > 0 and (not factored or _limit_footprints(c, 93, 96) > 0)
-    set_variant(stages)
-    try:
+        c = limit_case(factored)
+        assert limit_footprints(c, 85, 88) > 0 and (not factored or limit_footprints(c, 93, 96) > 0)
+    with forced_kernel(stages):
         for kw in ([{}, dict(bg=False)] if factored else [{}]):
             for tau in (None, 1e-3):
                 h, f, fell_back = run_pair(c, stages, tau=tau, **kw)
                 assert not fell_back
                 assert_bitwise(h, f, (factored, stages, tau, kw))
-    finally:
-        set_variant("auto")
 
 
 def test_fp16_that_requires_grad_renders_under_no_grad():
@@ -369,7 +260,7 @@ def test_fp16_that_requires_grad_renders_under_no_grad():
                  (g.render_frames(rgba=x, dhw=c.dhw, view2mpi=c.view2mpi, ray_dir=c.ray_dir, eye=c.eye, z_dir=c.z_dir),
                   g.render_frames(rgba=x.float(), dhw=c.dhw, view2mpi=c.view2mpi, ray_dir=c.ray_dir, eye=c.eye, z_dir=c.z_dir))]
     for a, b in pairs:
-        assert_bitwise([t.cpu().numpy() for t in a], [t.cpu().numpy() for t in b], "no_grad")
+        assert_bitwise(a, b, "no_grad")
     v2m = c.view2mpi.cpu().numpy()
     idx = [np.nonzero(v2m == m)[0] for m in range(2)]
     kw = lambda rgba: dict(batch_rgba=rgba, batch_dhw=c.dhw, batch_ray_dir=[c.ray_dir[i] for i in idx],
@@ -377,4 +268,4 @@ def test_fp16_that_requires_grad_renders_under_no_grad():
     with torch.no_grad():
         a = g.MPI(validate="full")(**kw(x))
         b = g.MPI(validate="full")(**kw(x.float()))
-    assert_bitwise([t.cpu().numpy() for t in a], [t.cpu().numpy() for t in b], "MPI.forward under no_grad")
+    assert_bitwise(a, b, "MPI.forward under no_grad")

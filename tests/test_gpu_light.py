@@ -8,13 +8,9 @@ import torch
 from ml_gmpi_b200.light import LightRenderer, alpha_depth, apply_shading
 from ml_gmpi_b200 import expand_factored
 from conftest import load_golden, rel_err
+from testlib import dev
 
 pytestmark = pytest.mark.gpu
-
-
-def dev():
-    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
-    return torch.device("cuda:0")
 
 
 def make_lr():

@@ -44,16 +44,12 @@ import torch
 from ml_gmpi_b200 import light
 from ml_gmpi_b200.geometry import FFHQ, plane_dhw_table, texel_xyzd
 from ml_gmpi_b200.light import LightRenderer, alpha_depth, apply_shading
+from testlib import dev
 
 pytestmark = pytest.mark.gpu
 U = 2.0 ** -24
 MIN_NORMAL = 2.0 ** -126
 MIN_SUBNORMAL = 2.0 ** -149
-
-
-def dev():
-    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
-    return torch.device("cuda:0")
 
 
 def report(tag, **kw):

@@ -46,7 +46,7 @@ import mpi_oracle
 from ml_gmpi_b200 import _lib, synth
 from ml_gmpi_b200.camera import cam_params
 from conftest import MPI_CASES, load_golden, rel_err
-from test_gpu_early_stop import set_variant
+from testlib import assert_bitwise, dev, forced_kernel, kernel_fixture, set_kernel
 
 gpu = pytest.mark.gpu
 EXPECT = 2e-5
@@ -56,30 +56,13 @@ OPT_AC, OPT_CHECK, OPT_M11, OPT_ES, OPT_F16 = (_lib.OPT_ALIGN_CORNERS, _lib.OPT_
                                                _lib.OPT_EARLY_STOP, _lib.OPT_MPI_F16)
 
 
-def dev():
-    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
-    return torch.device("cuda:0")
-
-
-@pytest.fixture(params=["direct", "staged2", "staged3"])
-def variant(request):
-    """The direct kernels, or the staged forward forced at a 2- or 3-stage ring whatever the number of tiles (the factored forward
-    keeps its 3-stage ring).  Restores the automatic choice."""
-    set_variant(request.param)
-    yield request.param
-    set_variant("auto")
+# The direct kernels, or the staged forward forced at a 2- or 3-stage ring whatever the number of tiles (the factored forward keeps
+# its 3-stage ring).
+variant = kernel_fixture("direct", "staged2", "staged3")
 
 
 def _t(a):
     return torch.from_numpy(np.ascontiguousarray(a)).to(dev())
-
-
-def _bits(x):
-    return x.contiguous().view(torch.int32)
-
-
-def _same_bits(a, b):
-    return a.shape == b.shape and torch.equal(_bits(a), _bits(b))
 
 
 def _sentinel(n):
@@ -193,9 +176,9 @@ def check_frames(bufs, ref, offset, label):
     V = ref.shape[0]
     for r, b in enumerate(bufs):
         got = b[offset:offset + V]
-        assert _same_bits(got, ref), (label, r, float((got - ref).abs().nan_to_num(float("inf")).max()))
+        assert_bitwise(got, ref, (label, r))
         rest = torch.cat([b[:offset].flatten(), b[offset + V:].flatten()])
-        assert bool((_bits(rest) == SENTINEL).all()), (label, r, "a store outside slots [offset, offset + V)")
+        assert bool((rest.view(torch.int32) == SENTINEL).all()), (label, r, "a store outside slots [offset, offset + V)")
 
 
 def _gather_matrix():
@@ -214,7 +197,7 @@ def test_fused_gather_frames_are_the_packed_plain_render(shape, form, variant):
     if variant != "direct":
         assert p == "staged"             # Wt = 64: the staged kernel also in fp16
     ref, ref_flags = packed_reference(inputs)
-    assert not bool((_bits(ref) == SENTINEL).any()), "the plain call left pixels unwritten"
+    assert not bool((ref.view(torch.int32) == SENTINEL).any()), "the plain call left pixels unwritten"
     V = c["V"]
     F = V + 3
     for n_peers, offset in ((1, 0), (2, F - V), (2, 1)):
@@ -228,7 +211,7 @@ def test_fused_gather_frames_are_the_packed_plain_render(shape, form, variant):
 @pytest.mark.parametrize("form", ["fp32", "factored_bg", "fp16", "early_stop_1e-3", "cam", "view_group2"])
 def test_fused_gather_plans_the_staged_kernel_at_120_tiles(form):
     """4 views of 256^2 = 144 tiles of 64 x 30: the automatic choice is the staged kernel, with peer_frames set."""
-    set_variant("auto")
+    set_kernel("auto")
     c = gather_case(256, 256, n_mpi=2, views=2, N=16, tex=128, img=256, seed=12)
     inputs = _form_inputs(c, form)
     ref, ref_flags = packed_reference(inputs)
@@ -242,7 +225,7 @@ def test_fused_gather_plans_the_staged_kernel_at_120_tiles(form):
 def test_fused_gather_one_rank_of_the_two_gpu_headline():
     """One rank's share of the 2-GPU headline: 4 MPIs x 96 planes x 1024^2, frames 4..7 of two [8,4,1024,1024] buffers, automatic
     choice (the staged kernel on its 2-stage ring: every view has its own MPI, larger than L2)."""
-    set_variant("auto")
+    set_kernel("auto")
     d = dev()
     M, N, R = 4, 96, 1024
     geo = synth.make_case(n_planes=N, tex=8, img=R, n_mpi=M, seed=1234, rgba=False)
@@ -449,9 +432,9 @@ def _t_buffer(V, N, H, W):
 
 
 def _check_t_buffer(buf, T, label):
-    b = _bits(buf)
+    b = buf.view(torch.int32)
     assert bool((b[:PAD] == SENTINEL).all()) and bool((b[-PAD:] == SENTINEL).all()), (label, "store outside the T buffer")
-    assert not bool((_bits(T) == SENTINEL).any()), (label, "T element left unwritten")
+    assert not bool((T.view(torch.int32) == SENTINEL).any()), (label, "T element left unwritten")
 
 
 def _out(V, H, W):
@@ -471,7 +454,7 @@ def training_forward(c, factored=False, classic=True):
     tr_flags = _fwd(inputs, transmittance=T, **tr)
     _check_t_buffer(buf, T, "descriptor")
     for k in ("color", "depth"):
-        assert _same_bits(tr[k], inf[k]), (k, "training forward != inference forward")
+        assert_bitwise(tr[k], inf[k], (k, "training forward != inference forward"))
     assert tr_flags == inf_flags
     if classic and not factored:
         lib = _lib.load()
@@ -488,10 +471,10 @@ def training_forward(c, factored=False, classic=True):
         _lib.check(lib.gmpi_mpi_render_fwd(*geo, cf["color"].data_ptr(), cf["depth"].data_ptr(), fflags.data_ptr(), *sizes, None))
         torch.cuda.synchronize()
         _check_t_buffer(cbuf, cT, "gmpi_mpi_render_fwd_train")
-        assert _same_bits(cT, T), "gmpi_mpi_render_fwd_train T != descriptor T"
+        assert_bitwise(cT, T, "gmpi_mpi_render_fwd_train T != descriptor T")
         for k in ("color", "depth"):
-            assert _same_bits(ct[k], inf[k]), (k, "gmpi_mpi_render_fwd_train != inference forward")
-            assert _same_bits(cf[k], inf[k]), (k, "gmpi_mpi_render_fwd != gmpi_mpi_render_fwd_ex")
+            assert_bitwise(ct[k], inf[k], (k, "gmpi_mpi_render_fwd_train != inference forward"))
+            assert_bitwise(cf[k], inf[k], (k, "gmpi_mpi_render_fwd != gmpi_mpi_render_fwd_ex"))
         assert int(cflags.item()) == inf_flags and int(fflags.item()) == inf_flags
     return dict(T=T, flags=tr_flags, plan=_plan(_lib.make_desc(**inputs))[0], **tr)
 
@@ -527,7 +510,7 @@ def test_saved_transmittance_against_float64_and_training_equals_inference(name,
             assert (T[v, :, y, x] == 1).all(), (v, y, x, T[v, :, y, x])
     fac = training_forward(c, factored=True)
     assert fac["plan"] == ours["plan"] or variant == "direct"
-    assert _same_bits(fac["T"], ours["T"]), (name, variant, "factored T != expanded T")
+    assert_bitwise(fac["T"], ours["T"], (name, variant, "factored T != expanded T"))
 
 
 @gpu
@@ -584,16 +567,13 @@ def test_classic_backward_entry_points_match_the_oracle(name):
         torch.cuda.synchronize()
         return g.cpu().numpy()
 
-    try:
-        set_variant("direct")
+    with forced_kernel("direct"):
         T_direct = train_t()
         grads = dict(bwd_two_pass=bwd(), bwd_saved_direct=bwd(T_direct))
-        set_variant("staged3")
+    with forced_kernel("staged3"):
         assert _plan(_lib.make_desc(**i))[0] == "staged"
         T_staged = train_t()
         grads.update(bwd_saved_box=bwd(T_staged), bwd_saved_box_direct_T=bwd(T_direct))
-    finally:
-        set_variant("auto")
     e = {k: rel_err(v, ref) for k, v in grads.items()}
     print("CLASSIC_BWD " + json.dumps(dict(case=name, err={k: float("%.3g" % v) for k, v in e.items()},
                                            T_forms_differ=float((T_direct - T_staged).abs().max()))))

@@ -14,6 +14,7 @@ import mpi_oracle
 import ml_gmpi_b200 as g
 from ml_gmpi_b200 import _lib
 from conftest import MPI_CASES, load_golden, rel_err
+from testlib import dev, each_alpha, kernel_fixture
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-4          # the north star's bar
@@ -22,36 +23,11 @@ TOL = 1e-4          # the north star's bar
 EXPECT = 2e-5
 
 
-def dev():
-    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
-    return torch.device("cuda:0")
-
-
-_VARIANTS = {"direct": (1, 0), "staged": (2, 0), "staged2": (2, 2), "staged3": (2, 3)}   # (kernel variant, ring depth)
-
-
-def _variant(request):
-    lib = _lib.load()
-    variant, stages = _VARIANTS[request.param]
-    _lib.check(lib.gmpi_debug_set_fwd_variant(variant))
-    _lib.check(lib.gmpi_debug_set_fwd_stages(stages))
-    yield request.param
-    _lib.check(lib.gmpi_debug_set_fwd_variant(0))
-    _lib.check(lib.gmpi_debug_set_fwd_stages(0))
-
-
-@pytest.fixture(params=["direct", "staged", "staged2", "staged3"])
-def fwd_variant(request):
-    """Runs a test once per forward kernel: the direct gather (1), and the TMA-staged kernel (2) at the ring depth it picks itself
-    and forced to a 2- and a 3-stage ring (the expanded forward's two depths; the factored forward's ring is always 3 deep).
-    Then restores auto."""
-    yield from _variant(request)
-
-
-@pytest.fixture(params=["direct", "staged"])
-def fwd_variant_auto(request):
-    """Direct gather, or the TMA-staged kernel at the ring depth it picks itself (the full-size cases)."""
-    yield from _variant(request)
+# Each test runs once per forward kernel: the direct gather, and the TMA-staged kernel at the ring depth it picks itself and forced
+# to a 2- and a 3-stage ring (the expanded forward's two depths; the factored forward's ring is always 3 deep).  The full-size cases
+# run the direct gather and the staged kernel at the ring depth it picks itself.
+fwd_variant = kernel_fixture("direct", "staged", "staged2", "staged3")
+fwd_variant_auto = kernel_fixture("direct", "staged")
 
 
 def groups(gd, device):
@@ -220,7 +196,6 @@ def _ffhq_case(N, res, V, seed=1234, device=None):
 # The full-size cases run on two MPIs: U(0, 1) alpha, and equal-weight alpha (synth.equal_weight_alpha).  Under U(0, 1) alpha the
 # transmittance falls as e^-i and planes past ~25 move the render and its gradient by less than the bar, so only the equal-weight
 # MPI checks the back planes, where the widest box classes occur (tests/test_every_plane_weight.py).
-ALPHAS = ["uniform", "equal_weight"]
 _C4_YAWS = np.linspace(0.5, -0.5, 120).astype(np.float32)[::8]
 FULL = {   # name: synth.make_case arguments
     "full_32x256": dict(n_planes=32, tex=256, img=256, n_mpi=8, seed=1234),
@@ -246,18 +221,6 @@ def _oracle_forward(name, alpha):
     rc, rd, _ = mpi_oracle.forward(n(case.rgba), n(case.view2mpi), n(case.dhw), n(case.ray_dir), n(case.eye), n(case.z_dir),
                                    nthreads=_NT)
     return rc, rd
-
-
-def each_alpha(argnames, sets, indirect=()):
-    """parametrize(argnames + ",alpha") over sets x ALPHAS.  The U(0, 1) sets keep the ids they had before the equal-weight input
-    was added; the equal-weight ones end in "-equal_weight"."""
-    params = []
-    for alpha in ALPHAS:
-        for vals in sets:
-            vals = vals if isinstance(vals, tuple) else (vals,)
-            ident = "-".join(str(v) for v in vals) + ("" if alpha == "uniform" else "-" + alpha)
-            params.append(pytest.param(*vals, alpha, id=ident))
-    return pytest.mark.parametrize(argnames + ",alpha", params, indirect=list(indirect))
 
 
 @each_alpha("N,res,V", [(32, 256, 8), (96, 512, 2), (96, 1024, 1)])

@@ -23,44 +23,16 @@ from ml_gmpi_b200.camera import cam_params, focal_from_fov
 from ml_gmpi_b200.geometry import AFHQCAT, FFHQ, METFACES
 from ml_gmpi_b200.mpi import unorm8_to_float
 from conftest import load_golden, rel_err
-from test_early_stop import max_plane_depth
-from test_gpu_features import _video_reference
+from testlib import ALPHAS, assert_bitwise, dev, forced_kernel, kernel_fixture, max_plane_depth, video_reference
 
 pytestmark = pytest.mark.gpu
 EXPECT = 2e-5
 GEOMETRIES = {"ffhq": FFHQ, "afhqcat": AFHQCAT, "metfaces": METFACES}
-ALPHAS = ["uniform", "equal_weight"]
-_VARIANTS = {"direct": (1, 0), "staged": (2, 0), "staged2": (2, 2), "staged3": (2, 3)}   # (kernel variant, ring depth)
 _NT = max(1, min(64, os.cpu_count() or 8))
-
-
-def dev():
-    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
-    return torch.device("cuda:0")
-
-
-def set_variant(name):
-    lib = _lib.load()
-    variant, stages = _VARIANTS.get(name, (0, 0))
-    _lib.check(lib.gmpi_debug_set_fwd_variant(variant))
-    _lib.check(lib.gmpi_debug_set_fwd_stages(stages))
-
-
-@pytest.fixture(params=list(_VARIANTS))
-def variant(request):
-    """The direct kernels, or the staged forward at the ring depth it picks itself or forced to a 2- or 3-stage ring.  Restores the
-    automatic choice."""
-    set_variant(request.param)
-    yield request.param
-    set_variant("auto")
-
-
-@pytest.fixture(params=["staged2", "staged3"])
-def ring(request):
-    """The staged forward at both ring depths (the opt-in forms' relations hold on the kernel that runs them)."""
-    set_variant(request.param)
-    yield request.param
-    set_variant("auto")
+# The direct kernels, or the staged forward at the ring depth it picks itself or forced to a 2- or 3-stage ring; and the staged
+# forward at both ring depths (the opt-in forms' relations hold on the kernel that runs them).
+variant = kernel_fixture("direct", "staged", "staged2", "staged3")
+ring = kernel_fixture("staged2", "staged3")
 
 
 def n(t):
@@ -165,20 +137,16 @@ def test_forward_every_view_against_the_oracle(name, alpha):
     case = full_case(name, alpha)
     rc, rd, rflags = oracle_forward(name, alpha)
     assert rflags == 0
-    try:
-        for v in ("direct", "staged2", "staged3"):
-            set_variant(v)
-            flags = torch.zeros(1, dtype=torch.int32, device=dev())
-            with torch.no_grad():
-                color, depth = g.render_views(case.rgba, case.dhw, case.view2mpi, case.ray_dir, case.eye, case.z_dir,
-                                              check_last_plane=True, flags=flags)
-            ec = [rel_err(n(color[i]), rc[i]) for i in range(rc.shape[0])]
-            ed = [rel_err(n(depth[i]), rd[i]) for i in range(rd.shape[0])]
-            report("ENVELOPE_FWD", case=name, alpha=alpha, variant=v, color=max(ec), depth=max(ed))
-            assert max(ec) <= EXPECT and max(ed) <= EXPECT, (v, ec, ed)
-            assert int(flags.item()) == rflags, (v, int(flags.item()))
-    finally:
-        set_variant("auto")
+    for v in ("direct", "staged2", "staged3"):
+        flags = torch.zeros(1, dtype=torch.int32, device=dev())
+        with forced_kernel(v), torch.no_grad():
+            color, depth = g.render_views(case.rgba, case.dhw, case.view2mpi, case.ray_dir, case.eye, case.z_dir, check_last_plane=True,
+                                          flags=flags)
+        ec = [rel_err(n(color[i]), rc[i]) for i in range(rc.shape[0])]
+        ed = [rel_err(n(depth[i]), rd[i]) for i in range(rd.shape[0])]
+        report("ENVELOPE_FWD", case=name, alpha=alpha, variant=v, color=max(ec), depth=max(ed))
+        assert max(ec) <= EXPECT and max(ed) <= EXPECT, (v, ec, ed)
+        assert int(flags.item()) == rflags, (v, int(flags.item()))
 
 
 @pytest.mark.parametrize("tag", list(GEOMETRIES))
@@ -218,19 +186,17 @@ def test_backward_against_the_oracle(name, alpha):
     the deterministic backward, which must repeat bit for bit."""
     case = full_case(name, alpha)
     ref = oracle_backward(name, alpha)
-    try:
-        for v in ("direct", "staged"):
-            set_variant(v)
+    for v in ("direct", "staged"):
+        with forced_kernel(v):
             e = rel_err(_grad(case), ref)
-            report("ENVELOPE_BWD", case=name, alpha=alpha, variant=v, grad=e)
-            assert e <= EXPECT, (v, e)
-    finally:
-        set_variant("auto")
+        report("ENVELOPE_BWD", case=name, alpha=alpha, variant=v, grad=e)
+        assert e <= EXPECT, (v, e)
     if name.startswith("afhqcat"):
         a, b = _grad(case, deterministic=True), _grad(case, deterministic=True)
         e = rel_err(a, ref)
         report("ENVELOPE_BWD", case=name, alpha=alpha, variant="deterministic", grad=e)
-        assert e <= EXPECT and np.array_equal(a.view(np.uint32), b.view(np.uint32)), e
+        assert e <= EXPECT, e
+        assert_bitwise(a, b, "deterministic")
 
 
 # ------------------------------------------------------------------------------------------------------------------------------
@@ -242,10 +208,6 @@ FORM_TAGS = ["afhqcat", "metfaces"]        # the two envelopes that put the most
 @functools.lru_cache(maxsize=1)
 def form_case(tag):
     return envelope_case(tag, 96, 512, CORNERS, alpha="equal_weight", seed=7)
-
-
-def _same_bits(a, b):
-    return a.shape == b.shape and a.dtype == b.dtype and torch.equal(a.contiguous().view(torch.uint8), b.contiguous().view(torch.uint8))
 
 
 @pytest.mark.parametrize("tag", FORM_TAGS)
@@ -264,7 +226,7 @@ def test_factored_equals_expanded_and_its_backward_matches_the_oracle(tag, ring)
                                          color_minus1_1=True)
         ce, de = g.render_views(g.expand_factored(rgb, alpha, bg), c.dhw, c.view2mpi, c.ray_dir, c.eye, c.z_dir, check_last_plane=True,
                                 color_minus1_1=True)
-    assert _same_bits(cf, ce) and _same_bits(df, de)
+    assert_bitwise((cf, df), (ce, de), "factored != expanded")
     leaves = [t.clone().requires_grad_(True) for t in (rgb, alpha, bg)]
     color, depth = g.render_views_factored(leaves[0], leaves[1], c.dhw, c.view2mpi, c.ray_dir, c.eye, c.z_dir, bg_rgb=leaves[2])
     gc, gd = upstream(c)
@@ -286,13 +248,13 @@ def test_fp16_and_uint8_are_bitwise_their_fp32_conversions(tag, ring):
         x16 = c.rgba.half()
         h = g.render_views(x16, *args, **kw)
         f = g.render_views(x16.float(), *args, **kw)
-        assert all(_same_bits(a, b) for a, b in zip(h, f)), "fp16"
+        assert_bitwise(h, f, "fp16")
         u8 = torch.from_numpy(np.clip(np.rint(n(c.rgba).astype(np.float64) * 255), 0, 255).astype(np.uint8)).to(c.rgba.device)
         conv = (u8.cpu().float() / 255).to(c.rgba.device)           # torch's CPU division: each quotient rounded once
         assert torch.equal(unorm8_to_float(u8), conv)
         q = g.render_views(u8, *args, unorm8=True, **kw)
         f = g.render_views(conv, *args, **kw)
-        assert all(_same_bits(a, b) for a, b in zip(q, f)), "uint8"
+        assert_bitwise(q, f, "uint8")
 
 
 @pytest.mark.parametrize("tag", FORM_TAGS)
@@ -302,7 +264,7 @@ def test_skip_empty_is_bitwise_the_plain_render(tag, ring):
     for extra in ({}, dict(video={"near": GEOMETRIES[tag]["plane_min_d"], "far": GEOMETRIES[tag]["plane_max_d"]})):
         plain = g.render_frames(**kw, **extra)
         skipped = g.render_frames(**kw, **extra, skip_empty=True)
-        assert all(_same_bits(a, b) for a, b in zip(plain, skipped)), extra
+        assert_bitwise(plain, skipped, extra)
 
 
 @pytest.mark.parametrize("tau", [1e-3, 0.05])
@@ -313,7 +275,7 @@ def test_early_stop_stays_within_its_bound(tag, tau, ring):
     c = envelope_case(tag, 96, 512, CORNERS, head=True)
     kw = dict(rgba=c.rgba, dhw=c.dhw, view2mpi=c.view2mpi, ray_dir=c.ray_dir, eye=c.eye, z_dir=c.z_dir)
     rc, rd = (n(t) for t in g.render_frames(**kw))
-    assert all(_same_bits(a, b) for a, b in zip(g.render_frames(**kw), g.render_frames(**kw, early_stop=0.0)))
+    assert_bitwise(g.render_frames(**kw), g.render_frames(**kw, early_stop=0.0), "tau = 0")
     gc, gd = (n(t) for t in g.render_frames(**kw, early_stop=tau))
     assert np.max(np.abs(gc - rc)) <= 2 * tau + 2 * EXPECT, float(np.max(np.abs(gc - rc)))
     zmax = max_plane_depth(dict(ray_dir=n(c.ray_dir), eye=n(c.eye), z_dir=n(c.z_dir), dhw=n(c.dhw), view2mpi=n(c.view2mpi)))
@@ -337,12 +299,12 @@ def test_in_kernel_rays_and_video_epilogue(tag, ring):
     assert err <= 2.5e-7, err
     cf, df = g.render_frames(rgba=c.rgba, dhw=c.dhw, view2mpi=c.view2mpi, cam=cam, H=H, W=W, check_last_plane=True)
     cp, dp = g.render_views(c.rgba, c.dhw, c.view2mpi, rays, c.eye, c.z_dir, check_last_plane=True, color_minus1_1=True)
-    assert _same_bits(cf, cp) and _same_bits(df, dp)
+    assert_bitwise((cf, df), (cp, dp), "cam rays")
     near, far = geo["plane_min_d"], geo["plane_max_d"]
     u8, d8 = g.render_frames(rgba=c.rgba, dhw=c.dhw, view2mpi=c.view2mpi, ray_dir=c.ray_dir, eye=c.eye, z_dir=c.z_dir,
                              video={"near": near, "far": far})
     c11, d11 = g.render_views(c.rgba, c.dhw, c.view2mpi, c.ray_dir, c.eye, c.z_dir, color_minus1_1=True)
-    ref_img, ref_depth = _video_reference(c11, d11, near, far)
+    ref_img, ref_depth = video_reference(c11, d11, near, far)
     assert np.array_equal(n(u8), ref_img) and np.array_equal(n(d8), ref_depth)
     assert int(ref_depth.max()) > 100 and int(ref_depth.min()) < 100        # depth spans 2.55-2.8, not one clipped code
 

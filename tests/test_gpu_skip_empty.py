@@ -2,51 +2,19 @@
 
 The map must equal a numpy restatement of its definition bit for bit, its fused range flags those of check_range, and every render
 with skipping must be bitwise the same render without it (colour, depth, uint8 frames, flags) on the same kernel and ring depth."""
-import ctypes
-
 import numpy as np
 import pytest
 import torch
 
 import ml_gmpi_b200 as g
-from ml_gmpi_b200 import _lib, synth
-from conftest import MPI_CASES, load_golden
+from ml_gmpi_b200 import synth
+from conftest import MPI_CASES
+from testlib import assert_bitwise, case, dev, early_stop_stats, forced_kernel, kernel_fixture, skip_stats
 
 pytestmark = pytest.mark.gpu
 B = 8
-_VARIANTS = {"direct": (1, 0), "staged2": (2, 2), "staged3": (2, 3)}   # (kernel variant, ring depth)
-
-
-def dev():
-    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
-    return torch.device("cuda:0")
-
-
-def set_variant(name):
-    lib = _lib.load()
-    variant, stages = _VARIANTS.get(name, (0, 0))
-    _lib.check(lib.gmpi_debug_set_fwd_variant(variant))
-    _lib.check(lib.gmpi_debug_set_fwd_stages(stages))
-
-
-@pytest.fixture(params=["direct", "staged2", "staged3"])
-def variant(request):
-    set_variant(request.param)
-    yield request.param
-    set_variant("auto")
-
-
-@pytest.fixture(params=["staged2", "staged3"])
-def staged(request):
-    set_variant(request.param)
-    yield request.param
-    set_variant("auto")
-
-
-def skip_stats():
-    s, t = ctypes.c_ulonglong(0), ctypes.c_ulonglong(0)
-    _lib.check(_lib.load().gmpi_debug_fwd_skip_stats(ctypes.byref(s), ctypes.byref(t)))
-    return s.value, t.value
+variant = kernel_fixture("direct", "staged2", "staged3")
+staged = kernel_fixture("staged2", "staged3")
 
 
 # ------------------------------------------------------------------------------------------------------------------------
@@ -143,20 +111,6 @@ def _frames(c, skip, **kw):
     return [o.cpu().numpy() for o in out if o is not None] + [int(flags.item())]
 
 
-def assert_same(a, b):
-    assert len(a) == len(b)
-    for x, y in zip(a[:-1], b[:-1]):
-        assert x.dtype == y.dtype and x.shape == y.shape
-        assert np.array_equal(x.view(np.uint8), y.view(np.uint8)), np.argwhere(x.view(np.uint8) != y.view(np.uint8))[:5]
-    assert a[-1] == b[-1]
-
-
-def _golden(name):
-    gd = load_golden(name)
-    return dict(rgba=gd["rgba"], view2mpi=gd["view2mpi"], dhw=gd["dhw"], ray_dir=gd["ray_dir"], eye=gd["eye"], z_dir=gd["z_dir"],
-                ac=bool(gd["align_corners"]))
-
-
 def _head(n_planes=32, tex=256, img=256, n_mpi=2, views=1, seed=0, **extra):
     case = synth.make_head_case(n_planes=n_planes, tex=tex, img=img, n_mpi=n_mpi, views_per_mpi=views, seed=seed)
     c = dict(rgba=case.rgba.numpy(), view2mpi=case.view2mpi.numpy(), dhw=case.dhw.numpy(), ray_dir=case.ray_dir.numpy(),
@@ -232,20 +186,20 @@ CASES = {
 @pytest.mark.parametrize("name", sorted(CASES))
 def test_skip_is_bitwise_invisible(staged, name):
     c = CASES[name]()
-    assert_same(_frames(c, True), _frames(c, False))
+    assert_bitwise(_frames(c, True), _frames(c, False), name)
 
 
 @pytest.mark.parametrize("name", ["head", "factored_bg", "fp16", "cam_video", "shuffled_and_degenerate_rays"])
 @pytest.mark.parametrize("tau", [0.0, 0.05])
 def test_skip_with_early_stop_equals_early_stop_alone(staged, name, tau):
     c = CASES[name]()
-    assert_same(_frames(c, True, early_stop=tau), _frames(c, False, early_stop=tau))
+    assert_bitwise(_frames(c, True, early_stop=tau), _frames(c, False, early_stop=tau), (name, tau))
 
 
 @pytest.mark.parametrize("name", MPI_CASES)
 def test_golden_fixtures(variant, name):
-    c = _golden(name)
-    assert_same(_frames(c, True), _frames(c, False))
+    c = case(name)
+    assert_bitwise(_frames(c, True), _frames(c, False), name)
 
 
 def test_nan_colour_under_zero_alpha_stays_nan(staged):
@@ -267,12 +221,6 @@ def test_stats_random_mpi_skips_nothing_and_head_skips_the_front(staged):
     assert skipped >= total * 12 // 32, (skipped, total)
 
 
-def early_stop_stats():
-    s, t = ctypes.c_ulonglong(0), ctypes.c_ulonglong(0)
-    _lib.check(_lib.load().gmpi_debug_fwd_early_stop_stats(ctypes.byref(s), ctypes.byref(t)))
-    return s.value, t.value
-
-
 @pytest.mark.parametrize("name", ["head", "fp16"])
 def test_stats_of_skip_with_early_stop(staged, name):
     """A skipping launch with early stop reports the early-stop stages of the kernel that ran: it walked the stages the skip stats
@@ -285,13 +233,10 @@ def test_stats_of_skip_with_early_stop(staged, name):
 
 
 def test_direct_kernel_skips_nothing():
-    set_variant("direct")
-    try:
+    with forced_kernel("direct"):
         c = _head()
-        assert_same(_frames(c, True), _frames(c, False))
+        assert_bitwise(_frames(c, True), _frames(c, False), "direct")
         assert skip_stats() == (0, 0)
-    finally:
-        set_variant("auto")
 
 
 def test_render_views_reuses_a_map_and_refuses_a_stale_one():

@@ -16,23 +16,12 @@ import ml_gmpi_b200 as g
 from ml_gmpi_b200 import _lib, synth
 from ml_gmpi_b200.camera import cam_params
 from conftest import ROOT
-from test_gpu_early_stop import CASES, case, set_variant
-from test_gpu_half import _limit_case, assert_class_88_behind_plane_25, footprints, headline_case
+from testlib import (CASES, assert_bitwise, assert_class_88_behind_plane_25, case, dev, early_stop_stats, footprints, forced_kernel,
+                     forward_desc, headline_case, kernel_fixture, limit_case, misaligned, native_vs_fp32, render_fwd, skip_stats)
 
 pytestmark = pytest.mark.gpu
 TAUS = [None, 0.0, 2.0 ** -24, 1e-3]
-
-
-def dev():
-    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
-    return torch.device("cuda:0")
-
-
-@pytest.fixture(params=["direct", "staged2", "staged3"])
-def variant(request):
-    set_variant(request.param)
-    yield request.param
-    set_variant("auto")
+variant = kernel_fixture("direct", "staged2", "staged3")
 
 
 def quantize(rgba):
@@ -43,75 +32,15 @@ def converted(u8):
     return u8.astype(np.float32) / 255.0
 
 
-def _misaligned(x):
-    """x's values in a buffer whose base is 8 bytes past a 16-byte boundary."""
-    buf = torch.empty(x.numel() * x.element_size() + 64, dtype=torch.uint8, device=x.device)
-    off = (8 - buf.data_ptr()) % 16
-    y = buf[off:off + x.numel() * x.element_size()].view(x.dtype).view(x.shape)
-    y.copy_(x)
-    assert y.data_ptr() % 16 == 8
-    return y
+def _mpi(u8, native, misalign=False):
+    """The MPI of uint8 codes `u8` on the device: native (GMPI_MPI_U8) or its fp32 conversion."""
+    rgba = torch.from_numpy(np.ascontiguousarray(u8 if native else converted(u8))).to(dev())
+    return dict(rgba=misaligned(rgba, 8) if misalign else rgba)
 
 
-def _desc(c, u8, native, tau=None, cam=None, u8_round=False, view_group=None, misalign=False, gather=None):
-    """Descriptor of a forward of case c's MPI given as uint8 codes `u8`: native (GMPI_MPI_U8) or its fp32 conversion."""
-    d = dev()
-    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(d)
-    rgba = t(u8) if native else t(converted(u8))
-    if misalign:
-        rgba = _misaligned(rgba)
-    V, _, H, W = c["ray_dir"].shape
-    if gather is not None:
-        out = dict(peer_frames=gather[1], n_peers=1, frame_offset=0)
-    elif c.get("video"):
-        out = dict(video_rgb=torch.empty((V, H, W, 3), dtype=torch.uint8, device=d),
-                   video_depth=torch.empty((V, H, W, 1), dtype=torch.uint8, device=d), depth_near=0.9, depth_range=np.float32(0.3).item())
-    else:
-        out = dict(color=torch.empty((V, 3, H, W), device=d), depth=torch.empty((V, 1, H, W), device=d))
-    rays = dict(cam=cam) if cam is not None else dict(ray_dir=t(c["ray_dir"]), eye=t(c["eye"]), z_dir=t(c["z_dir"]))
-    opts = (_lib.OPT_ALIGN_CORNERS if c["ac"] else 0) | _lib.OPT_COLOR_MINUS1_1 | (_lib.OPT_U8_ROUND_HALF_UP if u8_round else 0) \
-        | (_lib.OPT_EARLY_STOP if tau is not None else 0) | (_lib.OPT_MPI_U8 if native else 0)
-    flags = torch.zeros(1, dtype=torch.int32, device=d)
-    keep = dict(view2mpi=t(c["view2mpi"]), dhw=t(c["dhw"]), flags=flags, rgba=rgba, **rays, **out)
-    desc = _lib.make_desc(options=opts, M=u8.shape[0], V=V, N=u8.shape[1], Ht=u8.shape[-2], Wt=u8.shape[-1], H=H, W=W,
-                          view_group=c.get("view_group", 1) if view_group is None else view_group, early_stop=tau, **keep)
-    return desc, keep
-
-
-def run(c, u8, native, **kw):
-    """(outputs..., flags) of one gmpi_mpi_render_fwd_ex call, as numpy."""
-    V, _, H, W = c["ray_dir"].shape
-    gather = None
-    if kw.pop("gather", False):
-        frames = torch.full((V, 4, H, W), float("nan"), device=dev())
-        gather = (frames, torch.tensor([frames.data_ptr()], dtype=torch.int64, device=dev()))
-    desc, keep = _desc(c, u8, native, gather=gather, **kw)
-    _lib.check(_lib.load().gmpi_mpi_render_fwd_ex(ctypes.byref(desc)))
-    torch.cuda.synchronize()
-    if gather is not None:
-        return gather[0].cpu().numpy(), keep["flags"].cpu().numpy()
-    names = ("video_rgb", "video_depth") if "video_rgb" in keep else ("color", "depth")
-    return tuple(keep[n].cpu().numpy() for n in names) + (keep["flags"].cpu().numpy(),)
-
-
-def assert_bitwise(a, b, what):
-    for x, y in zip(a, b):
-        assert x.dtype == y.dtype and np.array_equal(x.view(np.uint8), y.view(np.uint8)), \
-            (what, float(np.nanmax(np.abs(x.astype(np.float64) - y))))
-
-
-def run_pair(c, u8, variant, **kw):
+def run_pair(c, u8, variant, misalign=False, **kw):
     """uint8 render and the fp32 render of its conversion, on the kernel the uint8 call gets under `variant`."""
-    h = run(c, u8, True, **kw)
-    desc, _ = _desc(c, u8, True, **{k: v for k, v in kw.items() if k != "gather"})
-    fell_back = variant != "direct" and _lib.fwd_plan(desc)[0] == _lib.PLAN_DIRECT
-    if fell_back:
-        set_variant("direct")
-    try:
-        f = run(c, u8, False, **kw)
-    finally:
-        set_variant(variant)
-    return h, f, fell_back
+    return native_vs_fp32(c, _mpi(u8, True, misalign), _mpi(u8, False, misalign), variant, **kw)
 
 
 def test_device_conversion_is_exact_for_every_code():
@@ -190,7 +119,7 @@ def test_host_entry_point_takes_u8_host_buffers(name):
         _lib.check(lib.gmpi_mpi_render_host_ex(ctypes.byref(d), 0))
         outs.append(tuple(o.values()) + (flags.view(np.int32),))
     assert_bitwise(outs[0], outs[1], name)
-    assert_bitwise(outs[0], run(c, u8, True, view_group=1), (name, "device entry point"))
+    assert_bitwise(outs[0], render_fwd(c, _mpi(u8, True), view_group=1), (name, "device entry point"))
 
 
 def _shift_footprints(c, lo, hi):
@@ -208,31 +137,27 @@ def test_u8_at_the_widest_box_class_at_every_shift(stages, shape):
     """Footprints at the widest class (width need 81..88, class 88) whose fp32 box starts 0, 4, 8 and 12 texels past a multiple of 16:
     the uint8 kernel stages a 112-wide box from that multiple and decides fast / generic body exactly as fp32 does.  "headline": 96 x
     1024^2 with equal-weight alpha, where those footprints lie on planes that reach the render."""
-    c = _limit_case(False) if shape == "limit" else headline_case()
+    c = limit_case(False) if shape == "limit" else headline_case()
     counts = _shift_footprints(c, 81, 88)
     assert all(n > 0 for n in counts.values()), counts
     if shape == "headline":
         assert_class_88_behind_plane_25(c)
     u8 = quantize(c["rgba"])
-    set_variant(stages)
-    try:
+    with forced_kernel(stages):
         for tau in (None, 1e-3):
             h, f, fell_back = run_pair(c, u8, stages, tau=tau)
             assert not fell_back
             assert_bitwise(h, f, (stages, tau))
-    finally:
-        set_variant("auto")
 
 
 def test_narrow_and_misaligned_u8_take_the_direct_kernel():
     """Wt % 16 != 0 (with Wt % 4 == 0) or a base 8 bytes off a 16-byte boundary: the plan query says why, the C call runs the direct
     kernel natively, bitwise the direct kernel on the conversion; render_views takes the fp32 conversion instead, bitwise the render
     of unorm8_to_float(rgba)."""
-    set_variant("staged3")
-    try:
+    with forced_kernel("staged3"):
         c = case("small")
         u8 = quantize(c["rgba"])
-        desc, _ = _desc(c, u8, True, misalign=True)
+        desc, _ = forward_desc(c, _mpi(u8, True, misalign=True))
         assert _lib.fwd_plan(desc) == (_lib.PLAN_DIRECT, 8)
         for tau in (None, 1e-3):
             h, f, fell_back = run_pair(c, u8, "staged3", misalign=True, tau=tau)
@@ -240,15 +165,13 @@ def test_narrow_and_misaligned_u8_take_the_direct_kernel():
             assert_bitwise(h, f, ("misaligned", tau))
         n = case("partial_acfalse_nonsquare")        # texture 72 x 116: 116 % 16 == 4
         un = quantize(n["rgba"])
-        desc, _ = _desc(n, un, True)
+        desc, _ = forward_desc(n, _mpi(un, True))
         assert _lib.fwd_plan(desc) == (_lib.PLAN_DIRECT, 1)
-        desc32, _ = _desc(n, un, False)
+        desc32, _ = forward_desc(n, _mpi(un, False))
         assert _lib.fwd_plan(desc32) == (_lib.PLAN_STAGED, 0)
         h, f, fell_back = run_pair(n, un, "staged3")
         assert fell_back
         assert_bitwise(h, f, "Wt % 16")
-    finally:
-        set_variant("auto")
     # render_views: the fallback renders the conversion on the fp32 plan (staged here), and equals render_views of the conversion
     cs = synth.make_case(n_planes=8, tex=8, img=256, n_mpi=2, views_per_mpi=2, seed=4, last_alpha_one=True).to(dev())
     x = torch.randint(0, 256, (2, 8, 4, 64, 120), dtype=torch.uint8, generator=torch.Generator().manual_seed(9)).to(dev())
@@ -256,7 +179,7 @@ def test_narrow_and_misaligned_u8_take_the_direct_kernel():
     with torch.no_grad():
         a = g.render_views(x, *args, unorm8=True)
         b = g.render_views(g.unorm8_to_float(x), *args)
-    assert_bitwise([t.cpu().numpy() for t in a], [t.cpu().numpy() for t in b], "render_views fallback")
+    assert_bitwise(a, b, "render_views fallback")
 
 
 @functools.lru_cache(maxsize=None)
@@ -279,33 +202,21 @@ def test_render_views_and_frames_take_u8_natively_without_an_fp32_copy():
         peak = torch.cuda.max_memory_allocated() - base
     outputs = sum(t.numel() * t.element_size() for t in out)
     assert peak <= outputs + (1 << 20), (peak, outputs, x.numel() * 4)       # no fp32 copy of the MPI (8 MB here)
-    assert_bitwise([t.cpu().numpy() for t in out], [t.cpu().numpy() for t in ref], "render_views")
+    assert_bitwise(out, ref, "render_views")
     kw = dict(dhw=c.dhw, view2mpi=c.view2mpi, ray_dir=c.ray_dir, eye=c.eye, z_dir=c.z_dir)
     for extra in (dict(early_stop=1e-3), dict(video={"near": 0.9, "far": 1.2}), dict(video={"near": 0.9, "far": 1.2}, u8_round=True)):
         v = g.render_frames(rgba=x, unorm8=True, **kw, **extra)
         w = g.render_frames(rgba=f32, **kw, **extra)
-        assert_bitwise([t.cpu().numpy() for t in v], [t.cpu().numpy() for t in w], ("render_frames", extra))
+        assert_bitwise(v, w, ("render_frames", extra))
     # unorm8 left at False: a uint8 tensor is upcast without scaling, as before
     with torch.no_grad():
         a = g.render_views(x, *args)
         b = g.render_views(x.float(), *args)
-    assert_bitwise([t.cpu().numpy() for t in a], [t.cpu().numpy() for t in b], "unorm8=False")
+    assert_bitwise(a, b, "unorm8=False")
     with pytest.raises(TypeError, match="uint8"):
         g.render_views(f32, *args, unorm8=True)
     with pytest.raises(TypeError, match="uint8"):
         g.render_frames(rgba=x.half(), unorm8=True, **kw)
-
-
-def _skip_stats():
-    s, t = ctypes.c_ulonglong(), ctypes.c_ulonglong()
-    _lib.check(_lib.load().gmpi_debug_fwd_skip_stats(ctypes.byref(s), ctypes.byref(t)))
-    return s.value, t.value
-
-
-def _es_stats():
-    s, t = ctypes.c_ulonglong(), ctypes.c_ulonglong()
-    _lib.check(_lib.load().gmpi_debug_fwd_early_stop_stats(ctypes.byref(s), ctypes.byref(t)))
-    return s.value, t.value
 
 
 @pytest.mark.parametrize("stages", ["staged2", "staged3"])
@@ -321,24 +232,21 @@ def test_skip_empty_on_u8_is_bitwise(stages):
     torch.cuda.synchronize()
     assert o8.nbytes == o32.nbytes and torch.equal(o8.occ, o32.occ)
     kw = dict(dhw=h.dhw, view2mpi=h.view2mpi, ray_dir=h.ray_dir, eye=h.eye, z_dir=h.z_dir, view_group=V)
-    set_variant(stages)
-    try:
+    with forced_kernel(stages):
         for extra in ({}, dict(video={"near": 0.9, "far": 1.2}), dict(early_stop=1e-3)):
             a = g.render_frames(rgba=x, unorm8=True, skip_empty=o8, **kw, **extra)
-            skipped, total = _skip_stats()
+            skipped, total = skip_stats()
             assert 0 < skipped < total, (skipped, total)
             if "early_stop" in extra:
-                es, es_total = _es_stats()
+                es, es_total = early_stop_stats()
                 assert es_total == total and 0 < es < es_total
             b = g.render_frames(rgba=f32, skip_empty=o32, **kw, **extra)
-            assert (skipped, total) == _skip_stats()
+            assert (skipped, total) == skip_stats()
             c = g.render_frames(rgba=f32, **kw, **extra)
-            assert_bitwise([t.cpu().numpy() for t in a], [t.cpu().numpy() for t in b], (stages, extra, "skip"))
-            assert_bitwise([t.cpu().numpy() for t in a], [t.cpu().numpy() for t in c], (stages, extra, "no skip"))
+            assert_bitwise(a, b, (stages, extra, "skip"))
+            assert_bitwise(a, c, (stages, extra, "no skip"))
         a, c = g.render_frames(rgba=x, unorm8=True, skip_empty=True, **kw), g.render_frames(rgba=f32, **kw)
-        assert_bitwise([t.cpu().numpy() for t in a], [t.cpu().numpy() for t in c], (stages, "skip_empty=True"))
-    finally:
-        set_variant("auto")
+        assert_bitwise(a, c, (stages, "skip_empty=True"))
 
 
 def test_u8_planes_against_the_reference():
@@ -348,14 +256,10 @@ def test_u8_planes_against_the_reference():
     t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev())
     args = (t(gd["dhw"]), t(gd["view2mpi"]), t(gd["ray_dir"]), t(gd["eye"]), t(gd["z_dir"]))
     for v in ("direct", "staged2", "staged3"):
-        set_variant(v)
-        try:
-            with torch.no_grad():
-                color, depth = g.render_views(t(gd["rgba_u8"]), *args, align_corners=bool(gd["align_corners"]), unorm8=True)
-                c32, d32 = g.render_views(t(gd["rgba"]), *args, align_corners=bool(gd["align_corners"]))
-        finally:
-            set_variant("auto")
-        assert_bitwise([color.cpu().numpy(), depth.cpu().numpy()], [c32.cpu().numpy(), d32.cpu().numpy()], v)
+        with forced_kernel(v), torch.no_grad():
+            color, depth = g.render_views(t(gd["rgba_u8"]), *args, align_corners=bool(gd["align_corners"]), unorm8=True)
+            c32, d32 = g.render_views(t(gd["rgba"]), *args, align_corners=bool(gd["align_corners"]))
+        assert_bitwise((color, depth), (c32, d32), v)
         for got, ref in ((color, gd["color"]), (depth, gd["depth"])):
             err = float(np.max(np.abs(got.cpu().numpy() - ref)) / max(float(np.max(np.abs(ref))), 1e-30))
             assert err <= 2e-5, (v, err)

@@ -11,15 +11,9 @@ import ml_gmpi_b200 as g
 from ml_gmpi_b200 import _lib
 from ml_gmpi_b200.mpi import _half_mpi
 from conftest import ROOT
-from test_library_build import KEY_F16, library_kernels, render_kernels
+from testlib import KEY_F16, lib, library_kernels, render_kernels
 
 UNSUPPORTED = 3
-
-
-@pytest.fixture(scope="module")
-def lib():
-    g.build_library()
-    return _lib.load()
 
 
 def test_option_bit_matches_the_header():

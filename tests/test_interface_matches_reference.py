@@ -1,16 +1,9 @@
 """Drop-in boundary: the host-side mirrors must accept exactly what the reference's callers pass (SURVEY.md 8b).
 The reference's signatures are recorded in tests/golden/reference_signatures.json (oracle/make_golden_signatures.py)."""
 import inspect
-import json
-import os
 
-from conftest import GOLDEN
 from make_golden_signatures import params as _params
-
-
-def reference_signatures():
-    with open(os.path.join(GOLDEN, "reference_signatures.json")) as f:
-        return json.load(f)
+from testlib import reference_signatures
 
 
 def test_mpi_signatures():

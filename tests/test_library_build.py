@@ -1,17 +1,14 @@
 """CPU checks of the built library: one artifact holds every kernel, the skipping (mpi_skip.cu) and uint8 (mpi_u8.cu) ones included,
-and every kernel keeps the machine code recorded in tests/golden/sass_digests.json.  library_kernels() reads a built library's kernels
-for the machine-code tests of the other modules too.
+and every kernel keeps the machine code recorded in tests/golden/sass_digests.json (testlib.library_kernels reads the machine code).
 
     python tests/test_library_build.py --record-sass   # rewrites tests/golden/sass_digests.json
 """
-import hashlib
 import json
 import os
 import re
 import shutil
 import subprocess
 import sys
-from typing import NamedTuple, Optional
 
 import pytest
 
@@ -20,6 +17,7 @@ if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
 
 import ml_gmpi_b200 as g  # noqa: E402
+from testlib import KEY_U8, library_kernels, render_kernels  # noqa: E402
 
 SASS_DIGESTS = os.path.join(ROOT, "tests", "golden", "sass_digests.json")
 
@@ -28,51 +26,6 @@ def _nvcc_release():
     out = subprocess.run([g._build.nvcc_path(), "--version"], capture_output=True, text=True).stdout
     m = re.search(r"release [0-9.]+, V[0-9.]+", out)
     return m.group(0) if m else out.strip()
-
-
-# The render-kernel key bits (kKey*, csrc/mpi_kernel_keys.cuh)
-KEY_AC, KEY_FAC, KEY_EMIT, KEY_ES, KEY_F16, KEY_STAGED, KEY_BWD, KEY_DET, KEY_SKIP, KEY_U8 = 1, 2, 4, 8, 16, 32, 64, 128, 256, 512
-
-
-class Kernel(NamedTuple):
-    template: str           # the C++ name: a kernel template, or a plain or extern "C" kernel
-    key: Optional[int]      # the render kernel's key (template<uint32_t K>), None for other kernels
-    sass: str
-    regs: int
-    stack: int
-    local: int
-
-    def digest(self):
-        """sha256 of the SASS instructions (addresses and encodings included, no names or comments)"""
-        lines = [l.strip() for l in self.sass.split("\n") if re.match(r"\s+/\*[0-9a-f]{4,}\*/", l)]
-        return hashlib.sha256("\n".join(lines).encode()).hexdigest()
-
-
-def library_kernels(path=None):
-    """{mangled name: Kernel} of a built library (cuobjdump -sass and -res-usage).  Kernels of namespace gmpi are
-    _ZN4gmpi<length><name>..., and a uint32_t template argument K mangles as ILj<K>E."""
-    path = path or g._build.LIB_PATH
-    run = lambda flag: subprocess.run(["cuobjdump", flag, path], capture_output=True, text=True, check=True).stdout
-    usage = {m[1]: (int(m[2]), int(m[3]), int(m[4]))
-             for m in re.finditer(r"Function (\S+):\s*\n\s*REG:(\d+) STACK:(\d+) SHARED:\d+ LOCAL:(\d+)", run("-res-usage"))}
-    out = {}
-    for f in re.split(r"\n\s*Function : ", run("-sass"))[1:]:
-        name, body = f.split("\n", 1)
-        name = name.strip()
-        template, key = name, None
-        m = re.match(r"_ZN4gmpi(\d+)", name)
-        if m:
-            end = m.end() + int(m[1])
-            template = name[m.end():end]
-            k = re.match(r"ILj(\d+)EE", name[end:])
-            key = int(k[1]) if k else None
-        out[name] = Kernel(template, key, body, *usage[name])
-    return out
-
-
-def render_kernels(kernels, template, has=0, lacks=0):
-    """{name: Kernel} of the instantiations of `template` whose key has every bit of `has` and none of `lacks`"""
-    return {n: k for n, k in kernels.items() if k.template == template and k.key & has == has and not k.key & lacks}
 
 
 def test_sass_of_every_kernel_is_recorded_by_template_and_key():

@@ -11,30 +11,11 @@ import torch
 import mpi_oracle
 import torch_port
 from conftest import MPI_CASES, load_golden, rel_err
+from testlib import FLAG_CASES, FORWARD_FLAGS
 
 TOL = 2e-6
-
-# The flag word each verdict of the reference implies (oracle/make_golden_flags.py): the forward's with the last-plane check, and
-# the range check's.  The forward never sets the range bits; without the last-plane check it never sets LAST_PLANE_OOB.
-FORWARD_FLAGS = {"ok": 0, "alpha": 0, "behind-eye": mpi_oracle.FLAG_PLANE_BEHIND_EYE, "out-of-plane": mpi_oracle.FLAG_LAST_PLANE_OOB}
+# The range check's flag word for each verdict of the reference (the forward's: testlib.FORWARD_FLAGS).
 RANGE_FLAGS = {"ok": 0, "alpha": mpi_oracle.FLAG_ALPHA_RANGE | mpi_oracle.FLAG_RGBA_RANGE, "behind-eye": 0, "out-of-plane": 0}
-
-
-def load_flag_cases():
-    """[(name, verdict, case)] of tests/golden/flags_edges.npz; a case has rgba, dhw, view2mpi, ray_dir, eye, z_dir, align_corners."""
-    z = load_golden("flags_edges")
-    out = []
-    for name, verdict in zip(z["names"].tolist(), z["verdicts"].tolist()):
-        c = {k: z["pool_%d" % int(z[f"{name}__{k}"])] for k in ("dhw", "view2mpi", "ray_dir", "eye", "z_dir", "align_corners")}
-        r = z[f"{name}__rgba"]
-        c["rgba"] = np.random.default_rng(int(r[0])).random(tuple(z[f"{name}__rgba_shape"].tolist()), dtype=np.float32)
-        if len(r) > 1:
-            c["rgba"][tuple(int(i) for i in r[1:])] = z[f"{name}__rgba_value"]
-        out.append((name, verdict, c))
-    return out
-
-
-FLAG_CASES = load_flag_cases()
 _fz = load_golden("flags_edges")
 FIXTURE_VERDICTS = dict(zip(_fz["fixtures"].tolist(), _fz["fixture_verdicts"].tolist()))
 

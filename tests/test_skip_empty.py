@@ -14,16 +14,10 @@ if ROOT not in sys.path:
 
 import ml_gmpi_b200 as g  # noqa: E402
 from ml_gmpi_b200 import _lib  # noqa: E402
-from test_library_build import KEY_U8, library_kernels, render_kernels  # noqa: E402
+from testlib import KEY_U8, lib, library_kernels, render_kernels  # noqa: E402
 
 ERR_INVALID, ERR_UNSUPPORTED = 1, 3
 B = 8
-
-
-@pytest.fixture(scope="module")
-def lib():
-    g.build_library()
-    return _lib.load()
 
 
 def _buf():

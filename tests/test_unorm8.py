@@ -13,16 +13,10 @@ import ml_gmpi_b200 as g
 from ml_gmpi_b200 import _lib
 from ml_gmpi_b200.mpi import _check_unorm8, _unorm8_mpi
 from conftest import ROOT
-from test_library_build import KEY_AC, KEY_U8, library_kernels, render_kernels
+from testlib import KEY_AC, KEY_U8, lib, library_kernels, render_kernels
 
 INVALID, UNSUPPORTED = 1, 3
 U8 = 128
-
-
-@pytest.fixture(scope="module")
-def lib():
-    g.build_library()
-    return _lib.load()
 
 
 def exact_codes():

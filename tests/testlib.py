@@ -1,0 +1,420 @@
+"""Helpers the test modules share.  pytest does not collect this module; the tests import it as they import conftest.
+
+  dev, lib                        the device of the GPU tests; the built library (module fixture of the CPU tests)
+  KERNELS, set_kernel,            the forward-kernel switch: set both of its halves, force a kernel for a with block, or declare a
+  forced_kernel, kernel_fixture   fixture that runs a test once per kernel
+  misaligned, assert_bitwise      a copy at a given offset from a 16-byte boundary; dtype, shape and bytes equal
+  early_stop_stats, skip_stats    the stage counters of the last staged forward
+  case, CASES                     the forward tests' catalogue: the golden fixtures and the synthetic cases
+  forward_desc, render_fwd,       one gmpi_mpi_render_fwd_ex of a catalogue case, and the render of a native (fp16 / uint8) MPI
+  native_vs_fp32                  beside the fp32 MPI it stands for, on the same kernel
+and the helpers several modules read: the machine code of the built library, the staged forward's footprints and its limit cases,
+oracle-side bounds and references, and the flag cases of tests/golden/flags_edges.npz."""
+import contextlib
+import ctypes
+import dataclasses
+import functools
+import hashlib
+import json
+import os
+import re
+import subprocess
+from typing import NamedTuple, Optional
+
+import numpy as np
+import pytest
+import torch
+
+from conftest import GOLDEN, MPI_CASES, load_golden     # first: it puts the repository and oracle/ on sys.path
+import mpi_oracle  # noqa: E402
+import ml_gmpi_b200 as g  # noqa: E402
+from ml_gmpi_b200 import _lib, synth  # noqa: E402
+
+
+def dev():
+    assert torch.cuda.is_available(), "GPU tests need a CUDA device"
+    return torch.device("cuda:0")
+
+
+@pytest.fixture(scope="module")
+def lib():
+    g.build_library()
+    return _lib.load()
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# the kernel switch (process-wide: every render after set_kernel takes the forced kernel)
+# ------------------------------------------------------------------------------------------------------------------------------
+# name: (gmpi_debug_set_fwd_variant, gmpi_debug_set_fwd_stages) -- the kernel (automatic, direct, TMA-staged) and the staged
+# forward's ring depth (0: the depth it picks itself; the factored forward's ring is always 3 deep)
+KERNELS = {"auto": (0, 0), "direct": (1, 0), "staged": (2, 0), "staged2": (2, 2), "staged3": (2, 3)}
+
+
+def set_kernel(name):
+    """Forces the kernel and the ring depth of `name`, both."""
+    variant, stages = KERNELS[name]
+    lib = _lib.load()
+    _lib.check(lib.gmpi_debug_set_fwd_variant(variant))
+    _lib.check(lib.gmpi_debug_set_fwd_stages(stages))
+
+
+@contextlib.contextmanager
+def forced_kernel(name):
+    """The kernel `name` inside the with block, the automatic choice after it, also when the block raises."""
+    set_kernel(name)
+    try:
+        yield name
+    finally:
+        set_kernel("auto")
+
+
+def kernel_fixture(*names):
+    """A fixture that runs each test once per kernel name, forced as by forced_kernel; its value is the name.  The module attribute
+    it is assigned to names it: `variant = kernel_fixture("direct", "staged2", "staged3")`."""
+    @pytest.fixture(params=list(names))
+    def fixture(request):
+        with forced_kernel(request.param):
+            yield request.param
+    return fixture
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# buffers, bits, counters
+# ------------------------------------------------------------------------------------------------------------------------------
+def misaligned(x, offset):
+    """x's values in a buffer whose base is `offset` bytes (a multiple of x's element size) past a 16-byte boundary."""
+    size = x.element_size()
+    buf = torch.empty(x.numel() + 16 // size, dtype=x.dtype, device=x.device)
+    start = (offset - buf.data_ptr()) % 16 // size
+    y = buf[start:start + x.numel()].view(x.shape)
+    y.copy_(x)
+    assert y.data_ptr() % 16 == offset, (y.data_ptr() % 16, offset)
+    return y
+
+
+def assert_bitwise(a, b, what=None):
+    """a and b have the same dtype, shape and bytes.  Each is a numpy array, a torch tensor or a number, or a list or tuple of them
+    (then both have the same length and are compared element by element).  `what` names the case in the message."""
+    if isinstance(a, (list, tuple)):
+        assert isinstance(b, (list, tuple)) and len(a) == len(b), (what, "lengths differ")
+        for i, (x, y) in enumerate(zip(a, b)):
+            assert_bitwise(x, y, (what, i))
+        return
+    x, y = (t.detach().cpu().numpy() if isinstance(t, torch.Tensor) else np.asarray(t) for t in (a, b))
+    assert x.dtype == y.dtype and x.shape == y.shape, (what, x.dtype, x.shape, y.dtype, y.shape)
+    if x.tobytes() != y.tobytes():
+        with np.errstate(invalid="ignore"):
+            diff = np.abs(x.astype(np.float64) - y.astype(np.float64))
+        raise AssertionError((what, "max |a - b|", float(np.nanmax(diff, initial=0.0))))
+
+
+def _stage_counts(fn):
+    s, t = ctypes.c_ulonglong(0), ctypes.c_ulonglong(0)
+    _lib.check(fn(ctypes.byref(s), ctypes.byref(t)))
+    return s.value, t.value
+
+
+def early_stop_stats():
+    """(stages stopped early, stages counted) of the last forward (gmpi_debug_fwd_early_stop_stats)."""
+    return _stage_counts(_lib.load().gmpi_debug_fwd_early_stop_stats)
+
+
+def skip_stats():
+    """(stages skipped as empty, stages counted) of the last forward (gmpi_debug_fwd_skip_stats)."""
+    return _stage_counts(_lib.load().gmpi_debug_fwd_skip_stats)
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# the case catalogue of the forward tests: numpy inputs of a render, the factors of a factored case, video and view-group settings
+# ------------------------------------------------------------------------------------------------------------------------------
+def golden_case(name):
+    gd = load_golden(name)
+    return dict(rgba=gd["rgba"], view2mpi=gd["view2mpi"], dhw=gd["dhw"], ray_dir=gd["ray_dir"], eye=gd["eye"], z_dir=gd["z_dir"],
+                ac=bool(gd["align_corners"]))
+
+
+def synth_case(n_planes, tex, img, n_mpi, views=1, seed=0, alpha_scale=None, crop=None, tex_hw=None, ac=True, view_group=1,
+               factored=False, video=False):
+    case = synth.make_case(n_planes=n_planes, tex=tex, img=img, n_mpi=n_mpi, views_per_mpi=views, seed=seed, last_alpha_one=True)
+    rgba = case.rgba
+    if tex_hw is not None:
+        rgba = torch.rand((n_mpi, n_planes, 4) + tex_hw, generator=torch.Generator().manual_seed(seed))
+        rgba[:, -1, 3] = 1.0
+    if alpha_scale is not None:
+        rgba = rgba.clone()
+        rgba[:, :-1, 3] *= alpha_scale
+    ray = case.ray_dir if crop is None else case.ray_dir[:, :, crop[0]:crop[1]].contiguous()
+    c = dict(rgba=rgba.numpy(), view2mpi=case.view2mpi.numpy(), dhw=case.dhw.numpy(), ray_dir=ray.numpy(), eye=case.eye.numpy(),
+             z_dir=case.z_dir.numpy(), ac=ac, view_group=view_group, video=video)
+    if factored:      # one shared colour image, the last plane's own colour, per-plane alpha
+        gen = torch.Generator().manual_seed(seed + 1)
+        rgb, bg = torch.rand((n_mpi, 3) + rgba.shape[-2:], generator=gen), torch.rand((n_mpi, 3) + rgba.shape[-2:], generator=gen)
+        alpha = torch.from_numpy(c["rgba"][:, :, 3:4].copy())
+        c.update(factored=(rgb.numpy(), alpha.numpy(), bg.numpy()), rgba=g.expand_factored(rgb, alpha, bg).numpy())
+    return c
+
+
+SYNTH = {
+    "small": lambda: synth_case(16, 64, 96, 2, views=2, seed=1),
+    "view_group3": lambda: synth_case(24, 96, 128, 1, views=3, seed=2, view_group=3),
+    "factored": lambda: synth_case(24, 96, 128, 2, views=2, seed=3, factored=True),
+    "factored_view_group2": lambda: synth_case(12, 64, 96, 1, views=2, seed=4, factored=True, view_group=2),
+    "uint8": lambda: synth_case(16, 64, 96, 2, views=2, seed=5, video=True),
+    "N1": lambda: synth_case(1, 128, 160, 2, seed=6),
+    "N2": lambda: synth_case(2, 128, 160, 2, seed=7),
+    "N512": lambda: synth_case(512, 96, 128, 2, seed=8, alpha_scale=0.02),
+    "partial_acfalse_nonsquare": lambda: synth_case(10, 8, 136, 2, views=2, seed=9, crop=(18, 118), tex_hw=(72, 116), ac=False),
+}
+
+
+@functools.lru_cache(maxsize=None)
+def case(name):
+    return SYNTH[name]() if name in SYNTH else golden_case(name)
+
+
+CASES = MPI_CASES + ["c1_full_256"] + list(SYNTH)
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# one forward through the descriptor, and the native-versus-fp32 harness of the fp16 and uint8 tests
+# ------------------------------------------------------------------------------------------------------------------------------
+_ELEMENT_OPTION = {torch.float32: 0, torch.float16: _lib.OPT_MPI_F16, torch.uint8: _lib.OPT_MPI_U8}
+
+
+def forward_desc(c, mpi, tau=None, cam=None, u8_round=False, view_group=None, gather=False):
+    """The descriptor of a forward of catalogue case c on the device MPI `mpi` ({"rgba": ...} or {"rgb", "alpha", "bg_rgb"}; its
+    dtype sets the element option): the case's rays or the camera `cam`; colour and depth in [-1, 1], the uint8 video frames of a
+    video case, or with `gather` the frames of a fused gather into one local buffer ("frames"); early stop at tau; the case's view
+    group unless one is given.  Returns (descriptor, the tensors behind its pointers)."""
+    d = dev()
+    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(d)
+    ref = mpi["alpha"] if "alpha" in mpi else mpi["rgba"]
+    V, _, H, W = c["ray_dir"].shape
+    if gather:
+        frames = torch.full((V, 4, H, W), float("nan"), device=d)
+        out = dict(peer_frames=torch.tensor([frames.data_ptr()], dtype=torch.int64, device=d), n_peers=1, frame_offset=0)
+    elif c.get("video"):
+        out = dict(video_rgb=torch.empty((V, H, W, 3), dtype=torch.uint8, device=d),
+                   video_depth=torch.empty((V, H, W, 1), dtype=torch.uint8, device=d), depth_near=0.9, depth_range=np.float32(0.3).item())
+    else:
+        out = dict(color=torch.empty((V, 3, H, W), device=d), depth=torch.empty((V, 1, H, W), device=d))
+    rays = dict(cam=cam) if cam is not None else dict(ray_dir=t(c["ray_dir"]), eye=t(c["eye"]), z_dir=t(c["z_dir"]))
+    opts = (_lib.OPT_ALIGN_CORNERS if c["ac"] else 0) | _lib.OPT_COLOR_MINUS1_1 | (_lib.OPT_U8_ROUND_HALF_UP if u8_round else 0) \
+        | (_lib.OPT_EARLY_STOP if tau is not None else 0) | _ELEMENT_OPTION[ref.dtype]
+    keep = dict(view2mpi=t(c["view2mpi"]), dhw=t(c["dhw"]), flags=torch.zeros(1, dtype=torch.int32, device=d), **rays, **out, **mpi)
+    desc = _lib.make_desc(options=opts, M=ref.shape[0], V=V, N=ref.shape[1], Ht=ref.shape[-2], Wt=ref.shape[-1], H=H, W=W,
+                          view_group=c.get("view_group", 1) if view_group is None else view_group, early_stop=tau, **keep)
+    return desc, dict(keep, frames=frames) if gather else keep
+
+
+def render_fwd(c, mpi, **kw):
+    """(outputs..., flags) of one gmpi_mpi_render_fwd_ex of forward_desc(c, mpi, **kw), as numpy."""
+    desc, keep = forward_desc(c, mpi, **kw)
+    _lib.check(_lib.load().gmpi_mpi_render_fwd_ex(ctypes.byref(desc)))
+    torch.cuda.synchronize()
+    names = ("frames",) if "frames" in keep else ("video_rgb", "video_depth") if "video_rgb" in keep else ("color", "depth")
+    return tuple(keep[n].cpu().numpy() for n in names + ("flags",))
+
+
+def native_vs_fp32(c, native, fp32, variant, **kw):
+    """render_fwd of the native MPI `native` (fp16 or uint8) and of the fp32 MPI `fp32` it stands for, both on the kernel the native
+    call gets under the forced kernel `variant`: where the plan query sends the native MPI to the direct kernel, the fp32 MPI renders
+    there too.  Returns (native outputs, fp32 outputs, whether the native call fell back to the direct kernel)."""
+    h = render_fwd(c, native, **kw)
+    desc, _ = forward_desc(c, native, **{k: v for k, v in kw.items() if k != "gather"})
+    fell_back = variant != "direct" and _lib.fwd_plan(desc)[0] == _lib.PLAN_DIRECT
+    if fell_back:
+        set_kernel("direct")
+    try:
+        f = render_fwd(c, fp32, **kw)
+    finally:
+        set_kernel(variant)
+    return h, f, fell_back
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# the staged forward's footprints and the cases at its widest box classes
+# ------------------------------------------------------------------------------------------------------------------------------
+def footprints(c):
+    """mpi_oracle.footprints of case c's staged forward (the producer's box of every (view, tile, plane) stage)."""
+    M, N, _, Ht, Wt = c["rgba"].shape
+    return mpi_oracle.footprints(c["view2mpi"], c["dhw"], c["ray_dir"], c["eye"], Ht, Wt, c["ac"])
+
+
+def limit_footprints(c, lo, hi):
+    """(tile, plane) stages whose fp32 box lies under the tile with rows that fit a stage (mode 0, or mode 2 only for a width need
+    above kMaxBW = 88) with a width need in [lo, hi] and an origin 4 texels past a multiple of 8."""
+    f = footprints(c)
+    fits = (f["mode"] != 1) & (-(-f["need_h"] // 4) * 4 <= mpi_oracle.FWD_TILE[1])
+    return int((fits & (f["need_w"] >= lo) & (f["need_w"] <= hi) & (f["bx0"] % 8 == 4)).sum())
+
+
+@functools.lru_cache(maxsize=None)
+def limit_case(factored):
+    """A 512 x 1024 texture seen at 720^2 from three random poses: 1.4 texels per pixel across a tile (64 pixels), 0.7 down it.
+    Many (tile, plane) footprints need the widest box classes, at origins where the fp16 box starts 4 texels further west."""
+    return synth_case(16, 8, 720, 1, views=3, seed=21, tex_hw=(512, 1024), factored=factored)
+
+
+@functools.lru_cache(maxsize=None)
+def headline_case():
+    """One view of the headline MPI, 96 x 1024^2, with equal-weight alpha (synth.equal_weight_alpha): every plane, the back ones
+    with the widest boxes included, reaches the render, so a back-plane tap the native kernel staged or converted wrongly changes
+    the bits of the output (with U(0, 1) alpha it would be absorbed by the rounding of the accumulator)."""
+    cs = synth.make_case(n_planes=96, tex=1024, img=1024, n_mpi=1, seed=1234, alpha="equal_weight")
+    return dict(rgba=cs.rgba.numpy(), view2mpi=cs.view2mpi.numpy(), dhw=cs.dhw.numpy(), ray_dir=cs.ray_dir.numpy(),
+                eye=cs.eye.numpy(), z_dir=cs.z_dir.numpy(), ac=True)
+
+
+def assert_class_88_behind_plane_25(c):
+    cls = footprints(c)["cls"]
+    assert (cls[..., 25:] == 88).any() and all((cls == k).any() for k in range(56, 96, 8))
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# references and bounds
+# ------------------------------------------------------------------------------------------------------------------------------
+def max_plane_depth(gd):
+    """[V,1,H,W]: the largest |z-depth| of a pixel over the planes, (d - e_z) / r_z * (r . z_dir) (mpi.py:74-76,149-151)."""
+    ray, eye, z = gd["ray_dir"].astype(np.float64), gd["eye"].astype(np.float64), gd["z_dir"].astype(np.float64)
+    d = gd["dhw"][gd["view2mpi"], :, 0].astype(np.float64)                      # [V,N]
+    zlen = np.einsum("vchw,vc->vhw", ray, z)
+    t = (d[:, :, None, None] - eye[:, 2, None, None, None]) / ray[:, None, 2]    # [V,N,H,W]
+    return np.max(np.abs(t * zlen[:, None]), axis=1, keepdims=True)
+
+
+def video_reference(color_m11, depth, near, far):
+    """gmpi/eval/vis/render_video.py:118-126, verbatim arithmetic on numpy float32 arrays."""
+    img = color_m11.permute(0, 2, 3, 1).cpu().numpy()
+    img = (img + 1) / 2.0
+    img = (img * 255).astype(np.uint8)
+    depth_map = depth.permute(0, 2, 3, 1).cpu().numpy()
+    depth_map = (depth_map - near) / (far - near)
+    depth_map = np.clip(depth_map, 0, 1)
+    depth_map = (depth_map * 255).astype(np.uint8)
+    return img, depth_map
+
+
+ALPHAS = ["uniform", "equal_weight"]
+
+
+def each_alpha(argnames, sets, indirect=()):
+    """parametrize(argnames + ",alpha") over sets x ALPHAS.  The U(0, 1) sets keep the ids they had before the equal-weight input
+    was added; the equal-weight ones end in "-equal_weight"."""
+    params = []
+    for alpha in ALPHAS:
+        for vals in sets:
+            vals = vals if isinstance(vals, tuple) else (vals,)
+            ident = "-".join(str(v) for v in vals) + ("" if alpha == "uniform" else "-" + alpha)
+            params.append(pytest.param(*vals, alpha, id=ident))
+    return pytest.mark.parametrize(argnames + ",alpha", params, indirect=list(indirect))
+
+
+def reference_signatures():
+    with open(os.path.join(GOLDEN, "reference_signatures.json")) as f:
+        return json.load(f)
+
+
+# The flag word each verdict of the reference implies (oracle/make_golden_flags.py): the forward's with the last-plane check.  The
+# forward never sets the range bits; without the last-plane check it never sets LAST_PLANE_OOB.
+FORWARD_FLAGS = {"ok": 0, "alpha": 0, "behind-eye": mpi_oracle.FLAG_PLANE_BEHIND_EYE, "out-of-plane": mpi_oracle.FLAG_LAST_PLANE_OOB}
+
+
+def load_flag_cases():
+    """[(name, verdict, case)] of tests/golden/flags_edges.npz; a case has rgba, dhw, view2mpi, ray_dir, eye, z_dir, align_corners."""
+    z = load_golden("flags_edges")
+    out = []
+    for name, verdict in zip(z["names"].tolist(), z["verdicts"].tolist()):
+        c = {k: z["pool_%d" % int(z[f"{name}__{k}"])] for k in ("dhw", "view2mpi", "ray_dir", "eye", "z_dir", "align_corners")}
+        r = z[f"{name}__rgba"]
+        c["rgba"] = np.random.default_rng(int(r[0])).random(tuple(z[f"{name}__rgba_shape"].tolist()), dtype=np.float32)
+        if len(r) > 1:
+            c["rgba"][tuple(int(i) for i in r[1:])] = z[f"{name}__rgba_value"]
+        out.append((name, verdict, c))
+    return out
+
+
+FLAG_CASES = load_flag_cases()
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# gradients through the wrappers (tests of the staged backward's box)
+# ------------------------------------------------------------------------------------------------------------------------------
+def expanded_grad(rgba, case, gc, gd, ray=None):
+    """d rgba of sum(colour * gc) (+ sum(depth * gd)) through render_views, as numpy."""
+    x = rgba.clone().requires_grad_(True)
+    color, depth = g.render_views(x, case.dhw, case.view2mpi, case.ray_dir if ray is None else ray, case.eye, case.z_dir)
+    loss = (color * gc).sum()
+    if gd is not None:
+        loss = loss + (depth * gd).sum()
+    loss.backward()
+    return x.grad.cpu().numpy()
+
+
+def factored_grads(rgb, alpha, bg, case, gc, gd, ray=None):
+    """(d rgb, d alpha, d bg_rgb) of the same loss through render_views_factored, as numpy."""
+    r, a, b = (t.clone().requires_grad_(True) for t in (rgb, alpha, bg))
+    color, depth = g.render_views_factored(r, a, case.dhw, case.view2mpi, case.ray_dir if ray is None else ray, case.eye, case.z_dir,
+                                           bg_rgb=b)
+    loss = (color * gc).sum()
+    if gd is not None:
+        loss = loss + (depth * gd).sum()
+    loss.backward()
+    return r.grad.cpu().numpy(), a.grad.cpu().numpy(), b.grad.cpu().numpy()
+
+
+def one_tile_per_mpi_case(d):
+    """Two MPIs, one near-frontal view each, of ONE 64 x 24 backward tile (rows 20..43 of a 64^2 pinhole image): every
+    (tile, plane) takes the box, and every texel of g_rgba receives exactly one flush per plane, so the result does not
+    depend on the order of fp32 atomics."""
+    case = synth.make_case(n_planes=6, tex=64, img=64, n_mpi=2, seed=13, device=d, last_alpha_one=True,
+                           yaws=[0.05, -0.08], pitches=[0.02, -0.03])
+    return dataclasses.replace(case, ray_dir=case.ray_dir[:, :, 20:44].contiguous())
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# the machine code of a built library
+# ------------------------------------------------------------------------------------------------------------------------------
+# The render-kernel key bits (kKey*, csrc/mpi_kernel_keys.cuh)
+KEY_AC, KEY_FAC, KEY_EMIT, KEY_ES, KEY_F16, KEY_STAGED, KEY_BWD, KEY_DET, KEY_SKIP, KEY_U8 = 1, 2, 4, 8, 16, 32, 64, 128, 256, 512
+
+
+class Kernel(NamedTuple):
+    template: str           # the C++ name: a kernel template, or a plain or extern "C" kernel
+    key: Optional[int]      # the render kernel's key (template<uint32_t K>), None for other kernels
+    sass: str
+    regs: int
+    stack: int
+    local: int
+
+    def digest(self):
+        """sha256 of the SASS instructions (addresses and encodings included, no names or comments)"""
+        lines = [l.strip() for l in self.sass.split("\n") if re.match(r"\s+/\*[0-9a-f]{4,}\*/", l)]
+        return hashlib.sha256("\n".join(lines).encode()).hexdigest()
+
+
+def library_kernels(path=None):
+    """{mangled name: Kernel} of a built library (cuobjdump -sass and -res-usage).  Kernels of namespace gmpi are
+    _ZN4gmpi<length><name>..., and a uint32_t template argument K mangles as ILj<K>E."""
+    path = path or g._build.LIB_PATH
+    run = lambda flag: subprocess.run(["cuobjdump", flag, path], capture_output=True, text=True, check=True).stdout
+    usage = {m[1]: (int(m[2]), int(m[3]), int(m[4]))
+             for m in re.finditer(r"Function (\S+):\s*\n\s*REG:(\d+) STACK:(\d+) SHARED:\d+ LOCAL:(\d+)", run("-res-usage"))}
+    out = {}
+    for f in re.split(r"\n\s*Function : ", run("-sass"))[1:]:
+        name, body = f.split("\n", 1)
+        name = name.strip()
+        template, key = name, None
+        m = re.match(r"_ZN4gmpi(\d+)", name)
+        if m:
+            end = m.end() + int(m[1])
+            template = name[m.end():end]
+            k = re.match(r"ILj(\d+)EE", name[end:])
+            key = int(k[1]) if k else None
+        out[name] = Kernel(template, key, body, *usage[name])
+    return out
+
+
+def render_kernels(kernels, template, has=0, lacks=0):
+    """{name: Kernel} of the instantiations of `template` whose key has every bit of `has` and none of `lacks`"""
+    return {n: k for n, k in kernels.items() if k.template == template and k.key & has == has and not k.key & lacks}
