@@ -115,9 +115,9 @@ def test_view_order_does_not_change_a_bit(form, variant):
 
 @each_alpha("variant", ["staged", "direct"], indirect=["variant"])
 def test_full_size_training_shape_is_repeatable(variant, alpha):
-    """4 MPIs x 1 view, 96 planes, 1024^2 texture and image (13.7 GB of scratch); the first MPI's gradient (its one view's) against
-    the oracle.  With equal-weight alpha every plane's gradient is far from 0, so repeatability is not met trivially on the back
-    planes."""
+    """4 MPIs x 1 view, 96 planes, 1024^2 texture and image (12.9 GB of sums: MPIs 2 and 3 start past 2^31 bytes of the gradient,
+    their sums past 2^32); every MPI's gradient (its one view's) against the oracle, on its own scale.  With equal-weight alpha every
+    plane's gradient is far from 0, so repeatability is not met trivially on the back planes."""
     d = dev()
     case = synth.make_case(n_planes=96, tex=1024, img=1024, n_mpi=4, seed=3, device=d, last_alpha_one=True, alpha=alpha)
     gc, gd = _upstream(4, 1024, 1024, 9, d)
@@ -125,11 +125,10 @@ def test_full_size_training_shape_is_repeatable(variant, alpha):
     assert_bitwise(a, _grads(case, gc, gd, deterministic=True))
     e = rel_err(a[0], _grads(case, gc, gd, deterministic=False)[0])
     assert e <= EXPECT, e
-    v0 = lambda t: n(t[:1])
-    ref = mpi_oracle.backward(v0(case.rgba), v0(case.view2mpi), v0(case.dhw), v0(case.ray_dir), v0(case.eye), v0(case.z_dir),
-                              v0(gc), v0(gd), nthreads=_NT)
-    e = rel_err(a[0][:1], ref)
-    assert e <= EXPECT, e
+    ref = mpi_oracle.backward(n(case.rgba), n(case.view2mpi), n(case.dhw), n(case.ray_dir), n(case.eye), n(case.z_dir), n(gc), n(gd),
+                              nthreads=_NT)
+    errs = [rel_err(a[0][m], ref[m]) for m in range(4)]
+    assert max(errs) <= EXPECT, errs
 
 
 def test_fifteen_views_of_one_mpi_are_repeatable(variant):

@@ -202,6 +202,7 @@ FULL = {   # name: synth.make_case arguments
     "full_96x512": dict(n_planes=96, tex=512, img=512, n_mpi=2, seed=1234),
     "full_96x1024": dict(n_planes=96, tex=1024, img=1024, n_mpi=1, seed=1234),
     "c3": dict(n_planes=96, tex=1024, img=1024, n_mpi=1, seed=1234, last_alpha_one=True),
+    "ffhq1024_batch4": dict(n_planes=96, tex=1024, img=1024, n_mpi=4, seed=1234, last_alpha_one=True),   # bench.py's batch: 6.4 GB
     "c5": dict(n_planes=96, tex=512, img=512, n_mpi=4, seed=99, last_alpha_one=True),
     "four_views": dict(n_planes=48, tex=512, img=512, n_mpi=1, views_per_mpi=4, seed=21, last_alpha_one=True),
     "c4_video": dict(n_planes=96, tex=512, img=512, n_mpi=1, views_per_mpi=15, seed=1234, yaws=_C4_YAWS, pitches=np.zeros(15, np.float32)),
@@ -223,10 +224,14 @@ def _oracle_forward(name, alpha):
     return rc, rd
 
 
-@each_alpha("N,res,V", [(32, 256, 8), (96, 512, 2), (96, 1024, 1)])
+_FULL_FWD = {(32, 256, 8): "full_32x256", (96, 512, 2): "full_96x512", (96, 1024, 1): "full_96x1024", (96, 1024, 4): "ffhq1024_batch4"}
+
+
+@each_alpha("N,res,V", list(_FULL_FWD))
 def test_full_size_against_oracle(N, res, V, alpha, fwd_variant_auto):
-    """The BASELINE.json shapes, every view."""
-    name = f"full_{N}x{res}"
+    """The BASELINE.json shapes, every view; (96, 1024, 4) is the benchmark's batch of four, whose MPIs 2 and 3 start past 2^31 and
+    2^32 bytes."""
+    name = _FULL_FWD[N, res, V]
     assert FULL[name]["n_mpi"] == V
     case = _full_case(name, alpha)
     color, depth = g.render_views(case.rgba, case.dhw, case.view2mpi, case.ray_dir, case.eye, case.z_dir,
@@ -451,6 +456,16 @@ def test_full_size_backward_c3_one_view_96x1024_vs_oracle(fwd_variant_auto, alph
     """BASELINE configs[2] (FFHQ1024 forward+backward): one 96-plane 1024^2 view, production alpha==1 last plane, colour and
     depth upstream gradients.  (gmpi/core/mpi.py:411-436 autograd; train.py:733-740.)"""
     assert _full_grad_check("c3", alpha, with_depth=True) <= EXPECT
+
+
+@each_alpha("fwd_variant_auto", _AUTO, indirect=["fwd_variant_auto"])
+def test_full_size_backward_ffhq1024_batch4_vs_oracle(fwd_variant_auto, alpha):
+    """BASELINE configs[2] at bench.py's batch: 4 MPIs x 96 planes x 1024^2 in one 6.4 GB tensor (MPI 2 starts past 2^31 bytes, MPI
+    3 past 2^32), one view each, colour and depth upstream gradients.  Each MPI's gradient against the oracle's, on its own scale."""
+    ours = _render_and_grad(_full_case("ffhq1024_batch4", alpha), with_depth=True)[2]
+    ref = _oracle_backward("ffhq1024_batch4", alpha, True)
+    errs = [rel_err(ours[m], ref[m]) for m in range(4)]
+    assert max(errs) <= EXPECT, errs
 
 
 @each_alpha("fwd_variant_auto", _AUTO, indirect=["fwd_variant_auto"])

@@ -8,6 +8,7 @@
   case, CASES                     the forward tests' catalogue: the golden fixtures and the synthetic cases
   forward_desc, render_fwd,       one gmpi_mpi_render_fwd_ex of a catalogue case, and the render of a native (fp16 / uint8) MPI
   native_vs_fp32                  beside the fp32 MPI it stands for, on the same kernel
+  BIG_*, big_views                the shapes, views and declared device peaks of the buffers past 2^31 elements
 and the helpers several modules read: the machine code of the built library, the staged forward's footprints and its limit cases,
 oracle-side bounds and references, and the flag cases of tests/golden/flags_edges.npz."""
 import contextlib
@@ -264,6 +265,64 @@ def headline_case():
     cs = synth.make_case(n_planes=96, tex=1024, img=1024, n_mpi=1, seed=1234, alpha="equal_weight")
     return dict(rgba=cs.rgba.numpy(), view2mpi=cs.view2mpi.numpy(), dhw=cs.dhw.numpy(), ray_dir=cs.ray_dir.numpy(),
                 eye=cs.eye.numpy(), z_dir=cs.z_dir.numpy(), ac=True)
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# buffers past 2^31 elements (tests/test_gpu_large_offsets.py runs them; tests/test_large_offsets.py checks their arithmetic)
+# ------------------------------------------------------------------------------------------------------------------------------
+BIG_N, BIG_R = 96, 1024
+BIG_IMG = BIG_R * BIG_R
+BIG_MPI = BIG_N * 4 * BIG_IMG       # elements of one expanded 96 x 1024^2 MPI
+BIG_SLABS = BIG_N * BIG_IMG         # elements of one factored alpha, or of one view's saved transmittance
+BIG_M = 6                           # expanded MPIs in the far buffer: MPI 5 starts at element 2,013,265,920
+BIG_M_FACTORED = 22                 # factored alphas, and views of saved transmittance: the last starts at 2,113,929,216
+BIG_V_COLOR, BIG_V_GATHER = 684, 513        # colour / video frames, fused-gather frames of 1024^2 pixels
+SMALL_MPI = dict(N=8, R=256)        # the MPI of the output tests
+BIG_SLACK = 1 << 28                 # views, rays, outputs of a few views, flags and occupancy maps: under 256 MiB in every test
+
+# test key: the device bytes its buffers hold at its peak, from the shapes above (BIG_SLACK on top)
+BIG_PEAK_BYTES = {
+    # far buffer, the fp32 MPI uploaded, the native MPI and its fp32 conversion
+    "expanded_forward-fp32": BIG_M * BIG_MPI * 4 + BIG_MPI * 4,
+    "expanded_forward-fp16": BIG_M * BIG_MPI * 2 + BIG_MPI * 4 + BIG_MPI * 2 + BIG_MPI * 4,
+    "expanded_forward-uint8": BIG_M * BIG_MPI + BIG_MPI * 4 + BIG_MPI + BIG_MPI * 4,
+    "wrong_inputs": BIG_M * BIG_MPI * 4 + 2 * BIG_MPI * 4,
+    "skipping": BIG_M * BIG_MPI * 4 + BIG_MPI * 4,
+    # rgba and g_rgba, the upload, two views' transmittance
+    "expanded_backward": 2 * BIG_M * BIG_MPI * 4 + BIG_MPI * 4 + 2 * BIG_SLABS * 4,
+    # alpha and g_alpha, rgb / bg_rgb and their gradients, the one MPI's factors, two views' transmittance
+    "factored": 2 * BIG_M_FACTORED * BIG_SLABS * 4 + 4 * BIG_M_FACTORED * 3 * BIG_IMG * 4 + (BIG_SLABS + 6 * BIG_IMG) * 4
+                + 2 * BIG_SLABS * 4,
+    # transmittance, rgba and g_rgba, 8 B of deterministic scratch per gradient element, rays / colour / upstream of 22 views
+    "saved_transmittance": BIG_M_FACTORED * BIG_SLABS * 4 + 2 * BIG_MPI * 4 + BIG_MPI * 8 + 4 * BIG_M_FACTORED * 4 * BIG_IMG * 4,
+    # the frames, and in front of those past 2^31 elements 2^31 sentinels (where a signed 32-bit offset would wrap to)
+    "outputs-color": (BIG_V_COLOR * 4 * BIG_IMG + (1 << 31)) * 4,
+    "outputs-video": BIG_V_COLOR * 4 * BIG_IMG + (1 << 31),
+    "outputs-gather": (BIG_V_GATHER * 4 * BIG_IMG + (1 << 31)) * 4,
+    "range_check-fp32-vector": BIG_M * BIG_MPI * 4,
+    "range_check-fp32-scalar": BIG_M * BIG_N * 4 * 1023 * 1023 * 4,
+    "range_check-fp16-vector": BIG_M * BIG_MPI * 2,
+    "range_check-fp16-scalar": BIG_M * BIG_N * 4 * 1023 * 1023 * 2,
+    # the uint8 MPI on the device, and the host entry point's two staging slots (the library's own cudaMalloc: this is what the
+    # test needs free, but torch's peak, which the budget fixture checks, does not see them)
+    "host_entry_point": 3 * BIG_MPI,
+    # the fp32 batch of four and the three temporaries of its equal-weight alpha (synth.equal_weight_alpha); the later steps (the
+    # factored form, the fp16 and uint8 copies and their conversions) hold less
+    "batch_of_four": 4 * BIG_MPI * 4 + 3 * 4 * BIG_SLABS * 4,
+}
+
+
+@functools.lru_cache(maxsize=None)
+def big_views():
+    """The two views of tests/test_gpu_large_offsets.py, both of MPI 0 (the caller moves them): view 0 is headline_case's pinhole
+    view, whose stages take the staged forward's fast body at every box class; view 1 holds the same rays shuffled over the image,
+    so no tile's corner rays bound its taps and every stage takes the generic body.  Geometry only: headline_case has the MPI."""
+    cs = synth.make_case(n_planes=96, tex=1024, img=1024, n_mpi=1, seed=1234, rgba=False)
+    perm = torch.randperm(1024 * 1024, generator=torch.Generator().manual_seed(7))
+    shuffled = cs.ray_dir.reshape(1, 3, -1)[:, :, perm].reshape(cs.ray_dir.shape)
+    two = lambda t: torch.cat([t, t]).numpy()
+    return dict(view2mpi=np.zeros(2, np.int32), dhw=cs.dhw.numpy(), ray_dir=torch.cat([cs.ray_dir, shuffled]).numpy(),
+                eye=two(cs.eye), z_dir=two(cs.z_dir), ac=True)
 
 
 def assert_class_88_behind_plane_25(c):
