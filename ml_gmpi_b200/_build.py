@@ -11,8 +11,8 @@ PKG_DIR = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG_DIR, "csrc")
 LIB_PATH = os.path.join(PKG_DIR, "libgmpi_mpi_render.so")
 SOURCES = ["mpi_render.cu", "mpi_skip.cu", "mpi_u8.cu"]
-HEADERS = ["mpi_common.cuh", "mpi_fwd_staged.cuh", "mpi_fwd_direct.cuh", "mpi_kernel_keys.cuh", "mpi_bwd_box.cuh", "tma_utils.cuh",
-           os.path.join("..", "..", "include", "gmpi_mpi_render.h")]
+HEADERS = ["mpi_common.cuh", "mpi_fwd_staged.cuh", "mpi_fwd_direct.cuh", "mpi_kernel_keys.cuh", "mpi_bwd_box.cuh", "mpi_bwd_direct.cuh",
+           "mpi_range_check.cuh", "mpi_light.cuh", "mpi_debug.cuh", "tma_utils.cuh", os.path.join("..", "..", "include", "gmpi_mpi_render.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-diag-suppress", "1886", "-shared",
               "-Xcompiler", "-fPIC"]
 

@@ -210,6 +210,79 @@ __device__ __forceinline__ long long det_rescale(int s, int te, int ue) {
     const long long q = (a + (1ll << (-sh - 1))) >> -sh;
     return s < 0 ? -q : q;
 }
+
+// The call's scale pre-pass and the finish pass of the deterministic backward.
+// bounds[0] = max over every pixel of every view of the box kernel's per-pixel alpha bound |G_r| + |G_g| + |G_b| + |G_d dz| *
+// max_i |z_diff_i| / |ray_z| (the same float operations as the tile bound of bwd_box_body, so no tile's exponent exceeds the
+// call's); bounds[1] = max |G_c|.  Pixels with an inf/NaN upstream gradient are left out of bounds[0] and non-finite
+// components out of bounds[1]: their contributions go to the non-finite bits.  Integer atomicMax on the bits of non-negative
+// floats: independent of order.  Grid (pixel blocks, min(V, 65535)) of 256 threads; block row y takes views y, y + gridDim.y, ...
+__global__ void __launch_bounds__(256)
+mpi_bwd_det_bounds_kernel(const RenderParams p, uint32_t* __restrict__ bounds) {
+    __shared__ unsigned s_zmax;
+    const size_t img = (size_t)p.H * p.W, pix = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const float gscale = (p.options & GMPI_COLOR_MINUS1_1) ? 2.0f : 1.0f;
+    float qmax = 0.0f, gmax = 0.0f;
+    for (int v = blockIdx.y; v < p.V; v += gridDim.y) {
+        const int m = __ldg(p.view2mpi + v);
+        const float ev[3] = {__ldg(p.eye + 3 * v), __ldg(p.eye + 3 * v + 1), __ldg(p.eye + 3 * v + 2)};
+        const float zd[3] = {__ldg(p.z_dir + 3 * v), __ldg(p.z_dir + 3 * v + 1), __ldg(p.z_dir + 3 * v + 2)};
+        __syncthreads();
+        if (threadIdx.x == 0) s_zmax = 0u;
+        __syncthreads();
+        float zm = 0.0f;
+        for (int i = threadIdx.x; i < p.N; i += blockDim.x)
+            zm = fmaxf(zm, fabsf(make_plane_const(p.dhw + ((size_t)m * p.N + i) * 3, ev[2]).z_diff));
+        atomicMax(&s_zmax, __float_as_uint(zm));
+        __syncthreads();
+        const float zmax = __uint_as_float(s_zmax);
+        if (pix < img) {
+            const float* rd = p.ray_dir + (size_t)v * 3 * img + pix;
+            const RayConst rc = make_ray_const(__ldg(rd), __ldg(rd + img), __ldg(rd + 2 * img), ev, zd);
+            const float* gc = p.g_color + (size_t)v * 3 * img + pix;
+            const float g0 = gscale * __ldg(gc), g1 = gscale * __ldg(gc + img), g2 = gscale * __ldg(gc + 2 * img);
+            const float g3 = p.g_depth ? __ldg(p.g_depth + (size_t)v * img + pix) * rc.dz : 0.0f;
+            const float ga = fabsf(g0) + fabsf(g1) + fabsf(g2), gd = fabsf(g3);
+            if (ga + gd <= 0x1.fffffep127f) qmax = fmaxf(qmax, ga + gd * (zmax * fabsf(rc.yrz)));   // NaN (0 * inf) is dropped
+            const auto fin = [](float x) { return fabsf(x) <= 0x1.fffffep127f ? fabsf(x) : 0.0f; };
+            gmax = fmaxf(gmax, fmaxf(fin(g0), fmaxf(fin(g1), fin(g2))));
+        }
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+        qmax = fmaxf(qmax, __shfl_xor_sync(0xffffffffu, qmax, o));
+        gmax = fmaxf(gmax, __shfl_xor_sync(0xffffffffu, gmax, o));
+    }
+    if ((threadIdx.x & 31) == 0) {
+        if (qmax > 0.0f) atomicMax(bounds, __float_as_uint(qmax));
+        if (gmax > 0.0f) atomicMax(bounds + 1, __float_as_uint(gmax));
+    }
+}
+
+// The finish pass: element i of the sums (layout: g_rgba, or g_rgb | g_alpha | g_bg_rgb) -> fp32, written (`zero`) or added into
+// the caller's gradient.  Non-finite bits give what an fp32 sum of the contributions gives: NaN if a NaN or both infinities were
+// added, else the infinity.  seg1 / seg2: first elements of g_alpha and g_bg_rgb in the sums (factored; G otherwise).
+__global__ void __launch_bounds__(256)
+mpi_bwd_det_finish_kernel(const DetAcc da, float* __restrict__ g0, float* __restrict__ g1, float* __restrict__ g2, size_t G, size_t seg1,
+                          size_t seg2, size_t tex, bool factored, bool zero) {
+    const DetUnit ua = det_unit(__uint_as_float(__ldg(da.bounds)), da.k_a);
+    const DetUnit urgb = det_unit(0.5f * __uint_as_float(__ldg(da.bounds + 1)), da.k_rgb);
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < G; i += (size_t)gridDim.x * blockDim.x) {
+        const bool alpha = factored ? (i >= seg1 && i < seg2) : (i / tex) % 4 == 3;
+        const uint32_t nf = (__ldcs(da.nf + (i >> 3)) >> ((i & 7) * 4)) & 7u;
+        float x;
+        if (nf) {
+            x = (nf & 4u) || nf == 3u ? __int_as_float(0x7fffffff) : nf == 1u ? INFINITY : -INFINITY;
+        } else {
+            // RN to fp32, then an exact power-of-two scale in two normal steps (a result below the normal range rounds once more)
+            const int ue = alpha ? ua.ue : urgb.ue, h = ue / 2;
+            x = __ll2float_rn((long long)__ldcs(da.acc + i));
+            x = __fmul_rn(__fmul_rn(x, __uint_as_float((unsigned)(127 + h) << 23)), __uint_as_float((unsigned)(127 + ue - h) << 23));
+        }
+        float* dst = i < seg1 ? g0 + i : i < seg2 ? g1 + (i - seg1) : g2 + (i - seg2);
+        *dst = zero ? x : *dst + x;
+    }
+}
+
 __device__ __noinline__ void scatter_plane_det(const DetAcc& da, const DetUnit& ua, const DetUnit& urgb, float* __restrict__ gplane,
                                                size_t tex, int Wt, int Ht, int x0, int y0, float v0, float v1, float v2, float v3,
                                                float w00, float w01, float w10, float w11) {

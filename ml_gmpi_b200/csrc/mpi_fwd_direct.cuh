@@ -1,6 +1,7 @@
 // Forward, direct-gather variant: one thread = one output pixel, a warp = 32 consecutive x.  Taps are read straight from global
 // memory through L1 (per channel a warp touches one or two 128-byte lines per tap row).  Works for every shape; the TMA-staged
-// variant is the fast path.  Shared by the library's kernels (mpi_render.cu) and the uint8 kernels (mpi_u8.cu).
+// variant is the fast path.  Shared by the library's kernels (mpi_render.cu) and the uint8 kernels (mpi_u8.cu); the direct backward
+// is in mpi_bwd_direct.cuh.
 #pragma once
 #include "mpi_common.cuh"
 #include "mpi_kernel_keys.cuh"

@@ -45,8 +45,9 @@ extern const KernelUnit u8_unit;       // mpi_u8.cu: every uint8 kernel
 
 }  // namespace gmpi
 
-// The kernels of mpi_skip.cu and mpi_u8.cu that are not render kernels: mpi_render.cu launches them by their own symbols.  Their
-// files include this header, so a definition that does not match its declaration here does not compile.
+// The kernels of mpi_skip.cu and mpi_u8.cu that are not render kernels: mpi_render.cu launches them by their own symbols through
+// launch_kernel, which checks each launch's arguments against these declarations.  Their files include this header, so a definition
+// that does not match its declaration here does not compile.
 extern "C" {
 // mpi_skip.cu: the occupancy-map builds
 __global__ void gmpi_occ_expanded_f32(const uint32_t*, uint32_t*, uint32_t*, int, int, int, int, int);

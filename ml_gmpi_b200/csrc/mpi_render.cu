@@ -1,6 +1,9 @@
-// MPI over-composite renderer for H100 (sm_90a): kernels + C ABI (include/gmpi_mpi_render.h).
+// MPI over-composite renderer for H100 (sm_90a): the C ABI (include/gmpi_mpi_render.h) and the table of this file's render kernels.
 //
-// Replaces gmpi/core/mpi.py MPI.forward (:308-436) + homography (:26-153) and their autograd.
+// Replaces gmpi/core/mpi.py MPI.forward (:308-436) + homography (:26-153) and their autograd.  The kernels live beside their
+// siblings: the staged forward (mpi_fwd_staged.cuh), the direct forward and backward (mpi_fwd_direct.cuh, mpi_bwd_direct.cuh), the
+// box backward and the deterministic backward's passes (mpi_bwd_box.cuh), the range check (mpi_range_check.cuh), the LightRenderer
+// kernels (mpi_light.cuh) and the test hooks' kernels (mpi_debug.cuh).  Every kernel is launched through launch_args.
 // DESIGN.md describes the data layout, each kernel and its roofline.
 #include <cuda_runtime.h>
 #include <stdarg.h>
@@ -13,6 +16,9 @@
 #include <atomic>
 #include <iterator>
 #include <mutex>
+#include <tuple>
+#include <type_traits>
+#include <utility>
 
 #include "../../include/gmpi_mpi_render.h"
 #include "mpi_common.cuh"
@@ -20,6 +26,9 @@
 #include "mpi_bwd_box.cuh"
 #include "mpi_light.cuh"
 #include "mpi_fwd_direct.cuh"
+#include "mpi_bwd_direct.cuh"
+#include "mpi_range_check.cuh"
+#include "mpi_debug.cuh"
 #include "mpi_kernel_keys.cuh"
 
 namespace gmpi {
@@ -45,339 +54,6 @@ static int fail(int code, const char* fmt, ...) {
                         __FILE__, __LINE__);                                                      \
     } while (0)
 
-// ------------------------------------------------------------------------------------------
-// Backward, direct variant.
-//   pass A (front to back, alpha only): T_i = prod_{j<i}(1 - a_j + 1e-10), stashed per thread in
-//           shared memory ([plane][thread], conflict free).
-//   pass B (back to front, all channels): R_{i-1} = a_i q_i + s_i R_i with R_{N-1} = 0,
-//           q_i = G.rgb_i + Gd*depth_i, s_i = 1 - a_i + 1e-10, and
-//             dL/d rgb_i = G * a_i T_i
-//             dL/d a_i   = T_i (q_i - R_i)
-//           which equals autograd's  T_i q_i - (sum_{k>i} a_k q_k P_k)/s_i  (cumprod_backward)
-//           without the division by s_i (1e-10 when a_i == 1) and without cancellation.
-//           The four bilinear weights scatter each value with red.global.add.f32.
-// kDet: the deterministic backward's variant, which adds each contribution to the int64 sums of `da` instead (det_add).
-// ------------------------------------------------------------------------------------------
-template <bool kAlignCorners, bool kDet>
-__device__ __forceinline__ void bwd_direct_body(const RenderParams p, const int tile_w, const int tile_h, const DetAcc da) {
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    PlaneConst* s_pc = reinterpret_cast<PlaneConst*>(smem_raw);
-    const int nthreads = tile_w * tile_h;
-    float* s_T = reinterpret_cast<float*>(smem_raw + sizeof(PlaneConst) * p.N);   // [N][nthreads]
-
-    const int v = blockIdx.z;
-    const int m = __ldg(p.view2mpi + v);
-    const int tid = threadIdx.y * tile_w + threadIdx.x;
-    const float* e = p.eye + 3 * v;
-    for (int i = tid; i < p.N; i += nthreads) {
-        s_pc[i] = make_plane_const(p.dhw + ((size_t)m * p.N + i) * 3, __ldg(e + 2));
-    }
-    __syncthreads();
-
-    const int px = blockIdx.x * tile_w + threadIdx.x;
-    const int py = blockIdx.y * tile_h + threadIdx.y;
-    if (px >= p.W || py >= p.H) return;
-
-    const size_t img = (size_t)p.H * p.W;
-    const size_t pix = (size_t)py * p.W + px;
-    const float* rd = p.ray_dir + (size_t)v * 3 * img + pix;
-    const float ev[3] = {__ldg(e), __ldg(e + 1), __ldg(e + 2)};
-    const float zd[3] = {__ldg(p.z_dir + 3 * v), __ldg(p.z_dir + 3 * v + 1), __ldg(p.z_dir + 3 * v + 2)};
-    const RayConst rc = make_ray_const(__ldg(rd), __ldg(rd + img), __ldg(rd + 2 * img), ev, zd);
-
-    const int Ht = p.Ht, Wt = p.Wt, N = p.N;
-    const float fWt = (float)Wt, fHt = (float)Ht;
-    const float hsx = 0.5f * (float)(Wt - 1), hsy = 0.5f * (float)(Ht - 1);
-    const size_t tex = (size_t)Ht * Wt;
-
-    float gscale = (p.options & GMPI_COLOR_MINUS1_1) ? 2.0f : 1.0f;
-    const float* gc = p.g_color + (size_t)v * 3 * img + pix;
-    const float G0 = gscale * __ldg(gc), G1 = gscale * __ldg(gc + img), G2 = gscale * __ldg(gc + 2 * img);
-    const float Gd = p.g_depth ? __ldg(p.g_depth + (size_t)v * img + pix) : 0.0f;
-    const float Gdz = Gd * rc.dz;   // depth_i = scale_i * dz
-    DetUnit ua{}, urgb{};
-    if constexpr (kDet) {
-        ua = det_unit(__uint_as_float(__ldg(da.bounds)), da.k_a);
-        urgb = det_unit(0.5f * __uint_as_float(__ldg(da.bounds + 1)), da.k_rgb);
-    }
-
-    // pass A
-    float T = 1.0f;
-    for (int i = 0; i < N; ++i) {
-        s_T[(size_t)i * nthreads + tid] = T;
-        const TexCoord tc = plane_coord<kAlignCorners>(s_pc[i], rc, hsx, hsy, fWt, fHt);
-        if (coord_hits(tc.ix, tc.iy, fWt, fHt)) {
-            const Taps t = make_taps(tc.ix, tc.iy, Ht, Wt);
-            const float a = tap4(plane_chans(p, m, i, tex).c[3], t);
-            T *= (1.0f - a) + 1e-10f;
-        }
-    }
-    // pass B
-    float R = 0.0f;
-    for (int i = N - 1; i >= 0; --i) {
-        const TexCoord tc = plane_coord<kAlignCorners>(s_pc[i], rc, hsx, hsy, fWt, fHt);
-        if (!coord_hits(tc.ix, tc.iy, fWt, fHt)) continue;
-        const Taps t = make_taps(tc.ix, tc.iy, Ht, Wt);
-        const PlaneChans plane = plane_chans(p, m, i, tex);
-        const float r = tap4(plane.c[0], t);
-        const float g = tap4(plane.c[1], t);
-        const float b = tap4(plane.c[2], t);
-        const float a = tap4(plane.c[3], t);
-        const float Ti = s_T[(size_t)i * nthreads + tid];
-        const float q = fmaf(G0, r, fmaf(G1, g, fmaf(G2, b, Gdz * tc.scale)));
-        const float w = a * Ti;
-        const float gv[4] = {G0 * w, G1 * w, G2 * w, Ti * (q - R)};
-        R = fmaf(a, q, ((1.0f - a) + 1e-10f) * R);
-        const GradChans gp = grad_chans(p, m, i, tex);
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-            float* gch = gp.c[c];
-            if constexpr (kDet) {
-                const DetUnit& u = c == 3 ? ua : urgb;
-                if (t.w00 != 0.0f) det_add(da, u, gch + t.o00, gv[c] * t.w00);
-                if (t.w01 != 0.0f) det_add(da, u, gch + t.o01, gv[c] * t.w01);
-                if (t.w10 != 0.0f) det_add(da, u, gch + t.o10, gv[c] * t.w10);
-                if (t.w11 != 0.0f) det_add(da, u, gch + t.o11, gv[c] * t.w11);
-            } else {
-                if (t.w00 != 0.0f) atomicAdd(gch + t.o00, gv[c] * t.w00);
-                if (t.w01 != 0.0f) atomicAdd(gch + t.o01, gv[c] * t.w01);
-                if (t.w10 != 0.0f) atomicAdd(gch + t.o10, gv[c] * t.w10);
-                if (t.w11 != 0.0f) atomicAdd(gch + t.o11, gv[c] * t.w11);
-            }
-        }
-    }
-}
-
-// The direct backward kernels by key (KeyTraits), and the deterministic ones (kKeyDet), which take the DetAcc too.
-template <uint32_t K>
-__global__ void __launch_bounds__(128)
-mpi_bwd_direct_kernel(const RenderParams p, const int tile_w, const int tile_h) {
-    static_assert((K & ~kKeyAC) == kKeyBwd, "a direct backward key");
-    bwd_direct_body<KeyTraits<K>::kAlignCorners, false>(p, tile_w, tile_h, DetAcc{});
-}
-
-template <uint32_t K>
-__global__ void __launch_bounds__(128)
-mpi_bwd_direct_det_kernel(const RenderParams p, const int tile_w, const int tile_h, const DetAcc da) {
-    static_assert((K & ~kKeyAC) == (kKeyBwd | kKeyDet), "a deterministic direct backward key");
-    bwd_direct_body<KeyTraits<K>::kAlignCorners, true>(p, tile_w, tile_h, da);
-}
-
-// ------------------------------------------------------------------------------------------
-// Deterministic backward: the call's scale pre-pass and the finish pass (see DetAcc in mpi_bwd_box.cuh).
-// ------------------------------------------------------------------------------------------
-// bounds[0] = max over every pixel of every view of the box kernel's per-pixel alpha bound |G_r| + |G_g| + |G_b| + |G_d dz| *
-// max_i |z_diff_i| / |ray_z| (the same float operations as the tile bound of bwd_box_body, so no tile's exponent exceeds the
-// call's); bounds[1] = max |G_c|.  Pixels with an inf/NaN upstream gradient are left out of bounds[0] and non-finite
-// components out of bounds[1]: their contributions go to the non-finite bits.  Integer atomicMax on the bits of non-negative
-// floats: independent of order.  Grid (pixel blocks, min(V, 65535)) of 256 threads; block row y takes views y, y + gridDim.y, ...
-__global__ void __launch_bounds__(256)
-mpi_bwd_det_bounds_kernel(const RenderParams p, uint32_t* __restrict__ bounds) {
-    __shared__ unsigned s_zmax;
-    const size_t img = (size_t)p.H * p.W, pix = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const float gscale = (p.options & GMPI_COLOR_MINUS1_1) ? 2.0f : 1.0f;
-    float qmax = 0.0f, gmax = 0.0f;
-    for (int v = blockIdx.y; v < p.V; v += gridDim.y) {
-        const int m = __ldg(p.view2mpi + v);
-        const float ev[3] = {__ldg(p.eye + 3 * v), __ldg(p.eye + 3 * v + 1), __ldg(p.eye + 3 * v + 2)};
-        const float zd[3] = {__ldg(p.z_dir + 3 * v), __ldg(p.z_dir + 3 * v + 1), __ldg(p.z_dir + 3 * v + 2)};
-        __syncthreads();
-        if (threadIdx.x == 0) s_zmax = 0u;
-        __syncthreads();
-        float zm = 0.0f;
-        for (int i = threadIdx.x; i < p.N; i += blockDim.x)
-            zm = fmaxf(zm, fabsf(make_plane_const(p.dhw + ((size_t)m * p.N + i) * 3, ev[2]).z_diff));
-        atomicMax(&s_zmax, __float_as_uint(zm));
-        __syncthreads();
-        const float zmax = __uint_as_float(s_zmax);
-        if (pix < img) {
-            const float* rd = p.ray_dir + (size_t)v * 3 * img + pix;
-            const RayConst rc = make_ray_const(__ldg(rd), __ldg(rd + img), __ldg(rd + 2 * img), ev, zd);
-            const float* gc = p.g_color + (size_t)v * 3 * img + pix;
-            const float g0 = gscale * __ldg(gc), g1 = gscale * __ldg(gc + img), g2 = gscale * __ldg(gc + 2 * img);
-            const float g3 = p.g_depth ? __ldg(p.g_depth + (size_t)v * img + pix) * rc.dz : 0.0f;
-            const float ga = fabsf(g0) + fabsf(g1) + fabsf(g2), gd = fabsf(g3);
-            if (ga + gd <= 0x1.fffffep127f) qmax = fmaxf(qmax, ga + gd * (zmax * fabsf(rc.yrz)));   // NaN (0 * inf) is dropped
-            const auto fin = [](float x) { return fabsf(x) <= 0x1.fffffep127f ? fabsf(x) : 0.0f; };
-            gmax = fmaxf(gmax, fmaxf(fin(g0), fmaxf(fin(g1), fin(g2))));
-        }
-    }
-    for (int o = 16; o > 0; o >>= 1) {
-        qmax = fmaxf(qmax, __shfl_xor_sync(0xffffffffu, qmax, o));
-        gmax = fmaxf(gmax, __shfl_xor_sync(0xffffffffu, gmax, o));
-    }
-    if ((threadIdx.x & 31) == 0) {
-        if (qmax > 0.0f) atomicMax(bounds, __float_as_uint(qmax));
-        if (gmax > 0.0f) atomicMax(bounds + 1, __float_as_uint(gmax));
-    }
-}
-
-// The finish pass: element i of the sums (layout: g_rgba, or g_rgb | g_alpha | g_bg_rgb) -> fp32, written (`zero`) or added into
-// the caller's gradient.  Non-finite bits give what an fp32 sum of the contributions gives: NaN if a NaN or both infinities were
-// added, else the infinity.  seg1 / seg2: first elements of g_alpha and g_bg_rgb in the sums (factored; G otherwise).
-__global__ void __launch_bounds__(256)
-mpi_bwd_det_finish_kernel(const DetAcc da, float* __restrict__ g0, float* __restrict__ g1, float* __restrict__ g2, size_t G, size_t seg1,
-                          size_t seg2, size_t tex, bool factored, bool zero) {
-    const DetUnit ua = det_unit(__uint_as_float(__ldg(da.bounds)), da.k_a);
-    const DetUnit urgb = det_unit(0.5f * __uint_as_float(__ldg(da.bounds + 1)), da.k_rgb);
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < G; i += (size_t)gridDim.x * blockDim.x) {
-        const bool alpha = factored ? (i >= seg1 && i < seg2) : (i / tex) % 4 == 3;
-        const uint32_t nf = (__ldcs(da.nf + (i >> 3)) >> ((i & 7) * 4)) & 7u;
-        float x;
-        if (nf) {
-            x = (nf & 4u) || nf == 3u ? __int_as_float(0x7fffffff) : nf == 1u ? INFINITY : -INFINITY;
-        } else {
-            // RN to fp32, then an exact power-of-two scale in two normal steps (a result below the normal range rounds once more)
-            const int ue = alpha ? ua.ue : urgb.ue, h = ue / 2;
-            x = __ll2float_rn((long long)__ldcs(da.acc + i));
-            x = __fmul_rn(__fmul_rn(x, __uint_as_float((unsigned)(127 + h) << 23)), __uint_as_float((unsigned)(127 + ue - h) << 23));
-        }
-        float* dst = i < seg1 ? g0 + i : i < seg2 ? g1 + (i - seg1) : g2 + (i - seg2);
-        *dst = zero ? x : *dst + x;
-    }
-}
-
-// ------------------------------------------------------------------------------------------
-// Range check: one streaming pass over rgba, testing each element's bit pattern (ElemTraits<E>::out_of_unit).
-// ------------------------------------------------------------------------------------------
-using F32Elem = ElemTraits<float>;
-using F16Elem = ElemTraits<__half>;
-
-__global__ void __launch_bounds__(256)
-mpi_check_range_kernel(const float4* __restrict__ rgba4, size_t n_slabs, size_t slab4, uint32_t* flags) {
-    // one slab = one (mpi, plane, channel) image of slab4 float4's; channel = slab % 4
-    uint32_t flag = 0;
-    const size_t total = n_slabs * slab4;
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-        const float4 x = __ldcs(rgba4 + i);
-        if (F32Elem::out_of_unit(__float_as_uint(x.x)) || F32Elem::out_of_unit(__float_as_uint(x.y)) ||
-            F32Elem::out_of_unit(__float_as_uint(x.z)) || F32Elem::out_of_unit(__float_as_uint(x.w))) {
-            const size_t slab = i / slab4;
-            flag |= ((slab & 3) == 3) ? (GMPI_FLAG_ALPHA_RANGE | GMPI_FLAG_RGBA_RANGE) : GMPI_FLAG_RGBA_RANGE;
-        }
-    }
-    flag = __reduce_or_sync(0xffffffffu, flag);
-    if (flag && (threadIdx.x & 31) == 0) atomicOr(flags, flag);
-}
-
-__global__ void mpi_check_range_scalar_kernel(const float* __restrict__ rgba, size_t n_slabs, size_t slab,
-                                              uint32_t* flags) {
-    uint32_t flag = 0;
-    const size_t total = n_slabs * slab;
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-        if (F32Elem::out_of_unit(__float_as_uint(__ldcs(rgba + i)))) {
-            flag |= (((i / slab) & 3) == 3) ? (GMPI_FLAG_ALPHA_RANGE | GMPI_FLAG_RGBA_RANGE) : GMPI_FLAG_RGBA_RANGE;
-        }
-    }
-    if (flag) atomicOr(flags, flag);
-}
-
-// The same check of an fp16 MPI, with the flags the fp32 check sets on its upcast.
-
-__global__ void __launch_bounds__(256)
-mpi_check_range_f16_kernel(const uint4* __restrict__ rgba8, size_t n_slabs, size_t slab8, uint32_t* flags) {
-    // one slab = one (mpi, plane, channel) image of slab8 groups of eight halves; channel = slab % 4
-    uint32_t flag = 0;
-    const size_t total = n_slabs * slab8;
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-        const uint4 x = __ldcs(rgba8 + i);
-        const uint32_t w[4] = {x.x, x.y, x.z, x.w};
-        bool out = false;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) out = out || F16Elem::out_of_unit(w[k] & 0xffffu) || F16Elem::out_of_unit(w[k] >> 16);
-        if (out) flag |= (((i / slab8) & 3) == 3) ? (GMPI_FLAG_ALPHA_RANGE | GMPI_FLAG_RGBA_RANGE) : GMPI_FLAG_RGBA_RANGE;
-    }
-    flag = __reduce_or_sync(0xffffffffu, flag);
-    if (flag && (threadIdx.x & 31) == 0) atomicOr(flags, flag);
-}
-
-__global__ void mpi_check_range_f16_scalar_kernel(const unsigned short* __restrict__ rgba, size_t n_slabs, size_t slab, uint32_t* flags) {
-    uint32_t flag = 0;
-    const size_t total = n_slabs * slab;
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-        if (F16Elem::out_of_unit(__ldcs(rgba + i)))
-            flag |= (((i / slab) & 3) == 3) ? (GMPI_FLAG_ALPHA_RANGE | GMPI_FLAG_RGBA_RANGE) : GMPI_FLAG_RGBA_RANGE;
-    }
-    if (flag) atomicOr(flags, flag);
-}
-
-// ------------------------------------------------------------------------------------------
-// Test hook: texel coordinates.
-// ------------------------------------------------------------------------------------------
-template <bool kAlignCorners>
-__global__ void mpi_debug_coords_kernel(const int32_t* view2mpi, const float* dhw, const float* ray_dir,
-                                        const float* eye, float* out, int V, int N, int Ht, int Wt, int H, int W) {
-    const size_t img = (size_t)H * W;
-    const size_t pix = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const int v = blockIdx.y;
-    if (pix >= img) return;
-    const int m = view2mpi[v];
-    const float* e = eye + 3 * v;
-    const float ev[3] = {e[0], e[1], e[2]};
-    const float zd[3] = {0.f, 0.f, 1.f};
-    const float* rd = ray_dir + (size_t)v * 3 * img + pix;
-    const RayConst rc = make_ray_const(rd[0], rd[img], rd[2 * img], ev, zd);
-    const float hsx = 0.5f * (float)(Wt - 1), hsy = 0.5f * (float)(Ht - 1);
-    for (int i = 0; i < N; ++i) {
-        const PlaneConst pc = make_plane_const(dhw + ((size_t)m * N + i) * 3, ev[2]);
-        const TexCoord tc = plane_coord<kAlignCorners>(pc, rc, hsx, hsy, (float)Wt, (float)Ht);
-        out[(((size_t)v * N + i) * 2 + 0) * img + pix] = tc.ix;
-        out[(((size_t)v * N + i) * 2 + 1) * img + pix] = tc.iy;
-    }
-}
-
-// Test hook for the pixel-pair coordinate path of the staged kernel: pixels 2k, 2k+1 of a row form a pair (both of the staged
-// kernel's pairs per thread hold it).
-template <bool kAlignCorners>
-__global__ void mpi_debug_coords_packed_kernel(const int32_t* view2mpi, const float* dhw, const float* ray_dir,
-                                               const float* eye, float* out, int V, int N, int Ht, int Wt, int H, int W) {
-    const size_t img = (size_t)H * W;
-    const size_t pair = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const int v = blockIdx.y;
-    if (pair * 2 + 1 >= img) return;
-    const int m = view2mpi[v];
-    const float* e = eye + 3 * v;
-    const float ev[3] = {e[0], e[1], e[2]};
-    const float zd[3] = {0.f, 0.f, 1.f};
-    RayConst rc[kPix];
-    for (int q = 0; q < kPix; ++q) {
-        const float* rd = ray_dir + (size_t)v * 3 * img + pair * 2 + (q & 1);
-        rc[q] = make_ray_const(rd[0], rd[img], rd[2 * img], ev, zd);
-    }
-    RayPairs rp;
-    pack_ray_pairs(rc, rp);
-    const float hsx = 0.5f * (float)(Wt - 1), hsy = 0.5f * (float)(Ht - 1);
-    for (int i = 0; i < N; ++i) {
-        const PlaneConst pc = make_plane_const(dhw + ((size_t)m * N + i) * 3, ev[2]);
-        CoordPairs c;
-        coords_pairs<kAlignCorners>(pc, rp, splat(rc[0].ex2), splat(rc[0].ey2), splat(hsx), splat(hsy), (float)Wt, (float)Ht, c);
-        float* o = out + (((size_t)v * N + i) * 2) * img + pair * 2;
-        o[0] = c.ix[0].x; o[1] = c.ix[0].y; o[img] = c.iy[0].x; o[img + 1] = c.iy[0].y;
-    }
-}
-
-__global__ void mpi_debug_division_kernel(const float* a, const float* b, float* out_fast, float* out_ieee, size_t n) {
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-        const float x = a[i], y = b[i];
-        out_fast[i] = in_safe_range(y) && (x == 0.0f || in_safe_range(x)) ? div_by_rcp(x, y, __frcp_rn(y)) : __fdiv_rn(x, y);
-        out_ieee[i] = __fdiv_rn(x, y);
-    }
-}
-
-__global__ void mpi_debug_cam_rays_kernel(const float* __restrict__ cam, float* __restrict__ ray_dir, int V, int H, int W) {
-    const size_t img = (size_t)H * W;
-    const size_t pix = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const int v = blockIdx.y;
-    if (pix >= img) return;
-    float rx, ry, rz;
-    cam_ray(cam + 16 * (size_t)v, (int)(pix % W), (int)(pix / W), H, W, rx, ry, rz);
-    float* o = ray_dir + (size_t)v * 3 * img + pix;
-    o[0] = rx; o[img] = ry; o[2 * img] = rz;
-}
-
-// ------------------------------------------------------------------------------------------
-// host side
-// ------------------------------------------------------------------------------------------
 }  // namespace gmpi
 
 using namespace gmpi;
@@ -662,13 +338,28 @@ struct Launch {
     void arg(void* a) { args[n_args++] = a; }
 };
 
-static int launch(Launch& l, cudaStream_t st) {
-    const void* kernel = render_kernel(l.key);
-    if (l.smem > 48 * 1024) GMPI_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)l.smem));
-    cudaLaunchConfig_t cfg = {l.grid, l.block, l.smem, st, nullptr, 0};
-    GMPI_CUDA_OK(cudaLaunchKernelExC(&cfg, kernel, l.args));
+// Every kernel launch of the library: `args` holds the address of each of the kernel's arguments, in order.  Reports this launch's
+// own error, not one the calling thread left pending, and lifts the kernel's dynamic shared-memory limit when smem exceeds 48 KB.
+static int launch_args(const void* kernel, dim3 grid, dim3 block, size_t smem, cudaStream_t st, void** args) {
+    if (smem > 48 * 1024) GMPI_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    cudaLaunchConfig_t cfg = {grid, block, smem, st, nullptr, 0};
+    GMPI_CUDA_OK(cudaLaunchKernelExC(&cfg, kernel, args));
     return GMPI_OK;
 }
+
+// A launch of every kernel but the render kernels (whose arguments vary by key: Launch).  Each argument is converted to its
+// parameter's type P, so the compiler checks the arguments against the kernel's parameter list.
+template <class... P, class... A>
+static int launch_kernel(void (*kernel)(P...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, A&&... a) {
+    static_assert(sizeof...(P) == sizeof...(A), "one argument per kernel parameter");
+    std::tuple<P...> params(std::forward<A>(a)...);
+    return std::apply([&](P&... x) {
+        void* arg_addrs[] = {&x...};
+        return launch_args(reinterpret_cast<const void*>(kernel), grid, block, smem, st, arg_addrs);
+    }, params);
+}
+
+static int launch(Launch& l, cudaStream_t st) { return launch_args(render_kernel(l.key), l.grid, l.block, l.smem, st, l.args); }
 
 // The persistent grid of the staged forward and the box backward: tiles of kTileW x tile_h pixels in every view, at most one CTA
 // per SM.  Also adds the arguments both kernels take after p: maps, tiles_x, tiles_y.
@@ -926,15 +617,12 @@ static int launch_bwd_deterministic(RenderParams p, void* scratch, size_t scratc
     if ((rc = bwd_launch(l, bwd_uses_box(p), true)) != 0) return rc;
     GMPI_CUDA_OK(cudaMemsetAsync(scratch, 0, L.bytes, st));
     dim3 bgrid((unsigned)(((size_t)p.H * p.W + 255) / 256), (unsigned)(p.V < 65535 ? p.V : 65535));
-    mpi_bwd_det_bounds_kernel<<<bgrid, 256, 0, st>>>(l.p, da.bounds);
-    GMPI_CUDA_OK(cudaGetLastError());
+    if ((rc = launch_kernel(mpi_bwd_det_bounds_kernel, bgrid, 256, 0, st, l.p, da.bounds)) != 0) return rc;
     if ((rc = launch(l, st)) != 0) return rc;
     int sms = 0;
     if ((rc = device_attr(cudaDevAttrMultiProcessorCount, &sms)) != 0) return rc;
-    mpi_bwd_det_finish_kernel<<<sms * 8, 256, 0, st>>>(da, fac ? p.g_rgb : p.g_rgba, p.g_alpha, p.g_bg_rgb, L.G, L.seg1, L.seg2,
-                                                      (size_t)p.Ht * p.Wt, fac, (p.options & GMPI_ZERO_GRAD) != 0);
-    GMPI_CUDA_OK(cudaGetLastError());
-    return GMPI_OK;
+    return launch_kernel(mpi_bwd_det_finish_kernel, sms * 8, 256, 0, st, da, fac ? p.g_rgb : p.g_rgba, p.g_alpha, p.g_bg_rgb, L.G, L.seg1,
+                         L.seg2, (size_t)p.Ht * p.Wt, fac, (p.options & GMPI_ZERO_GRAD) != 0);
 }
 
 static RenderParams params_from_desc(const gmpi_render_desc* d) {
@@ -990,28 +678,51 @@ static gmpi_render_desc classic_desc(const float* rgba, const int32_t* view2mpi,
     return d;
 }
 
-// The occupancy-map build of an MPI (mpi_kernel_keys.cuh) by element type and form, and whether it takes the range check's flags (the
-// expanded fp32 and fp16 builds set them from the same loads; uint8 MPIs are expanded, and every code is inside [0, 1]).
-struct OccBuild { const void* kernel; bool range_flags; };
-static OccBuild occ_build(ElemTraits<float>, bool fac) { return {fac ? (const void*)gmpi_occ_factored_f32 : (const void*)gmpi_occ_expanded_f32, !fac}; }
-static OccBuild occ_build(ElemTraits<__half>, bool fac) { return {fac ? (const void*)gmpi_occ_factored_f16 : (const void*)gmpi_occ_expanded_f16, !fac}; }
-static OccBuild occ_build(ElemTraits<uint8_t>, bool) { return {(const void*)gmpi_occ_expanded_u8, false}; }
+// The occupancy-map build of a checked call (mpi_kernel_keys.cuh), by element type and form.  The expanded fp32 and fp16 builds also
+// set the range check's flags from the same loads; uint8 MPIs are expanded, and every code is inside [0, 1].  The kernels read the
+// MPI as the bit patterns U of its elements.
+template <class U> static const U* elem_bits(const float* mpi) { return reinterpret_cast<const U*>(mpi); }
+
+static int occ_build(const RenderParams& p, uint32_t* map, int words, int rows, cudaStream_t st) {
+    const int M = p.M, N = p.N, Ht = p.Ht, Wt = p.Wt;
+    const dim3 block(32 * kOccB);
+    if (factored(p)) {
+        const dim3 grid(words, rows, M < 65535 ? M : 65535);
+        if (p.options & GMPI_MPI_F16)
+            return launch_kernel(gmpi_occ_factored_f16, grid, block, 0, st, elem_bits<uint16_t>(p.rgb), elem_bits<uint16_t>(p.bg_rgb),
+                                 elem_bits<uint16_t>(p.alpha), map, M, N, Ht, Wt, words, rows);
+        return launch_kernel(gmpi_occ_factored_f32, grid, block, 0, st, elem_bits<uint32_t>(p.rgb), elem_bits<uint32_t>(p.bg_rgb),
+                             elem_bits<uint32_t>(p.alpha), map, M, N, Ht, Wt, words, rows);
+    }
+    const long long P = (long long)M * N;
+    if (P > 0x7fffffffLL) return fail(GMPI_ERR_UNSUPPORTED, "%lld planes exceed the occupancy build (2^31)", P);
+    const int planes = (int)P;
+    const dim3 grid(words, rows, planes < 65535 ? planes : 65535);
+    if (p.options & GMPI_MPI_U8)
+        return launch_kernel(gmpi_occ_expanded_u8, grid, block, 0, st, elem_bits<uint8_t>(p.rgba), map, planes, Ht, Wt, words, rows);
+    if (p.options & GMPI_MPI_F16)
+        return launch_kernel(gmpi_occ_expanded_f16, grid, block, 0, st, elem_bits<uint16_t>(p.rgba), map, p.flags, planes, Ht, Wt, words, rows);
+    return launch_kernel(gmpi_occ_expanded_f32, grid, block, 0, st, elem_bits<uint32_t>(p.rgba), map, p.flags, planes, Ht, Wt, words, rows);
+}
 
 // The range check of an fp32 or (f16) fp16 rgba: 16-byte loads when every slab is a whole number of them on an aligned base.
 static int check_range(const void* rgba, bool f16, int M, int N, int Ht, int Wt, uint32_t* flags, cudaStream_t st) {
     if (!rgba || !flags) return fail(GMPI_ERR_INVALID_ARGUMENT, "null pointer");
     if (M < 1 || N < 1 || Ht < 1 || Wt < 1) return fail(GMPI_ERR_INVALID_ARGUMENT, "bad sizes");
-    const size_t slab = (size_t)Ht * Wt, n_slabs = (size_t)M * N * 4, per_load = f16 ? 8 : 4;
+    const size_t slab = (size_t)Ht * Wt, n_slabs = (size_t)M * N * 4;
     int sms = 132;
     if (int rc = device_attr(cudaDevAttrMultiProcessorCount, &sms)) return rc;
     const int grid = sms * 8;
-    const bool vec = slab % per_load == 0 && aligned16(rgba);
-    if (f16 && vec) mpi_check_range_f16_kernel<<<grid, 256, 0, st>>>(static_cast<const uint4*>(rgba), n_slabs, slab / 8, flags);
-    else if (f16) mpi_check_range_f16_scalar_kernel<<<grid, 256, 0, st>>>(static_cast<const unsigned short*>(rgba), n_slabs, slab, flags);
-    else if (vec) mpi_check_range_kernel<<<grid, 256, 0, st>>>(static_cast<const float4*>(rgba), n_slabs, slab / 4, flags);
-    else mpi_check_range_scalar_kernel<<<grid, 256, 0, st>>>(static_cast<const float*>(rgba), n_slabs, slab, flags);
-    GMPI_CUDA_OK(cudaGetLastError());
-    return GMPI_OK;
+    const auto run = [&](auto e) {
+        using T = decltype(e);
+        using E = typename T::Elem;
+        using Bits = typename T::Bits;
+        if (slab % T::kAlign == 0 && aligned16(rgba))
+            return launch_kernel(mpi_check_range_kernel<E, uint4>, grid, 256, 0, st, static_cast<const uint4*>(rgba), n_slabs,
+                                 slab / T::kAlign, flags);
+        return launch_kernel(mpi_check_range_kernel<E, Bits>, grid, 256, 0, st, static_cast<const Bits*>(rgba), n_slabs, slab, flags);
+    };
+    return f16 ? run(ElemTraits<__half>{}) : run(ElemTraits<float>{});
 }
 
 extern "C" {
@@ -1180,29 +891,7 @@ int gmpi_mpi_build_occupancy(const gmpi_render_desc* d, void* occ, size_t bytes)
     if (rc) return rc;
     const int words = occ_words(p.Wt), rows = occ_rows(p.Ht);
     if (rows > 65535) return fail(GMPI_ERR_UNSUPPORTED, "Ht=%d exceeds the occupancy build's grid (%d texel rows)", p.Ht, 65535 * kOccB);
-    const OccBuild build = with_mpi_elem(p.options, [&](auto e) { return occ_build(e, factored(p)); });
-    const int M = p.M, N = p.N, Ht = p.Ht, Wt = p.Wt;
-    cudaLaunchConfig_t cfg = {};
-    cfg.blockDim = dim3(32 * kOccB);
-    cfg.stream = (cudaStream_t)d->stream;
-    uint32_t* map = static_cast<uint32_t*>(occ);
-    if (factored(p)) {
-        cfg.gridDim = dim3(words, rows, M < 65535 ? M : 65535);
-        const void *rgb = p.rgb, *bg = p.bg_rgb, *alpha = p.alpha;
-        void* args[] = {&rgb, &bg, &alpha, &map, (void*)&M, (void*)&N, (void*)&Ht, (void*)&Wt, (void*)&words, (void*)&rows};
-        GMPI_CUDA_OK(cudaLaunchKernelExC(&cfg, build.kernel, args));
-    } else {
-        const long long P = (long long)M * N;
-        if (P > 0x7fffffffLL) return fail(GMPI_ERR_UNSUPPORTED, "%lld planes exceed the occupancy build (2^31)", P);
-        const int planes = (int)P;
-        cfg.gridDim = dim3(words, rows, planes < 65535 ? planes : 65535);
-        const void* rgba = p.rgba;
-        uint32_t* flags = p.flags;
-        void* args[] = {&rgba, &map, &flags, (void*)&planes, (void*)&Ht, (void*)&Wt, (void*)&words, (void*)&rows};
-        void* args_no_flags[] = {&rgba, &map, (void*)&planes, (void*)&Ht, (void*)&Wt, (void*)&words, (void*)&rows};
-        GMPI_CUDA_OK(cudaLaunchKernelExC(&cfg, build.kernel, build.range_flags ? args : args_no_flags));
-    }
-    return GMPI_OK;
+    return occ_build(p, static_cast<uint32_t*>(occ), words, rows, (cudaStream_t)d->stream);
 }
 
 int gmpi_mpi_render_fwd_skip_ex(const gmpi_render_desc* d, const void* occ, size_t bytes) {
@@ -1232,10 +921,7 @@ int gmpi_debug_u8_codes_host(float* out) {
 
 int gmpi_debug_u8_codes(float* out, void* stream) {
     if (!out) return fail(GMPI_ERR_INVALID_ARGUMENT, "null pointer");
-    cudaLaunchConfig_t cfg = {dim3(1), dim3(256), 0, (cudaStream_t)stream, nullptr, 0};
-    void* args[] = {&out};
-    GMPI_CUDA_OK(cudaLaunchKernelExC(&cfg, (const void*)gmpi_u8_codes, args));
-    return GMPI_OK;
+    return launch_kernel(gmpi_u8_codes, 1, 256, 0, (cudaStream_t)stream, out);
 }
 
 int gmpi_mpi_check_range(const float* rgba, int M, int N, int Ht, int Wt, uint32_t* flags, void* stream) {
@@ -1254,9 +940,7 @@ int gmpi_debug_plane_coords(const int32_t* view2mpi, const float* dhw, const flo
     const size_t img = (size_t)H * W;
     dim3 grid((unsigned)((img + 255) / 256), V);
     const auto kernel = (options & GMPI_ALIGN_CORNERS) ? mpi_debug_coords_kernel<true> : mpi_debug_coords_kernel<false>;
-    kernel<<<grid, 256, 0, st>>>(view2mpi, dhw, ray_dir, eye, out, V, N, Ht, Wt, H, W);
-    GMPI_CUDA_OK(cudaGetLastError());
-    return GMPI_OK;
+    return launch_kernel(kernel, grid, 256, 0, st, view2mpi, dhw, ray_dir, eye, out, V, N, Ht, Wt, H, W);
 }
 
 int gmpi_debug_plane_coords_packed(const int32_t* view2mpi, const float* dhw, const float* ray_dir, const float* eye,
@@ -1267,24 +951,18 @@ int gmpi_debug_plane_coords_packed(const int32_t* view2mpi, const float* dhw, co
     const size_t pairs = (size_t)H * W / 2;
     dim3 grid((unsigned)((pairs + 255) / 256), V);
     const auto kernel = (options & GMPI_ALIGN_CORNERS) ? mpi_debug_coords_packed_kernel<true> : mpi_debug_coords_packed_kernel<false>;
-    kernel<<<grid, 256, 0, st>>>(view2mpi, dhw, ray_dir, eye, out, V, N, Ht, Wt, H, W);
-    GMPI_CUDA_OK(cudaGetLastError());
-    return GMPI_OK;
+    return launch_kernel(kernel, grid, 256, 0, st, view2mpi, dhw, ray_dir, eye, out, V, N, Ht, Wt, H, W);
 }
 
 int gmpi_debug_division(const float* a, const float* b, float* out_fast, float* out_ieee, size_t n, void* stream) {
     if (!a || !b || !out_fast || !out_ieee) return fail(GMPI_ERR_INVALID_ARGUMENT, "null pointer");
-    mpi_debug_division_kernel<<<1184, 256, 0, (cudaStream_t)stream>>>(a, b, out_fast, out_ieee, n);
-    GMPI_CUDA_OK(cudaGetLastError());
-    return GMPI_OK;
+    return launch_kernel(mpi_debug_division_kernel, 1184, 256, 0, (cudaStream_t)stream, a, b, out_fast, out_ieee, n);
 }
 
 int gmpi_debug_cam_rays(const float* cam, float* ray_dir, int V, int H, int W, void* stream) {
     if (!cam || !ray_dir || V < 1 || H < 1 || W < 1) return fail(GMPI_ERR_INVALID_ARGUMENT, "bad argument");
     dim3 grid((unsigned)(((size_t)H * W + 255) / 256), V);
-    mpi_debug_cam_rays_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(cam, ray_dir, V, H, W);
-    GMPI_CUDA_OK(cudaGetLastError());
-    return GMPI_OK;
+    return launch_kernel(mpi_debug_cam_rays_kernel, grid, 256, 0, (cudaStream_t)stream, cam, ray_dir, V, H, W);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1306,10 +984,8 @@ int gmpi_mpi_alpha_depth_fwd(const float* alpha, long long mpi_stride, long long
     const long long tex4 = (long long)Ht * Wt / 4;
     AlphaView a{alpha, mpi_stride, plane_stride};
     dim3 grid((unsigned)((tex4 + 255) / 256), M);
-    if (transmittance) mpi_alpha_depth_fwd_kernel<true><<<grid, 256, 0, (cudaStream_t)stream>>>(a, plane_d, depth, transmittance, N, tex4);
-    else mpi_alpha_depth_fwd_kernel<false><<<grid, 256, 0, (cudaStream_t)stream>>>(a, plane_d, depth, nullptr, N, tex4);
-    GMPI_CUDA_OK(cudaGetLastError());
-    return GMPI_OK;
+    const auto kernel = transmittance ? mpi_alpha_depth_fwd_kernel<true> : mpi_alpha_depth_fwd_kernel<false>;
+    return launch_kernel(kernel, grid, 256, 0, (cudaStream_t)stream, a, plane_d, depth, transmittance, N, tex4);
 }
 
 int gmpi_mpi_alpha_depth_bwd(const float* alpha, long long mpi_stride, long long plane_stride, const float* plane_d,
@@ -1323,10 +999,8 @@ int gmpi_mpi_alpha_depth_bwd(const float* alpha, long long mpi_stride, long long
     const long long tex4 = (long long)Ht * Wt / 4;
     AlphaView a{alpha, mpi_stride, plane_stride};
     dim3 grid((unsigned)((tex4 + 255) / 256), M);
-    mpi_alpha_depth_bwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(a, plane_d, transmittance, g_depth, g_alpha, g_mpi_stride,
-                                                                        g_plane_stride, N, tex4);
-    GMPI_CUDA_OK(cudaGetLastError());
-    return GMPI_OK;
+    return launch_kernel(mpi_alpha_depth_bwd_kernel, grid, 256, 0, (cudaStream_t)stream, a, plane_d, transmittance, g_depth, g_alpha,
+                         g_mpi_stride, g_plane_stride, N, tex4);
 }
 
 int gmpi_mpi_apply_shading_fwd(const float* rgba, const float* shade, float* out, int M, int N, int Ht, int Wt, void* stream) {
@@ -1336,9 +1010,7 @@ int gmpi_mpi_apply_shading_fwd(const float* rgba, const float* shade, float* out
         return fail(GMPI_ERR_UNSUPPORTED, "tensors must be 16-byte aligned with Ht*Wt %% 4 == 0 (float4 streaming)");
     const long long tex4 = (long long)Ht * Wt / 4;
     dim3 grid((unsigned)((tex4 + 255) / 256), N, M);
-    mpi_apply_shading_fwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(rgba, shade, out, N, tex4);
-    GMPI_CUDA_OK(cudaGetLastError());
-    return GMPI_OK;
+    return launch_kernel(mpi_apply_shading_fwd_kernel, grid, 256, 0, (cudaStream_t)stream, rgba, shade, out, N, tex4);
 }
 
 int gmpi_mpi_apply_shading_bwd(const float* rgba, const float* shade, const float* g_out, float* g_rgba, float* g_shade, int M, int N,
@@ -1350,9 +1022,7 @@ int gmpi_mpi_apply_shading_bwd(const float* rgba, const float* shade, const floa
         return fail(GMPI_ERR_UNSUPPORTED, "tensors must be 16-byte aligned with Ht*Wt %% 4 == 0 (float4 streaming)");
     const long long tex4 = (long long)Ht * Wt / 4;
     dim3 grid((unsigned)((tex4 + 255) / 256), M);
-    mpi_apply_shading_bwd_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(rgba, shade, g_out, g_rgba, g_shade, N, tex4);
-    GMPI_CUDA_OK(cudaGetLastError());
-    return GMPI_OK;
+    return launch_kernel(mpi_apply_shading_bwd_kernel, grid, 256, 0, (cudaStream_t)stream, rgba, shade, g_out, g_rgba, g_shade, N, tex4);
 }
 
 // ------------------------------------------------------------------------------------------

@@ -110,4 +110,4 @@ def test_sass_of_the_fp16_staged_kernel_keys():
         assert " STL" not in b and " LDL" not in b, n
         assert (k.regs, k.stack, k.local) == (128, 0, 0), (n, k.regs, k.stack, k.local)
     assert len(render_kernels(funcs, "mpi_fwd_direct_kernel", has=KEY_F16)) == 4
-    assert any(k.template == "mpi_check_range_f16_kernel" for k in funcs.values())
+    assert "_ZN4gmpi22mpi_check_range_kernelI6__half5uint4EEvPKT0_mmPj" in funcs     # mpi_check_range_kernel<__half, uint4>
