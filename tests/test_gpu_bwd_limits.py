@@ -5,21 +5,17 @@ from the tile's largest upstream gradient (csrc/mpi_bwd_box.cuh).  These tests p
 pixels per texel (magnification), upstream gradients near the ends of the fp32 range, inf/NaN upstream gradients -- and
 compare with the oracle (fp32 autograd formula), through the expanded and the factored backward.  The kernel must then take
 its generic body (fp32 global atomics) instead of wrapping or rounding to garbage."""
-import os
-
 import numpy as np
 import pytest
 import torch
 
-import mpi_oracle
 import ml_gmpi_b200 as g
 from ml_gmpi_b200 import synth
 from conftest import rel_err
-from testlib import dev, expanded_grad, factored_grads, forced_kernel, kernel_fixture, one_tile_per_mpi_case
+from testlib import (EXPECT, FACTORED_RGB_EXPECT, check_factored, dev, expanded_grad, factored_grads, factored_refs, forced_kernel,
+                     kernel_fixture, oracle_backward, one_tile_per_mpi_case, upstream)
 
 pytestmark = pytest.mark.gpu
-EXPECT = 2e-5
-_NT = max(1, min(64, (os.cpu_count() or 8)))
 bwd_variant = kernel_fixture("staged", "direct")
 
 
@@ -28,28 +24,6 @@ def staged():
     """TMA-staged forward and box backward whatever the number of tiles."""
     with forced_kernel("staged"):
         yield
-
-
-n = lambda t: t.detach().cpu().numpy()
-
-
-def _oracle(rgba, case, gc, gd, ray=None):
-    return mpi_oracle.backward(n(rgba), n(case.view2mpi), n(case.dhw), n(case.ray_dir if ray is None else ray), n(case.eye),
-                               n(case.z_dir), n(gc), None if gd is None else n(gd), nthreads=_NT)
-
-
-def _factored_refs(ref):
-    """The oracle's expanded gradient -> (d rgb, d alpha, d bg) of a factored MPI with a background plane: d rgb is the sum over
-    the planes that share the colour image."""
-    return ref[:, :-1, :3].astype(np.float64).sum(1), ref[:, :, 3:4], ref[:, -1, :3]
-
-
-def _check_factored(ours, ref, tol=EXPECT):
-    """d rgb sums N-1 planes' rounding errors (fixed point here, fp32 in the oracle): twice the per-plane bar, as in
-    test_gpu_features.test_factored_backward_equals_expanded_autograd."""
-    r_rgb, r_alpha, r_bg = _factored_refs(ref)
-    e = (rel_err(ours[0], r_rgb), rel_err(ours[1], r_alpha), rel_err(ours[2], r_bg))
-    assert e[0] <= 2 * tol and e[1] <= tol and e[2] <= tol, e
 
 
 # ------------------------------------------------------------------------------------------------------------------------
@@ -87,12 +61,12 @@ def test_magnified_texture_gradient_box_does_not_wrap(tex, pose, loss, staged):
         gd = None
     else:
         gc, gd = torch.ones((1, 3, img, img), device=d), torch.ones((1, 1, img, img), device=d)
-    ref = _oracle(rgba, case, gc, gd)
+    ref = oracle_backward(case, gc, gd, rgba=rgba)
     assert float(np.abs(ref).max()) > 0
     e = rel_err(expanded_grad(rgba, case, gc, gd), ref)
     assert e <= EXPECT, e
     rgba_f = g.expand_factored(rgb, alpha, bg)
-    _check_factored(factored_grads(rgb, alpha, bg, case, gc, gd), _oracle(rgba_f, case, gc, gd))
+    check_factored(factored_grads(rgb, alpha, bg, case, gc, gd), oracle_backward(case, gc, gd, rgba=rgba_f))
 
 
 # ------------------------------------------------------------------------------------------------------------------------
@@ -102,14 +76,12 @@ def test_magnified_texture_gradient_box_does_not_wrap(tex, pose, loss, staged):
 def test_power_of_two_scaled_upstream_gradient_scales_the_result_bitwise(k, staged):
     d = dev()
     case = one_tile_per_mpi_case(d)
-    gen = torch.Generator().manual_seed(4)
-    gc = torch.randn((2, 3, 24, 64), generator=gen).to(d)
-    gd = torch.randn((2, 1, 24, 64), generator=gen).to(d)
+    gc, gd = upstream(2, 24, 64, 4, device=d)
     s = 2.0 ** k
     base = expanded_grad(case.rgba, case, gc, gd)
     scaled = expanded_grad(case.rgba, case, gc * s, gd * s)
     assert np.array_equal(scaled, base * np.float32(s))
-    assert rel_err(base, _oracle(case.rgba, case, gc, gd)) <= EXPECT
+    assert rel_err(base, oracle_backward(case, gc, gd)) <= EXPECT
     # factored: per-plane alpha and the background colour get one flush per texel; the shared colour image sums the planes'
     # flushes with fp32 atomics in flusher order, which is exact only up to that order
     gen = torch.Generator(device=d).manual_seed(6)
@@ -122,7 +94,7 @@ def test_power_of_two_scaled_upstream_gradient_scales_the_result_bitwise(k, stag
     fs = factored_grads(rgb, alpha, bg, case, gc * s, gd * s)
     assert np.array_equal(fs[1], fb[1] * np.float32(s)) and np.array_equal(fs[2], fb[2] * np.float32(s))
     assert rel_err(fs[0], fb[0] * np.float32(s)) <= 1e-6
-    _check_factored(fb, _oracle(g.expand_factored(rgb, alpha, bg), case, gc, gd))
+    check_factored(fb, oracle_backward(case, gc, gd, rgba=g.expand_factored(rgb, alpha, bg)))
 
 
 # ------------------------------------------------------------------------------------------------------------------------
@@ -134,17 +106,16 @@ def test_extreme_upstream_gradient_magnitudes(scale, staged):
     scale constants would no longer be normal floats.  The oracle is fp32 too and handles all three."""
     d = dev()
     case = synth.make_case(n_planes=6, tex=128, img=128, n_mpi=2, seed=17, device=d, last_alpha_one=True)
-    gen = torch.Generator().manual_seed(8)
-    gc = (torch.randn((2, 3, 128, 128), generator=gen) * scale).to(d)
-    gd = (torch.randn((2, 1, 128, 128), generator=gen) * scale).to(d)
-    ref = _oracle(case.rgba, case, gc, gd)
+    gc, gd = ((t * scale).to(d) for t in upstream(2, 128, 128, 8))
+    ref = oracle_backward(case, gc, gd)
     assert np.isfinite(ref).all() and float(np.abs(ref).max()) > 0
     e = rel_err(expanded_grad(case.rgba, case, gc, gd), ref)
     assert e <= EXPECT, e
     gen = torch.Generator(device=d).manual_seed(9)
     rgb, alpha, bg = (torch.rand(sh, generator=gen, device=d) for sh in ((2, 3, 128, 128), (2, 6, 1, 128, 128), (2, 3, 128, 128)))
     alpha[:, -1] = 1.0
-    _check_factored(factored_grads(rgb, alpha, bg, case, gc, gd), _oracle(g.expand_factored(rgb, alpha, bg), case, gc, gd))
+    check_factored(factored_grads(rgb, alpha, bg, case, gc, gd),
+                   oracle_backward(case, gc, gd, rgba=g.expand_factored(rgb, alpha, bg)))
 
 
 # ------------------------------------------------------------------------------------------------------------------------
@@ -170,17 +141,15 @@ def _check_poisoned(ours, ref, variant, tol=EXPECT):
 def test_nan_and_inf_upstream_gradients_propagate_like_autograd(bwd_variant):
     d = dev()
     case = synth.make_case(n_planes=6, tex=128, img=128, n_mpi=1, seed=23, device=d, last_alpha_one=True)
-    gen = torch.Generator().manual_seed(10)
-    gc = torch.randn((1, 3, 128, 128), generator=gen).to(d)
-    gd = torch.randn((1, 1, 128, 128), generator=gen).to(d)
+    gc, gd = upstream(1, 128, 128, 10, device=d)
     gc[0, 0, 30, 40] = float("nan")          # backward tile (px0, py0) = (0, 24)
     gd[0, 0, 100, 100] = float("inf")        # backward tile (64, 96)
-    ref = _oracle(case.rgba, case, gc, gd)
+    ref = oracle_backward(case, gc, gd)
     _check_poisoned(expanded_grad(case.rgba, case, gc, gd), ref, bwd_variant)
     gen = torch.Generator(device=d).manual_seed(11)
     rgb, alpha, bg = (torch.rand(sh, generator=gen, device=d) for sh in ((1, 3, 128, 128), (1, 6, 1, 128, 128), (1, 3, 128, 128)))
     alpha[:, -1] = 1.0
     ours = factored_grads(rgb, alpha, bg, case, gc, gd)
-    refs = _factored_refs(_oracle(g.expand_factored(rgb, alpha, bg), case, gc, gd))
-    for o, r, tol in zip(ours, refs, (2 * EXPECT, EXPECT, EXPECT)):      # d rgb: see _check_factored
+    refs = factored_refs(oracle_backward(case, gc, gd, rgba=g.expand_factored(rgb, alpha, bg)))
+    for o, r, tol in zip(ours, refs, (FACTORED_RGB_EXPECT, EXPECT, EXPECT)):
         _check_poisoned(o, r, bwd_variant, tol)

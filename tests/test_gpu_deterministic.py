@@ -3,22 +3,18 @@ parity bar of the oracle and of the default backward, on the staged box kernel a
 kernel takes its generic body, with inf/NaN upstream gradients, accumulating without GMPI_ZERO_GRAD, and through torch's
 deterministic switch."""
 import ctypes
-import os
 
 import numpy as np
 import pytest
 import torch
 
-import mpi_oracle
 import ml_gmpi_b200 as g
 from ml_gmpi_b200 import _lib, synth
 from conftest import rel_err
-from testlib import assert_bitwise, dev, each_alpha, kernel_fixture
+from testlib import (EXPECT, FACTORED_RGB_EXPECT, assert_bitwise, dev, each_alpha, factored_refs, kernel_fixture, oracle_backward,
+                     to_np, upstream)
 
 pytestmark = pytest.mark.gpu
-EXPECT = 2e-5
-_NT = max(1, min(64, (os.cpu_count() or 8)))
-n = lambda t: t.detach().cpu().numpy()
 
 
 variant = kernel_fixture("staged", "direct")     # staged forward + box backward (whatever the number of tiles), or the direct kernels
@@ -42,16 +38,7 @@ def _grads(case, gc, gd, *, deterministic, factored=None, align_corners=True, vi
         color, depth = g.render_views_factored(leaves[0], leaves[1], case.dhw, v2m, ray, eye, z, bg_rgb=leaves[2], **kw)
     loss = (color * gc).sum() + ((depth * gd).sum() if gd is not None else 0.0)
     loss.backward()
-    return [n(t.grad) for t in leaves]
-
-
-def _oracle(rgba, case, gc, gd, align_corners=True, ray=None):
-    return mpi_oracle.backward(n(rgba), n(case.view2mpi), n(case.dhw), n(case.ray_dir if ray is None else ray), n(case.eye),
-                               n(case.z_dir), n(gc), None if gd is None else n(gd), align_corners=align_corners, nthreads=_NT)
-
-
-def _factored_refs(ref):
-    return [ref[:, :-1, :3].astype(np.float64).sum(1), ref[:, :, 3:4], ref[:, -1, :3]]
+    return [to_np(t.grad) for t in leaves]
 
 
 def _factored_mpi(M, N, tex, seed, d):
@@ -66,18 +53,11 @@ def _check_accuracy(ours, default, ref, factored):
     """Within the oracle's bar (2e-5; the factored colour sums N-1 planes' roundings: twice that), and within the same bar of the
     default backward: the deterministic sums add at most 2^(E-k-1) per contribution and one fp32 rounding to the box kernel's
     per-tile fixed point, which the default backward has too (DESIGN.md section 4.3)."""
-    refs = _factored_refs(ref) if factored else [ref]
-    tols = (2 * EXPECT, EXPECT, EXPECT) if factored else (EXPECT,)
+    refs = factored_refs(ref) if factored else [ref]
+    tols = (FACTORED_RGB_EXPECT, EXPECT, EXPECT) if factored else (EXPECT,)
     for o, d_, r, tol in zip(ours, default, refs, tols):
         assert rel_err(o, r) <= tol, rel_err(o, r)
         assert rel_err(o, d_) <= tol, rel_err(o, d_)
-
-
-def _upstream(V, H, W, seed, d, depth=True):
-    gen = torch.Generator().manual_seed(seed)
-    gc = torch.randn((V, 3, H, W), generator=gen).to(d)
-    gd = torch.randn((V, 1, H, W), generator=gen).to(d) if depth else None
-    return gc, gd
 
 
 # ------------------------------------------------------------------------------------------------------------------------
@@ -90,14 +70,15 @@ def test_repeatable_and_accurate(form, depth, align_corners, variant):
     d = dev()
     M, vpm, N, tex, img = 2, 2, 12, 128, 256
     case = synth.make_case(n_planes=N, tex=tex, img=img, n_mpi=M, views_per_mpi=vpm, seed=31, device=d, last_alpha_one=True)
-    gc, gd = _upstream(M * vpm, img, img, 5, d, depth)
+    gc, gd = upstream(M * vpm, img, img, 5, depth, d)
     fac = _factored_mpi(M, N, tex, 7, d) if form == "factored" else None
     kw = dict(factored=fac, align_corners=align_corners, view_group=vpm)
     a = _grads(case, gc, gd, deterministic=True, **kw)
     b = _grads(case, gc, gd, deterministic=True, **kw)
     assert_bitwise(a, b)
     rgba = case.rgba if fac is None else g.expand_factored(*fac)
-    _check_accuracy(a, _grads(case, gc, gd, deterministic=False, **kw), _oracle(rgba, case, gc, gd, align_corners), fac is not None)
+    ref = oracle_backward(case, gc, gd, rgba=rgba, align_corners=align_corners)
+    _check_accuracy(a, _grads(case, gc, gd, deterministic=False, **kw), ref, fac is not None)
 
 
 @pytest.mark.parametrize("form", ["expanded", "factored"])
@@ -106,7 +87,7 @@ def test_view_order_does_not_change_a_bit(form, variant):
     d = dev()
     M, vpm, N, tex, img = 2, 3, 8, 128, 192
     case = synth.make_case(n_planes=N, tex=tex, img=img, n_mpi=M, views_per_mpi=vpm, seed=41, device=d, last_alpha_one=True)
-    gc, gd = _upstream(M * vpm, img, img, 6, d)
+    gc, gd = upstream(M * vpm, img, img, 6, device=d)
     fac = _factored_mpi(M, N, tex, 8, d) if form == "factored" else None
     base = _grads(case, gc, gd, deterministic=True, factored=fac)
     for order in ([2, 0, 1, 5, 3, 4], [4, 5, 3, 1, 2, 0]):
@@ -120,13 +101,12 @@ def test_full_size_training_shape_is_repeatable(variant, alpha):
     plane's gradient is far from 0, so repeatability is not met trivially on the back planes."""
     d = dev()
     case = synth.make_case(n_planes=96, tex=1024, img=1024, n_mpi=4, seed=3, device=d, last_alpha_one=True, alpha=alpha)
-    gc, gd = _upstream(4, 1024, 1024, 9, d)
+    gc, gd = upstream(4, 1024, 1024, 9, device=d)
     a = _grads(case, gc, gd, deterministic=True)
     assert_bitwise(a, _grads(case, gc, gd, deterministic=True))
     e = rel_err(a[0], _grads(case, gc, gd, deterministic=False)[0])
     assert e <= EXPECT, e
-    ref = mpi_oracle.backward(n(case.rgba), n(case.view2mpi), n(case.dhw), n(case.ray_dir), n(case.eye), n(case.z_dir), n(gc), n(gd),
-                              nthreads=_NT)
+    ref = oracle_backward(case, gc, gd)
     errs = [rel_err(a[0][m], ref[m]) for m in range(4)]
     assert max(errs) <= EXPECT, errs
 
@@ -135,7 +115,7 @@ def test_fifteen_views_of_one_mpi_are_repeatable(variant):
     """The C4 shape: 15 views of one 96 x 512^2 MPI, all adding into the same gradient."""
     d = dev()
     case = synth.make_case(n_planes=96, tex=512, img=512, n_mpi=1, views_per_mpi=15, seed=4, device=d, last_alpha_one=True)
-    gc, gd = _upstream(15, 512, 512, 10, d)
+    gc, gd = upstream(15, 512, 512, 10, device=d)
     a = _grads(case, gc, gd, deterministic=True, view_group=15)
     assert_bitwise(a, _grads(case, gc, gd, deterministic=True, view_group=15))
     e = rel_err(a[0], _grads(case, gc, gd, deterministic=False, view_group=15)[0])
@@ -153,29 +133,29 @@ def test_magnified_texture(tex, variant):
     gc, gd = torch.ones((1, 3, img, img), device=d), torch.ones((1, 1, img, img), device=d)
     a = _grads(case, gc, gd, deterministic=True)
     assert_bitwise(a, _grads(case, gc, gd, deterministic=True))
-    _check_accuracy(a, _grads(case, gc, gd, deterministic=False), _oracle(case.rgba, case, gc, gd), False)
+    _check_accuracy(a, _grads(case, gc, gd, deterministic=False), oracle_backward(case, gc, gd), False)
     fac = _factored_mpi(1, N, tex, 12, d)
     a = _grads(case, gc, gd, deterministic=True, factored=fac)
     assert_bitwise(a, _grads(case, gc, gd, deterministic=True, factored=fac))
-    _check_accuracy(a, _grads(case, gc, gd, deterministic=False, factored=fac), _oracle(g.expand_factored(*fac), case, gc, gd), True)
+    ref = oracle_backward(case, gc, gd, rgba=g.expand_factored(*fac))
+    _check_accuracy(a, _grads(case, gc, gd, deterministic=False, factored=fac), ref, True)
 
 
 @pytest.mark.parametrize("scale", [1e-32, 1e-30, 1e27])
 def test_extreme_upstream_gradient_magnitudes(scale, variant):
     d = dev()
     case = synth.make_case(n_planes=6, tex=128, img=128, n_mpi=2, seed=17, device=d, last_alpha_one=True)
-    gen = torch.Generator().manual_seed(8)
-    gc = (torch.randn((2, 3, 128, 128), generator=gen) * scale).to(d)
-    gd = (torch.randn((2, 1, 128, 128), generator=gen) * scale).to(d)
+    gc, gd = ((t * scale).to(d) for t in upstream(2, 128, 128, 8))
     a = _grads(case, gc, gd, deterministic=True)
     assert_bitwise(a, _grads(case, gc, gd, deterministic=True))
-    ref = _oracle(case.rgba, case, gc, gd)
+    ref = oracle_backward(case, gc, gd)
     assert np.isfinite(ref).all() and float(np.abs(ref).max()) > 0
     _check_accuracy(a, _grads(case, gc, gd, deterministic=False), ref, False)
     fac = _factored_mpi(2, 6, 128, 9, d)
     a = _grads(case, gc, gd, deterministic=True, factored=fac)
     assert_bitwise(a, _grads(case, gc, gd, deterministic=True, factored=fac))
-    _check_accuracy(a, _grads(case, gc, gd, deterministic=False, factored=fac), _oracle(g.expand_factored(*fac), case, gc, gd), True)
+    ref = oracle_backward(case, gc, gd, rgba=g.expand_factored(*fac))
+    _check_accuracy(a, _grads(case, gc, gd, deterministic=False, factored=fac), ref, True)
 
 
 # ------------------------------------------------------------------------------------------------------------------------
@@ -186,7 +166,7 @@ def test_non_finite_upstream_gradients(variant):
     is finite, repeatable, and within the bar of the default backward."""
     d = dev()
     case = synth.make_case(n_planes=6, tex=128, img=128, n_mpi=1, seed=23, device=d, last_alpha_one=True)
-    gc, gd = _upstream(1, 128, 128, 10, d)
+    gc, gd = upstream(1, 128, 128, 10, device=d)
     gc[0, 0, 30, 40] = float("nan")
     gd[0, 0, 100, 100] = float("inf")
     gc[0, 1, 70, 20] = float("-inf")
@@ -212,7 +192,7 @@ def test_accumulates_without_zero_grad(variant):
     lib = _lib.load()
     case = synth.make_case(n_planes=8, tex=128, img=256, n_mpi=2, views_per_mpi=2, seed=51, device=d, last_alpha_one=True)
     M, N, V, H, W = 2, 8, 4, 256, 256
-    gc, gd = _upstream(V, H, W, 12, d)
+    gc, gd = upstream(V, H, W, 12, device=d)
     color, depth = torch.empty((V, 3, H, W), device=d), torch.empty((V, 1, H, W), device=d)
     trans = torch.empty((V, N, H, W), device=d)
     flags = torch.zeros(1, dtype=torch.int32, device=d)
@@ -228,11 +208,11 @@ def test_accumulates_without_zero_grad(variant):
         _lib.check(lib.gmpi_mpi_render_bwd_deterministic_ex(ctypes.byref(desc), scratch.data_ptr(), nbytes))
         return g_rgba
 
-    fresh = n(bwd(torch.full_like(case.rgba, float("nan")), _lib.OPT_ALIGN_CORNERS | _lib.OPT_ZERO_GRAD))
+    fresh = to_np(bwd(torch.full_like(case.rgba, float("nan")), _lib.OPT_ALIGN_CORNERS | _lib.OPT_ZERO_GRAD))
     prefill = torch.randn(case.rgba.shape, generator=torch.Generator().manual_seed(13)).to(d)
-    added = n(bwd(prefill.clone(), _lib.OPT_ALIGN_CORNERS))
+    added = to_np(bwd(prefill.clone(), _lib.OPT_ALIGN_CORNERS))
     assert np.isfinite(fresh).all()
-    assert np.array_equal(added, n(prefill) + fresh)
+    assert np.array_equal(added, to_np(prefill) + fresh)
 
 
 # ------------------------------------------------------------------------------------------------------------------------
@@ -240,12 +220,12 @@ def test_accumulates_without_zero_grad(variant):
 # ------------------------------------------------------------------------------------------------------------------------
 def _train_step(case, gc, gd, mpi):
     x = case.rgba.clone().requires_grad_(True)
-    v2m = n(case.view2mpi)
+    v2m = to_np(case.view2mpi)
     idx = [np.nonzero(v2m == m)[0] for m in range(case.rgba.shape[0])]
     color, depth = mpi(batch_rgba=x, batch_dhw=case.dhw, batch_ray_dir=[case.ray_dir[i] for i in idx],
                        batch_eye_pos=[case.eye[i] for i in idx], batch_z_dir=[case.z_dir[i] for i in idx], separate_background=None)
     ((color * gc).sum() + (depth * gd).sum()).backward()
-    return n(x.grad)
+    return to_np(x.grad)
 
 
 def test_torch_deterministic_switch_selects_the_deterministic_backward(monkeypatch):
@@ -260,7 +240,7 @@ def test_torch_deterministic_switch_selects_the_deterministic_backward(monkeypat
 
     monkeypatch.setattr(lib, "gmpi_mpi_render_bwd_deterministic_ex", spy)
     case = synth.make_case(n_planes=16, tex=256, img=256, n_mpi=2, views_per_mpi=2, seed=61, device=d, last_alpha_one=True)
-    gc, gd = _upstream(4, 256, 256, 14, d)
+    gc, gd = upstream(4, 256, 256, 14, device=d)
     mpi = g.MPI(align_corners=True, validate="full")
     default = _train_step(case, gc, gd, mpi)
     assert calls == []

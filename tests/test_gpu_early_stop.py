@@ -11,13 +11,12 @@ import numpy as np
 import pytest
 import torch
 
-import mpi_oracle
 import ml_gmpi_b200 as g
 from ml_gmpi_b200 import _lib, synth
-from testlib import CASES, assert_bitwise, case, dev, early_stop_stats, forced_kernel, kernel_fixture, max_plane_depth
+from testlib import (CASES, EXPECT, assert_bitwise, case, dev, early_stop_stats, forced_kernel, kernel_fixture, max_plane_depth,
+                     oracle_forward)
 
 pytestmark = pytest.mark.gpu
-EXPECT = 2e-5
 TAUS = [2.0 ** -24, 1e-3, 0.05]
 variant = kernel_fixture("direct", "staged2", "staged3")
 
@@ -25,8 +24,7 @@ variant = kernel_fixture("direct", "staged2", "staged3")
 @functools.lru_cache(maxsize=None)
 def oracle(name):
     c = case(name)
-    color, depth, _ = mpi_oracle.forward(c["rgba"], c["view2mpi"], c["dhw"], c["ray_dir"], c["eye"], c["z_dir"], align_corners=c["ac"],
-                                         nthreads=8)
+    color, depth, _ = oracle_forward(c, align_corners=c["ac"])
     return 2 * color - 1, depth
 
 
@@ -142,7 +140,7 @@ def test_structured_workload_skips_stages_within_the_bound(stages, factored):
     for tau_ in (tau, 0.05):      # the producer lags a stopped tile by at most the ring depth; these tiles stop ~N/2 planes early
         skipped, total = out[("stats", tau_)]
         assert total == tiles * N and 0 < skipped < total, (tau_, skipped, total)
-    rc, rd, _ = mpi_oracle.forward(c["rgba"], c["view2mpi"], c["dhw"], c["ray_dir"], c["eye"], c["z_dir"], nthreads=8)
+    rc, rd, _ = oracle_forward(c)
     for tau_ in (tau, 0.05):
         got = out[tau_]
         for ref in (out[None], (2 * rc - 1, rd)):

@@ -12,7 +12,7 @@ d rgb = the sum of g_rgba[:, :last, :3] over planes, in float64 (last = N - 1 wi
 
 Bars (derived, not fitted):
   forward      bitwise the expanded render on the same kernel (DESIGN.md, N1), and rel_err <= EXPECT against the oracle for
-               colour and depth (EXPECT: the expanded kernels' bar, tests/test_gpu_parity.py).
+               colour and depth (EXPECT: the expanded kernels' bar, tests/testlib.py).
   d alpha      rel_err <= EXPECT: the alpha box is the expanded path's 26-bit fixed point, one plane per texel.
   d rgb, d bg  max|ours - ref| / S, S = max|oracle g_rgba| over all planes and channels.  The box backward rounds every colour
                contribution to a multiple of 2^(e_rgb - kFixBitsRgb) (kFixBitsRgb = 22, csrc/mpi_bwd_box.cuh) with 2^e_rgb <= 4 gmax
@@ -32,24 +32,20 @@ import ctypes
 import dataclasses
 import functools
 import json
-import os
 
 import numpy as np
 import pytest
 import torch
 
-import mpi_oracle
 import ml_gmpi_b200 as g
 from ml_gmpi_b200 import _lib, synth
 from conftest import MPI_CASES, load_golden, rel_err
-from testlib import (assert_bitwise, dev, expanded_grad, factored_grads, forced_kernel, kernel_fixture, limit_footprints, misaligned,
-                     one_tile_per_mpi_case)
+from testlib import (EXPECT, assert_bitwise, dev, expanded_grad, factored_grads, forced_kernel, kernel_fixture, limit_footprints,
+                     misaligned, one_tile_per_mpi_case, oracle_backward, oracle_forward, to_np, upstream)
 
 pytestmark = pytest.mark.gpu
-EXPECT = 2e-5
 FIX_BITS_RGB = 22                  # kFixBitsRgb, csrc/mpi_bwd_box.cuh
 ROUND_RGB = 2.0 ** -(FIX_BITS_RGB - 1)   # largest rounding of one colour contribution, in units of gmax: 2^(e_rgb - 23) / gmax
-_NT = max(1, min(64, (os.cpu_count() or 8)))
 
 
 # The direct kernels, or the staged forward + box backward forced whatever the number of tiles (the factored ring is always 3 deep:
@@ -87,9 +83,10 @@ def _synth(geo, M, N, tex_hw, seed, alpha_scale=None, last_one=True, ray=None, d
     gc = torch.randn((V, 3, H, W), generator=gen)
     gd = torch.randn((V, 1, H, W), generator=gen) if depth_grad else None
     dhw = geo.dhw[:1].expand(Mt, -1, -1) if extra_mpis else geo.dhw
-    n = lambda t: None if t is None else np.ascontiguousarray(t.cpu().numpy())
-    return dict(rgb=n(rgb), alpha=n(alpha), bg=n(bg), view2mpi=n(geo.view2mpi), dhw=n(dhw), ray_dir=n(ray), eye=n(geo.eye),
-                z_dir=n(geo.z_dir), ac=ac, gc=n(gc), gd=n(gd), m11=m11, visible=visible)
+    arrays = dict(rgb=rgb, alpha=alpha, bg=bg, view2mpi=geo.view2mpi, dhw=dhw, ray_dir=ray, eye=geo.eye, z_dir=geo.z_dir, gc=gc,
+                  gd=gd)
+    c = {k: None if t is None else np.ascontiguousarray(to_np(t)) for k, t in arrays.items()}
+    return dict(c, ac=ac, m11=m11, visible=visible)
 
 
 def _mk(**kw):
@@ -239,10 +236,9 @@ def reference(name, with_bg, wrong=None):
         v2m = c["view2mpi"].copy()
         c["view2mpi"] = np.where(v2m == 0, 1, np.where(v2m == 1, 0, v2m)).astype(np.int32)
     rgba = _expand(c, expand_bg)
-    args = (rgba, c["view2mpi"], c["dhw"], c["ray_dir"], c["eye"], c["z_dir"])
-    color, depth, flags = mpi_oracle.forward(*args, align_corners=c["ac"], check_last_plane=True, nthreads=_NT)
+    color, depth, flags = oracle_forward(c, rgba=rgba, align_corners=c["ac"], check_last_plane=True)
     gc = c["gc"] * (2.0 if c["m11"] else 1.0)         # the kernel's upstream gradient w.r.t. c when the output is 2c - 1
-    G = mpi_oracle.backward(*args, gc, c["gd"], align_corners=c["ac"], nthreads=_NT)
+    G = oracle_backward(c, gc, c["gd"], rgba=rgba, align_corners=c["ac"])
     del rgba
     N = G.shape[1]
     last = N - 1 if with_bg else N
@@ -373,9 +369,8 @@ def run(name, with_bg, mpi=None, view_group=1):
     if c["gd"] is not None:
         loss = loss + (dep * torch.from_numpy(c["gd"]).to(d)).sum()
     loss.backward()
-    n = lambda t: None if t is None else t.detach().cpu().numpy()
-    out = dict(color=n(col), depth=n(dep), flags=int(ft.item()), g_rgb=n(leaves[0].grad), g_alpha=n(leaves[1].grad),
-               g_bg=n(leaves[2].grad) if with_bg else None)
+    out = dict(color=to_np(col), depth=to_np(dep), flags=int(ft.item()), g_rgb=to_np(leaves[0].grad), g_alpha=to_np(leaves[1].grad),
+               g_bg=to_np(leaves[2].grad) if with_bg else None)
     assert int(ff.item()) == out["flags"]
     return out
 
@@ -430,9 +425,7 @@ def test_one_tile_per_mpi_factored_gradients_are_bitwise_the_expanded_ones():
     d = dev()
     with forced_kernel("staged"):
         geo = one_tile_per_mpi_case(d)
-        gen = torch.Generator().manual_seed(4)
-        gc = torch.randn((2, 3, 24, 64), generator=gen).to(d)
-        gd = torch.randn((2, 1, 24, 64), generator=gen).to(d)
+        gc, gd = upstream(2, 24, 64, 4, device=d)
         gen = torch.Generator(device=d).manual_seed(6)
         rgb, alpha, bg = (torch.rand(sh, generator=gen, device=d) for sh in ((2, 3, 64, 64), (2, 6, 1, 64, 64), (2, 3, 64, 64)))
         alpha[:, :-1] *= 0.3
@@ -473,8 +466,7 @@ def test_zero_grad_poisoned_buffers_any_view_order(order, variant):
         torch.cuda.synchronize()
         return [t.cpu().numpy() for t in (gr, ga, gb)]
 
-    n = lambda t: t.cpu().numpy()
-    out = dict(color=n(color), depth=n(depth), flags=int(flags.item()))
+    out = dict(color=to_np(color), depth=to_np(depth), flags=int(flags.item()))
     z_rgb, z_alpha, z_bg = bwd(float("nan"), opt | _lib.OPT_ZERO_GRAD)
     assert not (z_rgb[3].any() or z_alpha[3].any() or z_bg[3].any()), "an MPI without views must get exactly 0"
     check(f"{name}/zero_grad/{variant}", dict(out, g_rgb=z_rgb, g_alpha=z_alpha, g_bg=z_bg), name, True)

@@ -32,7 +32,7 @@ from ml_gmpi_b200 import _lib
 from ml_gmpi_b200.mpi import MPI, MPIOutOfPlaneError
 from ml_gmpi_b200.synth import ffhq_dhw, make_poses
 from ml_gmpi_b200.camera import cam_params
-from testlib import FLAG_CASES, FORWARD_FLAGS, dev, forced_kernel, kernel_fixture
+from testlib import FLAG_CASES, FORWARD_FLAGS, dev, forced_kernel, kernel_fixture, oracle_forward
 
 gpu = pytest.mark.gpu
 OOB, BEHIND = mpi_oracle.FLAG_LAST_PLANE_OOB, mpi_oracle.FLAG_PLANE_BEHIND_EYE
@@ -151,8 +151,7 @@ def cam_cases():
 
 
 def oracle_flags(c, check):
-    return mpi_oracle.forward(c["rgba"], c["view2mpi"], c["dhw"], c["ray_dir"], c["eye"], c["z_dir"],
-                              align_corners=bool(c["align_corners"]), check_last_plane=check)[2]
+    return oracle_forward(c, align_corners=bool(c["align_corners"]), check_last_plane=check)[2]
 
 
 def test_built_cases_sit_on_their_edges():

@@ -12,7 +12,6 @@ Each test skips unless the card has its declared peak free, prints "LARGE_OFFSET
 and fails if it held more than it declared."""
 import ctypes
 import json
-import os
 import time
 
 import numpy as np
@@ -25,14 +24,12 @@ from ml_gmpi_b200 import _lib, synth
 from ml_gmpi_b200.camera import cam_params, focal_from_fov, sphere_poses
 from ml_gmpi_b200.geometry import FFHQ
 from conftest import rel_err
-from testlib import (BIG_IMG, BIG_M, BIG_M_FACTORED, BIG_N, BIG_PEAK_BYTES, BIG_R, BIG_SLACK, BIG_V_COLOR, BIG_V_GATHER, SMALL_MPI,
-                     assert_bitwise, big_views, dev, forced_kernel, headline_case, kernel_fixture, native_vs_fp32, render_fwd, set_kernel,
-                     skip_stats)
+from testlib import (BIG_IMG, BIG_M, BIG_M_FACTORED, BIG_N, BIG_PEAK_BYTES, BIG_R, BIG_SLACK, BIG_V_COLOR, BIG_V_GATHER, EXPECT,
+                     SMALL_MPI, assert_bitwise, big_views, dev, factored_refs, forced_kernel, headline_case, kernel_fixture,
+                     native_vs_fp32, oracle_backward, oracle_forward, render_fwd, set_kernel, skip_stats, upstream)
 
 pytestmark = pytest.mark.gpu
-EXPECT = 2e-5       # the parity bar (tests/test_gpu_parity.py)
 NEAR_FAR = 1e-6     # near against far where only the order of fp32 atomics differs
-_NT = max(1, min(64, os.cpu_count() or 8))
 N, R, M, MF = BIG_N, BIG_R, BIG_M, BIG_M_FACTORED
 variant = kernel_fixture("auto", "direct")
 
@@ -127,25 +124,17 @@ def _drop_oracle_cache():
 def _oracle_forward():
     """(colour in [-1, 1], depth) of the oracle on the headline MPI alone, both views of big_views."""
     if "fwd" not in _oracle_cache:
-        h, v = headline_case(), big_views()
-        rc, rd, _ = mpi_oracle.forward(h["rgba"], np.zeros(2, np.int32), v["dhw"], v["ray_dir"], v["eye"], v["z_dir"], nthreads=_NT)
+        rc, rd, _ = oracle_forward(big_views(), rgba=headline_case()["rgba"])
         _oracle_cache["fwd"] = (_minus1_1(rc), rd)
     return _oracle_cache["fwd"]
 
 
-def _upstream(V=1, seed=3):
-    gen = torch.Generator().manual_seed(seed)
-    return torch.randn((V, 3, R, R), generator=gen), torch.randn((V, 1, R, R), generator=gen)
-
-
 def _oracle_backward(views):
-    """d rgba of the oracle on the headline MPI alone, big_views' views `views`, under _upstream(len(views))'s gradients (colour in
-    [0, 1])."""
+    """d rgba of the oracle on the headline MPI alone, big_views' views `views`, under upstream(len(views), R, R, 3)'s gradients
+    (colour in [0, 1])."""
     if ("bwd", views) not in _oracle_cache:
-        h, v = headline_case(), _views(0, 1, views)
-        gc, gd = _upstream(len(views))
-        _oracle_cache["bwd", views] = mpi_oracle.backward(h["rgba"], v["view2mpi"], v["dhw"], v["ray_dir"], v["eye"], v["z_dir"],
-                                                          gc.numpy(), gd.numpy(), nthreads=_NT)[0]
+        gc, gd = upstream(len(views), R, R, 3)
+        _oracle_cache["bwd", views] = oracle_backward(_views(0, 1, views), gc, gd, rgba=headline_case()["rgba"])[0]
     return _oracle_cache["bwd", views]
 
 
@@ -286,7 +275,7 @@ def test_expanded_backward_near_equals_far(variant, budget):
     big = torch.full((M, N, 4, R, R), float("nan"), device=dev())
     big[0].copy_(_content())
     big.requires_grad_(True)
-    gc, gd = (t.to(dev()) for t in _upstream(2))
+    gc, gd = upstream(2, R, R, 3, device=dev())
     kept = {}
     for slot in (0, M - 1):
         v = {k: torch.from_numpy(a).to(dev()) for k, a in _views(slot, M).items() if isinstance(a, np.ndarray)}
@@ -334,7 +323,7 @@ def test_factored_near_equals_far(budget):
         del near
         if dt == torch.float16:
             del mpi
-    gc, gd = (t.to(d) for t in _upstream(2))
+    gc, gd = upstream(2, R, R, 3, device=d)
     kept = {}
     for slot in (MF - 1, 0):
         leaves = [t.requires_grad_(True) for t in mpi]
@@ -357,9 +346,8 @@ def test_factored_near_equals_far(budget):
                     _move(t, MF - 1, 0, float("nan"))
     del mpi, leaves
     h, v = [x.cpu() for x in one], _views(0, 1)
-    ref = mpi_oracle.backward(g.expand_factored(*h).numpy(), v["view2mpi"], v["dhw"], v["ray_dir"], v["eye"], v["z_dir"],
-                              gc.cpu().numpy(), gd.cpu().numpy(), nthreads=_NT)
-    refs = [ref[:, :-1, :3].astype(np.float64).sum(1), ref[:, :, 3:4], ref[:, -1, :3]]
+    ref = oracle_backward(v, gc, gd, rgba=g.expand_factored(*h))
+    refs = factored_refs(ref)
     # the bars of tests/test_gpu_factored.py: relative to the largest expanded gradient S, the colour gradients add the rounding of
     # each tap's fixed-point contribution (2^-21 of the largest upstream colour gradient) to the parity bar
     kf, kl = _most_taps(v)
@@ -399,7 +387,7 @@ def test_saved_transmittance_past_2_31(twin, budget):
     assert torch.equal(trans[V - 1].view(torch.int32), trans[0].view(torch.int32))
     assert_bitwise((color[V - 1], depth[V - 1]), (color[0], depth[0]), "view 21 != view 0")
     del color, depth
-    gc1, gd1 = _upstream()
+    gc1, gd1 = upstream(1, R, R, 3)
     g_rgba = torch.full_like(rgba, float("nan"))
     grads = {}
     for det in (True, False):

@@ -32,7 +32,7 @@ C. The training instantiations (mpi_fwd_staged_kernel<kKeyEmit | ...>, the direc
    descriptor and through the classic gmpi_mpi_render_fwd_train.
 
 D. The classic entry points with data: gmpi_mpi_render_fwd is bitwise gmpi_mpi_render_fwd_ex; gmpi_mpi_render_bwd (no T: the
-   two-pass direct kernel) and gmpi_mpi_render_bwd_saved (the box kernel) are within 2e-5 of mpi_oracle.backward, also when the
+   two-pass direct kernel) and gmpi_mpi_render_bwd_saved (the box kernel) are within 2e-5 of the oracle's backward, also when the
    box kernel is fed the T of the direct forward (the T*((1-a)+1e-10) form)."""
 import ctypes
 import functools
@@ -46,10 +46,10 @@ import mpi_oracle
 from ml_gmpi_b200 import _lib, synth
 from ml_gmpi_b200.camera import cam_params
 from conftest import MPI_CASES, load_golden, rel_err
-from testlib import assert_bitwise, dev, forced_kernel, kernel_fixture, set_kernel
+from testlib import (EXPECT, assert_bitwise, dev, forced_kernel, kernel_fixture, oracle_backward, oracle_forward, set_kernel, to_np,
+                     upstream)
 
 gpu = pytest.mark.gpu
-EXPECT = 2e-5
 U = 2.0 ** -24
 SENTINEL = 0x7FC0DEAD          # a quiet NaN no kernel writes
 OPT_AC, OPT_CHECK, OPT_M11, OPT_ES, OPT_F16 = (_lib.OPT_ALIGN_CORNERS, _lib.OPT_CHECK_LAST_PLANE, _lib.OPT_COLOR_MINUS1_1,
@@ -327,12 +327,12 @@ def _golden(name):
 
 @pytest.mark.parametrize("name", MPI_CASES)
 def test_float64_transmittance_reference_composites_the_oracle_and_golden_colours(name):
-    """CPU self-check of composite64: the colour and depth it composites from its own T64 match mpi_oracle.forward and the
+    """CPU self-check of composite64: the colour and depth it composites from its own T64 match the oracle's forward and the
     reference's golden colour and depth within 1e-6 (relative to the largest value)."""
     c = _golden(name)
     T64, col, dep = composite64(c, with_color=True)
     assert (T64[:, 0] == 1).all() and (T64 >= 0).all() and (T64 <= 1).all()
-    oc, od, _ = mpi_oracle.forward(c["rgba"], c["view2mpi"], c["dhw"], c["ray_dir"], c["eye"], c["z_dir"], align_corners=c["ac"])
+    oc, od, _ = oracle_forward(c, align_corners=c["ac"])
     e = dict(oracle_color=rel_err(col, oc), oracle_depth=rel_err(dep, od), golden_color=rel_err(col, c["color"]),
              golden_depth=rel_err(dep, c["depth"]))
     assert max(e.values()) <= 1e-6, e
@@ -352,8 +352,8 @@ def _synth(n_planes, tex, img, n_mpi, views=1, seed=0, alpha_scale=None, ray=Non
     if last_one:
         rgba[:, -1, 3] = 1.0
     ray = geo.ray_dir if ray is None else ray(geo.ray_dir)
-    n = lambda t: np.ascontiguousarray(t.numpy())
-    return dict(rgba=n(rgba), view2mpi=n(geo.view2mpi), dhw=n(dhw), ray_dir=n(ray), eye=n(geo.eye), z_dir=n(geo.z_dir), ac=ac)
+    arrays = dict(rgba=rgba, view2mpi=geo.view2mpi, dhw=dhw, ray_dir=ray, eye=geo.eye, z_dir=geo.z_dir)
+    return dict({k: np.ascontiguousarray(to_np(t)) for k, t in arrays.items()}, ac=ac)
 
 
 def _shuffle(ray):
@@ -534,18 +534,16 @@ def test_transmittance_bars_fail_on_wrong_problems(variant):
 @pytest.mark.parametrize("name", ["tiny_2mpi_3view", "staged_shape"])
 def test_classic_backward_entry_points_match_the_oracle(name):
     """gmpi_mpi_render_bwd (two-pass direct kernel), gmpi_mpi_render_bwd_saved with the direct forward's T (direct kernels forced,
-    and the box kernel) and with the staged forward's T (box kernel): each within EXPECT of mpi_oracle.backward."""
+    and the box kernel) and with the staged forward's T (box kernel): each within EXPECT of the oracle's backward."""
     c = case(name)
     lib = _lib.load()
-    gen = torch.Generator().manual_seed(17)
     V, _, H, W = c["ray_dir"].shape
-    gc, gd = torch.randn((V, 3, H, W), generator=gen).numpy(), torch.randn((V, 1, H, W), generator=gen).numpy()
-    ref = mpi_oracle.backward(c["rgba"], c["view2mpi"], c["dhw"], c["ray_dir"], c["eye"], c["z_dir"], gc, gd, align_corners=c["ac"],
-                              nthreads=8)
+    gc, gd = upstream(V, H, W, 17)
+    ref = oracle_backward(c, gc, gd, align_corners=c["ac"])
     i = _train_inputs(c)
     geo = [i[k].data_ptr() for k in ("rgba", "view2mpi", "dhw", "ray_dir", "eye", "z_dir")]
     sizes = [i["M"], V, i["N"], i["Ht"], i["Wt"], H, W]
-    g_color, g_depth = _t(gc), _t(gd)
+    g_color, g_depth = gc.to(dev()), gd.to(dev())
     st = torch.cuda.current_stream().cuda_stream
 
     def train_t():

@@ -9,6 +9,11 @@
   forward_desc, render_fwd,       one gmpi_mpi_render_fwd_ex of a catalogue case, and the render of a native (fp16 / uint8) MPI
   native_vs_fp32                  beside the fp32 MPI it stands for, on the same kernel
   BIG_*, big_views                the shapes, views and declared device peaks of the buffers past 2^31 elements
+  EXPECT, FACTORED_RGB_EXPECT     the parity bar against the CPU oracle, and the bar of a factored MPI's d rgb
+  ORACLE_THREADS, to_np           the oracle's threads; a tensor as numpy
+  upstream, oracle_forward,       the upstream gradients of a backward test; the oracle's forward and backward of a case; its
+  oracle_backward, factored_refs, gradient split into a factored MPI's (d rgb, d alpha, d bg_rgb), and the check of a factored
+  check_factored                  backward against it
 and the helpers several modules read: the machine code of the built library, the staged forward's footprints and its limit cases,
 oracle-side bounds and references, and the flag cases of tests/golden/flags_edges.npz."""
 import contextlib
@@ -26,7 +31,7 @@ import numpy as np
 import pytest
 import torch
 
-from conftest import GOLDEN, MPI_CASES, load_golden     # first: it puts the repository and oracle/ on sys.path
+from conftest import GOLDEN, MPI_CASES, load_golden, rel_err     # first: it puts the repository and oracle/ on sys.path
 import mpi_oracle  # noqa: E402
 import ml_gmpi_b200 as g  # noqa: E402
 from ml_gmpi_b200 import _lib, synth  # noqa: E402
@@ -328,6 +333,67 @@ def big_views():
 def assert_class_88_behind_plane_25(c):
     cls = footprints(c)["cls"]
     assert (cls[..., 25:] == 88).any() and all((cls == k).any() for k in range(56, 96, 8))
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# the CPU oracle (oracle/mpi_oracle.py): the parity bar, upstream gradients, the oracle's forward and backward of a case
+# ------------------------------------------------------------------------------------------------------------------------------
+# The parity bar: max |ours - oracle| / max |oracle| of colour, depth and d rgba.  The texel coordinates are bit-exact with the
+# oracle's; the rest differs from it by fp32 summation order and FMA contraction, and by T <- T - w * 1 instead of
+# T * (1 - a + 1e-10) (~1 ulp of T per plane): a few 1e-6.
+EXPECT = 2e-5
+# d rgb of a factored MPI sums the gradients of the N - 1 planes that share the colour image, so it sums their rounding errors too
+# (fixed point in the kernels, fp32 in the oracle): twice the per-plane bar.
+FACTORED_RGB_EXPECT = 2 * EXPECT
+# The oracle's pthreads.  Its forward is the same on any number of them; the order of its backward's atomic float adds, hence
+# the last ulp of the gradient, is not.
+ORACLE_THREADS = max(1, min(64, os.cpu_count() or 8))
+
+
+def to_np(t):
+    """t as numpy: a tensor detached and copied to the CPU; an array, or None, as it is."""
+    return t.detach().cpu().numpy() if isinstance(t, torch.Tensor) else t
+
+
+def upstream(V, H, W, seed, depth=True, device=None):
+    """(g_color [V,3,H,W], g_depth [V,1,H,W], or None without depth) of a backward test: randn, colour then depth, from a CPU
+    generator seeded with `seed`, on `device` (the CPU if None)."""
+    gen = torch.Generator().manual_seed(seed)
+    gc = torch.randn((V, 3, H, W), generator=gen).to(device)
+    return gc, torch.randn((V, 1, H, W), generator=gen).to(device) if depth else None
+
+
+def _oracle_inputs(case, rgba, ray_dir):
+    get = (lambda k: case[k]) if isinstance(case, dict) else (lambda k: getattr(case, k))
+    given = dict(rgba=rgba, ray_dir=ray_dir)
+    return [to_np(get(k) if given.get(k) is None else given[k]) for k in ("rgba", "view2mpi", "dhw", "ray_dir", "eye", "z_dir")]
+
+
+def oracle_forward(case, rgba=None, ray_dir=None, align_corners=True, check_last_plane=False):
+    """mpi_oracle.forward of a case -> (colour, depth, flags).  The case is a dict or an object (synth.Case) with the fields rgba,
+    view2mpi, dhw, ray_dir, eye and z_dir, as numpy arrays or tensors; rgba and ray_dir, when given, replace the case's."""
+    return mpi_oracle.forward(*_oracle_inputs(case, rgba, ray_dir), align_corners=align_corners, check_last_plane=check_last_plane,
+                              nthreads=ORACLE_THREADS)
+
+
+def oracle_backward(case, g_color, g_depth=None, rgba=None, ray_dir=None, align_corners=True, minus1_1=False):
+    """mpi_oracle.backward of a case (as oracle_forward takes it) under the upstream gradients -> d rgba.  minus1_1: g_color is the
+    gradient of the colour in [-1, 1], 2 c - 1, whose gradient with respect to c is 2 g_color."""
+    gc = to_np(g_color)
+    return mpi_oracle.backward(*_oracle_inputs(case, rgba, ray_dir), 2.0 * gc if minus1_1 else gc, to_np(g_depth),
+                               align_corners=align_corners, nthreads=ORACLE_THREADS)
+
+
+def factored_refs(ref):
+    """The oracle's expanded gradient -> (d rgb, d alpha, d bg_rgb) of a factored MPI with a background plane: d rgb is the sum, in
+    float64, over the planes that share the colour image."""
+    return ref[:, :-1, :3].astype(np.float64).sum(1), ref[:, :, 3:4], ref[:, -1, :3]
+
+
+def check_factored(ours, ref):
+    """ours = (d rgb, d alpha, d bg_rgb) against factored_refs(ref): d rgb within FACTORED_RGB_EXPECT, the others within EXPECT."""
+    e = [rel_err(o, r) for o, r in zip(ours, factored_refs(ref))]
+    assert e[0] <= FACTORED_RGB_EXPECT and e[1] <= EXPECT and e[2] <= EXPECT, e
 
 
 # ------------------------------------------------------------------------------------------------------------------------------
