@@ -13,8 +13,8 @@ import torch
 
 import ml_gmpi_b200 as g
 from ml_gmpi_b200 import _lib, synth
-from testlib import (CASES, EXPECT, assert_bitwise, case, dev, early_stop_stats, forced_kernel, kernel_fixture, max_plane_depth,
-                     oracle_forward)
+from testlib import (CASES, EXPECT, GEOMETRY, assert_bitwise, case, dev, early_stop_stats, forced_kernel, kernel_fixture,
+                     max_plane_depth, on_device, oracle_forward)
 
 pytestmark = pytest.mark.gpu
 TAUS = [2.0 ** -24, 1e-3, 0.05]
@@ -31,13 +31,11 @@ def oracle(name):
 def render(name, early_stop=None):
     """render_frames on the case: (colour in [-1,1], depth) as numpy, or (uint8 colour, uint8 depth) for the video cases."""
     c = case(name)
-    d = dev()
-    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(d)
-    mpi = dict(rgb=t(c["factored"][0]), alpha=t(c["factored"][1]), bg_rgb=t(c["factored"][2])) if "factored" in c else dict(rgba=t(c["rgba"]))
+    mpi = dict(zip(("rgb", "alpha", "bg_rgb"), on_device(c, "rgb", "alpha", "bg"))) if c.get("factored") else dict(rgba=on_device(c, "rgba")[0])
     video = {"near": 0.9, "far": 1.2} if c.get("video") else None
     with torch.no_grad():
-        a, b = g.render_frames(dhw=t(c["dhw"]), view2mpi=t(c["view2mpi"]), ray_dir=t(c["ray_dir"]), eye=t(c["eye"]), z_dir=t(c["z_dir"]),
-                               align_corners=c["ac"], view_group=c.get("view_group", 1), video=video, early_stop=early_stop, **mpi)
+        a, b = g.render_frames(**dict(zip(GEOMETRY, on_device(c, *GEOMETRY))), align_corners=c["ac"], view_group=c.get("view_group", 1),
+                               video=video, early_stop=early_stop, **mpi)
     torch.cuda.synchronize()
     return a.cpu().numpy(), b.cpu().numpy()
 

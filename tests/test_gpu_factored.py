@@ -2,8 +2,8 @@
 oracle on the expanded stack, on the direct kernels and on the TMA-staged forward + box backward (run on an H100: pytest -m gpu).
 
 The factored kernels are template instantiations of their own (mpi_fwd_staged_kernel<kKeyFac | ...>, mpi_bwd_box_kernel<kKeyFac | ...>) with
-their own ring and box layout, so every edge the expanded kernels are tested at is repeated here: align_corners=False, non-square
-textures, partial tiles, N = 1 and N = 512, footprints 89..96 texels wide (they fit the factored forward's 96-wide box but take the
+their own ring and box layout, so every edge the expanded kernels are tested at (tests/testlib.py's case catalogue) is repeated here:
+align_corners=False, non-square textures, partial tiles, N = 1 and N = 512, footprints 89..96 texels wide (they fit the factored forward's 96-wide box but take the
 generic body, as in the expanded ring) and wider than 96, non-pinhole and degenerate rays, MPIs without views, views in any order, GMPI_ZERO_GRAD, view_group, unaligned
 factors, the host entry point and the benchmark's own shapes.
 
@@ -29,7 +29,6 @@ Bars (derived, not fitted):
                that sent the background's gradient to d rgb.
 test_the_bars_fail_on_a_slightly_wrong_problem shows that these bars fail by 10x or more on slightly wrong problems."""
 import ctypes
-import dataclasses
 import functools
 import json
 
@@ -38,10 +37,11 @@ import pytest
 import torch
 
 import ml_gmpi_b200 as g
-from ml_gmpi_b200 import _lib, synth
-from conftest import MPI_CASES, load_golden, rel_err
-from testlib import (EXPECT, assert_bitwise, dev, expanded_grad, factored_grads, forced_kernel, kernel_fixture, limit_footprints,
-                     misaligned, one_tile_per_mpi_case, oracle_backward, oracle_forward, to_np, upstream)
+from ml_gmpi_b200 import _lib
+from conftest import MPI_CASES, rel_err
+from testlib import (EXPECT, GEOMETRY, assert_bitwise, case, dev, expanded_grad, factored_grads, forced_kernel, kernel_fixture,
+                     limit_footprints, misaligned, on_device, one_tile_per_mpi_case, oracle_backward, oracle_forward, pixels, to_np,
+                     upstream)
 
 pytestmark = pytest.mark.gpu
 FIX_BITS_RGB = 22                  # kFixBitsRgb, csrc/mpi_bwd_box.cuh
@@ -53,163 +53,16 @@ ROUND_RGB = 2.0 ** -(FIX_BITS_RGB - 1)   # largest rounding of one colour contri
 variant = kernel_fixture("direct", "staged")
 
 
-# ------------------------------------------------------------------------------------------------------------------------------
-# cases: geometry + factors + upstream gradients, all numpy
-# ------------------------------------------------------------------------------------------------------------------------------
-def _golden(name):
-    gd = load_golden(name)
-    rgba = gd["rgba"]
-    return dict(rgb=rgba[:, 0, :3], alpha=rgba[:, :, 3:4], bg=rgba[:, -1, :3], view2mpi=gd["view2mpi"], dhw=gd["dhw"],
-                ray_dir=gd["ray_dir"], eye=gd["eye"], z_dir=gd["z_dir"], ac=bool(gd["align_corners"]), gc=gd["g_color"],
-                gd=gd.get("g_depth"))
-
-
-def _synth(geo, M, N, tex_hw, seed, alpha_scale=None, last_one=True, ray=None, depth_grad=True, m11=False, ac=True, visible=False,
-           extra_mpis=0, alpha="uniform"):
-    """A synth.make_case geometry (rgba=False) with random factors.  alpha_scale scales the alphas in front of the last plane (visible:
-    the background shows through, T in front of it mostly >= 0.1).  extra_mpis: MPIs that no view looks at.  alpha: "uniform"
-    (U(0, 1)) or "equal_weight" (synth.equal_weight_alpha: every plane reaches the render)."""
-    ray = geo.ray_dir if ray is None else ray
-    gen = torch.Generator().manual_seed(seed)
-    Mt = M + extra_mpis
-    rgb, bg = torch.rand((Mt, 3) + tex_hw, generator=gen), torch.rand((Mt, 3) + tex_hw, generator=gen)
-    alpha = synth.equal_weight_alpha((Mt, N) + tex_hw, gen).unsqueeze(2) if alpha == "equal_weight" else \
-        torch.rand((Mt, N, 1) + tex_hw, generator=gen)
-    if alpha_scale is not None:
-        alpha[:, :-1] *= alpha_scale
-    if last_one:
-        alpha[:, -1] = 1.0
-    V, _, H, W = ray.shape
-    gc = torch.randn((V, 3, H, W), generator=gen)
-    gd = torch.randn((V, 1, H, W), generator=gen) if depth_grad else None
-    dhw = geo.dhw[:1].expand(Mt, -1, -1) if extra_mpis else geo.dhw
-    arrays = dict(rgb=rgb, alpha=alpha, bg=bg, view2mpi=geo.view2mpi, dhw=dhw, ray_dir=ray, eye=geo.eye, z_dir=geo.z_dir, gc=gc,
-                  gd=gd)
-    c = {k: None if t is None else np.ascontiguousarray(to_np(t)) for k, t in arrays.items()}
-    return dict(c, ac=ac, m11=m11, visible=visible)
-
-
-def _mk(**kw):
-    return synth.make_case(rgba=False, **kw)
-
-
-def _partial_acfalse():
-    """test_gpu_parity.test_partial_tiles_align_corners_false_nonsquare_vs_oracle's shape: 100 x 136 pixels, 72 x 116 textures."""
-    geo = _mk(n_planes=10, tex=8, img=136, n_mpi=2, views_per_mpi=2, seed=47)
-    return _synth(geo, 2, 10, (72, 116), 47, alpha_scale=0.2, ray=geo.ray_dir[:, :, 18:118].contiguous(), ac=False, visible=True)
-
-
-def _n1():
-    geo = _mk(n_planes=8, tex=128, img=160, n_mpi=2, seed=41)
-    geo = dataclasses.replace(geo, dhw=geo.dhw[:, 3:4].contiguous())
-    return _synth(geo, 2, 1, (128, 128), 41, last_one=False, visible=True)      # with bg_rgb the one plane IS the background
-
-
-def _n512():
-    geo = _mk(n_planes=512, tex=96, img=128, n_mpi=2, seed=43)
-    return _synth(geo, 2, 512, (96, 96), 43, alpha_scale=0.02)                     # the back planes show through
-
-
-def _wide(tex_hw, seed):
-    """16 planes of a wide texture at 720^2 from three random poses (testlib.limit_case): 512 x 1024 gives many footprints 89..96
-    texels wide, which the factored forward's 96-wide box could hold but which take the generic body in the forward (as in the expanded
-    ring: the bodies' bilinear weights differ in the last bit) and in the backward (classes 56..88); 512 x 1536 gives footprints wider
-    than 96."""
-    geo = _mk(n_planes=16, tex=8, img=720, n_mpi=1, views_per_mpi=3, seed=seed)
-    return _synth(geo, 1, 16, tex_hw, seed, alpha_scale=0.1, visible=True)
-
-
-def _shuffled():
-    """Rays shuffled within the image (test_staged_falls_back_per_thread_for_non_projective_rays): not a pinhole camera's."""
-    geo = _mk(n_planes=12, tex=96, img=200, n_mpi=1, views_per_mpi=2, seed=3)
-    perm = torch.randperm(200 * 200, generator=torch.Generator().manual_seed(0))
-    ray = geo.ray_dir.reshape(2, 3, -1)[:, :, perm].reshape(2, 3, 200, 200).contiguous()
-    return _synth(geo, 1, 12, (96, 96), 3, alpha_scale=0.2, ray=ray, visible=True)
-
-
-def _corners_off():
-    """Every 64 x 30 tile's corner rays pushed far off the planes, interior rays kept
-    (test_non_projective_rays_outside_the_corner_box_still_render)."""
-    geo = _mk(n_planes=6, tex=64, img=128, n_mpi=1, views_per_mpi=2, seed=9)
-    ray = geo.ray_dir.clone()
-    for ty in range(0, 128, 30):
-        for tx in range(0, 128, 64):
-            for (cy, cx) in ((ty, tx), (ty, min(tx + 63, 127)), (min(ty + 29, 127), tx), (min(ty + 29, 127), min(tx + 63, 127))):
-                ray[:, 0, cy, cx] = 5.0
-    return _synth(geo, 1, 6, (64, 64), 9, alpha_scale=0.4, ray=ray, visible=True)
-
-
-def _degenerate():
-    """ray_z == 0 and NaN rays (test_degenerate_rays_do_not_poison_neighbours); the rest of the image must match.  Those pixels get
-    no upstream gradient."""
-    geo = _mk(n_planes=8, tex=64, img=64, n_mpi=1, seed=4)
-    ray = geo.ray_dir.clone()
-    ray[0, 2, 10, 10:14] = 0.0
-    ray[0, :, 20, 20] = float("nan")
-    c = _synth(geo, 1, 8, (64, 64), 4, alpha_scale=0.3, ray=ray, depth_grad=False, visible=True)
-    ok = np.ones((1, 64, 64), bool)
-    ok[0, 10, 10:14] = False
-    ok[0, 20, 20] = False
-    c["gc"] = c["gc"] * ok[:, None]
-    c["ok"] = ok
-    return c
-
-
-def _op_bench(alpha="uniform"):
-    """bench.py's N1 shape for one view: 96 planes, 1024^2, random alpha (make_factored), colour-only upstream gradient w.r.t.
-    2c - 1 (fb_factored)."""
-    geo = _mk(n_planes=96, tex=1024, img=1024, n_mpi=1, seed=1234)
-    return _synth(geo, 1, 96, (1024, 1024), 99, last_one=False, depth_grad=False, m11=True, alpha=alpha)
-
-
-def _op_views4(alpha="uniform"):
-    """One 48-plane 512^2 MPI seen from four views, colour and depth upstream gradients, alpha == 1 last plane."""
-    geo = _mk(n_planes=48, tex=512, img=512, n_mpi=1, views_per_mpi=4, seed=21)
-    return _synth(geo, 1, 48, (512, 512), 21, alpha=alpha)
-
-
-def _abi(order):
-    """3 MPIs x 2 views (views sorted by MPI, interleaved or reversed) and a fourth MPI no view looks at."""
-    geo = _mk(n_planes=12, tex=256, img=256, n_mpi=3, views_per_mpi=2, seed=77)
-    pi = torch.tensor({"sorted": [0, 1, 2, 3, 4, 5], "interleaved": [0, 2, 4, 1, 3, 5], "reversed": [5, 4, 3, 2, 1, 0]}[order])
-    geo = dataclasses.replace(geo, view2mpi=geo.view2mpi[pi].contiguous(), ray_dir=geo.ray_dir[pi].contiguous(),
-                              eye=geo.eye[pi].contiguous(), z_dir=geo.z_dir[pi].contiguous())
-    return _synth(geo, 3, 12, (256, 256), 77, alpha_scale=0.15, extra_mpis=1, visible=True)
-
-
-SYNTH = {
-    "partial_acfalse_nonsquare": _partial_acfalse,
-    "N1": _n1,
-    "N512": _n512,
-    "band_89_96": lambda: _wide((512, 1024), 21),
-    "wider_than_96": lambda: _wide((512, 1536), 22),
-    "shuffled_rays": _shuffled,
-    "corners_off_the_planes": _corners_off,
-    "degenerate_rays": _degenerate,
-    "bench_96x1024": _op_bench,
-    "views4_48x512": _op_views4,
-    # the operating points with every plane visible: U(0, 1) alpha hides the planes past ~25 from every bar
-    "bench_96x1024_equal_weight": lambda: _op_bench("equal_weight"),
-    "views4_48x512_equal_weight": lambda: _op_views4("equal_weight"),
-    "view_group": lambda: _synth(_mk(n_planes=16, tex=256, img=256, n_mpi=2, views_per_mpi=4, seed=8), 2, 16, (256, 256), 8,
-                                 alpha_scale=0.12, visible=True),
-    "small": lambda: _synth(_mk(n_planes=12, tex=96, img=128, n_mpi=2, views_per_mpi=2, seed=5), 2, 12, (96, 96), 5,
-                            alpha_scale=0.18, visible=True),
-    "abi_sorted": lambda: _abi("sorted"),
-    "abi_interleaved": lambda: _abi("interleaved"),
-    "abi_reversed": lambda: _abi("reversed"),
-}
+# the catalogue's cases (tests/testlib.py): geometry, factors and upstream gradients
 GOLDEN = MPI_CASES + ["edge_odd_sizes", "edge_single_plane", "edge_acfalse_nonsquare", "edge_ragged_zero_views"]
 MATRIX = GOLDEN + ["partial_acfalse_nonsquare", "N1", "N512", "band_89_96", "wider_than_96", "shuffled_rays", "corners_off_the_planes",
                    "degenerate_rays", "bench_96x1024", "views4_48x512", "bench_96x1024_equal_weight", "views4_48x512_equal_weight"]
 
 
-@functools.lru_cache(maxsize=None)
-def case(name):
-    c = SYNTH[name]() if name in SYNTH else _golden(name)
-    c.setdefault("m11", False)
-    c.setdefault("visible", False)
-    return c
+def _mpi(c, with_bg):
+    """The factored MPI (rgb, alpha, bg_rgb or None) of case c on the device."""
+    rgb, alpha, bg = on_device(c, "rgb", "alpha", "bg")
+    return rgb, alpha, bg if with_bg else None
 
 
 def _expand(c, with_bg):
@@ -237,12 +90,12 @@ def reference(name, with_bg, wrong=None):
         c["view2mpi"] = np.where(v2m == 0, 1, np.where(v2m == 1, 0, v2m)).astype(np.int32)
     rgba = _expand(c, expand_bg)
     color, depth, flags = oracle_forward(c, rgba=rgba, align_corners=c["ac"], check_last_plane=True)
-    gc = c["gc"] * (2.0 if c["m11"] else 1.0)         # the kernel's upstream gradient w.r.t. c when the output is 2c - 1
+    gc = c["gc"] * (2.0 if c.get("m11") else 1.0)         # the kernel's upstream gradient w.r.t. c when the output is 2c - 1
     G = oracle_backward(c, gc, c["gd"], rgba=rgba, align_corners=c["ac"])
     del rgba
     N = G.shape[1]
     last = N - 1 if with_bg else N
-    return dict(color=2 * color - 1 if c["m11"] else color, depth=depth, flags=flags, g_rgb=G[:, :last, :3].astype(np.float64).sum(1),
+    return dict(color=2 * color - 1 if c.get("m11") else color, depth=depth, flags=flags, g_rgb=G[:, :last, :3].astype(np.float64).sum(1),
                 g_alpha=G[:, :, 3:4].copy(), g_bg=G[:, -1, :3].copy() if with_bg else None, S=float(np.abs(G).max()),
                 gmax=float(np.abs(gc).max()))
 
@@ -254,7 +107,7 @@ def _tap_counts(name):
     c = case(name)
     d = dev()
     lib = _lib.load()
-    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(d)
+    dhws, rays, eyes = on_device(c, "dhw", "ray_dir", "eye")
     M, N, _, Ht, Wt = c["alpha"].shape
     V, _, H, W = c["ray_dir"].shape
     front, last = torch.zeros((M, Ht * Wt), dtype=torch.int64, device=d), torch.zeros((M, Ht * Wt), dtype=torch.int64, device=d)
@@ -262,9 +115,9 @@ def _tap_counts(name):
     out = torch.empty((1, 1, 2, H, W), device=d)
     for v in range(V):
         m = int(c["view2mpi"][v])
-        ray, eye = t(c["ray_dir"][v:v + 1]), t(c["eye"][v:v + 1])
+        ray, eye = rays[v:v + 1], eyes[v:v + 1]
         for i in range(N):
-            dhw = t(c["dhw"][m:m + 1, i:i + 1])
+            dhw = dhws[m:m + 1, i:i + 1]
             _lib.check(lib.gmpi_debug_plane_coords(zero.data_ptr(), dhw.data_ptr(), ray.data_ptr(), eye.data_ptr(), out.data_ptr(),
                                                     1, 1, Ht, Wt, H, W, _lib.OPT_ALIGN_CORNERS if c["ac"] else 0, None))
             ix, iy = out[0, 0, 0].flatten(), out[0, 0, 1].flatten()
@@ -286,22 +139,20 @@ def bars(name, with_bg, ref):
     b = dict(color=EXPECT, depth=EXPECT, g_alpha=EXPECT, g_rgb=k_rgb * ROUND_RGB * ref["gmax"] / ref["S"] + EXPECT)
     if with_bg:
         b["g_bg"] = kl * ROUND_RGB * ref["gmax"] / ref["S"] + EXPECT
-        if case(name)["visible"]:
+        if case(name).get("visible"):
             b["g_bg_own"] = EXPECT
     return b
 
 
 def errors(ours, ref, c):
     """The measured figure of every check (compare with bars())."""
-    ok = c.get("ok")
-    px = (lambda a: a.transpose(1, 0, 2, 3)[:, ok]) if ok is not None else (lambda a: a)
     S = ref["S"]
-    e = dict(color=rel_err(px(ours["color"]), px(ref["color"])), depth=rel_err(px(ours["depth"]), px(ref["depth"])),
+    e = dict(color=rel_err(pixels(c, ours["color"]), pixels(c, ref["color"])), depth=rel_err(pixels(c, ours["depth"]), pixels(c, ref["depth"])),
              g_alpha=rel_err(ours["g_alpha"], ref["g_alpha"]),
              g_rgb=float(np.max(np.abs(ours["g_rgb"].astype(np.float64) - ref["g_rgb"]))) / S)
     if ref["g_bg"] is not None:
         e["g_bg"] = float(np.max(np.abs(ours["g_bg"].astype(np.float64) - ref["g_bg"]))) / S
-        if c["visible"]:
+        if c.get("visible"):
             e["g_bg_own"] = rel_err(ours["g_bg"], ref["g_bg"])
     return e
 
@@ -322,14 +173,6 @@ def check(label, ours, name, with_bg, plan_=None):
 # ------------------------------------------------------------------------------------------------------------------------------
 # running the factored render
 # ------------------------------------------------------------------------------------------------------------------------------
-def _dev_tensors(c, with_bg):
-    d = dev()
-    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(d)
-    mpi = (t(c["rgb"]), t(c["alpha"]), t(c["bg"]) if with_bg else None)
-    geo = tuple(t(c[k]) for k in ("dhw", "view2mpi", "ray_dir", "eye", "z_dir"))
-    return mpi, geo
-
-
 def fwd_plan(c, mpi, view_group=1):
     V, _, H, W = c["ray_dir"].shape
     M, N, _, Ht, Wt = c["alpha"].shape
@@ -343,9 +186,9 @@ def run(name, with_bg, mpi=None, view_group=1):
     backward.  mpi: (rgb, alpha, bg_rgb) device tensors to render instead of the case's (their storage is kept)."""
     c = case(name)
     d = dev()
-    base, geo = _dev_tensors(c, with_bg)
+    base, geo = _mpi(c, with_bg), on_device(c, *GEOMETRY)
     mpi = base if mpi is None else mpi
-    kw = dict(align_corners=c["ac"], check_last_plane=True, color_minus1_1=c["m11"], view_group=view_group)
+    kw = dict(align_corners=c["ac"], check_last_plane=True, color_minus1_1=c.get("m11", False), view_group=view_group)
     flags = lambda: torch.zeros(1, dtype=torch.int32, device=d)
     x = g.expand_factored(*base)
     if any(t is not None and t.data_ptr() % 16 for t in mpi):
@@ -364,10 +207,10 @@ def run(name, with_bg, mpi=None, view_group=1):
     assert_bitwise((col, dep), (ce2, de2), (name, "training forward != expanded"))
     assert_bitwise((col, dep), (cf, df), (name, "training forward != forward-only kernel"))
     del ce2, de2, xe, x
-    gc = torch.from_numpy(c["gc"]).to(d)
+    gc, gd = on_device(c, "gc", "gd")
     loss = (col * gc).sum()
-    if c["gd"] is not None:
-        loss = loss + (dep * torch.from_numpy(c["gd"]).to(d)).sum()
+    if gd is not None:
+        loss = loss + (dep * gd).sum()
     loss.backward()
     out = dict(color=to_np(col), depth=to_np(dep), flags=int(ft.item()), g_rgb=to_np(leaves[0].grad), g_alpha=to_np(leaves[1].grad),
                g_bg=to_np(leaves[2].grad) if with_bg else None)
@@ -391,7 +234,7 @@ def _matrix_params():
 @pytest.mark.parametrize("name,with_bg", list(_matrix_params()))
 def test_factored_matches_the_oracle(name, with_bg, variant):
     c = case(name)
-    mpi, _ = _dev_tensors(c, with_bg)
+    mpi = _mpi(c, with_bg)
     Wt = c["alpha"].shape[-1]
     p, why = fwd_plan(c, mpi)
     if variant == "direct":
@@ -401,19 +244,13 @@ def test_factored_matches_the_oracle(name, with_bg, variant):
     else:
         assert p == "staged", why
     if name == "band_89_96":
-        assert limit_footprints(_shim(c), 89, 96) > 0
+        assert limit_footprints(c, 89, 96) > 0
     if name == "wider_than_96":
-        assert limit_footprints(_shim(c), 97, 1 << 30) > 0
+        assert limit_footprints(c, 97, 1 << 30) > 0
     ours = run(name, with_bg)
     if name == "N1" and with_bg:
         assert not ours["g_rgb"].any()              # the one plane is the background: nothing reaches rgb
     check(f"{name}/{'bg' if with_bg else 'nobg'}/{variant}", ours, name, with_bg, p)
-
-
-def _shim(c):
-    """c as testlib.limit_footprints reads it (it takes the sizes from an expanded stack)."""
-    M, N, _, Ht, Wt = c["alpha"].shape
-    return dict(c, rgba=np.broadcast_to(np.float32(0), (M, N, 4, Ht, Wt)))
 
 
 # ------------------------------------------------------------------------------------------------------------------------------
@@ -442,11 +279,11 @@ def test_one_tile_per_mpi_factored_gradients_are_bitwise_the_expanded_ones():
 # ------------------------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("order", ["sorted", "interleaved", "reversed"])
 def test_zero_grad_poisoned_buffers_any_view_order(order, variant):
-    name = "abi_" + order
+    name = "three_mpis_" + order
     c = case(name)
     d = dev()
     lib = _lib.load()
-    (rgb, alpha, bg), (dhw, v2m, ray, eye, z) = _dev_tensors(c, True)
+    (rgb, alpha, bg), (dhw, v2m, ray, eye, z) = _mpi(c, True), on_device(c, *GEOMETRY)
     M, N, _, Ht, Wt = alpha.shape
     V, _, H, W = ray.shape
     opt = _lib.OPT_ALIGN_CORNERS | _lib.OPT_CHECK_LAST_PLANE
@@ -457,7 +294,7 @@ def test_zero_grad_poisoned_buffers_any_view_order(order, variant):
                   z_dir=z, stream=torch.cuda.current_stream(d).cuda_stream)
     _lib.check(lib.gmpi_mpi_render_fwd_ex(ctypes.byref(_lib.make_desc(options=opt, color=color, depth=depth, transmittance=trans,
                                                                       flags=flags, **common))))
-    gc, gd = torch.from_numpy(c["gc"]).to(d), torch.from_numpy(c["gd"]).to(d)
+    gc, gd = on_device(c, "gc", "gd")
 
     def bwd(fill, options):
         gr, ga, gb = torch.full_like(rgb, fill), torch.full_like(alpha, fill), torch.full_like(bg, fill)
@@ -496,9 +333,9 @@ def test_view_group_changes_no_output_bit_and_no_gradient_beyond_the_bar(variant
 
 @pytest.mark.parametrize("which", ["rgb", "alpha", "bg_rgb"])
 def test_one_unaligned_factor_takes_the_direct_kernels(which, variant):
-    name = "small"
+    name = "small_12x96"
     c = case(name)
-    mpi, _ = _dev_tensors(c, True)
+    mpi = _mpi(c, True)
     i = ["rgb", "alpha", "bg_rgb"].index(which)
     mpi = tuple(misaligned(t, 4) if j == i else t for j, t in enumerate(mpi))
     p, why = fwd_plan(c, mpi)
@@ -508,7 +345,7 @@ def test_one_unaligned_factor_takes_the_direct_kernels(which, variant):
 
 @pytest.mark.parametrize("with_bg", [False, True])
 def test_host_entry_point_with_ray_tensors_is_bitwise_the_device_call(with_bg, variant):
-    name = "small"
+    name = "small_12x96"
     c = case(name)
     d = dev()
     lib = _lib.load()
@@ -541,7 +378,7 @@ def test_the_bars_fail_on_a_slightly_wrong_problem(variant):
     """The kernel's result on the right problem, checked with the same helpers against the oracle of a slightly wrong one (and, for
     the visibility check, with the background's gradient moved to d rgb): each must fail some bar by 10x or more, and every bar must
     fail by 10x somewhere -- so the matrix above would catch a kernel that made any of these mistakes."""
-    name = "small"
+    name = "small_12x96"
     c = case(name)
     ours = run(name, True)
     right = reference(name, True)

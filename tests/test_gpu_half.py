@@ -15,7 +15,7 @@ import ml_gmpi_b200 as g
 from ml_gmpi_b200 import _lib, synth
 from ml_gmpi_b200.camera import cam_params
 from testlib import (CASES, assert_bitwise, assert_class_88_behind_plane_25, case, dev, forced_kernel, forward_desc, headline_case,
-                     kernel_fixture, limit_case, limit_footprints, misaligned, native_vs_fp32, render_fwd)
+                     kernel_fixture, limit_footprints, misaligned, native_vs_fp32, render_fwd)
 
 pytestmark = pytest.mark.gpu
 TAUS = [None, 0.0, 2.0 ** -24, 1e-3]
@@ -26,9 +26,8 @@ def _mpi(c, half, bg=True, misalign=False):
     """The case's MPI on the device: fp16 (half) or the fp32 upcast of that fp16 MPI."""
     d = dev()
     q = lambda a: (lambda h: h if half else h.float())(torch.from_numpy(np.ascontiguousarray(a)).to(d).half())
-    if "factored" in c:
-        rgb, alpha, bg_rgb = c["factored"]
-        m = dict(rgb=q(rgb), alpha=q(alpha), bg_rgb=q(bg_rgb) if bg else None)
+    if c.get("factored"):
+        m = dict(rgb=q(c["rgb"]), alpha=q(c["alpha"]), bg_rgb=q(c["bg"]) if bg else None)
     else:
         m = dict(rgba=q(c["rgba"]))
     if misalign:
@@ -47,7 +46,7 @@ def test_fp16_render_is_bitwise_the_upcast_render(name, variant):
     partial tiles, N = 1 / 2 / 512, view_group > 1, uint8 video with both roundings) with early stop off and at tau = 0, 2^-24,
     1e-3: colour, depth and flags bitwise."""
     c = case(name)
-    extra = [dict(bg=False)] if "factored" in c else [dict(u8_round=True)] if c.get("video") else []
+    extra = [dict(bg=False)] if c.get("factored") else [dict(u8_round=True)] if c.get("video") else []
     for kw in [{}] + extra:
         for tau in TAUS:
             h, f, _ = run_pair(c, variant, tau=tau, **kw)
@@ -100,8 +99,7 @@ def test_host_entry_point_takes_fp16_host_buffers(name):
     outs = []
     for half in (True, False):
         conv = lambda a: np.ascontiguousarray(a.astype(np.float16) if half else a.astype(np.float16).astype(np.float32))
-        mpi = dict(rgb=conv(c["factored"][0]), alpha=conv(c["factored"][1]), bg_rgb=conv(c["factored"][2])) \
-            if "factored" in c else dict(rgba=conv(c["rgba"]))
+        mpi = dict(rgb=conv(c["rgb"]), alpha=conv(c["alpha"]), bg_rgb=conv(c["bg"])) if c.get("factored") else dict(rgba=conv(c["rgba"]))
         ref = mpi.get("alpha", mpi.get("rgba"))
         h = {k: np.ascontiguousarray(c[k]) for k in ("view2mpi", "dhw", "ray_dir", "eye", "z_dir")}
         flags = np.zeros(1, np.uint32)
@@ -238,7 +236,7 @@ def test_fp16_at_the_widest_box_classes(factored, stages):
         assert_class_88_behind_plane_25(c)
         factored = False
     else:
-        c = limit_case(factored)
+        c = dict(case("band_89_96"), factored=factored)      # the factored forward renders its factors
         assert limit_footprints(c, 85, 88) > 0 and (not factored or limit_footprints(c, 93, 96) > 0)
     with forced_kernel(stages):
         for kw in ([{}, dict(bg=False)] if factored else [{}]):

@@ -14,7 +14,8 @@ import mpi_oracle
 import ml_gmpi_b200 as g
 from ml_gmpi_b200 import _lib
 from conftest import MPI_CASES, load_golden, rel_err
-from testlib import EXPECT, dev, each_alpha, kernel_fixture, oracle_backward, oracle_forward, to_np, upstream
+from testlib import (C4_YAWS, EXPECT, FULL, GEOMETRY, case, dev, each_alpha, kernel_fixture, on_device, oracle_backward, oracle_forward,
+                     pixels, to_np, upstream)
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-4          # the north star's bar
@@ -189,20 +190,9 @@ def _ffhq_case(N, res, V, seed=1234, device=None):
     return synth.make_case(n_planes=N, tex=res, img=res, n_mpi=V, seed=seed, device=device)
 
 
-# The full-size cases run on two MPIs: U(0, 1) alpha, and equal-weight alpha (synth.equal_weight_alpha).  Under U(0, 1) alpha the
-# transmittance falls as e^-i and planes past ~25 move the render and its gradient by less than the bar, so only the equal-weight
-# MPI checks the back planes, where the widest box classes occur (tests/test_every_plane_weight.py).
-_C4_YAWS = np.linspace(0.5, -0.5, 120).astype(np.float32)[::8]
-FULL = {   # name: synth.make_case arguments
-    "full_32x256": dict(n_planes=32, tex=256, img=256, n_mpi=8, seed=1234),
-    "full_96x512": dict(n_planes=96, tex=512, img=512, n_mpi=2, seed=1234),
-    "full_96x1024": dict(n_planes=96, tex=1024, img=1024, n_mpi=1, seed=1234),
-    "c3": dict(n_planes=96, tex=1024, img=1024, n_mpi=1, seed=1234, last_alpha_one=True),
-    "ffhq1024_batch4": dict(n_planes=96, tex=1024, img=1024, n_mpi=4, seed=1234, last_alpha_one=True),   # bench.py's batch: 6.4 GB
-    "c5": dict(n_planes=96, tex=512, img=512, n_mpi=4, seed=99, last_alpha_one=True),
-    "four_views": dict(n_planes=48, tex=512, img=512, n_mpi=1, views_per_mpi=4, seed=21, last_alpha_one=True),
-    "c4_video": dict(n_planes=96, tex=512, img=512, n_mpi=1, views_per_mpi=15, seed=1234, yaws=_C4_YAWS, pitches=np.zeros(15, np.float32)),
-}
+# The full-size cases (testlib.FULL) run on two MPIs: U(0, 1) alpha, and equal-weight alpha (synth.equal_weight_alpha).  Under U(0, 1)
+# alpha the transmittance falls as e^-i and planes past ~25 move the render and its gradient by less than the bar, so only the
+# equal-weight MPI checks the back planes, where the widest box classes occur (tests/test_every_plane_weight.py).
 
 
 def _full_case(name, alpha):
@@ -279,32 +269,17 @@ def test_backward_96_planes_small_image_shared_mpi_vs_oracle(fwd_variant):
 
 def test_staged_falls_back_per_thread_for_non_projective_rays(fwd_variant):
     """The staged kernel estimates a tile's texel footprint from its corner rays.  With rays that are NOT a pinhole
-    camera's (here: shuffled within the image), taps fall outside the staged box and every such thread must take the
-    direct-sampling fallback: results stay exact."""
-    d = dev()
-    from ml_gmpi_b200 import synth
-    case = synth.make_case(n_planes=12, tex=96, img=200, n_mpi=1, views_per_mpi=2, seed=3, device=d)   # 200 = partial tiles
-    gen = torch.Generator(device="cpu").manual_seed(0)
-    perm = torch.randperm(200 * 200, generator=gen).to(d)
-    ray = case.ray_dir.reshape(2, 3, -1)[:, :, perm].reshape(2, 3, 200, 200).contiguous()
-    color, depth = g.render_views(case.rgba, case.dhw, case.view2mpi, ray, case.eye, case.z_dir)
-    rc, rd, _ = oracle_forward(case, ray_dir=ray)
-    assert rel_err(to_np(color), rc) <= EXPECT and rel_err(to_np(depth), rd) <= EXPECT
+    camera's (here: shuffled within the image, 200^2 pixels: partial tiles), taps fall outside the staged box and every such thread
+    must take the direct-sampling fallback: results stay exact."""
+    _edge_vs_oracle("shuffled_rays")
 
 
 def test_degenerate_rays_do_not_poison_neighbours(fwd_variant):
-    """ray_z == 0 (ray parallel to the planes) makes scale inf/NaN for that pixel only."""
-    d = dev()
-    from ml_gmpi_b200 import synth
-    case = synth.make_case(n_planes=8, tex=64, img=64, n_mpi=1, seed=4, device=d)
-    ray = case.ray_dir.clone()
-    ray[0, 2, 10, 10:14] = 0.0
-    ray[0, :, 20, 20] = float("nan")
-    color, depth = g.render_views(case.rgba, case.dhw, case.view2mpi, ray, case.eye, case.z_dir)
-    rc, rd, _ = oracle_forward(case, ray_dir=ray)
-    ok = np.ones((64, 64), bool); ok[10, 10:14] = False; ok[20, 20] = False
-    assert rel_err(to_np(color)[0][:, ok], rc[0][:, ok]) <= EXPECT
-    assert np.all(to_np(color)[0][:, 10, 10:14] == 0) and np.all(rc[0][:, 10, 10:14] == 0)
+    """ray_z == 0 (ray parallel to the planes) makes scale inf/NaN for that pixel only; those pixels render 0."""
+    c = case("degenerate_rays")
+    color, rc = _edge_vs_oracle("degenerate_rays")
+    parallel = c["ray_dir"][:, 2] == 0                         # [V,H,W]
+    assert parallel.any() and np.all(color.transpose(1, 0, 2, 3)[:, parallel] == 0) and np.all(rc.transpose(1, 0, 2, 3)[:, parallel] == 0)
 
 
 def test_renderer_facade_matches_reference_render():
@@ -471,7 +446,7 @@ def test_the_bars_fail_on_a_slightly_wrong_problem():
 def test_full_size_forward_c4_video_every_view_vs_oracle(fwd_variant_auto, alpha):
     """BASELINE configs[3] shape: ONE 96-plane 512^2 MPI, 15 views (one rank's share of the 120) spread over the whole
     yaw = linspace(0.5, -0.5, 120) sweep, pitch 0 (render_video.py:95-107); every view against the oracle."""
-    assert len(_C4_YAWS) == 15
+    assert len(C4_YAWS) == 15
     case = _full_case("c4_video", alpha)
     color, depth = g.render_views(case.rgba, case.dhw, case.view2mpi, case.ray_dir, case.eye, case.z_dir, check_last_plane=True)
     rc, rd = _oracle_forward("c4_video", alpha)
@@ -483,23 +458,8 @@ def test_non_projective_rays_outside_the_corner_box_still_render(fwd_variant):
     """ADVICE r1: the producer's "nothing under the tile" (mode 1) comes from the four corner rays only.  Rays that are not a
     pinhole camera's can have all four tile corners miss the texture while interior pixels hit it: those pixels must still
     be rendered (and get gradient), exactly as the direct kernel and the oracle do."""
-    from ml_gmpi_b200 import synth
-    d = dev()
-    case = synth.make_case(n_planes=6, tex=64, img=128, n_mpi=1, views_per_mpi=2, seed=9, device=d)   # 2x5 tiles per view
-    ray = case.ray_dir.clone()
-    # push the corner pixels of every 64x30 tile far outside the planes, keep the interior as it is
-    for ty in range(0, 128, 30):
-        for tx in range(0, 128, 64):
-            for (cy, cx) in ((ty, tx), (ty, min(tx + 63, 127)), (min(ty + 29, 127), tx), (min(ty + 29, 127), min(tx + 63, 127))):
-                ray[:, 0, cy, cx] = 5.0
-    rgba = case.rgba.clone().requires_grad_(True)
-    color, depth = g.render_views(rgba, case.dhw, case.view2mpi, ray, case.eye, case.z_dir)
-    gc, _ = upstream(2, 128, 128, 2, depth=False, device=d)
-    (color * gc).sum().backward()
-    rc, rd, _ = oracle_forward(case, ray_dir=ray)
+    _, rc = _edge_vs_oracle("corners_off_the_planes")
     assert float(np.abs(rc).max()) > 0.1                       # the interior really renders something
-    assert rel_err(to_np(color), rc) <= EXPECT and rel_err(to_np(depth), rd) <= EXPECT
-    assert rel_err(to_np(rgba.grad), oracle_backward(case, gc, ray_dir=ray)) <= EXPECT
 
 
 def test_plan_query_names_the_direct_kernel_cliffs():
@@ -534,53 +494,38 @@ def test_backward_twice_and_interleaved_graphs_use_fresh_gradient_buffers():
     assert float(g1.abs().max()) > 0
 
 
-def _bwd_c_abi(case, trans, gc, gdp, g_rgba, options):
-    """gmpi_mpi_render_bwd_ex straight through the C ABI into a caller-owned gradient buffer."""
-    import ctypes
-    from ml_gmpi_b200 import _lib
-    lib = _lib.load()
-    M, N, _, Ht, Wt = case.rgba.shape
-    V, _, H, W = case.ray_dir.shape
-    d = _lib.make_desc(options=options, M=M, V=V, N=N, Ht=Ht, Wt=Wt, H=H, W=W, rgba=case.rgba, view2mpi=case.view2mpi, dhw=case.dhw,
-                       ray_dir=case.ray_dir, eye=case.eye, z_dir=case.z_dir, transmittance=trans, g_color=gc, g_depth=gdp,
-                       g_rgba=g_rgba, stream=torch.cuda.current_stream(case.rgba.device).cuda_stream)
-    _lib.check(lib.gmpi_mpi_render_bwd_ex(ctypes.byref(d)))
-    torch.cuda.synchronize()
-
-
 @pytest.mark.parametrize("order", ["sorted", "interleaved", "reversed"])
 def test_zero_grad_poisoned_buffer_any_view_order(order):
     """GMPI_ZERO_GRAD on the staged backward.  The buffer arrives full of NaN; views of three MPIs come sorted by MPI (MPI.forward's
-    layout), interleaved or reversed; the result must equal the oracle."""
+    layout), interleaved or reversed, and a fourth MPI has no view; the result must equal the oracle."""
     import ctypes
-    from ml_gmpi_b200 import synth, _lib
     lib = _lib.load()
     d = dev()
-    case = synth.make_case(n_planes=12, tex=256, img=256, n_mpi=3, views_per_mpi=2, seed=77, device=d, last_alpha_one=True)
-    perm = {"sorted": [0, 1, 2, 3, 4, 5], "interleaved": [0, 2, 4, 1, 3, 5], "reversed": [5, 4, 3, 2, 1, 0]}[order]
-    pi = torch.tensor(perm, device=d)
-    import dataclasses
-    case = dataclasses.replace(case, view2mpi=case.view2mpi[pi].contiguous(), ray_dir=case.ray_dir[pi].contiguous(),
-                               eye=case.eye[pi].contiguous(), z_dir=case.z_dir[pi].contiguous())
-    M, N, _, Ht, Wt = case.rgba.shape
-    V, _, H, W = case.ray_dir.shape
+    c = case("three_mpis_" + order)
+    rgba, gc, gdp = on_device(c, "rgba", "gc", "gd")
+    geo = dict(zip(GEOMETRY, on_device(c, *GEOMETRY)))
+    M, N, _, Ht, Wt = rgba.shape
+    V, _, H, W = geo["ray_dir"].shape
     opt = _lib.OPT_ALIGN_CORNERS
-    color, depth = torch.empty((V, 3, H, W), device=d), torch.empty((V, 1, H, W), device=d)
-    trans = torch.empty((V, N, H, W), device=d)
-    flags = torch.zeros(1, dtype=torch.int32, device=d)
-    fd = _lib.make_desc(options=opt, M=M, V=V, N=N, Ht=Ht, Wt=Wt, H=H, W=W, rgba=case.rgba, view2mpi=case.view2mpi, dhw=case.dhw,
-                        ray_dir=case.ray_dir, eye=case.eye, z_dir=case.z_dir, color=color, depth=depth, transmittance=trans, flags=flags,
-                        stream=torch.cuda.current_stream(d).cuda_stream)
+    common = dict(M=M, V=V, N=N, Ht=Ht, Wt=Wt, H=H, W=W, rgba=rgba, transmittance=torch.empty((V, N, H, W), device=d),
+                  stream=torch.cuda.current_stream(d).cuda_stream, **geo)
+    fd = _lib.make_desc(options=opt, color=torch.empty((V, 3, H, W), device=d), depth=torch.empty((V, 1, H, W), device=d),
+                        flags=torch.zeros(1, dtype=torch.int32, device=d), **common)
     _lib.check(lib.gmpi_mpi_render_fwd_ex(ctypes.byref(fd)))
-    gc, gdp = upstream(V, H, W, 9, device=d)
-    ref = oracle_backward(case, gc, gdp)
-    gbuf = torch.full_like(case.rgba, float("nan"))
-    _bwd_c_abi(case, trans, gc, gdp, gbuf, opt | _lib.OPT_ZERO_GRAD)
+    ref = oracle_backward(c, c["gc"], c["gd"])
+
+    def bwd(g_rgba, options):
+        """gmpi_mpi_render_bwd_ex straight through the C ABI into a caller-owned gradient buffer."""
+        _lib.check(lib.gmpi_mpi_render_bwd_ex(ctypes.byref(_lib.make_desc(options=options, g_color=gc, g_depth=gdp, g_rgba=g_rgba,
+                                                                          **common))))
+        torch.cuda.synchronize()
+        return g_rgba
+
+    gbuf = bwd(torch.full_like(rgba, float("nan")), opt | _lib.OPT_ZERO_GRAD)
     assert bool(torch.isfinite(gbuf).all()), "poison survived"
     assert rel_err(to_np(gbuf), ref) <= 2e-5
     # without GMPI_ZERO_GRAD the kernel accumulates into what it is given
-    gacc = torch.ones_like(case.rgba)
-    _bwd_c_abi(case, trans, gc, gdp, gacc, opt)
+    gacc = bwd(torch.ones_like(rgba), opt)
     assert rel_err(to_np(gacc) - 1.0, ref) <= 2e-5
 
 
@@ -598,49 +543,44 @@ def test_zero_grad_one_mpi_many_views_poisoned_allocator_block():
 # Shapes at the edges of the staged forward's ring (fwd_variant runs each at both ring depths): one plane, kMaxPlanesStaged = 512
 # planes (the plane table then ends the shared-memory allocation of either depth), partial tiles with align_corners=False
 # ------------------------------------------------------------------------------------------------------------------------------
-def _fwd_bwd_vs_oracle(rgba, case, ray, align_corners=True, seed=0):
-    d = rgba.device
-    x = rgba.clone().requires_grad_(True)
-    color, depth = g.render_views(x, case.dhw, case.view2mpi, ray, case.eye, case.z_dir, align_corners=align_corners,
-                                  check_last_plane=True)
-    V, _, H, W = color.shape
-    gc, gdp = upstream(V, H, W, seed, device=d)
-    ((color * gc).sum() + (depth * gdp).sum()).backward()
-    rc, rd, _ = oracle_forward(case, rgba=rgba, ray_dir=ray, align_corners=align_corners)
-    assert rel_err(to_np(color), rc) <= EXPECT and rel_err(to_np(depth), rd) <= EXPECT
-    ref = oracle_backward(case, gc, gdp, rgba=rgba, ray_dir=ray, align_corners=align_corners)
+@functools.lru_cache(maxsize=1)
+def _edge_oracle(name):
+    """The oracle's (colour, depth, d rgba) of a catalogue case, once for all the kernels a test runs."""
+    c = case(name)
+    rc, rd, _ = oracle_forward(c, align_corners=c["ac"])
+    return rc, rd, oracle_backward(c, c["gc"], c["gd"], align_corners=c["ac"])
+
+
+def _edge_vs_oracle(name):
+    """Colour and depth (at the pixels the case checks) and d rgba under the case's upstream gradients, against the oracle.
+    Returns (colour, the oracle's colour) as numpy."""
+    c = case(name)
+    rgba, gc, gdp = on_device(c, "rgba", "gc", "gd")
+    x = rgba.requires_grad_(True)
+    color, depth = g.render_views(x, *on_device(c, *GEOMETRY), align_corners=c["ac"], check_last_plane=True)
+    loss = (color * gc).sum()
+    if gdp is not None:
+        loss = loss + (depth * gdp).sum()
+    loss.backward()
+    rc, rd, ref = _edge_oracle(name)
+    assert rel_err(pixels(c, to_np(color)), pixels(c, rc)) <= EXPECT and rel_err(pixels(c, to_np(depth)), pixels(c, rd)) <= EXPECT
     assert rel_err(to_np(x.grad), ref) <= EXPECT
+    return to_np(color), rc
 
 
 def test_single_plane_vs_oracle(fwd_variant):
-    from ml_gmpi_b200 import synth
-    import dataclasses
-    case = synth.make_case(n_planes=8, tex=128, img=160, n_mpi=2, seed=41, device=dev())
-    case = dataclasses.replace(case, rgba=case.rgba[:, 3:4].contiguous(), dhw=case.dhw[:, 3:4].contiguous())
-    _fwd_bwd_vs_oracle(case.rgba, case, case.ray_dir, seed=1)
+    _edge_vs_oracle("N1")
 
 
 def test_512_planes_vs_oracle(fwd_variant):
     """N = kMaxPlanesStaged, 96^2 textures at 128^2.  Alpha is scaled down so that the back planes still show through."""
-    from ml_gmpi_b200 import synth
-    case = synth.make_case(n_planes=512, tex=96, img=128, n_mpi=2, seed=43, device=dev())
-    rgba = case.rgba.clone()
-    rgba[:, :, 3] *= 0.02
-    rgba[:, -1, 3] = 1.0
-    _fwd_bwd_vs_oracle(rgba, case, case.ray_dir, seed=2)
+    _edge_vs_oracle("N512")
 
 
 def test_partial_tiles_align_corners_false_nonsquare_vs_oracle(fwd_variant):
     """100 x 136 pixels (partial tiles in both directions for the forward's 64 x 30 and the backward's 64 x 24 tiles) cut out of
     a pinhole image, 72 x 116 textures, align_corners=False."""
-    from ml_gmpi_b200 import synth
-    d = dev()
-    case = synth.make_case(n_planes=10, tex=8, img=136, n_mpi=2, views_per_mpi=2, seed=47, device=d, rgba=False)
-    gen = torch.Generator(device=d).manual_seed(47)
-    rgba = torch.rand((2, 10, 4, 72, 116), generator=gen, device=d)
-    rgba[:, -1, 3] = 1.0
-    ray = case.ray_dir[:, :, 18:118].contiguous()
-    _fwd_bwd_vs_oracle(rgba, case, ray, align_corners=False, seed=3)
+    _edge_vs_oracle("partial_acfalse_nonsquare")
 
 
 def test_ring_depth_policy():

@@ -17,7 +17,7 @@ from ml_gmpi_b200 import _lib, synth
 from ml_gmpi_b200.camera import cam_params
 from conftest import ROOT
 from testlib import (CASES, assert_bitwise, assert_class_88_behind_plane_25, case, dev, early_stop_stats, footprints, forced_kernel,
-                     forward_desc, headline_case, kernel_fixture, limit_case, misaligned, native_vs_fp32, render_fwd, skip_stats)
+                     forward_desc, headline_case, kernel_fixture, misaligned, native_vs_fp32, render_fwd, skip_stats)
 
 pytestmark = pytest.mark.gpu
 TAUS = [None, 0.0, 2.0 ** -24, 1e-3]
@@ -137,7 +137,7 @@ def test_u8_at_the_widest_box_class_at_every_shift(stages, shape):
     """Footprints at the widest class (width need 81..88, class 88) whose fp32 box starts 0, 4, 8 and 12 texels past a multiple of 16:
     the uint8 kernel stages a 112-wide box from that multiple and decides fast / generic body exactly as fp32 does.  "headline": 96 x
     1024^2 with equal-weight alpha, where those footprints lie on planes that reach the render."""
-    c = limit_case(False) if shape == "limit" else headline_case()
+    c = case("band_89_96") if shape == "limit" else headline_case()
     counts = _shift_footprints(c, 81, 88)
     assert all(n > 0 for n in counts.values()), counts
     if shape == "headline":

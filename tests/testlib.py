@@ -5,7 +5,11 @@
   forced_kernel, kernel_fixture   fixture that runs a test once per kernel
   misaligned, assert_bitwise      a copy at a given offset from a 16-byte boundary; dtype, shape and bytes equal
   early_stop_stats, skip_stats    the stage counters of the last staged forward
-  case, CASES                     the forward tests' catalogue: the golden fixtures and the synthetic cases
+  case, synth_case, golden_case,  the case catalogue: every case of the GPU tests' edges as one record (geometry, expanded and
+  CASES, FULL, on_device, pixels  factored MPI, upstream gradients); the forward tests' cases; the full-size shapes; a case's
+                                  arrays on the device; the pixels a check compares
+  shuffled_rays, corners_off,     the ray perturbations of the edge cases, and the views of a case in another order
+  degenerate_rays, view_order
   forward_desc, render_fwd,       one gmpi_mpi_render_fwd_ex of a catalogue case, and the render of a native (fp16 / uint8) MPI
   native_vs_fp32                  beside the fp32 MPI it stands for, on the same kernel
   BIG_*, big_views                the shapes, views and declared device peaks of the buffers past 2^31 elements
@@ -14,7 +18,7 @@
   upstream, oracle_forward,       the upstream gradients of a backward test; the oracle's forward and backward of a case; its
   oracle_backward, factored_refs, gradient split into a factored MPI's (d rgb, d alpha, d bg_rgb), and the check of a factored
   check_factored                  backward against it
-and the helpers several modules read: the machine code of the built library, the staged forward's footprints and its limit cases,
+and the helpers several modules read: the machine code of the built library, the staged forward's footprints,
 oracle-side bounds and references, and the flag cases of tests/golden/flags_edges.npz."""
 import contextlib
 import ctypes
@@ -131,45 +135,182 @@ def skip_stats():
 
 
 # ------------------------------------------------------------------------------------------------------------------------------
-# the case catalogue of the forward tests: numpy inputs of a render, the factors of a factored case, video and view-group settings
+# the case catalogue: every case of the GPU tests' edges, as one record of numpy arrays, built once
 # ------------------------------------------------------------------------------------------------------------------------------
+# A record holds the geometry (view2mpi, dhw, ray_dir, eye, z_dir, ac: align_corners, view_group); an expanded MPI rgba with its own
+# colour on every plane; a factored MPI (rgb, alpha, bg) over the same texture, whose alpha is rgba's; the upstream gradients of a
+# backward (gc, and gd or None without a depth gradient).  Optional fields: factored (the forward tests render the factors: rgba is
+# then their expanded stack), video (uint8 video frames), m11 (colour in [-1, 1]), visible (the background shows through: the
+# alphas in front of the last plane are scaled down), ok ([V,H,W]: the pixels the checks compare; the others get no upstream
+# gradient), and for the golden fixtures the reference's colour and depth.
+GEOMETRY = ("dhw", "view2mpi", "ray_dir", "eye", "z_dir")      # in the order render_views takes them
+
+
 def golden_case(name):
+    """A golden fixture as a record: its inputs, the reference's colour and depth, its upstream gradients; the factored MPI is
+    plane 0's colour, every plane's alpha and the last plane's colour."""
     gd = load_golden(name)
-    return dict(rgba=gd["rgba"], view2mpi=gd["view2mpi"], dhw=gd["dhw"], ray_dir=gd["ray_dir"], eye=gd["eye"], z_dir=gd["z_dir"],
-                ac=bool(gd["align_corners"]))
+    rgba = gd["rgba"]
+    return dict({k: gd[k] for k in ("rgba", "view2mpi", "dhw", "ray_dir", "eye", "z_dir", "color", "depth")}, ac=bool(gd["align_corners"]),
+                rgb=rgba[:, 0, :3].copy(), alpha=rgba[:, :, 3:4].copy(), bg=rgba[:, -1, :3].copy(), gc=gd["g_color"], gd=gd.get("g_depth"))
 
 
-def synth_case(n_planes, tex, img, n_mpi, views=1, seed=0, alpha_scale=None, crop=None, tex_hw=None, ac=True, view_group=1,
-               factored=False, video=False):
-    case = synth.make_case(n_planes=n_planes, tex=tex, img=img, n_mpi=n_mpi, views_per_mpi=views, seed=seed, last_alpha_one=True)
-    rgba = case.rgba
-    if tex_hw is not None:
-        rgba = torch.rand((n_mpi, n_planes, 4) + tex_hw, generator=torch.Generator().manual_seed(seed))
-        rgba[:, -1, 3] = 1.0
+def synth_case(*, n_planes, tex, img, n_mpi, views_per_mpi=1, seed, last_alpha_one=True, alpha="uniform", yaws=None, pitches=None,
+               tex_hw=None, alpha_scale=None, plane=None, crop=None, rays=None, extra_mpis=0, ac=True, view_group=1, factored=False,
+               video=False, depth_grad=True, m11=False, visible=False):
+    """A record of synth.make_case's geometry (its first arguments, FULL's keys) and an MPI drawn as make_case draws it, U(0, 1) from
+    a CPU generator seeded with `seed` (alpha: "uniform", or "equal_weight", synth.equal_weight_alpha), [n_mpi + extra_mpis, n_planes,
+    4, *tex_hw] (tex_hw: (tex, tex)); alpha_scale scales the alphas in front of the last plane.  rgb and bg are drawn from seed + 1.
+    plane: take plane `plane` of an n_planes table (then the MPI has one plane); crop: rows crop[0]:crop[1] of the image; rays: a
+    function of the ray tensor (shuffled_rays, corners_off, degenerate_rays); extra_mpis: MPIs that no view looks at.  The upstream
+    gradients are upstream(V, H, W, seed, depth_grad)."""
+    geo = synth.make_case(n_planes=n_planes, tex=8, img=img, n_mpi=n_mpi, views_per_mpi=views_per_mpi, seed=seed, yaws=yaws,
+                          pitches=pitches, rgba=False)
+    dhw = geo.dhw if plane is None else geo.dhw[:, plane:plane + 1]
+    M, N, tex_hw = n_mpi + extra_mpis, dhw.shape[1], tex_hw or (tex, tex)
+    gen = torch.Generator().manual_seed(seed)
+    rgba = torch.rand((M, N, 4) + tex_hw, generator=gen)
+    if alpha == "equal_weight":
+        rgba[:, :, 3] = synth.equal_weight_alpha((M, N) + tex_hw, gen)
     if alpha_scale is not None:
-        rgba = rgba.clone()
         rgba[:, :-1, 3] *= alpha_scale
-    ray = case.ray_dir if crop is None else case.ray_dir[:, :, crop[0]:crop[1]].contiguous()
-    c = dict(rgba=rgba.numpy(), view2mpi=case.view2mpi.numpy(), dhw=case.dhw.numpy(), ray_dir=ray.numpy(), eye=case.eye.numpy(),
-             z_dir=case.z_dir.numpy(), ac=ac, view_group=view_group, video=video)
+    if last_alpha_one:
+        rgba[:, -1, 3] = 1.0
+    gen = torch.Generator().manual_seed(seed + 1)
+    rgb, bg = torch.rand((M, 3) + tex_hw, generator=gen), torch.rand((M, 3) + tex_hw, generator=gen)
+    alpha = rgba[:, :, 3:4].contiguous()
     if factored:      # one shared colour image, the last plane's own colour, per-plane alpha
-        gen = torch.Generator().manual_seed(seed + 1)
-        rgb, bg = torch.rand((n_mpi, 3) + rgba.shape[-2:], generator=gen), torch.rand((n_mpi, 3) + rgba.shape[-2:], generator=gen)
-        alpha = torch.from_numpy(c["rgba"][:, :, 3:4].copy())
-        c.update(factored=(rgb.numpy(), alpha.numpy(), bg.numpy()), rgba=g.expand_factored(rgb, alpha, bg).numpy())
+        rgba = g.expand_factored(rgb, alpha, bg)
+    ray = geo.ray_dir if crop is None else geo.ray_dir[:, :, crop[0]:crop[1]]
+    ray = ray.contiguous() if rays is None else rays(ray)
+    V, _, H, W = ray.shape
+    gc, gd = upstream(V, H, W, seed, depth_grad)
+    c = dict(rgba=rgba, rgb=rgb, alpha=alpha, bg=bg, view2mpi=geo.view2mpi, dhw=dhw[:1].expand(M, -1, -1), ray_dir=ray, eye=geo.eye,
+             z_dir=geo.z_dir, gc=gc, gd=gd)
+    c = {k: None if t is None else np.ascontiguousarray(t.numpy()) for k, t in c.items()}
+    c.update(ac=ac, view_group=view_group, video=video, m11=m11, visible=visible)
+    if factored:
+        c["factored"] = True
+    ok = np.isfinite(c["ray_dir"]).all(1) & (c["ray_dir"][:, 2] != 0)
+    if not ok.all():
+        c["ok"] = ok
+        c["gc"] *= ok[:, None]
     return c
 
 
+def shuffled_rays(ray):
+    """The rays shuffled over the image (one permutation for every view): not a pinhole camera's, so no tile's corner rays bound
+    its taps."""
+    V, _, H, W = ray.shape
+    perm = torch.randperm(H * W, generator=torch.Generator().manual_seed(0))
+    return ray.reshape(V, 3, -1)[:, :, perm].reshape(V, 3, H, W).contiguous()
+
+
+TILE_W = 64          # kTileW: the pixel columns of a tile of the staged kernels (csrc/mpi_fwd_staged.cuh)
+
+
+def corners_off(ray):
+    """The four corner rays of every TILE_W x FWD_TILE[0] tile of the staged forward pushed far off the planes, the interior rays
+    kept."""
+    ray = ray.clone()
+    H, W = ray.shape[-2:]
+    tw, th = TILE_W, mpi_oracle.FWD_TILE[0]
+    for ty in range(0, H, th):
+        for tx in range(0, W, tw):
+            for cy in (ty, min(ty + th - 1, H - 1)):
+                for cx in (tx, min(tx + tw - 1, W - 1)):
+                    ray[:, 0, cy, cx] = 5.0
+    return ray
+
+
+def degenerate_rays(ray):
+    """View 0's rays at (10, 10:14) parallel to the planes (ray_z == 0), and a NaN ray at (20, 20)."""
+    ray = ray.clone()
+    ray[0, 2, 10, 10:14] = 0.0
+    ray[0, :, 20, 20] = float("nan")
+    return ray
+
+
+VIEW_ORDERS = {"sorted": [0, 1, 2, 3, 4, 5], "interleaved": [0, 2, 4, 1, 3, 5], "reversed": [5, 4, 3, 2, 1, 0]}
+
+
+def view_order(c, order):
+    """Case c with its views (rays, poses and upstream gradients) in the order VIEW_ORDERS[order] of six views."""
+    perm = VIEW_ORDERS[order]
+    return dict(c, **{k: None if c[k] is None else np.ascontiguousarray(c[k][perm]) for k in ("view2mpi", "ray_dir", "eye", "z_dir",
+                                                                                                 "gc", "gd")})
+
+
+# The full-size shapes (BASELINE.json's configs): synth.make_case arguments
+C4_YAWS = np.linspace(0.5, -0.5, 120).astype(np.float32)[::8]
+FULL = {
+    "full_32x256": dict(n_planes=32, tex=256, img=256, n_mpi=8, seed=1234),
+    "full_96x512": dict(n_planes=96, tex=512, img=512, n_mpi=2, seed=1234),
+    "full_96x1024": dict(n_planes=96, tex=1024, img=1024, n_mpi=1, seed=1234),
+    "c3": dict(n_planes=96, tex=1024, img=1024, n_mpi=1, seed=1234, last_alpha_one=True),
+    "ffhq1024_batch4": dict(n_planes=96, tex=1024, img=1024, n_mpi=4, seed=1234, last_alpha_one=True),   # bench.py's batch: 6.4 GB
+    "c5": dict(n_planes=96, tex=512, img=512, n_mpi=4, seed=99, last_alpha_one=True),
+    "four_views": dict(n_planes=48, tex=512, img=512, n_mpi=1, views_per_mpi=4, seed=21, last_alpha_one=True),
+    "c4_video": dict(n_planes=96, tex=512, img=512, n_mpi=1, views_per_mpi=15, seed=1234, yaws=C4_YAWS, pitches=np.zeros(15, np.float32)),
+}
+
+
+def _bench(alpha):
+    """bench.py's shape for one view: 96 planes, 1024^2, no opaque last plane, colour-only upstream gradient w.r.t. 2c - 1."""
+    return synth_case(**FULL["full_96x1024"], last_alpha_one=False, alpha=alpha, depth_grad=False, m11=True)
+
+
+def _views4(alpha):
+    """One 48-plane 512^2 MPI seen from four views, colour and depth upstream gradients, alpha == 1 last plane."""
+    return synth_case(**FULL["four_views"], alpha=alpha)
+
+
+def _wide(wt, seed):
+    """16 planes of a 512 x wt texture at 720^2 from three random poses: 1.4 texels per pixel across a tile (64 pixels), 0.7 down
+    it.  wt = 1024: many (tile, plane) footprints need the widest box classes (85..88; 89..96, which the factored forward's 96-wide
+    box could hold but which take the generic body), at origins where the fp16 box starts 4 texels further west and at every
+    offset from the uint8 box's multiple of 16; wt = 1536: footprints wider than 96."""
+    return synth_case(n_planes=16, tex=None, img=720, n_mpi=1, views_per_mpi=3, seed=seed, tex_hw=(512, wt), alpha_scale=0.1,
+                      visible=True)
+
+
 SYNTH = {
-    "small": lambda: synth_case(16, 64, 96, 2, views=2, seed=1),
-    "view_group3": lambda: synth_case(24, 96, 128, 1, views=3, seed=2, view_group=3),
-    "factored": lambda: synth_case(24, 96, 128, 2, views=2, seed=3, factored=True),
-    "factored_view_group2": lambda: synth_case(12, 64, 96, 1, views=2, seed=4, factored=True, view_group=2),
-    "uint8": lambda: synth_case(16, 64, 96, 2, views=2, seed=5, video=True),
-    "N1": lambda: synth_case(1, 128, 160, 2, seed=6),
-    "N2": lambda: synth_case(2, 128, 160, 2, seed=7),
-    "N512": lambda: synth_case(512, 96, 128, 2, seed=8, alpha_scale=0.02),
-    "partial_acfalse_nonsquare": lambda: synth_case(10, 8, 136, 2, views=2, seed=9, crop=(18, 118), tex_hw=(72, 116), ac=False),
+    "small": lambda: synth_case(n_planes=16, tex=64, img=96, n_mpi=2, views_per_mpi=2, seed=1),
+    "view_group3": lambda: synth_case(n_planes=24, tex=96, img=128, n_mpi=1, views_per_mpi=3, seed=2, view_group=3),
+    "factored": lambda: synth_case(n_planes=24, tex=96, img=128, n_mpi=2, views_per_mpi=2, seed=3, factored=True),
+    "factored_view_group2": lambda: synth_case(n_planes=12, tex=64, img=96, n_mpi=1, views_per_mpi=2, seed=4, factored=True,
+                                               view_group=2),
+    "uint8": lambda: synth_case(n_planes=16, tex=64, img=96, n_mpi=2, views_per_mpi=2, seed=5, video=True),
+    # the edges: one plane that is not opaque (plane 3 of an 8-plane table); N = kMaxPlanesStaged, whose back planes show through;
+    # 100 x 136 pixels (partial tiles of the forward's 64 x 30 and the backward's 64 x 24) cut out of a pinhole image, a 72 x 116
+    # texture (116 % 8 == 116 % 16 == 4), align_corners=False
+    "N1": lambda: synth_case(n_planes=8, plane=3, tex=128, img=160, n_mpi=2, seed=41, last_alpha_one=False, visible=True),
+    "N2": lambda: synth_case(n_planes=2, tex=128, img=160, n_mpi=2, seed=7),
+    "N512": lambda: synth_case(n_planes=512, tex=96, img=128, n_mpi=2, seed=43, alpha_scale=0.02),
+    "partial_acfalse_nonsquare": lambda: synth_case(n_planes=10, tex=None, img=136, n_mpi=2, views_per_mpi=2, seed=47, tex_hw=(72, 116),
+                                                    alpha_scale=0.2, crop=(18, 118), ac=False, visible=True),
+    "shuffled_rays": lambda: synth_case(n_planes=12, tex=96, img=200, n_mpi=1, views_per_mpi=2, seed=3, alpha_scale=0.2,
+                                        rays=shuffled_rays, visible=True),
+    "corners_off_the_planes": lambda: synth_case(n_planes=6, tex=64, img=128, n_mpi=1, views_per_mpi=2, seed=9, alpha_scale=0.4,
+                                                 rays=corners_off, visible=True),
+    "degenerate_rays": lambda: synth_case(n_planes=8, tex=64, img=64, n_mpi=1, seed=4, alpha_scale=0.3, rays=degenerate_rays,
+                                          depth_grad=False, visible=True),
+    # three MPIs of two views each and a fourth MPI that no view looks at, views in every order of VIEW_ORDERS
+    "three_mpis": lambda: synth_case(n_planes=12, tex=256, img=256, n_mpi=3, views_per_mpi=2, seed=77, alpha_scale=0.15, extra_mpis=1,
+                                     visible=True),
+    **{f"three_mpis_{o}": (lambda o=o: view_order(case("three_mpis"), o)) for o in VIEW_ORDERS},
+    "band_89_96": lambda: _wide(1024, 21),
+    "wider_than_96": lambda: _wide(1536, 22),
+    "bench_96x1024": lambda: _bench("uniform"),
+    "views4_48x512": lambda: _views4("uniform"),
+    # the operating points with every plane visible: U(0, 1) alpha hides the planes past ~25 from every bar
+    "bench_96x1024_equal_weight": lambda: _bench("equal_weight"),
+    "views4_48x512_equal_weight": lambda: _views4("equal_weight"),
+    # the cases of the transmittance and factored suites' own tests
+    "small_12x96": lambda: synth_case(n_planes=12, tex=96, img=128, n_mpi=2, views_per_mpi=2, seed=5, alpha_scale=0.18, visible=True),
+    "staged_shape": lambda: synth_case(n_planes=12, tex=96, img=256, n_mpi=2, views_per_mpi=2, seed=6, alpha_scale=0.25),
+    "bench_96x512_one_view": lambda: synth_case(n_planes=96, tex=512, img=512, n_mpi=1, seed=1234, alpha_scale=0.06),
+    "view_group": lambda: synth_case(n_planes=16, tex=256, img=256, n_mpi=2, views_per_mpi=4, seed=8, alpha_scale=0.12, visible=True),
 }
 
 
@@ -178,7 +319,19 @@ def case(name):
     return SYNTH[name]() if name in SYNTH else golden_case(name)
 
 
-CASES = MPI_CASES + ["c1_full_256"] + list(SYNTH)
+# the forward tests' cases (fp16, uint8, early stop)
+CASES = MPI_CASES + ["c1_full_256", "small", "view_group3", "factored", "factored_view_group2", "uint8", "N1", "N2", "N512",
+                     "partial_acfalse_nonsquare"]
+
+
+def on_device(c, *keys):
+    """The arrays `keys` of case c as tensors on the device (None stays None)."""
+    return tuple(None if c[k] is None else torch.from_numpy(np.ascontiguousarray(c[k])).to(dev()) for k in keys)
+
+
+def pixels(c, a):
+    """a [V,C,H,W] at the pixels the checks compare: every pixel, or those of the case's mask ok, as [C, pixels]."""
+    return a if c.get("ok") is None else a.transpose(1, 0, 2, 3)[:, c["ok"]]
 
 
 # ------------------------------------------------------------------------------------------------------------------------------
@@ -193,7 +346,7 @@ def forward_desc(c, mpi, tau=None, cam=None, u8_round=False, view_group=None, ga
     video case, or with `gather` the frames of a fused gather into one local buffer ("frames"); early stop at tau; the case's view
     group unless one is given.  Returns (descriptor, the tensors behind its pointers)."""
     d = dev()
-    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(d)
+    geo = dict(zip(GEOMETRY, on_device(c, *GEOMETRY)))
     ref = mpi["alpha"] if "alpha" in mpi else mpi["rgba"]
     V, _, H, W = c["ray_dir"].shape
     if gather:
@@ -204,10 +357,10 @@ def forward_desc(c, mpi, tau=None, cam=None, u8_round=False, view_group=None, ga
                    video_depth=torch.empty((V, H, W, 1), dtype=torch.uint8, device=d), depth_near=0.9, depth_range=np.float32(0.3).item())
     else:
         out = dict(color=torch.empty((V, 3, H, W), device=d), depth=torch.empty((V, 1, H, W), device=d))
-    rays = dict(cam=cam) if cam is not None else dict(ray_dir=t(c["ray_dir"]), eye=t(c["eye"]), z_dir=t(c["z_dir"]))
+    rays = dict(cam=cam) if cam is not None else {k: geo[k] for k in ("ray_dir", "eye", "z_dir")}
     opts = (_lib.OPT_ALIGN_CORNERS if c["ac"] else 0) | _lib.OPT_COLOR_MINUS1_1 | (_lib.OPT_U8_ROUND_HALF_UP if u8_round else 0) \
         | (_lib.OPT_EARLY_STOP if tau is not None else 0) | _ELEMENT_OPTION[ref.dtype]
-    keep = dict(view2mpi=t(c["view2mpi"]), dhw=t(c["dhw"]), flags=torch.zeros(1, dtype=torch.int32, device=d), **rays, **out, **mpi)
+    keep = dict(view2mpi=geo["view2mpi"], dhw=geo["dhw"], flags=torch.zeros(1, dtype=torch.int32, device=d), **rays, **out, **mpi)
     desc = _lib.make_desc(options=opts, M=ref.shape[0], V=V, N=ref.shape[1], Ht=ref.shape[-2], Wt=ref.shape[-1], H=H, W=W,
                           view_group=c.get("view_group", 1) if view_group is None else view_group, early_stop=tau, **keep)
     return desc, dict(keep, frames=frames) if gather else keep
@@ -253,13 +406,6 @@ def limit_footprints(c, lo, hi):
     f = footprints(c)
     fits = (f["mode"] != 1) & (-(-f["need_h"] // 4) * 4 <= mpi_oracle.FWD_TILE[1])
     return int((fits & (f["need_w"] >= lo) & (f["need_w"] <= hi) & (f["bx0"] % 8 == 4)).sum())
-
-
-@functools.lru_cache(maxsize=None)
-def limit_case(factored):
-    """A 512 x 1024 texture seen at 720^2 from three random poses: 1.4 texels per pixel across a tile (64 pixels), 0.7 down it.
-    Many (tile, plane) footprints need the widest box classes, at origins where the fp16 box starts 4 texels further west."""
-    return synth_case(16, 8, 720, 1, views=3, seed=21, tex_hw=(512, 1024), factored=factored)
 
 
 @functools.lru_cache(maxsize=None)
