@@ -78,8 +78,8 @@ const char* gmpi_mpi_render_fwd_variant(int N, int Ht, int Wt, int H, int W);
  * instead of finding it in a profile.  rgba may be NULL (alignment unknown: not checked).  gmpi_mpi_render_fwd_plan_ex answers
  * for a whole descriptor (M MPIs, factored, fp16).  The early-stop and training forwards get the same plan as the plain one.  The
  * plan assumes the MPI's tensor maps encode; if cuTensorMapEncodeTiled refuses them, the forward takes the direct kernels (or
- * fails, under gmpi_debug_set_fwd_variant(2)).  The
- * backward has conditions of its own (gmpi_mpi_render_bwd_saved).
+ * fails, under gmpi_debug_set_fwd_variant(2)).  The backward's kernel, and every reason it is not the staged one, comes from
+ * gmpi_mpi_render_bwd_plan_ex (GMPI_WHY_NO_TRANSMITTANCE and up).
  */
 #define GMPI_PLAN_DIRECT 1
 #define GMPI_PLAN_STAGED 2
@@ -89,6 +89,12 @@ const char* gmpi_mpi_render_fwd_variant(int N, int Ht, int Wt, int H, int W);
                                     M*N >= 2^31 planes over all MPIs                                                    */
 #define GMPI_WHY_ALIGNMENT 8u    /* an MPI base (rgba, rgb, alpha or bg_rgb) not 16-byte aligned                        */
 #define GMPI_WHY_FORCED 16u      /* gmpi_debug_set_fwd_variant(1)                                                        */
+/* the backward's own reasons (gmpi_mpi_render_bwd_plan_ex) */
+#define GMPI_WHY_NO_TRANSMITTANCE 32u   /* no saved transmittance: the forward did not save one for the box kernel's sweep       */
+#define GMPI_WHY_IMG_WIDTH 64u          /* W % 4 != 0: the transmittance's rows are not 16-byte multiples, no tensor map         */
+#define GMPI_WHY_GRAD_ALIGNMENT 128u    /* a gradient base (g_rgba, or g_rgb, g_alpha, g_bg_rgb) or the transmittance base is
+                                           not 16-byte aligned                                                                 */
+#define GMPI_WHY_MANY_PIXEL_PLANES 256u /* V*N >= 2^31 pixel planes of transmittance                                            */
 int gmpi_mpi_render_fwd_plan(int V, int N, int Ht, int Wt, int H, int W, const void* rgba, uint32_t* why);
 
 /*
@@ -141,10 +147,8 @@ int gmpi_mpi_render_bwd(const float* rgba, const int32_t* view2mpi, const float*
  * Training pair.  gmpi_mpi_render_fwd_train = gmpi_mpi_render_fwd that additionally saves the transmittance in front of
  * every plane, transmittance [V,N,H,W] (T_i = prod_{j<i}(1 - alpha_j), mpi.py:421-423) -- what torch autograd keeps alive as
  * `weights`/`cumprod` tensors, here 4 bytes per (pixel, plane).  gmpi_mpi_render_bwd_saved consumes it: one staged
- * back-to-front sweep instead of the two-pass kernel.  That staged box backward runs when the forward plan of the same call is
- * GMPI_PLAN_STAGED (gmpi_mpi_render_fwd_plan) and also W % 4 == 0, V*N < 2^31 and the gradient and transmittance bases are
- * 16-byte aligned; otherwise the call runs gmpi_mpi_render_bwd's two-pass kernel.  The same holds for gmpi_mpi_render_bwd_ex with
- * a transmittance (its plan: gmpi_mpi_render_fwd_plan_ex).
+ * back-to-front sweep instead of the two-pass kernel, where gmpi_mpi_render_bwd_plan_ex of the same call answers
+ * GMPI_PLAN_STAGED; otherwise the call runs gmpi_mpi_render_bwd's two-pass kernel.
  */
 int gmpi_mpi_render_fwd_train(const float* rgba, const int32_t* view2mpi, const float* dhw,
                               const float* ray_dir, const float* eye, const float* z_dir,
@@ -275,6 +279,20 @@ int gmpi_mpi_render_fwd_ex(const gmpi_render_desc* desc);
  * aligned (GMPI_WHY_ALIGNMENT); NULL ones are not checked.  Forward only, like gmpi_mpi_render_fwd_plan.  Returns the plan, or a
  * negative GMPI_ERR_* code for a bad descriptor. */
 int gmpi_mpi_render_fwd_plan_ex(const gmpi_render_desc* desc, uint32_t* why);
+/* The backward kernel gmpi_mpi_render_bwd_ex and gmpi_mpi_render_bwd_deterministic_ex (which makes the same choice) launch for a
+ * descriptor, asked before the training forward runs: GMPI_PLAN_STAGED (the box kernel, one back-to-front sweep over the saved
+ * transmittance) or GMPI_PLAN_DIRECT (the two-pass kernel, which walks every plane twice).  *why (nullable) receives the GMPI_WHY_*
+ * bits of every reason it is not the box kernel: those of gmpi_mpi_render_fwd_plan_ex for the same descriptor (the box kernel reads
+ * the MPI as the staged forward does), and GMPI_WHY_NO_TRANSMITTANCE (transmittance NULL), GMPI_WHY_IMG_WIDTH,
+ * GMPI_WHY_GRAD_ALIGNMENT and GMPI_WHY_MANY_PIXEL_PLANES.  It reads the sizes, the options, view_group, cam, the MPI pointers, the
+ * gradient pointers and the transmittance pointer, and nothing else; no pointer need be set, and NULL MPI and gradient pointers count
+ * as aligned.  It needs no GPU.  It refuses what the backward calls refuse before launching, with the same negative GMPI_ERR_* code
+ * and gmpi_last_error() text, except that it asks for no pointer: the forward-only options (GMPI_MPI_F16, GMPI_MPI_U8,
+ * GMPI_EARLY_STOP), cam, bad sizes or view_group, and the direct kernel's limits (more than 65535 views, too tall an image, more
+ * planes than its stash holds) where it takes the direct kernel with V > 0; on that last refusal *why is still written.  It assumes the
+ * tensor maps encode, as gmpi_mpi_render_fwd_plan_ex does.  The deterministic backward's own refusals (its scratch, and shapes that
+ * leave fewer than 24 fraction bits) are not the plan's. */
+int gmpi_mpi_render_bwd_plan_ex(const gmpi_render_desc* desc, uint32_t* why);
 int gmpi_mpi_render_bwd_ex(const gmpi_render_desc* desc);
 
 /*
@@ -399,6 +417,10 @@ int gmpi_debug_fwd_early_stop_stats(unsigned long long* skipped, unsigned long l
 /* Test hook: the last gmpi_mpi_render_fwd_skip_ex launch on this device (synchronises the device): *skipped = the (tile, plane)
  * stages the staged kernel armed empty, *total = the stages it walked (0 when the direct kernel ran). */
 int gmpi_debug_fwd_skip_stats(unsigned long long* skipped, unsigned long long* total);
+
+/* Test hook (host only, does not synchronise): *key = the variant key (the kKey* bits of csrc/mpi_kernel_keys.cuh) of the last render
+ * kernel, forward or backward, the library launched on `device` from any thread; GMPI_ERR_INVALID_ARGUMENT before the first. */
+int gmpi_debug_last_render_key(int device, uint32_t* key);
 
 /* Test hook (host only): the staged producer's box-versus-map test on one plane's map (host memory, the layout of
  * gmpi_mpi_build_occupancy): 1 when a block under the texels [bx0, bx0 + bw) x [by0, by0 + rows) inside the Ht x Wt texture is

@@ -20,7 +20,10 @@ OPT_ZERO_GRAD = 8
 PLAN_DIRECT, PLAN_STAGED = 1, 2
 WHY = {1: "texture width is not a multiple of 4 (8 in fp16, 16 in uint8)", 2: "fewer than 120 tiles of 64x30 pixels",
        4: "more than 512 planes, or 2^31 planes over all MPIs", 8: "an MPI base pointer is not 16-byte aligned",
-       16: "direct kernel forced by gmpi_debug_set_fwd_variant"}
+       16: "direct kernel forced by gmpi_debug_set_fwd_variant",
+       # the backward's own (gmpi_mpi_render_bwd_plan_ex)
+       32: "no saved transmittance", 64: "image width is not a multiple of 4",
+       128: "a gradient or transmittance base pointer is not 16-byte aligned", 256: "2^31 or more pixel planes (V*N)"}
 
 ABI_VERSION = 2
 
@@ -62,6 +65,7 @@ SIGNATURES = {
     "gmpi_mpi_zero_async": (_i, [_vp, _size, _vp]),
     "gmpi_mpi_render_fwd_ex": (_i, [_desc]),
     "gmpi_mpi_render_fwd_plan_ex": (_i, [_desc, _vp]),
+    "gmpi_mpi_render_bwd_plan_ex": (_i, [_desc, _vp]),
     "gmpi_mpi_render_bwd_ex": (_i, [_desc]),
     "gmpi_mpi_render_bwd_deterministic_scratch_bytes": (_ll, [_desc]),
     "gmpi_mpi_render_bwd_deterministic_ex": (_i, [_desc, _vp, _size]),
@@ -83,6 +87,7 @@ SIGNATURES = {
     "gmpi_debug_set_fwd_stages": (_i, [_i]),
     "gmpi_debug_fwd_early_stop_stats": (_i, [_vp, _vp]),
     "gmpi_debug_fwd_skip_stats": (_i, [_vp, _vp]),
+    "gmpi_debug_last_render_key": (_i, [_i, _vp]),
     "gmpi_debug_box_occupied": (_i, [_vp] + [_i] * 6),
     "gmpi_debug_u8_codes_host": (_i, [_vp]),
     "gmpi_debug_u8_codes": (_i, [_vp, _vp]),
@@ -163,3 +168,18 @@ def fwd_plan(desc: RenderDesc):
     if plan < 0:
         check(-plan)
     return plan, why.value
+
+
+def bwd_plan(desc: RenderDesc):
+    """(plan, why) of the backward `desc` describes (gmpi_mpi_render_bwd_plan_ex): PLAN_STAGED (the box kernel) or PLAN_DIRECT, and
+    the WHY bits; raises what the backward call would raise on the host."""
+    why = ctypes.c_uint32(0)
+    plan = load().gmpi_mpi_render_bwd_plan_ex(ctypes.byref(desc), ctypes.byref(why))
+    if plan < 0:
+        check(-plan)
+    return plan, why.value
+
+
+def reasons(why: int):
+    """The WHY texts of the bits of `why`, in bit order."""
+    return [t for b, t in WHY.items() if why & b]

@@ -90,6 +90,7 @@ enum CallKind {
     kSkipCall,        // gmpi_mpi_render_fwd_skip_ex
     kHostCall,        // gmpi_mpi_render_host_ex (host buffers); the classic fwd_host
     kBwdCall,         // gmpi_mpi_render_bwd_ex and gmpi_mpi_render_bwd_deterministic_ex; the classic bwd and bwd_saved
+    kBwdPlanCall,     // gmpi_mpi_render_bwd_plan_ex: kBwdCall's checks less those that a pointer is set (it reads pointer values only)
     kOccQueryCall,    // gmpi_mpi_occupancy_bytes
     kOccBuildCall,    // gmpi_mpi_build_occupancy
     kScratchCall,     // gmpi_mpi_render_bwd_deterministic_scratch_bytes
@@ -127,7 +128,8 @@ static int check_call(const RenderParams& p, const Call& c) {
         return fail(GMPI_ERR_INVALID_ARGUMENT, "GMPI_MPI_U8 and GMPI_MPI_F16 are exclusive");
     // Of the forward-only options, the occupancy calls and the scratch query check GMPI_MPI_U8 alone: the scratch query returns a size
     // for GMPI_MPI_F16 and GMPI_EARLY_STOP, which the deterministic backward refuses.
-    const bool occ = c.kind == kOccQueryCall || c.kind == kOccBuildCall, bwd = c.kind == kBwdCall || c.kind == kScratchCall;
+    const bool occ = c.kind == kOccQueryCall || c.kind == kOccBuildCall, plan = c.kind == kBwdPlanCall,
+               bwd = c.kind == kBwdCall || c.kind == kScratchCall || plan;
     const uint32_t opts = p.options & (occ || c.kind == kScratchCall ? GMPI_MPI_U8 : GMPI_MPI_F16 | GMPI_MPI_U8 | GMPI_EARLY_STOP);
     for (const ForwardOnly& o : kForwardOnly)
         if (bwd && (opts & o.bit)) return fail(GMPI_ERR_UNSUPPORTED, "%s is forward-only: %s", o.name, o.why);
@@ -141,20 +143,21 @@ static int check_call(const RenderParams& p, const Call& c) {
     if ((opts & GMPI_EARLY_STOP) && !(p.early_stop >= 0.0f && p.early_stop < 1.0f))
         return fail(GMPI_ERR_INVALID_ARGUMENT, "early_stop = %g must be in [0, 1) (gmpi_render_desc.early_stop)", (double)p.early_stop);
     if (c.kind == kScratchCall) return check_sizes(p, true, false);
-    if (factored(p) ? !p.rgb || p.rgba : !p.rgba || p.rgb)
+    if (!plan && (factored(p) ? !p.rgb || p.rgba : !p.rgba || p.rgb))
         return fail(GMPI_ERR_INVALID_ARGUMENT, "null input pointer (MPI: pass rgba, or rgb + alpha)");
     if (occ) {
         if (int rc = check_sizes(p, false, true)) return rc;
         return c.kind == kOccBuildCall ? check_occ_map(p, c) : GMPI_OK;
     }
-    if (!p.view2mpi || !p.dhw) return fail(GMPI_ERR_INVALID_ARGUMENT, "null input pointer");
-    if (!p.cam && (!p.ray_dir || !p.eye || !p.z_dir))
+    if (!plan && (!p.view2mpi || !p.dhw)) return fail(GMPI_ERR_INVALID_ARGUMENT, "null input pointer");
+    if (!plan && !p.cam && (!p.ray_dir || !p.eye || !p.z_dir))
         return fail(GMPI_ERR_INVALID_ARGUMENT, "null input pointer (camera: pass ray_dir + eye + z_dir, or cam)");
     if (int rc = check_sizes(p, true, true)) return rc;
     if (p.view_group < 0 || (p.view_group > 1 && p.V % p.view_group != 0))
         return fail(GMPI_ERR_INVALID_ARGUMENT, "view_group=%d does not divide V=%d", p.view_group, p.V);
     if (bwd) {
         if (p.cam) return fail(GMPI_ERR_UNSUPPORTED, "the backward needs the reference's ray tensors (cam is forward-only)");
+        if (plan) return GMPI_OK;
         if (!p.g_color) return fail(GMPI_ERR_INVALID_ARGUMENT, "null gradient pointer");
         if (factored(p) ? (!p.g_rgb || !p.g_alpha || (p.bg_rgb && !p.g_bg_rgb) || p.g_rgba) : !p.g_rgba)
             return fail(GMPI_ERR_INVALID_ARGUMENT, "null gradient pointer (pass g_rgba, or g_rgb + g_alpha [+ g_bg_rgb])");
@@ -359,7 +362,17 @@ static int launch_kernel(void (*kernel)(P...), dim3 grid, dim3 block, size_t sme
     }, params);
 }
 
-static int launch(Launch& l, cudaStream_t st) { return launch_args(render_kernel(l.key), l.grid, l.block, l.smem, st, l.args); }
+// The test hook gmpi_debug_last_render_key: per device, 1 + the key of the last render kernel launch() launched there (0: none yet).
+constexpr int kMaxKeyDevices = 64;
+static std::atomic<uint64_t> g_last_render_key[kMaxKeyDevices];
+
+static int launch(Launch& l, cudaStream_t st) {
+    if (int rc = launch_args(render_kernel(l.key), l.grid, l.block, l.smem, st, l.args)) return rc;
+    int dev = 0;
+    if (cudaGetDevice(&dev) == cudaSuccess && dev >= 0 && dev < kMaxKeyDevices)
+        g_last_render_key[dev].store((uint64_t)l.key + 1, std::memory_order_relaxed);
+    return GMPI_OK;
+}
 
 // The persistent grid of the staged forward and the box backward: tiles of kTileW x tile_h pixels in every view, at most one CTA
 // per SM.  Also adds the arguments both kernels take after p: maps, tiles_x, tiles_y.
@@ -489,17 +502,38 @@ static int zero_grads(const RenderParams& p, cudaStream_t st) {
     return GMPI_OK;
 }
 
-// Backward kernel choice: the staged box kernel when the forward saved the transmittance, the staged forward would be launched
-// (fwd_why) and the backward's own conditions hold (16-byte aligned gradient and transmittance bases, W % 4 == 0, V*N < 2^31), else
-// the direct kernel.  The deterministic backward makes the same choice from the caller's descriptor.
-static bool bwd_uses_box(const RenderParams& p) {
-    const bool fac = factored(p);
-    const bool grads_aligned = fac ? aligned16(p.g_rgb) && aligned16(p.g_alpha) && (!p.g_bg_rgb || aligned16(p.g_bg_rgb)) : aligned16(p.g_rgba);
-    return p.transmittance && fwd_why(p) == 0 && grads_aligned && p.W % 4 == 0 && aligned16(p.transmittance) &&
-           (size_t)p.V * p.N < ((size_t)1 << 31);
+// The GMPI_WHY_* bits of every reason the staged box backward is not launched for p (0 = box): the one decision behind launch_bwd,
+// launch_bwd_deterministic (from the caller's descriptor) and gmpi_mpi_render_bwd_plan_ex.  The box kernel reads the MPI through the
+// staged forward's tensor maps on its persistent grid, so every reason of fwd_why carries over; its own conditions are a saved
+// transmittance, W % 4 == 0, 16-byte aligned gradient bases of the MPI's form and transmittance base (NULL counts as aligned), and
+// V*N < 2^31 (pixel planes of the transmittance's tensor map).
+static uint32_t bwd_why(const RenderParams& p) {
+    uint32_t w = fwd_why(p);
+    if (!p.transmittance) w |= GMPI_WHY_NO_TRANSMITTANCE;
+    if (p.W % 4 != 0) w |= GMPI_WHY_IMG_WIDTH;
+    const bool grads = factored(p) ? aligned16(p.g_rgb) && aligned16(p.g_alpha) && aligned16(p.g_bg_rgb) : aligned16(p.g_rgba);
+    if (!grads || !aligned16(p.transmittance)) w |= GMPI_WHY_GRAD_ALIGNMENT;
+    if ((size_t)p.V * p.N >= ((size_t)1 << 31)) w |= GMPI_WHY_MANY_PIXEL_PLANES;
+    return w;
 }
 
-// The backward kernel of a checked call with V > 0, with its launch: the box kernel when `box` (bwd_uses_box), else the two-pass
+// The direct backward's CTA of a checked call: as many threads (<=128) as the per-thread transmittance stash allows, and its grid.
+// Refuses what exceeds the kernel's limits; the launch and the plan query both take them from here.
+static int bwd_direct_shape(const RenderParams& p, dim3& block, dim3& grid, size_t& smem) {
+    int tile_w = 32, tile_h = 4;
+    for (;; tile_h >>= 1) {
+        if (tile_h == 0) return fail(GMPI_ERR_UNSUPPORTED, "N=%d planes exceed the backward stash (227 KB / 32 threads)", p.N);
+        smem = sizeof(PlaneConst) * (size_t)p.N + sizeof(float) * (size_t)p.N * tile_w * tile_h;
+        if (smem <= 227 * 1024) break;
+    }
+    block = dim3(tile_w, tile_h);
+    grid = dim3((p.W + tile_w - 1) / tile_w, (p.H + tile_h - 1) / tile_h, p.V);
+    if (grid.y > 65535) return fail(GMPI_ERR_UNSUPPORTED, "image height %d too large", p.H);
+    if (p.V > 65535) return fail(GMPI_ERR_UNSUPPORTED, "V=%d views exceed one launch of the direct kernel (65535); split the batch", p.V);
+    return GMPI_OK;
+}
+
+// The backward kernel of a checked call with V > 0, with its launch: the box kernel when `box` (bwd_why(p) == 0), else the two-pass
 // direct kernel (any shape, no saved state).  det: the deterministic variant, adding into the sums of l.da.
 static int bwd_launch(Launch& l, bool box, bool det) {
     const RenderParams& p = l.p;
@@ -513,19 +547,9 @@ static int bwd_launch(Launch& l, bool box, bool det) {
         l.smem = kBwdSmem;
         key |= kKeyStaged | (factored(p) ? kKeyFac : 0);
     } else {
-        // tile: as many threads (<=128) as the per-thread transmittance stash allows
-        int tile_w = 32, tile_h = 4;
-        for (;; tile_h >>= 1) {
-            if (tile_h == 0) return fail(GMPI_ERR_UNSUPPORTED, "N=%d planes exceed the backward stash (227 KB / 32 threads)", p.N);
-            l.smem = sizeof(PlaneConst) * (size_t)p.N + sizeof(float) * (size_t)p.N * tile_w * tile_h;
-            if (l.smem <= 227 * 1024) break;
-        }
-        l.block = dim3(tile_w, tile_h);
-        l.grid = dim3((p.W + tile_w - 1) / tile_w, (p.H + tile_h - 1) / tile_h, p.V);
-        if (l.grid.y > 65535) return fail(GMPI_ERR_UNSUPPORTED, "image height %d too large", p.H);
-        if (p.V > 65535) return fail(GMPI_ERR_UNSUPPORTED, "V=%d views exceed one launch of the direct kernel (65535); split the batch", p.V);
-        l.ints[0] = tile_w;
-        l.ints[1] = tile_h;
+        if (int rc = bwd_direct_shape(p, l.block, l.grid, l.smem)) return rc;
+        l.ints[0] = (int)l.block.x;
+        l.ints[1] = (int)l.block.y;
         l.arg(&l.ints[0]);
         l.arg(&l.ints[1]);
     }
@@ -538,7 +562,7 @@ static int launch_bwd(RenderParams p, cudaStream_t st) {
     const bool zero = (p.options & GMPI_ZERO_GRAD) != 0;
     if (p.V == 0) return zero ? zero_grads(p, st) : GMPI_OK;
     Launch l(p);
-    int rc = bwd_launch(l, bwd_uses_box(p), false);
+    int rc = bwd_launch(l, bwd_why(p) == 0, false);
     if (rc) return rc;
     if (zero && (rc = zero_grads(p, st)) != 0) return rc;
     return launch(l, st);
@@ -614,7 +638,7 @@ static int launch_bwd_deterministic(RenderParams p, void* scratch, size_t scratc
     } else {
         l.p.g_rgba = da.base;
     }
-    if ((rc = bwd_launch(l, bwd_uses_box(p), true)) != 0) return rc;
+    if ((rc = bwd_launch(l, bwd_why(p) == 0, true)) != 0) return rc;
     GMPI_CUDA_OK(cudaMemsetAsync(scratch, 0, L.bytes, st));
     dim3 bgrid((unsigned)(((size_t)p.H * p.W + 255) / 256), (unsigned)(p.V < 65535 ? p.V : 65535));
     if ((rc = launch_kernel(mpi_bwd_det_bounds_kernel, bgrid, 256, 0, st, l.p, da.bounds)) != 0) return rc;
@@ -805,6 +829,28 @@ int gmpi_mpi_render_fwd_plan_ex(const gmpi_render_desc* d, uint32_t* why) {
     const uint32_t w = fwd_why(params_from_desc(d));
     if (why) *why = w;
     return w == 0 ? GMPI_PLAN_STAGED : GMPI_PLAN_DIRECT;
+}
+
+int gmpi_mpi_render_bwd_plan_ex(const gmpi_render_desc* d, uint32_t* why) {
+    RenderParams p{};
+    int rc = check_desc_call(d, Call{kBwdPlanCall}, p);
+    if (rc) return -rc;
+    const uint32_t w = bwd_why(p);
+    if (why) *why = w;
+    // the direct kernel's limits refuse a call that launches it (launch_bwd: a call with V = 0 launches nothing)
+    dim3 block, grid;
+    size_t smem = 0;
+    if (w != 0 && p.V > 0 && (rc = bwd_direct_shape(p, block, grid, smem)) != 0) return -rc;
+    return w == 0 ? GMPI_PLAN_STAGED : GMPI_PLAN_DIRECT;
+}
+
+int gmpi_debug_last_render_key(int device, uint32_t* key) {
+    if (!key) return fail(GMPI_ERR_INVALID_ARGUMENT, "null pointer");
+    if (device < 0 || device >= kMaxKeyDevices) return fail(GMPI_ERR_INVALID_ARGUMENT, "device %d out of range", device);
+    const uint64_t k = g_last_render_key[device].load(std::memory_order_relaxed);
+    if (k == 0) return fail(GMPI_ERR_INVALID_ARGUMENT, "no render kernel was launched on device %d", device);
+    *key = (uint32_t)(k - 1);
+    return GMPI_OK;
 }
 
 const char* gmpi_mpi_render_fwd_variant(int N, int Ht, int Wt, int H, int W) {

@@ -8,7 +8,7 @@ No CPU path: tensors must live on a CUDA device, otherwise this raises.
 """
 import ctypes
 import warnings
-from typing import List, Optional, Union
+from typing import List, NamedTuple, Optional, Tuple, Union
 
 import numpy as np
 import torch
@@ -335,6 +335,15 @@ def render_views_factored(rgb, alpha, dhw, view2mpi, ray_dir, eye, z_dir, *, bg_
                          flags, view_group, early_stop, deterministic, skip_empty)
 
 
+def _check_factored_shapes(mpi):
+    """The shapes of a factored MPI `mpi` = [None, rgb, alpha, bg_rgb] (an expanded one passes)."""
+    rgba, rgb, alpha, bg_rgb = mpi
+    if rgba is None:
+        assert rgb.ndim == 4 and rgb.shape[1] == 3 and alpha.ndim == 5 and alpha.shape[2] == 1 and rgb.shape[0] == alpha.shape[0] \
+            and rgb.shape[-2:] == alpha.shape[-2:], f"expected rgb [M,3,Ht,Wt] and alpha [M,N,1,Ht,Wt], got {rgb.shape}, {alpha.shape}"
+        assert bg_rgb is None or bg_rgb.shape == rgb.shape, f"bg_rgb must have rgb's shape, got {bg_rgb.shape}"
+
+
 def _render_views(mpi, dhw, view2mpi, ray_dir, eye, z_dir, align_corners, check_last_plane, color_minus1_1, flags, view_group,
                   early_stop, deterministic, skip_empty, unorm8=False):
     """render_views of the MPI tensors `mpi` = [rgba, rgb, alpha, bg_rgb] (None where absent), and render_views_factored."""
@@ -342,11 +351,7 @@ def _render_views(mpi, dhw, view2mpi, ray_dir, eye, z_dir, align_corners, check_
     _check_forward_only("skip_empty", skip_empty is not False and skip_empty is not None, *mpi)
     ref = _mpi_ref(mpi)
     _require_cuda(ref)
-    rgba, rgb, alpha, bg_rgb = mpi
-    if rgba is None:
-        assert rgb.ndim == 4 and rgb.shape[1] == 3 and alpha.ndim == 5 and alpha.shape[2] == 1 and rgb.shape[0] == alpha.shape[0] \
-            and rgb.shape[-2:] == alpha.shape[-2:], f"expected rgb [M,3,Ht,Wt] and alpha [M,N,1,Ht,Wt], got {rgb.shape}, {alpha.shape}"
-        assert bg_rgb is None or bg_rgb.shape == rgb.shape, f"bg_rgb must have rgb's shape, got {bg_rgb.shape}"
+    _check_factored_shapes(mpi)
     if flags is None:
         flags = _zero_flags(ref.device)
     V, _, H, W = ray_dir.shape
@@ -357,6 +362,52 @@ def _render_views(mpi, dhw, view2mpi, ray_dir, eye, z_dir, align_corners, check_
     _warn_if_direct(_mpi_desc(mpi, V, H, W, options))
     return _RenderFn.apply(*mpi, _as_f32c(dhw), view2mpi, _as_f32c(ray_dir), _as_f32c(eye), _as_f32c(z_dir),
                            options, flags, int(view_group), early_stop, deterministic, occ)
+
+
+class TrainPlan(NamedTuple):
+    """The kernels of a training render (train_plan): for each pass _lib.PLAN_STAGED (the TMA-staged forward, the box backward) or
+    _lib.PLAN_DIRECT (the direct kernels: one thread per pixel forward, two passes over every plane backward), the GMPI_WHY_* bits of
+    every reason it is not the staged kernel, and those reasons in words (_lib.WHY)."""
+    forward: int
+    forward_why: int
+    forward_reasons: Tuple[str, ...]
+    backward: int
+    backward_why: int
+    backward_reasons: Tuple[str, ...]
+
+
+# What a descriptor holds for a buffer the render allocates itself (torch.empty / empty_like: a fresh allocation, 512-byte aligned):
+# the plan queries read its alignment, never its memory.
+_FRESH_BUFFER = 512
+
+
+def train_plan(*, dhw, view2mpi, ray_dir, eye, z_dir, rgba=None, rgb=None, alpha=None, bg_rgb=None, align_corners=True,
+               check_last_plane=False, color_minus1_1=False, view_group: int = 1, deterministic: Optional[bool] = None) -> TrainPlan:
+    """Which kernels the training render of these inputs gets, asked before it runs: render_views(rgba, ...) or
+    render_views_factored(rgb, alpha, ..., bg_rgb=...) with the same tensors and keywords, with autograd recording for the MPI, then
+    its backward (gmpi_mpi_render_fwd_plan_ex and gmpi_mpi_render_bwd_plan_ex).  The descriptor is the one the render launches: the
+    MPI tensors as _launch_mpi hands them to the kernels (a copy where they are not contiguous fp32), and the transmittance and
+    gradient buffers the render allocates, which are fresh and aligned.  The MPI tensors need not be on the GPU and nothing is
+    launched; no other input is read.  deterministic (None: torch.are_deterministic_algorithms_enabled()): the deterministic backward
+    makes the same kernel choice, and its scratch-size query must accept the call too.  Raises ValueError when no MPI tensor requires
+    grad (the render then has no backward), and GmpiLibraryError where the backward call would refuse the inputs."""
+    mpi = [rgba, rgb, alpha, bg_rgb]
+    _check_factored_shapes(mpi)
+    if not any(t is not None and t.requires_grad for t in mpi):
+        raise ValueError("train_plan answers for a training render: no MPI tensor requires grad, so the render has no backward")
+    V, _, H, W = ray_dir.shape
+    with torch.enable_grad():            # what the training render sees: autograd records for the MPI
+        mpi, options = _launch_mpi(mpi, V, H, W, _options(align_corners, check_last_plane, color_minus1_1))
+    fresh = lambda t: None if t is None else _FRESH_BUFFER
+    d = _mpi_desc(mpi, V, H, W, options, view_group=int(view_group), transmittance=_FRESH_BUFFER)
+    fwd, fwd_why = _lib.fwd_plan(d)
+    # _RenderFn.backward: the same descriptor with GMPI_ZERO_GRAD and an empty_like gradient of every MPI tensor
+    d.options |= _lib.OPT_ZERO_GRAD
+    d.g_rgba, d.g_rgb, d.g_alpha, d.g_bg_rgb = (fresh(t) for t in mpi)
+    bwd, bwd_why = _lib.bwd_plan(d)
+    if torch.are_deterministic_algorithms_enabled() if deterministic is None else deterministic:
+        _lib.deterministic_scratch_bytes(d)
+    return TrainPlan(fwd, fwd_why, tuple(_lib.reasons(fwd_why)), bwd, bwd_why, tuple(_lib.reasons(bwd_why)))
 
 
 def expand_factored(rgb, alpha, bg_rgb=None):
